@@ -519,57 +519,63 @@ __global__ void __launch_bounds__(256, EVG_OCC_GUNIT) k_gunit(DDistros D, DWork 
 __global__ void __launch_bounds__(256, EVG_OCC_GBEST) k_gbest(DTasks T, DDistros D, DWork W, DGen G, int want_best_pair) {
   if (*W.err) return;
   const unsigned int n = *G.ccount;
-  for (unsigned int k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x) {
-    const WlTask x = wl_task(T, D, W, G, k);
-    const uint32_t t = x.t, li = x.li;
-    const int d = x.d;
-    bool have = false;
-    int64_t bv = 0;
-    uint32_t ba = 0, brk = 0, bp = kInactive, bslot = kInactive, bn = 1, bkx = 0;
-    if (!x.own_complex) { have = true; bv = G.tv[t]; ba = li; }  // its own single-task unit, scored by k_gtask
-    wl_pairs(T, W, x, [&](uint32_t pair, uint32_t slot) {
-      const uint4 u = G.usum[slot];
-      const uint32_t kx = W.next[pair];  // this task's place in that unit's run (requested together with the summary)
-      const uint32_t a = u.z;
-      if (a == kNoAnchor) return;
-      const int64_t v = int64_t((unsigned long long)u.x | ((unsigned long long)u.y << 32));
-      if (!have || v > bv || (v == bv && a < ba)) { have = true; bv = v; ba = a; bp = pair; bslot = slot; bn = u.w; bkx = kx; }
-    });
-    if (bp != kInactive) {  // rank among ALL members of the chosen unit; the task's own fields are its record in the run
-      const URec* run = G.rec + W.head[bslot];
-      const URec me = rec_load(run + bkx);
-      for (uint32_t i = 0; i < bn; i++) {
-        const URec r = rec_load(run + i);
-        if (in_unit_less(r.tgo, r.nd, r.prio, r.exp_ns, rec_li(r), me.tgo, me.nd, me.prio, me.exp_ns, li)) brk++;
+  const unsigned full = 0xffffffffu;
+  const int lane = threadIdx.x & 31;
+  // Warp-uniform trips (every lane of a warp runs the same ones, lanes past n idle), so that the value-range fold at the
+  // end of a trip is a full-warp reduction that needs no assumption about which lanes reconverged.
+  for (unsigned int kw = blockIdx.x * blockDim.x + (threadIdx.x & ~31u); kw < n; kw += gridDim.x * blockDim.x) {
+    const unsigned int k = kw + lane;
+    int d = -1;
+    unsigned long long kk = 0ull;
+    if (k < n) {
+      const WlTask x = wl_task(T, D, W, G, k);
+      const uint32_t t = x.t, li = x.li;
+      d = x.d;
+      bool have = false;
+      int64_t bv = 0;
+      uint32_t ba = 0, brk = 0, bp = kInactive, bslot = kInactive, bn = 1, bkx = 0;
+      if (!x.own_complex) { have = true; bv = G.tv[t]; ba = li; }  // its own single-task unit, scored by k_gtask
+      wl_pairs(T, W, x, [&](uint32_t pair, uint32_t slot) {
+        const uint4 u = G.usum[slot];
+        const uint32_t kx = W.next[pair];  // this task's place in that unit's run (requested together with the summary)
+        const uint32_t a = u.z;
+        if (a == kNoAnchor) return;
+        const int64_t v = int64_t((unsigned long long)u.x | ((unsigned long long)u.y << 32));
+        if (!have || v > bv || (v == bv && a < ba)) { have = true; bv = v; ba = a; bp = pair; bslot = slot; bn = u.w; bkx = kx; }
+      });
+      if (bp != kInactive) {  // rank among ALL members of the chosen unit; the task's own fields are its record in the run
+        const URec* run = G.rec + W.head[bslot];
+        const URec me = rec_load(run + bkx);
+        for (uint32_t i = 0; i < bn; i++) {
+          const URec r = rec_load(run + i);
+          if (in_unit_less(r.tgo, r.nd, r.prio, r.exp_ns, rec_li(r), me.tgo, me.nd, me.prio, me.exp_ns, li)) brk++;
+        }
+        if (bn <= 64) atomicOr(&W.unit_mask[bslot], 1ull << brk);  // ranks emitted from the unit: k_gplace_disp counts below its own
       }
-      if (bn <= 64) atomicOr(&W.unit_mask[bslot], 1ull << brk);  // ranks emitted from the unit: k_gplace_disp counts below its own
+      G.tv[t] = bv;
+      G.tie[t] = make_uint4(ba, brk, bslot, 0u);
+      if (want_best_pair) W.best_pair[t] = bp;  // k_breakdown's way back to the unit
+      const bool displaced = !(ba == li && brk == 0);
+      if (displaced) W.has_dep[t] |= 2;  // only this thread touches the byte now (k_gmark and k_gtask are done)
+      atomicAdd(G.e + x.base + ba, 1u);
+      kk = ord_i64(bv);
     }
-    G.tv[t] = bv;
-    G.tie[t] = make_uint4(ba, brk, bslot, 0u);
-    if (want_best_pair) W.best_pair[t] = bp;  // k_breakdown's way back to the unit
-    const bool displaced = !(ba == li && brk == 0);
-    if (displaced) W.has_dep[t] |= 2;  // only this thread touches the byte now (k_gmark and k_gtask are done)
-    atomicAdd(G.e + x.base + ba, 1u);
     // The distro's value range.  The work list is in task order, so a warp nearly always sits inside one distro: its 32
-    // values are folded with shuffles and ONE lane looks at the distro's pair (instead of every thread polling the same
-    // two L2 lines).
-    const unsigned long long kk = ord_i64(bv);
-    const unsigned act = __activemask();
-    const int d0 = __shfl_sync(act, d, __ffs(act) - 1);
-    if (__all_sync(act, d == d0)) {
-      unsigned long long hi = kk, lo = kk;
+    // values are folded with full-warp shuffles (idle lanes hold the identities 0 / ~0) and ONE lane looks at the
+    // distro's pair (instead of every thread polling the same two L2 lines).  Lane 0 is never idle (kw < n).
+    const int d0 = __shfl_sync(full, d, 0);
+    if (__all_sync(full, d < 0 || d == d0)) {
+      unsigned long long hi = d < 0 ? 0ull : kk, lo = d < 0 ? ~0ull : kk;
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) {
-        const unsigned long long h2 = __shfl_xor_sync(act, hi, o), l2 = __shfl_xor_sync(act, lo, o);
-        const bool other = (act >> ((threadIdx.x & 31) ^ o)) & 1u;  // an exited lane's register is not a value
-        hi = (other && h2 > hi) ? h2 : hi;
-        lo = (other && l2 < lo) ? l2 : lo;
+        hi = max(hi, __shfl_xor_sync(full, hi, o));
+        lo = min(lo, __shfl_xor_sync(full, lo, o));
       }
-      if ((threadIdx.x & 31) == __ffs(act) - 1) {
-        if (hi > __ldcg(G.vmm + 2 * d)) atomicMax(G.vmm + 2 * d, hi);
-        if (lo < __ldcg(G.vmm + 2 * d + 1)) atomicMin(G.vmm + 2 * d + 1, lo);
+      if (lane == 0) {
+        if (hi > __ldcg(G.vmm + 2 * d0)) atomicMax(G.vmm + 2 * d0, hi);
+        if (lo < __ldcg(G.vmm + 2 * d0 + 1)) atomicMin(G.vmm + 2 * d0 + 1, lo);
       }
-    } else {
+    } else if (d >= 0) {
       if (kk > __ldcg(G.vmm + 2 * d)) atomicMax(G.vmm + 2 * d, kk);
       if (kk < __ldcg(G.vmm + 2 * d + 1)) atomicMin(G.vmm + 2 * d + 1, kk);
     }

@@ -1059,7 +1059,8 @@ int upload_tasks(evg_ctx* c, const evg_task_soa* t, const evg_distro_table* dt, 
     CK(c->b_unitmask.ensure(sizeof(uint64_t) * size_t(U + 1)));
     CK(c->b_bestpair.ensure(sizeof(uint32_t) * size_t(T + 1)));
   }
-  if (on_chip_cta) CK(c->b_kv.ensure(sizeof(uint64_t) * size_t(T + 1)));  // k_plan_smem's scratch for value ranges above 32 bits
+  // k_plan_smem's scratch for value ranges above 32 bits; a breakdown run plans the tiny distros with it too
+  if (on_chip_cta || !listW.empty()) CK(c->b_kv.ensure(sizeof(uint64_t) * size_t(T + 1)));
   if (n_general > 0) {  // the general path's buffers exist only when a distro takes it
     for (int k = 0; k < 2; k++) {
       CK(c->b_klo[k].ensure(sizeof(uint32_t) * size_t(T + 1)));

@@ -258,6 +258,148 @@ def make(sizes: np.ndarray, seed: int, *, name: str = "synthetic", now: int = NO
     return Workload(name, now, tasks, distros, hosts)
 
 
+# ---------------------------------------------------------------- edge values
+# make() stays inside the domain of the kernels' 32-bit scorer (evg_score.cuh: factors below 2^14, priority and
+# NumDependents below 2^15, time in queue and expected duration below 2^50 ns, a clock and bases at or after 1970).
+# sprinkle_edges() overwrites rows of a tick with values at and beyond those limits -- and with the values production
+# does produce: compile tasks with thousands of dependents, stale patches, admin priorities, clock skew, epoch-zero
+# times, TotalValue wrapping int64 (DESIGN.md §3).
+I64_MAX = 2 ** 63 - 1
+FAST_LIMIT_NS = (1 << 15) * M.MINUTE  # evg_score.cuh kFastLimit: 2^15 minutes
+WEEK_NS = 7 * 24 * M.HOUR
+EDGE_SALT = 0x3DCE0D6E
+
+EDGE_VALUES = {
+    "nd": [-1, 32, 63, 64, 65, 2 ** 15 - 1, 2 ** 15, 2 ** 31 - 1],                    # NumDependents
+    "prio": [-2 ** 31, -1, 2 ** 15 - 1, 2 ** 15, 2 ** 31 - 1],                        # priority
+    "tiq": [2 ** 50 - 1, 2 ** 50, FAST_LIMIT_NS - 1, FAST_LIMIT_NS + 1, WEEK_NS - 1,  # time in queue (basis = now - tiq)
+            WEEK_NS + 1, 0, FAST_LIMIT_NS],
+    "basis": ["now+1", 0, -2 ** 63 + 1, M.ZERO_TIME],                                 # queue and wait basis
+    # expected duration; 2^62 + 1 twice in a distro wraps its int64 expected-duration sums
+    "exp": [2 ** 50 - 1, 2 ** 50, FAST_LIMIT_NS - 1, FAST_LIMIT_NS, FAST_LIMIT_NS + 1, -1, 0, 2 ** 62 + 1],
+    "thresh": [-1, 0, 1],                                                             # offset from the distro's target time
+    "u32": ["high", "low"],   # TotalValue 2^32 + 401 (merge queue, priority 2^31 - 1) and 2: a range of 33 bits
+    "wrap": ["neg", "pos"],   # TotalValue wrapped to below -2^62 / above 2^62: a range beyond 2^63
+}
+ROW_KINDS = tuple(EDGE_VALUES)
+# distro-level knobs, dealt to the distros in turn (None: left as make() drew it)
+EDGE_FACTORS = [None, 2 ** 14 - 1, None, 0, None, -5, 2 ** 14]   # the seven integer factors (<= 0 clamps to 1)
+EDGE_NDF = [None, 2.5, 7.0, 2.0 ** 27 + 0.5, 2 ** 14 - 1.0, 0.01]  # NumDependentsFactor; 2^27+.5: table entries pass 2^32 at n = 32
+DISTRO_KINDS = ("factors", "ndf", "clock")
+_INT_FACTORS = ("patch_factor", "patch_time_in_queue_factor", "commit_queue_factor", "mainline_time_in_queue_factor",
+                "expected_runtime_factor", "generate_task_factor", "stepback_task_factor")
+
+
+def _wrap64(x: int) -> int:
+    return (x + 2 ** 63) % 2 ** 64 - 2 ** 63
+
+
+def _floor_minutes(d: int) -> int:
+    """int64(math.Floor(time.Duration(d).Minutes())) for d >= 0 (the stdlib's two-term FP64 formula)."""
+    return int(np.floor(float(d // M.MINUTE) + float(d % M.MINUTE) / (60 * 1e9)))
+
+
+def _wrapping_expected(cfg, negative: bool) -> int:
+    """An expected duration (whole minutes) at which a lone patch task of priority 2^31 - 1 with the generator flag, a
+    saturated time in queue and no dependents has TotalValue (unitInfo.value, planner.go:209-300) in
+    [-2^62 - 2^61, -2^62) (negative) or in [2^62 + 2^60, 2^63).  Each minute moves the wrapped value by
+    2^31 * GenerateTaskFactor * ExpectedRuntimeFactor (2^37.6 or more), so some minute below 2^64 / that step
+    (< 1.6e8 minutes, inside int64 nanoseconds) lands in the window."""
+    f = {k: (int(cfg[k]) if int(cfg[k]) > 0 else 1) for k in _INT_FACTORS}
+    prio = 2 ** 31 * f["generate_task_factor"]
+    a = prio * (1 + f["patch_factor"] + f["patch_time_in_queue_factor"] * _floor_minutes(I64_MAX)) + 1
+    step = prio * f["expected_runtime_factor"]
+    lo, hi = (-2 ** 62 - 2 ** 61, -2 ** 62) if negative else (2 ** 62 + 2 ** 60, 2 ** 63)
+    m = -(-((lo - a) % 2 ** 64) // step)
+    assert lo <= _wrap64(a + step * m) < hi and m * M.MINUTE <= I64_MAX
+    return m * M.MINUTE
+
+
+def sprinkle_edges(w: Workload, seed: int, *, kinds, frac: Optional[float] = None, positions=None) -> dict:
+    """Overwrite rows of `w` in place with edge values.  Row kinds (EDGE_VALUES) are dealt to the chosen rows in turn,
+    each kind's values in turn; the distro kinds ("factors", "ndf", "clock") set distro d's knob to entry d of their
+    list.  Rows: `positions` (global row indices), else a `frac` of all rows, else one in 32.  A stream of its own, so
+    make() draws the same tick for every seed whether or not edges are sprinkled afterwards.  Group ids, versions and
+    dependency edges are left alone: the tick stays valid.  Returns {kind: global rows it wrote}."""
+    rng = Rng(seed ^ EDGE_SALT)
+    t, dt = w.tasks, w.distros
+    cfg = dt.cfg
+    D = dt.n_distros
+    kinds = tuple(kinds)
+    unknown = [k for k in kinds if k not in EDGE_VALUES and k not in DISTRO_KINDS]
+    if unknown:
+        raise ValueError(f"unknown edge kinds {unknown}")
+    now = int(w.now)
+    for d in range(D):
+        if "factors" in kinds and EDGE_FACTORS[d % len(EDGE_FACTORS)] is not None:
+            for f in _INT_FACTORS:
+                cfg[f][d] = EDGE_FACTORS[d % len(EDGE_FACTORS)]
+        if "ndf" in kinds and EDGE_NDF[d % len(EDGE_NDF)] is not None:
+            cfg["num_dependents_factor"][d] = EDGE_NDF[d % len(EDGE_NDF)]
+        if "clock" in kinds and d % 3 == 2:
+            cfg["target_time_ns"][d] = now + M.HOUR  # a threshold in the future: the literal time.Since comparison
+    row_kinds = [k for k in kinds if k in EDGE_VALUES]
+    out = {k: [] for k in row_kinds}
+    if not row_kinds or t.n_tasks == 0:
+        return {k: np.zeros(0, np.int64) for k in out}
+    if positions is not None:
+        rows = np.unique(np.asarray(positions, dtype=np.int64))
+    else:
+        rows = np.nonzero(rng.uniform(t.n_tasks) < (frac if frac is not None else 1.0 / 32))[0]
+    distro_of = np.searchsorted(dt.task_off, rows, side="right") - 1
+    aim = {}  # (distro, sign) -> expected duration that wraps TotalValue to that sign
+    for j, (r, d) in enumerate(zip(rows.tolist(), distro_of.tolist())):
+        kind = row_kinds[j % len(row_kinds)]
+        vals = EDGE_VALUES[kind]
+        v = vals[(j // len(row_kinds)) % len(vals)]
+        if kind == "u32" and (t.group_id[r] >= 0 or cfg["group_versions"][d]):
+            continue  # a lone task's value: a unit's would add its other members' terms
+        out[kind].append(r)
+        if kind == "nd":
+            t.num_dependents[r] = v
+        elif kind == "prio":
+            t.priority[r] = v
+        elif kind == "tiq":
+            t.queue_basis_ns[r] = now - v
+        elif kind == "basis":
+            b = now + 1 if v == "now+1" else v
+            t.queue_basis_ns[r] = b
+            t.wait_basis_ns[r] = b
+        elif kind == "exp":
+            t.expected_ns[r] = v
+        elif kind == "thresh":
+            target = int(cfg["target_time_ns"][d])
+            t.wait_basis_ns[r] = _wrap64(now - target + v)
+            t.expected_ns[r] = target + v
+            t.flags[r] |= L.EVG_TF_DEPS_MET
+        elif kind == "u32":
+            keep = int(t.flags[r]) & (L.EVG_TF_DEPS_MET | L.EVG_TF_OTHER_DISTRO)
+            cfg["commit_queue_factor"][d] = 1
+            cfg["num_dependents_factor"][d] = 0.0
+            t.num_dependents[r] = 0
+            t.expected_ns[r] = 0
+            if v == "high":  # (1 + 2^31 - 1 + 200) * (1 + CommitQueueFactor) + 1
+                t.priority[r] = 2 ** 31 - 1
+                t.flags[r] = keep | L.EVG_TF_REQ_MERGE_QUEUE
+            else:            # mainline, waited over a week: 1 * 1 + 1
+                t.priority[r] = -1
+                t.flags[r] = keep | L.EVG_TF_REQ_OTHER
+                t.queue_basis_ns[r] = now - 2 * WEEK_NS
+        elif kind == "wrap":
+            # priority 2^31 - 1 times GenerateTaskFactor 100, times a rank that holds the saturated time.Since of a basis
+            # at the start of int64: the product wraps; the expected duration aims the wrap at the wanted sign
+            keep = int(t.flags[r]) & (L.EVG_TF_DEPS_MET | L.EVG_TF_OTHER_DISTRO)
+            cfg["generate_task_factor"][d] = 100
+            if (d, v) not in aim:
+                aim[(d, v)] = _wrapping_expected(cfg[d], v == "neg")
+            t.priority[r] = 2 ** 31 - 1
+            t.flags[r] = keep | L.EVG_TF_REQ_PATCH | L.EVG_TF_GENERATE
+            t.queue_basis_ns[r] = -2 ** 63 + 1
+            t.num_dependents[r] = 0
+            t.expected_ns[r] = aim[(d, v)]
+    return {k: np.asarray(v, dtype=np.int64) for k, v in out.items()}
+
+
 def power_law_sizes(rng: Rng, D: int, alpha: float = 1.2, lo: int = 1, hi: int = 1_000_000) -> np.ndarray:
     u = np.maximum(rng.uniform(D), 1e-12)
     return np.floor(lo * u ** (-1.0 / alpha)).clip(lo, min(hi, L.MAX_TASKS_PER_DISTRO)).astype(np.int64)

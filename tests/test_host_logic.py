@@ -216,6 +216,188 @@ def test_score_fast_paths_equal_the_fp64_formulas(tmp_path):
     assert "mismatches 0" in out, out
 
 
+# ---------------------------------------------------------------- the scorer's warp votes, restated
+FAST_LIMIT = np.uint64((1 << 15) * M.MINUTE)
+
+
+def scorer_domains(w):
+    """numpy restatement of the kernels' per-task domain tests (evg_score.cuh): `bad32` is score32_bad != 0 with the
+    NumDependents term resolved as k_gtask / k_plan_cta do (the per-distro table int64(factor * n) for n < 64, capped
+    at 2^29; factor * n with an integral factor below 2^14 for 64 <= n < 2^15; else not representable); `fast` is
+    score_fast_domain.  Also per distro: Factors32::ok_base (the 32-bit vote can pass) and the 64-bit fast form's
+    preconditions."""
+    t, dt, now = w.tasks, w.distros, int(w.now)
+    cfg, D = dt.cfg, dt.n_distros
+    sizes = np.diff(dt.task_off)
+    distro_of = np.repeat(np.arange(D), sizes)
+    ints = np.stack([np.where(cfg[f] > 0, cfg[f], 1) for f in synth._INT_FACTORS])
+    ok_base = (now >= 0) & np.all(ints < 2 ** 14, axis=0)
+    ndf = np.where(cfg["num_dependents_factor"] > 0, cfg["num_dependents_factor"], 1.0)
+    nd_int = np.where((ndf < 2.0 ** 20) & (ndf == np.trunc(ndf)), np.trunc(ndf), 0).astype(np.int64)
+    ok = ok_base & (nd_int != 0) & (nd_int < 2 ** 14)
+    entry = np.trunc(ndf[:, None] * np.arange(64, dtype=np.float64)[None, :])
+    table = np.where((entry >= 0) & (entry < 2 ** 29), entry, 0xFFFFFFFF).astype(np.int64)
+    ndc = np.maximum(t.num_dependents, 0).astype(np.int64)
+    mul = np.where(ok[distro_of] & (ndc < 2 ** 15), nd_int[distro_of] * ndc, 0xFFFFFFFF)
+    nd_term = np.where(ndc < 64, table[distro_of, np.minimum(ndc, 63)], mul)
+    qb = t.queue_basis_ns
+    with np.errstate(over="ignore"):
+        tiq = np.where(qb == M.ZERO_TIME, np.uint64(0), np.uint64(now % 2 ** 64) - qb.view(np.uint64))
+    ex = t.expected_ns.view(np.uint64)
+    bad32 = (((tiq | ex) >> np.uint64(50)) != 0) | ((np.maximum(t.priority, 0) >> 15) != 0) | ((nd_term >> 29) != 0)
+    fast = ((qb == M.ZERO_TIME) | ((qb >= 0) & (tiq < FAST_LIMIT))) & (ex < FAST_LIMIT)
+    fast_clock = np.full(D, now >= 0) & (nd_int != 0)
+    return distro_of, bad32, fast, ok_base, fast_clock
+
+
+def scoring_tasks(w, route):
+    """Tasks that vote: those whose own unit is {the task} (the rest are scored as units)."""
+    t, dt = w.tasks, w.distros
+    D = dt.n_distros
+    sizes = np.diff(dt.task_off)
+    distro_of = np.repeat(np.arange(D), sizes)
+    has_dependents = np.zeros(t.n_tasks, dtype=bool)
+    edges = np.zeros(D, dtype=bool)
+    if t.n_edges:
+        owner = np.repeat(np.arange(t.n_tasks), np.diff(t.dep_off))
+        has_dependents[dt.task_off[distro_of[owner]] + t.dep_idx] = True
+        edges = np.bincount(distro_of[owner], minlength=D) > 0
+    gv = dt.cfg["group_versions"] != 0
+    complex_distro = (np.diff(dt.group_off) > 0) | gv | edges
+    if route == "warp":  # k_plan_warp votes only in distros without multi-member units
+        return ~complex_distro[distro_of]
+    return ~(complex_distro[distro_of] & ((t.group_id >= 0) | gv[distro_of] | has_dependents))
+
+
+def vote_groups(w, route):
+    """Per task: the (distro, warp vote) it takes part in, as one integer, for each kernel's lane layout.
+      k_plan_warp  one warp per distro
+      k_plan_smem  task i of a distro is lane i % 32 of a warp covering tasks 32*(i // 32) ..
+      k_plan_cta   tile k holds slots a0 + k*2*THREADS .., a0 = the distro's first task rounded down to a multiple of 4;
+                   slot j of a tile is lane j % 32 of warp (j % THREADS) // 32, whose vote spans both THREADS halves
+      k_gtask      2048-slot tiles from a0; thread q of half u owns slots 4*(u*256 + q) .. +3: a warp votes on 128
+                   consecutive slots"""
+    import test_gpu_score_edges as E
+    dt = w.distros
+    sizes = np.diff(dt.task_off)
+    distro_of = np.repeat(np.arange(dt.n_distros), sizes)
+    s = np.arange(w.n_tasks, dtype=np.int64)
+    a = dt.task_off[distro_of]
+    rel = s - (a & ~3)
+    if route == "warp":
+        g = np.zeros_like(s)
+    elif route == "smem":
+        g = (s - a) // 32
+    elif route == "cta":
+        th = np.array([E.cta_threads(int(n)) for n in sizes], dtype=np.int64)[distro_of]
+        g = (rel // (2 * th)) * 64 + (rel % th) // 32
+    else:
+        g = rel // E.GTASK_WARP
+    return distro_of * (1 << 24) + g
+
+
+def mixed_votes(w, route):
+    """Number of warp votes on `route` where some voting tasks are inside the scorer's domain and some are not --
+    the votes that send in-domain tasks down a fallback."""
+    distro_of, bad32, fast, ok_base, fast_clock = scorer_domains(w)
+    if route in ("cta", "general"):
+        out, live = bad32, ok_base[distro_of]
+    else:
+        out, live = ~fast, fast_clock[distro_of]
+    sel = scoring_tasks(w, route) & live
+    g = vote_groups(w, route)[sel]
+    o = out[sel]
+    if g.size == 0:
+        return 0
+    ids, inv = np.unique(g, return_inverse=True)
+    n_out = np.bincount(inv, weights=o.astype(np.float64))
+    n_all = np.bincount(inv)
+    return int(((n_out > 0) & (n_out < n_all)).sum())
+
+
+@pytest.mark.parametrize("route", ["warp", "cta", "smem", "general"])
+def test_score_edge_ticks_hold_mixed_warps(route):
+    """Every edge tick of test_gpu_score_edges.py (except the `thresh` kind, whose values are inside the domain by
+    design) holds mixed warp votes on its route, and its edges reach task-group members (and GroupVersions members
+    where the route has such distros); the undisturbed ticks hold none -- so the GPU tests cannot drift back into the
+    32-bit scorer's domain unnoticed."""
+    import test_gpu_score_edges as E
+    assert mixed_votes(E._route_tick(route, 500), route) == 0
+    # the 64-bit fast form of k_plan_warp / k_plan_smem takes any priority and NumDependents: only times leave its domain
+    leaves = ("tiq", "basis", "exp", "wrap") if route in ("warp", "smem") else tuple(k for k in E.KINDS if k != "thresh")
+    for density in E.DENSITIES:
+        for kind in E.KINDS:
+            w = E.edge_tick(route, kind, density)
+            if kind in leaves:
+                assert mixed_votes(w, route) > 0, (route, kind, density)
+            seed = 500 + 17 * E.ROUTES.index(route) + E.KINDS.index(kind)
+            base = E._route_tick(route, seed)
+            changed = np.zeros(w.n_tasks, dtype=bool)
+            for name, _ in w.tasks.COLUMNS:
+                changed |= getattr(w.tasks, name) != getattr(base.tasks, name)
+            assert changed.any(), (route, kind, density)
+            if kind == "u32":  # lone tasks only: the value of a unit would add its other members' terms
+                continue
+            assert (changed & (w.tasks.group_id >= 0)).any(), (route, kind, density)
+            gv = (w.distros.cfg["group_versions"] != 0)[np.repeat(np.arange(w.distros.n_distros), np.diff(w.distros.task_off))]
+            if route != "cta":  # k_plan_cta plans no GroupVersions distro
+                assert (changed & gv).any(), (route, kind, density)
+
+
+def test_scorer_domain_restatement_sees_each_limit():
+    """The restatement flags exactly the values past each limit of score32_bad."""
+    w = synth.make(np.array([40]), 3, tg_frac=0.0)
+    t, now = w.tasks, w.now
+    t.num_dependents[:] = 1
+    t.priority[:] = 0
+    t.expected_ns[:] = M.MINUTE
+    t.queue_basis_ns[:] = now
+    t.queue_basis_ns[1], t.queue_basis_ns[2] = now - (2 ** 50 - 1), now - 2 ** 50
+    t.expected_ns[3], t.expected_ns[4], t.expected_ns[5] = 2 ** 50 - 1, 2 ** 50, -1
+    t.priority[6], t.priority[7], t.priority[8] = 2 ** 15 - 1, 2 ** 15, -2 ** 31
+    t.num_dependents[9], t.num_dependents[10] = 2 ** 15 - 1, 2 ** 15
+    t.queue_basis_ns[11], t.queue_basis_ns[12] = now + 1, M.ZERO_TIME
+    w.distros.cfg["num_dependents_factor"] = 7.0
+    w.distros.cfg["patch_factor"] = 0
+    _, bad, fast, ok_base, _ = scorer_domains(w)
+    assert bool(ok_base[0])
+    assert np.nonzero(bad[:13])[0].tolist() == [2, 4, 5, 7, 10, 11]  # 7 * (2^15 - 1) < 2^29; 7 * 2^15 needs n < 2^15
+    w.distros.cfg["num_dependents_factor"] = 2.5  # fractional: only the table (n < 64) keeps the 32-bit form
+    _, bad, _, _, _ = scorer_domains(w)
+    assert np.nonzero(bad[:13])[0].tolist() == [2, 4, 5, 7, 9, 10, 11]
+    w.distros.cfg["num_dependents_factor"] = 2.0 ** 27 + 0.5  # table entries reach 2^29 at n = 4
+    t.num_dependents[13:16] = [3, 4, 32]
+    _, bad, _, _, _ = scorer_domains(w)
+    assert bad[14] and bad[15] and not bad[13]
+
+
+def test_sprinkle_edges_keeps_make_and_the_tick_valid():
+    """The injector draws from a stream of its own (make() is unchanged for every seed), writes every value of every
+    kind, and leaves group ids, versions and TaskGroupMaxHosts alone."""
+    a = synth.make(np.array([300, 2000, 40]), 12, tg_frac=0.2, zipf_priority=True)
+    b = synth.make(np.array([300, 2000, 40]), 12, tg_frac=0.2, zipf_priority=True)
+    written = synth.sprinkle_edges(b, 12, kinds=synth.ROW_KINDS + synth.DISTRO_KINDS, frac=0.5)
+    c = synth.make(np.array([300, 2000, 40]), 12, tg_frac=0.2, zipf_priority=True)
+    for name, _ in a.tasks.COLUMNS:
+        assert np.array_equal(getattr(a.tasks, name), getattr(c.tasks, name))
+    for name in ("group_id", "version_id", "task_group_order"):
+        assert np.array_equal(getattr(a.tasks, name), getattr(b.tasks, name))
+    assert np.array_equal(a.distros.group_max_hosts, b.distros.group_max_hosts)
+    t = b.tasks
+    assert set(synth.EDGE_VALUES["nd"]) <= set(t.num_dependents[written["nd"]].tolist())
+    assert set(synth.EDGE_VALUES["prio"]) <= set(t.priority[written["prio"]].tolist())
+    assert set(synth.EDGE_VALUES["exp"]) <= set(t.expected_ns[written["exp"]].tolist())
+    assert {b.now - v for v in synth.EDGE_VALUES["tiq"]} <= set(t.queue_basis_ns[written["tiq"]].tolist())
+    assert {b.now + 1, 0, -2 ** 63 + 1, M.ZERO_TIME} <= set(t.queue_basis_ns[written["basis"]].tolist())
+    assert int(b.distros.cfg["target_time_ns"][2]) > b.now
+    # marshal_tasks takes the int32 edges and refuses what does not fit
+    d = M.Distro(id="d")
+    soa, _, _ = S.marshal_tasks([(d, [M.Task(id="t", num_dependents=2 ** 31 - 1, priority=-2 ** 31)])], NOW)
+    assert soa.num_dependents.tolist() == [2 ** 31 - 1]
+    with pytest.raises(ValueError):
+        S.marshal_tasks([(d, [M.Task(id="t", num_dependents=2 ** 31)])], NOW)
+
+
 def test_marshal_runnable_bits():
     """soa.marshal_runnable: the byte columns of evg_runnable_in against the reference's field semantics."""
     from evergreen_b200 import _lib as L
