@@ -4,10 +4,12 @@
 // segmented LSD radix sort (20 B/task each way per pass).  This one:
 //   k_gtask        per 2048-task tile: 128-bit column loads, 32-bit scoring (single_task_value32) where the
 //                  distro allows it, queue-info sums folded per tile, TotalValue of single-task units, per-distro
-//                  value range; tasks of multi-member units are linked and compacted into a work list
-//   k_gunit/k_gbest  per work-list task: the member at the head of a unit's list computes Unit.info / value / anchor once;
-//                  then every task makes its first-occurrence choice (planner.go:467-477) and walks the chosen unit
-//                  for its rank; anchor histogram e[]
+//                  value range; tasks of multi-member units are compacted into a work list of packed entries (unit
+//                  slots + member payload, written from registers)
+//   k_glink/k_galloc/k_gfill  the unit table: every membership draws its place in its unit's run of entry ids
+//   k_gunit/k_grank  per unit: Unit.info / value / anchor, and every member's rank in the unit, once
+//   k_gbest        per work-list task: its first-occurrence choice (planner.go:467-477) and that unit's rank of it;
+//                  anchor histogram e[]
 //   k_gsum/k_gscan/k_gplace(+_disp)
 //                  canonical pre-arrangement by COUNTING instead of sorting tie bytes: an exclusive scan of e[] over
 //                  the distro gives every anchor's run start; tasks are written to (key, index) buffers in
@@ -59,14 +61,24 @@ struct DGen {
   uint32_t* e;                 // [T] anchor histogram, then exclusive positions
   uint32_t* tile_sum;          // [NT] sum of e over the tile, then the tile's exclusive offset inside its distro
   uint32_t* tile_hist;         // [NT*256]
-  uint32_t* clist;             // work list: global task index of every task that touches a multi-member unit
-  int32_t* clist_d;            // its distro
-  unsigned int* ccount;        // [1]
-  uint4* tie;                  // [T] work-list tasks: x = anchor of the unit the task is emitted from, y = rank inside it,
+  uint4* wl;                   // work list, one entry per task that touches a multi-member unit: x = global task index,
+                               //     y = distro, z = global slot of its own-key unit (kInactive: not a member of it),
+                               //     w = global slot of its version unit (kInactive: none)
+  struct URec* pay;            // [work list] the entry's member payload (what k_gunit and k_gbest ask of a member)
+  unsigned int* ccount;        // [1] work-list entries
+  uint4* tie;                  // [work list] x = anchor of the unit the task is emitted from, y = rank inside it,
                                //     z = that unit's slot (kInactive: its own single-task unit)
   int32_t* maxpass;            // [1]
-  struct URec* rec;            // unit table: the members of every multi-member unit, one contiguous run per unit
-  unsigned int* rcount;        // [1] records reserved
+  uint32_t* run;               // unit table: the members of every multi-member unit as work-list entry ids (bit 31: an
+                               //     own-key membership), one contiguous run per unit
+  uint32_t* pown;              // [work list] place of the entry's own-key membership in its unit's run
+  uint32_t* pver;              // [work list] place of its version membership
+  uint32_t* pedge;             // [E] place of the edge's dependency membership
+  uint32_t* sedge;             // [E] unit slot of that membership (kInactive: the task already joined that unit)
+  uint32_t* rank;              // [run positions] the member's rank inside its unit (TaskList.Less)
+  unsigned int* rcount;        // [1] run positions reserved
+  uint2* blist;                // units above kRankOne members, in 32-member chunks: x = slot, y = chunk (k_grank ranks them)
+  unsigned int* bcount;        // [1]
   uint4* usum;                 // [unit slots] what k_gbest asks of a candidate unit, in one 16-byte load: x|y<<32 = TotalValue, z = anchor
                                //     (kNoAnchor: never exported), w = members
   uint2* hlist;                // multi-member units of the tick: x = slot, y = distro (k_galloc lists them, k_gunit folds them)
@@ -80,9 +92,33 @@ __device__ __forceinline__ int gen_bits(const DGen& G, int d) {  // significant 
 }
 __device__ __forceinline__ int gen_npass(int bits) { return (bits + 7) >> 3; }
 
+// A work-list entry's member payload: the fields Unit.info, the in-unit order and TaskGroupInfo need.
+struct __align__(16) URec {
+  int32_t prio, nd;
+  int64_t exp_ns, qb;
+  int32_t tgo;
+  uint32_t lif;  // bits 0..20 distro-local task index, 22 group_id >= 0, 23 wait over threshold (k_gtask's verdict),
+                 // 24..29 task flags
+};
+static_assert(sizeof(URec) == 32, "one L2 sector per member");
+constexpr uint32_t kRecGrouped = 1u << 22, kRecWaitOver = 1u << 23;
+constexpr uint32_t kRunOwn = 1u << 31, kRunEntry = kRunOwn - 1u;  // a run position: entry id | own-key membership
+__device__ __forceinline__ uint32_t rec_li(const URec& r) { return r.lif & 0x1FFFFFu; }
+__device__ __forceinline__ URec rec_load(const URec* p) {  // two 128-bit loads
+  const uint4 a = reinterpret_cast<const uint4*>(p)[0], b = reinterpret_cast<const uint4*>(p)[1];
+  URec r;
+  r.prio = int32_t(a.x); r.nd = int32_t(a.y); r.exp_ns = int64_t((unsigned long long)a.z | ((unsigned long long)a.w << 32));
+  r.qb = int64_t((unsigned long long)b.x | ((unsigned long long)b.y << 32)); r.tgo = int32_t(b.z); r.lif = b.w;
+  return r;
+}
+__device__ __forceinline__ void rec_store(URec* p, const URec& r) {
+  reinterpret_cast<uint4*>(p)[0] = make_uint4(uint32_t(r.prio), uint32_t(r.nd), uint32_t(uint64_t(r.exp_ns)), uint32_t(uint64_t(r.exp_ns) >> 32));
+  reinterpret_cast<uint4*>(p)[1] = make_uint4(uint32_t(uint64_t(r.qb)), uint32_t(uint64_t(r.qb) >> 32), uint32_t(r.tgo), r.lif);
+}
+
 __global__ void k_ginit(DGen G, const int32_t* __restrict__ general_list, int n) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
-  if (k == 0) { *G.ccount = 0u; *G.maxpass = 0; *G.rcount = 0u; *G.hcount = 0u; }
+  if (k == 0) { *G.ccount = 0u; *G.maxpass = 0; *G.rcount = 0u; *G.hcount = 0u; *G.bcount = 0u; }
   if (k >= n) return;
   const int d = general_list[k];
   G.vmm[2 * d] = 0ull;
@@ -128,6 +164,7 @@ __global__ void __launch_bounds__(256, EVG_GTASK_OCC) k_gtask(DTasks T, DDistros
   const int64_t base = D.task_off[d], end = D.task_off[d + 1];
   const int64_t ts = G.tile_start[tile];
   const uint32_t ng = uint32_t(D.group_off[d + 1] - D.group_off[d]);
+  const uint32_t ub = uint32_t(D.unit_base[d]);
   const bool gv = cfg.group_versions != 0;
   const int64_t threshold = cfg.target_time_ns;
   const PlannerFactors pf = clamp_factors(cfg);
@@ -146,14 +183,18 @@ __global__ void __launch_bounds__(256, EVG_GTASK_OCC) k_gtask(DTasks T, DDistros
   unsigned int c_dm = 0, c_mq = 0, c_over = 0, c_wait = 0, c_sec = 0, c_ung = 0, c_ucnt = 0, c_uover = 0, c_uwait = 0, c_umq = 0;
   int64_t s_exp = 0, s_over = 0, s_uexp = 0, s_uover = 0;
   unsigned long long kmax = 0ull, kmin = ~0ull;
-  uint32_t cmask = 0;  // bit 4*u + m: task ts + 4*(u*256 + tid) + m goes on the work list
 
 #pragma unroll 1
   for (int u = 0; u < 2; u++) {
     const int64_t t4 = ts + 4 * int64_t(u * 256 + tid);  // multiple of 4: 16-byte aligned in every column
     const bool live = t4 < end;  // the columns are readable 8 slots past the last task (upload pads them)
-    int4 prio4 = make_int4(0, 0, 0, 0), nd4 = prio4, gid4 = make_int4(-1, -1, -1, -1);
+    int4 prio4 = make_int4(0, 0, 0, 0), nd4 = prio4, gid4 = make_int4(-1, -1, -1, -1), tgo4 = prio4, vid4 = prio4;
     uint4 fl4 = make_uint4(0, 0, 0, 0);
+    uint32_t cmask = 0, womask = 0;  // bit m: task t4 + m goes on the work list / its wait is over the threshold
+    if (live && dcomplex) {  // what only the work list's payload needs
+      tgo4 = *reinterpret_cast<const int4*>(T.tgo + t4);
+      if (gv) vid4 = *reinterpret_cast<const int4*>(T.vid + t4);
+    }
     longlong2 ex01 = make_longlong2(0, 0), ex23 = ex01, qb01 = ex01, qb23 = ex01, wb01 = ex01, wb23 = ex01;
     if (live) {
       prio4 = *reinterpret_cast<const int4*>(T.priority + t4);
@@ -217,7 +258,8 @@ __global__ void __launch_bounds__(256, EVG_GTASK_OCC) k_gtask(DTasks T, DDistros
       wr_v[m] = scores;
       solo[m] = scores & !complex_task;  // final: the task is emitted from its own unit
       eout[m] = (valid & !complex_task) ? 1u : 0u;
-      cmask |= (complex_task ? 1u : 0u) << (4 * u + m);
+      cmask |= (complex_task ? 1u : 0u) << m;
+      womask |= (wait_over ? 1u : 0u) << m;
     }
     if (f32.ok_base && __all_sync(full, dom)) {  // one warp vote per four tasks; the 64-bit scorers stay out of line
 #pragma unroll
@@ -250,31 +292,44 @@ __global__ void __launch_bounds__(256, EVG_GTASK_OCC) k_gtask(DTasks T, DDistros
           if (t4 + m >= base && t4 + m < end) G.e[t4 + m] = eout[m];
       }
     }
-  }
-  // Work list: ONE global atomic per tile (a block scan of the per-thread counts gives every entry its place) -- an
-  // atomic per warp and task slot serialised every tile of the tick on one L2 address.
-  if (dcomplex) {
-    __shared__ uint32_t s_wsum[8];
-    __shared__ uint32_t s_lbase;
-    const uint32_t mine = __popc(cmask);
-    uint32_t inc = mine;
+    // Work list: ONE global atomic per half tile (a block scan of the per-thread counts gives every entry its
+    // place) -- an atomic per warp and task slot serialised every tile of the tick on one L2 address.  The entry carries
+    // what every later kernel asks of the task (its unit slots and member payload), written here from registers, so
+    // that those kernels read it coalesced instead of gathering the columns again.
+    if (dcomplex) {  // block-uniform
+      __shared__ uint32_t s_wsum[8];
+      __shared__ uint32_t s_lbase;
+      const uint32_t mine = __popc(cmask);
+      uint32_t inc = mine;
 #pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const uint32_t x = __shfl_up_sync(full, inc, o); if (lane >= o) inc += x; }
-    if (lane == 31) s_wsum[tid >> 5] = inc;
-    __syncthreads();
-    uint32_t before = 0, total = 0;
-#pragma unroll
-    for (int w = 0; w < 8; w++) { const uint32_t x = s_wsum[w]; before += w < (tid >> 5) ? x : 0u; total += x; }
-    if (total) {  // block-uniform
-      if (tid == 0) s_lbase = atomicAdd(G.ccount, total);
+      for (int o = 1; o < 32; o <<= 1) { const uint32_t x = __shfl_up_sync(full, inc, o); if (lane >= o) inc += x; }
+      if (lane == 31) s_wsum[tid >> 5] = inc;
       __syncthreads();
-      uint32_t pos = s_lbase + before + inc - mine;
-      for (uint32_t b = cmask; b; b &= b - 1u) {
-        const int bit = __ffs(b) - 1;
-        G.clist[pos] = uint32_t(ts + 4 * int64_t((bit >> 2) * 256 + tid) + (bit & 3));
-        G.clist_d[pos] = d;
-        pos++;
+      uint32_t before = 0, total = 0;
+#pragma unroll
+      for (int w = 0; w < 8; w++) { const uint32_t x = s_wsum[w]; before += w < (tid >> 5) ? x : 0u; total += x; }
+      if (total) {  // block-uniform
+        if (tid == 0) s_lbase = atomicAdd(G.ccount, total);
+        __syncthreads();
+        uint32_t pos = s_lbase + before + inc - mine;
+        const int32_t vid_[4] = {vid4.x, vid4.y, vid4.z, vid4.w}, tgo_[4] = {tgo4.x, tgo4.y, tgo4.z, tgo4.w};
+#pragma unroll
+        for (int m = 0; m < 4; m++) {
+          if (!((cmask >> m) & 1u)) continue;
+          const uint32_t t = uint32_t(t4 + m), li = uint32_t(t4 + m - base);
+          const int32_t gid = gid_[m], vid = vid_[m];
+          const bool own_complex = (gid >= 0) | gv | (((hd4 >> (8 * m)) & 0xFFu) != 0);
+          const uint32_t s_own = own_complex ? ub + own_slot_local(gid, vid, li, ng, gv) : kInactive;
+          const uint32_t s_ver = (gid >= 0 && gv) ? ub + ng + uint32_t(vid) : kInactive;
+          G.wl[pos] = make_uint4(t, uint32_t(d), s_own, s_ver);
+          URec r;
+          r.prio = prio_[m]; r.nd = nd_[m]; r.exp_ns = ex_[m]; r.qb = qb_[m]; r.tgo = tgo_[m];
+          r.lif = li | (gid >= 0 ? kRecGrouped : 0u) | (((womask >> m) & 1u) ? kRecWaitOver : 0u) | ((fl_[m] & 0x3Fu) << 24);
+          rec_store(G.pay + pos, r);
+          pos++;
+        }
       }
+      __syncthreads();  // s_wsum / s_lbase are rewritten by the next half
     }
   }
   // fold: warp, then block (shared atomics), then one set of global atomics per tile
@@ -325,82 +380,69 @@ __global__ void __launch_bounds__(256, EVG_GTASK_OCC) k_gtask(DTasks T, DDistros
 // ---- multi-member units: the unit table ----
 // A membership ("pair": a task filed under a unit slot by its own key, by its version, or by one of its in-queue
 // dependencies' keys; planner.go:431-456) used to be a node of a linked list per slot, and every walk a chain of
-// dependent scattered loads through six task columns.  Now the members of a unit are one contiguous run of packed
-// 32-byte records:
+// dependent scattered loads through six task columns.  Now the members of a unit are one contiguous run of work-list
+// entry ids, each naming the 32-byte payload k_gtask wrote for the task:
 //   k_glink   per pair: k = atomicAdd(unit_n[slot], 1) -- its place in the run (any order: everything computed from a
-//             run is order-free); TaskGroupInfo sums of task-group tasks
-//   k_galloc  the pair that drew k == 0 reserves unit_n[slot] records: head[slot] = start of the run
-//   k_gfill   every pair writes its task's record at head[slot] + k
-//   k_gunit   the k == 0 pair folds the run into Unit.info (planner.go:302-337), value (planner.go:209-300), anchor
-//   k_gbest   per task: the first unit it is emitted from among its memberships (TaskPlan.Export, planner.go:467-477),
-//             then its rank inside it (TaskList.Less, planner.go:387-405) by one pass over the run
-// pair ids: own-key pair of task t = t, version pair = T.n + t, pair of dependency edge e = 2*T.n + e.
-struct __align__(16) URec {
-  int32_t prio, nd;
-  int64_t exp_ns, qb;
-  int32_t tgo;
-  uint32_t lif;  // bits 0..20 distro-local task index, 21 own-key pair, 22 group_id >= 0, 24..29 task flags
-};
-static_assert(sizeof(URec) == 32, "one L2 sector per member");
-constexpr uint32_t kRecOwn = 1u << 21, kRecGrouped = 1u << 22;
-__device__ __forceinline__ uint32_t rec_li(const URec& r) { return r.lif & 0x1FFFFFu; }
-__device__ __forceinline__ URec rec_load(const URec* p) {  // two 128-bit loads
-  const uint4 a = reinterpret_cast<const uint4*>(p)[0], b = reinterpret_cast<const uint4*>(p)[1];
-  URec r;
-  r.prio = int32_t(a.x); r.nd = int32_t(a.y); r.exp_ns = int64_t((unsigned long long)a.z | ((unsigned long long)a.w << 32));
-  r.qb = int64_t((unsigned long long)b.x | ((unsigned long long)b.y << 32)); r.tgo = int32_t(b.z); r.lif = b.w;
-  return r;
-}
-__device__ __forceinline__ void rec_store(URec* p, const URec& r) {
-  reinterpret_cast<uint4*>(p)[0] = make_uint4(uint32_t(r.prio), uint32_t(r.nd), uint32_t(uint64_t(r.exp_ns)), uint32_t(uint64_t(r.exp_ns) >> 32));
-  reinterpret_cast<uint4*>(p)[1] = make_uint4(uint32_t(uint64_t(r.qb)), uint32_t(uint64_t(r.qb) >> 32), uint32_t(r.tgo), r.lif);
-}
+//             run is order-free); TaskGroupInfo sums of task-group tasks, from the payload
+//   k_galloc  the pair that drew k == 0 reserves unit_n[slot] run positions: head[slot] = start of the run
+//   k_gfill   every pair writes its entry id at head[slot] + k
+//   k_gunit   per unit: the run folded into Unit.info (planner.go:302-337), value (planner.go:209-300), anchor; the
+//             members' ranks (TaskList.Less, planner.go:387-405) for units of up to kRankOne members
+//   k_grank   the ranks of the larger units, a warp per 32 members
+//   k_gbest   per task: the first unit it is emitted from among its memberships (TaskPlan.Export, planner.go:467-477)
+//             and its rank there, one load
+// A membership's place in its run is kept next to the membership, so every access is coalesced: by work-list entry for
+// the own-key (pown) and version (pver) memberships, by edge for dependency memberships (pedge, with the edge's unit slot
+// in sedge).  The on-chip planner's next[] / pair_slot[], indexed by pair id over 2T+E entries of which the general path
+// would touch about a quarter (a sector per access), are not used here.
 
-// what a work-list task is filed under (the same answers in every kernel below)
+// what a work-list task is filed under: one 16-byte entry k_gtask wrote (the same answers in every kernel below)
 struct WlTask {
-  uint32_t t; int d; int64_t base; uint32_t li, ub, ng; int32_t gid, vid; bool gv, own_complex; uint32_t s_own, s_ver;
+  uint32_t t; int d; int64_t base; uint32_t li; bool own_complex; uint32_t s_own, s_ver;  // global slots
 };
-__device__ __forceinline__ WlTask wl_task(const DTasks& T, const DDistros& D, const DWork& W, const DGen& G, unsigned int k) {
+__device__ __forceinline__ WlTask wl_task(const DDistros& D, const DGen& G, unsigned int k) {
+  const uint4 e = G.wl[k];
   WlTask x;
-  x.t = G.clist[k]; x.d = G.clist_d[k];
+  x.t = e.x; x.d = int(e.y); x.s_own = e.z; x.s_ver = e.w;
   x.base = D.task_off[x.d];
-  x.gid = T.gid[x.t]; x.vid = T.vid[x.t];
-  x.ng = uint32_t(D.group_off[x.d + 1] - D.group_off[x.d]);
-  x.ub = uint32_t(D.unit_base[x.d]);
-  x.gv = D.cfg[x.d].group_versions != 0;
   x.li = uint32_t(int64_t(x.t) - x.base);
-  x.own_complex = x.gid >= 0 || x.gv || (W.has_dep[x.t] & 1) != 0;
-  x.s_own = own_slot_local(x.gid, x.vid, x.li, x.ng, x.gv);
-  x.s_ver = (x.gid >= 0 && x.gv) ? x.ng + uint32_t(x.vid) : kInactive;
+  x.own_complex = x.s_own != kInactive;
   return x;
 }
-// f(pair, slot) for every membership of the task (after k_glink: pair_slot / edge_live are final)
+// f(place, slot, own) for every membership of work-list entry k: `place` points at its place in the unit's run, `own`
+// marks the own-key membership (after k_glink: the places and sedge are final)
 template <typename F>
-__device__ __forceinline__ void wl_pairs(const DTasks& T, const DWork& W, const WlTask& x, F&& f) {
-  if (x.own_complex) f(x.t, x.ub + x.s_own);
-  if (x.s_ver != kInactive) f(uint32_t(T.n + x.t), x.ub + x.s_ver);
+__device__ __forceinline__ void wl_pairs(const DTasks& T, const DGen& G, const WlTask& x, unsigned int k, F&& f) {
+  if (x.own_complex) f(G.pown + k, x.s_own, true);
+  if (x.s_ver != kInactive) f(G.pver + k, x.s_ver, false);
   if (T.n_edges > 0)
-    for (int64_t e = T.dep_off[x.t]; e < T.dep_off[x.t + 1]; e++)
-      if (W.edge_live[e]) f(uint32_t(2 * T.n + e), W.pair_slot[2 * T.n + e]);
+    for (int64_t e = T.dep_off[x.t]; e < T.dep_off[x.t + 1]; e++) {
+      const uint32_t sl = G.sedge[e];
+      if (sl != kInactive) f(G.pedge + e, sl, false);
+    }
 }
 
 __global__ void __launch_bounds__(256, EVG_OCC_GLINK) k_glink(DTasks T, DDistros D, DWork W, DGen G, int64_t now) {
   if (*W.err) return;
   const unsigned int n = *G.ccount;
   for (unsigned int k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x) {
-    const WlTask x = wl_task(T, D, W, G, k);
+    const WlTask x = wl_task(D, G, k);
     const uint32_t t = x.t;
     const int d = x.d;
-    if (x.gid >= 0) {
+    const uint32_t ub = uint32_t(D.unit_base[d]), ng = uint32_t(D.group_off[d + 1] - D.group_off[d]);
+    // own_slot_local files a task with group_id >= 0 under its group's slot (local slot = group_id < ng) and every other
+    // task at ng or above, so the own-key slot tells task-group tasks apart without loading the payload
+    if (x.own_complex && x.s_own - ub < ng) {
+      const URec me = rec_load(G.pay + k);
       const evg_distro_cfg* cf = D.cfg + d;
-      const uint32_t fl = T.flags[t];
-      const int64_t exp_ns = T.expected[t], threshold = cf->target_time_ns;
+      const uint32_t fl = (me.lif >> 24) & 0x3Fu;
+      const int64_t exp_ns = me.exp_ns, threshold = cf->target_time_ns;
       const bool dm = (fl & EVG_TF_DEPS_MET) != 0;
       const bool counted = !cf->includes_dependencies || dm;
       const bool over = counted && exp_ns > threshold;
-      const bool wait_over = counted && dm && since(now, T.wbasis[t]) > threshold;
+      const bool wait_over = (me.lif & kRecWaitOver) != 0;
       const bool mq_dm = dm && (fl & EVG_TF_REQ_MASK) == EVG_TF_REQ_MERGE_QUEUE;
-      evg_group_info* g = W.ginfo + D.group_off[d] + x.gid;
+      evg_group_info* g = W.ginfo + D.group_off[d] + (x.s_own - ub);
       atomic_add64(&g->count, counted);
       atomic_add64(&g->expected_duration, counted ? exp_ns : 0);
       atomic_add64(&g->count_duration_over_threshold, over);
@@ -408,25 +450,24 @@ __global__ void __launch_bounds__(256, EVG_OCC_GLINK) k_glink(DTasks T, DDistros
       atomic_add64(&g->count_wait_over_threshold, wait_over);
       atomic_add64(&g->count_dep_filled_merge_queue_tasks, mq_dm);
     }
-    auto join = [&](uint32_t pair, uint32_t slot) {
-      W.pair_slot[pair] = slot;
-      W.next[pair] = atomicAdd(W.unit_n + slot, 1u);  // the pair's place in the unit's run
-    };
-    if (x.own_complex) join(t, x.ub + x.s_own);
-    if (x.s_ver != kInactive) join(uint32_t(T.n + t), x.ub + x.s_ver);  // planner.go:439
+    // a membership's place in its unit's run: any order, everything computed from a run is order-free
+    if (x.own_complex) G.pown[k] = atomicAdd(W.unit_n + x.s_own, 1u);
+    if (x.s_ver != kInactive) G.pver[k] = atomicAdd(W.unit_n + x.s_ver, 1u);  // planner.go:439
     if (T.n_edges > 0) {
+      const bool gv = D.cfg[d].group_versions != 0;
       const int64_t e0 = T.dep_off[t], e1 = T.dep_off[t + 1];
       for (int64_t e = e0; e < e1; e++) {
         const uint32_t dl = uint32_t(T.dep_idx[e]);
-        const uint32_t sl = own_slot_local(T.gid[x.base + dl], T.vid[x.base + dl], dl, x.ng, x.gv);
-        bool dup = (sl == x.s_own) || (sl == x.s_ver);  // Unit.Add is keyed by task id (planner.go:131): join each unit once
+        const uint32_t sl = ub + own_slot_local(T.gid[x.base + dl], T.vid[x.base + dl], dl, ng, gv);
+        // Unit.Add is keyed by task id (planner.go:131): join each unit once.  A task without an own-key membership
+        // has no dependents, so no edge of its own leads back to its own-key slot.
+        bool dup = (sl == x.s_own) || (sl == x.s_ver);
         for (int64_t f = e0; f < e && !dup; f++) {
           const uint32_t fl2 = uint32_t(T.dep_idx[f]);
-          dup = own_slot_local(T.gid[x.base + fl2], T.vid[x.base + fl2], fl2, x.ng, x.gv) == sl;
+          dup = ub + own_slot_local(T.gid[x.base + fl2], T.vid[x.base + fl2], fl2, ng, gv) == sl;
         }
-        W.edge_task[e] = t;
-        W.edge_live[e] = dup ? 0 : 1;
-        if (!dup) join(uint32_t(2 * T.n + e), x.ub + sl);
+        G.sedge[e] = dup ? kInactive : sl;
+        if (!dup) G.pedge[e] = atomicAdd(W.unit_n + sl, 1u);
       }
     }
   }
@@ -445,8 +486,8 @@ __global__ void __launch_bounds__(256, EVG_OCC_GALLOC) k_galloc(DTasks T, DDistr
     WlTask x;
     uint32_t need = 0, heads = 0;  // records / units this thread's k == 0 pairs stand for
     if (k < n) {
-      x = wl_task(T, D, W, G, k);
-      wl_pairs(T, W, x, [&](uint32_t pair, uint32_t slot) { if (W.next[pair] == 0u) { need += W.unit_n[slot]; heads++; } });
+      x = wl_task(D, G, k);
+      wl_pairs(T, G, x, k, [&](const uint32_t* place, uint32_t slot, bool) { if (*place == 0u) { need += W.unit_n[slot]; heads++; } });
     }
     uint32_t inc = need, hinc = heads;
 #pragma unroll
@@ -466,8 +507,8 @@ __global__ void __launch_bounds__(256, EVG_OCC_GALLOC) k_galloc(DTasks T, DDistr
     __syncthreads();
     if (heads) {
       uint32_t pos = s_base + before + inc - need, hp = s_hbase + hbefore + hinc - heads;
-      wl_pairs(T, W, x, [&](uint32_t pair, uint32_t slot) {
-        if (W.next[pair] == 0u) { W.head[slot] = pos; pos += W.unit_n[slot]; G.hlist[hp++] = make_uint2(slot, uint32_t(x.d)); }
+      wl_pairs(T, G, x, k, [&](const uint32_t* place, uint32_t slot, bool) {
+        if (*place == 0u) { W.head[slot] = pos; pos += W.unit_n[slot]; G.hlist[hp++] = make_uint2(slot, uint32_t(x.d)); }
       });
     }
     __syncthreads();  // the shared scratch is rewritten by the next trip
@@ -478,14 +519,9 @@ __global__ void __launch_bounds__(256, EVG_OCC_GFILL) k_gfill(DTasks T, DDistros
   if (*W.err) return;
   const unsigned int n = *G.ccount;
   for (unsigned int k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x) {
-    const WlTask x = wl_task(T, D, W, G, k);
-    URec r;
-    r.prio = T.priority[x.t]; r.nd = T.numdep[x.t]; r.exp_ns = T.expected[x.t]; r.qb = T.qbasis[x.t]; r.tgo = T.tgo[x.t];
-    r.lif = x.li | (x.gid >= 0 ? kRecGrouped : 0u) | ((T.flags[x.t] & 0x3Fu) << 24);
-    wl_pairs(T, W, x, [&](uint32_t pair, uint32_t slot) {
-      URec q = r;
-      if (pair < uint32_t(T.n)) q.lif |= kRecOwn;  // own-key pairs are the SetDistro members (planner.go:446)
-      rec_store(G.rec + W.head[slot] + W.next[pair], q);
+    const WlTask x = wl_task(D, G, k);
+    wl_pairs(T, G, x, k, [&](const uint32_t* place, uint32_t slot, bool own) {
+      G.run[W.head[slot] + *place] = k | (own ? kRunOwn : 0u);  // own-key members are the SetDistro members (planner.go:446)
     });
   }
 }
@@ -493,26 +529,94 @@ __global__ void __launch_bounds__(256, EVG_OCC_GFILL) k_gfill(DTasks T, DDistros
 __device__ __forceinline__ void rec_acc(UnitAcc& a, int64_t now, const URec& r) {
   acc_add(a, now, r.prio, r.exp_ns, r.qb, r.nd, (r.lif & kRecGrouped) ? 0 : -1, (r.lif >> 24) & 0x3Fu);
 }
+__device__ __forceinline__ bool rec_less(const URec& x, const URec& y) {  // TaskList.Less, then input index
+  return in_unit_less(x.tgo, x.nd, x.prio, x.exp_ns, rec_li(x), y.tgo, y.nd, y.prio, y.exp_ns, rec_li(y));
+}
+// Units up to this many members are ranked by the thread that folds them (at most kRankOne^2 comparisons on the keys it
+// stashed in shared memory while folding); larger ones by k_grank, a warp per 32 members.
+constexpr uint32_t kRankOne = 8;
+constexpr int kRankKey = 6;  // tgo, nd, prio, expected (two words), index
 
 // One thread per multi-member unit (dense warps: the unit list, not the work list).
 __global__ void __launch_bounds__(256, EVG_OCC_GUNIT) k_gunit(DDistros D, DWork W, DGen G, int64_t now) {
   if (*W.err) return;
   const unsigned int n = *G.hcount;
+  __shared__ uint32_t s_key[kRankOne * kRankKey][256];  // this thread's column: the rank keys of a small unit's members
   for (unsigned int k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x) {  // the host cannot know n: fixed grid
     const uint2 u = G.hlist[k];
-    const uint32_t cnt = W.unit_n[u.x];
-    const URec* run = G.rec + W.head[u.x];
+    const uint32_t cnt = W.unit_n[u.x], h = W.head[u.x];
+    const uint32_t* run = G.run + h;
     UnitAcc a;
     acc_init(a);
     uint32_t anchor = kNoAnchor;
+    const bool small = cnt <= kRankOne;
     for (uint32_t i = 0; i < cnt; i++) {
-      const URec r = rec_load(run + i);
+      const uint32_t q = run[i];
+      const URec r = rec_load(G.pay + (q & kRunEntry));
       rec_acc(a, now, r);
-      if (r.lif & kRecOwn) anchor = min(anchor, rec_li(r));
+      if (q & kRunOwn) anchor = min(anchor, rec_li(r));
+      if (small) {
+        uint32_t* kx = &s_key[i * kRankKey][threadIdx.x];
+        kx[0] = uint32_t(r.tgo); kx[256] = uint32_t(r.nd); kx[512] = uint32_t(r.prio);
+        kx[768] = uint32_t(uint64_t(r.exp_ns)); kx[1024] = uint32_t(uint64_t(r.exp_ns) >> 32); kx[1280] = rec_li(r);
+      }
     }
     const unsigned long long v = (unsigned long long)unit_value(a, D.cfg[u.y], nullptr);
     G.usum[u.x] = make_uint4(uint32_t(v), uint32_t(v >> 32), anchor, cnt);  // kNoAnchor: the unit never got a distro -> not exported (planner.go:81-83)
     W.unit_mask[u.x] = 0ull;  // k_gbest ORs the emitted ranks in (cleared here, unit by unit, instead of a slot-wide memset)
+    // every member's rank in the unit: a count over the member set, so the order of the run does not matter
+    if (small) {
+      auto key = [&](uint32_t i, URec& r) {
+        const uint32_t* kx = &s_key[i * kRankKey][threadIdx.x];
+        r.tgo = int32_t(kx[0]); r.nd = int32_t(kx[256]); r.prio = int32_t(kx[512]);
+        r.exp_ns = int64_t((unsigned long long)kx[768] | ((unsigned long long)kx[1024] << 32)); r.lif = kx[1280];
+      };
+      for (uint32_t i = 0; i < cnt; i++) {
+        URec me, o;
+        key(i, me);
+        uint32_t rk = 0;
+        for (uint32_t j = 0; j < cnt; j++) { key(j, o); rk += rec_less(o, me) ? 1u : 0u; }
+        G.rank[h + i] = rk;
+      }
+    } else {
+      const uint32_t nch = (cnt + 31) >> 5;
+      const uint32_t b = atomicAdd(G.bcount, nch);
+      for (uint32_t c = 0; c < nch; c++) G.blist[b + c] = make_uint2(u.x, c);
+    }
+  }
+}
+
+// Ranks of the units above kRankOne members: a warp per 32 members (lane = member), the whole run streamed past them 32
+// records at a time (coalesced) and broadcast with shuffles.  n members cost n comparisons per lane, in parallel over
+// the ceil(n / 32) warps of the unit.
+__global__ void __launch_bounds__(256, EVG_OCC_GUNIT) k_grank(DWork W, DGen G) {
+  if (*W.err) return;
+  const unsigned int n = *G.bcount;
+  const unsigned full = 0xffffffffu;
+  const int lane = threadIdx.x & 31;
+  const unsigned int nw = gridDim.x * (blockDim.x >> 5);
+  for (unsigned int c = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); c < n; c += nw) {  // warp-uniform
+    const uint2 ch = G.blist[c];
+    const uint32_t cnt = W.unit_n[ch.x], h = W.head[ch.x];
+    const uint32_t* run = G.run + h;
+    const uint32_t i = ch.y * 32u + uint32_t(lane);
+    URec me;
+    me.tgo = 0; me.nd = 0; me.prio = 0; me.exp_ns = 0; me.lif = 0;
+    if (i < cnt) me = rec_load(G.pay + (run[i] & kRunEntry));
+    uint32_t rk = 0;
+    for (uint32_t j0 = 0; j0 < cnt; j0 += 32) {
+      URec o;
+      o.tgo = 0; o.nd = 0; o.prio = 0; o.exp_ns = 0; o.lif = 0;
+      if (j0 + lane < cnt) o = rec_load(G.pay + (run[j0 + lane] & kRunEntry));
+      const uint32_t m = min(32u, cnt - j0);
+      for (uint32_t q = 0; q < m; q++) {
+        URec y;
+        y.tgo = __shfl_sync(full, o.tgo, q); y.nd = __shfl_sync(full, o.nd, q); y.prio = __shfl_sync(full, o.prio, q);
+        y.exp_ns = __shfl_sync(full, o.exp_ns, q); y.lif = __shfl_sync(full, o.lif, q);
+        rk += (i < cnt && rec_less(y, me)) ? 1u : 0u;
+      }
+    }
+    if (i < cnt) G.rank[h + i] = rk;
   }
 }
 
@@ -528,33 +632,28 @@ __global__ void __launch_bounds__(256, EVG_OCC_GBEST) k_gbest(DTasks T, DDistros
     int d = -1;
     unsigned long long kk = 0ull;
     if (k < n) {
-      const WlTask x = wl_task(T, D, W, G, k);
+      const WlTask x = wl_task(D, G, k);
       const uint32_t t = x.t, li = x.li;
       d = x.d;
       bool have = false;
       int64_t bv = 0;
-      uint32_t ba = 0, brk = 0, bp = kInactive, bslot = kInactive, bn = 1, bkx = 0;
+      uint32_t ba = 0, brk = 0, bslot = kInactive, bn = 1, bkx = 0;
       if (!x.own_complex) { have = true; bv = G.tv[t]; ba = li; }  // its own single-task unit, scored by k_gtask
-      wl_pairs(T, W, x, [&](uint32_t pair, uint32_t slot) {
+      wl_pairs(T, G, x, k, [&](const uint32_t* place, uint32_t slot, bool) {
         const uint4 u = G.usum[slot];
-        const uint32_t kx = W.next[pair];  // this task's place in that unit's run (requested together with the summary)
+        const uint32_t kx = *place;  // this task's place in that unit's run (requested together with the summary)
         const uint32_t a = u.z;
         if (a == kNoAnchor) return;
         const int64_t v = int64_t((unsigned long long)u.x | ((unsigned long long)u.y << 32));
-        if (!have || v > bv || (v == bv && a < ba)) { have = true; bv = v; ba = a; bp = pair; bslot = slot; bn = u.w; bkx = kx; }
+        if (!have || v > bv || (v == bv && a < ba)) { have = true; bv = v; ba = a; bslot = slot; bn = u.w; bkx = kx; }
       });
-      if (bp != kInactive) {  // rank among ALL members of the chosen unit; the task's own fields are its record in the run
-        const URec* run = G.rec + W.head[bslot];
-        const URec me = rec_load(run + bkx);
-        for (uint32_t i = 0; i < bn; i++) {
-          const URec r = rec_load(run + i);
-          if (in_unit_less(r.tgo, r.nd, r.prio, r.exp_ns, rec_li(r), me.tgo, me.nd, me.prio, me.exp_ns, li)) brk++;
-        }
+      if (bslot != kInactive) {  // its rank among ALL members of the chosen unit, as k_gunit / k_grank counted it
+        brk = G.rank[W.head[bslot] + bkx];
         if (bn <= 64) atomicOr(&W.unit_mask[bslot], 1ull << brk);  // ranks emitted from the unit: k_gplace_disp counts below its own
       }
       G.tv[t] = bv;
-      G.tie[t] = make_uint4(ba, brk, bslot, 0u);
-      if (want_best_pair) W.best_pair[t] = bp;  // k_breakdown's way back to the unit
+      G.tie[k] = make_uint4(ba, brk, bslot, 0u);
+      if (want_best_pair) W.best_pair[t] = bslot;  // k_breakdown's way back to the unit (general path: its slot)
       const bool displaced = !(ba == li && brk == 0);
       if (displaced) W.has_dep[t] |= 2;  // only this thread touches the byte now (k_gmark and k_gtask are done)
       atomicAdd(G.e + x.base + ba, 1u);
@@ -784,20 +883,21 @@ __global__ void __launch_bounds__(256) k_gplace(DDistros D, DWork W, DGen G, int
 __global__ void __launch_bounds__(256) k_gplace_disp(DTasks T, DDistros D, DWork W, DGen G) {
   const unsigned int n = *G.ccount;
   for (unsigned int k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x) {
-  const uint32_t t = G.clist[k];
+  const uint4 ent = G.wl[k];
+  const uint32_t t = ent.x;
   if (!(W.has_dep[t] & 2)) continue;
-  const int d = G.clist_d[k];
+  const int d = int(ent.y);
   const int64_t base = D.task_off[d];
-  const uint4 tie = G.tie[t];
+  const uint4 tie = G.tie[k];
   const uint32_t a = tie.x, myrk = tie.y, slot = tie.z;
   uint32_t pos = G.e[base + a];
   const uint32_t cnt = W.unit_n[slot];
   if (cnt <= 64) {
     pos += __popcll(W.unit_mask[slot] & ((1ull << myrk) - 1ull));
   } else {
-    const URec* run = G.rec + W.head[slot];
+    const uint32_t* run = G.run + W.head[slot];
     for (uint32_t i = 0; i < cnt; i++) {
-      const uint4 tq = G.tie[base + rec_li(rec_load(run + i))];
+      const uint4 tq = G.tie[run[i] & kRunEntry];
       if (tq.z == slot && tq.y < myrk) pos++;
     }
   }

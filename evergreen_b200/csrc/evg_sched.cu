@@ -504,7 +504,7 @@ __global__ void __launch_bounds__(256) k_dur_final(DDur X, evg_duration_stat* ou
 
 // The 13-field SortingValueBreakdown of the unit each ranked task was emitted
 // from (planner.go:472-476, model/task/task.go:3990-4038); both paths.
-__global__ void __launch_bounds__(256) k_breakdown(DTasks T, DDistros D, DWork W, const URec* rec, int64_t now, int any_complex,
+__global__ void __launch_bounds__(256) k_breakdown(DTasks T, DDistros D, DWork W, const uint32_t* run_all, const URec* pay, int64_t now, int any_complex,
                                                    const int32_t* order, int64_t* breakdown) {
   if (*W.err) return;
   const int64_t t = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -522,11 +522,11 @@ __global__ void __launch_bounds__(256) k_breakdown(DTasks T, DDistros D, DWork W
       const uint32_t tq = pair_task(T, W, q);
       acc_add(a, now, T.priority[tq], T.expected[tq], T.qbasis[tq], T.numdep[tq], T.gid[tq], T.flags[tq]);
     }
-  } else {  // general path: the unit table
-    const uint32_t slot = W.pair_slot[bp];
-    const URec* run = rec + W.head[slot];
+  } else {  // general path: the unit table (k_gbest stored the chosen unit's slot)
+    const uint32_t slot = bp;
+    const uint32_t* run = run_all + W.head[slot];
     const uint32_t cnt = W.unit_n[slot];
-    for (uint32_t i = 0; i < cnt; i++) rec_acc(a, now, rec_load(run + i));
+    for (uint32_t i = 0; i < cnt; i++) rec_acc(a, now, rec_load(pay + (run[i] & kRunEntry)));
   }
   int64_t bd[EVG_BD_N];
   unit_value(a, D.cfg[d], bd);
@@ -852,7 +852,7 @@ struct evg_ctx {
   int general_complex = 0;
   int64_t Tgc = 0;  // tasks in general-path distros that can hold multi-member units (work-list capacity)
   DevBuf b_kv, b_vmm, b_klo[2], b_khi[2], b_ix[2], b_e, b_tilesum, b_gmisc;
-  DevBuf b_tiledistro, b_tilestart, b_dtileoff, b_tilehist, b_clist, b_rec, b_tie, b_hlist, b_usum, b_upd;
+  DevBuf b_tiledistro, b_tilestart, b_dtileoff, b_tilehist, b_wl, b_pay, b_place, b_eplace, b_run, b_rank, b_blist, b_tie, b_hlist, b_usum, b_upd;
   DevBuf b_qinfo, b_ginfo, b_order, b_tv, b_bd;
   DevBuf b_hflags, b_hgid, b_hexp, b_hstd, b_hstart, b_hostoff, b_acfg, b_gs, b_result, b_status;
   bool bd_valid = false;
@@ -971,6 +971,7 @@ int upload_tasks(evg_ctx* c, const evg_task_soa* t, const evg_distro_table* dt, 
   const int64_t U = unit_base[D];
   if (U >= int64_t(0xFFFFFFF0u)) return fail(EVG_ERR_INVALID, "unit slot space exceeds 32 bits");
   if (Prec >= int64_t(0xFFFFFFF0u)) return fail(EVG_ERR_INVALID, "unit table exceeds 32 bits");
+  if (Tgc >= int64_t(kRunOwn)) return fail(EVG_ERR_INVALID, "work list exceeds 31 bits (a run position is entry id | own bit)");
   const int64_t NT = int64_t(tile_distro.size());
   const int64_t P = 2 * T + E;
   cudaStream_t s = c->stream;
@@ -1049,8 +1050,10 @@ int upload_tasks(evg_ctx* c, const evg_task_soa* t, const evg_distro_table* dt, 
   if (any_complex) {
     CK(c->b_hasdep.ensure(size_t(T) + 16));
     CK(c->b_head.ensure(sizeof(uint32_t) * size_t(U + 1)));
-    CK(c->b_next.ensure(sizeof(uint32_t) * size_t(P + 1)));
-    CK(c->b_pslot.ensure(sizeof(uint32_t) * size_t(P + 1)));
+    if (on_chip_cta || !listW.empty()) {  // k_plan_smem's member lists, by pair id (a breakdown run plans tiny distros with it)
+      CK(c->b_next.ensure(sizeof(uint32_t) * size_t(P + 1)));
+      CK(c->b_pslot.ensure(sizeof(uint32_t) * size_t(P + 1)));
+    }
     CK(c->b_etask.ensure(sizeof(uint32_t) * size_t(E + 1)));
     CK(c->b_elive.ensure(size_t(E) + 1));
     CK(c->b_unitv.ensure(sizeof(int64_t) * size_t(U + 1)));
@@ -1073,11 +1076,16 @@ int upload_tasks(evg_ctx* c, const evg_task_soa* t, const evg_distro_table* dt, 
     CK(c->b_tilehist.ensure(sizeof(uint32_t) * 256 * size_t(NT + 1)));
     if (general_complex) {
       CK(c->b_e.ensure(sizeof(uint32_t) * size_t(T + kColPad)));
-      CK(c->b_clist.ensure(sizeof(uint32_t) * 2 * size_t(Tgc + 1)));
-      CK(c->b_rec.ensure(sizeof(URec) * size_t(Prec + 1)));
+      CK(c->b_wl.ensure(sizeof(uint4) * size_t(Tgc + 1)));
+      CK(c->b_pay.ensure(sizeof(URec) * size_t(Tgc + 1)));
+      CK(c->b_tie.ensure(sizeof(uint4) * size_t(Tgc + 1)));
+      CK(c->b_place.ensure(sizeof(uint32_t) * 2 * size_t(Tgc + 1)));
+      CK(c->b_eplace.ensure(sizeof(uint32_t) * 2 * size_t(E + 1)));
+      CK(c->b_run.ensure(sizeof(uint32_t) * size_t(Prec + 1)));
+      CK(c->b_rank.ensure(sizeof(uint32_t) * size_t(Prec + 1)));
+      CK(c->b_blist.ensure(sizeof(uint2) * size_t(Prec / kRankOne + 1)));  // a unit of n > kRankOne members: ceil(n/32) <= n/kRankOne chunks
       CK(c->b_hlist.ensure(sizeof(uint2) * size_t(Prec + 1)));
       CK(c->b_usum.ensure(sizeof(uint4) * size_t(U + 1)));
-      CK(c->b_tie.ensure(sizeof(uint4) * size_t(T + 1)));
     }
   }
   CK(c->b_punt.ensure(sizeof(int32_t) * size_t(D + 1)));
@@ -1204,15 +1212,22 @@ DGen dgen(const evg_ctx* c) {
     g.key_lo[k] = c->b_klo[k].as<uint32_t>(); g.key_hi[k] = c->b_khi[k].as<uint32_t>(); g.idx[k] = c->b_ix[k].as<uint32_t>();
   }
   g.e = c->b_e.as<uint32_t>(); g.tile_sum = c->b_tilesum.as<uint32_t>(); g.tile_hist = c->b_tilehist.as<uint32_t>();
-  g.clist = c->b_clist.as<uint32_t>();
-  g.clist_d = c->b_clist.as<int32_t>() + (c->Tgc + 1);
+  g.wl = c->b_wl.as<uint4>();
+  g.pay = c->b_pay.as<URec>();
+  g.pown = c->b_place.as<uint32_t>();
+  g.pver = c->b_place.as<uint32_t>() + (c->Tgc + 1);
+  g.pedge = c->b_eplace.as<uint32_t>();
+  g.sedge = c->b_eplace.as<uint32_t>() + (c->E + 1);
   g.ccount = c->b_gmisc.as<unsigned int>();
   g.maxpass = c->b_gmisc.as<int32_t>() + 1;
   g.rcount = c->b_gmisc.as<unsigned int>() + 2;
   g.hcount = c->b_gmisc.as<unsigned int>() + 3;
+  g.bcount = c->b_gmisc.as<unsigned int>() + 4;
+  g.blist = c->b_blist.as<uint2>();
+  g.rank = c->b_rank.as<uint32_t>();
   g.hlist = c->b_hlist.as<uint2>();
   g.usum = c->b_usum.as<uint4>();
-  g.rec = c->b_rec.as<URec>();
+  g.run = c->b_run.as<uint32_t>();
   g.tie = c->b_tie.as<uint4>();
   g.tv = c->b_tv.as<int64_t>();
   return g;
@@ -1330,6 +1345,7 @@ int run_general(evg_ctx* c, cudaStream_t st, const DTasks& dt, const DDistros& d
     LAUNCH_ON(c, st, k_galloc, wl_grid, 256, dt, dd, w, g);
     LAUNCH_ON(c, st, k_gfill, wl_grid, 256, dt, dd, w, g);
     LAUNCH_ON(c, st, k_gunit, wl_grid, 256, dd, w, g, now);
+    LAUNCH_ON(c, st, k_grank, wl_grid, 256, w, g);
     LAUNCH_ON(c, st, k_gbest, wl_grid, 256, dt, dd, w, g, c->bd_valid ? 1 : 0);
   }
   LAUNCH_ON(c, st, k_gsched, grid_for(gcount, 128), 128, g, gl, gcount);
@@ -1443,7 +1459,7 @@ int run_plan(evg_ctx* c, int64_t now, uint32_t opts) {
       CK(cudaStreamWaitEvent(s, c->ev_join[k], 0));
     }
   }
-  if (bd) LAUNCH(c, k_breakdown, grid_for(T, 256), 256, dt, dd, w, c->b_rec.as<URec>(), now, c->any_complex, c->b_order.as<int32_t>(), bd);
+  if (bd) LAUNCH(c, k_breakdown, grid_for(T, 256), 256, dt, dd, w, c->b_run.as<uint32_t>(), c->b_pay.as<URec>(), now, c->any_complex, c->b_order.as<int32_t>(), bd);
   CK(cudaGetLastError());
   return EVG_OK;
 }
@@ -1495,7 +1511,7 @@ void evg_shutdown(evg_ctx* c) {
                    &c->b_route, &c->b_listW, &c->b_listA, &c->b_listB, &c->b_listC, &c->b_listG, &c->b_listNA, &c->b_listNB,
                    &c->b_listNC, &c->b_lptA, &c->b_lptB, &c->b_lptC, &c->b_lptNA, &c->b_lptNB, &c->b_lptNC, &c->b_punt, &c->b_puntcnt, &c->b_ca, &c->b_crk, &c->b_bestpair, &c->b_kv, &c->b_vmm,
                    &c->b_klo[0], &c->b_klo[1], &c->b_khi[0], &c->b_khi[1], &c->b_ix[0], &c->b_ix[1], &c->b_e, &c->b_tilesum,
-                   &c->b_gmisc, &c->b_clist, &c->b_rec, &c->b_tie, &c->b_hlist, &c->b_usum, &c->b_upd, &c->b_tiledistro, &c->b_tilestart, &c->b_dtileoff, &c->b_tilehist,
+                   &c->b_gmisc, &c->b_wl, &c->b_pay, &c->b_place, &c->b_eplace, &c->b_run, &c->b_rank, &c->b_blist, &c->b_tie, &c->b_hlist, &c->b_usum, &c->b_upd, &c->b_tiledistro, &c->b_tilestart, &c->b_dtileoff, &c->b_tilehist,
                    &c->b_qinfo, &c->b_ginfo, &c->b_order, &c->b_tv, &c->b_bd, &c->b_hflags, &c->b_hgid, &c->b_hexp, &c->b_hstd,
                    &c->b_hstart, &c->b_hostoff, &c->b_acfg, &c->b_gs, &c->b_result, &c->b_status};
   for (DevBuf* b : all) b->release();
