@@ -70,6 +70,12 @@ struct DevBuf {
   void* p = nullptr;
   size_t cap = 0;
   bool owned = true;  // false: p is caller-owned device memory (evg_upload_device)
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  ~DevBuf() {
+    if (p && owned) cudaFree(p);
+  }
   void adopt(void* q) {
     if (owned && p) cudaFree(p);
     p = q; cap = 0; owned = false;
@@ -86,15 +92,31 @@ struct DevBuf {
     cap = want;
     return cudaSuccess;
   }
-  void release() {
-    if (p && owned) cudaFree(p);
-    p = nullptr;
-    cap = 0;
-    owned = true;
-  }
   template <class T>
   T* as() const { return reinterpret_cast<T*>(p); }
 };
+
+// Grow `buf` to `count` elements of `type` (at least one) and copy them from host memory at `ptr` on stream `st`.
+#define UP(st, buf, ptr, count, type)                                                                             \
+  do {                                                                                                            \
+    CK((buf).ensure(sizeof(type) * size_t((count) > 0 ? (count) : 1)));                                           \
+    if ((count) > 0) CK(cudaMemcpyAsync((buf).p, (ptr), sizeof(type) * size_t(count), cudaMemcpyHostToDevice, st)); \
+  } while (0)
+
+// The planner's size classes.  upload_tasks routes every distro to one (route_of); each class has its own list.
+enum Route : int {
+  kWarp,                    // <= 32 tasks: k_plan_warp
+  kGeneral,                 // the general path
+  kSmemA, kSmemB, kSmemC,   // k_plan_smem's classes
+  kCtaA, kCtaB, kCtaC,      // k_plan_cta's classes (kCtaA: the <128,1280> and <64,384> instances)
+  kRoutes,
+  kPunted = kRoutes,        // not a list: the distros the k_plan_cta classes hand back, replanned by k_plan_smem
+};
+constexpr bool is_cta(int r) { return r == kCtaA || r == kCtaB || r == kCtaC; }
+// the resident tick launches the on-chip classes largest distro first (upload_tasks keeps a second copy of their lists)
+constexpr bool largest_first(int r) { return r != kWarp && r != kGeneral; }
+// the resident tick's stream of each class (kPunted runs behind the k_plan_cta classes)
+constexpr int kRouteStream[kRoutes + 1] = {4, 5, 3, 2, 1, 0, 0, 0, 0};
 
 // on-chip planner classes <THREADS, ITEMS>: capacity = THREADS*ITEMS tasks per distro
 #ifndef EVG_C_THREADS  // shape of the largest on-chip class (threads x tasks per thread = 12288 tasks in 218 KB)
@@ -830,22 +852,33 @@ struct evg_ctx {
   bool deps_resident = false;  // evg_upload_with_deps left the verdicts and stamps of this tick on the device
   DevBuf b_prio, b_exp, b_qb, b_wb, b_nd, b_tgo, b_gid, b_vid, b_flags, b_depoff, b_depidx;
   DevBuf b_taskoff, b_groupoff, b_cfg, b_gmax, b_unitbase;
-  DevBuf b_hasdep, b_head, b_next, b_pslot, b_etask, b_elive, b_ca, b_crk, b_bestpair;
+  DevBuf b_hasdep, b_head, b_next, b_pslot, b_etask, b_elive, b_bestpair;
   DevBuf b_rn0, b_rn1, b_rn2, b_rn3, b_rn4, b_rn5, b_rn6, b_rn7;
-  DevBuf b_pf[36];  // evg_plan_from_finder: finder tables, candidate columns, compacted columns, edge scratch
+  struct TaskCols { DevBuf prio, nd, tgo, gid, vid, flags, exp, qb, wb; };  // the nine planner columns of a task table
+  struct {
+    DevBuf task_off, sched, project, project_flags, valid_off, valid_idx, finder;  // the finder tables
+    DevBuf kept, count;                // k_runnable's kept lists and per-distro counts
+    TaskCols cand, out;                // candidate columns, compacted columns
+    DevBuf new_off, new_idx, src_row;  // compacted task_off; candidate row -> compacted index, and back
+    DevBuf dep_off, dep_idx, edge_cnt, new_dep_off, scan_sum, new_dep_idx;  // candidate edges, surviving edges
+  } pf;  // evg_plan_from_finder's own buffers (deps_to_device holds b_rn6 / b_rn7)
   DevBuf b_err, b_dx0, b_dx1, b_dx2, b_dx3, b_dx4, b_dx5, b_dx6, b_dx7;
-  DevBuf b_route, b_listW, b_listA, b_listB, b_listC, b_listG, b_listNA, b_listNB, b_listNC, b_unitv, b_unita, b_unitn, b_unitmask;
+  DevBuf b_route, b_unitv, b_unita, b_unitn, b_unitmask;
   DevBuf b_punt, b_puntcnt;
-  int32_t nW = 0, nA = 0, nB = 0, nC = 0, nNA = 0, nNB = 0, nNC = 0, n_general = 0;  // distros per route
+  // The distros of each size class: ascending ids on the host and the device (the pipelined call cuts them by distro
+  // range), and for the on-chip classes the same list largest distro first (the resident tick's launch order).
+  struct RouteList {
+    std::vector<int32_t> h;
+    DevBuf b, lpt;
+    int32_t n() const { return int32_t(h.size()); }
+  };
+  RouteList routes[kRoutes];
   int64_t max_cta_tasks = 0;  // largest distro routed to k_plan_cta: picks the fallback instance for what it hands back
-  int32_t nNA_big = 0;  // leading entries of the largest-first NA list that need the 128-thread instance
-  std::vector<int32_t> h_listW, h_listA, h_listB, h_listC, h_listNA, h_listNB, h_listNC;  // host copies (ascending distro ids)
+  int32_t nNA_big = 0;  // leading entries of the largest-first kCtaA list that need the 128-thread instance
   DevBuf b_alist;            // distros k_alloc plans itself (task groups, or more than kGrouplessHosts hosts), listed by upload_hosts
   int64_t n_alist = 0;
   bool alist_valid = false;
-  DevBuf b_lptA, b_lptB, b_lptC, b_lptNA, b_lptNB, b_lptNC;  // the same lists, largest distro first: the resident tick's launch order
   std::vector<int64_t> h_taskoff, h_groupoff, h_unitbase, h_edgeoff, h_dtileoff;
-  std::vector<int32_t> h_listG;
   cudaStream_t s_h2d = nullptr, s_d2h = nullptr;
   static constexpr int kMaxChunks = 16;
   cudaEvent_t ev_h[kMaxChunks] = {}, ev_c[kMaxChunks] = {};
@@ -890,46 +923,51 @@ int upload_tasks(evg_ctx* c, const evg_task_soa* t, const evg_distro_table* dt, 
   if (E > 0 && (!t->dep_off || !t->dep_idx)) return fail(EVG_ERR_INVALID, "n_edges > 0 but dep_off/dep_idx null");
   if (D == 0 && T != 0) return fail(EVG_ERR_INVALID, "tasks without distros");
   std::vector<int64_t> unit_base(size_t(D) + 1, 0), dtile_off(size_t(D) + 1, 0);
-  std::vector<int32_t> tile_distro, listW, listA, listB, listC, listG, listNA, listNB, listNC;
+  std::vector<int32_t> tile_distro, list[kRoutes];
   std::vector<int64_t> tile_start;
   std::vector<uint8_t> route(size_t(D) + 1, 0);
-  int32_t n_general = 0;
   int general_complex = 0;
   int any_complex = E > 0 ? 1 : 0;
   int64_t Tgc = 0, Prec = 0;
   constexpr int kGA = PlanCta<kNT_A, kNCapA>::kGroupCap, kGB = PlanCta<kNT_B, kNCapB>::kGroupCap, kGC = PlanCta<kNT_C, kNCapC>::kGroupCap;
-  // Size class of distro d (no side effects): W warp, 1..3 k_plan_cta classes, 4..6 k_plan_smem classes, 7 general path.
-  auto classify = [&](int32_t d) -> int {
+  // Size class of distro d by its own shape (no side effects).  kBigUnits: a GroupVersions distro of k_plan_smem's
+  // smallest class above kBigUnitTasks tasks, whose version units of dozens of tasks are walked member by member.
+  constexpr int kBigUnits = kRoutes;
+  auto size_class = [&](int32_t d) -> int {
     const int64_t a = dt->task_off[d], b = dt->task_off[d + 1];
     const int64_t n = b - a, g = dt->group_off[d + 1] - dt->group_off[d];
     const evg_distro_cfg& cf = dt->cfg[d];
     const int64_t de = (E > 0) ? (edge_off ? edge_off[d + 1] - edge_off[d] : t->dep_off[b] - t->dep_off[a]) : 0;
     const bool narrow = !cf.group_versions && de == 0;  // k_plan_cta: task groups are the only multi-member units it knows
-    if (n <= kCapW) return 0;
-    if (narrow && n <= kNCapA && g <= kGA) return 1;
-    if (narrow && n <= kNCapB && g <= kGB) return 2;
-    if (narrow && n <= kNCapC && g <= kGC) return 3;
-    if (n <= kCapA) return (cf.group_versions && n > kBigUnitTasks) ? 8 : 4;  // 8: version units of dozens of tasks, walked member by member
-    if (n <= kCapB) return 5;
-    if (n <= kCapC) return 6;
-    return 7;
+    if (n <= kCapW) return kWarp;
+    if (narrow && n <= kNCapA && g <= kGA) return kCtaA;
+    if (narrow && n <= kNCapB && g <= kGB) return kCtaB;
+    if (narrow && n <= kNCapC && g <= kGC) return kCtaC;
+    if (n <= kCapA) return (cf.group_versions && n > kBigUnitTasks) ? kBigUnits : kSmemA;
+    if (n <= kCapB) return kSmemB;
+    if (n <= kCapC) return kSmemC;
+    return kGeneral;
   };
   // k_plan_smem walks the unit lists of GroupVersions / dependency distros with ONE CTA per distro: fine when a class
   // has enough distros to fill the GPU, a millisecond-long tail when it has a handful (configs[4]: ~20 distros of 1-6k
   // tasks held the whole tick, then ~50 GroupVersions distros of 129-1024 tasks whose version units are walked member by
   // member).  The general path spreads every distro over all SMs, so sparse classes go there.
-  int64_t n_class[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+  int64_t n_class[kBigUnits + 1] = {};
   for (int32_t d = 0; d < D; d++) {
     const int64_t a = dt->task_off[d], b = dt->task_off[d + 1];
     if (d == 0 && (a != 0 || dt->group_off[0] != 0)) return fail(EVG_ERR_INVALID, "offsets must start at 0");
     if (b < a || dt->group_off[d + 1] < dt->group_off[d]) return fail(EVG_ERR_INVALID, "offsets of distro %d decrease", d);
     if (b > T) return fail(EVG_ERR_INVALID, "task_off of distro %d exceeds n_tasks", d);
-    n_class[classify(d)]++;
+    n_class[size_class(d)]++;
   }
   const char* sparse_env = getenv("EVG_SPARSE_CLASS");  // tests set 0 to keep every class on its own kernel
   const int64_t sparse = sparse_env ? atoll(sparse_env) : kSparseClass;
-  const bool sparse_b = n_class[5] > 0 && n_class[5] < sparse, sparse_c = n_class[6] > 0 && n_class[6] < sparse;
-  const bool sparse_v = n_class[8] > 0 && n_class[8] < sparse;
+  // The route of distro d: its size class, after the sparse-class rule (needs every class's size: the count above).
+  auto route_of = [&](int32_t d) -> int {
+    const int k = size_class(d);
+    if ((k == kSmemB || k == kSmemC || k == kBigUnits) && n_class[k] < sparse) return kGeneral;
+    return k == kBigUnits ? kSmemA : k;
+  };
   for (int32_t d = 0; d < D; d++) {
     const int64_t a = dt->task_off[d], b = dt->task_off[d + 1];
     const int64_t ga = dt->group_off[d], gb = dt->group_off[d + 1];
@@ -940,28 +978,17 @@ int upload_tasks(evg_ctx* c, const evg_task_soa* t, const evg_distro_table* dt, 
     unit_base[d + 1] = unit_base[d] + (gb - ga) + (cf.group_versions ? int64_t(cf.n_versions) : (b - a));
     const int64_t n = b - a;
     const int64_t de = (E > 0) ? (edge_off ? edge_off[d + 1] - edge_off[d] : t->dep_off[b] - t->dep_off[a]) : 0;
-    int cls = classify(d);
-    if ((cls == 5 && sparse_b) || (cls == 6 && sparse_c)) cls = 7;
-    if (cls == 8) cls = sparse_v ? 7 : 4;
-    switch (cls) {
-      case 0: listW.push_back(d); route[d] = 1; break;
-      case 1: listNA.push_back(d); route[d] = 1; break;
-      case 2: listNB.push_back(d); route[d] = 1; break;
-      case 3: listNC.push_back(d); route[d] = 1; break;
-      case 4: listA.push_back(d); route[d] = 1; break;
-      case 5: listB.push_back(d); route[d] = 1; break;
-      case 6: listC.push_back(d); route[d] = 1; break;
-      default: {
-        n_general++;
-        listG.push_back(d);
-        if (gb > ga || cf.group_versions || de > 0) {
-          general_complex = 1;
-          Tgc += n;
-          Prec += n + ((cf.group_versions && gb > ga) ? n : 0) + de;  // own-key, version and dependency memberships at most
-        }
-        const int64_t a0 = a & ~int64_t(3);  // tiles start 16-byte aligned in every column
-        for (int64_t s = a0; s < b; s += kGTile) { tile_distro.push_back(d); tile_start.push_back(s); }
+    const int r = route_of(d);
+    list[r].push_back(d);
+    route[d] = r != kGeneral;
+    if (r == kGeneral) {
+      if (gb > ga || cf.group_versions || de > 0) {
+        general_complex = 1;
+        Tgc += n;
+        Prec += n + ((cf.group_versions && gb > ga) ? n : 0) + de;  // own-key, version and dependency memberships at most
       }
+      const int64_t a0 = a & ~int64_t(3);  // tiles start 16-byte aligned in every column
+      for (int64_t s = a0; s < b; s += kGTile) { tile_distro.push_back(d); tile_start.push_back(s); }
     }
     dtile_off[d + 1] = int64_t(tile_distro.size());
   }
@@ -975,11 +1002,6 @@ int upload_tasks(evg_ctx* c, const evg_task_soa* t, const evg_distro_table* dt, 
   const int64_t NT = int64_t(tile_distro.size());
   const int64_t P = 2 * T + E;
   cudaStream_t s = c->stream;
-#define UP(buf, ptr, count, type)                                                                     \
-  do {                                                                                                \
-    CK((buf).ensure(sizeof(type) * size_t((count) > 0 ? (count) : 1)));                               \
-    if ((count) > 0) CK(cudaMemcpyAsync((buf).p, (ptr), sizeof(type) * size_t(count), cudaMemcpyHostToDevice, s)); \
-  } while (0)
 #define UPC(buf, ptr, count, type)                                                                    \
   do {                                                                                                \
     if (adopt) {                                                                                      \
@@ -1004,53 +1026,47 @@ int upload_tasks(evg_ctx* c, const evg_task_soa* t, const evg_distro_table* dt, 
     UPC(c->b_depidx, t->dep_idx, E, int32_t);
   }
 #undef UPC
-  UP(c->b_taskoff, dt->task_off, D + 1, int64_t);
-  UP(c->b_groupoff, dt->group_off, D + 1, int64_t);
-  UP(c->b_cfg, dt->cfg, D, evg_distro_cfg);
-  UP(c->b_gmax, dt->group_max_hosts, G, int32_t);
-  UP(c->b_unitbase, unit_base.data(), D + 1, int64_t);
-  UP(c->b_tiledistro, tile_distro.data(), NT, int32_t);
-  UP(c->b_tilestart, tile_start.data(), NT, int64_t);
-  UP(c->b_dtileoff, dtile_off.data(), D + 1, int64_t);
-  UP(c->b_route, route.data(), D + 1, uint8_t);
-  UP(c->b_listW, listW.data(), int64_t(listW.size()), int32_t);
-  UP(c->b_listG, listG.data(), int64_t(listG.size()), int32_t);
-  UP(c->b_listA, listA.data(), int64_t(listA.size()), int32_t);
-  UP(c->b_listB, listB.data(), int64_t(listB.size()), int32_t);
-  UP(c->b_listC, listC.data(), int64_t(listC.size()), int32_t);
-  UP(c->b_listNA, listNA.data(), int64_t(listNA.size()), int32_t);
-  UP(c->b_listNB, listNB.data(), int64_t(listNB.size()), int32_t);
-  UP(c->b_listNC, listNC.data(), int64_t(listNC.size()), int32_t);
+  UP(s, c->b_taskoff, dt->task_off, D + 1, int64_t);
+  UP(s, c->b_groupoff, dt->group_off, D + 1, int64_t);
+  UP(s, c->b_cfg, dt->cfg, D, evg_distro_cfg);
+  UP(s, c->b_gmax, dt->group_max_hosts, G, int32_t);
+  UP(s, c->b_unitbase, unit_base.data(), D + 1, int64_t);
+  UP(s, c->b_tiledistro, tile_distro.data(), NT, int32_t);
+  UP(s, c->b_tilestart, tile_start.data(), NT, int64_t);
+  UP(s, c->b_dtileoff, dtile_off.data(), D + 1, int64_t);
+  UP(s, c->b_route, route.data(), D + 1, uint8_t);
+  for (int r = 0; r < kRoutes; r++) UP(s, c->routes[r].b, list[r].data(), int64_t(list[r].size()), int32_t);
   // One CTA per distro: with the largest first, the last (partial) wave of a launch holds the smallest distros and the
   // tail is short (configs[4]: 1371 distros of 33..1024 tasks on 132 x 8 = 1056 CTA slots).  The ascending lists stay: the
   // pipelined one-shot call cuts them by distro range.
-  std::vector<int32_t> lptA(listA), lptB(listB), lptC(listC), lptNA(listNA), lptNB(listNB), lptNC(listNC);
-  for (std::vector<int32_t>* v : {&lptA, &lptB, &lptC, &lptNA, &lptNB, &lptNC})
-    std::stable_sort(v->begin(), v->end(), [&](int32_t x, int32_t y) {
+  std::vector<int32_t> lpt[kRoutes];
+  for (int r = 0; r < kRoutes; r++) {
+    if (!largest_first(r)) continue;
+    lpt[r] = list[r];
+    std::stable_sort(lpt[r].begin(), lpt[r].end(), [&](int32_t x, int32_t y) {
       return dt->task_off[x + 1] - dt->task_off[x] > dt->task_off[y + 1] - dt->task_off[y];
     });
+  }
   // the tail of the smallest class that fits the 64-thread instance (size AND task groups) goes last, largest first
   constexpr int kGS = PlanCta<kNT_S, kNCapS>::kGroupCap;
   auto fits_s = [&](int32_t x) { return dt->task_off[x + 1] - dt->task_off[x] <= kNCapS && dt->group_off[x + 1] - dt->group_off[x] <= kGS; };
-  std::stable_partition(lptNA.begin(), lptNA.end(), [&](int32_t x) { return !fits_s(x); });
-  c->nNA_big = int32_t(std::count_if(lptNA.begin(), lptNA.end(), [&](int32_t x) { return !fits_s(x); }));
+  std::vector<int32_t>& lpt_a = lpt[kCtaA];
+  std::stable_partition(lpt_a.begin(), lpt_a.end(), [&](int32_t x) { return !fits_s(x); });
+  c->nNA_big = int32_t(std::count_if(lpt_a.begin(), lpt_a.end(), [&](int32_t x) { return !fits_s(x); }));
   c->max_cta_tasks = 0;
-  for (const std::vector<int32_t>* v : {&listNA, &listNB, &listNC})
-    for (int32_t x : *v) c->max_cta_tasks = std::max<int64_t>(c->max_cta_tasks, dt->task_off[x + 1] - dt->task_off[x]);
-  UP(c->b_lptA, lptA.data(), int64_t(lptA.size()), int32_t);
-  UP(c->b_lptB, lptB.data(), int64_t(lptB.size()), int32_t);
-  UP(c->b_lptC, lptC.data(), int64_t(lptC.size()), int32_t);
-  UP(c->b_lptNA, lptNA.data(), int64_t(lptNA.size()), int32_t);
-  UP(c->b_lptNB, lptNB.data(), int64_t(lptNB.size()), int32_t);
-  UP(c->b_lptNC, lptNC.data(), int64_t(lptNC.size()), int32_t);
+  for (int r = 0; r < kRoutes; r++)
+    if (is_cta(r))
+      for (int32_t x : list[r]) c->max_cta_tasks = std::max<int64_t>(c->max_cta_tasks, dt->task_off[x + 1] - dt->task_off[x]);
+  for (int r = 0; r < kRoutes; r++)
+    if (largest_first(r)) UP(s, c->routes[r].lpt, lpt[r].data(), int64_t(lpt[r].size()), int32_t);
   // the staging vectors above must outlive the async copies
   CK(cudaStreamSynchronize(s));
   // work buffers
-  const bool on_chip_cta = !(listA.empty() && listB.empty() && listC.empty() && listNA.empty() && listNB.empty() && listNC.empty());
+  const bool on_chip = list[kGeneral].size() < size_t(D);  // some distro is planned by k_plan_cta, k_plan_smem or k_plan_warp
   if (any_complex) {
     CK(c->b_hasdep.ensure(size_t(T) + 16));
     CK(c->b_head.ensure(sizeof(uint32_t) * size_t(U + 1)));
-    if (on_chip_cta || !listW.empty()) {  // k_plan_smem's member lists, by pair id (a breakdown run plans tiny distros with it)
+    if (on_chip) {  // k_plan_smem's member lists, by pair id (a breakdown run plans tiny distros with it)
       CK(c->b_next.ensure(sizeof(uint32_t) * size_t(P + 1)));
       CK(c->b_pslot.ensure(sizeof(uint32_t) * size_t(P + 1)));
     }
@@ -1063,8 +1079,8 @@ int upload_tasks(evg_ctx* c, const evg_task_soa* t, const evg_distro_table* dt, 
     CK(c->b_bestpair.ensure(sizeof(uint32_t) * size_t(T + 1)));
   }
   // k_plan_smem's scratch for value ranges above 32 bits; a breakdown run plans the tiny distros with it too
-  if (on_chip_cta || !listW.empty()) CK(c->b_kv.ensure(sizeof(uint64_t) * size_t(T + 1)));
-  if (n_general > 0) {  // the general path's buffers exist only when a distro takes it
+  if (on_chip) CK(c->b_kv.ensure(sizeof(uint64_t) * size_t(T + 1)));
+  if (!list[kGeneral].empty()) {  // the general path's buffers exist only when a distro takes it
     for (int k = 0; k < 2; k++) {
       CK(c->b_klo[k].ensure(sizeof(uint32_t) * size_t(T + 1)));
       CK(c->b_khi[k].ensure(sizeof(uint32_t) * size_t(T + 1)));
@@ -1102,16 +1118,10 @@ int upload_tasks(evg_ctx* c, const evg_task_soa* t, const evg_distro_table* dt, 
   c->max_groups = 0;
   for (int32_t d = 0; d < D; d++) c->max_groups = std::max(c->max_groups, dt->group_off[d + 1] - dt->group_off[d]);
   c->any_complex = any_complex;
-  c->nW = int32_t(listW.size());
-  c->nA = int32_t(listA.size()); c->nB = int32_t(listB.size()); c->nC = int32_t(listC.size());
-  c->nNA = int32_t(listNA.size()); c->nNB = int32_t(listNB.size()); c->nNC = int32_t(listNC.size());
-  c->n_general = n_general;
   c->general_complex = general_complex;
   CK(c->b_err.ensure(sizeof(int) * 4));
   CK(cudaMemsetAsync(c->b_err.p, 0, sizeof(int) * 4, s));
-  c->h_listW.swap(listW);
-  c->h_listA.swap(listA); c->h_listB.swap(listB); c->h_listC.swap(listC);
-  c->h_listNA.swap(listNA); c->h_listNB.swap(listNB); c->h_listNC.swap(listNC);
+  for (int r = 0; r < kRoutes; r++) c->routes[r].h.swap(list[r]);
   c->h_taskoff.assign(dt->task_off, dt->task_off + D + 1);
   c->h_groupoff.assign(dt->group_off, dt->group_off + D + 1);
   c->h_edgeoff.assign(size_t(D) + 1, 0);
@@ -1119,7 +1129,6 @@ int upload_tasks(evg_ctx* c, const evg_task_soa* t, const evg_distro_table* dt, 
     for (int32_t d = 0; d <= D; d++) c->h_edgeoff[size_t(d)] = edge_off ? edge_off[d] : t->dep_off[dt->task_off[d]];
   c->h_unitbase.swap(unit_base);
   c->h_dtileoff.swap(dtile_off);
-  c->h_listG.swap(listG);
   c->have_tasks = true;
   c->alist_valid = false;  // upload_hosts lists the allocator's distros against THIS table
   c->have_hosts = false;
@@ -1147,19 +1156,19 @@ int upload_hosts(evg_ctx* c, const evg_host_soa* h, const int64_t* host_off, con
   if (D > 0 && host_off[D] != H) return fail(EVG_ERR_INVALID, "host_off[n_distros] != n_hosts");
   if (H > 0 && (!h->flags || !h->group_id || !h->expected_ns || !h->std_ns || !h->start_ns)) return fail(EVG_ERR_INVALID, "null host column");
   cudaStream_t s = c->stream;
-  UP(c->b_hflags, h->flags, H, uint32_t);
-  UP(c->b_hgid, h->group_id, H, int32_t);
-  UP(c->b_hexp, h->expected_ns, H, int64_t);
-  UP(c->b_hstd, h->std_ns, H, int64_t);
-  UP(c->b_hstart, h->start_ns, H, int64_t);
-  if (D > 0) UP(c->b_hostoff, host_off, D + 1, int64_t);
-  UP(c->b_acfg, acfg, D, evg_alloc_cfg);
+  UP(s, c->b_hflags, h->flags, H, uint32_t);
+  UP(s, c->b_hgid, h->group_id, H, int32_t);
+  UP(s, c->b_hexp, h->expected_ns, H, int64_t);
+  UP(s, c->b_hstd, h->std_ns, H, int64_t);
+  UP(s, c->b_hstart, h->start_ns, H, int64_t);
+  if (D > 0) UP(s, c->b_hostoff, host_off, D + 1, int64_t);
+  UP(s, c->b_acfg, acfg, D, evg_alloc_cfg);
   c->alist_valid = false;
   std::vector<int32_t> alist;
   if (c->have_tasks && c->Dn == D && int64_t(c->h_groupoff.size()) == int64_t(D) + 1) {
     for (int32_t d = 0; d < D; d++)
       if (c->h_groupoff[d + 1] != c->h_groupoff[d] || host_off[d + 1] - host_off[d] > kGrouplessHosts) alist.push_back(d);
-    UP(c->b_alist, alist.data(), int64_t(alist.size()), int32_t);
+    UP(s, c->b_alist, alist.data(), int64_t(alist.size()), int32_t);
     CK(cudaStreamSynchronize(s));  // `alist` is a local
     c->n_alist = int64_t(alist.size());
     c->alist_valid = true;
@@ -1170,7 +1179,6 @@ int upload_hosts(evg_ctx* c, const evg_host_soa* h, const int64_t* host_off, con
   c->have_hosts = true;
   return EVG_OK;
 }
-#undef UP
 
 DTasks dtasks(const evg_ctx* c) {
   DTasks t;
@@ -1324,16 +1332,17 @@ int prepare_general(evg_ctx* c, cudaStream_t s, int32_t d0, int32_t d1) {
   return EVG_OK;
 }
 
-// The general path on stream `st` for the general-path distros listG[gfirst .. gfirst + gcount) (evg_plan_general.cuh).
+// The general path on stream `st` for the general-path distros routes[kGeneral][gfirst .. gfirst + gcount) (evg_plan_general.cuh).
 int run_general(evg_ctx* c, cudaStream_t st, const DTasks& dt, const DDistros& dd, const DWork& w, int64_t now, int32_t gfirst,
                 int32_t gcount) {
   if (gcount <= 0) return EVG_OK;
   DGen g = dgen(c);
   const int gc = c->general_complex;
-  const int32_t d_first = c->h_listG[size_t(gfirst)], d_last = c->h_listG[size_t(gfirst + gcount - 1)];
+  const std::vector<int32_t>& gh = c->routes[kGeneral].h;
+  const int32_t d_first = gh[size_t(gfirst)], d_last = gh[size_t(gfirst + gcount - 1)];
   g.tile0 = c->h_dtileoff[size_t(d_first)];
   const unsigned nt = unsigned(c->h_dtileoff[size_t(d_last) + 1] - g.tile0);
-  const int32_t* gl = c->b_listG.as<int32_t>() + gfirst;
+  const int32_t* gl = c->routes[kGeneral].b.as<int32_t>() + gfirst;
   LAUNCH_ON(c, st, k_ginit, grid_for(gcount, 256), 256, g, gl, gcount);
   if (gc && c->E > 0) LAUNCH_ON(c, st, k_gmark, nt, 256, dt, dd, w, g);
   if (c->timed) CK(cudaEventRecord(c->ev_gt0, st));
@@ -1378,6 +1387,50 @@ int ensure_aux_streams(evg_ctx* c) {
   return EVG_OK;
 }
 
+// The resident tick, the resident tick with the unit lists EVG_OPT_BREAKDOWN reads, or one chunk of the pipelined
+// one-shot call.
+enum class Mode { kResident, kBreakdown, kPipelined };
+
+// The planner launch of size class r in `mode`: entries [first, first + n) of its list -- the largest-first copy on the
+// resident tick, the ascending list (cut by chunk) on the pipelined call -- on stream st.  The k_plan_cta classes hand
+// distros back into punt[0 .. *punt_count); r = kPunted replans them, n being how many could come back.
+int plan_route(evg_ctx* c, int r, Mode mode, cudaStream_t st, const DTasks& dt, const DDistros& dd, const DWork& w, int64_t now,
+               int32_t first, int32_t n, int32_t* punt, int32_t* punt_count) {
+  if (n <= 0) return EVG_OK;
+  const int bd = mode == Mode::kBreakdown ? 1 : 0;
+  const int32_t* list = punt;
+  if (r != kPunted) list = (mode != Mode::kPipelined && largest_first(r) ? c->routes[r].lpt : c->routes[r].b).as<int32_t>() + first;
+  // breakdown needs the unit lists: every k_plan_cta distro goes through k_plan_smem (its largest class holds them all)
+  if (bd && is_cta(r)) return launch_smem<EVG_C_THREADS, EVG_C_ITEMS, 1>(c, st, dt, dd, w, list, n, now, 1);
+  int rc;
+  switch (r) {
+    case kCtaC: return launch_cta<kNT_C, kNCapC, kNOccC>(c, st, dt, dd, w, list, n, now, punt, punt_count);
+    case kCtaB: return launch_cta<kNT_B, kNCapB, kNOccB>(c, st, dt, dd, w, list, n, now, punt, punt_count);
+    case kCtaA:
+      if (mode == Mode::kResident) {  // the distros that fit the 64-thread instance are the tail of the largest-first list
+        if ((rc = launch_cta<kNT_A, kNCapA, kNOccA>(c, st, dt, dd, w, list, c->nNA_big, now, punt, punt_count)) != EVG_OK) return rc;
+        return launch_cta<kNT_S, kNCapS, kNOccS>(c, st, dt, dd, w, list + c->nNA_big, n - c->nNA_big, now, punt, punt_count);
+      }
+      return launch_cta<kNT_A, kNCapA, kNOccA>(c, st, dt, dd, w, list, n, now, punt, punt_count);
+    case kPunted:
+      // the resident tick takes the smallest k_plan_smem instance that holds the largest distro given to k_plan_cta (the
+      // launch has one CTA per distro that COULD come back; CTAs beyond *punt_count exit at once, and 10^4 empty
+      // 1024-thread CTAs are not free); the pipelined call always takes the largest
+      if (mode == Mode::kResident && c->max_cta_tasks <= kCapA) return launch_smem<128, 8, 8>(c, st, dt, dd, w, list, n, now, 0, punt_count);
+      if (mode == Mode::kResident && c->max_cta_tasks <= kCapB) return launch_smem<256, 16, 3>(c, st, dt, dd, w, list, n, now, 0, punt_count);
+      return launch_smem<EVG_C_THREADS, EVG_C_ITEMS, 1>(c, st, dt, dd, w, list, n, now, 0, punt_count);
+    case kSmemC: return launch_smem<EVG_C_THREADS, EVG_C_ITEMS, 1>(c, st, dt, dd, w, list, n, now, bd);
+    case kSmemB: return launch_smem<256, 16, 3>(c, st, dt, dd, w, list, n, now, bd);
+    case kSmemA: return launch_smem<128, 8, 8>(c, st, dt, dd, w, list, n, now, bd);
+    case kWarp: return launch_tiny(c, st, dt, dd, w, list, n, now, bd);
+    default: {  // kGeneral; the resident tick prepares all its general-path distros before the routes fork
+      const std::vector<int32_t>& gh = c->routes[kGeneral].h;
+      if (mode == Mode::kPipelined && (rc = prepare_general(c, st, gh[size_t(first)], gh[size_t(first + n - 1)] + 1)) != EVG_OK) return rc;
+      return run_general(c, st, dt, dd, w, now, first, n);
+    }
+  }
+}
+
 int run_plan(evg_ctx* c, int64_t now, uint32_t opts) {
   const int64_t T = c->T;
   const int32_t D = c->Dn;
@@ -1397,62 +1450,39 @@ int run_plan(evg_ctx* c, int64_t now, uint32_t opts) {
     if (c->timed) { CK(cudaEventRecord(c->ev_sort0, s)); CK(cudaEventRecord(c->ev_sort1, s)); }
     return EVG_OK;
   }
-  const bool general = c->n_general > 0;
+  const std::vector<int32_t>& gh = c->routes[kGeneral].h;
+  const bool general = !gh.empty();
   // breakdown mode reads best_pair for every task: tasks emitted from their own single-task unit keep kInactive
   if (bd && c->any_complex) CK(cudaMemsetAsync(c->b_bestpair.p, 0xFF, sizeof(uint32_t) * size_t(T + 1), s));
-  const int32_t n_new = bd ? 0 : c->nNA + c->nNB + c->nNC;
+  const int32_t n_new = bd ? 0 : c->routes[kCtaA].n() + c->routes[kCtaB].n() + c->routes[kCtaC].n();  // could be handed back
   if (n_new > 0) CK(cudaMemsetAsync(c->b_puntcnt.p, 0, sizeof(int32_t), s));
-  if (general) { int rcg = prepare_general(c, s, c->h_listG.front(), c->h_listG.back() + 1); if (rcg != EVG_OK) return rcg; }
+  if (general) { int rcg = prepare_general(c, s, gh.front(), gh.back() + 1); if (rcg != EVG_OK) return rcg; }
   // Routes run side by side when the tick has more than one: fork the aux streams off the context stream here, join
   // them before returning (the allocator and the caller's later work are ordered behind every planner kernel).
-  struct Route { int id; int64_t weight; };
-  const int64_t routes_present = (c->nW > 0) + (c->nA > 0) + (c->nB > 0) + (c->nC > 0) + (n_new > 0 || (bd && (c->nNA + c->nNB + c->nNC) > 0)) + (general ? 1 : 0);
-  const bool fork = routes_present > 1;
+  bool busy[evg_ctx::kAux] = {};
+  for (int r = 0; r < kRoutes; r++) busy[kRouteStream[r]] |= c->routes[r].n() > 0;
+  const bool fork = std::count(busy, busy + evg_ctx::kAux, true) > 1;
   if (fork) {
     int rc0 = ensure_aux_streams(c);
     if (rc0 != EVG_OK) return rc0;
     CK(cudaEventRecord(c->ev_fork, s));
     for (int k = 0; k < evg_ctx::kAux; k++) CK(cudaStreamWaitEvent(c->s_aux[k], c->ev_fork, 0));
   }
-  auto st = [&](int k) { return fork ? c->s_aux[k] : s; };
   int rc;
   const int slot = int(c->runs % evg_ctx::kRing);
-  // --- stream 0: the second-generation on-chip planner (the dominant kernel of configs[1]-like ticks), then the
-  //     distros it handed back
-  if (bd) {  // breakdown needs the unit lists: every on-chip distro goes through k_plan_smem (its largest class holds them all)
-    if ((rc = launch_smem<EVG_C_THREADS, EVG_C_ITEMS, 1>(c, st(0), dt, dd, w, c->b_lptNC.as<int32_t>(), c->nNC, now, 1)) != EVG_OK) return rc;
-    if ((rc = launch_smem<EVG_C_THREADS, EVG_C_ITEMS, 1>(c, st(0), dt, dd, w, c->b_lptNB.as<int32_t>(), c->nNB, now, 1)) != EVG_OK) return rc;
-    if ((rc = launch_smem<EVG_C_THREADS, EVG_C_ITEMS, 1>(c, st(0), dt, dd, w, c->b_lptNA.as<int32_t>(), c->nNA, now, 1)) != EVG_OK) return rc;
-  } else if (n_new > 0) {
-    int32_t* pl = c->b_punt.as<int32_t>();
-    int32_t* pc = c->b_puntcnt.as<int32_t>();
-    const bool time_it = c->timed && !general && c->nNC > 0;
-    if (time_it) CK(cudaEventRecord(c->ring0[slot], st(0)));
-    if ((rc = launch_cta<kNT_C, kNCapC, kNOccC>(c, st(0), dt, dd, w, c->b_lptNC.as<int32_t>(), c->nNC, now, pl, pc)) != EVG_OK) return rc;
-    if (time_it) { CK(cudaEventRecord(c->ring1[slot], st(0))); c->runs++; c->sort_slot = slot; }
-    if ((rc = launch_cta<kNT_B, kNCapB, kNOccB>(c, st(0), dt, dd, w, c->b_lptNB.as<int32_t>(), c->nNB, now, pl, pc)) != EVG_OK) return rc;
-    if ((rc = launch_cta<kNT_A, kNCapA, kNOccA>(c, st(0), dt, dd, w, c->b_lptNA.as<int32_t>(), c->nNA_big, now, pl, pc)) != EVG_OK) return rc;
-    if ((rc = launch_cta<kNT_S, kNCapS, kNOccS>(c, st(0), dt, dd, w, c->b_lptNA.as<int32_t>() + c->nNA_big, c->nNA - c->nNA_big, now, pl, pc)) != EVG_OK) return rc;
-    // the distros handed back: the smallest k_plan_smem instance that holds the largest of them (the launch has one CTA
-    // per distro that COULD come back; CTAs beyond *pc exit at once, and 10^4 empty 1024-thread CTAs are not free)
-    if (c->max_cta_tasks <= kCapA) rc = launch_smem<128, 8, 8>(c, st(0), dt, dd, w, pl, n_new, now, 0, pc);
-    else if (c->max_cta_tasks <= kCapB) rc = launch_smem<256, 16, 3>(c, st(0), dt, dd, w, pl, n_new, now, 0, pc);
-    else rc = launch_smem<EVG_C_THREADS, EVG_C_ITEMS, 1>(c, st(0), dt, dd, w, pl, n_new, now, 0, pc);
-    if (rc != EVG_OK) return rc;
+  const Mode mode = bd ? Mode::kBreakdown : Mode::kResident;
+  // stream 0: k_plan_cta (the dominant kernel of configs[1]-like ticks), then the distros it handed back; streams 1..3:
+  // k_plan_smem (GroupVersions, in-queue dependency edges, very many task groups); 4: tiny distros; 5: the general path
+  for (int r : {kCtaC, kCtaB, kCtaA, kPunted, kSmemC, kSmemB, kSmemA, kWarp, kGeneral}) {
+    const int32_t n = r == kPunted ? n_new : c->routes[r].n();
+    cudaStream_t sr = fork ? c->s_aux[kRouteStream[r]] : s;
+    // the timing ring brackets k_plan_cta's largest class (not in breakdown mode), else k_plan_smem's largest class; a
+    // tick with general-path distros has its own sort events instead
+    const bool time_it = c->timed && !general && c->sort_slot < 0 && n > 0 && (r == kSmemC || (r == kCtaC && !bd));
+    if (time_it) CK(cudaEventRecord(c->ring0[slot], sr));
+    if ((rc = plan_route(c, r, mode, sr, dt, dd, w, now, 0, n, c->b_punt.as<int32_t>(), c->b_puntcnt.as<int32_t>())) != EVG_OK) return rc;
+    if (time_it) { CK(cudaEventRecord(c->ring1[slot], sr)); c->runs++; c->sort_slot = slot; }
   }
-  // --- streams 1..3: first-generation classes (GroupVersions, in-queue dependency edges, very many task groups)
-  {
-    const bool time_it = c->timed && !general && c->sort_slot < 0 && c->nC > 0;
-    if (time_it) CK(cudaEventRecord(c->ring0[slot], st(1)));
-    if ((rc = launch_smem<EVG_C_THREADS, EVG_C_ITEMS, 1>(c, st(1), dt, dd, w, c->b_lptC.as<int32_t>(), c->nC, now, bd ? 1 : 0)) != EVG_OK) return rc;
-    if (time_it) { CK(cudaEventRecord(c->ring1[slot], st(1))); c->runs++; c->sort_slot = slot; }
-  }
-  if ((rc = launch_smem<256, 16, 3>(c, st(2), dt, dd, w, c->b_lptB.as<int32_t>(), c->nB, now, bd ? 1 : 0)) != EVG_OK) return rc;
-  if ((rc = launch_smem<128, 8, 8>(c, st(3), dt, dd, w, c->b_lptA.as<int32_t>(), c->nA, now, bd ? 1 : 0)) != EVG_OK) return rc;
-  // --- stream 4: one warp per tiny distro
-  if ((rc = launch_tiny(c, st(4), dt, dd, w, c->b_listW.as<int32_t>(), c->nW, now, bd ? 1 : 0)) != EVG_OK) return rc;
-  // --- stream 5: the general path
-  if (general && (rc = run_general(c, st(5), dt, dd, w, now, 0, c->n_general)) != EVG_OK) return rc;
   if (fork) {
     for (int k = 0; k < evg_ctx::kAux; k++) {
       CK(cudaEventRecord(c->ev_join[k], c->s_aux[k]));
@@ -1503,20 +1533,6 @@ void evg_shutdown(evg_ctx* c) {
   if (!c) return;
   cudaSetDevice(c->device);
   cudaStreamSynchronize(c->stream);
-  DevBuf* all[] = {&c->b_prio, &c->b_exp, &c->b_qb, &c->b_wb, &c->b_nd, &c->b_tgo, &c->b_gid, &c->b_vid, &c->b_flags,
-                   &c->b_depoff, &c->b_depidx, &c->b_taskoff, &c->b_groupoff, &c->b_cfg, &c->b_gmax, &c->b_unitbase,
-                   &c->b_hasdep, &c->b_head, &c->b_next, &c->b_pslot, &c->b_etask, &c->b_elive, &c->b_unitv, &c->b_unita,
-                   &c->b_unitn, &c->b_unitmask, &c->b_rn0, &c->b_rn1, &c->b_rn2, &c->b_rn3, &c->b_rn4, &c->b_rn5, &c->b_rn6,
-                   &c->b_rn7, &c->b_err, &c->b_dx0, &c->b_dx1, &c->b_dx2, &c->b_dx3, &c->b_dx4, &c->b_dx5, &c->b_dx6, &c->b_dx7,
-                   &c->b_route, &c->b_listW, &c->b_listA, &c->b_listB, &c->b_listC, &c->b_listG, &c->b_listNA, &c->b_listNB,
-                   &c->b_listNC, &c->b_lptA, &c->b_lptB, &c->b_lptC, &c->b_lptNA, &c->b_lptNB, &c->b_lptNC, &c->b_punt, &c->b_puntcnt, &c->b_ca, &c->b_crk, &c->b_bestpair, &c->b_kv, &c->b_vmm,
-                   &c->b_klo[0], &c->b_klo[1], &c->b_khi[0], &c->b_khi[1], &c->b_ix[0], &c->b_ix[1], &c->b_e, &c->b_tilesum,
-                   &c->b_gmisc, &c->b_wl, &c->b_pay, &c->b_place, &c->b_eplace, &c->b_run, &c->b_rank, &c->b_blist, &c->b_tie, &c->b_hlist, &c->b_usum, &c->b_upd, &c->b_tiledistro, &c->b_tilestart, &c->b_dtileoff, &c->b_tilehist,
-                   &c->b_qinfo, &c->b_ginfo, &c->b_order, &c->b_tv, &c->b_bd, &c->b_hflags, &c->b_hgid, &c->b_hexp, &c->b_hstd,
-                   &c->b_hstart, &c->b_hostoff, &c->b_acfg, &c->b_gs, &c->b_result, &c->b_status};
-  for (DevBuf* b : all) b->release();
-  for (DevBuf& b : c->b_pf) b.release();
-  c->b_alist.release();
   for (int k = 0; k < evg_ctx::kRing; k++) { if (c->ring0[k]) cudaEventDestroy(c->ring0[k]); if (c->ring1[k]) cudaEventDestroy(c->ring1[k]); }
   cudaEventDestroy(c->ev_begin); cudaEventDestroy(c->ev_sort0); cudaEventDestroy(c->ev_sort1); cudaEventDestroy(c->ev_end);
   cudaEventDestroy(c->ev_gt0); cudaEventDestroy(c->ev_gt1);
@@ -1526,7 +1542,7 @@ void evg_shutdown(evg_ctx* c) {
   for (int k = 0; k < evg_ctx::kAux; k++) { if (c->s_aux[k]) cudaStreamDestroy(c->s_aux[k]); if (c->ev_join[k]) cudaEventDestroy(c->ev_join[k]); }
   if (c->ev_fork) cudaEventDestroy(c->ev_fork);
   if (c->own_stream) cudaStreamDestroy(c->stream);
-  delete c;
+  delete c;  // its buffers free themselves, on the device selected above
 }
 
 int evg_upload(evg_ctx* c, const evg_task_soa* tasks, const evg_distro_table* distros, const evg_host_soa* hosts,
@@ -1857,30 +1873,17 @@ static int plan_and_alloc_pipelined(evg_ctx* c, const evg_task_soa* t, const evg
     CK(cudaEventRecord(c->ev_h[k], c->s_h2d));
     CK(cudaStreamWaitEvent(s, c->ev_h[k], 0));
     k_validate<<<grid_for(n, 256), 256, 0, s>>>(dtk, dd, w, t0, t0 + n);
-    int32_t first, cnt;
-    {  // second-generation on-chip classes; the distros they hand back are replanned by k_plan_smem right behind them
-      int32_t fC, fB, fA;
-      const int32_t nC = sub(c->h_listNC, d0, d1, &fC), nB = sub(c->h_listNB, d0, d1, &fB), nA = sub(c->h_listNA, d0, d1, &fA);
-      int32_t* pl = c->b_punt.as<int32_t>() + d0;  // a chunk hands back at most its own d1 - d0 distros
-      int32_t* pc = c->b_puntcnt.as<int32_t>() + 1 + k;
-      if ((rc = launch_cta<kNT_C, kNCapC, kNOccC>(c, s, dtk, dd, w, c->b_listNC.as<int32_t>() + fC, nC, now, pl, pc)) != EVG_OK) return rc;
-      if ((rc = launch_cta<kNT_B, kNCapB, kNOccB>(c, s, dtk, dd, w, c->b_listNB.as<int32_t>() + fB, nB, now, pl, pc)) != EVG_OK) return rc;
-      if ((rc = launch_cta<kNT_A, kNCapA, kNOccA>(c, s, dtk, dd, w, c->b_listNA.as<int32_t>() + fA, nA, now, pl, pc)) != EVG_OK) return rc;
-      if ((rc = launch_smem<EVG_C_THREADS, EVG_C_ITEMS, 1>(c, s, dtk, dd, w, pl, nC + nB + nA, now, 0, pc)) != EVG_OK) return rc;
+    // the chunk's distros of each class; what k_plan_cta hands back is replanned by k_plan_smem right behind it, and the
+    // general path runs restricted to the chunk's tiles
+    int32_t* pl = c->b_punt.as<int32_t>() + d0;  // a chunk hands back at most its own d1 - d0 distros
+    int32_t* pc = c->b_puntcnt.as<int32_t>() + 1 + k;
+    int32_t n_cta = 0;
+    for (int r : {kCtaC, kCtaB, kCtaA, kPunted, kGeneral, kSmemC, kSmemB, kSmemA, kWarp}) {
+      int32_t first = 0, cnt = n_cta;
+      if (r != kPunted) cnt = sub(c->routes[r].h, d0, d1, &first);
+      if (is_cta(r)) n_cta += cnt;
+      if ((rc = plan_route(c, r, Mode::kPipelined, s, dtk, dd, w, now, first, cnt, pl, pc)) != EVG_OK) return rc;
     }
-    cnt = sub(c->h_listG, d0, d1, &first);
-    if (cnt > 0) {  // the chunk's general-path distros: same kernels, restricted to their tiles
-      if ((rc = prepare_general(c, s, c->h_listG[size_t(first)], c->h_listG[size_t(first + cnt - 1)] + 1)) != EVG_OK) return rc;
-      if ((rc = run_general(c, s, dtk, dd, w, now, first, cnt)) != EVG_OK) return rc;
-    }
-    cnt = sub(c->h_listC, d0, d1, &first);
-    if ((rc = launch_smem<EVG_C_THREADS, EVG_C_ITEMS, 1>(c, s, dtk, dd, w, c->b_listC.as<int32_t>() + first, cnt, now)) != EVG_OK) return rc;
-    cnt = sub(c->h_listB, d0, d1, &first);
-    if ((rc = launch_smem<256, 16, 3>(c, s, dtk, dd, w, c->b_listB.as<int32_t>() + first, cnt, now)) != EVG_OK) return rc;
-    cnt = sub(c->h_listA, d0, d1, &first);
-    if ((rc = launch_smem<128, 8, 8>(c, s, dtk, dd, w, c->b_listA.as<int32_t>() + first, cnt, now)) != EVG_OK) return rc;
-    cnt = sub(c->h_listW, d0, d1, &first);
-    if ((rc = launch_tiny(c, s, dtk, dd, w, c->b_listW.as<int32_t>() + first, cnt, now, 0)) != EVG_OK) return rc;
     if ((rc = run_alloc_range(c, now, d0, d1)) != EVG_OK) return rc;
     CK(cudaEventRecord(c->ev_c[k], s));
     CK(cudaStreamWaitEvent(c->s_d2h, c->ev_c[k], 0));
@@ -1977,19 +1980,13 @@ static int deps_to_device(evg_ctx* c, const evg_deps_in* in, int both, const int
   if (X > 0 && !in->ext_state) return fail(EVG_ERR_INVALID, "null ext_state");
   if (in->dep_off[0] != 0 || in->dep_off[T] != E) return fail(EVG_ERR_INVALID, "dep_off does not span n_deps");
   cudaStream_t s = c->stream;
-#define UPD(buf, ptr, count, type)                                                                                 \
-  do {                                                                                                             \
-    CK((buf).ensure(sizeof(type) * size_t((count) > 0 ? (count) : 1)));                                            \
-    if ((count) > 0) CK(cudaMemcpyAsync((buf).p, (ptr), sizeof(type) * size_t(count), cudaMemcpyHostToDevice, s)); \
-  } while (0)
-  UPD(c->b_dx0, in->dep_off, T + 1, int64_t);
-  UPD(c->b_dx1, in->dep_kind, E, uint8_t);
-  UPD(c->b_dx2, in->dep_ref, E, int32_t);
-  UPD(c->b_dx3, in->dep_want, E, uint8_t);
-  UPD(c->b_dx4, in->task_state, T, uint8_t);
-  UPD(c->b_dx5, in->task_pre, T, uint8_t);
-  UPD(c->b_dx6, in->ext_state, X, uint8_t);
-#undef UPD
+  UP(s, c->b_dx0, in->dep_off, T + 1, int64_t);
+  UP(s, c->b_dx1, in->dep_kind, E, uint8_t);
+  UP(s, c->b_dx2, in->dep_ref, E, int32_t);
+  UP(s, c->b_dx3, in->dep_want, E, uint8_t);
+  UP(s, c->b_dx4, in->task_state, T, uint8_t);
+  UP(s, c->b_dx5, in->task_pre, T, uint8_t);
+  UP(s, c->b_dx6, in->ext_state, X, uint8_t);
   CK(c->b_dx7.ensure(size_t(T)));
   int64_t* stamp = nullptr;
   const int64_t* fin = nullptr;
@@ -2082,17 +2079,11 @@ int evg_expected_durations_batch(evg_ctx* c, const evg_duration_rows* in, evg_du
   cudaStream_t s = c->stream;
   c->launches = 0;
   c->have_tasks = false;  // shares scratch buffers with the finder entry points
-#define UPX(buf, ptr, count, type)                                                                                 \
-  do {                                                                                                             \
-    CK((buf).ensure(sizeof(type) * size_t((count) > 0 ? (count) : 1)));                                            \
-    if ((count) > 0) CK(cudaMemcpyAsync((buf).p, (ptr), sizeof(type) * size_t(count), cudaMemcpyHostToDevice, s)); \
-  } while (0)
-  UPX(c->b_rn0, in->key, R, int32_t);
-  UPX(c->b_rn1, in->time_taken_ns, R, int64_t);
-  UPX(c->b_rn2, in->start_ns, R, int64_t);
-  UPX(c->b_rn3, in->finish_ns, R, int64_t);
-  UPX(c->b_rn4, in->flags, R, uint8_t);
-#undef UPX
+  UP(s, c->b_rn0, in->key, R, int32_t);
+  UP(s, c->b_rn1, in->time_taken_ns, R, int64_t);
+  UP(s, c->b_rn2, in->start_ns, R, int64_t);
+  UP(s, c->b_rn3, in->finish_ns, R, int64_t);
+  UP(s, c->b_rn4, in->flags, R, uint8_t);
   CK(c->b_rn5.ensure(sizeof(unsigned long long) * 4 * size_t(K)));
   CK(c->b_rn6.ensure(sizeof(evg_duration_stat) * size_t(K)));
   CK(c->b_err.ensure(sizeof(int) * 4));
@@ -2149,19 +2140,13 @@ int evg_find_runnable_batch(evg_ctx* c, const evg_runnable_in* in, int32_t* runn
     int rc = deps_to_device(c, in->deps, 1);
     if (rc != EVG_OK) return rc;
   }
-#define UPR(buf, ptr, count, type)                                                                                 \
-  do {                                                                                                             \
-    CK((buf).ensure(sizeof(type) * size_t((count) > 0 ? (count) : 1)));                                            \
-    if ((count) > 0) CK(cudaMemcpyAsync((buf).p, (ptr), sizeof(type) * size_t(count), cudaMemcpyHostToDevice, s)); \
-  } while (0)
-  UPR(c->b_rn0, in->task_off, D + 1, int64_t);
-  UPR(c->b_rn1, in->sched, T, uint8_t);
-  UPR(c->b_rn2, in->project, T, int32_t);
-  UPR(c->b_rn3, in->project_flags, P, uint8_t);
-  UPR(c->b_rn4, in->valid_off, D + 1, int64_t);
-  UPR(c->b_rn5, in->valid_idx, V, int32_t);
-  UPR(c->b_rn6, in->finder, D, uint8_t);
-#undef UPR
+  UP(s, c->b_rn0, in->task_off, D + 1, int64_t);
+  UP(s, c->b_rn1, in->sched, T, uint8_t);
+  UP(s, c->b_rn2, in->project, T, int32_t);
+  UP(s, c->b_rn3, in->project_flags, P, uint8_t);
+  UP(s, c->b_rn4, in->valid_off, D + 1, int64_t);
+  UP(s, c->b_rn5, in->valid_idx, V, int32_t);
+  UP(s, c->b_rn6, in->finder, D, uint8_t);
   CK(c->b_order.ensure(sizeof(int32_t) * size_t(T + 1)));
   CK(c->b_rn7.ensure(sizeof(int64_t) * size_t(D)));
   DRunnable r;
@@ -2336,34 +2321,30 @@ int evg_plan_from_finder(evg_ctx* c, const evg_runnable_in* in, const evg_task_s
   // 1. Task.DependenciesMet / AllDependenciesSatisfied of every candidate, with the DependenciesMetTime stamps
   int rc = deps_to_device(c, in->deps, 1, dep_finished_ns, now_ns, /*want_stamp=*/true);
   if (rc != EVG_OK) return rc;
-  // 2. the finders (buffers of their own: deps_to_device holds b_rn6 / b_rn7)
-#define UPF(buf, ptr, cnt_, type)                                                                                  \
-  do {                                                                                                             \
-    CK((buf).ensure(sizeof(type) * size_t((cnt_) > 0 ? (cnt_) : 1)));                                              \
-    if ((cnt_) > 0) CK(cudaMemcpyAsync((buf).p, (ptr), sizeof(type) * size_t(cnt_), cudaMemcpyHostToDevice, s));   \
-  } while (0)
-  UPF(c->b_pf[0], in->task_off, D + 1, int64_t);
-  UPF(c->b_pf[1], in->sched, T, uint8_t);
-  UPF(c->b_pf[2], in->project, T, int32_t);
-  UPF(c->b_pf[3], in->project_flags, P, uint8_t);
-  UPF(c->b_pf[4], in->valid_off, D + 1, int64_t);
-  UPF(c->b_pf[5], in->valid_idx, V, int32_t);
-  UPF(c->b_pf[6], in->finder, D, uint8_t);
-  CK(c->b_pf[7].ensure(sizeof(int32_t) * size_t(T + 1)));  // kept lists
-  CK(c->b_pf[8].ensure(sizeof(int64_t) * size_t(D + 1)));  // counts
+  // 2. the finders
+  auto& pf = c->pf;
+  UP(s, pf.task_off, in->task_off, D + 1, int64_t);
+  UP(s, pf.sched, in->sched, T, uint8_t);
+  UP(s, pf.project, in->project, T, int32_t);
+  UP(s, pf.project_flags, in->project_flags, P, uint8_t);
+  UP(s, pf.valid_off, in->valid_off, D + 1, int64_t);
+  UP(s, pf.valid_idx, in->valid_idx, V, int32_t);
+  UP(s, pf.finder, in->finder, D, uint8_t);
+  CK(pf.kept.ensure(sizeof(int32_t) * size_t(T + 1)));
+  CK(pf.count.ensure(sizeof(int64_t) * size_t(D + 1)));
   DRunnable r;
   r.n_tasks = T; r.n_distros = D; r.n_projects = P;
-  r.task_off = c->b_pf[0].as<int64_t>(); r.sched = c->b_pf[1].as<uint8_t>(); r.project = c->b_pf[2].as<int32_t>();
-  r.project_flags = c->b_pf[3].as<uint8_t>(); r.valid_off = c->b_pf[4].as<int64_t>(); r.valid_idx = c->b_pf[5].as<int32_t>();
-  r.finder = c->b_pf[6].as<uint8_t>(); r.met = c->b_dx7.as<uint8_t>();
-  k_runnable<<<unsigned(D), 256, 0, s>>>(r, c->b_pf[7].as<int32_t>(), c->b_pf[8].as<int64_t>(), c->b_err.as<int>());
+  r.task_off = pf.task_off.as<int64_t>(); r.sched = pf.sched.as<uint8_t>(); r.project = pf.project.as<int32_t>();
+  r.project_flags = pf.project_flags.as<uint8_t>(); r.valid_off = pf.valid_off.as<int64_t>(); r.valid_idx = pf.valid_idx.as<int32_t>();
+  r.finder = pf.finder.as<uint8_t>(); r.met = c->b_dx7.as<uint8_t>();
+  k_runnable<<<unsigned(D), 256, 0, s>>>(r, pf.kept.as<int32_t>(), pf.count.as<int64_t>(), c->b_err.as<int>());
   c->launches++;
   CK(cudaGetLastError());
   // 3. the only thing the host needs before the planner can be routed: how many tasks each distro kept
   int bad = 0;
-  CK(cudaMemcpyAsync(count, c->b_pf[8].p, sizeof(int64_t) * size_t(D), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(count, pf.count.p, sizeof(int64_t) * size_t(D), cudaMemcpyDeviceToHost, s));
   CK(cudaMemcpyAsync(&bad, c->b_err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
-  if (runnable) CK(cudaMemcpyAsync(runnable, c->b_pf[7].p, sizeof(int32_t) * size_t(T), cudaMemcpyDeviceToHost, s));
+  if (runnable) CK(cudaMemcpyAsync(runnable, pf.kept.p, sizeof(int32_t) * size_t(T), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   if (bad) return fail(EVG_ERR_INVALID, "a project row or dep_ref is out of range");
   std::vector<int64_t> new_off(size_t(D) + 1, 0);
@@ -2373,69 +2354,73 @@ int evg_plan_from_finder(evg_ctx* c, const evg_runnable_in* in, const evg_task_s
   }
   const int64_t Tn = new_off[size_t(D)];
   // 4. candidate columns to the device, compaction into the context's own buffers
-  UPF(c->b_pf[9], cand->priority, T, int32_t);
-  UPF(c->b_pf[10], cand->num_dependents, T, int32_t);
-  UPF(c->b_pf[11], cand->task_group_order, T, int32_t);
-  UPF(c->b_pf[12], cand->group_id, T, int32_t);
-  UPF(c->b_pf[13], cand->version_id, T, int32_t);
-  UPF(c->b_pf[14], cand->flags, T, uint32_t);
-  UPF(c->b_pf[15], cand->expected_ns, T, int64_t);
-  UPF(c->b_pf[16], cand->queue_basis_ns, T, int64_t);
-  UPF(c->b_pf[17], cand->wait_basis_ns, T, int64_t);
-  UPF(c->b_pf[18], new_off.data(), D + 1, int64_t);
+  UP(s, pf.cand.prio, cand->priority, T, int32_t);
+  UP(s, pf.cand.nd, cand->num_dependents, T, int32_t);
+  UP(s, pf.cand.tgo, cand->task_group_order, T, int32_t);
+  UP(s, pf.cand.gid, cand->group_id, T, int32_t);
+  UP(s, pf.cand.vid, cand->version_id, T, int32_t);
+  UP(s, pf.cand.flags, cand->flags, T, uint32_t);
+  UP(s, pf.cand.exp, cand->expected_ns, T, int64_t);
+  UP(s, pf.cand.qb, cand->queue_basis_ns, T, int64_t);
+  UP(s, pf.cand.wb, cand->wait_basis_ns, T, int64_t);
+  UP(s, pf.new_off, new_off.data(), D + 1, int64_t);
   const size_t np = size_t(Tn + kColPad);
-  for (int k = 19; k <= 23; k++) { CK(c->b_pf[k].ensure(sizeof(int32_t) * np)); CK(cudaMemsetAsync(c->b_pf[k].p, 0, sizeof(int32_t) * np, s)); }
-  CK(c->b_pf[24].ensure(sizeof(uint32_t) * np)); CK(cudaMemsetAsync(c->b_pf[24].p, 0, sizeof(uint32_t) * np, s));
-  for (int k = 25; k <= 27; k++) { CK(c->b_pf[k].ensure(sizeof(int64_t) * np)); CK(cudaMemsetAsync(c->b_pf[k].p, 0, sizeof(int64_t) * np, s)); }
-  CK(c->b_pf[28].ensure(sizeof(int32_t) * size_t(T + 1)));   // new_idx
-  CK(cudaMemsetAsync(c->b_pf[28].p, 0xFF, sizeof(int32_t) * size_t(T + 1), s));
-  CK(c->b_pf[29].ensure(sizeof(int64_t) * size_t(Tn + 1)));  // src_row
+  for (DevBuf* b : {&pf.out.prio, &pf.out.nd, &pf.out.tgo, &pf.out.gid, &pf.out.vid, &pf.out.flags}) {  // 4-byte columns
+    CK(b->ensure(4 * np));
+    CK(cudaMemsetAsync(b->p, 0, 4 * np, s));
+  }
+  for (DevBuf* b : {&pf.out.exp, &pf.out.qb, &pf.out.wb}) {  // 8-byte columns
+    CK(b->ensure(8 * np));
+    CK(cudaMemsetAsync(b->p, 0, 8 * np, s));
+  }
+  CK(pf.new_idx.ensure(sizeof(int32_t) * size_t(T + 1)));
+  CK(cudaMemsetAsync(pf.new_idx.p, 0xFF, sizeof(int32_t) * size_t(T + 1), s));
+  CK(pf.src_row.ensure(sizeof(int64_t) * size_t(Tn + 1)));
   PfCols pc;
-  pc.priority = c->b_pf[9].as<int32_t>(); pc.numdep = c->b_pf[10].as<int32_t>(); pc.tgo = c->b_pf[11].as<int32_t>();
-  pc.gid = c->b_pf[12].as<int32_t>(); pc.vid = c->b_pf[13].as<int32_t>(); pc.flags = c->b_pf[14].as<uint32_t>();
-  pc.expected = c->b_pf[15].as<int64_t>(); pc.qbasis = c->b_pf[16].as<int64_t>(); pc.wbasis = c->b_pf[17].as<int64_t>();
-  pc.o_priority = c->b_pf[19].as<int32_t>(); pc.o_numdep = c->b_pf[20].as<int32_t>(); pc.o_tgo = c->b_pf[21].as<int32_t>();
-  pc.o_gid = c->b_pf[22].as<int32_t>(); pc.o_vid = c->b_pf[23].as<int32_t>(); pc.o_flags = c->b_pf[24].as<uint32_t>();
-  pc.o_expected = c->b_pf[25].as<int64_t>(); pc.o_qbasis = c->b_pf[26].as<int64_t>(); pc.o_wbasis = c->b_pf[27].as<int64_t>();
-  const int64_t* d_new_off = c->b_pf[18].as<int64_t>();
-  const int64_t* d_cand_off = c->b_pf[0].as<int64_t>();
+  pc.priority = pf.cand.prio.as<int32_t>(); pc.numdep = pf.cand.nd.as<int32_t>(); pc.tgo = pf.cand.tgo.as<int32_t>();
+  pc.gid = pf.cand.gid.as<int32_t>(); pc.vid = pf.cand.vid.as<int32_t>(); pc.flags = pf.cand.flags.as<uint32_t>();
+  pc.expected = pf.cand.exp.as<int64_t>(); pc.qbasis = pf.cand.qb.as<int64_t>(); pc.wbasis = pf.cand.wb.as<int64_t>();
+  pc.o_priority = pf.out.prio.as<int32_t>(); pc.o_numdep = pf.out.nd.as<int32_t>(); pc.o_tgo = pf.out.tgo.as<int32_t>();
+  pc.o_gid = pf.out.gid.as<int32_t>(); pc.o_vid = pf.out.vid.as<int32_t>(); pc.o_flags = pf.out.flags.as<uint32_t>();
+  pc.o_expected = pf.out.exp.as<int64_t>(); pc.o_qbasis = pf.out.qb.as<int64_t>(); pc.o_wbasis = pf.out.wb.as<int64_t>();
+  const int64_t* d_new_off = pf.new_off.as<int64_t>();
+  const int64_t* d_cand_off = pf.task_off.as<int64_t>();
   if (Tn > 0) {
-    k_pf_gather<<<grid_for(Tn, 256), 256, 0, s>>>(Tn, D, d_new_off, d_cand_off, c->b_pf[7].as<int32_t>(), pc, c->b_dx7.as<uint8_t>(),
-                                                  c->b_rn7.as<int64_t>(), c->b_pf[28].as<int32_t>(), c->b_pf[29].as<int64_t>());
+    k_pf_gather<<<grid_for(Tn, 256), 256, 0, s>>>(Tn, D, d_new_off, d_cand_off, pf.kept.as<int32_t>(), pc, c->b_dx7.as<uint8_t>(),
+                                                  c->b_rn7.as<int64_t>(), pf.new_idx.as<int32_t>(), pf.src_row.as<int64_t>());
     c->launches++;
   }
   // 5. in-queue dependency edges between kept tasks
   int64_t En = 0;
   std::vector<int64_t> edge_off;
   if (E > 0 && Tn > 0) {
-    UPF(c->b_pf[30], cand->dep_off, T + 1, int64_t);
-    UPF(c->b_pf[31], cand->dep_idx, E, int32_t);
-    CK(c->b_pf[32].ensure(sizeof(int32_t) * size_t(Tn + 1)));                 // surviving edges per kept task
-    CK(c->b_pf[33].ensure(sizeof(int64_t) * size_t(Tn + 1 + kColPad)));       // new dep_off
+    UP(s, pf.dep_off, cand->dep_off, T + 1, int64_t);
+    UP(s, pf.dep_idx, cand->dep_idx, E, int32_t);
+    CK(pf.edge_cnt.ensure(sizeof(int32_t) * size_t(Tn + 1)));               // surviving edges per kept task
+    CK(pf.new_dep_off.ensure(sizeof(int64_t) * size_t(Tn + 1 + kColPad)));
     const int64_t nb = (Tn + 1023) / 1024;
-    CK(c->b_pf[34].ensure(sizeof(int64_t) * size_t(nb + 1)));
-    k_pf_edge_count<<<grid_for(Tn, 256), 256, 0, s>>>(Tn, D, d_new_off, d_cand_off, c->b_pf[29].as<int64_t>(), c->b_pf[30].as<int64_t>(),
-                                                      c->b_pf[31].as<int32_t>(), c->b_pf[28].as<int32_t>(), c->b_pf[32].as<int32_t>());
-    k_scan_blocks<<<unsigned(nb), 1024, 0, s>>>(c->b_pf[32].as<int32_t>(), Tn, c->b_pf[33].as<int64_t>(), c->b_pf[34].as<int64_t>());
-    k_scan_sums<<<1, 1024, 0, s>>>(c->b_pf[34].as<int64_t>(), nb);
-    k_scan_add<<<unsigned(nb), 1024, 0, s>>>(c->b_pf[33].as<int64_t>(), Tn, c->b_pf[34].as<int64_t>(), nb);
+    CK(pf.scan_sum.ensure(sizeof(int64_t) * size_t(nb + 1)));
+    k_pf_edge_count<<<grid_for(Tn, 256), 256, 0, s>>>(Tn, D, d_new_off, d_cand_off, pf.src_row.as<int64_t>(), pf.dep_off.as<int64_t>(),
+                                                      pf.dep_idx.as<int32_t>(), pf.new_idx.as<int32_t>(), pf.edge_cnt.as<int32_t>());
+    k_scan_blocks<<<unsigned(nb), 1024, 0, s>>>(pf.edge_cnt.as<int32_t>(), Tn, pf.new_dep_off.as<int64_t>(), pf.scan_sum.as<int64_t>());
+    k_scan_sums<<<1, 1024, 0, s>>>(pf.scan_sum.as<int64_t>(), nb);
+    k_scan_add<<<unsigned(nb), 1024, 0, s>>>(pf.new_dep_off.as<int64_t>(), Tn, pf.scan_sum.as<int64_t>(), nb);
     c->launches += 4;
-    CK(cudaMemcpyAsync(&En, c->b_pf[33].as<int64_t>() + Tn, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(&En, pf.new_dep_off.as<int64_t>() + Tn, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
     // dep_off sampled at the distro boundaries: what the routing needs of the edges
     edge_off.resize(size_t(D) + 1);
     CK(c->b_rn0.ensure(sizeof(int64_t) * size_t(D + 1)));
-    k_gather_i64<<<grid_for(D + 1, 256), 256, 0, s>>>(c->b_pf[33].as<int64_t>(), d_new_off, c->b_rn0.as<int64_t>(), D + 1);
+    k_gather_i64<<<grid_for(D + 1, 256), 256, 0, s>>>(pf.new_dep_off.as<int64_t>(), d_new_off, c->b_rn0.as<int64_t>(), D + 1);
     CK(cudaMemcpyAsync(edge_off.data(), c->b_rn0.p, sizeof(int64_t) * size_t(D + 1), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
-    CK(c->b_pf[35].ensure(sizeof(int32_t) * size_t(En + 1)));
+    CK(pf.new_dep_idx.ensure(sizeof(int32_t) * size_t(En + 1)));
     if (En > 0) {
-      k_pf_edge_write<<<grid_for(Tn, 256), 256, 0, s>>>(Tn, D, d_new_off, d_cand_off, c->b_pf[29].as<int64_t>(), c->b_pf[30].as<int64_t>(),
-                                                        c->b_pf[31].as<int32_t>(), c->b_pf[28].as<int32_t>(), c->b_pf[33].as<int64_t>(),
-                                                        c->b_pf[35].as<int32_t>());
+      k_pf_edge_write<<<grid_for(Tn, 256), 256, 0, s>>>(Tn, D, d_new_off, d_cand_off, pf.src_row.as<int64_t>(), pf.dep_off.as<int64_t>(),
+                                                        pf.dep_idx.as<int32_t>(), pf.new_idx.as<int32_t>(), pf.new_dep_off.as<int64_t>(),
+                                                        pf.new_dep_idx.as<int32_t>());
       c->launches++;
     }
   }
-#undef UPF
   CK(cudaGetLastError());
   // 6. the compacted table becomes the resident tick (columns stay where they are: context-owned device memory)
   evg_task_soa ts;
@@ -2443,7 +2428,7 @@ int evg_plan_from_finder(evg_ctx* c, const evg_runnable_in* in, const evg_task_s
   ts.n_tasks = Tn; ts.n_edges = En;
   ts.priority = pc.o_priority; ts.num_dependents = pc.o_numdep; ts.task_group_order = pc.o_tgo; ts.group_id = pc.o_gid; ts.version_id = pc.o_vid;
   ts.flags = pc.o_flags; ts.expected_ns = pc.o_expected; ts.queue_basis_ns = pc.o_qbasis; ts.wait_basis_ns = pc.o_wbasis;
-  if (En > 0) { ts.dep_off = c->b_pf[33].as<int64_t>(); ts.dep_idx = c->b_pf[35].as<int32_t>(); }
+  if (En > 0) { ts.dep_off = pf.new_dep_off.as<int64_t>(); ts.dep_idx = pf.new_dep_idx.as<int32_t>(); }
   evg_distro_table dn = *distros;
   dn.task_off = new_off.data();
   rc = upload_tasks(c, &ts, &dn, /*copy_columns=*/false, /*adopt=*/true, (En > 0) ? edge_off.data() : nullptr);
@@ -2565,25 +2550,19 @@ int evg_prioritize_legacy_batch(evg_ctx* c, const evg_legacy_soa* in, const int6
   cudaStream_t s = c->stream;
   c->launches = 0;
   c->have_tasks = false;  // shares scratch buffers with the other entry points
-#define UPL(buf, ptr, count_, type)                                                                                \
-  do {                                                                                                             \
-    CK((buf).ensure(sizeof(type) * size_t((count_) > 0 ? (count_) : 1)));                                          \
-    if ((count_) > 0) CK(cudaMemcpyAsync((buf).p, (ptr), sizeof(type) * size_t(count_), cudaMemcpyHostToDevice, s)); \
-  } while (0)
-  UPL(c->b_exp, in->priority, T, int64_t);
-  UPL(c->b_qb, in->ingest_ns, T, int64_t);
-  UPL(c->b_wb, in->expected_ns, T, int64_t);
-  UPL(c->b_nd, in->num_dependents, T, int32_t);
-  UPL(c->b_prio, in->revision_order, T, int32_t);
-  UPL(c->b_vid, in->project_id, T, int32_t);
-  UPL(c->b_gid, in->tg_rank, T, int32_t);
-  UPL(c->b_rn0, in->tg_pair_id, T, int32_t);
-  UPL(c->b_tgo, in->task_group_order, T, int32_t);
-  UPL(c->b_rn1, in->presort_rank, T, int32_t);
-  UPL(c->b_flags, in->flags, T, uint32_t);
-  UPL(c->b_rn2, list_mode, 3 * int64_t(D), uint8_t);
-  UPL(c->b_taskoff, task_off, D + 1, int64_t);
-#undef UPL
+  UP(s, c->b_exp, in->priority, T, int64_t);
+  UP(s, c->b_qb, in->ingest_ns, T, int64_t);
+  UP(s, c->b_wb, in->expected_ns, T, int64_t);
+  UP(s, c->b_nd, in->num_dependents, T, int32_t);
+  UP(s, c->b_prio, in->revision_order, T, int32_t);
+  UP(s, c->b_vid, in->project_id, T, int32_t);
+  UP(s, c->b_gid, in->tg_rank, T, int32_t);
+  UP(s, c->b_rn0, in->tg_pair_id, T, int32_t);
+  UP(s, c->b_tgo, in->task_group_order, T, int32_t);
+  UP(s, c->b_rn1, in->presort_rank, T, int32_t);
+  UP(s, c->b_flags, in->flags, T, uint32_t);
+  UP(s, c->b_rn2, list_mode, 3 * int64_t(D), uint8_t);
+  UP(s, c->b_taskoff, task_off, D + 1, int64_t);
   CK(c->b_order.ensure(sizeof(int32_t) * size_t(T + 1)));
   CK(c->b_rn3.ensure(sizeof(int32_t) * size_t(T + 1)));
   CK(c->b_rn4.ensure(sizeof(int32_t) * size_t(T + 1)));
@@ -2650,18 +2629,12 @@ int evg_dag_rebuild_batch(evg_ctx* c, const evg_dag_in* in, const int64_t* item_
   cudaStream_t s = c->stream;
   c->launches = 0;
   c->have_tasks = false;  // shares scratch buffers with the planner's resident inputs
-#define UPG(buf, ptr, count_, type)                                                                                \
-  do {                                                                                                             \
-    CK((buf).ensure(sizeof(type) * size_t((count_) > 0 ? (count_) : 1)));                                          \
-    if ((count_) > 0) CK(cudaMemcpyAsync((buf).p, (ptr), sizeof(type) * size_t(count_), cudaMemcpyHostToDevice, s)); \
-  } while (0)
-  UPG(c->b_taskoff, item_off, D + 1, int64_t);
-  UPG(c->b_groupoff, group_off, D + 1, int64_t);
-  UPG(c->b_depoff, in->dep_off, N + 1, int64_t);
-  UPG(c->b_depidx, in->dep_item, E, int32_t);
-  UPG(c->b_gid, in->group_id, N, int32_t);
-  UPG(c->b_tgo, in->group_index, N, int32_t);
-#undef UPG
+  UP(s, c->b_taskoff, item_off, D + 1, int64_t);
+  UP(s, c->b_groupoff, group_off, D + 1, int64_t);
+  UP(s, c->b_depoff, in->dep_off, N + 1, int64_t);
+  UP(s, c->b_depidx, in->dep_item, E, int32_t);
+  UP(s, c->b_gid, in->group_id, N, int32_t);
+  UP(s, c->b_tgo, in->group_index, N, int32_t);
   DevBuf* scratch[] = {&c->b_prio, &c->b_nd, &c->b_vid, &c->b_flags, &c->b_rn0, &c->b_rn1, &c->b_rn2, &c->b_rn3, &c->b_rn4};
   for (DevBuf* b : scratch) CK(b->ensure(sizeof(int32_t) * size_t(N + D + 1)));
   CK(c->b_rn5.ensure(sizeof(int32_t) * size_t(E + 1)));
