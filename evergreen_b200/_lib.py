@@ -90,6 +90,12 @@ class DistroTableStruct(C.Structure):
                 ("group_off", C.c_void_p), ("cfg", C.c_void_p), ("group_max_hosts", C.c_void_p)]
 
 
+class TaskEditStruct(C.Structure):
+    _fields_ = [("n_remove", C.c_int64), ("remove_rows", C.c_void_p), ("insert", C.POINTER(TaskSoAStruct)),
+                ("insert_off", C.c_void_p), ("n_add_edges", C.c_int64), ("add_edge_task", C.c_void_p),
+                ("add_edge_dep", C.c_void_p), ("group_remap", C.c_void_p), ("version_remap", C.c_void_p)]
+
+
 class PlanOutStruct(C.Structure):
     _fields_ = [("order", C.c_void_p), ("total_value", C.c_void_p), ("breakdown", C.c_void_p),
                 ("info", C.c_void_p), ("group_info", C.c_void_p)]
@@ -176,6 +182,7 @@ SYMBOLS = {
     "evg_upload": (C.c_int, [_P, _P, _P, _P, _P, _P]),
     "evg_upload_device": (C.c_int, [_P, _P, _P, _P, _P, _P]),
     "evg_update_tasks": (C.c_int, [_P, C.c_int64, _P, _P]),
+    "evg_edit_tasks": (C.c_int, [_P, _P, _P, _P, _P, _P]),
     "evg_plan_from_finder": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, C.c_int64, _P, _P]),
     "evg_intern_columns": (C.c_int, [_P, _P, C.c_int32]),
     "evg_run_resident": (C.c_int, [_P, C.c_int64, C.c_uint32]),

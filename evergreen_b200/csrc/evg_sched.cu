@@ -80,6 +80,11 @@ struct DevBuf {
     if (owned && p) cudaFree(p);
     p = q; cap = 0; owned = false;
   }
+  void swap(DevBuf& o) {
+    std::swap(p, o.p);
+    std::swap(cap, o.cap);
+    std::swap(owned, o.owned);
+  }
   cudaError_t ensure(size_t bytes) {
     if (!owned) { p = nullptr; cap = 0; owned = true; }
     if (bytes <= cap) return cudaSuccess;
@@ -862,6 +867,17 @@ struct evg_ctx {
     DevBuf new_off, new_idx, src_row;  // compacted task_off; candidate row -> compacted index, and back
     DevBuf dep_off, dep_idx, edge_cnt, new_dep_off, scan_sum, new_dep_idx;  // candidate edges, surviving edges
   } pf;  // evg_plan_from_finder's own buffers (deps_to_device holds b_rn6 / b_rn7)
+  // evg_edit_tasks: resident columns an edit may start from (evg_upload, evg_upload_with_deps, evg_plan_from_finder,
+  // evg_edit_tasks; not borrowed columns, not what a one-shot call left)
+  bool editable = false;
+  struct {
+    TaskCols out;            // the shadow set: the composed table is written here, then swapped with the resident columns
+    DevBuf dep_off, dep_idx; // the composed edges (swapped too)
+    TaskCols ins;            // the inserted rows, staged
+    DevBuf ins_dep_off, ins_dep_idx, rm, add_task, add_dep, gremap, vremap;
+    DevBuf new_off, old_off, old_goff, ins_off, old_vbase, edge_at;  // D+1 tables
+    DevBuf keep, pos, src, scan_sum, edge_cnt, err;
+  } ed;
   DevBuf b_err, b_dx0, b_dx1, b_dx2, b_dx3, b_dx4, b_dx5, b_dx6, b_dx7;
   DevBuf b_route, b_unitv, b_unita, b_unitn, b_unitmask;
   DevBuf b_punt, b_puntcnt;
@@ -879,6 +895,7 @@ struct evg_ctx {
   int64_t n_alist = 0;
   bool alist_valid = false;
   std::vector<int64_t> h_taskoff, h_groupoff, h_unitbase, h_edgeoff, h_dtileoff;
+  std::vector<int32_t> h_nver;  // n_versions of each distro (evg_edit_tasks sizes version_remap by it)
   cudaStream_t s_h2d = nullptr, s_d2h = nullptr;
   static constexpr int kMaxChunks = 16;
   cudaEvent_t ev_h[kMaxChunks] = {}, ev_c[kMaxChunks] = {};
@@ -905,11 +922,20 @@ inline unsigned grid_for(int64_t n, int block) { return unsigned((n + block - 1)
 // Columns are padded so that 128-bit loads and TMA copies that start inside the table may run past its last row.
 constexpr int64_t kColPad = 8;
 
-// Route every distro of the tick, stage the small tables, size the work buffers.  Columns: copied from the host
-// (copy_columns), left for the pipelined call to copy chunk by chunk, or adopted from caller-owned device memory.
+// Where upload_tasks finds the task columns.
+enum class Cols {
+  kCopy,      // host memory: copied into the context's buffers
+  kChunked,   // host memory: the pipelined call copies them chunk by chunk
+  kAdopt,     // device memory the context borrows (evg_upload_device, evg_plan_from_finder's compacted table)
+  kResident,  // already in the context's own buffers (evg_edit_tasks swapped them in): `t` points at them
+};
+
+// Route every distro of the tick, stage the small tables, size the work buffers.  Every mode but kChunked range-checks
+// the ids here (the pipelined call checks chunk by chunk).
 // `edge_off` (D+1, host) is dep_off sampled at the distro boundaries; NULL when the host can read t->dep_off itself.
-int upload_tasks(evg_ctx* c, const evg_task_soa* t, const evg_distro_table* dt, bool copy_columns = true, bool adopt = false,
+int upload_tasks(evg_ctx* c, const evg_task_soa* t, const evg_distro_table* dt, Cols cols = Cols::kCopy,
                  const int64_t* edge_off = nullptr) {
+  const bool copy_columns = cols == Cols::kCopy, adopt = cols == Cols::kAdopt;
   if (!t || !dt) return fail(EVG_ERR_INVALID, "null task table / distro table");
   const int64_t T = t->n_tasks, E = t->n_edges;
   const int32_t D = dt->n_distros;
@@ -1004,6 +1030,7 @@ int upload_tasks(evg_ctx* c, const evg_task_soa* t, const evg_distro_table* dt, 
   cudaStream_t s = c->stream;
 #define UPC(buf, ptr, count, type)                                                                    \
   do {                                                                                                \
+    if (cols == Cols::kResident) break;                                                               \
     if (adopt) {                                                                                      \
       if ((reinterpret_cast<uintptr_t>(ptr) & 15u) != 0) return fail(EVG_ERR_INVALID, "device column %s is not 16-byte aligned", #ptr); \
       (buf).adopt(const_cast<void*>(static_cast<const void*>(ptr)));                                  \
@@ -1127,12 +1154,15 @@ int upload_tasks(evg_ctx* c, const evg_task_soa* t, const evg_distro_table* dt, 
   c->h_edgeoff.assign(size_t(D) + 1, 0);
   if (E > 0)
     for (int32_t d = 0; d <= D; d++) c->h_edgeoff[size_t(d)] = edge_off ? edge_off[d] : t->dep_off[dt->task_off[d]];
+  c->h_nver.resize(size_t(D));
+  for (int32_t d = 0; d < D; d++) c->h_nver[size_t(d)] = dt->cfg[d].n_versions;
   c->h_unitbase.swap(unit_base);
   c->h_dtileoff.swap(dtile_off);
   c->have_tasks = true;
+  c->editable = false;  // the entry point that uploaded says whether evg_edit_tasks may follow
   c->alist_valid = false;  // upload_hosts lists the allocator's distros against THIS table
   c->have_hosts = false;
-  if ((copy_columns || adopt) && T > 0) {  // range-check the ids the kernels index with (the pipelined call checks chunk by chunk)
+  if (cols != Cols::kChunked && T > 0) {  // range-check the ids the kernels index with
     DTasks dtv = dtasks(c);
     DDistros ddv = ddistros(c);
     DWork wv = dwork(c);
@@ -1557,6 +1587,7 @@ int evg_upload(evg_ctx* c, const evg_task_soa* tasks, const evg_distro_table* di
     if (rc != EVG_OK) return rc;
     CK(cudaStreamSynchronize(c->stream));
   }
+  c->editable = true;
   return EVG_OK;
 }
 
@@ -1640,7 +1671,7 @@ int evg_upload_device(evg_ctx* c, const evg_task_soa* tasks, const evg_distro_ta
     CK(cudaMemcpyAsync(edge_off.data(), c->b_rn1.p, sizeof(int64_t) * size_t(D + 1), cudaMemcpyDeviceToHost, c->stream));
     CK(cudaStreamSynchronize(c->stream));
   }
-  int rc = upload_tasks(c, tasks, distros, /*copy_columns=*/false, /*adopt=*/true, edge_off.empty() ? nullptr : edge_off.data());
+  int rc = upload_tasks(c, tasks, distros, Cols::kAdopt, edge_off.empty() ? nullptr : edge_off.data());
   if (rc != EVG_OK) return rc;
   if (hosts) {
     rc = upload_hosts(c, hosts, host_off, acfg, distros->n_distros);
@@ -1797,6 +1828,7 @@ int evg_plan_batch(evg_ctx* c, const evg_task_soa* tasks, const evg_distro_table
   LOCK(c);
   int rc = evg_upload(c, tasks, distros, nullptr, nullptr, nullptr);
   if (rc != EVG_OK) return rc;
+  c->editable = false;  // a one-shot call's tick is not a resident one to edit
   rc = evg_run_resident(c, now_ns, opts);
   if (rc != EVG_OK) return rc;
   return evg_download(c, out, nullptr);
@@ -1919,7 +1951,7 @@ int evg_plan_and_alloc_batch(evg_ctx* c, const evg_task_soa* tasks, const evg_di
   if (!(opts & EVG_OPT_BREAKDOWN) && tasks && distros && tasks->n_tasks >= (int64_t(1) << 21)) {
     // large tick: stage the small tables, then pipeline the columns chunk by chunk
     CK(cudaSetDevice(c->device));
-    int rc0 = upload_tasks(c, tasks, distros, /*copy_columns=*/false);
+    int rc0 = upload_tasks(c, tasks, distros, Cols::kChunked);
     if (rc0 != EVG_OK) return rc0;
     rc0 = upload_hosts(c, hosts, host_off, acfg, distros->n_distros);
     if (rc0 != EVG_OK) return rc0;
@@ -1928,6 +1960,7 @@ int evg_plan_and_alloc_batch(evg_ctx* c, const evg_task_soa* tasks, const evg_di
   }
   int rc = evg_upload(c, tasks, distros, hosts, host_off, acfg);
   if (rc != EVG_OK) return rc;
+  c->editable = false;  // a one-shot call's tick is not a resident one to edit
   rc = evg_run_resident(c, now_ns, opts);
   if (rc != EVG_OK) return rc;
   return evg_download(c, plan_out, alloc_out);
@@ -2431,13 +2464,325 @@ int evg_plan_from_finder(evg_ctx* c, const evg_runnable_in* in, const evg_task_s
   if (En > 0) { ts.dep_off = pf.new_dep_off.as<int64_t>(); ts.dep_idx = pf.new_dep_idx.as<int32_t>(); }
   evg_distro_table dn = *distros;
   dn.task_off = new_off.data();
-  rc = upload_tasks(c, &ts, &dn, /*copy_columns=*/false, /*adopt=*/true, (En > 0) ? edge_off.data() : nullptr);
+  rc = upload_tasks(c, &ts, &dn, Cols::kAdopt, (En > 0) ? edge_off.data() : nullptr);
   if (rc != EVG_OK) return rc;
   if (hosts) {
     rc = upload_hosts(c, hosts, host_off, acfg, D);
     if (rc != EVG_OK) return rc;
   }
   CK(cudaStreamSynchronize(s));
+  c->editable = true;  // the compacted columns are the context's own (pf.out), not the caller's
+  return EVG_OK;
+}
+
+// --------------------------------------------------------------------------
+// evg_edit_tasks: the composed table (survivors, then inserted rows, per distro) built on the device
+// --------------------------------------------------------------------------
+struct EdDst {  // the shadow column set the composed table is written to
+  int32_t *priority, *numdep, *tgo, *gid, *vid;
+  uint32_t* flags;
+  int64_t *expected, *qbasis, *wbasis;
+};
+// Where row i of the composed table comes from.  Distro d's composed rows are its survivors in their resident order
+// (S_d of them), then its inserted rows ins_off[d] .. ins_off[d+1].
+struct EdMap {
+  int32_t D;
+  const int64_t* new_off;    // D+1: composed task_off
+  const int64_t* old_off;    // D+1: resident task_off
+  const int64_t* ins_off;    // D+1: CSR of the inserted rows over distros
+  const int32_t* keep;       // [resident T]: 1 = survives
+  const int64_t* pos;        // [resident T + 1]: exclusive scan of keep (survivors before a resident row, all distros)
+  const int32_t* src;        // [composed T]: resident row of a survivor (unset for inserted rows)
+  const int64_t* old_goff;   // D+1: resident group_off
+  const int64_t* old_vbase;  // D+1: prefix sum of the resident n_versions
+  const int32_t* gremap;     // per resident group slot: new distro-local id, -1 = none; NULL = ids kept
+  const int32_t* vremap;     // per resident (distro, version): new id; NULL = ids kept
+  int64_t n_add;
+  const int64_t* add_task;   // ascending composed row of a survivor that gains an edge
+  const int32_t* add_dep;    // its new distro-local dependency
+};
+__device__ __forceinline__ int64_t ed_survivors(const EdMap& m, int d) {
+  return (m.new_off[d + 1] - m.new_off[d]) - (m.ins_off[d + 1] - m.ins_off[d]);
+}
+// first index in add_task[0, n) that is >= row
+__device__ __forceinline__ int64_t ed_lower(const int64_t* __restrict__ a, int64_t n, int64_t row) {
+  int64_t lo = 0, hi = n;
+  while (lo < hi) {
+    const int64_t mid = (lo + hi) >> 1;
+    if (a[mid] < row) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+// keep[t] = 0 for the removed rows (ascending rm), 1 otherwise
+__global__ void __launch_bounds__(256) k_ed_keep(int64_t n_old, const int64_t* __restrict__ rm, int64_t n_rm, int32_t* __restrict__ keep) {
+  const int64_t t = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (t >= n_old) return;
+  const int64_t k = ed_lower(rm, n_rm, t);
+  keep[t] = (k < n_rm && rm[k] == t) ? 0 : 1;
+}
+// src[composed row of survivor t] = t: a distro's survivors keep their order, behind the inserted rows of the distros before it
+__global__ void __launch_bounds__(256) k_ed_src(int64_t n_old, EdMap m, int32_t* __restrict__ src) {
+  const int64_t t = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  const int d = block_find_distro(m.old_off, m.D, t, n_old);
+  if (d < 0 || !m.keep[t]) return;
+  src[m.pos[t] + m.ins_off[d]] = int32_t(t);
+}
+// One thread per composed row: a survivor's row of the resident columns (group and version ids remapped), or a staged
+// inserted row.  err[0] = 1 when a survivor's task group maps to -1.
+__global__ void __launch_bounds__(256) k_ed_gather(int64_t n_new, EdMap m, DTasks O, DTasks I, EdDst o, int* __restrict__ err) {
+  const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  const int d = block_find_distro(m.new_off, m.D, i, n_new);
+  if (d < 0) return;
+  const int64_t k = i - m.new_off[d], S = ed_survivors(m, d);
+  if (k < S) {
+    const int64_t t = m.src[i];
+    int32_t gid = O.gid[t], vid = O.vid[t];
+    if (m.gremap && gid >= 0) {
+      gid = m.gremap[m.old_goff[d] + gid];
+      if (gid < 0) *err = 1;
+    }
+    if (m.vremap) vid = m.vremap[m.old_vbase[d] + vid];
+    o.priority[i] = O.priority[t]; o.numdep[i] = O.numdep[t]; o.tgo[i] = O.tgo[t]; o.gid[i] = gid; o.vid[i] = vid;
+    o.flags[i] = O.flags[t]; o.expected[i] = O.expected[t]; o.qbasis[i] = O.qbasis[t]; o.wbasis[i] = O.wbasis[t];
+  } else {
+    const int64_t j = m.ins_off[d] + (k - S);
+    o.priority[i] = I.priority[j]; o.numdep[i] = I.numdep[j]; o.tgo[i] = I.tgo[j]; o.gid[i] = I.gid[j]; o.vid[i] = I.vid[j];
+    o.flags[i] = I.flags[j]; o.expected[i] = I.expected[j]; o.qbasis[i] = I.qbasis[j]; o.wbasis[i] = I.wbasis[j];
+  }
+}
+// Edges of composed row i: a survivor's resident edges whose dependency survived, re-indexed and in their order, then
+// its added edges; an inserted row's own edges.  cnt != NULL: count them; otherwise write them at o_dep_off[i].
+__device__ __forceinline__ int64_t ed_edges(const EdMap& m, const DTasks& O, const DTasks& I, int64_t i, int d,
+                                            const int64_t* __restrict__ o_dep_off, int32_t* __restrict__ o_dep_idx) {
+  const int64_t k = i - m.new_off[d], S = ed_survivors(m, d);
+  int64_t w = o_dep_off ? o_dep_off[i] : 0, n = 0;
+  if (k < S) {
+    const int64_t t = m.src[i], base = m.old_off[d];
+    if (O.n_edges > 0) {
+      const int64_t first = m.pos[base];
+      for (int64_t e = O.dep_off[t]; e < O.dep_off[t + 1]; e++) {
+        const int64_t u = base + O.dep_idx[e];
+        if (!m.keep[u]) continue;
+        if (o_dep_idx) o_dep_idx[w + n] = int32_t(m.pos[u] - first);
+        n++;
+      }
+    }
+    if (m.n_add > 0)
+      for (int64_t a = ed_lower(m.add_task, m.n_add, i); a < m.n_add && m.add_task[a] == i; a++) {
+        if (o_dep_idx) o_dep_idx[w + n] = m.add_dep[a];
+        n++;
+      }
+  } else if (I.n_edges > 0) {
+    const int64_t j = m.ins_off[d] + (k - S);
+    for (int64_t e = I.dep_off[j]; e < I.dep_off[j + 1]; e++) {
+      if (o_dep_idx) o_dep_idx[w + n] = I.dep_idx[e];
+      n++;
+    }
+  }
+  return n;
+}
+__global__ void __launch_bounds__(256) k_ed_edge_count(int64_t n_new, EdMap m, DTasks O, DTasks I, int32_t* __restrict__ cnt) {
+  const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  const int d = block_find_distro(m.new_off, m.D, i, n_new);
+  if (d < 0) return;
+  cnt[i] = int32_t(ed_edges(m, O, I, i, d, nullptr, nullptr));
+}
+__global__ void __launch_bounds__(256) k_ed_edge_write(int64_t n_new, EdMap m, DTasks O, DTasks I, const int64_t* __restrict__ o_dep_off,
+                                                       int32_t* __restrict__ o_dep_idx) {
+  const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  const int d = block_find_distro(m.new_off, m.D, i, n_new);
+  if (d < 0) return;
+  ed_edges(m, O, I, i, d, o_dep_off, o_dep_idx);
+}
+
+int evg_edit_tasks(evg_ctx* c, const evg_task_edit* ed, const evg_distro_table* distros, const evg_host_soa* hosts,
+                   const int64_t* host_off, const evg_alloc_cfg* acfg) {
+  if (!c) return fail(EVG_ERR_INVALID, "null context");
+  LOCK(c);
+  if (!c->have_tasks) return fail(EVG_ERR_STATE, "evg_edit_tasks before evg_upload");
+  if (!c->editable)
+    return fail(EVG_ERR_STATE, c->adopted ? "the resident columns are borrowed (evg_upload_device): edit them in place instead"
+                                          : "the resident tick was left by a one-shot call: evg_upload it first");
+  if (!ed || !distros) return fail(EVG_ERR_INVALID, "evg_edit_tasks: null edit / distro table");
+  // ---- every check the host can make, before anything resident changes
+  const int32_t D = c->Dn;
+  const int64_t T0 = c->T, R = ed->n_remove, NA = ed->n_add_edges;
+  const evg_task_soa* ins = ed->insert;
+  const int64_t I = ins ? ins->n_tasks : 0, EI = ins ? ins->n_edges : 0;
+  if (distros->n_distros != D) return fail(EVG_ERR_INVALID, "evg_edit_tasks: n_distros %d, the resident tick has %d", distros->n_distros, D);
+  if (R < 0 || I < 0 || EI < 0 || NA < 0) return fail(EVG_ERR_INVALID, "evg_edit_tasks: negative sizes");
+  if (R > 0 && !ed->remove_rows) return fail(EVG_ERR_INVALID, "evg_edit_tasks: null remove_rows");
+  if (I > 0 && (!ed->insert_off || !ins->priority || !ins->expected_ns || !ins->queue_basis_ns || !ins->wait_basis_ns ||
+                !ins->num_dependents || !ins->task_group_order || !ins->group_id || !ins->version_id || !ins->flags))
+    return fail(EVG_ERR_INVALID, "evg_edit_tasks: null insert_off / inserted column");
+  if (EI > 0 && (I == 0 || !ins->dep_off || !ins->dep_idx)) return fail(EVG_ERR_INVALID, "evg_edit_tasks: inserted edges without dep_off / dep_idx");
+  if (NA > 0 && (!ed->add_edge_task || !ed->add_edge_dep)) return fail(EVG_ERR_INVALID, "evg_edit_tasks: null added edges");
+  if (D > 0 && (!distros->task_off || !distros->group_off || !distros->cfg)) return fail(EVG_ERR_INVALID, "evg_edit_tasks: null distro arrays");
+  if (D == 0 && (R > 0 || I > 0)) return fail(EVG_ERR_INVALID, "evg_edit_tasks: rows without distros");
+  std::vector<int64_t> removed(size_t(D) + 1, 0), ins_off(size_t(D) + 1, 0), old_vbase(size_t(D) + 1, 0);
+  for (int64_t k = 0; k < R; k++) {
+    const int64_t r = ed->remove_rows[k];
+    if (r < 0 || r >= T0 || (k > 0 && r <= ed->remove_rows[k - 1]))
+      return fail(EVG_ERR_INVALID, "evg_edit_tasks: remove_rows[%lld] = %lld is not ascending inside [0, %lld)", (long long)k, (long long)r, (long long)T0);
+    removed[size_t(std::upper_bound(c->h_taskoff.begin(), c->h_taskoff.end(), r) - c->h_taskoff.begin() - 1)]++;
+  }
+  if (I > 0) {
+    if (ed->insert_off[0] != 0 || ed->insert_off[D] != I) return fail(EVG_ERR_INVALID, "evg_edit_tasks: insert_off does not span the inserted rows");
+    ins_off.assign(ed->insert_off, ed->insert_off + D + 1);
+  }
+  if (EI > 0) {
+    if (ins->dep_off[0] != 0 || ins->dep_off[I] != EI) return fail(EVG_ERR_INVALID, "evg_edit_tasks: the inserted dep_off does not span n_edges");
+    for (int64_t j = 0; j < I; j++)
+      if (ins->dep_off[j + 1] < ins->dep_off[j]) return fail(EVG_ERR_INVALID, "evg_edit_tasks: the inserted dep_off decreases at row %lld", (long long)j);
+  }
+  if (D > 0 && (distros->task_off[0] != 0 || distros->group_off[0] != 0)) return fail(EVG_ERR_INVALID, "evg_edit_tasks: offsets must start at 0");
+  for (int32_t d = 0; d < D; d++) {
+    if (ins_off[d + 1] < ins_off[d]) return fail(EVG_ERR_INVALID, "evg_edit_tasks: insert_off decreases at distro %d", d);
+    if (distros->group_off[d + 1] < distros->group_off[d]) return fail(EVG_ERR_INVALID, "evg_edit_tasks: group_off decreases at distro %d", d);
+    const int64_t want = (c->h_taskoff[d + 1] - c->h_taskoff[d]) - removed[d] + (ins_off[d + 1] - ins_off[d]);
+    if (distros->task_off[d + 1] - distros->task_off[d] != want)
+      return fail(EVG_ERR_INVALID, "evg_edit_tasks: distro %d holds %lld tasks after the edit, task_off says %lld", d, (long long)want,
+                  (long long)(distros->task_off[d + 1] - distros->task_off[d]));
+    old_vbase[d + 1] = old_vbase[d] + c->h_nver[d];
+  }
+  const int64_t Tn = D > 0 ? distros->task_off[D] : 0;
+  for (int64_t k = 0, d = 0; k < NA; k++) {
+    const int64_t row = ed->add_edge_task[k];
+    if (k > 0 && row < ed->add_edge_task[k - 1]) return fail(EVG_ERR_INVALID, "evg_edit_tasks: add_edge_task is not ascending at %lld", (long long)k);
+    if (row < 0 || row >= Tn) return fail(EVG_ERR_INVALID, "evg_edit_tasks: add_edge_task[%lld] = %lld is outside the composed table", (long long)k, (long long)row);
+    while (distros->task_off[d + 1] <= row) d++;
+    const int64_t survivors = (c->h_taskoff[d + 1] - c->h_taskoff[d]) - removed[d];
+    if (row - distros->task_off[d] >= survivors)
+      return fail(EVG_ERR_INVALID, "evg_edit_tasks: add_edge_task[%lld] = %lld is not a surviving task", (long long)k, (long long)row);
+  }
+  CK(cudaSetDevice(c->device));
+  cudaStream_t s = c->stream;
+  auto& e = c->ed;
+  c->launches = 0;
+  // ---- stage the edit
+  UP(s, e.rm, ed->remove_rows, R, int64_t);
+  UP(s, e.ins.prio, ins ? ins->priority : nullptr, I, int32_t);
+  UP(s, e.ins.nd, ins ? ins->num_dependents : nullptr, I, int32_t);
+  UP(s, e.ins.tgo, ins ? ins->task_group_order : nullptr, I, int32_t);
+  UP(s, e.ins.gid, ins ? ins->group_id : nullptr, I, int32_t);
+  UP(s, e.ins.vid, ins ? ins->version_id : nullptr, I, int32_t);
+  UP(s, e.ins.flags, ins ? ins->flags : nullptr, I, uint32_t);
+  UP(s, e.ins.exp, ins ? ins->expected_ns : nullptr, I, int64_t);
+  UP(s, e.ins.qb, ins ? ins->queue_basis_ns : nullptr, I, int64_t);
+  UP(s, e.ins.wb, ins ? ins->wait_basis_ns : nullptr, I, int64_t);
+  UP(s, e.ins_dep_off, EI > 0 ? ins->dep_off : nullptr, EI > 0 ? I + 1 : 0, int64_t);
+  UP(s, e.ins_dep_idx, EI > 0 ? ins->dep_idx : nullptr, EI, int32_t);
+  UP(s, e.add_task, ed->add_edge_task, NA, int64_t);
+  UP(s, e.add_dep, ed->add_edge_dep, NA, int32_t);
+  const int64_t G0 = c->h_groupoff[size_t(D)];
+  UP(s, e.gremap, ed->group_remap, ed->group_remap ? G0 : 0, int32_t);
+  UP(s, e.vremap, ed->version_remap, ed->version_remap ? old_vbase[D] : 0, int32_t);
+  UP(s, e.new_off, distros->task_off, D + 1, int64_t);
+  UP(s, e.old_off, c->h_taskoff.data(), D + 1, int64_t);
+  UP(s, e.old_goff, c->h_groupoff.data(), D + 1, int64_t);
+  UP(s, e.ins_off, ins_off.data(), D + 1, int64_t);
+  UP(s, e.old_vbase, old_vbase.data(), D + 1, int64_t);
+  CK(e.keep.ensure(sizeof(int32_t) * size_t(T0 + 1)));
+  CK(e.pos.ensure(sizeof(int64_t) * size_t(T0 + 1)));
+  CK(e.src.ensure(sizeof(int32_t) * size_t(Tn + 1)));
+  CK(e.scan_sum.ensure(sizeof(int64_t) * size_t((std::max(T0, Tn) + 1023) / 1024 + 1)));  // both scans' block sums
+  CK(e.err.ensure(sizeof(int)));
+  CK(cudaMemsetAsync(e.err.p, 0, sizeof(int), s));
+  EdMap m;
+  m.D = D; m.new_off = e.new_off.as<int64_t>(); m.old_off = e.old_off.as<int64_t>(); m.ins_off = e.ins_off.as<int64_t>();
+  m.keep = e.keep.as<int32_t>(); m.pos = e.pos.as<int64_t>(); m.src = e.src.as<int32_t>();
+  m.old_goff = e.old_goff.as<int64_t>(); m.old_vbase = e.old_vbase.as<int64_t>();
+  m.gremap = ed->group_remap ? e.gremap.as<int32_t>() : nullptr;
+  m.vremap = ed->version_remap ? e.vremap.as<int32_t>() : nullptr;
+  m.n_add = NA; m.add_task = e.add_task.as<int64_t>(); m.add_dep = e.add_dep.as<int32_t>();
+  const DTasks O = dtasks(c);
+  DTasks In;
+  memset(&In, 0, sizeof(In));
+  In.n = I; In.n_edges = EI;
+  In.priority = e.ins.prio.as<int32_t>(); In.expected = e.ins.exp.as<int64_t>(); In.qbasis = e.ins.qb.as<int64_t>();
+  In.wbasis = e.ins.wb.as<int64_t>(); In.numdep = e.ins.nd.as<int32_t>(); In.tgo = e.ins.tgo.as<int32_t>();
+  In.gid = e.ins.gid.as<int32_t>(); In.vid = e.ins.vid.as<int32_t>(); In.flags = e.ins.flags.as<uint32_t>();
+  In.dep_off = e.ins_dep_off.as<int64_t>(); In.dep_idx = e.ins_dep_idx.as<int32_t>();
+  // ---- 1. survivors: keep mask, its scan (each survivor's place), composed row -> resident row
+  if (T0 > 0) {
+    const int64_t nb = (T0 + 1023) / 1024;
+    k_ed_keep<<<grid_for(T0, 256), 256, 0, s>>>(T0, e.rm.as<int64_t>(), R, e.keep.as<int32_t>());
+    k_scan_blocks<<<unsigned(nb), 1024, 0, s>>>(e.keep.as<int32_t>(), T0, e.pos.as<int64_t>(), e.scan_sum.as<int64_t>());
+    k_scan_sums<<<1, 1024, 0, s>>>(e.scan_sum.as<int64_t>(), nb);
+    k_scan_add<<<unsigned(nb), 1024, 0, s>>>(e.pos.as<int64_t>(), T0, e.scan_sum.as<int64_t>(), nb);
+    k_ed_src<<<grid_for(T0, 256), 256, 0, s>>>(T0, m, e.src.as<int32_t>());
+    c->launches += 5;
+  }
+  // ---- 2. the nine columns of the composed table into the shadow set (its padding zeroed, as an upload leaves it)
+  auto& sh = e.out;
+  const size_t np = size_t(Tn + kColPad);
+  for (DevBuf* b : {&sh.prio, &sh.nd, &sh.tgo, &sh.gid, &sh.vid, &sh.flags}) {
+    CK(b->ensure(4 * np));
+    CK(cudaMemsetAsync(b->as<int32_t>() + Tn, 0, 4 * kColPad, s));
+  }
+  for (DevBuf* b : {&sh.exp, &sh.qb, &sh.wb}) {
+    CK(b->ensure(8 * np));
+    CK(cudaMemsetAsync(b->as<int64_t>() + Tn, 0, 8 * kColPad, s));
+  }
+  EdDst o;
+  o.priority = sh.prio.as<int32_t>(); o.numdep = sh.nd.as<int32_t>(); o.tgo = sh.tgo.as<int32_t>(); o.gid = sh.gid.as<int32_t>();
+  o.vid = sh.vid.as<int32_t>(); o.flags = sh.flags.as<uint32_t>(); o.expected = sh.exp.as<int64_t>(); o.qbasis = sh.qb.as<int64_t>();
+  o.wbasis = sh.wb.as<int64_t>();
+  if (Tn > 0) {
+    k_ed_gather<<<grid_for(Tn, 256), 256, 0, s>>>(Tn, m, O, In, o, e.err.as<int>());
+    c->launches++;
+  }
+  // ---- 3. edges: count, scan, dep_off at the distro boundaries for the routing (one D2H, one sync), write
+  int64_t En = 0;
+  std::vector<int64_t> edge_off;
+  int bad = 0;
+  const bool edges = Tn > 0 && (c->E > 0 || EI > 0 || NA > 0);
+  if (edges) {
+    const int64_t nb = (Tn + 1023) / 1024;
+    CK(e.edge_cnt.ensure(sizeof(int32_t) * size_t(Tn + 1)));
+    CK(e.dep_off.ensure(sizeof(int64_t) * size_t(Tn + 1 + kColPad)));
+    k_ed_edge_count<<<grid_for(Tn, 256), 256, 0, s>>>(Tn, m, O, In, e.edge_cnt.as<int32_t>());
+    k_scan_blocks<<<unsigned(nb), 1024, 0, s>>>(e.edge_cnt.as<int32_t>(), Tn, e.dep_off.as<int64_t>(), e.scan_sum.as<int64_t>());
+    k_scan_sums<<<1, 1024, 0, s>>>(e.scan_sum.as<int64_t>(), nb);
+    k_scan_add<<<unsigned(nb), 1024, 0, s>>>(e.dep_off.as<int64_t>(), Tn, e.scan_sum.as<int64_t>(), nb);
+    CK(e.edge_at.ensure(sizeof(int64_t) * size_t(D + 1)));
+    k_gather_i64<<<grid_for(D + 1, 256), 256, 0, s>>>(e.dep_off.as<int64_t>(), e.new_off.as<int64_t>(), e.edge_at.as<int64_t>(), D + 1);
+    c->launches += 5;
+    edge_off.resize(size_t(D) + 1);
+    CK(cudaMemcpyAsync(edge_off.data(), e.edge_at.p, sizeof(int64_t) * size_t(D + 1), cudaMemcpyDeviceToHost, s));
+  }
+  CK(cudaMemcpyAsync(&bad, e.err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  if (bad) { c->have_tasks = false; return fail(EVG_ERR_INVALID, "evg_edit_tasks: group_remap maps the task group of a surviving task to -1"); }
+  if (edges) {
+    En = edge_off[size_t(D)];
+    CK(e.dep_idx.ensure(sizeof(int32_t) * size_t(En + kColPad)));
+    if (En > 0) {
+      k_ed_edge_write<<<grid_for(Tn, 256), 256, 0, s>>>(Tn, m, O, In, e.dep_off.as<int64_t>(), e.dep_idx.as<int32_t>());
+      c->launches++;
+      CK(cudaGetLastError());
+    }
+  }
+  // ---- 4. the shadow set becomes the resident one; route, size and range-check the composed table like an upload
+  c->b_prio.swap(sh.prio); c->b_nd.swap(sh.nd); c->b_tgo.swap(sh.tgo); c->b_gid.swap(sh.gid); c->b_vid.swap(sh.vid);
+  c->b_flags.swap(sh.flags); c->b_exp.swap(sh.exp); c->b_qb.swap(sh.qb); c->b_wb.swap(sh.wb);
+  if (En > 0) { c->b_depoff.swap(e.dep_off); c->b_depidx.swap(e.dep_idx); }
+  evg_task_soa ts;
+  memset(&ts, 0, sizeof(ts));
+  ts.n_tasks = Tn; ts.n_edges = En;
+  ts.priority = c->b_prio.as<int32_t>(); ts.num_dependents = c->b_nd.as<int32_t>(); ts.task_group_order = c->b_tgo.as<int32_t>();
+  ts.group_id = c->b_gid.as<int32_t>(); ts.version_id = c->b_vid.as<int32_t>(); ts.flags = c->b_flags.as<uint32_t>();
+  ts.expected_ns = c->b_exp.as<int64_t>(); ts.queue_basis_ns = c->b_qb.as<int64_t>(); ts.wait_basis_ns = c->b_wb.as<int64_t>();
+  if (En > 0) { ts.dep_off = c->b_depoff.as<int64_t>(); ts.dep_idx = c->b_depidx.as<int32_t>(); }
+  int rc = upload_tasks(c, &ts, distros, Cols::kResident, En > 0 ? edge_off.data() : nullptr);
+  if (rc != EVG_OK) { c->have_tasks = false; return rc; }
+  if (hosts) {
+    rc = upload_hosts(c, hosts, host_off, acfg, D);
+    if (rc != EVG_OK) return rc;
+    CK(cudaStreamSynchronize(s));
+  }
+  c->editable = true;
   return EVG_OK;
 }
 

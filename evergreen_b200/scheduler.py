@@ -163,6 +163,20 @@ class Engine:
         vs = values.struct()
         L.check(self.lib.evg_update_tasks(self.ctx, int(rows.shape[0]), L.ptr(rows), C.byref(vs)))
 
+    def edit_tasks(self, edit: S.TaskEdit, distros: S.DistroTable, hosts: Optional[S.HostSoA] = None) -> None:
+        """evg_edit_tasks: rows leave and join the resident queues on the device; `distros` is the new distro table
+        (soa.apply_edit builds it).  The context then holds the tick a fresh upload of the composed table would."""
+        es, keep = edit.normalize().struct()
+        ds = distros.struct()
+        hargs = (None, None, None)
+        if hosts is not None:
+            hs = hosts.struct()
+            hargs = (C.byref(hs), L.ptr(hosts.host_off), L.ptr(hosts.cfg) if hosts.cfg.shape[0] else None)
+        L.check(self.lib.evg_edit_tasks(self.ctx, C.byref(es), C.byref(ds), *hargs))
+        del keep
+        self._n_tasks, self._n_distros, self._n_groups = int(distros.task_off[-1]), distros.n_distros, distros.n_groups
+        self._has_hosts = hosts is not None
+
     def run(self, now: int, opts: int = 0) -> None:
         L.check(self.lib.evg_run_resident(self.ctx, int(now), int(opts)))
 
@@ -397,6 +411,11 @@ def plan_distros(batch: Sequence[Tuple[M.Distro, List[M.Task]]], now: int, *, en
     eng = engine or default_engine()
     soa, table, keys = S.marshal_tasks(batch, now, dependency_db)
     _upload_with_device_deps(eng, batch, soa, table, None, now, dependency_db)
+    return _ranked_results(eng, batch, table, keys, now, breakdown, secondary)
+
+
+def _ranked_results(eng: Engine, batch, table, keys, now: int, breakdown: bool, secondary: bool):
+    """Run the resident tick and turn its outputs into plan_distros' result: per distro (ranked [Task], DistroQueueInfo)."""
     eng.run(now, L.EVG_OPT_BREAKDOWN if breakdown else 0)
     po, _ = eng.download(want_breakdown=breakdown, want_alloc=False)
     out = []
@@ -415,6 +434,143 @@ def plan_distros(batch: Sequence[Tuple[M.Distro, List[M.Task]]], now: int, *, en
         info.secondary_queue = secondary  # scheduler.go:44
         out.append((ranked, info))
     return out
+
+
+class ResidentTick:
+    """The tick-to-tick cache a shim keeps so that only changes cross PCIe: the last batch's marshalled columns, each
+    distro's task ids in resident order and a map from task id to row.  plan() takes the next Go-level batch, derives
+    the edit (tasks dispatched or gone, arrivals, the in-queue dependencies survivors gained, group and version ids
+    remapped to what marshal_tasks assigns on the composed order) and the evg_update_tasks rows of changed scalars, runs
+    the tick and returns what plan_distros returns.  A change an edit cannot express (another distro list, a survivor
+    that moved task group or lost a dependency that stays queued) uploads the batch instead.
+
+    Canonical input order: survivors in their previous order, then arrivals in batch order (input order reaches the
+    output only through the tie policy, and the reference's is arbitrary).  Task.DependenciesMet is evaluated on the host
+    for every task of the batch (soa.dependencies_met), so the inserted rows carry their bit and survivors whose verdict
+    changed are updated.  The engine must not run other ticks between two plan() calls."""
+
+    SCALARS = ("priority", "expected_ns", "queue_basis_ns", "wait_basis_ns", "num_dependents", "task_group_order", "flags")
+
+    def __init__(self, engine: Optional[Engine] = None, dependency_db: Optional[Dict[str, M.Task]] = None):
+        self.engine = engine  # None: default_engine() at the first plan()
+        self.dependency_db = dependency_db
+        self.distro_ids: Optional[List[str]] = None
+        self.ids: List[List[str]] = []   # per distro: task ids in resident order
+        self.row: Dict[str, int] = {}    # task id -> row of the resident table
+        self.soa = self.table = self.keys = None
+        self.last = None                 # (edit, update rows) of the last plan(), None when it uploaded
+
+    def canonical(self, batch):
+        """The batch in canonical order: survivors in their previous order, then arrivals in batch order."""
+        if self.distro_ids is None or [d.id for d, _ in batch] != self.distro_ids:
+            return [(d, list(ts)) for d, ts in batch]
+        out = []
+        for (d, ts), prev in zip(batch, self.ids):
+            by_id = {t.id: t for t in ts}
+            seen = set(prev)
+            out.append((d, [by_id[i] for i in prev if i in by_id] + [t for t in ts if t.id not in seen]))
+        return out
+
+    def diff(self, canon, soa: S.TaskSoA, table: S.DistroTable, keys):
+        """(edit, update rows, update values) that take the resident tick to the marshalled `canon`, or None when an
+        edit cannot express the change."""
+        if self.distro_ids is None or [d.id for d, _ in canon] != self.distro_ids:
+            return None
+        old, ot = self.soa, self.table
+        remove, n_surv, new_pos = [], [], {}
+        for d, ((_, ts), prev) in enumerate(zip(canon, self.ids)):
+            ids = {t.id for t in ts}
+            gone = [i for i in prev if i not in ids]
+            remove.extend(self.row[i] for i in gone)
+            n_surv.append(len(prev) - len(gone))
+            for k, t in enumerate(ts):
+                new_pos[(d, t.id)] = k
+        D = table.n_distros
+        toff = table.task_off
+        n_surv = np.array(n_surv, dtype=np.int64)
+        ins_rows = np.concatenate([np.arange(toff[d] + n_surv[d], toff[d + 1]) for d in range(D)] or [np.zeros(0, np.int64)]).astype(np.int64)
+        ins_n = np.diff(toff) - n_surv
+        cols = {name: getattr(soa, name)[ins_rows] for name, _ in S.TaskSoA.COLUMNS}
+        dep_off = dep_idx = None
+        if soa.n_edges:
+            deg = soa.dep_off[ins_rows + 1] - soa.dep_off[ins_rows]
+            dep_off = np.concatenate([[0], np.cumsum(deg)]).astype(np.int64)
+            dep_idx = np.concatenate([soa.dep_idx[soa.dep_off[r]:soa.dep_off[r + 1]] for r in ins_rows] or [np.zeros(0, np.int32)])
+        # remaps by name: the ids marshal_tasks gave the composed order
+        gremap, vremap = [], []
+        for d in range(D):
+            gnew = {n: g for g, n in enumerate(keys[d].group_names)}
+            vnew = {n: v for v, n in enumerate(keys[d].versions)}
+            gremap.extend(gnew.get(n, -1) for n in self.keys[d].group_names)
+            vremap.extend(vnew.get(n, -1) for n in self.keys[d].versions)
+        # edges survivors gained: their marshalled edges minus the old edges that survive (as a multiset, in order)
+        add_task, add_dep = [], []
+        for d, prev in enumerate(self.ids):
+            a0 = int(ot.task_off[d])
+            for k_old, tid in enumerate(prev):
+                k_new = new_pos.get((d, tid))
+                if k_new is None:
+                    continue
+                r_old, r_new = a0 + k_old, int(toff[d]) + k_new
+                want = soa.dep_idx[soa.dep_off[r_new]:soa.dep_off[r_new + 1]].tolist() if soa.n_edges else []
+                kept = []
+                if old.n_edges:
+                    for j in old.dep_idx[old.dep_off[r_old]:old.dep_off[r_old + 1]].tolist():
+                        p = new_pos.get((d, prev[j]))
+                        if p is not None:
+                            kept.append(p)
+                rest = list(want)
+                for p in kept:
+                    if p not in rest:
+                        return None  # the survivor lost a dependency that is still queued
+                    rest.remove(p)
+                add_task.extend([r_new] * len(rest))
+                add_dep.extend(rest)
+        edit = S.TaskEdit(np.sort(np.array(remove, dtype=np.int64)), S.TaskSoA(**cols, dep_off=dep_off, dep_idx=dep_idx),
+                          np.concatenate([[0], np.cumsum(ins_n)]).astype(np.int64), np.array(add_task, dtype=np.int64),
+                          np.array(add_dep, dtype=np.int32), np.array(gremap, dtype=np.int32), np.array(vremap, dtype=np.int32),
+                          table.group_off, table.group_max_hosts, table.cfg).normalize()
+        if edit.group_remap.shape[0] == 0:
+            edit.group_remap = None
+        try:
+            composed, _ = S.apply_edit(old, ot, edit)
+        except ValueError:
+            return None
+        if not (np.array_equal(composed.group_id, soa.group_id) and np.array_equal(composed.version_id, soa.version_id)):
+            return None  # a survivor changed task group or version
+        changed = np.zeros(soa.n_tasks, dtype=bool)
+        for name in self.SCALARS:
+            changed |= getattr(composed, name) != getattr(soa, name)
+        rows = np.nonzero(changed)[0].astype(np.int64)
+        values = S.TaskSoA(**{name: getattr(soa, name)[rows] for name, _ in S.TaskSoA.COLUMNS})
+        return edit, rows, values
+
+    def plan(self, batch: Sequence[Tuple[M.Distro, List[M.Task]]], now: int, *, breakdown: bool = True, secondary: bool = False):
+        """One tick: what plan_distros returns for the batch in canonical order (self.canonical)."""
+        eng = self.engine = self.engine or default_engine()
+        canon = self.canonical(batch)
+        soa, table, keys = S.marshal_tasks(canon, now, self.dependency_db, resolve_deps=True)
+        change = self.diff(canon, soa, table, keys)
+        if change is None:
+            eng.upload(soa, table)
+        else:
+            edit, rows, values = change
+            eng.edit_tasks(edit, table)
+            if rows.shape[0]:
+                eng.update_tasks(rows, values)
+        self.last = None if change is None else change[:2]
+        self.remember(canon, soa, table, keys)
+        return _ranked_results(eng, canon, table, keys, now, breakdown, secondary)
+
+    def remember(self, canon, soa: S.TaskSoA, table: S.DistroTable, keys) -> None:
+        """Make the marshalled `canon` the resident tick the next diff starts from."""
+        self.soa, self.table, self.keys = soa, table, keys
+        self.distro_ids = [d.id for d, _ in canon]
+        self.ids = [[t.id for t in ts] for _, ts in canon]
+        self.row = {}
+        for d, ids in enumerate(self.ids):
+            a = int(table.task_off[d])
+            self.row.update((i, a + k) for k, i in enumerate(ids))
 
 
 def persist_task_queues(batch: Sequence[Tuple[M.Distro, List[M.Task]]], now: int, *, engine: Optional[Engine] = None,

@@ -165,6 +165,119 @@ class AllocOutput:
         return self.result.nbytes + self.status.nbytes
 
 
+def _empty_tasks() -> TaskSoA:
+    return TaskSoA(**{name: np.zeros(0, dtype=dt) for name, dt in TaskSoA.COLUMNS})
+
+
+@dataclass
+class TaskEdit:
+    """evg_task_edit: rows leave, rows join, surviving tasks gain in-queue dependencies (include/evg_sched.h).
+    `group_off`, `group_max_hosts` and `cfg` describe the new distro table (None: the old one's); apply_edit builds it."""
+    remove_rows: np.ndarray                       # int64, strictly ascending rows of the current table
+    insert: TaskSoA                               # rows appended after their distro's survivors, ids in the new id space
+    insert_off: np.ndarray                        # int64 [D+1]: CSR of `insert` over distros
+    add_edge_task: np.ndarray                     # int64, ascending composed row of a surviving task
+    add_edge_dep: np.ndarray                      # int32, new distro-local index of its new dependency
+    group_remap: Optional[np.ndarray] = None      # int32 per old group slot: new distro-local id, -1 = no survivor in it
+    version_remap: Optional[np.ndarray] = None    # int32 per old (distro, version), CSR by the old n_versions
+    group_off: Optional[np.ndarray] = None
+    group_max_hosts: Optional[np.ndarray] = None
+    cfg: Optional[np.ndarray] = None
+
+    def normalize(self) -> "TaskEdit":
+        self.remove_rows = np.ascontiguousarray(self.remove_rows, dtype=np.int64)
+        self.insert = (self.insert if self.insert is not None else _empty_tasks()).normalize()
+        self.insert_off = np.ascontiguousarray(self.insert_off, dtype=np.int64)
+        self.add_edge_task = np.ascontiguousarray(self.add_edge_task, dtype=np.int64)
+        self.add_edge_dep = np.ascontiguousarray(self.add_edge_dep, dtype=np.int32)
+        if self.group_remap is not None:
+            self.group_remap = np.ascontiguousarray(self.group_remap, dtype=np.int32)
+        if self.version_remap is not None:
+            self.version_remap = np.ascontiguousarray(self.version_remap, dtype=np.int32)
+        return self
+
+    def struct(self):
+        """-> (TaskEditStruct, the inserted rows' struct it points to: keep both alive for the call)."""
+        ins = self.insert.struct()
+        p = lambda a: L.ptr(a) if a is not None and a.shape[0] else None  # noqa: E731
+        s = L.TaskEditStruct(int(self.remove_rows.shape[0]), p(self.remove_rows), C.pointer(ins), L.ptr(self.insert_off),
+                             int(self.add_edge_task.shape[0]), p(self.add_edge_task), p(self.add_edge_dep),
+                             L.ptr(self.group_remap), L.ptr(self.version_remap))
+        return s, ins
+
+    def nbytes(self) -> int:
+        """What the edit moves to the device (the new distro table aside)."""
+        n = self.remove_rows.nbytes + self.insert.nbytes() + self.insert_off.nbytes + self.add_edge_task.nbytes + self.add_edge_dep.nbytes
+        return n + sum(a.nbytes for a in (self.group_remap, self.version_remap) if a is not None)
+
+
+def apply_edit(tasks: TaskSoA, distros: DistroTable, edit: TaskEdit):
+    """The composed table of evg_edit_tasks, in numpy: -> (TaskSoA, DistroTable).  Distro d's queue is its surviving
+    rows in their previous order, then its inserted rows; a survivor keeps (or remaps) its group and version ids and its
+    edges to survivors (re-indexed, in order), then gains its added edges; inserted rows bring their own edges."""
+    edit.normalize()
+    D, T0 = distros.n_distros, tasks.n_tasks
+    toff = distros.task_off
+    ins = edit.insert
+    keep = np.ones(T0, dtype=bool)
+    keep[edit.remove_rows] = False
+    distro_of = np.repeat(np.arange(D, dtype=np.int64), np.diff(toff))
+    surv = np.nonzero(keep)[0]
+    surv_d = distro_of[surv]
+    n_surv = np.bincount(surv_d, minlength=D).astype(np.int64)
+    n_ins = np.diff(edit.insert_off)
+    new_off = np.concatenate([[0], np.cumsum(n_surv + n_ins)]).astype(np.int64)
+    surv_first = np.concatenate([[0], np.cumsum(n_surv)])
+    surv_new = new_off[surv_d] + np.arange(surv.shape[0]) - surv_first[surv_d]
+    ins_d = np.repeat(np.arange(D, dtype=np.int64), n_ins)
+    ins_new = new_off[ins_d] + n_surv[ins_d] + np.arange(ins.n_tasks) - edit.insert_off[ins_d]
+    Tn = int(new_off[-1])
+    cols = {}
+    for name, dt in TaskSoA.COLUMNS:
+        col = np.zeros(Tn, dtype=dt)
+        col[surv_new] = getattr(tasks, name)[surv]
+        col[ins_new] = getattr(ins, name)
+        cols[name] = col
+    if edit.group_remap is not None:
+        g = tasks.group_id[surv].astype(np.int64)
+        m = g >= 0
+        g[m] = edit.group_remap[distros.group_off[surv_d[m]] + g[m]]
+        if np.any(g[m] < 0):
+            raise ValueError("group_remap maps the task group of a surviving task to -1")
+        cols["group_id"][surv_new] = g
+    if edit.version_remap is not None:
+        vbase = np.concatenate([[0], np.cumsum(distros.cfg["n_versions"].astype(np.int64))])
+        cols["version_id"][surv_new] = edit.version_remap[vbase[surv_d] + tasks.version_id[surv]]
+    # edges: (owner composed row, dependency) from three sources; a stable sort by owner keeps each source's order and
+    # a survivor's old edges ahead of its added ones
+    owners, deps = [], []
+    if tasks.n_edges:
+        new_local = np.full(T0, -1, dtype=np.int64)
+        new_local[surv] = surv_new - new_off[surv_d]
+        deg = np.diff(tasks.dep_off)
+        own = np.repeat(np.arange(T0, dtype=np.int64), deg)
+        tgt = toff[distro_of[own]] + tasks.dep_idx
+        live = keep[own] & keep[tgt]
+        old_to_new = np.full(T0, -1, dtype=np.int64)
+        old_to_new[surv] = surv_new
+        owners.append(old_to_new[own[live]])
+        deps.append(new_local[tgt[live]])
+    owners.append(edit.add_edge_task)
+    deps.append(edit.add_edge_dep.astype(np.int64))
+    if ins.n_edges:
+        owners.append(np.repeat(ins_new, np.diff(ins.dep_off)))
+        deps.append(ins.dep_idx.astype(np.int64))
+    owner = np.concatenate(owners) if owners else np.zeros(0, np.int64)
+    dep = np.concatenate(deps) if deps else np.zeros(0, np.int64)
+    o = np.argsort(owner, kind="stable")
+    dep_off = np.concatenate([[0], np.cumsum(np.bincount(owner, minlength=Tn))]).astype(np.int64)
+    new_tasks = TaskSoA(**cols, dep_off=dep_off, dep_idx=dep[o].astype(np.int32)).normalize()
+    new_distros = DistroTable(new_off, distros.group_off if edit.group_off is None else edit.group_off,
+                              distros.cfg if edit.cfg is None else edit.cfg,
+                              distros.group_max_hosts if edit.group_max_hosts is None else edit.group_max_hosts)
+    return new_tasks, DistroTable(**{k: np.array(v, copy=True) for k, v in vars(new_distros).items()}).normalize()
+
+
 # ---------------------------------------------------------------------------
 # marshalling reference-shaped structs -> SoA
 # ---------------------------------------------------------------------------

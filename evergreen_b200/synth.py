@@ -15,7 +15,7 @@ import numpy as np
 
 from . import _lib as L
 from . import model as M
-from .soa import DistroTable, HostSoA, TaskSoA
+from .soa import DistroTable, HostSoA, TaskEdit, TaskSoA, apply_edit
 
 GOLDEN = np.uint64(0x9E3779B97F4A7C15)
 NOW_NS = 1_800_000_000 * 10 ** 9
@@ -398,6 +398,176 @@ def sprinkle_edges(w: Workload, seed: int, *, kinds, frac: Optional[float] = Non
             t.num_dependents[r] = 0
             t.expected_ns[r] = aim[(d, v)]
     return {k: np.asarray(v, dtype=np.int64) for k, v in out.items()}
+
+
+# ---------------------------------------------------------------- the next tick
+EDIT_SALT = 0x7E11C0DE
+
+
+@dataclass
+class EditTick:
+    edit: TaskEdit            # membership change (evg_edit_tasks)
+    rows: np.ndarray          # composed rows whose scalars changed (evg_update_tasks)
+    values: TaskSoA           # their new values
+    workload: Workload        # the composed tick with the changes: what a fresh upload of the next tick holds
+
+
+def _rank_within(keys: np.ndarray) -> np.ndarray:
+    """Position of each element among the elements with the same (sorted-run) key before it."""
+    n = keys.shape[0]
+    if n == 0:
+        return np.zeros(0, dtype=np.int64)
+    start = np.ones(n, dtype=bool)
+    start[1:] = keys[1:] != keys[:-1]
+    first = np.maximum.accumulate(np.where(start, np.arange(n), 0))
+    return np.arange(n) - first
+
+
+def next_tick(w: Workload, seed: int, *, dispatch: float = 0.05, arrive: float = 0.05, change: float = 0.05,
+              order: Optional[np.ndarray] = None, remap: bool = True, dep_frac: float = 0.1,
+              add_edge_frac: float = 0.01) -> EditTick:
+    """The tick after `w`: a `dispatch` fraction of rows leaves (biased to the heads of the queues `order` ranked, the
+    planner's last order, when given), an `arrive` fraction of each queue's size joins -- some rows join existing or new
+    task groups and versions, a `dep_frac` of them depend on survivors or other arrivals -- an `add_edge_frac` of the
+    survivors gain a dependency, and a `change` fraction of the composed rows take new scalars.  With `remap`, group and
+    version ids are re-densified in first-appearance order over the composed queue (no dead slots); without it they are
+    kept and new ones appended.  A stream of its own: make()'s ticks are unchanged."""
+    rng = Rng(seed ^ EDIT_SALT)
+    t, dt = w.tasks, w.distros
+    D, T0 = dt.n_distros, t.n_tasks
+    toff, goff = dt.task_off, dt.group_off
+    sizes = np.diff(toff)
+    distro_of = np.repeat(np.arange(D, dtype=np.int64), sizes)
+    # dispatch
+    p = np.full(T0, dispatch)
+    if order is not None and T0:
+        rank = np.empty(T0, dtype=np.int64)
+        rank[toff[distro_of] + order.astype(np.int64)] = np.arange(T0) - toff[distro_of]
+        p = 2.0 * dispatch * (1.0 - rank / np.maximum(sizes[distro_of], 1))
+    keep = rng.uniform(T0) >= p
+    remove = np.nonzero(~keep)[0].astype(np.int64)
+    surv = np.nonzero(keep)[0]
+    surv_d = distro_of[surv]
+    n_surv = np.bincount(surv_d, minlength=D).astype(np.int64)
+    # group / version ids of the survivors in the new id space
+    nver_old = dt.cfg["n_versions"].astype(np.int64)
+    vbase = np.concatenate([[0], np.cumsum(nver_old)])
+    ng_old = np.diff(goff)
+    if remap:
+        grouped = t.group_id[surv] >= 0
+        gremap = np.full(int(goff[-1]), -1, dtype=np.int64)
+        vremap = np.full(int(vbase[-1]), -1, dtype=np.int64)
+        for slot, dd, out in ((goff[surv_d[grouped]] + t.group_id[surv][grouped], surv_d[grouped], gremap),
+                              (vbase[surv_d] + t.version_id[surv], surv_d, vremap)):
+            u, first = np.unique(slot, return_index=True)
+            by_first = np.argsort(first)  # survivors ascend by distro: first-appearance order is grouped by distro
+            out[u[by_first]] = _rank_within(dd[first[by_first]])
+        ng_cur = np.bincount(np.repeat(np.arange(D), ng_old)[gremap >= 0], minlength=D).astype(np.int64)
+        nv_cur = np.bincount(np.repeat(np.arange(D), nver_old)[vremap >= 0], minlength=D).astype(np.int64)
+        group_of_old = np.full(T0, -1, dtype=np.int64)
+        mm = t.group_id >= 0
+        group_of_old[mm] = gremap[goff[distro_of[mm]] + t.group_id[mm]]
+        version_of_old = vremap[vbase[distro_of] + t.version_id]
+    else:
+        gremap = vremap = None
+        ng_cur, nv_cur = ng_old.astype(np.int64), nver_old.copy()
+        group_of_old, version_of_old = t.group_id.astype(np.int64), t.version_id.astype(np.int64)
+    # each current group's version (a task group lives in one version)
+    gbase_cur = np.concatenate([[0], np.cumsum(ng_cur)])
+    grp_ver = np.zeros(int(gbase_cur[-1]), dtype=np.int64)
+    m = group_of_old >= 0
+    grp_ver[gbase_cur[distro_of[m]] + group_of_old[m]] = version_of_old[m]
+    # arrivals
+    n_ins = np.floor(arrive * sizes + rng.uniform(D)).astype(np.int64)
+    I = int(n_ins.sum())
+    ins_d = np.repeat(np.arange(D, dtype=np.int64), n_ins)
+    ins_k = _rank_within(ins_d)
+    new_n = n_surv + n_ins
+    newv = (rng.uniform(I) < 0.2) | (nv_cur[ins_d] == 0)
+    vid = np.minimum((rng.uniform(I) * nv_cur[ins_d]).astype(np.int64), np.maximum(nv_cur[ins_d] - 1, 0))
+    o = np.lexsort((ins_k, ins_d, ~newv))
+    nv_rank = np.empty(I, dtype=np.int64)
+    nv_rank[o] = _rank_within((ins_d * 2 + newv)[o])
+    vid = np.where(newv, nv_cur[ins_d] + nv_rank // 5, vid)
+    nv_new = nv_cur.copy()
+    np.maximum.at(nv_new, ins_d, vid + 1)
+    is_tg = rng.uniform(I) < 0.15
+    join = is_tg & (rng.uniform(I) < 0.5) & (ng_cur[ins_d] > 0)
+    newg = is_tg & ~join
+    gid = np.full(I, -1, dtype=np.int64)
+    gj = np.minimum((rng.uniform(I) * ng_cur[ins_d]).astype(np.int64), np.maximum(ng_cur[ins_d] - 1, 0))
+    gid[join] = gj[join]
+    vid[join] = grp_ver[gbase_cur[ins_d[join]] + gj[join]]
+    o = np.lexsort((ins_k, ins_d, ~newg))
+    ng_rank = np.empty(I, dtype=np.int64)
+    ng_rank[o] = _rank_within((ins_d * 2 + newg)[o])
+    gid[newg] = ng_cur[ins_d[newg]] + ng_rank[newg] // 3
+    ng_new = ng_cur.copy()
+    np.maximum.at(ng_new, ins_d[newg], gid[newg] + 1)
+    # a new group's members take the version of its first member
+    key = ins_d * (1 << 32) + np.where(newg, gid, -1)
+    _, first, inv = np.unique(key, return_index=True, return_inverse=True)
+    vid[newg] = vid[first[inv]][newg]
+    tgo = np.where(is_tg, rng.integers(I, 1, 8), 0).astype(np.int32)
+    # the arrivals' own edges, as new distro-local indices (never to themselves)
+    has_dep = (rng.uniform(I) < dep_frac) & (new_n[ins_d] > 1)
+    self_loc = n_surv[ins_d] + ins_k
+    tgt = np.minimum((rng.uniform(I) * (new_n[ins_d] - 1)).astype(np.int64), np.maximum(new_n[ins_d] - 2, 0))
+    tgt = np.where(tgt >= self_loc, tgt + 1, tgt)
+    ins_dep_off = np.concatenate([[0], np.cumsum(has_dep)]).astype(np.int64)
+    now = int(w.now)
+    u = rng.uniform(I)
+    flags = np.where(u < 0.4, L.EVG_TF_REQ_PATCH, np.where(u < 0.45, L.EVG_TF_REQ_MERGE_QUEUE, L.EVG_TF_REQ_OTHER)).astype(np.uint32)
+    flags |= np.where(rng.uniform(I) < 0.95, L.EVG_TF_DEPS_MET, 0).astype(np.uint32)
+    flags |= np.where(rng.uniform(I) < 0.01, L.EVG_TF_GENERATE, 0).astype(np.uint32)
+    insert = TaskSoA(_zipf_priorities(rng, I), rng.integers(I, 10 * M.SECOND, 2 * M.HOUR), now - rng.integers(I, 0, 3 * M.HOUR),
+                     now - rng.integers(I, 0, M.HOUR), rng.integers(I, 0, 3).astype(np.int32), tgo, gid.astype(np.int32),
+                     vid.astype(np.int32), flags, ins_dep_off, tgt[has_dep].astype(np.int32)).normalize()
+    # survivors that gain a dependency
+    gain = rng.uniform(surv.shape[0]) < add_edge_frac
+    surv_loc = _rank_within(surv_d)
+    new_off = np.concatenate([[0], np.cumsum(new_n)])
+    gain &= new_n[surv_d] > 1
+    gt = np.minimum((rng.uniform(surv.shape[0]) * (new_n[surv_d] - 1)).astype(np.int64), np.maximum(new_n[surv_d] - 2, 0))
+    gt = np.where(gt >= surv_loc, gt + 1, gt)
+    # the new distro table
+    G_new = int(ng_new.sum())
+    goff_new = np.concatenate([[0], np.cumsum(ng_new)]).astype(np.int64)
+    gmax = rng.integers(G_new, 1, 3).astype(np.int32)
+    if remap:
+        live = gremap >= 0
+        old_d = np.repeat(np.arange(D, dtype=np.int64), ng_old)
+        gmax[goff_new[old_d[live]] + gremap[live]] = dt.group_max_hosts[live]
+    else:
+        old_d = np.repeat(np.arange(D, dtype=np.int64), ng_old)
+        gmax[goff_new[old_d] + (np.arange(int(goff[-1])) - goff[old_d])] = dt.group_max_hosts
+    cfg = dt.cfg.copy()
+    cfg["n_versions"] = nv_new.astype(np.int32)
+    edit = TaskEdit(remove, insert, np.concatenate([[0], np.cumsum(n_ins)]).astype(np.int64),
+                    (new_off[surv_d] + surv_loc)[gain].astype(np.int64), gt[gain].astype(np.int32),
+                    None if gremap is None or gremap.shape[0] == 0 else gremap.astype(np.int32),
+                    None if vremap is None else vremap.astype(np.int32), goff_new, gmax, cfg).normalize()
+    tasks, distros = apply_edit(t, dt, edit)
+    # value changes on the composed rows
+    Tn = tasks.n_tasks
+    rows = np.nonzero(rng.uniform(Tn) < change)[0].astype(np.int64)
+    n = rows.shape[0]
+    tasks.priority[rows] = _zipf_priorities(rng, n)
+    tasks.expected_ns[rows] = rng.integers(n, 10 * M.SECOND, 2 * M.HOUR)
+    tasks.wait_basis_ns[rows] = now - rng.integers(n, 0, 3 * M.HOUR)
+    tasks.num_dependents[rows] = rng.integers(n, 0, 5).astype(np.int32)
+    tasks.flags[rows] ^= np.where(rng.uniform(n) < 0.3, L.EVG_TF_DEPS_MET, 0).astype(np.uint32)
+    values = TaskSoA(**{name: getattr(tasks, name)[rows] for name, _ in TaskSoA.COLUMNS}).normalize()
+    hosts = w.hosts
+    if hosts is not None and remap:
+        hd = np.repeat(np.arange(D, dtype=np.int64), np.diff(hosts.host_off))
+        hg = hosts.group_id.astype(np.int64)
+        m = hg >= 0
+        hg[m] = gremap[goff[hd[m]] + hg[m]]
+        hg[m & (hg < 0)] = L.EVG_HG_UNQUEUED
+        hosts = HostSoA(hosts.flags.copy(), hg.astype(np.int32), hosts.expected_ns.copy(), hosts.std_ns.copy(),
+                        hosts.start_ns.copy(), hosts.host_off.copy(), hosts.cfg.copy()).normalize()
+    return EditTick(edit, rows, values, Workload(w.name, w.now, tasks, distros, hosts))
 
 
 def power_law_sizes(rng: Rng, D: int, alpha: float = 1.2, lo: int = 1, hi: int = 1_000_000) -> np.ndarray:

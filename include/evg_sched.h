@@ -276,11 +276,51 @@ int evg_upload(evg_ctx* ctx, const evg_task_soa* tasks, const evg_distro_table* 
 /* Tick-to-tick update of the resident task table: row rows[i] (a task slot of the last evg_upload, 0 <= rows[i] <
  * n_tasks) gets priority, num_dependents, task_group_order, flags, expected_ns, queue_basis_ns and wait_basis_ns of row i
  * of `values` (values->n_tasks == n_rows; its group / version / dependency columns are not read: a task keeps its
- * distro, its task group, its version and its in-queue dependency edges -- a tick that adds or removes tasks uploads
- * again).  48 bytes cross PCIe per changed row instead of the whole table.  Not available after evg_upload_device (the
+ * distro, its task group, its version and its in-queue dependency edges -- a tick that adds or removes tasks calls
+ * evg_edit_tasks first).  48 bytes cross PCIe per changed row instead of the whole table.  Not available after evg_upload_device (the
  * caller owns those columns and edits them in place).  Replaces nothing in the reference: there the scheduler re-reads
  * every task document each tick (scheduler/task_finder.go:40-197). */
 int evg_update_tasks(evg_ctx* ctx, int64_t n_rows, const int64_t* rows, const evg_task_soa* values);
+
+/* A change in queue membership between two ticks: rows leave, rows join, surviving tasks gain in-queue dependencies.
+ * Host pointers. */
+typedef struct {
+  int64_t n_remove;
+  const int64_t* remove_rows;   /* strictly ascending rows of the current resident table */
+  const evg_task_soa* insert;   /* rows appended to their distro's queue after its survivors; n_tasks = rows inserted
+                                   (NULL = none).  Group / version ids are in the new id space; dep_off / dep_idx are the
+                                   rows' own in-queue edges as NEW distro-local indices */
+  const int64_t* insert_off;    /* n_distros + 1: CSR of `insert` over distros */
+  int64_t n_add_edges;          /* in-queue dependencies a SURVIVING task gains */
+  const int64_t* add_edge_task; /* ascending NEW global row of a surviving task */
+  const int32_t* add_edge_dep;  /* NEW distro-local index of the dependency (a survivor or an inserted row) */
+  const int32_t* group_remap;   /* NULL = ids kept; else per OLD group slot: the new distro-local id, -1 = no survivor is in it */
+  const int32_t* version_remap; /* NULL = ids kept; else per OLD (distro, version id), CSR by the old n_versions */
+} evg_task_edit;
+
+/* Tick-to-tick membership change of the resident task table, applied on the device: afterwards the context holds
+ * exactly the tick a fresh evg_upload of the COMPOSED table would hold (outputs, evg_download_queue and the breakdown
+ * match it bit for bit).  The composed table:
+ *   - distro d's queue is its surviving rows in their previous order, then insert rows insert_off[d] .. insert_off[d+1];
+ *   - a survivor keeps its group and version ids, or takes group_remap / version_remap of them;
+ *   - a survivor's edges are its old edges whose dependency survived (re-indexed, in their old order), then its added
+ *     edges in the order given; an inserted row's edges are its own;
+ *   - `distros` is the new distro table: the same n_distros, task_off = old count - removed + inserted for every
+ *     distro; cfg, group_off, group_max_hosts and n_versions may change as long as every id in use stays in range.
+ * `hosts`, `host_off`, `acfg` as for evg_upload (NULL: planner only).  Only the edit crosses PCIe: the survivors are
+ * gathered from the resident columns into a second column set the first edit allocates, which then becomes the
+ * resident one.  A survivor cannot LOSE an in-queue dependency that stays in the queue (upload again for that), and
+ * dependencies are not re-evaluated: pass EVG_TF_DEPS_MET for inserted rows and flip it for survivors with
+ * evg_update_tasks.  Any device-side dependency state of evg_upload_with_deps is dropped.
+ * Allowed after evg_upload, evg_upload_with_deps, evg_plan_from_finder and evg_edit_tasks; EVG_ERR_STATE otherwise
+ * (no table, borrowed columns of evg_upload_device, the tick a one-shot call left).  EVG_ERR_INVALID for an edit the
+ * host can reject (remove rows not strictly ascending or out of range, counts that disagree, another n_distros, an
+ * added edge on a task that is not a survivor) leaves the previous tick resident and runnable; an id found out of range
+ * on the device (or a survivor whose task group maps to -1) leaves no resident tick, as for evg_upload.
+ * Replaces nothing in the reference: there the scheduler re-reads every task document each tick
+ * (scheduler/task_finder.go:40-197). */
+int evg_edit_tasks(evg_ctx* ctx, const evg_task_edit* edit, const evg_distro_table* distros,
+                   const evg_host_soa* hosts, const int64_t* host_off, const evg_alloc_cfg* acfg);
 
 /* Like evg_upload, but the task columns already live in DEVICE memory (the finder's output, a generator kernel, a
  * previous tick edited in place): `tasks` holds device pointers, which the context borrows until the next upload or
