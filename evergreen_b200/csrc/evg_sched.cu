@@ -32,6 +32,7 @@
 #include <algorithm>
 #include <type_traits>
 #include <cstdlib>
+#include <future>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -825,6 +826,35 @@ __global__ void __launch_bounds__(128) k_alloc_groupless(DHosts H, int32_t d_beg
 // --------------------------------------------------------------------------
 // context
 // --------------------------------------------------------------------------
+struct TaskCols {  // the nine planner columns of a task table
+  DevBuf prio, nd, tgo, gid, vid, flags, exp, qb, wb;
+  int stage(const evg_task_soa* t, int64_t n, cudaStream_t s) {  // copy the first n rows of t's columns
+    UP(s, prio, t->priority, n, int32_t);
+    UP(s, nd, t->num_dependents, n, int32_t);
+    UP(s, tgo, t->task_group_order, n, int32_t);
+    UP(s, gid, t->group_id, n, int32_t);
+    UP(s, vid, t->version_id, n, int32_t);
+    UP(s, flags, t->flags, n, uint32_t);
+    UP(s, exp, t->expected_ns, n, int64_t);
+    UP(s, qb, t->queue_basis_ns, n, int64_t);
+    UP(s, wb, t->wait_basis_ns, n, int64_t);
+    return EVG_OK;
+  }
+  DTasks view(int64_t n) const {  // n rows, no edges
+    DTasks v;
+    memset(&v, 0, sizeof(v));
+    v.n = n;
+    v.priority = prio.as<int32_t>(); v.expected = exp.as<int64_t>(); v.qbasis = qb.as<int64_t>(); v.wbasis = wb.as<int64_t>();
+    v.numdep = nd.as<int32_t>(); v.tgo = tgo.as<int32_t>(); v.gid = gid.as<int32_t>(); v.vid = vid.as<int32_t>();
+    v.flags = flags.as<uint32_t>();
+    return v;
+  }
+  void swap(TaskCols& o) {
+    prio.swap(o.prio); nd.swap(o.nd); tgo.swap(o.tgo); gid.swap(o.gid); vid.swap(o.vid);
+    flags.swap(o.flags); exp.swap(o.exp); qb.swap(o.qb); wb.swap(o.wb);
+  }
+};
+
 struct evg_ctx {
   int device = 0;
   int num_sms = 0;  // the device's multiprocessor count: grid cap of the grid-stride work-list kernels
@@ -854,23 +884,26 @@ struct evg_ctx {
   int64_t launches = 0;
   bool timed = false;
   bool adopted = false;  // task columns are caller-owned device memory (evg_upload_device)
-  bool deps_resident = false;  // evg_upload_with_deps left the verdicts and stamps of this tick on the device
-  DevBuf b_prio, b_exp, b_qb, b_wb, b_nd, b_tgo, b_gid, b_vid, b_flags, b_depoff, b_depidx;
+  bool deps_resident = false;  // evg_upload_with_deps left the verdicts and stamps of this tick in `deps`
+  TaskCols tasks;  // the resident planner columns
+  DevBuf b_depoff, b_depidx;
   DevBuf b_taskoff, b_groupoff, b_cfg, b_gmax, b_unitbase;
   DevBuf b_hasdep, b_head, b_next, b_pslot, b_etask, b_elive, b_bestpair;
   DevBuf b_rn0, b_rn1, b_rn2, b_rn3, b_rn4, b_rn5, b_rn6, b_rn7;
-  struct TaskCols { DevBuf prio, nd, tgo, gid, vid, flags, exp, qb, wb; };  // the nine planner columns of a task table
+  struct {
+    DevBuf off, kind, ref, want, state, pre, ext;  // an evg_deps_in table, staged
+    DevBuf met, fin, stamp;                        // k_deps_met's verdicts, its dep_finished_ns input, its stamps
+  } deps;
   struct {
     DevBuf task_off, sched, project, project_flags, valid_off, valid_idx, finder;  // the finder tables
-    DevBuf kept, count;                // k_runnable's kept lists and per-distro counts
-    TaskCols cand, out;                // candidate columns, compacted columns
-    DevBuf new_off, new_idx, src_row;  // compacted task_off; candidate row -> compacted index, and back
-    DevBuf dep_off, dep_idx, edge_cnt, new_dep_off, scan_sum, new_dep_idx;  // candidate edges, surviving edges
-  } pf;  // evg_plan_from_finder's own buffers (deps_to_device holds b_rn6 / b_rn7)
+    DevBuf kept, count;  // k_runnable's kept lists and per-distro counts
+    TaskCols cand;       // evg_plan_from_finder: the candidates' columns
+    DevBuf dep_off, dep_idx;  // and their edges
+  } pf;
   // evg_edit_tasks: resident columns an edit may start from (evg_upload, evg_upload_with_deps, evg_plan_from_finder,
   // evg_edit_tasks; not borrowed columns, not what a one-shot call left)
   bool editable = false;
-  struct {
+  struct {  // compose_tick's buffers (the first evg_edit_tasks or evg_plan_from_finder allocates them) and the staged edit
     TaskCols out;            // the shadow set: the composed table is written here, then swapped with the resident columns
     DevBuf dep_off, dep_idx; // the composed edges (swapped too)
     TaskCols ins;            // the inserted rows, staged
@@ -878,7 +911,7 @@ struct evg_ctx {
     DevBuf new_off, old_off, old_goff, ins_off, old_vbase, edge_at;  // D+1 tables
     DevBuf keep, pos, src, scan_sum, edge_cnt, err;
   } ed;
-  DevBuf b_err, b_dx0, b_dx1, b_dx2, b_dx3, b_dx4, b_dx5, b_dx6, b_dx7;
+  DevBuf b_err;
   DevBuf b_route, b_unitv, b_unita, b_unitn, b_unitmask;
   DevBuf b_punt, b_puntcnt;
   // The distros of each size class: ascending ids on the host and the device (the pipelined call cuts them by distro
@@ -926,8 +959,8 @@ constexpr int64_t kColPad = 8;
 enum class Cols {
   kCopy,      // host memory: copied into the context's buffers
   kChunked,   // host memory: the pipelined call copies them chunk by chunk
-  kAdopt,     // device memory the context borrows (evg_upload_device, evg_plan_from_finder's compacted table)
-  kResident,  // already in the context's own buffers (evg_edit_tasks swapped them in): `t` points at them
+  kAdopt,     // device memory the context borrows (evg_upload_device)
+  kResident,  // already in the context's own buffers (compose_tick swapped them in): `t` points at them
 };
 
 // Route every distro of the tick, stage the small tables, size the work buffers.  Every mode but kChunked range-checks
@@ -1039,15 +1072,15 @@ int upload_tasks(evg_ctx* c, const evg_task_soa* t, const evg_distro_table* dt, 
       if (copy_columns && (count) > 0) CK(cudaMemcpyAsync((buf).p, (ptr), sizeof(type) * size_t(count), cudaMemcpyHostToDevice, s)); \
     }                                                                                                 \
   } while (0)
-  UPC(c->b_prio, t->priority, T, int32_t);
-  UPC(c->b_exp, t->expected_ns, T, int64_t);
-  UPC(c->b_qb, t->queue_basis_ns, T, int64_t);
-  UPC(c->b_wb, t->wait_basis_ns, T, int64_t);
-  UPC(c->b_nd, t->num_dependents, T, int32_t);
-  UPC(c->b_tgo, t->task_group_order, T, int32_t);
-  UPC(c->b_gid, t->group_id, T, int32_t);
-  UPC(c->b_vid, t->version_id, T, int32_t);
-  UPC(c->b_flags, t->flags, T, uint32_t);
+  UPC(c->tasks.prio, t->priority, T, int32_t);
+  UPC(c->tasks.exp, t->expected_ns, T, int64_t);
+  UPC(c->tasks.qb, t->queue_basis_ns, T, int64_t);
+  UPC(c->tasks.wb, t->wait_basis_ns, T, int64_t);
+  UPC(c->tasks.nd, t->num_dependents, T, int32_t);
+  UPC(c->tasks.tgo, t->task_group_order, T, int32_t);
+  UPC(c->tasks.gid, t->group_id, T, int32_t);
+  UPC(c->tasks.vid, t->version_id, T, int32_t);
+  UPC(c->tasks.flags, t->flags, T, uint32_t);
   if (E > 0) {
     UPC(c->b_depoff, t->dep_off, T + 1, int64_t);
     UPC(c->b_depidx, t->dep_idx, E, int32_t);
@@ -1211,12 +1244,8 @@ int upload_hosts(evg_ctx* c, const evg_host_soa* h, const int64_t* host_off, con
 }
 
 DTasks dtasks(const evg_ctx* c) {
-  DTasks t;
-  t.n = c->T; t.n_edges = c->E;
-  t.priority = c->b_prio.as<int32_t>(); t.expected = c->b_exp.as<int64_t>();
-  t.qbasis = c->b_qb.as<int64_t>(); t.wbasis = c->b_wb.as<int64_t>();
-  t.numdep = c->b_nd.as<int32_t>(); t.tgo = c->b_tgo.as<int32_t>();
-  t.gid = c->b_gid.as<int32_t>(); t.vid = c->b_vid.as<int32_t>(); t.flags = c->b_flags.as<uint32_t>();
+  DTasks t = c->tasks.view(c->T);
+  t.n_edges = c->E;
   t.dep_off = c->b_depoff.as<int64_t>(); t.dep_idx = c->b_depidx.as<int32_t>();
   return t;
 }
@@ -1641,8 +1670,8 @@ int evg_update_tasks(evg_ctx* c, int64_t n_rows, const int64_t* rows, const evg_
   CK(cudaMemcpyAsync(d_fl, v->flags, n * 4, cudaMemcpyHostToDevice, s));
   int* bad = reinterpret_cast<int*>(base + n * 48);
   CK(cudaMemsetAsync(bad, 0, sizeof(int), s));
-  k_update_rows<<<grid_for(n_rows, 256), 256, 0, s>>>(n_rows, d_rows, c->T, c->b_prio.as<int32_t>(), c->b_nd.as<int32_t>(), c->b_tgo.as<int32_t>(),
-                                                      c->b_flags.as<uint32_t>(), c->b_exp.as<int64_t>(), c->b_qb.as<int64_t>(), c->b_wb.as<int64_t>(),
+  k_update_rows<<<grid_for(n_rows, 256), 256, 0, s>>>(n_rows, d_rows, c->T, c->tasks.prio.as<int32_t>(), c->tasks.nd.as<int32_t>(), c->tasks.tgo.as<int32_t>(),
+                                                      c->tasks.flags.as<uint32_t>(), c->tasks.exp.as<int64_t>(), c->tasks.qb.as<int64_t>(), c->tasks.wb.as<int64_t>(),
                                                       d_prio, d_nd, d_tgo, d_fl, d_exp, d_qb, d_wb, bad);
   CK(cudaGetLastError());
   int h_bad = 0;
@@ -1888,15 +1917,15 @@ static int plan_and_alloc_pipelined(evg_ctx* c, const evg_task_soa* t, const evg
     if (d1 <= d0) continue;
     const int64_t t0 = c->h_taskoff[d0], n = c->h_taskoff[d1] - t0;
     const int64_t g0 = c->h_groupoff[d0], ng = c->h_groupoff[d1] - g0;
-    H2D(c->b_prio, t->priority, t0, n, int32_t);
-    H2D(c->b_exp, t->expected_ns, t0, n, int64_t);
-    H2D(c->b_qb, t->queue_basis_ns, t0, n, int64_t);
-    H2D(c->b_wb, t->wait_basis_ns, t0, n, int64_t);
-    H2D(c->b_nd, t->num_dependents, t0, n, int32_t);
-    H2D(c->b_tgo, t->task_group_order, t0, n, int32_t);
-    H2D(c->b_gid, t->group_id, t0, n, int32_t);
-    H2D(c->b_vid, t->version_id, t0, n, int32_t);
-    H2D(c->b_flags, t->flags, t0, n, uint32_t);
+    H2D(c->tasks.prio, t->priority, t0, n, int32_t);
+    H2D(c->tasks.exp, t->expected_ns, t0, n, int64_t);
+    H2D(c->tasks.qb, t->queue_basis_ns, t0, n, int64_t);
+    H2D(c->tasks.wb, t->wait_basis_ns, t0, n, int64_t);
+    H2D(c->tasks.nd, t->num_dependents, t0, n, int32_t);
+    H2D(c->tasks.tgo, t->task_group_order, t0, n, int32_t);
+    H2D(c->tasks.gid, t->group_id, t0, n, int32_t);
+    H2D(c->tasks.vid, t->version_id, t0, n, int32_t);
+    H2D(c->tasks.flags, t->flags, t0, n, uint32_t);
     if (E > 0) {
       const int64_t e0 = t->dep_off[t0], ne = t->dep_off[t0 + n] - e0;
       H2D(c->b_depoff, t->dep_off, t0, n + 1, int64_t);
@@ -2002,7 +2031,7 @@ int evg_alloc_batch(evg_ctx* c, const evg_host_soa* hosts, const int64_t* host_o
   return EVG_OK;
 }
 
-// Stage an evg_deps_in table and run k_deps_met into b_dx7 (left on the device); `both` adds the no-short-circuit bit.
+// Stage an evg_deps_in table and run k_deps_met into deps.met (left on the device); `both` adds the no-short-circuit bit.
 static int deps_to_device(evg_ctx* c, const evg_deps_in* in, int both, const int64_t* dep_finished = nullptr, int64_t now = 0,
                           bool want_stamp = false) {
   const int64_t T = in->n_tasks, E = in->n_deps, X = in->n_ext;
@@ -2013,30 +2042,30 @@ static int deps_to_device(evg_ctx* c, const evg_deps_in* in, int both, const int
   if (X > 0 && !in->ext_state) return fail(EVG_ERR_INVALID, "null ext_state");
   if (in->dep_off[0] != 0 || in->dep_off[T] != E) return fail(EVG_ERR_INVALID, "dep_off does not span n_deps");
   cudaStream_t s = c->stream;
-  UP(s, c->b_dx0, in->dep_off, T + 1, int64_t);
-  UP(s, c->b_dx1, in->dep_kind, E, uint8_t);
-  UP(s, c->b_dx2, in->dep_ref, E, int32_t);
-  UP(s, c->b_dx3, in->dep_want, E, uint8_t);
-  UP(s, c->b_dx4, in->task_state, T, uint8_t);
-  UP(s, c->b_dx5, in->task_pre, T, uint8_t);
-  UP(s, c->b_dx6, in->ext_state, X, uint8_t);
-  CK(c->b_dx7.ensure(size_t(T)));
+  auto& x = c->deps;
+  UP(s, x.off, in->dep_off, T + 1, int64_t);
+  UP(s, x.kind, in->dep_kind, E, uint8_t);
+  UP(s, x.ref, in->dep_ref, E, int32_t);
+  UP(s, x.want, in->dep_want, E, uint8_t);
+  UP(s, x.state, in->task_state, T, uint8_t);
+  UP(s, x.pre, in->task_pre, T, uint8_t);
+  UP(s, x.ext, in->ext_state, X, uint8_t);
+  CK(x.met.ensure(size_t(T)));
   int64_t* stamp = nullptr;
   const int64_t* fin = nullptr;
   if (want_stamp) {
-    CK(c->b_rn7.ensure(sizeof(int64_t) * size_t(T)));
-    stamp = c->b_rn7.as<int64_t>();
+    CK(x.stamp.ensure(sizeof(int64_t) * size_t(T)));
+    stamp = x.stamp.as<int64_t>();
     if (dep_finished && E > 0) {
-      CK(c->b_rn6.ensure(sizeof(int64_t) * size_t(E)));
-      CK(cudaMemcpyAsync(c->b_rn6.p, dep_finished, sizeof(int64_t) * size_t(E), cudaMemcpyHostToDevice, s));
-      fin = c->b_rn6.as<int64_t>();
+      UP(s, x.fin, dep_finished, E, int64_t);
+      fin = x.fin.as<int64_t>();
     }
   }
   DDeps d;
-  d.n_tasks = T; d.dep_off = c->b_dx0.as<int64_t>(); d.dep_kind = c->b_dx1.as<uint8_t>(); d.dep_ref = c->b_dx2.as<int32_t>();
-  d.dep_want = c->b_dx3.as<uint8_t>(); d.task_state = c->b_dx4.as<uint8_t>(); d.task_pre = c->b_dx5.as<uint8_t>();
-  d.ext_state = c->b_dx6.as<uint8_t>(); d.n_ext = X;
-  k_deps_met<<<grid_for(T, 256), 256, 0, s>>>(d, c->b_dx7.as<uint8_t>(), c->b_err.as<int>(), both, fin, now, stamp);
+  d.n_tasks = T; d.dep_off = x.off.as<int64_t>(); d.dep_kind = x.kind.as<uint8_t>(); d.dep_ref = x.ref.as<int32_t>();
+  d.dep_want = x.want.as<uint8_t>(); d.task_state = x.state.as<uint8_t>(); d.task_pre = x.pre.as<uint8_t>();
+  d.ext_state = x.ext.as<uint8_t>(); d.n_ext = X;
+  k_deps_met<<<grid_for(T, 256), 256, 0, s>>>(d, x.met.as<uint8_t>(), c->b_err.as<int>(), both, fin, now, stamp);
   c->launches++;
   CK(cudaGetLastError());
   return EVG_OK;
@@ -2051,10 +2080,11 @@ int evg_deps_met_batch(evg_ctx* c, const evg_deps_in* in, uint8_t* met) {
   CK(c->b_err.ensure(sizeof(int) * 4));
   CK(cudaMemsetAsync(c->b_err.p, 0, sizeof(int) * 4, s));
   c->launches = 0;
+  c->deps_resident = false;  // deps_to_device overwrites the resident tick's verdicts and stamps
   int rc = deps_to_device(c, in, 0);
   if (rc != EVG_OK) return rc;
   int bad = 0;
-  CK(cudaMemcpyAsync(met, c->b_dx7.p, size_t(in->n_tasks), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(met, c->deps.met.p, size_t(in->n_tasks), cudaMemcpyDeviceToHost, s));
   CK(cudaMemcpyAsync(&bad, c->b_err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   if (bad) return fail(EVG_ERR_INVALID, "a dep_ref is out of range");
@@ -2075,7 +2105,8 @@ int evg_upload_with_deps(evg_ctx* c, const evg_task_soa* tasks, const evg_distro
   cudaStream_t s = c->stream;
   rc = deps_to_device(c, deps, 0, dep_finished_ns, now_ns, /*want_stamp=*/true);
   if (rc != EVG_OK) { c->have_tasks = false; return rc; }
-  k_apply_deps<<<grid_for(T, 256), 256, 0, s>>>(T, c->b_dx7.as<uint8_t>(), c->b_rn7.as<int64_t>(), c->b_flags.as<uint32_t>(), c->b_wb.as<int64_t>());
+  k_apply_deps<<<grid_for(T, 256), 256, 0, s>>>(T, c->deps.met.as<uint8_t>(), c->deps.stamp.as<int64_t>(), c->tasks.flags.as<uint32_t>(),
+                                                c->tasks.wb.as<int64_t>());
   c->launches++;
   int bad = 0;
   CK(cudaGetLastError());
@@ -2093,8 +2124,8 @@ int evg_download_deps(evg_ctx* c, uint8_t* met, int64_t* met_time_ns) {
   CK(cudaSetDevice(c->device));
   if (c->T == 0) return EVG_OK;
   if (!c->deps_resident) return fail(EVG_ERR_STATE, "the resident tick was not uploaded with evg_upload_with_deps");
-  if (met) CK(cudaMemcpyAsync(met, c->b_dx7.p, size_t(c->T), cudaMemcpyDeviceToHost, c->stream));
-  if (met_time_ns) CK(cudaMemcpyAsync(met_time_ns, c->b_rn7.p, sizeof(int64_t) * size_t(c->T), cudaMemcpyDeviceToHost, c->stream));
+  if (met) CK(cudaMemcpyAsync(met, c->deps.met.p, size_t(c->T), cudaMemcpyDeviceToHost, c->stream));
+  if (met_time_ns) CK(cudaMemcpyAsync(met_time_ns, c->deps.stamp.p, sizeof(int64_t) * size_t(c->T), cudaMemcpyDeviceToHost, c->stream));
   CK(cudaStreamSynchronize(c->stream));
   return EVG_OK;
 }
@@ -2142,6 +2173,42 @@ int evg_expected_durations_batch(evg_ctx* c, const evg_duration_rows* in, evg_du
   return EVG_OK;
 }
 
+// The finder tables of evg_find_runnable_batch and evg_plan_from_finder: checked, staged into pf.*, and k_runnable's view
+// of them (the caller sets r->met).  `any_deps`: some distro's finder reads the dependency verdicts.  n_distros > 0.
+static int stage_finder(evg_ctx* c, const evg_runnable_in* in, DRunnable* r, bool* any_deps) {
+  const int64_t T = in->n_tasks;
+  const int32_t D = in->n_distros, P = in->n_projects;
+  if (!in->task_off || !in->valid_off || !in->finder) return fail(EVG_ERR_INVALID, "null distro arrays");
+  if (T > 0 && (!in->sched || !in->project)) return fail(EVG_ERR_INVALID, "null task column");
+  if (P > 0 && !in->project_flags) return fail(EVG_ERR_INVALID, "null project_flags");
+  if (in->task_off[0] != 0 || in->task_off[D] != T || in->valid_off[0] != 0) return fail(EVG_ERR_INVALID, "offsets do not span the tables");
+  *any_deps = false;
+  for (int32_t d = 0; d < D; d++) {
+    if (in->task_off[d + 1] < in->task_off[d] || in->valid_off[d + 1] < in->valid_off[d]) return fail(EVG_ERR_INVALID, "offsets of distro %d decrease", d);
+    if (in->finder[d] > EVG_FINDER_ALTERNATE) return fail(EVG_ERR_INVALID, "distro %d: unknown finder %d", d, int(in->finder[d]));
+    *any_deps = *any_deps || in->finder[d] != EVG_FINDER_NO_DEPS;
+  }
+  const int64_t V = in->valid_off[D];
+  if (V > 0 && !in->valid_idx) return fail(EVG_ERR_INVALID, "null valid_idx");
+  CK(cudaSetDevice(c->device));
+  cudaStream_t s = c->stream;
+  auto& pf = c->pf;
+  UP(s, pf.task_off, in->task_off, D + 1, int64_t);
+  UP(s, pf.sched, in->sched, T, uint8_t);
+  UP(s, pf.project, in->project, T, int32_t);
+  UP(s, pf.project_flags, in->project_flags, P, uint8_t);
+  UP(s, pf.valid_off, in->valid_off, D + 1, int64_t);
+  UP(s, pf.valid_idx, in->valid_idx, V, int32_t);
+  UP(s, pf.finder, in->finder, D, uint8_t);
+  CK(pf.kept.ensure(sizeof(int32_t) * size_t(T + 1)));
+  CK(pf.count.ensure(sizeof(int64_t) * size_t(D + 1)));
+  r->n_tasks = T; r->n_distros = D; r->n_projects = P;
+  r->task_off = pf.task_off.as<int64_t>(); r->sched = pf.sched.as<uint8_t>(); r->project = pf.project.as<int32_t>();
+  r->project_flags = pf.project_flags.as<uint8_t>(); r->valid_off = pf.valid_off.as<int64_t>(); r->valid_idx = pf.valid_idx.as<int32_t>();
+  r->finder = pf.finder.as<uint8_t>(); r->met = nullptr;
+  return EVG_OK;
+}
+
 int evg_find_runnable_batch(evg_ctx* c, const evg_runnable_in* in, int32_t* runnable, int64_t* count) {
   if (!c || !in) return fail(EVG_ERR_INVALID, "evg_find_runnable_batch: null argument");
   LOCK(c);
@@ -2150,49 +2217,27 @@ int evg_find_runnable_batch(evg_ctx* c, const evg_runnable_in* in, int32_t* runn
   if (T < 0 || D < 0 || P < 0) return fail(EVG_ERR_INVALID, "negative sizes");
   if (D == 0) return T == 0 ? EVG_OK : fail(EVG_ERR_INVALID, "tasks without distros");
   if (!count || (T > 0 && !runnable)) return fail(EVG_ERR_INVALID, "null output");
-  if (!in->task_off || !in->valid_off || !in->finder) return fail(EVG_ERR_INVALID, "null distro arrays");
-  if (T > 0 && (!in->sched || !in->project)) return fail(EVG_ERR_INVALID, "null task column");
-  if (P > 0 && !in->project_flags) return fail(EVG_ERR_INVALID, "null project_flags");
-  if (in->task_off[0] != 0 || in->task_off[D] != T || in->valid_off[0] != 0) return fail(EVG_ERR_INVALID, "offsets do not span the tables");
-  bool any_deps = false;
-  for (int32_t d = 0; d < D; d++) {
-    if (in->task_off[d + 1] < in->task_off[d] || in->valid_off[d + 1] < in->valid_off[d]) return fail(EVG_ERR_INVALID, "offsets of distro %d decrease", d);
-    if (in->finder[d] > EVG_FINDER_ALTERNATE) return fail(EVG_ERR_INVALID, "distro %d: unknown finder %d", d, int(in->finder[d]));
-    any_deps = any_deps || in->finder[d] != EVG_FINDER_NO_DEPS;
-  }
-  const int64_t V = in->valid_off[D];
-  if (V > 0 && !in->valid_idx) return fail(EVG_ERR_INVALID, "null valid_idx");
+  DRunnable r;
+  bool any_deps;
+  int rc = stage_finder(c, in, &r, &any_deps);
+  if (rc != EVG_OK) return rc;
   if (any_deps && T > 0 && (!in->deps || in->deps->n_tasks != T)) return fail(EVG_ERR_INVALID, "a finder checks dependencies but deps is null or of another size");
-  CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   CK(c->b_err.ensure(sizeof(int) * 4));
   CK(cudaMemsetAsync(c->b_err.p, 0, sizeof(int) * 4, s));
   c->launches = 0;
-  c->have_tasks = false;  // the scratch columns below are shared with nothing resident, but the order buffer is reused
+  c->have_tasks = false;  // the tick's dependency verdicts and stamps are overwritten: a finder batch ends the resident tick
   if (any_deps && T > 0) {
-    int rc = deps_to_device(c, in->deps, 1);
+    rc = deps_to_device(c, in->deps, 1);
     if (rc != EVG_OK) return rc;
+    r.met = c->deps.met.as<uint8_t>();
   }
-  UP(s, c->b_rn0, in->task_off, D + 1, int64_t);
-  UP(s, c->b_rn1, in->sched, T, uint8_t);
-  UP(s, c->b_rn2, in->project, T, int32_t);
-  UP(s, c->b_rn3, in->project_flags, P, uint8_t);
-  UP(s, c->b_rn4, in->valid_off, D + 1, int64_t);
-  UP(s, c->b_rn5, in->valid_idx, V, int32_t);
-  UP(s, c->b_rn6, in->finder, D, uint8_t);
-  CK(c->b_order.ensure(sizeof(int32_t) * size_t(T + 1)));
-  CK(c->b_rn7.ensure(sizeof(int64_t) * size_t(D)));
-  DRunnable r;
-  r.n_tasks = T; r.n_distros = D; r.n_projects = P;
-  r.task_off = c->b_rn0.as<int64_t>(); r.sched = c->b_rn1.as<uint8_t>(); r.project = c->b_rn2.as<int32_t>();
-  r.project_flags = c->b_rn3.as<uint8_t>(); r.valid_off = c->b_rn4.as<int64_t>(); r.valid_idx = c->b_rn5.as<int32_t>();
-  r.finder = c->b_rn6.as<uint8_t>(); r.met = (any_deps && T > 0) ? c->b_dx7.as<uint8_t>() : nullptr;
-  k_runnable<<<unsigned(D), 256, 0, s>>>(r, c->b_order.as<int32_t>(), c->b_rn7.as<int64_t>(), c->b_err.as<int>());
+  k_runnable<<<unsigned(D), 256, 0, s>>>(r, c->pf.kept.as<int32_t>(), c->pf.count.as<int64_t>(), c->b_err.as<int>());
   c->launches++;
   CK(cudaGetLastError());
   int bad = 0;
-  if (T > 0) CK(cudaMemcpyAsync(runnable, c->b_order.p, sizeof(int32_t) * size_t(T), cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(count, c->b_rn7.p, sizeof(int64_t) * size_t(D), cudaMemcpyDeviceToHost, s));
+  if (T > 0) CK(cudaMemcpyAsync(runnable, c->pf.kept.p, sizeof(int32_t) * size_t(T), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(count, c->pf.count.p, sizeof(int64_t) * size_t(D), cudaMemcpyDeviceToHost, s));
   CK(cudaMemcpyAsync(&bad, c->b_err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   if (bad) return fail(EVG_ERR_INVALID, "a project row or dep_ref is out of range");
@@ -2200,61 +2245,10 @@ int evg_find_runnable_batch(evg_ctx* c, const evg_runnable_in* in, int32_t* runn
 }
 
 // --------------------------------------------------------------------------
-// evg_plan_from_finder: finder -> dependency predicate -> compaction -> resident planner inputs, all on the device
+// compose_tick: a new resident table built on the device from the kept rows of a source table, in their order, and
+// each distro's inserted rows after them -- evg_edit_tasks (source: the resident tick) and evg_plan_from_finder
+// (source: the candidates; nothing inserted)
 // --------------------------------------------------------------------------
-struct PfCols {  // nine planner columns, candidate table (src) and compacted table (dst)
-  const int32_t *priority, *numdep, *tgo, *gid, *vid;
-  const uint32_t* flags;
-  const int64_t *expected, *qbasis, *wbasis;
-  int32_t *o_priority, *o_numdep, *o_tgo, *o_gid, *o_vid;
-  uint32_t* o_flags;
-  int64_t *o_expected, *o_qbasis, *o_wbasis;
-};
-// One thread per KEPT task: its row of the candidate table moves to its place in the compacted table; the
-// EVG_TF_DEPS_MET bit and the stamped wait basis come from the device's own evaluation (k_deps_met), like
-// evg_upload_with_deps.  new_idx[candidate row] = distro-local index in the compacted queue (memset to -1 before).
-__global__ void __launch_bounds__(256) k_pf_gather(int64_t n_new, int32_t D, const int64_t* __restrict__ new_off, const int64_t* __restrict__ cand_off,
-                                                   const int32_t* __restrict__ kept, PfCols C, const uint8_t* __restrict__ met,
-                                                   const int64_t* __restrict__ met_time, int32_t* __restrict__ new_idx, int64_t* __restrict__ src_row) {
-  const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
-  const int d = block_find_distro(new_off, D, i, n_new);
-  if (d < 0) return;
-  const int64_t k = i - new_off[d];
-  const int64_t src = cand_off[d] + kept[cand_off[d] + k];
-  C.o_priority[i] = C.priority[src]; C.o_numdep[i] = C.numdep[src]; C.o_tgo[i] = C.tgo[src]; C.o_gid[i] = C.gid[src]; C.o_vid[i] = C.vid[src];
-  C.o_expected[i] = C.expected[src]; C.o_qbasis[i] = C.qbasis[src];
-  C.o_flags[i] = (C.flags[src] & ~EVG_TF_DEPS_MET) | ((met[src] & 1) ? EVG_TF_DEPS_MET : 0u);
-  const int64_t wb = C.wbasis[src], st = met_time[src];
-  C.o_wbasis[i] = (st != EVG_TIME_ZERO && st > wb) ? st : wb;
-  new_idx[src] = int32_t(k);
-  src_row[i] = src;
-}
-// in-queue dependency edges that survive: both ends kept
-__global__ void __launch_bounds__(256) k_pf_edge_count(int64_t n_new, int32_t D, const int64_t* __restrict__ new_off, const int64_t* __restrict__ cand_off,
-                                                       const int64_t* __restrict__ src_row, const int64_t* __restrict__ dep_off,
-                                                       const int32_t* __restrict__ dep_idx, const int32_t* __restrict__ new_idx, int32_t* __restrict__ cnt) {
-  const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
-  const int d = block_find_distro(new_off, D, i, n_new);
-  if (d < 0) return;
-  const int64_t src = src_row[i], cb = cand_off[d];
-  int32_t n = 0;
-  for (int64_t e = dep_off[src]; e < dep_off[src + 1]; e++) n += new_idx[cb + dep_idx[e]] >= 0;
-  cnt[i] = n;
-}
-__global__ void __launch_bounds__(256) k_pf_edge_write(int64_t n_new, int32_t D, const int64_t* __restrict__ new_off, const int64_t* __restrict__ cand_off,
-                                                       const int64_t* __restrict__ src_row, const int64_t* __restrict__ dep_off,
-                                                       const int32_t* __restrict__ dep_idx, const int32_t* __restrict__ new_idx,
-                                                       const int64_t* __restrict__ o_dep_off, int32_t* __restrict__ o_dep_idx) {
-  const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
-  const int d = block_find_distro(new_off, D, i, n_new);
-  if (d < 0) return;
-  const int64_t src = src_row[i], cb = cand_off[d];
-  int64_t w = o_dep_off[i];
-  for (int64_t e = dep_off[src]; e < dep_off[src + 1]; e++) {
-    const int32_t j = new_idx[cb + dep_idx[e]];
-    if (j >= 0) o_dep_idx[w++] = j;
-  }
-}
 // exclusive scan of int32 counts into int64 offsets (n + 1 entries), three launches
 __global__ void __launch_bounds__(1024) k_scan_blocks(const int32_t* __restrict__ in, int64_t n, int64_t* __restrict__ out, int64_t* __restrict__ block_sum) {
   __shared__ int64_t sw[32];
@@ -2312,187 +2306,22 @@ __global__ void __launch_bounds__(1024) k_scan_add(int64_t* __restrict__ out, in
   if (i < n) out[i] += block_sum[blockIdx.x];
   if (i == 0) out[n] = block_sum[nb];
 }
-
-int evg_plan_from_finder(evg_ctx* c, const evg_runnable_in* in, const evg_task_soa* cand, const evg_distro_table* distros,
-                         const evg_host_soa* hosts, const int64_t* host_off, const evg_alloc_cfg* acfg, const int64_t* dep_finished_ns,
-                         int64_t now_ns, int32_t* runnable, int64_t* count) {
-  if (!c || !in || !cand || !distros) return fail(EVG_ERR_INVALID, "evg_plan_from_finder: null argument");
-  LOCK(c);
-  const int64_t T = in->n_tasks, E = cand->n_edges;
-  const int32_t D = in->n_distros, P = in->n_projects;
-  if (T < 0 || D < 0 || P < 0 || E < 0) return fail(EVG_ERR_INVALID, "negative sizes");
-  if (cand->n_tasks != T || distros->n_distros != D) return fail(EVG_ERR_INVALID, "the candidate table, the finder table and the distro table disagree on their sizes");
-  if (D == 0) return T == 0 ? evg_upload(c, cand, distros, hosts, host_off, acfg) : fail(EVG_ERR_INVALID, "tasks without distros");
-  if (!count) return fail(EVG_ERR_INVALID, "null count");
-  if (!in->task_off || !in->valid_off || !in->finder || !distros->task_off) return fail(EVG_ERR_INVALID, "null distro arrays");
-  if (T > 0 && (!in->sched || !in->project)) return fail(EVG_ERR_INVALID, "null task column");
-  if (P > 0 && !in->project_flags) return fail(EVG_ERR_INVALID, "null project_flags");
-  if (in->task_off[0] != 0 || in->task_off[D] != T || in->valid_off[0] != 0) return fail(EVG_ERR_INVALID, "offsets do not span the tables");
-  for (int32_t d = 0; d <= D; d++)
-    if (in->task_off[d] != distros->task_off[d]) return fail(EVG_ERR_INVALID, "the finder table and the distro table cut the candidates differently at distro %d", d);
-  for (int32_t d = 0; d < D; d++) {
-    if (in->task_off[d + 1] < in->task_off[d] || in->valid_off[d + 1] < in->valid_off[d]) return fail(EVG_ERR_INVALID, "offsets of distro %d decrease", d);
-    if (in->finder[d] > EVG_FINDER_ALTERNATE) return fail(EVG_ERR_INVALID, "distro %d: unknown finder %d", d, int(in->finder[d]));
-  }
-  const int64_t V = in->valid_off[D];
-  if (V > 0 && !in->valid_idx) return fail(EVG_ERR_INVALID, "null valid_idx");
-  if (T > 0 && (!in->deps || in->deps->n_tasks != T)) return fail(EVG_ERR_INVALID, "evg_plan_from_finder needs the candidates' dependency table (the planner's EVG_TF_DEPS_MET comes from it)");
-  if (T > 0 && (!cand->priority || !cand->expected_ns || !cand->queue_basis_ns || !cand->wait_basis_ns || !cand->num_dependents ||
-                !cand->task_group_order || !cand->group_id || !cand->version_id || !cand->flags))
-    return fail(EVG_ERR_INVALID, "null candidate column");
-  if (E > 0 && (!cand->dep_off || !cand->dep_idx)) return fail(EVG_ERR_INVALID, "null candidate dependency edges");
-  CK(cudaSetDevice(c->device));
-  cudaStream_t s = c->stream;
-  CK(c->b_err.ensure(sizeof(int) * 4));
-  CK(cudaMemsetAsync(c->b_err.p, 0, sizeof(int) * 4, s));
-  c->launches = 0;
-  c->have_tasks = false;
-  if (T == 0) {
-    for (int32_t d = 0; d < D; d++) count[d] = 0;
-    return evg_upload(c, cand, distros, hosts, host_off, acfg);
-  }
-  // 1. Task.DependenciesMet / AllDependenciesSatisfied of every candidate, with the DependenciesMetTime stamps
-  int rc = deps_to_device(c, in->deps, 1, dep_finished_ns, now_ns, /*want_stamp=*/true);
-  if (rc != EVG_OK) return rc;
-  // 2. the finders
-  auto& pf = c->pf;
-  UP(s, pf.task_off, in->task_off, D + 1, int64_t);
-  UP(s, pf.sched, in->sched, T, uint8_t);
-  UP(s, pf.project, in->project, T, int32_t);
-  UP(s, pf.project_flags, in->project_flags, P, uint8_t);
-  UP(s, pf.valid_off, in->valid_off, D + 1, int64_t);
-  UP(s, pf.valid_idx, in->valid_idx, V, int32_t);
-  UP(s, pf.finder, in->finder, D, uint8_t);
-  CK(pf.kept.ensure(sizeof(int32_t) * size_t(T + 1)));
-  CK(pf.count.ensure(sizeof(int64_t) * size_t(D + 1)));
-  DRunnable r;
-  r.n_tasks = T; r.n_distros = D; r.n_projects = P;
-  r.task_off = pf.task_off.as<int64_t>(); r.sched = pf.sched.as<uint8_t>(); r.project = pf.project.as<int32_t>();
-  r.project_flags = pf.project_flags.as<uint8_t>(); r.valid_off = pf.valid_off.as<int64_t>(); r.valid_idx = pf.valid_idx.as<int32_t>();
-  r.finder = pf.finder.as<uint8_t>(); r.met = c->b_dx7.as<uint8_t>();
-  k_runnable<<<unsigned(D), 256, 0, s>>>(r, pf.kept.as<int32_t>(), pf.count.as<int64_t>(), c->b_err.as<int>());
-  c->launches++;
-  CK(cudaGetLastError());
-  // 3. the only thing the host needs before the planner can be routed: how many tasks each distro kept
-  int bad = 0;
-  CK(cudaMemcpyAsync(count, pf.count.p, sizeof(int64_t) * size_t(D), cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(&bad, c->b_err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
-  if (runnable) CK(cudaMemcpyAsync(runnable, pf.kept.p, sizeof(int32_t) * size_t(T), cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  if (bad) return fail(EVG_ERR_INVALID, "a project row or dep_ref is out of range");
-  std::vector<int64_t> new_off(size_t(D) + 1, 0);
-  for (int32_t d = 0; d < D; d++) {
-    if (count[d] < 0 || count[d] > in->task_off[d + 1] - in->task_off[d]) return fail(EVG_ERR_CUDA, "finder count out of range");
-    new_off[size_t(d) + 1] = new_off[size_t(d)] + count[d];
-  }
-  const int64_t Tn = new_off[size_t(D)];
-  // 4. candidate columns to the device, compaction into the context's own buffers
-  UP(s, pf.cand.prio, cand->priority, T, int32_t);
-  UP(s, pf.cand.nd, cand->num_dependents, T, int32_t);
-  UP(s, pf.cand.tgo, cand->task_group_order, T, int32_t);
-  UP(s, pf.cand.gid, cand->group_id, T, int32_t);
-  UP(s, pf.cand.vid, cand->version_id, T, int32_t);
-  UP(s, pf.cand.flags, cand->flags, T, uint32_t);
-  UP(s, pf.cand.exp, cand->expected_ns, T, int64_t);
-  UP(s, pf.cand.qb, cand->queue_basis_ns, T, int64_t);
-  UP(s, pf.cand.wb, cand->wait_basis_ns, T, int64_t);
-  UP(s, pf.new_off, new_off.data(), D + 1, int64_t);
-  const size_t np = size_t(Tn + kColPad);
-  for (DevBuf* b : {&pf.out.prio, &pf.out.nd, &pf.out.tgo, &pf.out.gid, &pf.out.vid, &pf.out.flags}) {  // 4-byte columns
-    CK(b->ensure(4 * np));
-    CK(cudaMemsetAsync(b->p, 0, 4 * np, s));
-  }
-  for (DevBuf* b : {&pf.out.exp, &pf.out.qb, &pf.out.wb}) {  // 8-byte columns
-    CK(b->ensure(8 * np));
-    CK(cudaMemsetAsync(b->p, 0, 8 * np, s));
-  }
-  CK(pf.new_idx.ensure(sizeof(int32_t) * size_t(T + 1)));
-  CK(cudaMemsetAsync(pf.new_idx.p, 0xFF, sizeof(int32_t) * size_t(T + 1), s));
-  CK(pf.src_row.ensure(sizeof(int64_t) * size_t(Tn + 1)));
-  PfCols pc;
-  pc.priority = pf.cand.prio.as<int32_t>(); pc.numdep = pf.cand.nd.as<int32_t>(); pc.tgo = pf.cand.tgo.as<int32_t>();
-  pc.gid = pf.cand.gid.as<int32_t>(); pc.vid = pf.cand.vid.as<int32_t>(); pc.flags = pf.cand.flags.as<uint32_t>();
-  pc.expected = pf.cand.exp.as<int64_t>(); pc.qbasis = pf.cand.qb.as<int64_t>(); pc.wbasis = pf.cand.wb.as<int64_t>();
-  pc.o_priority = pf.out.prio.as<int32_t>(); pc.o_numdep = pf.out.nd.as<int32_t>(); pc.o_tgo = pf.out.tgo.as<int32_t>();
-  pc.o_gid = pf.out.gid.as<int32_t>(); pc.o_vid = pf.out.vid.as<int32_t>(); pc.o_flags = pf.out.flags.as<uint32_t>();
-  pc.o_expected = pf.out.exp.as<int64_t>(); pc.o_qbasis = pf.out.qb.as<int64_t>(); pc.o_wbasis = pf.out.wb.as<int64_t>();
-  const int64_t* d_new_off = pf.new_off.as<int64_t>();
-  const int64_t* d_cand_off = pf.task_off.as<int64_t>();
-  if (Tn > 0) {
-    k_pf_gather<<<grid_for(Tn, 256), 256, 0, s>>>(Tn, D, d_new_off, d_cand_off, pf.kept.as<int32_t>(), pc, c->b_dx7.as<uint8_t>(),
-                                                  c->b_rn7.as<int64_t>(), pf.new_idx.as<int32_t>(), pf.src_row.as<int64_t>());
-    c->launches++;
-  }
-  // 5. in-queue dependency edges between kept tasks
-  int64_t En = 0;
-  std::vector<int64_t> edge_off;
-  if (E > 0 && Tn > 0) {
-    UP(s, pf.dep_off, cand->dep_off, T + 1, int64_t);
-    UP(s, pf.dep_idx, cand->dep_idx, E, int32_t);
-    CK(pf.edge_cnt.ensure(sizeof(int32_t) * size_t(Tn + 1)));               // surviving edges per kept task
-    CK(pf.new_dep_off.ensure(sizeof(int64_t) * size_t(Tn + 1 + kColPad)));
-    const int64_t nb = (Tn + 1023) / 1024;
-    CK(pf.scan_sum.ensure(sizeof(int64_t) * size_t(nb + 1)));
-    k_pf_edge_count<<<grid_for(Tn, 256), 256, 0, s>>>(Tn, D, d_new_off, d_cand_off, pf.src_row.as<int64_t>(), pf.dep_off.as<int64_t>(),
-                                                      pf.dep_idx.as<int32_t>(), pf.new_idx.as<int32_t>(), pf.edge_cnt.as<int32_t>());
-    k_scan_blocks<<<unsigned(nb), 1024, 0, s>>>(pf.edge_cnt.as<int32_t>(), Tn, pf.new_dep_off.as<int64_t>(), pf.scan_sum.as<int64_t>());
-    k_scan_sums<<<1, 1024, 0, s>>>(pf.scan_sum.as<int64_t>(), nb);
-    k_scan_add<<<unsigned(nb), 1024, 0, s>>>(pf.new_dep_off.as<int64_t>(), Tn, pf.scan_sum.as<int64_t>(), nb);
-    c->launches += 4;
-    CK(cudaMemcpyAsync(&En, pf.new_dep_off.as<int64_t>() + Tn, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
-    // dep_off sampled at the distro boundaries: what the routing needs of the edges
-    edge_off.resize(size_t(D) + 1);
-    CK(c->b_rn0.ensure(sizeof(int64_t) * size_t(D + 1)));
-    k_gather_i64<<<grid_for(D + 1, 256), 256, 0, s>>>(pf.new_dep_off.as<int64_t>(), d_new_off, c->b_rn0.as<int64_t>(), D + 1);
-    CK(cudaMemcpyAsync(edge_off.data(), c->b_rn0.p, sizeof(int64_t) * size_t(D + 1), cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    CK(pf.new_dep_idx.ensure(sizeof(int32_t) * size_t(En + 1)));
-    if (En > 0) {
-      k_pf_edge_write<<<grid_for(Tn, 256), 256, 0, s>>>(Tn, D, d_new_off, d_cand_off, pf.src_row.as<int64_t>(), pf.dep_off.as<int64_t>(),
-                                                        pf.dep_idx.as<int32_t>(), pf.new_idx.as<int32_t>(), pf.new_dep_off.as<int64_t>(),
-                                                        pf.new_dep_idx.as<int32_t>());
-      c->launches++;
-    }
-  }
-  CK(cudaGetLastError());
-  // 6. the compacted table becomes the resident tick (columns stay where they are: context-owned device memory)
-  evg_task_soa ts;
-  memset(&ts, 0, sizeof(ts));
-  ts.n_tasks = Tn; ts.n_edges = En;
-  ts.priority = pc.o_priority; ts.num_dependents = pc.o_numdep; ts.task_group_order = pc.o_tgo; ts.group_id = pc.o_gid; ts.version_id = pc.o_vid;
-  ts.flags = pc.o_flags; ts.expected_ns = pc.o_expected; ts.queue_basis_ns = pc.o_qbasis; ts.wait_basis_ns = pc.o_wbasis;
-  if (En > 0) { ts.dep_off = pf.new_dep_off.as<int64_t>(); ts.dep_idx = pf.new_dep_idx.as<int32_t>(); }
-  evg_distro_table dn = *distros;
-  dn.task_off = new_off.data();
-  rc = upload_tasks(c, &ts, &dn, Cols::kAdopt, (En > 0) ? edge_off.data() : nullptr);
-  if (rc != EVG_OK) return rc;
-  if (hosts) {
-    rc = upload_hosts(c, hosts, host_off, acfg, D);
-    if (rc != EVG_OK) return rc;
-  }
-  CK(cudaStreamSynchronize(s));
-  c->editable = true;  // the compacted columns are the context's own (pf.out), not the caller's
-  return EVG_OK;
-}
-
-// --------------------------------------------------------------------------
-// evg_edit_tasks: the composed table (survivors, then inserted rows, per distro) built on the device
-// --------------------------------------------------------------------------
 struct EdDst {  // the shadow column set the composed table is written to
   int32_t *priority, *numdep, *tgo, *gid, *vid;
   uint32_t* flags;
   int64_t *expected, *qbasis, *wbasis;
 };
-// Where row i of the composed table comes from.  Distro d's composed rows are its survivors in their resident order
-// (S_d of them), then its inserted rows ins_off[d] .. ins_off[d+1].
+// Where row i of the composed table comes from.  Distro d's composed rows are its survivors in their source order
+// (S_d of them), then its inserted rows ins_off[d] .. ins_off[d+1].  The source is the resident table (an edit) or the
+// candidates (the finder).
 struct EdMap {
   int32_t D;
   const int64_t* new_off;    // D+1: composed task_off
-  const int64_t* old_off;    // D+1: resident task_off
+  const int64_t* old_off;    // D+1: source task_off
   const int64_t* ins_off;    // D+1: CSR of the inserted rows over distros
-  const int32_t* keep;       // [resident T]: 1 = survives
-  const int64_t* pos;        // [resident T + 1]: exclusive scan of keep (survivors before a resident row, all distros)
-  const int32_t* src;        // [composed T]: resident row of a survivor (unset for inserted rows)
+  const int32_t* keep;       // [source T]: 1 = survives
+  const int64_t* pos;        // [source T + 1]: exclusive scan of keep (survivors before a source row, all distros)
+  const int32_t* src;        // [composed T]: source row of a survivor (unset for inserted rows)
   const int64_t* old_goff;   // D+1: resident group_off
   const int64_t* old_vbase;  // D+1: prefix sum of the resident n_versions
   const int32_t* gremap;     // per resident group slot: new distro-local id, -1 = none; NULL = ids kept
@@ -2527,7 +2356,7 @@ __global__ void __launch_bounds__(256) k_ed_src(int64_t n_old, EdMap m, int32_t*
   if (d < 0 || !m.keep[t]) return;
   src[m.pos[t] + m.ins_off[d]] = int32_t(t);
 }
-// One thread per composed row: a survivor's row of the resident columns (group and version ids remapped), or a staged
+// One thread per composed row: a survivor's row of the source columns (group and version ids remapped), or a staged
 // inserted row.  err[0] = 1 when a survivor's task group maps to -1.
 __global__ void __launch_bounds__(256) k_ed_gather(int64_t n_new, EdMap m, DTasks O, DTasks I, EdDst o, int* __restrict__ err) {
   const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -2550,10 +2379,12 @@ __global__ void __launch_bounds__(256) k_ed_gather(int64_t n_new, EdMap m, DTask
     o.flags[i] = I.flags[j]; o.expected[i] = I.expected[j]; o.qbasis[i] = I.qbasis[j]; o.wbasis[i] = I.wbasis[j];
   }
 }
-// Edges of composed row i: a survivor's resident edges whose dependency survived, re-indexed and in their order, then
-// its added edges; an inserted row's own edges.  cnt != NULL: count them; otherwise write them at o_dep_off[i].
+// Edges of composed row i: a survivor's source edges whose dependency survived, re-indexed and in their order, then
+// its added edges; an inserted row's own edges.  o_dep_idx == NULL: count them, raising bit 2 of *err for a source
+// dep_idx outside its distro (the count pass runs before the source's ids are range-checked); otherwise write them at
+// o_dep_off[i].
 __device__ __forceinline__ int64_t ed_edges(const EdMap& m, const DTasks& O, const DTasks& I, int64_t i, int d,
-                                            const int64_t* __restrict__ o_dep_off, int32_t* __restrict__ o_dep_idx) {
+                                            const int64_t* __restrict__ o_dep_off, int32_t* __restrict__ o_dep_idx, int* err) {
   const int64_t k = i - m.new_off[d], S = ed_survivors(m, d);
   int64_t w = o_dep_off ? o_dep_off[i] : 0, n = 0;
   if (k < S) {
@@ -2561,7 +2392,9 @@ __device__ __forceinline__ int64_t ed_edges(const EdMap& m, const DTasks& O, con
     if (O.n_edges > 0) {
       const int64_t first = m.pos[base];
       for (int64_t e = O.dep_off[t]; e < O.dep_off[t + 1]; e++) {
-        const int64_t u = base + O.dep_idx[e];
+        const int32_t x = O.dep_idx[e];
+        if (err && (x < 0 || x >= m.old_off[d + 1] - base)) { atomicOr(err, 2); continue; }
+        const int64_t u = base + x;
         if (!m.keep[u]) continue;
         if (o_dep_idx) o_dep_idx[w + n] = int32_t(m.pos[u] - first);
         n++;
@@ -2581,20 +2414,243 @@ __device__ __forceinline__ int64_t ed_edges(const EdMap& m, const DTasks& O, con
   }
   return n;
 }
-__global__ void __launch_bounds__(256) k_ed_edge_count(int64_t n_new, EdMap m, DTasks O, DTasks I, int32_t* __restrict__ cnt) {
+__global__ void __launch_bounds__(256) k_ed_edge_count(int64_t n_new, EdMap m, DTasks O, DTasks I, int32_t* __restrict__ cnt, int* err) {
   const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
   const int d = block_find_distro(m.new_off, m.D, i, n_new);
   if (d < 0) return;
-  cnt[i] = int32_t(ed_edges(m, O, I, i, d, nullptr, nullptr));
+  cnt[i] = int32_t(ed_edges(m, O, I, i, d, nullptr, nullptr, err));
 }
 __global__ void __launch_bounds__(256) k_ed_edge_write(int64_t n_new, EdMap m, DTasks O, DTasks I, const int64_t* __restrict__ o_dep_off,
                                                        int32_t* __restrict__ o_dep_idx) {
   const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
   const int d = block_find_distro(m.new_off, m.D, i, n_new);
   if (d < 0) return;
-  ed_edges(m, O, I, i, d, o_dep_off, o_dep_idx);
+  ed_edges(m, O, I, i, d, o_dep_off, o_dep_idx, nullptr);
 }
 
+// keep[candidate] = 1 for every candidate k_runnable kept (keep zeroed before): kept[] holds each distro's kept
+// candidates as distro-local indices, its unused slots -1
+__global__ void __launch_bounds__(256) k_kept_mask(int64_t n, int32_t D, const int64_t* __restrict__ off, const int32_t* __restrict__ kept,
+                                                   int32_t* __restrict__ keep) {
+  const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  const int d = block_find_distro(off, D, i, n);
+  if (d < 0) return;
+  const int32_t k = kept[i];
+  if (k >= 0) keep[off[d] + k] = 1;
+}
+
+// A CSR offset array over n rows that spans `total` entries starts at 0, ends at total and never decreases: the first
+// row where `off` fails that (n: it does not start at 0 or end at total), -1 when it holds.
+static int64_t csr_bad_row(const int64_t* off, int64_t n, int64_t total) {
+  if (off[0] != 0 || off[n] != total) return n;
+  for (int64_t j = 0; j < n; j++)
+    if (off[j + 1] < off[j]) return j;
+  return -1;
+}
+static int check_csr(int64_t bad_row, int64_t n, const char* what) {
+  if (bad_row < 0) return EVG_OK;
+  if (bad_row == n) return fail(EVG_ERR_INVALID, "%s does not span n_edges", what);
+  return fail(EVG_ERR_INVALID, "%s decreases at row %lld", what, (long long)bad_row);
+}
+
+// The rows of O that ed.keep marks (O.n entries, staged by the caller) survive in their order, distro d's inserted rows
+// m.ins_off[d] .. m.ins_off[d+1] of In follow them, and the composed table over `distros` becomes the resident tick.  The
+// caller fills m but for new_off, keep, pos and src.  A device-side error leaves no resident tick.
+static int compose_tick(evg_ctx* c, EdMap m, const DTasks& O, const DTasks& In, const evg_distro_table* distros) {
+  cudaStream_t s = c->stream;
+  auto& e = c->ed;
+  const int32_t D = m.D;
+  const int64_t T0 = O.n, Tn = D > 0 ? distros->task_off[D] : 0;
+  UP(s, e.new_off, distros->task_off, D + 1, int64_t);
+  CK(e.pos.ensure(sizeof(int64_t) * size_t(T0 + 1)));
+  CK(e.src.ensure(sizeof(int32_t) * size_t(Tn + 1)));
+  CK(e.scan_sum.ensure(sizeof(int64_t) * size_t((std::max(T0, Tn) + 1023) / 1024 + 1)));  // both scans' block sums
+  CK(e.err.ensure(sizeof(int)));
+  CK(cudaMemsetAsync(e.err.p, 0, sizeof(int), s));
+  m.new_off = e.new_off.as<int64_t>(); m.keep = e.keep.as<int32_t>(); m.pos = e.pos.as<int64_t>(); m.src = e.src.as<int32_t>();
+  // ---- 1. survivors: the keep mask's scan (each survivor's place), composed row -> source row
+  if (T0 > 0) {
+    const int64_t nb = (T0 + 1023) / 1024;
+    k_scan_blocks<<<unsigned(nb), 1024, 0, s>>>(e.keep.as<int32_t>(), T0, e.pos.as<int64_t>(), e.scan_sum.as<int64_t>());
+    k_scan_sums<<<1, 1024, 0, s>>>(e.scan_sum.as<int64_t>(), nb);
+    k_scan_add<<<unsigned(nb), 1024, 0, s>>>(e.pos.as<int64_t>(), T0, e.scan_sum.as<int64_t>(), nb);
+    k_ed_src<<<grid_for(T0, 256), 256, 0, s>>>(T0, m, e.src.as<int32_t>());
+    c->launches += 4;
+  }
+  // ---- 2. the nine columns of the composed table into the shadow set (its padding zeroed, as an upload leaves it)
+  auto& sh = e.out;
+  const size_t np = size_t(Tn + kColPad);
+  for (DevBuf* b : {&sh.prio, &sh.nd, &sh.tgo, &sh.gid, &sh.vid, &sh.flags}) {
+    CK(b->ensure(4 * np));
+    CK(cudaMemsetAsync(b->as<int32_t>() + Tn, 0, 4 * kColPad, s));
+  }
+  for (DevBuf* b : {&sh.exp, &sh.qb, &sh.wb}) {
+    CK(b->ensure(8 * np));
+    CK(cudaMemsetAsync(b->as<int64_t>() + Tn, 0, 8 * kColPad, s));
+  }
+  EdDst o;
+  o.priority = sh.prio.as<int32_t>(); o.numdep = sh.nd.as<int32_t>(); o.tgo = sh.tgo.as<int32_t>(); o.gid = sh.gid.as<int32_t>();
+  o.vid = sh.vid.as<int32_t>(); o.flags = sh.flags.as<uint32_t>(); o.expected = sh.exp.as<int64_t>(); o.qbasis = sh.qb.as<int64_t>();
+  o.wbasis = sh.wb.as<int64_t>();
+  if (Tn > 0) {
+    k_ed_gather<<<grid_for(Tn, 256), 256, 0, s>>>(Tn, m, O, In, o, e.err.as<int>());
+    c->launches++;
+  }
+  // ---- 3. edges: count (range-checking the source's), scan, dep_off at the distro boundaries for the routing (one D2H,
+  // one sync), write
+  int64_t En = 0;
+  std::vector<int64_t> edge_off;
+  int bad = 0;
+  const bool edges = Tn > 0 && (O.n_edges > 0 || In.n_edges > 0 || m.n_add > 0);
+  if (edges) {
+    const int64_t nb = (Tn + 1023) / 1024;
+    CK(e.edge_cnt.ensure(sizeof(int32_t) * size_t(Tn + 1)));
+    CK(e.dep_off.ensure(sizeof(int64_t) * size_t(Tn + 1 + kColPad)));
+    k_ed_edge_count<<<grid_for(Tn, 256), 256, 0, s>>>(Tn, m, O, In, e.edge_cnt.as<int32_t>(), e.err.as<int>());
+    k_scan_blocks<<<unsigned(nb), 1024, 0, s>>>(e.edge_cnt.as<int32_t>(), Tn, e.dep_off.as<int64_t>(), e.scan_sum.as<int64_t>());
+    k_scan_sums<<<1, 1024, 0, s>>>(e.scan_sum.as<int64_t>(), nb);
+    k_scan_add<<<unsigned(nb), 1024, 0, s>>>(e.dep_off.as<int64_t>(), Tn, e.scan_sum.as<int64_t>(), nb);
+    CK(e.edge_at.ensure(sizeof(int64_t) * size_t(D + 1)));
+    k_gather_i64<<<grid_for(D + 1, 256), 256, 0, s>>>(e.dep_off.as<int64_t>(), e.new_off.as<int64_t>(), e.edge_at.as<int64_t>(), D + 1);
+    c->launches += 5;
+    edge_off.resize(size_t(D) + 1);
+    CK(cudaMemcpyAsync(edge_off.data(), e.edge_at.p, sizeof(int64_t) * size_t(D + 1), cudaMemcpyDeviceToHost, s));
+  }
+  CK(cudaMemcpyAsync(&bad, e.err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  if (bad & 1) { c->have_tasks = false; return fail(EVG_ERR_INVALID, "group_remap maps the task group of a surviving task to -1"); }
+  if (bad & 2) { c->have_tasks = false; return fail(EVG_ERR_INVALID, "an in-queue dep_idx is outside its distro"); }
+  if (edges) {
+    En = edge_off[size_t(D)];
+    CK(e.dep_idx.ensure(sizeof(int32_t) * size_t(En + kColPad)));
+    if (En > 0) {
+      k_ed_edge_write<<<grid_for(Tn, 256), 256, 0, s>>>(Tn, m, O, In, e.dep_off.as<int64_t>(), e.dep_idx.as<int32_t>());
+      c->launches++;
+      CK(cudaGetLastError());
+    }
+  }
+  // ---- 4. the shadow set becomes the resident one; route, size and range-check the composed table like an upload
+  c->tasks.swap(sh);
+  if (En > 0) { c->b_depoff.swap(e.dep_off); c->b_depidx.swap(e.dep_idx); }
+  evg_task_soa ts;
+  memset(&ts, 0, sizeof(ts));
+  ts.n_tasks = Tn; ts.n_edges = En;
+  ts.priority = c->tasks.prio.as<int32_t>(); ts.num_dependents = c->tasks.nd.as<int32_t>(); ts.task_group_order = c->tasks.tgo.as<int32_t>();
+  ts.group_id = c->tasks.gid.as<int32_t>(); ts.version_id = c->tasks.vid.as<int32_t>(); ts.flags = c->tasks.flags.as<uint32_t>();
+  ts.expected_ns = c->tasks.exp.as<int64_t>(); ts.queue_basis_ns = c->tasks.qb.as<int64_t>(); ts.wait_basis_ns = c->tasks.wb.as<int64_t>();
+  if (En > 0) { ts.dep_off = c->b_depoff.as<int64_t>(); ts.dep_idx = c->b_depidx.as<int32_t>(); }
+  int rc = upload_tasks(c, &ts, distros, Cols::kResident, En > 0 ? edge_off.data() : nullptr);
+  if (rc != EVG_OK) { c->have_tasks = false; return rc; }
+  return EVG_OK;
+}
+
+// --------------------------------------------------------------------------
+// evg_plan_from_finder: finder -> dependency predicate -> compaction -> resident planner inputs, all on the device
+// --------------------------------------------------------------------------
+int evg_plan_from_finder(evg_ctx* c, const evg_runnable_in* in, const evg_task_soa* cand, const evg_distro_table* distros,
+                         const evg_host_soa* hosts, const int64_t* host_off, const evg_alloc_cfg* acfg, const int64_t* dep_finished_ns,
+                         int64_t now_ns, int32_t* runnable, int64_t* count) {
+  if (!c || !in || !cand || !distros) return fail(EVG_ERR_INVALID, "evg_plan_from_finder: null argument");
+  LOCK(c);
+  const int64_t T = in->n_tasks, E = cand->n_edges;
+  const int32_t D = in->n_distros, P = in->n_projects;
+  if (T < 0 || D < 0 || P < 0 || E < 0) return fail(EVG_ERR_INVALID, "negative sizes");
+  if (cand->n_tasks != T || distros->n_distros != D) return fail(EVG_ERR_INVALID, "the candidate table, the finder table and the distro table disagree on their sizes");
+  if (D == 0) return T == 0 ? evg_upload(c, cand, distros, hosts, host_off, acfg) : fail(EVG_ERR_INVALID, "tasks without distros");
+  if (!count) return fail(EVG_ERR_INVALID, "null count");
+  // a composed row's source row is 32-bit (compose_tick's src)
+  if (T > (int64_t(1) << 31) - 2) return fail(EVG_ERR_INVALID, "evg_plan_from_finder: %lld candidates exceed 2^31-2", (long long)T);
+  if (!distros->task_off) return fail(EVG_ERR_INVALID, "null distro arrays");
+  if (T > 0 && (!in->deps || in->deps->n_tasks != T)) return fail(EVG_ERR_INVALID, "evg_plan_from_finder needs the candidates' dependency table (the planner's EVG_TF_DEPS_MET comes from it)");
+  if (T > 0 && (!cand->priority || !cand->expected_ns || !cand->queue_basis_ns || !cand->wait_basis_ns || !cand->num_dependents ||
+                !cand->task_group_order || !cand->group_id || !cand->version_id || !cand->flags))
+    return fail(EVG_ERR_INVALID, "null candidate column");
+  if (E > 0 && (!cand->dep_off || !cand->dep_idx)) return fail(EVG_ERR_INVALID, "null candidate dependency edges");
+  // The candidates' dep_off (8 B per candidate, ~10 ms of host memory reads at 8e6 candidates) is checked on a second
+  // host thread while this one stages the tables and the device runs the finders; it indexes nothing before step 4.
+  // (Where no thread can be started, the check runs at get().)
+  std::future<int64_t> dep_off_bad;
+  if (E > 0 && T > 0) dep_off_bad = std::async(std::launch::async | std::launch::deferred, csr_bad_row, cand->dep_off, T, E);
+  DRunnable r;
+  bool any_deps;
+  int rc = stage_finder(c, in, &r, &any_deps);
+  if (rc != EVG_OK) return rc;
+  for (int32_t d = 0; d <= D; d++)
+    if (in->task_off[d] != distros->task_off[d]) return fail(EVG_ERR_INVALID, "the finder table and the distro table cut the candidates differently at distro %d", d);
+  cudaStream_t s = c->stream;
+  CK(c->b_err.ensure(sizeof(int) * 4));
+  CK(cudaMemsetAsync(c->b_err.p, 0, sizeof(int) * 4, s));
+  c->launches = 0;
+  c->have_tasks = false;
+  if (T == 0) {
+    for (int32_t d = 0; d < D; d++) count[d] = 0;
+    return evg_upload(c, cand, distros, hosts, host_off, acfg);
+  }
+  // 1. Task.DependenciesMet / AllDependenciesSatisfied of every candidate, with the DependenciesMetTime stamps
+  rc = deps_to_device(c, in->deps, 1, dep_finished_ns, now_ns, /*want_stamp=*/true);
+  if (rc != EVG_OK) return rc;
+  // 2. the finders
+  auto& pf = c->pf;
+  r.met = c->deps.met.as<uint8_t>();
+  k_runnable<<<unsigned(D), 256, 0, s>>>(r, pf.kept.as<int32_t>(), pf.count.as<int64_t>(), c->b_err.as<int>());
+  c->launches++;
+  CK(cudaGetLastError());
+  // 3. the only thing the host needs before the planner can be routed: how many tasks each distro kept
+  int bad = 0;
+  CK(cudaMemcpyAsync(count, pf.count.p, sizeof(int64_t) * size_t(D), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(&bad, c->b_err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+  if (runnable) CK(cudaMemcpyAsync(runnable, pf.kept.p, sizeof(int32_t) * size_t(T), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  if (bad) return fail(EVG_ERR_INVALID, "a project row or dep_ref is out of range");
+  rc = dep_off_bad.valid() ? check_csr(dep_off_bad.get(), T, "evg_plan_from_finder: the candidate dep_off") : EVG_OK;
+  if (rc != EVG_OK) return rc;
+  std::vector<int64_t> new_off(size_t(D) + 1, 0);
+  for (int32_t d = 0; d < D; d++) {
+    if (count[d] < 0 || count[d] > in->task_off[d + 1] - in->task_off[d]) return fail(EVG_ERR_CUDA, "finder count out of range");
+    new_off[size_t(d) + 1] = new_off[size_t(d)] + count[d];
+  }
+  // 4. the candidates' columns, with the device's own verdict applied as evg_upload_with_deps applies it; the kept list
+  // as a keep mask
+  rc = pf.cand.stage(cand, T, s);
+  if (rc != EVG_OK) return rc;
+  DTasks O = pf.cand.view(T);
+  if (E > 0) {
+    UP(s, pf.dep_off, cand->dep_off, T + 1, int64_t);
+    UP(s, pf.dep_idx, cand->dep_idx, E, int32_t);
+    O.n_edges = E; O.dep_off = pf.dep_off.as<int64_t>(); O.dep_idx = pf.dep_idx.as<int32_t>();
+  }
+  k_apply_deps<<<grid_for(T, 256), 256, 0, s>>>(T, c->deps.met.as<uint8_t>(), c->deps.stamp.as<int64_t>(), pf.cand.flags.as<uint32_t>(),
+                                                pf.cand.wb.as<int64_t>());
+  auto& e = c->ed;
+  CK(e.keep.ensure(sizeof(int32_t) * size_t(T + 1)));
+  CK(cudaMemsetAsync(e.keep.p, 0, sizeof(int32_t) * size_t(T), s));
+  k_kept_mask<<<grid_for(T, 256), 256, 0, s>>>(T, D, pf.task_off.as<int64_t>(), pf.kept.as<int32_t>(), e.keep.as<int32_t>());
+  c->launches += 2;
+  CK(e.ins_off.ensure(sizeof(int64_t) * size_t(D + 1)));
+  CK(cudaMemsetAsync(e.ins_off.p, 0, sizeof(int64_t) * size_t(D + 1), s));
+  // 5. the kept candidates become the resident tick, in the context's own columns
+  EdMap m;
+  memset(&m, 0, sizeof(m));
+  m.D = D; m.old_off = pf.task_off.as<int64_t>(); m.ins_off = e.ins_off.as<int64_t>();
+  DTasks none;
+  memset(&none, 0, sizeof(none));
+  evg_distro_table dn = *distros;
+  dn.task_off = new_off.data();
+  rc = compose_tick(c, m, O, none, &dn);
+  if (rc != EVG_OK) return rc;
+  if (hosts) {
+    rc = upload_hosts(c, hosts, host_off, acfg, D);
+    if (rc != EVG_OK) return rc;
+  }
+  CK(cudaStreamSynchronize(s));
+  c->editable = true;
+  return EVG_OK;
+}
+
+// --------------------------------------------------------------------------
+// evg_edit_tasks: the composed table (survivors, then inserted rows, per distro) built on the device
+// --------------------------------------------------------------------------
 int evg_edit_tasks(evg_ctx* c, const evg_task_edit* ed, const evg_distro_table* distros, const evg_host_soa* hosts,
                    const int64_t* host_off, const evg_alloc_cfg* acfg) {
   if (!c) return fail(EVG_ERR_INVALID, "null context");
@@ -2631,9 +2687,8 @@ int evg_edit_tasks(evg_ctx* c, const evg_task_edit* ed, const evg_distro_table* 
     ins_off.assign(ed->insert_off, ed->insert_off + D + 1);
   }
   if (EI > 0) {
-    if (ins->dep_off[0] != 0 || ins->dep_off[I] != EI) return fail(EVG_ERR_INVALID, "evg_edit_tasks: the inserted dep_off does not span n_edges");
-    for (int64_t j = 0; j < I; j++)
-      if (ins->dep_off[j + 1] < ins->dep_off[j]) return fail(EVG_ERR_INVALID, "evg_edit_tasks: the inserted dep_off decreases at row %lld", (long long)j);
+    const int rc = check_csr(csr_bad_row(ins->dep_off, I, EI), I, "evg_edit_tasks: the inserted dep_off");
+    if (rc != EVG_OK) return rc;
   }
   if (D > 0 && (distros->task_off[0] != 0 || distros->group_off[0] != 0)) return fail(EVG_ERR_INVALID, "evg_edit_tasks: offsets must start at 0");
   for (int32_t d = 0; d < D; d++) {
@@ -2661,15 +2716,10 @@ int evg_edit_tasks(evg_ctx* c, const evg_task_edit* ed, const evg_distro_table* 
   c->launches = 0;
   // ---- stage the edit
   UP(s, e.rm, ed->remove_rows, R, int64_t);
-  UP(s, e.ins.prio, ins ? ins->priority : nullptr, I, int32_t);
-  UP(s, e.ins.nd, ins ? ins->num_dependents : nullptr, I, int32_t);
-  UP(s, e.ins.tgo, ins ? ins->task_group_order : nullptr, I, int32_t);
-  UP(s, e.ins.gid, ins ? ins->group_id : nullptr, I, int32_t);
-  UP(s, e.ins.vid, ins ? ins->version_id : nullptr, I, int32_t);
-  UP(s, e.ins.flags, ins ? ins->flags : nullptr, I, uint32_t);
-  UP(s, e.ins.exp, ins ? ins->expected_ns : nullptr, I, int64_t);
-  UP(s, e.ins.qb, ins ? ins->queue_basis_ns : nullptr, I, int64_t);
-  UP(s, e.ins.wb, ins ? ins->wait_basis_ns : nullptr, I, int64_t);
+  if (I > 0) {
+    int rc = e.ins.stage(ins, I, s);
+    if (rc != EVG_OK) return rc;
+  }
   UP(s, e.ins_dep_off, EI > 0 ? ins->dep_off : nullptr, EI > 0 ? I + 1 : 0, int64_t);
   UP(s, e.ins_dep_idx, EI > 0 ? ins->dep_idx : nullptr, EI, int32_t);
   UP(s, e.add_task, ed->add_edge_task, NA, int64_t);
@@ -2677,106 +2727,26 @@ int evg_edit_tasks(evg_ctx* c, const evg_task_edit* ed, const evg_distro_table* 
   const int64_t G0 = c->h_groupoff[size_t(D)];
   UP(s, e.gremap, ed->group_remap, ed->group_remap ? G0 : 0, int32_t);
   UP(s, e.vremap, ed->version_remap, ed->version_remap ? old_vbase[D] : 0, int32_t);
-  UP(s, e.new_off, distros->task_off, D + 1, int64_t);
   UP(s, e.old_off, c->h_taskoff.data(), D + 1, int64_t);
   UP(s, e.old_goff, c->h_groupoff.data(), D + 1, int64_t);
   UP(s, e.ins_off, ins_off.data(), D + 1, int64_t);
   UP(s, e.old_vbase, old_vbase.data(), D + 1, int64_t);
   CK(e.keep.ensure(sizeof(int32_t) * size_t(T0 + 1)));
-  CK(e.pos.ensure(sizeof(int64_t) * size_t(T0 + 1)));
-  CK(e.src.ensure(sizeof(int32_t) * size_t(Tn + 1)));
-  CK(e.scan_sum.ensure(sizeof(int64_t) * size_t((std::max(T0, Tn) + 1023) / 1024 + 1)));  // both scans' block sums
-  CK(e.err.ensure(sizeof(int)));
-  CK(cudaMemsetAsync(e.err.p, 0, sizeof(int), s));
+  if (T0 > 0) {
+    k_ed_keep<<<grid_for(T0, 256), 256, 0, s>>>(T0, e.rm.as<int64_t>(), R, e.keep.as<int32_t>());
+    c->launches++;
+  }
   EdMap m;
-  m.D = D; m.new_off = e.new_off.as<int64_t>(); m.old_off = e.old_off.as<int64_t>(); m.ins_off = e.ins_off.as<int64_t>();
-  m.keep = e.keep.as<int32_t>(); m.pos = e.pos.as<int64_t>(); m.src = e.src.as<int32_t>();
+  memset(&m, 0, sizeof(m));
+  m.D = D; m.old_off = e.old_off.as<int64_t>(); m.ins_off = e.ins_off.as<int64_t>();
   m.old_goff = e.old_goff.as<int64_t>(); m.old_vbase = e.old_vbase.as<int64_t>();
   m.gremap = ed->group_remap ? e.gremap.as<int32_t>() : nullptr;
   m.vremap = ed->version_remap ? e.vremap.as<int32_t>() : nullptr;
   m.n_add = NA; m.add_task = e.add_task.as<int64_t>(); m.add_dep = e.add_dep.as<int32_t>();
-  const DTasks O = dtasks(c);
-  DTasks In;
-  memset(&In, 0, sizeof(In));
-  In.n = I; In.n_edges = EI;
-  In.priority = e.ins.prio.as<int32_t>(); In.expected = e.ins.exp.as<int64_t>(); In.qbasis = e.ins.qb.as<int64_t>();
-  In.wbasis = e.ins.wb.as<int64_t>(); In.numdep = e.ins.nd.as<int32_t>(); In.tgo = e.ins.tgo.as<int32_t>();
-  In.gid = e.ins.gid.as<int32_t>(); In.vid = e.ins.vid.as<int32_t>(); In.flags = e.ins.flags.as<uint32_t>();
-  In.dep_off = e.ins_dep_off.as<int64_t>(); In.dep_idx = e.ins_dep_idx.as<int32_t>();
-  // ---- 1. survivors: keep mask, its scan (each survivor's place), composed row -> resident row
-  if (T0 > 0) {
-    const int64_t nb = (T0 + 1023) / 1024;
-    k_ed_keep<<<grid_for(T0, 256), 256, 0, s>>>(T0, e.rm.as<int64_t>(), R, e.keep.as<int32_t>());
-    k_scan_blocks<<<unsigned(nb), 1024, 0, s>>>(e.keep.as<int32_t>(), T0, e.pos.as<int64_t>(), e.scan_sum.as<int64_t>());
-    k_scan_sums<<<1, 1024, 0, s>>>(e.scan_sum.as<int64_t>(), nb);
-    k_scan_add<<<unsigned(nb), 1024, 0, s>>>(e.pos.as<int64_t>(), T0, e.scan_sum.as<int64_t>(), nb);
-    k_ed_src<<<grid_for(T0, 256), 256, 0, s>>>(T0, m, e.src.as<int32_t>());
-    c->launches += 5;
-  }
-  // ---- 2. the nine columns of the composed table into the shadow set (its padding zeroed, as an upload leaves it)
-  auto& sh = e.out;
-  const size_t np = size_t(Tn + kColPad);
-  for (DevBuf* b : {&sh.prio, &sh.nd, &sh.tgo, &sh.gid, &sh.vid, &sh.flags}) {
-    CK(b->ensure(4 * np));
-    CK(cudaMemsetAsync(b->as<int32_t>() + Tn, 0, 4 * kColPad, s));
-  }
-  for (DevBuf* b : {&sh.exp, &sh.qb, &sh.wb}) {
-    CK(b->ensure(8 * np));
-    CK(cudaMemsetAsync(b->as<int64_t>() + Tn, 0, 8 * kColPad, s));
-  }
-  EdDst o;
-  o.priority = sh.prio.as<int32_t>(); o.numdep = sh.nd.as<int32_t>(); o.tgo = sh.tgo.as<int32_t>(); o.gid = sh.gid.as<int32_t>();
-  o.vid = sh.vid.as<int32_t>(); o.flags = sh.flags.as<uint32_t>(); o.expected = sh.exp.as<int64_t>(); o.qbasis = sh.qb.as<int64_t>();
-  o.wbasis = sh.wb.as<int64_t>();
-  if (Tn > 0) {
-    k_ed_gather<<<grid_for(Tn, 256), 256, 0, s>>>(Tn, m, O, In, o, e.err.as<int>());
-    c->launches++;
-  }
-  // ---- 3. edges: count, scan, dep_off at the distro boundaries for the routing (one D2H, one sync), write
-  int64_t En = 0;
-  std::vector<int64_t> edge_off;
-  int bad = 0;
-  const bool edges = Tn > 0 && (c->E > 0 || EI > 0 || NA > 0);
-  if (edges) {
-    const int64_t nb = (Tn + 1023) / 1024;
-    CK(e.edge_cnt.ensure(sizeof(int32_t) * size_t(Tn + 1)));
-    CK(e.dep_off.ensure(sizeof(int64_t) * size_t(Tn + 1 + kColPad)));
-    k_ed_edge_count<<<grid_for(Tn, 256), 256, 0, s>>>(Tn, m, O, In, e.edge_cnt.as<int32_t>());
-    k_scan_blocks<<<unsigned(nb), 1024, 0, s>>>(e.edge_cnt.as<int32_t>(), Tn, e.dep_off.as<int64_t>(), e.scan_sum.as<int64_t>());
-    k_scan_sums<<<1, 1024, 0, s>>>(e.scan_sum.as<int64_t>(), nb);
-    k_scan_add<<<unsigned(nb), 1024, 0, s>>>(e.dep_off.as<int64_t>(), Tn, e.scan_sum.as<int64_t>(), nb);
-    CK(e.edge_at.ensure(sizeof(int64_t) * size_t(D + 1)));
-    k_gather_i64<<<grid_for(D + 1, 256), 256, 0, s>>>(e.dep_off.as<int64_t>(), e.new_off.as<int64_t>(), e.edge_at.as<int64_t>(), D + 1);
-    c->launches += 5;
-    edge_off.resize(size_t(D) + 1);
-    CK(cudaMemcpyAsync(edge_off.data(), e.edge_at.p, sizeof(int64_t) * size_t(D + 1), cudaMemcpyDeviceToHost, s));
-  }
-  CK(cudaMemcpyAsync(&bad, e.err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  CK(cudaGetLastError());
-  if (bad) { c->have_tasks = false; return fail(EVG_ERR_INVALID, "evg_edit_tasks: group_remap maps the task group of a surviving task to -1"); }
-  if (edges) {
-    En = edge_off[size_t(D)];
-    CK(e.dep_idx.ensure(sizeof(int32_t) * size_t(En + kColPad)));
-    if (En > 0) {
-      k_ed_edge_write<<<grid_for(Tn, 256), 256, 0, s>>>(Tn, m, O, In, e.dep_off.as<int64_t>(), e.dep_idx.as<int32_t>());
-      c->launches++;
-      CK(cudaGetLastError());
-    }
-  }
-  // ---- 4. the shadow set becomes the resident one; route, size and range-check the composed table like an upload
-  c->b_prio.swap(sh.prio); c->b_nd.swap(sh.nd); c->b_tgo.swap(sh.tgo); c->b_gid.swap(sh.gid); c->b_vid.swap(sh.vid);
-  c->b_flags.swap(sh.flags); c->b_exp.swap(sh.exp); c->b_qb.swap(sh.qb); c->b_wb.swap(sh.wb);
-  if (En > 0) { c->b_depoff.swap(e.dep_off); c->b_depidx.swap(e.dep_idx); }
-  evg_task_soa ts;
-  memset(&ts, 0, sizeof(ts));
-  ts.n_tasks = Tn; ts.n_edges = En;
-  ts.priority = c->b_prio.as<int32_t>(); ts.num_dependents = c->b_nd.as<int32_t>(); ts.task_group_order = c->b_tgo.as<int32_t>();
-  ts.group_id = c->b_gid.as<int32_t>(); ts.version_id = c->b_vid.as<int32_t>(); ts.flags = c->b_flags.as<uint32_t>();
-  ts.expected_ns = c->b_exp.as<int64_t>(); ts.queue_basis_ns = c->b_qb.as<int64_t>(); ts.wait_basis_ns = c->b_wb.as<int64_t>();
-  if (En > 0) { ts.dep_off = c->b_depoff.as<int64_t>(); ts.dep_idx = c->b_depidx.as<int32_t>(); }
-  int rc = upload_tasks(c, &ts, distros, Cols::kResident, En > 0 ? edge_off.data() : nullptr);
-  if (rc != EVG_OK) { c->have_tasks = false; return rc; }
+  DTasks In = e.ins.view(I);
+  In.n_edges = EI; In.dep_off = e.ins_dep_off.as<int64_t>(); In.dep_idx = e.ins_dep_idx.as<int32_t>();
+  int rc = compose_tick(c, m, dtasks(c), In, distros);
+  if (rc != EVG_OK) return rc;
   if (hosts) {
     rc = upload_hosts(c, hosts, host_off, acfg, D);
     if (rc != EVG_OK) return rc;
@@ -2895,17 +2865,17 @@ int evg_prioritize_legacy_batch(evg_ctx* c, const evg_legacy_soa* in, const int6
   cudaStream_t s = c->stream;
   c->launches = 0;
   c->have_tasks = false;  // shares scratch buffers with the other entry points
-  UP(s, c->b_exp, in->priority, T, int64_t);
-  UP(s, c->b_qb, in->ingest_ns, T, int64_t);
-  UP(s, c->b_wb, in->expected_ns, T, int64_t);
-  UP(s, c->b_nd, in->num_dependents, T, int32_t);
-  UP(s, c->b_prio, in->revision_order, T, int32_t);
-  UP(s, c->b_vid, in->project_id, T, int32_t);
-  UP(s, c->b_gid, in->tg_rank, T, int32_t);
+  UP(s, c->tasks.exp, in->priority, T, int64_t);
+  UP(s, c->tasks.qb, in->ingest_ns, T, int64_t);
+  UP(s, c->tasks.wb, in->expected_ns, T, int64_t);
+  UP(s, c->tasks.nd, in->num_dependents, T, int32_t);
+  UP(s, c->tasks.prio, in->revision_order, T, int32_t);
+  UP(s, c->tasks.vid, in->project_id, T, int32_t);
+  UP(s, c->tasks.gid, in->tg_rank, T, int32_t);
   UP(s, c->b_rn0, in->tg_pair_id, T, int32_t);
-  UP(s, c->b_tgo, in->task_group_order, T, int32_t);
+  UP(s, c->tasks.tgo, in->task_group_order, T, int32_t);
   UP(s, c->b_rn1, in->presort_rank, T, int32_t);
-  UP(s, c->b_flags, in->flags, T, uint32_t);
+  UP(s, c->tasks.flags, in->flags, T, uint32_t);
   UP(s, c->b_rn2, list_mode, 3 * int64_t(D), uint8_t);
   UP(s, c->b_taskoff, task_off, D + 1, int64_t);
   CK(c->b_order.ensure(sizeof(int32_t) * size_t(T + 1)));
@@ -2916,10 +2886,10 @@ int evg_prioritize_legacy_batch(evg_ctx* c, const evg_legacy_soa* in, const int6
   CK(c->b_status.ensure(sizeof(int32_t) * size_t(D + 1)));
   CK(cudaMemsetAsync(c->b_rn5.p, 0, sizeof(unsigned int) * 4 * size_t(D), s));
   DLegacy x;
-  x.n = T; x.priority = c->b_exp.as<int64_t>(); x.ingest = c->b_qb.as<int64_t>(); x.expected = c->b_wb.as<int64_t>();
-  x.numdep = c->b_nd.as<int32_t>(); x.revision = c->b_prio.as<int32_t>(); x.project = c->b_vid.as<int32_t>();
-  x.tg_rank = c->b_gid.as<int32_t>(); x.tg_pair = c->b_rn0.as<int32_t>(); x.tgo = c->b_tgo.as<int32_t>();
-  x.presort = c->b_rn1.as<int32_t>(); x.flags = c->b_flags.as<uint32_t>(); x.list_mode = c->b_rn2.as<uint8_t>();
+  x.n = T; x.priority = c->tasks.exp.as<int64_t>(); x.ingest = c->tasks.qb.as<int64_t>(); x.expected = c->tasks.wb.as<int64_t>();
+  x.numdep = c->tasks.nd.as<int32_t>(); x.revision = c->tasks.prio.as<int32_t>(); x.project = c->tasks.vid.as<int32_t>();
+  x.tg_rank = c->tasks.gid.as<int32_t>(); x.tg_pair = c->b_rn0.as<int32_t>(); x.tgo = c->tasks.tgo.as<int32_t>();
+  x.presort = c->b_rn1.as<int32_t>(); x.flags = c->tasks.flags.as<uint32_t>(); x.list_mode = c->b_rn2.as<uint8_t>();
   x.task_off = c->b_taskoff.as<int64_t>(); x.n_distros = D;
   int32_t* buf[2] = {c->b_rn3.as<int32_t>(), c->b_rn4.as<int32_t>()};
   int cur = 0;
@@ -2978,9 +2948,9 @@ int evg_dag_rebuild_batch(evg_ctx* c, const evg_dag_in* in, const int64_t* item_
   UP(s, c->b_groupoff, group_off, D + 1, int64_t);
   UP(s, c->b_depoff, in->dep_off, N + 1, int64_t);
   UP(s, c->b_depidx, in->dep_item, E, int32_t);
-  UP(s, c->b_gid, in->group_id, N, int32_t);
-  UP(s, c->b_tgo, in->group_index, N, int32_t);
-  DevBuf* scratch[] = {&c->b_prio, &c->b_nd, &c->b_vid, &c->b_flags, &c->b_rn0, &c->b_rn1, &c->b_rn2, &c->b_rn3, &c->b_rn4};
+  UP(s, c->tasks.gid, in->group_id, N, int32_t);
+  UP(s, c->tasks.tgo, in->group_index, N, int32_t);
+  DevBuf* scratch[] = {&c->tasks.prio, &c->tasks.nd, &c->tasks.vid, &c->tasks.flags, &c->b_rn0, &c->b_rn1, &c->b_rn2, &c->b_rn3, &c->b_rn4};
   for (DevBuf* b : scratch) CK(b->ensure(sizeof(int32_t) * size_t(N + D + 1)));
   CK(c->b_rn5.ensure(sizeof(int32_t) * size_t(E + 1)));
   CK(c->b_hasdep.ensure(size_t(N) + 16));
@@ -2990,9 +2960,9 @@ int evg_dag_rebuild_batch(evg_ctx* c, const evg_dag_in* in, const int64_t* item_
   DDag x;
   x.n = N; x.n_deps = E; x.n_distros = D;
   x.item_off = c->b_taskoff.as<int64_t>(); x.dep_off = c->b_depoff.as<int64_t>(); x.dep_item = c->b_depidx.as<int32_t>();
-  x.group_id = c->b_gid.as<int32_t>(); x.group_index = c->b_tgo.as<int32_t>();
-  x.succ_off = c->b_prio.as<int32_t>(); x.succ = c->b_rn5.as<int32_t>(); x.index = c->b_nd.as<int32_t>(); x.low = c->b_vid.as<int32_t>();
-  x.stack = c->b_flags.as<int32_t>(); x.cs_node = c->b_rn0.as<int32_t>(); x.cs_pos = c->b_rn1.as<int32_t>(); x.emit = c->b_rn2.as<int32_t>();
+  x.group_id = c->tasks.gid.as<int32_t>(); x.group_index = c->tasks.tgo.as<int32_t>();
+  x.succ_off = c->tasks.prio.as<int32_t>(); x.succ = c->b_rn5.as<int32_t>(); x.index = c->tasks.nd.as<int32_t>(); x.low = c->tasks.vid.as<int32_t>();
+  x.stack = c->tasks.flags.as<int32_t>(); x.cs_node = c->b_rn0.as<int32_t>(); x.cs_pos = c->b_rn1.as<int32_t>(); x.emit = c->b_rn2.as<int32_t>();
   x.on_stack = c->b_hasdep.as<uint8_t>();
   int32_t* d_nsorted = c->b_rn6.as<int32_t>();
   int32_t* d_ncycles = d_nsorted + (D + 1);

@@ -273,8 +273,9 @@ int evg_plan_and_alloc_batch(evg_ctx* ctx, const evg_task_soa* tasks, const evg_
  * may be NULL for planner-only use). */
 int evg_upload(evg_ctx* ctx, const evg_task_soa* tasks, const evg_distro_table* distros,
                const evg_host_soa* hosts, const int64_t* host_off, const evg_alloc_cfg* acfg);
-/* Tick-to-tick update of the resident task table: row rows[i] (a task slot of the last evg_upload, 0 <= rows[i] <
- * n_tasks) gets priority, num_dependents, task_group_order, flags, expected_ns, queue_basis_ns and wait_basis_ns of row i
+/* Tick-to-tick update of the resident task table: row rows[i] (a task slot of the resident table, 0 <= rows[i] <
+ * n_tasks: the table of evg_upload, evg_upload_with_deps or evg_edit_tasks, or the kept candidates of
+ * evg_plan_from_finder) gets priority, num_dependents, task_group_order, flags, expected_ns, queue_basis_ns and wait_basis_ns of row i
  * of `values` (values->n_tasks == n_rows; its group / version / dependency columns are not read: a task keeps its
  * distro, its task group, its version and its in-queue dependency edges -- a tick that adds or removes tasks calls
  * evg_edit_tasks first).  48 bytes cross PCIe per changed row instead of the whole table.  Not available after evg_upload_device (the
@@ -485,11 +486,14 @@ int evg_find_runnable_batch(evg_ctx* ctx, const evg_runnable_in* in, int32_t* ru
  * in-queue dependency edges between candidates as distro-local candidate indices); `distros` is the distro table over
  * the candidates (task_off == in->task_off; group / version ids may name groups no kept task is in).  On the device:
  * k_deps_met (both predicates, DependenciesMetTime stamps from dep_finished_ns, as evg_upload_with_deps) -> the finders
- * -> a stable compaction of the nine planner columns (EVG_TF_DEPS_MET and the stamped wait basis applied on the way)
- * -> the dependency edges whose two ends were kept, re-indexed.  The compacted table becomes the context's resident
- * tick: call evg_run_resident / evg_download next; ranks refer to the compacted queues, and `runnable` (n_tasks, may be
- * NULL) / `count` (n_distros) map them back exactly as evg_find_runnable_batch reports them.  The only values the host
- * reads in between are the n_distros counts (the routing needs queue lengths).
+ * -> EVG_TF_DEPS_MET and the stamped wait basis applied to the candidates' columns -> the compaction evg_edit_tasks
+ * uses, with the dropped candidates removed and nothing inserted: the kept rows in their order, and the dependency
+ * edges whose two ends were kept, re-indexed.  The kept table becomes the context's resident tick, in its own columns:
+ * call evg_run_resident / evg_download next (evg_update_tasks and evg_edit_tasks may follow, as after evg_upload); ranks
+ * refer to the compacted queues, and `runnable` (n_tasks, may be NULL) / `count` (n_distros) map them back exactly as
+ * evg_find_runnable_batch reports them.  The only values the host reads in between are the n_distros counts (the
+ * routing needs queue lengths).  EVG_ERR_INVALID for a candidate dep_off that does not start at 0, end at n_edges and
+ * never decrease, or a dep_idx outside its distro's candidates.
  * Replaces: the finder + checkDependenciesMet + PrioritizeTasks hand-over inside scheduler.PlanDistro
  * (scheduler/wrapper.go:60-118, scheduler/scheduler.go:56-168), where the filtered []task.Task is rebuilt on the host. */
 int evg_plan_from_finder(evg_ctx* ctx, const evg_runnable_in* in, const evg_task_soa* candidates, const evg_distro_table* distros,
