@@ -124,6 +124,18 @@ class RunnableInStruct(C.Structure):
                 ("valid_idx", C.c_void_p), ("finder", C.c_void_p), ("deps", C.POINTER(DepsInStruct))]
 
 
+class AliasInStruct(C.Structure):
+    _fields_ = [("tasks", TaskSoAStruct), ("n_groups", C.c_int32), ("n_versions", C.c_int32), ("group_max_hosts", C.c_void_p),
+                ("sched", C.c_void_p), ("task_group_max_hosts", C.c_void_p), ("primary", C.c_void_p),
+                ("secondary_off", C.c_void_p), ("secondary_idx", C.c_void_p), ("n_names", C.c_int32), ("_reserved", C.c_int32),
+                ("dest_off", C.c_void_p), ("dest_idx", C.c_void_p), ("deps", C.POINTER(DepsInStruct)),
+                ("dep_finished_ns", C.c_void_p)]
+
+
+class AliasOutStruct(C.Structure):
+    _fields_ = [("task_off", C.c_void_p), ("group_off", C.c_void_p), ("n_versions", C.c_void_p)]
+
+
 EVG_SQ_ACTIVATED, EVG_SQ_UNDISPATCHED, EVG_SQ_PRIORITY_OK, EVG_SQ_HOST_PLATFORM = 0x01, 0x02, 0x04, 0x08
 EVG_SQ_UNATTAINABLE, EVG_SQ_OVERRIDE_DEPS, EVG_SQ_GITHUB_PR, EVG_SQ_PATCH_REQUEST = 0x10, 0x20, 0x40, 0x80
 EVG_PF_ENABLED, EVG_PF_HIDDEN, EVG_PF_DISPATCHING_DISABLED, EVG_PF_PATCHING_DISABLED = 0x1, 0x2, 0x4, 0x8
@@ -184,6 +196,8 @@ SYMBOLS = {
     "evg_update_tasks": (C.c_int, [_P, C.c_int64, _P, _P]),
     "evg_edit_tasks": (C.c_int, [_P, _P, _P, _P, _P, _P]),
     "evg_plan_from_finder": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, C.c_int64, _P, _P]),
+    "evg_plan_aliases": (C.c_int, [_P, _P, _P, C.c_int32, C.c_int64, _P]),
+    "evg_download_alias_map": (C.c_int, [_P, _P, _P]),
     "evg_intern_columns": (C.c_int, [_P, _P, C.c_int32]),
     "evg_run_resident": (C.c_int, [_P, C.c_int64, C.c_uint32]),
     "evg_download": (C.c_int, [_P, _P, _P]),

@@ -911,6 +911,16 @@ struct evg_ctx {
     DevBuf new_off, old_off, old_goff, ins_off, old_vbase, edge_at;  // D+1 tables
     DevBuf keep, pos, src, scan_sum, edge_cnt, err;
   } ed;
+  // evg_plan_aliases (the first call allocates these): the staged source table, the (queue, task) pairs and the alias
+  // map evg_download_alias_map returns while `alias_map` holds (upload_tasks clears it)
+  bool alias_map = false;
+  struct {
+    TaskCols src;
+    DevBuf dep_off, dep_idx, gmax, sched, tgmax, primary, soff, sidx, doff, didx;  // the source table
+    DevBuf cnt, poff, keys[2], hist, hoff;     // pairs per row, their offsets, the pair keys, the radix pass counters
+    DevBuf hk, hv, gslot, vslot, fg, fv, pg, pv;  // first-appearance ids of groups and versions per queue
+    DevBuf qoff, samp, gout, srow, gsrc, err;  // queue offsets, per-distro samples, group slots, the alias map
+  } al;
   DevBuf b_err;
   DevBuf b_route, b_unitv, b_unita, b_unitn, b_unitmask;
   DevBuf b_punt, b_puntcnt;
@@ -1192,6 +1202,7 @@ int upload_tasks(evg_ctx* c, const evg_task_soa* t, const evg_distro_table* dt, 
   c->h_unitbase.swap(unit_base);
   c->h_dtileoff.swap(dtile_off);
   c->have_tasks = true;
+  c->alias_map = false;  // evg_plan_aliases sets it again after its upload
   c->editable = false;  // the entry point that uploaded says whether evg_edit_tasks may follow
   c->alist_valid = false;  // upload_hosts lists the allocator's distros against THIS table
   c->have_hosts = false;
@@ -2453,6 +2464,52 @@ static int check_csr(int64_t bad_row, int64_t n, const char* what) {
   return fail(EVG_ERR_INVALID, "%s decreases at row %lld", what, (long long)bad_row);
 }
 
+// Exclusive scan of n int32 counts into out[0 .. n] (int64; out[n] = the total); `sum` holds (n + 1023) / 1024 + 1 int64.
+static void scan_counts(evg_ctx* c, const int32_t* in, int64_t n, int64_t* out, int64_t* sum) {
+  const int64_t nb = (n + 1023) / 1024;
+  k_scan_blocks<<<unsigned(nb), 1024, 0, c->stream>>>(in, n, out, sum);
+  k_scan_sums<<<1, 1024, 0, c->stream>>>(sum, nb);
+  k_scan_add<<<unsigned(nb), 1024, 0, c->stream>>>(out, n, sum, nb);
+  c->launches += 3;
+}
+
+// The shadow column set sized for Tn rows, its padding zeroed as an upload leaves it: where a composed table is written.
+static int shadow_cols(evg_ctx* c, int64_t Tn, EdDst* o) {
+  cudaStream_t s = c->stream;
+  auto& sh = c->ed.out;
+  const size_t np = size_t(Tn + kColPad);
+  for (DevBuf* b : {&sh.prio, &sh.nd, &sh.tgo, &sh.gid, &sh.vid, &sh.flags}) {
+    CK(b->ensure(4 * np));
+    CK(cudaMemsetAsync(b->as<int32_t>() + Tn, 0, 4 * kColPad, s));
+  }
+  for (DevBuf* b : {&sh.exp, &sh.qb, &sh.wb}) {
+    CK(b->ensure(8 * np));
+    CK(cudaMemsetAsync(b->as<int64_t>() + Tn, 0, 8 * kColPad, s));
+  }
+  o->priority = sh.prio.as<int32_t>(); o->numdep = sh.nd.as<int32_t>(); o->tgo = sh.tgo.as<int32_t>(); o->gid = sh.gid.as<int32_t>();
+  o->vid = sh.vid.as<int32_t>(); o->flags = sh.flags.as<uint32_t>(); o->expected = sh.exp.as<int64_t>(); o->qbasis = sh.qb.as<int64_t>();
+  o->wbasis = sh.wb.as<int64_t>();
+  return EVG_OK;
+}
+
+// The composed table in the shadow set (Tn rows) and in ed.dep_off / ed.dep_idx (En edges; edge_off: dep_off at the
+// distro boundaries) becomes the resident one, routed, sized and range-checked like an upload.  An error leaves no tick.
+static int install_composed(evg_ctx* c, int64_t Tn, int64_t En, const int64_t* edge_off, const evg_distro_table* distros) {
+  auto& e = c->ed;
+  c->tasks.swap(e.out);
+  if (En > 0) { c->b_depoff.swap(e.dep_off); c->b_depidx.swap(e.dep_idx); }
+  evg_task_soa ts;
+  memset(&ts, 0, sizeof(ts));
+  ts.n_tasks = Tn; ts.n_edges = En;
+  ts.priority = c->tasks.prio.as<int32_t>(); ts.num_dependents = c->tasks.nd.as<int32_t>(); ts.task_group_order = c->tasks.tgo.as<int32_t>();
+  ts.group_id = c->tasks.gid.as<int32_t>(); ts.version_id = c->tasks.vid.as<int32_t>(); ts.flags = c->tasks.flags.as<uint32_t>();
+  ts.expected_ns = c->tasks.exp.as<int64_t>(); ts.queue_basis_ns = c->tasks.qb.as<int64_t>(); ts.wait_basis_ns = c->tasks.wb.as<int64_t>();
+  if (En > 0) { ts.dep_off = c->b_depoff.as<int64_t>(); ts.dep_idx = c->b_depidx.as<int32_t>(); }
+  int rc = upload_tasks(c, &ts, distros, Cols::kResident, En > 0 ? edge_off : nullptr);
+  if (rc != EVG_OK) { c->have_tasks = false; return rc; }
+  return EVG_OK;
+}
+
 // The rows of O that ed.keep marks (O.n entries, staged by the caller) survive in their order, distro d's inserted rows
 // m.ins_off[d] .. m.ins_off[d+1] of In follow them, and the composed table over `distros` becomes the resident tick.  The
 // caller fills m but for new_off, keep, pos and src.  A device-side error leaves no resident tick.
@@ -2470,28 +2527,14 @@ static int compose_tick(evg_ctx* c, EdMap m, const DTasks& O, const DTasks& In, 
   m.new_off = e.new_off.as<int64_t>(); m.keep = e.keep.as<int32_t>(); m.pos = e.pos.as<int64_t>(); m.src = e.src.as<int32_t>();
   // ---- 1. survivors: the keep mask's scan (each survivor's place), composed row -> source row
   if (T0 > 0) {
-    const int64_t nb = (T0 + 1023) / 1024;
-    k_scan_blocks<<<unsigned(nb), 1024, 0, s>>>(e.keep.as<int32_t>(), T0, e.pos.as<int64_t>(), e.scan_sum.as<int64_t>());
-    k_scan_sums<<<1, 1024, 0, s>>>(e.scan_sum.as<int64_t>(), nb);
-    k_scan_add<<<unsigned(nb), 1024, 0, s>>>(e.pos.as<int64_t>(), T0, e.scan_sum.as<int64_t>(), nb);
+    scan_counts(c, e.keep.as<int32_t>(), T0, e.pos.as<int64_t>(), e.scan_sum.as<int64_t>());
     k_ed_src<<<grid_for(T0, 256), 256, 0, s>>>(T0, m, e.src.as<int32_t>());
-    c->launches += 4;
+    c->launches++;
   }
-  // ---- 2. the nine columns of the composed table into the shadow set (its padding zeroed, as an upload leaves it)
-  auto& sh = e.out;
-  const size_t np = size_t(Tn + kColPad);
-  for (DevBuf* b : {&sh.prio, &sh.nd, &sh.tgo, &sh.gid, &sh.vid, &sh.flags}) {
-    CK(b->ensure(4 * np));
-    CK(cudaMemsetAsync(b->as<int32_t>() + Tn, 0, 4 * kColPad, s));
-  }
-  for (DevBuf* b : {&sh.exp, &sh.qb, &sh.wb}) {
-    CK(b->ensure(8 * np));
-    CK(cudaMemsetAsync(b->as<int64_t>() + Tn, 0, 8 * kColPad, s));
-  }
+  // ---- 2. the nine columns of the composed table into the shadow set
   EdDst o;
-  o.priority = sh.prio.as<int32_t>(); o.numdep = sh.nd.as<int32_t>(); o.tgo = sh.tgo.as<int32_t>(); o.gid = sh.gid.as<int32_t>();
-  o.vid = sh.vid.as<int32_t>(); o.flags = sh.flags.as<uint32_t>(); o.expected = sh.exp.as<int64_t>(); o.qbasis = sh.qb.as<int64_t>();
-  o.wbasis = sh.wb.as<int64_t>();
+  int rc = shadow_cols(c, Tn, &o);
+  if (rc != EVG_OK) return rc;
   if (Tn > 0) {
     k_ed_gather<<<grid_for(Tn, 256), 256, 0, s>>>(Tn, m, O, In, o, e.err.as<int>());
     c->launches++;
@@ -2503,16 +2546,13 @@ static int compose_tick(evg_ctx* c, EdMap m, const DTasks& O, const DTasks& In, 
   int bad = 0;
   const bool edges = Tn > 0 && (O.n_edges > 0 || In.n_edges > 0 || m.n_add > 0);
   if (edges) {
-    const int64_t nb = (Tn + 1023) / 1024;
     CK(e.edge_cnt.ensure(sizeof(int32_t) * size_t(Tn + 1)));
     CK(e.dep_off.ensure(sizeof(int64_t) * size_t(Tn + 1 + kColPad)));
     k_ed_edge_count<<<grid_for(Tn, 256), 256, 0, s>>>(Tn, m, O, In, e.edge_cnt.as<int32_t>(), e.err.as<int>());
-    k_scan_blocks<<<unsigned(nb), 1024, 0, s>>>(e.edge_cnt.as<int32_t>(), Tn, e.dep_off.as<int64_t>(), e.scan_sum.as<int64_t>());
-    k_scan_sums<<<1, 1024, 0, s>>>(e.scan_sum.as<int64_t>(), nb);
-    k_scan_add<<<unsigned(nb), 1024, 0, s>>>(e.dep_off.as<int64_t>(), Tn, e.scan_sum.as<int64_t>(), nb);
+    scan_counts(c, e.edge_cnt.as<int32_t>(), Tn, e.dep_off.as<int64_t>(), e.scan_sum.as<int64_t>());
     CK(e.edge_at.ensure(sizeof(int64_t) * size_t(D + 1)));
     k_gather_i64<<<grid_for(D + 1, 256), 256, 0, s>>>(e.dep_off.as<int64_t>(), e.new_off.as<int64_t>(), e.edge_at.as<int64_t>(), D + 1);
-    c->launches += 5;
+    c->launches += 2;
     edge_off.resize(size_t(D) + 1);
     CK(cudaMemcpyAsync(edge_off.data(), e.edge_at.p, sizeof(int64_t) * size_t(D + 1), cudaMemcpyDeviceToHost, s));
   }
@@ -2530,19 +2570,8 @@ static int compose_tick(evg_ctx* c, EdMap m, const DTasks& O, const DTasks& In, 
       CK(cudaGetLastError());
     }
   }
-  // ---- 4. the shadow set becomes the resident one; route, size and range-check the composed table like an upload
-  c->tasks.swap(sh);
-  if (En > 0) { c->b_depoff.swap(e.dep_off); c->b_depidx.swap(e.dep_idx); }
-  evg_task_soa ts;
-  memset(&ts, 0, sizeof(ts));
-  ts.n_tasks = Tn; ts.n_edges = En;
-  ts.priority = c->tasks.prio.as<int32_t>(); ts.num_dependents = c->tasks.nd.as<int32_t>(); ts.task_group_order = c->tasks.tgo.as<int32_t>();
-  ts.group_id = c->tasks.gid.as<int32_t>(); ts.version_id = c->tasks.vid.as<int32_t>(); ts.flags = c->tasks.flags.as<uint32_t>();
-  ts.expected_ns = c->tasks.exp.as<int64_t>(); ts.queue_basis_ns = c->tasks.qb.as<int64_t>(); ts.wait_basis_ns = c->tasks.wb.as<int64_t>();
-  if (En > 0) { ts.dep_off = c->b_depoff.as<int64_t>(); ts.dep_idx = c->b_depidx.as<int32_t>(); }
-  int rc = upload_tasks(c, &ts, distros, Cols::kResident, En > 0 ? edge_off.data() : nullptr);
-  if (rc != EVG_OK) { c->have_tasks = false; return rc; }
-  return EVG_OK;
+  // ---- 4. the shadow set becomes the resident one
+  return install_composed(c, Tn, En, edge_off.data(), distros);
 }
 
 // --------------------------------------------------------------------------
@@ -2753,6 +2782,442 @@ int evg_edit_tasks(evg_ctx* c, const evg_task_edit* ed, const evg_distro_table* 
     CK(cudaStreamSynchronize(s));
   }
   c->editable = true;
+  return EVG_OK;
+}
+
+// --------------------------------------------------------------------------
+// evg_plan_aliases: every distro's alias queue built on the device from the tick's schedulable tasks, each staged once
+// --------------------------------------------------------------------------
+// A (queue, task) pair is the 64-bit key distro << 32 | source row: sorted, the keys list every alias queue in
+// ascending source row, and a queue's rows are found by binary search.
+struct AlView {
+  int64_t n;
+  int32_t D, n_names, n_groups, n_versions;
+  const uint8_t* sched;
+  const int32_t* tgmax;
+  const int32_t* primary;
+  const int64_t* soff;
+  const int32_t* sidx;
+  const int64_t* doff;
+  const int32_t* didx;
+};
+// The distinct alias queues row t joins (FindHostSchedulableForAlias, model/task/task.go:3371-3386): their keys go to
+// out[0 ..] unless out is NULL; returns how many.  A destination counts once: the (name, destination) entries before it
+// are searched again rather than kept in a local array, which a long SecondaryDistros could overflow.  *err bit 0: a
+// name index out of range.
+__device__ int64_t al_dests(const AlView& v, int64_t t, uint64_t* __restrict__ out, int* err) {
+  constexpr uint32_t kBase = EVG_SQ_ACTIVATED | EVG_SQ_UNDISPATCHED | EVG_SQ_PRIORITY_OK | EVG_SQ_HOST_PLATFORM;  // db.go:671-689
+  const uint32_t sq = v.sched[t];
+  if ((sq & kBase) != kBase || ((sq & EVG_SQ_UNATTAINABLE) && !(sq & EVG_SQ_OVERRIDE_DEPS))) return 0;
+  if (v.tgmax[t] == 1) return 0;  // TaskGroupMaxHosts != 1, the raw field (task.go:3382)
+  const int64_t j0 = v.soff[t], j1 = v.soff[t + 1];
+  int64_t n = 0;
+  for (int64_t j = j0; j < j1; j++) {
+    const int32_t name = v.sidx[j];
+    if (name == -1) continue;  // a name no distro has
+    if (name < 0 || name >= v.n_names) { if (err) atomicOr(err, 1); continue; }
+    for (int64_t k = v.doff[name]; k < v.doff[name + 1]; k++) {
+      const int32_t e = v.didx[k];
+      bool seen = false;
+      for (int64_t j2 = j0; j2 <= j && !seen; j2++) {
+        const int32_t nm = v.sidx[j2];
+        if (nm < 0 || nm >= v.n_names) continue;
+        const int64_t k_end = j2 < j ? v.doff[nm + 1] : k;
+        for (int64_t k2 = v.doff[nm]; k2 < k_end && !seen; k2++) seen = v.didx[k2] == e;
+      }
+      if (seen) continue;
+      if (out) out[n] = (uint64_t(uint32_t(e)) << 32) | uint64_t(t);
+      n++;
+    }
+  }
+  return n;
+}
+// Per source row: its pair count, and the range check of the ids it carries (err bit 0).
+__global__ void __launch_bounds__(256) k_al_count(AlView v, DTasks S, int32_t* __restrict__ cnt, int* err) {
+  const int64_t t = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (t >= v.n) return;
+  const int32_t g = S.gid[t], ver = S.vid[t], p = v.primary[t];
+  if (g < -1 || g >= v.n_groups || ver < 0 || ver >= v.n_versions || p < -1 || p >= v.D) atomicOr(err, 1);
+  cnt[t] = int32_t(al_dests(v, t, nullptr, err));
+}
+// Per source row: its pairs at poff[t], so that the key array is in source-row order.
+__global__ void __launch_bounds__(256) k_al_pairs(AlView v, const int64_t* __restrict__ poff, uint64_t* __restrict__ keys) {
+  const int64_t t = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (t >= v.n) return;
+  al_dests(v, t, keys + poff[t], nullptr);
+}
+// Stable LSD radix sort of the keys by the distro bits, 8 bits a pass, 2048 keys a block: the keys start in source-row
+// order, so sorting by distro alone leaves every queue in source-row order.
+constexpr int kAlTile = 2048;
+// counters of digit b of tile k at hist[b * n_tiles + k] (digit-major: their exclusive scan is every tile's run start)
+__global__ void __launch_bounds__(256) k_al_hist(const uint64_t* __restrict__ keys, int64_t n, int shift, int32_t* __restrict__ hist,
+                                                 int64_t n_tiles) {
+  __shared__ uint32_t h[256];
+  h[threadIdx.x] = 0;
+  __syncthreads();
+  const int64_t t0 = int64_t(blockIdx.x) * kAlTile;
+  for (int k = threadIdx.x; k < kAlTile; k += 256)
+    if (t0 + k < n) atomicAdd(&h[uint32_t(keys[t0 + k] >> shift) & 255u], 1u);
+  __syncthreads();
+  hist[int64_t(threadIdx.x) * n_tiles + blockIdx.x] = int32_t(h[threadIdx.x]);
+}
+// The tile in chunks of 256 keys, in order: a key's place is its digit's run start + the keys of that digit in the
+// earlier chunks (base) + those of the earlier warps in this chunk (wcnt) + those of the earlier lanes (MATCH.ANY).
+__global__ void __launch_bounds__(256) k_al_scatter(const uint64_t* __restrict__ in, uint64_t* __restrict__ out, int64_t n, int shift,
+                                                    const int64_t* __restrict__ off, int64_t n_tiles) {
+  __shared__ uint32_t base[256];
+  __shared__ uint32_t wcnt[8][256];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  base[tid] = 0;
+  for (int w = 0; w < 8; w++) wcnt[w][tid] = 0;
+  __syncthreads();
+  const int64_t t0 = int64_t(blockIdx.x) * kAlTile;
+  for (int c0 = 0; c0 < kAlTile; c0 += 256) {
+    const int64_t i = t0 + c0 + tid;
+    const bool ok = i < n;
+    const uint64_t key = ok ? in[i] : 0;
+    const uint32_t dg = ok ? (uint32_t(key >> shift) & 255u) : 256u;
+    const uint32_t peers = __match_any_sync(0xffffffffu, dg);
+    const uint32_t rank = __popc(peers & ((1u << lane) - 1u));
+    if (ok && rank == 0) wcnt[warp][dg] = __popc(peers);
+    __syncthreads();
+    if (ok) {
+      uint32_t r = base[dg] + rank;
+      for (int w = 0; w < warp; w++) r += wcnt[w][dg];
+      out[off[int64_t(dg) * n_tiles + blockIdx.x] + r] = key;
+    }
+    __syncthreads();
+    uint32_t sum = 0;
+    for (int w = 0; w < 8; w++) { sum += wcnt[w][tid]; wcnt[w][tid] = 0; }
+    base[tid] += sum;
+    __syncthreads();
+  }
+}
+// qoff[e] = first pair of distro e (e = 0 .. D; qoff[D] = n): the alias queues' task_off
+__global__ void __launch_bounds__(256) k_al_qoff(const uint64_t* __restrict__ keys, int64_t n, int32_t D, int64_t* __restrict__ qoff) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e > D) return;
+  const uint64_t want = uint64_t(e) << 32;
+  int64_t lo = 0, hi = n;
+  while (lo < hi) {
+    const int64_t mid = (lo + hi) >> 1;
+    if (keys[mid] < want) lo = mid + 1; else hi = mid;
+  }
+  qoff[e] = lo;
+}
+constexpr uint64_t kAlEmpty = ~uint64_t(0);
+// Open-addressing slot of `key` in (hk, hv), inserted if new; hv[slot] becomes the smallest pair index that carries it.
+__device__ __forceinline__ int64_t al_insert(uint64_t* hk, uint32_t* hv, uint64_t mask, uint64_t key, uint32_t i) {
+  uint64_t h = key * 0x9E3779B97F4A7C15ull;
+  h ^= h >> 29;
+  for (uint64_t slot = h & mask;; slot = (slot + 1) & mask) {
+    const unsigned long long prev = atomicCAS(reinterpret_cast<unsigned long long*>(hk + slot), (unsigned long long)kAlEmpty,
+                                              (unsigned long long)key);
+    if (prev == kAlEmpty || prev == key) {
+      atomicMin(hv + slot, i);
+      return int64_t(slot);
+    }
+  }
+}
+// Per pair: the (queue, task group) and (queue, version) it belongs to, keyed queue << 32 | global id (bit 63 marks a
+// version), and the first pair of each.
+__global__ void __launch_bounds__(256) k_al_first(int64_t n, const uint64_t* __restrict__ keys, DTasks S, uint64_t* hk, uint32_t* hv,
+                                                  uint64_t mask, int64_t* __restrict__ gslot, int64_t* __restrict__ vslot) {
+  const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint64_t k = keys[i], q = k >> 32 << 32;
+  const uint32_t t = uint32_t(k);
+  const int32_t g = S.gid[t];
+  gslot[i] = g >= 0 ? al_insert(hk, hv, mask, q | uint32_t(g), uint32_t(i)) : -1;
+  vslot[i] = al_insert(hk, hv, mask, (uint64_t(1) << 63) | q | uint32_t(S.vid[t]), uint32_t(i));
+}
+// first-appearance flags: their exclusive scans number each queue's groups and versions in first-appearance order
+__global__ void __launch_bounds__(256) k_al_flag(int64_t n, const int64_t* __restrict__ gslot, const int64_t* __restrict__ vslot,
+                                                 const uint32_t* __restrict__ hv, int32_t* __restrict__ fg, int32_t* __restrict__ fv) {
+  const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  fg[i] = gslot[i] >= 0 && hv[gslot[i]] == uint32_t(i);
+  fv[i] = hv[vslot[i]] == uint32_t(i);
+}
+struct AlIds {
+  const int64_t *qoff, *gslot, *vslot, *pg, *pv;
+  const uint32_t* hv;
+};
+// Pair i = (queue e, source row t) becomes row i of the composed table: the source row's columns with the queue's
+// group and version ids and EVG_TF_OTHER_DISTRO for e; its alias map entry, and the group slot of a group's first pair.
+__global__ void __launch_bounds__(256) k_al_gather(int64_t n, const uint64_t* __restrict__ keys, AlIds a, DTasks S,
+                                                   const int32_t* __restrict__ primary, const int32_t* __restrict__ gmax, EdDst o,
+                                                   int32_t* __restrict__ srow, int32_t* __restrict__ gout, int32_t* __restrict__ gsrc) {
+  const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint64_t k = keys[i];
+  const int64_t t = uint32_t(k);
+  const int e = int(k >> 32);
+  const int64_t q0 = a.qoff[e];
+  int32_t g = S.gid[t];
+  if (g >= 0) {
+    const int64_t slot = a.pg[i];
+    if (a.hv[a.gslot[i]] == uint32_t(i)) { gout[slot] = gmax[g]; gsrc[slot] = g; }
+    g = int32_t(a.pg[a.hv[a.gslot[i]]] - a.pg[q0]);
+  }
+  o.priority[i] = S.priority[t]; o.numdep[i] = S.numdep[t]; o.tgo[i] = S.tgo[t]; o.gid[i] = g;
+  o.vid[i] = int32_t(a.pv[a.hv[a.vslot[i]]] - a.pv[q0]);
+  o.flags[i] = (S.flags[t] & ~EVG_TF_OTHER_DISTRO) | (primary[t] != e ? EVG_TF_OTHER_DISTRO : 0u);  // scheduler.go:75
+  o.expected[i] = S.expected[t]; o.qbasis[i] = S.qbasis[t]; o.wbasis[i] = S.wbasis[t];
+  srow[i] = int32_t(t);
+}
+// Edges of pair i = (e, t): t's source edges t -> u with (e, u) a pair, re-indexed to u's place in e, in DependsOn order
+// (duplicates kept).  o_dep_idx == NULL: count them, raising *err bit 1 for a dep_idx outside the table.
+__device__ int64_t al_edges(int64_t i, const uint64_t* __restrict__ keys, const int64_t* __restrict__ qoff, const DTasks& S,
+                            const int64_t* __restrict__ o_dep_off, int32_t* __restrict__ o_dep_idx, int* err) {
+  const uint64_t k = keys[i];
+  const int64_t t = uint32_t(k);
+  const uint64_t q = k >> 32 << 32;
+  const int64_t a = qoff[k >> 32], b = qoff[(k >> 32) + 1];
+  int64_t w = o_dep_off ? o_dep_off[i] : 0, n = 0;
+  for (int64_t j = S.dep_off[t]; j < S.dep_off[t + 1]; j++) {
+    const int32_t x = S.dep_idx[j];
+    if (x < 0 || x >= S.n) { if (err) atomicOr(err, 2); continue; }
+    const uint64_t want = q | uint32_t(x);
+    int64_t lo = a, hi = b;
+    while (lo < hi) {
+      const int64_t mid = (lo + hi) >> 1;
+      if (keys[mid] < want) lo = mid + 1; else hi = mid;
+    }
+    if (lo == b || keys[lo] != want) continue;
+    if (o_dep_idx) o_dep_idx[w + n] = int32_t(lo - a);
+    n++;
+  }
+  return n;
+}
+__global__ void __launch_bounds__(256) k_al_edge_count(int64_t n, const uint64_t* __restrict__ keys, const int64_t* __restrict__ qoff,
+                                                       DTasks S, int32_t* __restrict__ cnt, int* err) {
+  const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  cnt[i] = int32_t(al_edges(i, keys, qoff, S, nullptr, nullptr, err));
+}
+__global__ void __launch_bounds__(256) k_al_edge_write(int64_t n, const uint64_t* __restrict__ keys, const int64_t* __restrict__ qoff,
+                                                       DTasks S, const int64_t* __restrict__ o_dep_off, int32_t* __restrict__ o_dep_idx) {
+  const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  al_edges(i, keys, qoff, S, o_dep_off, o_dep_idx, nullptr);
+}
+
+int evg_plan_aliases(evg_ctx* c, const evg_alias_in* in, const evg_distro_cfg* cfg, int32_t D, int64_t now_ns, evg_alias_out* out) {
+  if (!c) return fail(EVG_ERR_INVALID, "null context");
+  LOCK(c);
+  if (!in || !out || !in->deps) return fail(EVG_ERR_INVALID, "evg_plan_aliases: null argument");
+  // ---- every check the host can make, before anything resident changes
+  const evg_task_soa* t = &in->tasks;
+  const evg_deps_in* dp = in->deps;
+  const int64_t T = t->n_tasks, E = t->n_edges;
+  const int32_t NG = in->n_groups, NV = in->n_versions, NN = in->n_names;
+  if (T < 0 || E < 0 || D < 0 || NG < 0 || NV < 0 || NN < 0 || dp->n_deps < 0 || dp->n_ext < 0)
+    return fail(EVG_ERR_INVALID, "evg_plan_aliases: negative sizes");
+  if (dp->n_tasks != T) return fail(EVG_ERR_INVALID, "evg_plan_aliases: deps covers %lld rows, the table %lld", (long long)dp->n_tasks, (long long)T);
+  if (T > (int64_t(1) << 31) - 2) return fail(EVG_ERR_INVALID, "evg_plan_aliases: %lld rows exceed 2^31-2", (long long)T);
+  if (!out->task_off || !out->group_off || (D > 0 && (!out->n_versions || !cfg))) return fail(EVG_ERR_INVALID, "evg_plan_aliases: null cfg / output");
+  if (!in->secondary_off || !in->dest_off || (NG > 0 && !in->group_max_hosts)) return fail(EVG_ERR_INVALID, "evg_plan_aliases: null offsets / group_max_hosts");
+  if (T > 0 && (!t->priority || !t->expected_ns || !t->queue_basis_ns || !t->wait_basis_ns || !t->num_dependents ||
+                !t->task_group_order || !t->group_id || !t->version_id || !t->flags || !in->sched || !in->task_group_max_hosts ||
+                !in->primary || !dp->dep_off || !dp->task_state || !dp->task_pre))
+    return fail(EVG_ERR_INVALID, "evg_plan_aliases: null task column");
+  if (E > 0 && (!t->dep_off || !t->dep_idx)) return fail(EVG_ERR_INVALID, "evg_plan_aliases: null dep_off / dep_idx");
+  if (dp->n_deps > 0 && (!dp->dep_kind || !dp->dep_ref || !dp->dep_want)) return fail(EVG_ERR_INVALID, "evg_plan_aliases: null dependency arrays");
+  if (dp->n_ext > 0 && !dp->ext_state) return fail(EVG_ERR_INVALID, "evg_plan_aliases: null ext_state");
+  const int64_t NS = in->secondary_off[T], ND = in->dest_off[NN];
+  int rc = check_csr(csr_bad_row(in->secondary_off, T, NS), T, "evg_plan_aliases: secondary_off");
+  if (rc == EVG_OK) rc = check_csr(csr_bad_row(in->dest_off, NN, ND), NN, "evg_plan_aliases: dest_off");
+  if (rc == EVG_OK && E > 0) rc = check_csr(csr_bad_row(t->dep_off, T, E), T, "evg_plan_aliases: dep_off");
+  if (rc == EVG_OK && T > 0) rc = check_csr(csr_bad_row(dp->dep_off, T, dp->n_deps), T, "evg_plan_aliases: deps->dep_off");
+  if (rc != EVG_OK) return rc;
+  if (NS > 0 && !in->secondary_idx) return fail(EVG_ERR_INVALID, "evg_plan_aliases: null secondary_idx");
+  if (ND > 0 && !in->dest_idx) return fail(EVG_ERR_INVALID, "evg_plan_aliases: null dest_idx");
+  for (int64_t k = 0; k < ND; k++)
+    if (in->dest_idx[k] < 0 || in->dest_idx[k] >= D)
+      return fail(EVG_ERR_INVALID, "evg_plan_aliases: dest_idx[%lld] = %d is outside [0, %d)", (long long)k, in->dest_idx[k], D);
+  // ---- from here the previous tick is gone: the dependency state and the resident columns are replaced
+  CK(cudaSetDevice(c->device));
+  cudaStream_t s = c->stream;
+  auto& a = c->al;
+  c->have_tasks = false;
+  c->launches = 0;
+  CK(c->b_err.ensure(sizeof(int) * 4));
+  CK(cudaMemsetAsync(c->b_err.p, 0, sizeof(int) * 4, s));
+  CK(a.err.ensure(sizeof(int)));
+  CK(cudaMemsetAsync(a.err.p, 0, sizeof(int), s));
+  int* err = a.err.as<int>();
+  // 1. the source table, Task.DependenciesMet with its stamps over the source rows, once
+  rc = a.src.stage(t, T, s);
+  if (rc != EVG_OK) return rc;
+  DTasks S = a.src.view(T);
+  UP(s, a.dep_off, E > 0 ? t->dep_off : nullptr, E > 0 ? T + 1 : 0, int64_t);
+  UP(s, a.dep_idx, t->dep_idx, E, int32_t);
+  S.n_edges = E; S.dep_off = a.dep_off.as<int64_t>(); S.dep_idx = a.dep_idx.as<int32_t>();
+  UP(s, a.gmax, in->group_max_hosts, NG, int32_t);
+  UP(s, a.sched, in->sched, T, uint8_t);
+  UP(s, a.tgmax, in->task_group_max_hosts, T, int32_t);
+  UP(s, a.primary, in->primary, T, int32_t);
+  UP(s, a.soff, in->secondary_off, T + 1, int64_t);
+  UP(s, a.sidx, in->secondary_idx, NS, int32_t);
+  UP(s, a.doff, in->dest_off, NN + 1, int64_t);
+  UP(s, a.didx, in->dest_idx, ND, int32_t);
+  if (T > 0) {
+    rc = deps_to_device(c, dp, 0, in->dep_finished_ns, now_ns, /*want_stamp=*/true);
+    if (rc != EVG_OK) return rc;
+    k_apply_deps<<<grid_for(T, 256), 256, 0, s>>>(T, c->deps.met.as<uint8_t>(), c->deps.stamp.as<int64_t>(), a.src.flags.as<uint32_t>(),
+                                                  a.src.wb.as<int64_t>());
+    c->launches++;
+  }
+  // 2. per row: eligibility and its distinct alias queues; the pair offsets (one value crosses to the host)
+  AlView v;
+  v.n = T; v.D = D; v.n_names = NN; v.n_groups = NG; v.n_versions = NV;
+  v.sched = a.sched.as<uint8_t>(); v.tgmax = a.tgmax.as<int32_t>(); v.primary = a.primary.as<int32_t>();
+  v.soff = a.soff.as<int64_t>(); v.sidx = a.sidx.as<int32_t>(); v.doff = a.doff.as<int64_t>(); v.didx = a.didx.as<int32_t>();
+  CK(a.cnt.ensure(sizeof(int32_t) * size_t(T + 1)));
+  CK(a.poff.ensure(sizeof(int64_t) * size_t(T + 1)));
+  CK(c->ed.scan_sum.ensure(sizeof(int64_t) * size_t((T + 1023) / 1024 + 1)));
+  int64_t P = 0;
+  int bad = 0;
+  if (T > 0) {
+    k_al_count<<<grid_for(T, 256), 256, 0, s>>>(v, S, a.cnt.as<int32_t>(), err);
+    c->launches++;
+    scan_counts(c, a.cnt.as<int32_t>(), T, a.poff.as<int64_t>(), c->ed.scan_sum.as<int64_t>());
+    CK(cudaMemcpyAsync(&P, a.poff.as<int64_t>() + T, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+  }
+  CK(cudaMemcpyAsync(&bad, err, sizeof(int), cudaMemcpyDeviceToHost, s));
+  int bad_ref = 0;
+  CK(cudaMemcpyAsync(&bad_ref, c->b_err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  if (bad_ref) return fail(EVG_ERR_INVALID, "evg_plan_aliases: a dep_ref is out of range");
+  if (bad) return fail(EVG_ERR_INVALID, "evg_plan_aliases: a secondary_idx, primary, group_id or version_id is out of range");
+  if (P > (int64_t(1) << 31) - 2) return fail(EVG_ERR_INVALID, "evg_plan_aliases: %lld (queue, task) pairs exceed 2^31-2", (long long)P);
+  // 3. the pairs, in source-row order, sorted by queue
+  for (int k = 0; k < 2; k++) CK(a.keys[k].ensure(sizeof(uint64_t) * size_t(P + 1)));
+  int cur = 0;
+  if (P > 0) {
+    k_al_pairs<<<grid_for(T, 256), 256, 0, s>>>(v, a.poff.as<int64_t>(), a.keys[0].as<uint64_t>());
+    c->launches++;
+    int bits = 0;
+    while (bits < 31 && (int64_t(1) << bits) < D) bits++;
+    const int64_t n_tiles = (P + kAlTile - 1) / kAlTile, nh = 256 * n_tiles;
+    if (bits > 0) {
+      CK(a.hist.ensure(sizeof(int32_t) * size_t(nh)));
+      CK(a.hoff.ensure(sizeof(int64_t) * size_t(nh + 1)));
+      CK(c->ed.scan_sum.ensure(sizeof(int64_t) * size_t((nh + 1023) / 1024 + 1)));
+    }
+    for (int shift = 32; shift < 32 + bits; shift += 8, cur ^= 1) {
+      k_al_hist<<<unsigned(n_tiles), 256, 0, s>>>(a.keys[cur].as<uint64_t>(), P, shift, a.hist.as<int32_t>(), n_tiles);
+      scan_counts(c, a.hist.as<int32_t>(), nh, a.hoff.as<int64_t>(), c->ed.scan_sum.as<int64_t>());
+      k_al_scatter<<<unsigned(n_tiles), 256, 0, s>>>(a.keys[cur].as<uint64_t>(), a.keys[cur ^ 1].as<uint64_t>(), P, shift,
+                                                     a.hoff.as<int64_t>(), n_tiles);
+      c->launches += 2;
+    }
+  }
+  const uint64_t* keys = a.keys[cur].as<uint64_t>();
+  CK(a.qoff.ensure(sizeof(int64_t) * size_t(D + 1)));
+  k_al_qoff<<<grid_for(D + 1, 256), 256, 0, s>>>(keys, P, D, a.qoff.as<int64_t>());
+  c->launches++;
+  // 4. per queue, dense group and version ids in first-appearance order
+  uint64_t cap = 64;
+  while (cap < 4 * uint64_t(P)) cap <<= 1;  // at most 2P keys: load factor <= 1/2
+  for (DevBuf* b : {&a.pg, &a.pv}) CK(b->ensure(sizeof(int64_t) * size_t(P + 1)));
+  for (DevBuf* b : {&a.gslot, &a.vslot}) CK(b->ensure(sizeof(int64_t) * size_t(P + 1)));
+  for (DevBuf* b : {&a.fg, &a.fv, &a.srow, &a.gout, &a.gsrc}) CK(b->ensure(sizeof(int32_t) * size_t(P + 1)));
+  CK(cudaMemsetAsync(a.pg.p, 0, sizeof(int64_t), s));  // P == 0: the scans do not run
+  CK(cudaMemsetAsync(a.pv.p, 0, sizeof(int64_t), s));
+  if (P > 0) {
+    CK(a.hk.ensure(sizeof(uint64_t) * cap));
+    CK(a.hv.ensure(sizeof(uint32_t) * cap));
+    CK(cudaMemsetAsync(a.hk.p, 0xFF, sizeof(uint64_t) * cap, s));
+    CK(cudaMemsetAsync(a.hv.p, 0xFF, sizeof(uint32_t) * cap, s));
+    k_al_first<<<grid_for(P, 256), 256, 0, s>>>(P, keys, S, a.hk.as<uint64_t>(), a.hv.as<uint32_t>(), cap - 1, a.gslot.as<int64_t>(),
+                                                a.vslot.as<int64_t>());
+    k_al_flag<<<grid_for(P, 256), 256, 0, s>>>(P, a.gslot.as<int64_t>(), a.vslot.as<int64_t>(), a.hv.as<uint32_t>(), a.fg.as<int32_t>(),
+                                               a.fv.as<int32_t>());
+    c->launches += 2;
+    CK(c->ed.scan_sum.ensure(sizeof(int64_t) * size_t((P + 1023) / 1024 + 1)));
+    scan_counts(c, a.fg.as<int32_t>(), P, a.pg.as<int64_t>(), c->ed.scan_sum.as<int64_t>());
+    scan_counts(c, a.fv.as<int32_t>(), P, a.pv.as<int64_t>(), c->ed.scan_sum.as<int64_t>());
+  }
+  // 5. the nine columns into the shadow set
+  EdDst o;
+  rc = shadow_cols(c, P, &o);
+  if (rc != EVG_OK) return rc;
+  AlIds ids;
+  ids.qoff = a.qoff.as<int64_t>(); ids.gslot = a.gslot.as<int64_t>(); ids.vslot = a.vslot.as<int64_t>();
+  ids.pg = a.pg.as<int64_t>(); ids.pv = a.pv.as<int64_t>(); ids.hv = a.hv.as<uint32_t>();
+  if (P > 0) {
+    k_al_gather<<<grid_for(P, 256), 256, 0, s>>>(P, keys, ids, S, a.primary.as<int32_t>(), a.gmax.as<int32_t>(), o, a.srow.as<int32_t>(),
+                                                 a.gout.as<int32_t>(), a.gsrc.as<int32_t>());
+    c->launches++;
+  }
+  // 6. edges: count, scan; the queue, group, version and edge offsets of every distro cross to the host (one sync)
+  auto& e = c->ed;
+  const bool edges = P > 0 && E > 0;
+  CK(a.samp.ensure(sizeof(int64_t) * 3 * size_t(D + 1)));
+  int64_t* samp = a.samp.as<int64_t>();
+  k_gather_i64<<<grid_for(D + 1, 256), 256, 0, s>>>(a.pg.as<int64_t>(), a.qoff.as<int64_t>(), samp, D + 1);
+  k_gather_i64<<<grid_for(D + 1, 256), 256, 0, s>>>(a.pv.as<int64_t>(), a.qoff.as<int64_t>(), samp + (D + 1), D + 1);
+  c->launches += 2;
+  if (edges) {
+    CK(e.edge_cnt.ensure(sizeof(int32_t) * size_t(P + 1)));
+    CK(e.dep_off.ensure(sizeof(int64_t) * size_t(P + 1 + kColPad)));
+    k_al_edge_count<<<grid_for(P, 256), 256, 0, s>>>(P, keys, a.qoff.as<int64_t>(), S, e.edge_cnt.as<int32_t>(), err);
+    scan_counts(c, e.edge_cnt.as<int32_t>(), P, e.dep_off.as<int64_t>(), c->ed.scan_sum.as<int64_t>());
+    k_gather_i64<<<grid_for(D + 1, 256), 256, 0, s>>>(e.dep_off.as<int64_t>(), a.qoff.as<int64_t>(), samp + 2 * (D + 1), D + 1);
+    c->launches += 2;
+  }
+  std::vector<int64_t> h(3 * size_t(D + 1), 0);
+  CK(cudaMemcpyAsync(out->task_off, a.qoff.p, sizeof(int64_t) * size_t(D + 1), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(h.data(), samp, sizeof(int64_t) * size_t(edges ? 3 : 2) * size_t(D + 1), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(&bad, err, sizeof(int), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  if (bad) return fail(EVG_ERR_INVALID, "evg_plan_aliases: a dep_idx is outside the table");
+  const int64_t* vs = h.data() + (D + 1);
+  const int64_t* edge_off = h.data() + 2 * (D + 1);
+  for (int32_t d = 0; d < D; d++) {
+    const int64_t len = out->task_off[d + 1] - out->task_off[d];
+    if (len > kMaxTasksPerDistro) return fail(EVG_ERR_INVALID, "evg_plan_aliases: the alias queue of distro %d holds %lld tasks (max %lld)", d, (long long)len, (long long)kMaxTasksPerDistro);
+    out->group_off[d] = h[size_t(d)];
+    out->n_versions[d] = int32_t(vs[d + 1] - vs[d]);
+  }
+  out->group_off[D] = h[size_t(D)];
+  const int64_t G = h[size_t(D)], En = edges ? edge_off[D] : 0;
+  // 7. the group slots' max hosts (O(alias groups) values) and the edges; then the composed table becomes the tick
+  std::vector<int32_t> gmax(size_t(G) + 1);
+  if (G > 0) CK(cudaMemcpyAsync(gmax.data(), a.gout.p, sizeof(int32_t) * size_t(G), cudaMemcpyDeviceToHost, s));
+  if (edges) {
+    CK(e.dep_idx.ensure(sizeof(int32_t) * size_t(En + kColPad)));
+    if (En > 0) {
+      k_al_edge_write<<<grid_for(P, 256), 256, 0, s>>>(P, keys, a.qoff.as<int64_t>(), S, e.dep_off.as<int64_t>(), e.dep_idx.as<int32_t>());
+      c->launches++;
+    }
+  }
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  std::vector<evg_distro_cfg> cf(cfg, cfg + D);
+  for (int32_t d = 0; d < D; d++) cf[size_t(d)].n_versions = out->n_versions[d];
+  evg_distro_table dt;
+  memset(&dt, 0, sizeof(dt));
+  dt.n_distros = D; dt.task_off = out->task_off; dt.group_off = out->group_off; dt.cfg = cf.data(); dt.group_max_hosts = gmax.data();
+  rc = install_composed(c, P, En, edge_off, &dt);
+  if (rc != EVG_OK) return rc;
+  c->editable = true;
+  c->alias_map = true;
+  return EVG_OK;
+}
+
+int evg_download_alias_map(evg_ctx* c, int32_t* source_row, int32_t* group_source) {
+  if (!c) return fail(EVG_ERR_INVALID, "null context");
+  LOCK(c);
+  if (!c->have_tasks || !c->alias_map) return fail(EVG_ERR_STATE, "evg_download_alias_map: the resident tick was not built by evg_plan_aliases");
+  CK(cudaSetDevice(c->device));
+  if (source_row && c->T) CK(cudaMemcpyAsync(source_row, c->al.srow.p, sizeof(int32_t) * size_t(c->T), cudaMemcpyDeviceToHost, c->stream));
+  if (group_source && c->G) CK(cudaMemcpyAsync(group_source, c->al.gsrc.p, sizeof(int32_t) * size_t(c->G), cudaMemcpyDeviceToHost, c->stream));
+  CK(cudaStreamSynchronize(c->stream));
   return EVG_OK;
 }
 

@@ -67,6 +67,9 @@ PROVIDER_MOCK = "mock"
 PROVIDER_SPAWNABLE = (PROVIDER_EC2_ONDEMAND, PROVIDER_EC2_FLEET, PROVIDER_MOCK, PROVIDER_DOCKER)  # globals.go:723-728
 # model/task_queue.go:216-219
 PERSISTED_QUEUE_CAP = 10000
+# model/task_queue.go:17-20: the collections TaskQueue.Save writes to
+TASK_QUEUES_COLLECTION = "task_queues"
+TASK_SECONDARY_QUEUES_COLLECTION = "task_alias_queues"
 DISABLED_TASK_PRIORITY = -1  # globals.go:187
 
 
@@ -125,6 +128,7 @@ class Task:
     dependencies_met_time: int = ZERO_TIME
     start_time: int = ZERO_TIME
     distro_id: str = ""
+    secondary_distros: List[str] = field(default_factory=list)  # Task.SecondaryDistros: the alias queues it may join
     status: str = TASK_UNDISPATCHED
     # finished-task history (expected_duration.go:36-55)
     finish_time: int = ZERO_TIME
@@ -224,6 +228,7 @@ class Distro:
     host_allocator_settings: HostAllocatorSettings = field(default_factory=HostAllocatorSettings)
     dispatcher_settings: DispatcherSettings = field(default_factory=lambda: DispatcherSettings(version=""))
     valid_projects: List[str] = field(default_factory=list)
+    aliases: List[str] = field(default_factory=list)  # Distro.Aliases (FindApplicableDistroIDs, model/distro/aliases.go:14-27)
 
     def max_duration_per_host(self) -> int:  # distro.go:422-432
         if self.container_pool != "":
@@ -314,6 +319,11 @@ class TaskQueue:  # model/task_queue.go:117-123
     generated_at: int = ZERO_TIME
     queue: List[TaskQueueItem] = field(default_factory=list)
     distro_queue_info: Optional["DistroQueueInfo"] = None
+
+    def collection(self) -> str:  # TaskQueue.Save routes on DistroQueueInfo.GetQueueCollection (model/task_queue.go:108-115)
+        if self.distro_queue_info is not None and self.distro_queue_info.secondary_queue:
+            return TASK_SECONDARY_QUEUES_COLLECTION
+        return TASK_QUEUES_COLLECTION
 
 
 @dataclass

@@ -303,6 +303,30 @@ class Engine:
         self._has_hosts = hosts is not None
         return runnable, count
 
+    def plan_aliases(self, table: "S.AliasTable", cfg: np.ndarray, now: int):
+        """evg_plan_aliases: every distro's alias queue built on the device from the tick's schedulable tasks, each
+        given once; the context then holds the alias queues as its tick (run / download, planner only).
+        -> (task_off, group_off, n_versions) of the alias queues."""
+        D = int(cfg.shape[0])
+        cfg = np.ascontiguousarray(cfg, dtype=L.DISTRO_CFG_DTYPE)
+        task_off, group_off = np.zeros(D + 1, np.int64), np.zeros(D + 1, np.int64)
+        n_versions = np.zeros(max(D, 1), np.int32)
+        st, keep = table.normalize().struct()
+        out = L.AliasOutStruct(L.ptr(task_off), L.ptr(group_off), L.ptr(n_versions))
+        L.check(self.lib.evg_plan_aliases(self.ctx, C.byref(st), L.ptr(cfg) if D else None, D, int(now), C.byref(out)))
+        del keep
+        self._n_tasks, self._n_distros, self._n_groups = int(task_off[D]), D, int(group_off[D])
+        self._has_hosts = False
+        return task_off, group_off, n_versions[:D]
+
+    def download_alias_map(self):
+        """evg_download_alias_map: (source row of every resident row, global group id of every group slot)."""
+        src = self._out("alias_source_row", self._n_tasks, np.int32)
+        gsrc = self._out("alias_group_source", self._n_groups, np.int32)
+        L.check(self.lib.evg_download_alias_map(self.ctx, L.ptr(src) if self._n_tasks else None,
+                                                L.ptr(gsrc) if self._n_groups else None))
+        return src, gsrc
+
     def expected_durations_batch(self, rows: "S.DurationRows") -> np.ndarray:
         """{$avg, $stdDevPop} of TimeTaken per key (evg_expected_durations_batch) -> DURATION_STAT_DTYPE[n_keys]."""
         out = self._out("duration_stats", rows.n_keys, L.DURATION_STAT_DTYPE)
@@ -728,6 +752,98 @@ def plan_candidates(batch: Sequence[Tuple[M.Distro, List[M.Task]]], project_refs
         a_new += len(kept)
         ga, gb = int(dtable.group_off[d]), int(dtable.group_off[d + 1])
         out.append((ranked, _queue_info_from_rows(po.info[d], po.group_info[ga:gb], keys[d].group_names)))
+    return out
+
+
+def find_host_schedulable_for_alias(distro_id: str, tasks: Sequence[M.Task], distros: Sequence[M.Distro]) -> List[M.Task]:
+    """task.FindHostSchedulableForAlias (model/task/task.go:3371-3386) over the tasks collection `tasks`, in its order:
+    schedulableHostTasksQuery (model/task/db.go:671-689), TaskGroupMaxHosts != 1, and some SecondaryDistros name in
+    FindApplicableDistroIDs(distro_id) = {distro_id} U Aliases (model/distro/aliases.go:14-27), looked up in `distros`."""
+    d = next((x for x in distros if x.id == distro_id), None)
+    if d is None:
+        raise LookupError(f"error finding distro '{distro_id}'")  # aliases.go:20-22
+    applicable = {d.id, *d.aliases}
+    out = []
+    for t in tasks:
+        if not (t.activated and t.status == M.TASK_UNDISPATCHED and t.priority > M.DISABLED_TASK_PRIORITY and
+                t.execution_platform in ("", "host")):
+            continue
+        if t.unattainable_dependency and not t.override_dependencies:
+            continue
+        if t.task_group_max_hosts == 1:  # single-host task groups stay out of alias queues (task.go:3379-3382)
+            continue
+        if any(name in applicable for name in t.secondary_distros):
+            out.append(t)
+    return out
+
+
+def _plan_aliases(eng: Engine, distros, tasks, now: int, dependency_db):
+    """evg_plan_aliases over the tick -> (task_off, group_off, source row of every resident row, group names per slot)."""
+    table, cfg, keys = S.marshal_aliases(distros, tasks, now, dependency_db)
+    task_off, group_off, _ = eng.plan_aliases(table, cfg, now)
+    src, gsrc = (a.copy() for a in eng.download_alias_map())
+    return task_off, group_off, src, [keys.group_names[int(g)] for g in gsrc]
+
+
+def plan_alias_queues(distros: Sequence[M.Distro], tasks: Sequence[M.Task], now: int, *, engine: Optional[Engine] = None,
+                      dependency_db: Optional[Dict[str, M.Task]] = None, breakdown: bool = False,
+                      started_at: int = M.ZERO_TIME):
+    """distroAliasSchedulerJob.Run for every distro at once, without Mongo (units/scheduler_alias.go:55-117): the tick's
+    schedulable `tasks` (each once) fan out to the alias queues on the device (evg_plan_aliases), which are planned
+    with IsSecondaryQueue (scheduler/scheduler.go:27-51).  Returns, per distro, (ranked [Task] with
+    SortingValueBreakdown stamped -- shallow copies: a task in several queues has one TotalValue in each --
+    DistroQueueInfo with secondary_queue and plan_created_at set)."""
+    import copy
+    eng = engine or default_engine()
+    task_off, group_off, src, names = _plan_aliases(eng, distros, tasks, now, dependency_db)
+    eng.run(now, L.EVG_OPT_BREAKDOWN if breakdown else 0)
+    po, _ = eng.download(want_breakdown=breakdown, want_alloc=False)
+    out = []
+    for d in range(len(distros)):
+        a, b = int(task_off[d]), int(task_off[d + 1])
+        ga, gb = int(group_off[d]), int(group_off[d + 1])
+        ranked = []
+        for r in range(a, b):
+            t = copy.copy(tasks[int(src[a + int(po.order[r])])])
+            if breakdown:
+                t.sorting_value_breakdown = M.SortingValueBreakdown.from_row(po.breakdown[r])
+            else:
+                t.sorting_value_breakdown = M.SortingValueBreakdown(total_value=int(po.total_value[r]))
+            ranked.append(t)
+        info = _queue_info_from_rows(po.info[d], po.group_info[ga:gb], names[ga:gb])
+        info.secondary_queue = True  # scheduler.go:44
+        info.plan_created_at = started_at
+        out.append((ranked, info))
+    return out
+
+
+def persist_alias_task_queues(distros: Sequence[M.Distro], tasks: Sequence[M.Task], now: int, *, engine: Optional[Engine] = None,
+                              dependency_db: Optional[Dict[str, M.Task]] = None, cap: int = 0) -> List[M.TaskQueue]:
+    """persist_task_queues for the alias queues: every distro's secondary TaskQueue document (TaskQueue.collection() is
+    the alias queues' collection) from the TaskQueueItem rows evg_download_queue projects on the device."""
+    eng = engine or default_engine()
+    task_off, group_off, src, names = _plan_aliases(eng, distros, tasks, now, dependency_db)
+    eng.run(now)
+    po, _ = eng.download(want_alloc=False)
+    item_off, items = eng.download_queue(cap, task_off)
+    out = []
+    for d, distro in enumerate(distros):
+        a, ga, gb = int(task_off[d]), int(group_off[d]), int(group_off[d + 1])
+        info = _queue_info_from_rows(po.info[d], po.group_info[ga:gb], names[ga:gb])
+        info.secondary_queue = True
+        queue = []
+        for row in items[int(item_off[d]):int(item_off[d + 1])]:
+            t = tasks[int(src[a + int(row["task"])])]
+            t.expected_duration = int(row["expected_ns"])
+            queue.append(M.TaskQueueItem(
+                id=t.id, display_name=t.display_name, build_variant=t.build_variant,
+                revision_order_number=t.revision_order_number, requester=t.requester, revision=t.revision, project=t.project,
+                expected_duration=int(row["expected_ns"]), priority=int(row["priority"]),
+                sorting_value_breakdown=M.SortingValueBreakdown(total_value=int(row["total_value"])), group=t.task_group,
+                group_max_hosts=t.task_group_max_hosts, group_index=int(row["group_index"]), version=t.version,
+                activated_by=t.activated_by, dependencies=[dep.task_id for dep in t.depends_on],
+                dependencies_met=bool(int(row["flags"]) & L.EVG_QI_DEPS_MET)))
+        out.append(M.TaskQueue(distro=distro.id, generated_at=now, queue=queue, distro_queue_info=info))
     return out
 
 

@@ -722,6 +722,173 @@ def marshal_runnable(batch: Sequence[tuple], project_refs: Sequence[M.ProjectRef
                          np.array(valid_idx, np.int32), np.array(fnd, np.uint8), deps)
 
 
+# ---------------------------------------------------------------------------
+# alias queues (evg_alias_in)
+# ---------------------------------------------------------------------------
+
+SQ_BASE = L.EVG_SQ_ACTIVATED | L.EVG_SQ_UNDISPATCHED | L.EVG_SQ_PRIORITY_OK | L.EVG_SQ_HOST_PLATFORM
+
+
+@dataclass
+class AliasTable:
+    """evg_alias_in: the tick's schedulable tasks, each once, and what decides the alias queues they join.
+    tasks.group_id / version_id are table-global; tasks.dep_idx are row indices; `deps` covers the same rows."""
+    tasks: TaskSoA
+    group_max_hosts: np.ndarray   # per global group
+    n_versions: int
+    sched: np.ndarray             # uint8 EVG_SQ_*
+    task_group_max_hosts: np.ndarray
+    primary: np.ndarray           # distro index of Task.DistroId, -1
+    secondary_off: np.ndarray     # CSR of Task.SecondaryDistros as name indices (-1: a name no distro has)
+    secondary_idx: np.ndarray
+    dest_off: np.ndarray          # CSR over names: the distros e with the name in {e} U e.Aliases
+    dest_idx: np.ndarray
+    deps: DepsTable
+    dep_finished: np.ndarray
+
+    @property
+    def n_tasks(self) -> int:
+        return self.tasks.n_tasks
+
+    @property
+    def n_names(self) -> int:
+        return int(self.dest_off.shape[0]) - 1
+
+    def normalize(self) -> "AliasTable":
+        self.tasks.normalize()
+        for f, dt in (("group_max_hosts", np.int32), ("sched", np.uint8), ("task_group_max_hosts", np.int32), ("primary", np.int32),
+                      ("secondary_off", np.int64), ("secondary_idx", np.int32), ("dest_off", np.int64), ("dest_idx", np.int32),
+                      ("dep_finished", np.int64)):
+            setattr(self, f, np.ascontiguousarray(getattr(self, f), dtype=dt))
+        return self
+
+    def struct(self):
+        """-> (AliasInStruct, keepalive)."""
+        s = L.AliasInStruct()
+        s.tasks = self.tasks.struct()
+        s.n_groups, s.n_versions = int(self.group_max_hosts.shape[0]), int(self.n_versions)
+        nz = lambda a: L.ptr(a) if a.shape[0] else None  # noqa: E731
+        s.group_max_hosts, s.sched, s.task_group_max_hosts, s.primary = (nz(self.group_max_hosts), nz(self.sched),
+                                                                         nz(self.task_group_max_hosts), nz(self.primary))
+        s.secondary_off, s.secondary_idx = L.ptr(self.secondary_off), nz(self.secondary_idx)
+        s.n_names = self.n_names
+        s.dest_off, s.dest_idx = L.ptr(self.dest_off), nz(self.dest_idx)
+        keep = self.deps.struct()
+        s.deps = C.pointer(keep)
+        s.dep_finished_ns = nz(self.dep_finished)
+        return s, keep
+
+
+def alias_name_table(distros: Sequence[M.Distro]):
+    """(name -> index, dest_off, dest_idx): every name some distro's applicable set {e} U e.Aliases holds
+    (FindApplicableDistroIDs, model/distro/aliases.go:14-27), and per name the distros whose set holds it."""
+    dests: Dict[str, List[int]] = {}
+    for i, d in enumerate(distros):
+        for name in [d.id] + list(d.aliases):
+            lst = dests.setdefault(name, [])
+            if not lst or lst[-1] != i:
+                lst.append(i)
+    index = {name: k for k, name in enumerate(dests)}
+    dest_off = np.zeros(len(dests) + 1, np.int64)
+    if dests:
+        np.cumsum([len(v) for v in dests.values()], out=dest_off[1:])
+    dest_idx = np.array([i for v in dests.values() for i in v], np.int32)
+    return index, dest_off, dest_idx
+
+
+def marshal_aliases(distros: Sequence[M.Distro], tasks: Sequence[M.Task], now: int,
+                    dependency_db: Optional[Dict[str, M.Task]] = None, duration_history: Optional[dict] = None):
+    """The alias side of a tick: every distro and the tick's schedulable tasks, each task ONCE -> (AliasTable, planner cfg
+    rows of the distros, MarshalledDistro of the whole table: global group names and versions).  Task groups and
+    versions are interned once over the table, dependencies resolve against the table first, then `dependency_db`."""
+    whole = M.Distro(id="")
+    soa, table, keys = marshal_tasks([(whole, list(tasks))], now, dependency_db, duration_history)
+    soa.flags &= np.uint32(~L.EVG_TF_OTHER_DISTRO & 0xFFFFFFFF)  # set per queue on the device
+    index, dest_off, dest_idx = alias_name_table(distros)
+    where = {d.id: i for i, d in enumerate(distros)}
+    sec_off = np.zeros(len(tasks) + 1, np.int64)
+    if len(tasks):
+        np.cumsum([len(t.secondary_distros) for t in tasks], out=sec_off[1:])
+    pairs = [(whole, list(tasks))]
+    at = AliasTable(soa, table.group_max_hosts, int(table.cfg["n_versions"][0]),
+                    np.array([sched_bits(t) for t in tasks], np.uint8), np.array([t.task_group_max_hosts for t in tasks], np.int32),
+                    np.array([where.get(t.distro_id, -1) for t in tasks], np.int32), sec_off,
+                    np.array([index.get(n, -1) for t in tasks for n in t.secondary_distros], np.int32), dest_off, dest_idx,
+                    marshal_deps(pairs, dependency_db), marshal_dep_finished(pairs)).normalize()
+    cfg = np.array([planner_cfg_row(d, d.dispatcher_settings.version == M.DISPATCHER_VERSION_REVISED_WITH_DEPENDENCIES, 0)
+                    for d in distros], dtype=L.DISTRO_CFG_DTYPE)
+    return at, cfg, keys[0]
+
+
+def alias_queues(at: AliasTable, n_distros: int) -> List[np.ndarray]:
+    """FindHostSchedulableForAlias restated over an AliasTable: per distro, the source rows of its alias queue in
+    ascending order (a row once, however many of its names reach the distro)."""
+    ok = ((at.sched & SQ_BASE) == SQ_BASE) & (((at.sched & L.EVG_SQ_UNATTAINABLE) == 0) | ((at.sched & L.EVG_SQ_OVERRIDE_DEPS) != 0))
+    ok &= at.task_group_max_hosts != 1
+    queues: List[set] = [set() for _ in range(n_distros)]
+    for t in np.nonzero(ok)[0]:
+        for name in at.secondary_idx[at.secondary_off[t]:at.secondary_off[t + 1]]:
+            if name >= 0:
+                for e in at.dest_idx[at.dest_off[name]:at.dest_off[name + 1]]:
+                    queues[int(e)].add(int(t))
+    return [np.array(sorted(q), dtype=np.int64) for q in queues]
+
+
+def compose_aliases(at: AliasTable, cfg: np.ndarray):
+    """The alias tick as a fresh evg_upload_with_deps would take it, built on the host (the route evg_plan_aliases
+    replaces): (TaskSoA, DistroTable, DepsTable, dep_finished, source_row, group_source).  Each queue lists its rows in
+    ascending source row with group and version ids renumbered in first-appearance order and its in-queue edges
+    re-indexed; the dependency table refers to every other task as an external one (its state is the task's own)."""
+    D = int(cfg.shape[0])
+    queues = alias_queues(at, D)
+    t = at.tasks
+    rows = np.concatenate(queues) if D else np.zeros(0, np.int64)
+    cols = {name: getattr(t, name)[rows].copy() for name, _ in TaskSoA.COLUMNS}
+    task_off, group_off, gmax, gsrc, nver = [0], [0], [], [], []
+    dep_off, dep_idx = [0], []
+    k = 0
+    for e, q in enumerate(queues):
+        place = {int(u): i for i, u in enumerate(q)}
+        groups: Dict[int, int] = {}
+        versions: Dict[int, int] = {}
+        for u in q:
+            g = int(t.group_id[u])
+            if g >= 0:
+                if g not in groups:
+                    groups[g] = len(groups)
+                    gmax.append(int(at.group_max_hosts[g]))
+                    gsrc.append(g)
+                cols["group_id"][k] = groups[g]
+            v = int(t.version_id[u])
+            cols["version_id"][k] = versions.setdefault(v, len(versions))
+            fl = int(t.flags[u]) & ~L.EVG_TF_OTHER_DISTRO
+            cols["flags"][k] = fl | (L.EVG_TF_OTHER_DISTRO if int(at.primary[u]) != e else 0)
+            if t.n_edges:
+                for x in t.dep_idx[t.dep_off[u]:t.dep_off[u + 1]]:
+                    if int(x) in place:
+                        dep_idx.append(place[int(x)])
+            dep_off.append(len(dep_idx))
+            k += 1
+        task_off.append(k)
+        group_off.append(len(gmax))
+        nver.append(len(versions))
+    c = cfg.copy()
+    c["n_versions"] = nver
+    soa = TaskSoA(**cols, dep_off=np.array(dep_off, np.int64), dep_idx=np.array(dep_idx, np.int32)).normalize()
+    table = DistroTable(np.array(task_off, np.int64), np.array(group_off, np.int64), c, np.array(gmax, np.int32)).normalize()
+    d = at.deps
+    T = at.n_tasks
+    kind = d.dep_kind.copy()
+    ref = np.where(kind == L.EVG_DEP_IN_QUEUE, d.dep_ref, np.where(kind == L.EVG_DEP_EXTERNAL, d.dep_ref + T, d.dep_ref)).astype(np.int32)
+    kind[kind == L.EVG_DEP_IN_QUEUE] = L.EVG_DEP_EXTERNAL
+    lens = (d.dep_off[1:] - d.dep_off[:-1])[rows] if T else np.zeros(0, np.int64)
+    take = np.concatenate([np.arange(d.dep_off[u], d.dep_off[u + 1]) for u in rows]).astype(np.int64) if lens.sum() else np.zeros(0, np.int64)
+    deps = DepsTable(np.concatenate([[0], np.cumsum(lens)]).astype(np.int64), kind[take], ref[take], d.dep_want[take],
+                     d.task_state[rows], d.task_pre[rows], np.concatenate([d.task_state, d.ext_state]).astype(np.uint8))
+    fin = at.dep_finished[take] if at.dep_finished.shape[0] else np.zeros(0, np.int64)
+    return soa, table, deps, fin, rows.astype(np.int32), np.array(gsrc, np.int32)
+
+
 @dataclass
 class DurationRows:
     """evg_duration_rows: finished tasks, the interned group-by key of each, and the aggregation window."""

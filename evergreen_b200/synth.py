@@ -15,7 +15,7 @@ import numpy as np
 
 from . import _lib as L
 from . import model as M
-from .soa import DistroTable, HostSoA, TaskEdit, TaskSoA, apply_edit
+from .soa import SQ_BASE, AliasTable, DepsTable, DistroTable, HostSoA, TaskEdit, TaskSoA, apply_edit
 
 GOLDEN = np.uint64(0x9E3779B97F4A7C15)
 NOW_NS = 1_800_000_000 * 10 ** 9
@@ -568,6 +568,95 @@ def next_tick(w: Workload, seed: int, *, dispatch: float = 0.05, arrive: float =
         hosts = HostSoA(hosts.flags.copy(), hg.astype(np.int32), hosts.expected_ns.copy(), hosts.std_ns.copy(),
                         hosts.start_ns.copy(), hosts.host_off.copy(), hosts.cfg.copy()).normalize()
     return EditTick(edit, rows, values, Workload(w.name, w.now, tasks, distros, hosts))
+
+
+ALIAS_SALT = 0xA11A5
+
+
+def make_aliases(w: Workload, seed: int, *, name_frac: float = 0.2, big: int = 0):
+    """The alias side of tick w, from its own random stream: w's rows are the tick's schedulable tasks (each once; a
+    row's primary distro is the one w files it under) and w's distros the alias distros -> (AliasTable, cfg).
+    A name_frac share of tasks carries 1-3 SecondaryDistros names: distro ids (the task's own among them), alias names
+    that several distros share, and names no distro has.  Some rows fail a base-query bit, carry an unattainable
+    dependency (with or without the override), or sit in a single-host task group (or carry TaskGroupMaxHosts == 1
+    without one).  big > 0: the first `big` rows also name an alias of distro 0 and pass every filter, so its alias
+    queue takes the general path once big > 12 288."""
+    t, dt = w.tasks, w.distros
+    T, D = t.n_tasks, dt.n_distros
+    rng = Rng(seed ^ ALIAS_SALT)
+    distro_of = np.repeat(np.arange(D, dtype=np.int64), np.diff(dt.task_off))
+    vbase = np.concatenate([[0], np.cumsum(dt.cfg["n_versions"].astype(np.int64))])
+    gid = np.where(t.group_id >= 0, dt.group_off[distro_of] + t.group_id, -1).astype(np.int32)
+    vid = (vbase[distro_of] + t.version_id).astype(np.int32)
+    flags = t.flags & np.uint32(~(L.EVG_TF_DEPS_MET | L.EVG_TF_OTHER_DISTRO) & 0xFFFFFFFF)
+    dep_off, dep_idx = t.dep_off, t.dep_idx
+    if t.n_edges:
+        owner = np.repeat(np.arange(T, dtype=np.int64), np.diff(t.dep_off))
+        dep_idx = (dt.task_off[distro_of[owner]] + t.dep_idx).astype(np.int32)
+    tasks = TaskSoA(t.priority, t.expected_ns, t.queue_basis_ns, t.wait_basis_ns, t.num_dependents, t.task_group_order, gid, vid,
+                    flags, dep_off, dep_idx).normalize()
+    gmax = dt.group_max_hosts.astype(np.int32)  # 1 .. 3: the groups of 1 are single-host groups
+    tgmax = np.where(gid >= 0, gmax[np.maximum(gid, 0)] if gmax.shape[0] else 0,
+                     np.where(rng.uniform(T) < 0.02, 1, 0)).astype(np.int32)
+    sched = np.full(T, SQ_BASE, dtype=np.uint8)
+    for bit in (L.EVG_SQ_ACTIVATED, L.EVG_SQ_UNDISPATCHED, L.EVG_SQ_PRIORITY_OK, L.EVG_SQ_HOST_PLATFORM):
+        sched &= np.where(rng.uniform(T) < 0.01, ~bit & 0xFF, 0xFF).astype(np.uint8)
+    sched |= np.where(rng.uniform(T) < 0.04, L.EVG_SQ_UNATTAINABLE, 0).astype(np.uint8)
+    sched |= np.where(rng.uniform(T) < 0.03, L.EVG_SQ_OVERRIDE_DEPS, 0).astype(np.uint8)
+    primary = np.where(rng.uniform(T) < 0.02, -1, distro_of).astype(np.int32)
+    # names: 0 .. D-1 the distros' own ids, then A alias names; each distro takes 0-2 of them (shared between distros)
+    A = max(2, D // 3)
+    n_alias = rng.integers(D, 0, 2)
+    pick = rng.integers(2 * D, 0, A - 1).reshape(2, D) if D else np.zeros((2, 0), np.int64)
+    dests = [[] for _ in range(D + A + (1 if big else 0))]
+    for e in range(D):
+        dests[e].append(e)
+        for k in range(int(n_alias[e])):
+            if e not in dests[D + int(pick[k, e])]:
+                dests[D + int(pick[k, e])].append(e)
+    if big:
+        dests[D + A].append(0)
+    carries = rng.uniform(T) < name_frac
+    n_names = np.where(carries, rng.integers(T, 1, 3), 0)
+    if big:
+        n_names[:big] += 1
+    sec_off = np.concatenate([[0], np.cumsum(n_names)]).astype(np.int64)
+    NS = int(sec_off[-1])
+    owner = np.repeat(np.arange(T, dtype=np.int64), n_names)
+    u = rng.uniform(NS)
+    own = distro_of[owner] if T else np.zeros(0, np.int64)
+    sec = np.where(u < 0.2, own, np.where(u < 0.5, rng.integers(NS, 0, max(D - 1, 0)),
+                                          np.where(u < 0.9, D + rng.integers(NS, 0, A - 1), -1))).astype(np.int32)
+    if big:
+        sec[sec_off[1:big + 1] - 1] = D + A
+        sched[:big] = SQ_BASE
+        tgmax[:big] = np.where(tgmax[:big] == 1, 0, tgmax[:big])
+    dest_off = np.concatenate([[0], np.cumsum([len(x) for x in dests])]).astype(np.int64)
+    dest_idx = np.array([e for x in dests for e in x], np.int32)
+    # dependencies: a row's in-table edges (the rows' own states), then a few outside the table or missing
+    E = tasks.n_edges
+    n_ext = np.where(rng.uniform(T) < 0.05, 1, 0)
+    per = (np.diff(tasks.dep_off) if E else np.zeros(T, np.int64)) + n_ext
+    doff = np.concatenate([[0], np.cumsum(per)]).astype(np.int64)
+    kind = np.full(int(doff[-1]), L.EVG_DEP_EXTERNAL, np.uint8)
+    ref = np.zeros(int(doff[-1]), np.int32)
+    X = 16
+    if E:
+        own_pos = doff[np.repeat(np.arange(T), np.diff(tasks.dep_off))] + (np.arange(E) - np.repeat(tasks.dep_off[:-1], np.diff(tasks.dep_off)))
+        kind[own_pos] = L.EVG_DEP_IN_QUEUE
+        ref[own_pos] = tasks.dep_idx
+    ext_pos = doff[1:][n_ext > 0] - 1
+    ref[ext_pos] = rng.integers(ext_pos.shape[0], 0, X - 1)
+    kind[ext_pos] = np.where(rng.uniform(ext_pos.shape[0]) < 0.3, L.EVG_DEP_MISSING, L.EVG_DEP_EXTERNAL)
+    us = rng.uniform(T)
+    state = np.where(us < 0.85, 0, np.where(us < 0.93, 1, 2)).astype(np.uint8)
+    state |= np.where(rng.uniform(T) < 0.03, L.EVG_TS_BLOCKED, 0).astype(np.uint8)
+    want = np.where(rng.uniform(int(doff[-1])) < 0.9, L.EVG_WANT_SUCCESS, L.EVG_WANT_ANY).astype(np.uint8)
+    pre = (np.where(rng.uniform(T) < 0.03, L.EVG_TP_OVERRIDE, 0) | np.where(rng.uniform(T) < 0.05, L.EVG_TP_MET_TIME, 0)).astype(np.uint8)
+    deps = DepsTable(doff, kind, ref, want, state, pre, np.where(rng.uniform(X) < 0.8, 0, 1).astype(np.uint8))
+    fin = np.where(rng.uniform(int(doff[-1])) < 0.7, w.now - rng.integers(int(doff[-1]), 0, 3 * M.HOUR), M.ZERO_TIME).astype(np.int64)
+    at = AliasTable(tasks, gmax, int(vbase[-1]), sched, tgmax, primary, sec_off, sec, dest_off, dest_idx, deps, fin).normalize()
+    return at, dt.cfg.copy()
 
 
 def power_law_sizes(rng: Rng, D: int, alpha: float = 1.2, lo: int = 1, hi: int = 1_000_000) -> np.ndarray:

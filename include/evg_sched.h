@@ -500,6 +500,65 @@ int evg_plan_from_finder(evg_ctx* ctx, const evg_runnable_in* in, const evg_task
                          const evg_host_soa* hosts, const int64_t* host_off, const evg_alloc_cfg* acfg,
                          const int64_t* dep_finished_ns, int64_t now_ns, int32_t* runnable, int64_t* count);
 
+/* ---- alias queues: the secondary queue of every distro (SURVEY.md §8 row A21) ---- */
+
+/* The tick's schedulable tasks, each ONCE (not once per queue it may join).  Host pointers. */
+typedef struct {
+  /* planner columns of the n_tasks source rows: group_id / version_id are TABLE-GLOBAL dense ids (what
+   * evg_intern_columns gives for the table as one distro), flags without EVG_TF_DEPS_MET and EVG_TF_OTHER_DISTRO (both
+   * are set on the device), wait_basis_ns = ScheduledTime as for evg_upload_with_deps; dep_off / dep_idx are the entries
+   * of Task.DependsOn that are rows of this table, as row indices, in DependsOn order with duplicates */
+  evg_task_soa tasks;
+  int32_t n_groups;                    /* global task groups */
+  int32_t n_versions;                  /* global versions */
+  const int32_t* group_max_hosts;      /* n_groups: TaskGroupMaxHosts of the group */
+  const uint8_t* sched;                /* n_tasks: EVG_SQ_* (the schedulableHostTasksQuery bits) */
+  const int32_t* task_group_max_hosts; /* n_tasks: raw Task.TaskGroupMaxHosts (== 1 keeps a task out, task group or not) */
+  const int32_t* primary;              /* n_tasks: distro index of Task.DistroId, -1 when it is not in the distro table */
+  const int64_t* secondary_off;        /* n_tasks + 1: CSR of Task.SecondaryDistros over the rows */
+  const int32_t* secondary_idx;        /* name index of each entry, -1 for a name no distro has */
+  int32_t n_names;
+  int32_t _reserved;
+  const int64_t* dest_off;             /* n_names + 1: CSR over names of the distros e whose {e} U e.Aliases holds the name */
+  const int32_t* dest_idx;             /* distro index */
+  const evg_deps_in* deps;             /* direct dependencies of the same n_tasks rows (required) */
+  const int64_t* dep_finished_ns;      /* per deps entry: Dependency.FinishedAt (NULL = unknown) */
+} evg_alias_in;
+
+typedef struct {
+  int64_t* task_off;   /* n_distros + 1: offsets of the alias queues in the resident tick */
+  int64_t* group_off;  /* n_distros + 1: their task-group slots */
+  int32_t* n_versions; /* n_distros */
+} evg_alias_out;
+
+/* task.FindHostSchedulableForAlias + scheduler.PrioritizeTasks(..., IsSecondaryQueue) for every distro at once.  Task t
+ * is in distro e's alias queue iff t passes schedulableHostTasksQuery (ACTIVATED, UNDISPATCHED, PRIORITY_OK,
+ * HOST_PLATFORM, and not UNATTAINABLE unless OVERRIDE_DEPS), task_group_max_hosts != 1, and some name of t's
+ * SecondaryDistros is e or one of e's aliases -- once, however many names match.  Each alias queue lists its tasks in
+ * ascending source row; its task groups and versions get dense ids in first-appearance order, as evg_intern_columns
+ * assigns them; a task's in-queue edges are its dependencies that are in the same alias queue.  Task.DependenciesMet and
+ * the DependenciesMetTime stamp are evaluated once per row (as evg_upload_with_deps does) and serve every queue the row
+ * joins; EVG_TF_OTHER_DISTRO is set per queue (primary[t] != e).  cfg[e] is alias distro e's planner settings (its
+ * n_versions is ignored: the device counts them).  The alias queues become the context's resident tick, planner only
+ * (no hosts): evg_run_resident, evg_download, evg_download_queue, evg_update_tasks and evg_edit_tasks work on it as
+ * after evg_upload; evg_download_alias_map maps its rows back to source rows.
+ * What crosses PCIe: the source table once (host to device); in between, the host reads one count, then the queue,
+ * group, version and edge offsets of every distro and the group_max_hosts of every alias group slot -- O(n_distros +
+ * alias groups) values, nothing per task.
+ * EVG_ERR_INVALID, previous tick still resident and runnable: negative sizes, null arrays, sizes that disagree, a CSR
+ * (secondary_off, dest_off, dep_off, deps->dep_off) that does not start at 0, end at its entry count and never
+ * decrease, a dest_idx outside [0, n_distros).  EVG_ERR_INVALID with no resident tick: an id found out of range on the
+ * device (secondary_idx, primary, group_id, version_id, dep_idx, dep_ref), more than 2^31-2 (queue, task) pairs, or an
+ * alias queue above 2^21-1 tasks.
+ * Replaces: distroAliasSchedulerJob.Run for every distro (units/scheduler_alias.go:55-117): FindHostSchedulableForAlias
+ * (model/task/task.go:3371-3386, model/distro/aliases.go:14-27) and PrioritizeTasks (scheduler/scheduler.go:27-51). */
+int evg_plan_aliases(evg_ctx* ctx, const evg_alias_in* in, const evg_distro_cfg* cfg, int32_t n_distros, int64_t now_ns,
+                     evg_alias_out* out);
+/* After evg_plan_aliases (and evg_update_tasks): source_row[r] = the source row of resident row r (task_off[n_distros]
+ * entries), group_source[s] = the global group id of alias group slot s (group_off[n_distros] entries).  Either may be
+ * NULL.  EVG_ERR_STATE once another call replaced the tick's rows. */
+int evg_download_alias_map(evg_ctx* ctx, int32_t* source_row, int32_t* group_source);
+
 /* ---- host-side string interning for the marshaller ------------------------ */
 
 /* A column of n strings: bytes[off[i] .. off[i+1]) is string i (not NUL-terminated). */
