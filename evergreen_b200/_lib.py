@@ -140,6 +140,15 @@ EVG_SQ_ACTIVATED, EVG_SQ_UNDISPATCHED, EVG_SQ_PRIORITY_OK, EVG_SQ_HOST_PLATFORM 
 EVG_SQ_UNATTAINABLE, EVG_SQ_OVERRIDE_DEPS, EVG_SQ_GITHUB_PR, EVG_SQ_PATCH_REQUEST = 0x10, 0x20, 0x40, 0x80
 EVG_PF_ENABLED, EVG_PF_HIDDEN, EVG_PF_DISPATCHING_DISABLED, EVG_PF_PATCHING_DISABLED = 0x1, 0x2, 0x4, 0x8
 EVG_FINDER_NO_DEPS, EVG_FINDER_LEGACY, EVG_FINDER_ALTERNATE = 0, 1, 2
+EVG_FINDER_PIPELINE, EVG_FINDER_PIPELINE_NO_DEPS = 3, 4
+EVG_STATUS_SUCCESS, EVG_STATUS_FAILED, EVG_STATUS_ANY = 0, 1, 2
+EVG_PR_ENABLED, EVG_PR_DISPATCHING_DISABLED, EVG_PR_PATCHING_FALSE = 0x1, 0x2, 0x4
+
+
+class PipelineInStruct(C.Structure):
+    _fields_ = [("n_status", C.c_int32), ("_reserved", C.c_int32), ("dep_status", C.c_void_p), ("task_status", C.c_void_p),
+                ("ext_status", C.c_void_p), ("task_unattainable", C.c_void_p), ("ext_unattainable", C.c_void_p),
+                ("project_raw", C.c_void_p)]
 
 
 class DurationRowsStruct(C.Structure):
@@ -196,6 +205,7 @@ SYMBOLS = {
     "evg_update_tasks": (C.c_int, [_P, C.c_int64, _P, _P]),
     "evg_edit_tasks": (C.c_int, [_P, _P, _P, _P, _P, _P]),
     "evg_plan_from_finder": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, C.c_int64, _P, _P]),
+    "evg_plan_from_finder_ex": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int64, _P, _P]),
     "evg_plan_aliases": (C.c_int, [_P, _P, _P, C.c_int32, C.c_int64, _P]),
     "evg_download_alias_map": (C.c_int, [_P, _P, _P]),
     "evg_intern_columns": (C.c_int, [_P, _P, C.c_int32]),
@@ -212,6 +222,7 @@ SYMBOLS = {
     "evg_upload_with_deps": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, C.c_int64]),
     "evg_download_deps": (C.c_int, [_P, _P, _P]),
     "evg_find_runnable_batch": (C.c_int, [_P, _P, _P, _P]),
+    "evg_find_runnable_ex": (C.c_int, [_P, _P, _P, _P, _P]),
     "evg_expected_durations_batch": (C.c_int, [_P, _P, _P]),
     "evg_prioritize_legacy_batch": (C.c_int, [_P, _P, _P, _P, C.c_int32, _P, _P, _P]),
     "evg_dag_rebuild_batch": (C.c_int, [_P, _P, _P, _P, C.c_int32, _P, _P, _P, _P, _P]),

@@ -21,6 +21,9 @@
 // The rows either side of the path (SURVEY.md §8f):
 //   k_deps_met            Task.DependenciesMet / AllDependenciesSatisfied (model/task/task.go:632-671,795-821)
 //   k_runnable            the task finders' filter + stable compaction (scheduler/task_finder.go:40-317)
+//   k_runnable_pipe       the same with the pipeline finder's codes (model/task/db.go:887-1066)
+//   k_pl_deps             the pipeline's $graphLookup dependency filter (db.go:923-996)
+//   k_pl_plan, k_pl_edge_*  what the planner receives from a pipeline distro (evg_plan_from_finder_ex)
 //   k_dur_sum/dev/final   expected-duration statistics (model/task/expected_duration.go:36-96)
 // No CPU fallback exists in this file: without a device every entry point fails.
 #include <cuda_runtime.h>
@@ -462,6 +465,225 @@ __global__ void __launch_bounds__(256) k_runnable(DRunnable R, int32_t* __restri
   for (int64_t i = base + running + threadIdx.x; i < end; i += 256) out[i] = -1;  // unused tail of the distro's slots
   if (threadIdx.x == 0) count[d] = running;
 }
+// k_runnable's filter (EVG_FINDER_NO_DEPS / LEGACY / ALTERNATE) for one candidate, as k_runnable_pipe applies it.
+__device__ __forceinline__ bool finder_keep(const DRunnable& R, uint32_t q, int32_t p, uint32_t mt, uint32_t met_bit, int64_t v0,
+                                            int64_t v1, int* err) {
+  // schedulableHostTasksQuery (model/task/db.go:671-689)
+  bool k = (q & EVG_SQ_ACTIVATED) && (q & EVG_SQ_UNDISPATCHED) && (q & EVG_SQ_PRIORITY_OK) && (q & EVG_SQ_HOST_PLATFORM) &&
+           (!(q & EVG_SQ_UNATTAINABLE) || (q & EVG_SQ_OVERRIDE_DEPS));
+  if (p >= R.n_projects) { atomicOr(err, 1); k = false; }
+  else if (p < 0) k = false;  // "could not find project for task" (task_finder.go:57-67)
+  else if (k) {
+    const uint32_t pf = R.project_flags[p];
+    // ProjectCanDispatchTask (model/project_ref.go:3441-3462)
+    if (!(pf & EVG_PF_ENABLED) && !((q & EVG_SQ_GITHUB_PR) && (pf & EVG_PF_HIDDEN))) k = false;
+    if (pf & EVG_PF_DISPATCHING_DISABLED) k = false;
+    if ((q & EVG_SQ_PATCH_REQUEST) && (pf & EVG_PF_PATCHING_DISABLED)) k = false;
+    if (k && v1 > v0) {  // len(d.ValidProjects) > 0 && !contains(ref.Id) (task_finder.go:74-84)
+      bool found = false;
+      for (int64_t x = v0; x < v1 && !found; x++) found = R.valid_idx[x] == p;
+      k = found;
+    }
+    if (k) k = (mt & met_bit) != 0;  // the finder's dependency predicate (NO_DEPS reads 3: always met)
+  }
+  return k;
+}
+// The pipeline finder's filter (task.FindHostRunnable, model/task/db.go:887-1066) for one candidate: the same base query
+// and ValidProjects match, the RAW project_ref document (filterDisabledProjects / filterPatchingDisabledProjects,
+// :1030-1048: no hidden-project exemption; patching_disabled must be stored false), and for EVG_FINDER_PIPELINE the
+// $graphLookup verdict, bit 2 of k_deps_met's byte (k_pl_deps).
+__device__ __forceinline__ bool pipeline_keep(const DRunnable& R, const uint8_t* __restrict__ praw, uint32_t q, int32_t p, uint32_t mt,
+                                              uint32_t finder, int64_t v0, int64_t v1, int* err) {
+  bool k = (q & EVG_SQ_ACTIVATED) && (q & EVG_SQ_UNDISPATCHED) && (q & EVG_SQ_PRIORITY_OK) && (q & EVG_SQ_HOST_PLATFORM) &&
+           (!(q & EVG_SQ_UNATTAINABLE) || (q & EVG_SQ_OVERRIDE_DEPS));
+  if (p >= R.n_projects) { atomicOr(err, 1); k = false; }
+  else if (p < 0) k = false;  // the $lookup finds no project_ref: project_ref.0.enabled is missing
+  else if (k) {
+    const uint32_t pr = praw[p];
+    if (!(pr & EVG_PR_ENABLED) || (pr & EVG_PR_DISPATCHING_DISABLED)) k = false;
+    if ((q & EVG_SQ_PATCH_REQUEST) && !(pr & EVG_PR_PATCHING_FALSE)) k = false;  // Requester $in PatchRequesters
+    if (k && v1 > v0) {  // filterInvalidDistros: project $in ValidProjects (db.go:1031-1033)
+      bool found = false;
+      for (int64_t x = v0; x < v1 && !found; x++) found = R.valid_idx[x] == p;
+      k = found;
+    }
+    if (k && finder == EVG_FINDER_PIPELINE) k = (mt & 4u) != 0;
+  }
+  return k;
+}
+// k_runnable with the pipeline finder's codes (evg_find_runnable_ex / evg_plan_from_finder_ex with an evg_pipeline_in;
+// praw: evg_pipeline_in.project_raw).  The same compaction; k_runnable itself is left as it was, so that its code does
+// not change for the callers that never use the pipeline.
+__global__ void __launch_bounds__(256) k_runnable_pipe(DRunnable R, const uint8_t* __restrict__ praw, int32_t* __restrict__ out,
+                                                       int64_t* __restrict__ count, int* err) {
+  constexpr int ITEMS = 4;  // candidates per thread and step: their loads are in flight together, one barrier pair per 1024
+  const int d = blockIdx.x;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const unsigned full = 0xffffffffu;
+  const int64_t base = R.task_off[d], end = R.task_off[d + 1];
+  const int64_t v0 = R.valid_off[d], v1 = R.valid_off[d + 1];
+  const uint32_t finder = R.finder[d];
+  const uint32_t met_bit = finder == EVG_FINDER_LEGACY ? 1u : 2u;
+  const bool reads_met = finder != EVG_FINDER_NO_DEPS && finder != EVG_FINDER_PIPELINE_NO_DEPS;
+  __shared__ uint32_t s_cnt[ITEMS * 8];  // survivors of (item j, warp w), in output order j-major
+  int64_t running = 0;  // kept identically by every thread
+  for (int64_t c0 = base; c0 < end; c0 += 256 * ITEMS) {
+    uint32_t sq[ITEMS], mt[ITEMS];
+    int32_t pj[ITEMS];
+#pragma unroll
+    for (int j = 0; j < ITEMS; j++) {
+      const int64_t t = c0 + j * 256 + threadIdx.x;
+      const bool in = t < end;
+      sq[j] = in ? R.sched[t] : 0u;
+      pj[j] = in ? R.project[t] : -1;
+      mt[j] = (in && reads_met) ? R.met[t] : 3u;
+    }
+    bool keep[ITEMS];
+    unsigned m[ITEMS];
+#pragma unroll
+    for (int j = 0; j < ITEMS; j++) {
+      bool k;
+      if (finder > EVG_FINDER_ALTERNATE) k = pipeline_keep(R, praw, sq[j], pj[j], mt[j], finder, v0, v1, err);
+      else k = finder_keep(R, sq[j], pj[j], mt[j], met_bit, v0, v1, err);
+      keep[j] = k;
+      m[j] = __ballot_sync(full, k);
+      if (lane == 0) s_cnt[j * 8 + warp] = __popc(m[j]);
+    }
+    __syncthreads();
+    uint32_t total = 0, before[ITEMS];
+#pragma unroll
+    for (int j = 0; j < ITEMS; j++) {
+#pragma unroll
+      for (int w = 0; w < 8; w++) {
+        if (w == warp) before[j] = total;
+        total += s_cnt[j * 8 + w];
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < ITEMS; j++)
+      if (keep[j]) out[base + running + before[j] + __popc(m[j] & ((1u << lane) - 1u))] = int32_t(c0 + j * 256 + threadIdx.x - base);
+    running += total;
+    __syncthreads();
+  }
+  for (int64_t i = base + running + threadIdx.x; i < end; i += 256) out[i] = -1;  // unused tail of the distro's slots
+  if (threadIdx.x == 0) count[d] = running;
+}
+// The pipeline's dependency filter (model/task/db.go:923-996, with removeDeps): met[t] |= 4 when t survives it.  The
+// $graphLookup finds the existing documents among the DependsOn ids, the two $unwinds and matchIds pair each entry with
+// its own document, and $group / $redact keep t iff every such pair is satisfied -- the entry's status string equals
+// the document's, or it is "*" and the document is success / failed or has an unattainable depends_on entry.  An entry
+// without a document pairs with nothing; a t whose entries ALL lack one leaves no row and is dropped; a t without
+// DependsOn is kept (both sides of matchIds are missing, which compares equal).  err bit 2: a status id out of range.
+struct DPipe {
+  int32_t n_status;
+  const int32_t* dep_status;
+  const int32_t* task_status;
+  const int32_t* ext_status;
+  const uint8_t* task_unatt;
+  const uint8_t* ext_unatt;
+};
+__global__ void __launch_bounds__(256) k_pl_deps(DDeps X, DPipe P, uint8_t* __restrict__ met, int* err) {
+  const int64_t t = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (t >= X.n_tasks) return;
+  const int64_t e0 = X.dep_off[t], e1 = X.dep_off[t + 1];
+  const int32_t own = P.task_status[t];
+  bool ok = true, paired = false;
+  if (own < 0 || own >= P.n_status) { atomicOr(err, 2); ok = false; }
+  for (int64_t e = e0; e < e1 && ok; e++) {
+    const uint8_t kind = X.dep_kind[e];
+    const int32_t ref = X.dep_ref[e];
+    int32_t st;
+    bool un;
+    if (kind == EVG_DEP_IN_QUEUE) {
+      if (ref < 0 || ref >= X.n_tasks) { atomicOr(err, 1); ok = false; break; }
+      st = P.task_status[ref]; un = P.task_unatt[ref] != 0;
+    } else if (kind == EVG_DEP_EXTERNAL) {
+      if (ref < 0 || ref >= X.n_ext) { atomicOr(err, 1); ok = false; break; }
+      st = P.ext_status[ref]; un = P.ext_unatt[ref] != 0;
+    } else {
+      continue;  // no document with that id: the entry pairs with nothing
+    }
+    const int32_t w = P.dep_status[e];
+    if (w < 0 || w >= P.n_status || st < 0 || st >= P.n_status) { atomicOr(err, 2); ok = false; break; }
+    paired = true;
+    ok = w == st || (w == EVG_STATUS_ANY && (st == EVG_STATUS_SUCCESS || st == EVG_STATUS_FAILED || un));
+  }
+  if (ok && (paired || e1 == e0)) met[t] |= 4u;
+}
+
+// What the planner receives from a pipeline distro, once the keep mask exists (evg_plan_from_finder_ex):
+//   EVG_FINDER_PIPELINE: the decoded task has no DependsOn, so HasDependenciesMet holds (task.go:3393-3395): met, no stamp;
+//   EVG_FINDER_PIPELINE_NO_DEPS: Task.DependenciesMet (task.go:632-671) as k_deps_met's bit 0 and stamp, except that a
+//     dependency that is a kept candidate of the same distro comes from the finder's output, whose depends_on.unattainable
+//     was projected away (db.go:916-921): it is never Blocked().
+// Other finders' rows are left as k_deps_met wrote them.
+__global__ void __launch_bounds__(256) k_pl_plan(DDeps X, int32_t D, const int64_t* __restrict__ off, const uint8_t* __restrict__ finder,
+                                                 const int32_t* __restrict__ keep, uint8_t* __restrict__ met,
+                                                 const int64_t* __restrict__ dep_fin, int64_t now, int64_t* __restrict__ met_time) {
+  const int64_t t = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  const int d = block_find_distro(off, D, t, X.n_tasks);
+  if (d < 0) return;
+  const uint32_t f = finder[d];
+  if (f == EVG_FINDER_PIPELINE) {
+    met[t] |= 1u;
+    met_time[t] = EVG_TIME_ZERO;
+    return;
+  }
+  if (f != EVG_FINDER_PIPELINE_NO_DEPS) return;
+  const int64_t e0 = X.dep_off[t], e1 = X.dep_off[t + 1], lo = off[d], hi = off[d + 1];
+  const bool shortcut = (X.task_pre[t] & (EVG_TP_OVERRIDE | EVG_TP_MET_TIME)) != 0;
+  bool ok = true;
+  if (e1 > e0 && !shortcut) {
+    for (int64_t e = e0; e < e1 && ok; e++) {
+      const int32_t ref = X.dep_ref[e];
+      uint8_t st;
+      if (X.dep_kind[e] == EVG_DEP_IN_QUEUE) {  // dep_ref was range-checked by k_deps_met
+        st = X.task_state[ref];
+        if (ref >= lo && ref < hi && keep[ref]) st &= ~EVG_TS_BLOCKED;
+      } else if (X.dep_kind[e] == EVG_DEP_EXTERNAL) {
+        st = X.ext_state[ref];
+      } else {
+        ok = false;
+        break;
+      }
+      const uint32_t status = st & EVG_TS_STATUS_MASK;
+      switch (X.dep_want[e]) {
+        case EVG_WANT_SUCCESS: ok = status == 0; break;
+        case EVG_WANT_FAILED: ok = status == 1; break;
+        case EVG_WANT_ANY: ok = status < 2 || (st & EVG_TS_BLOCKED); break;
+        default: ok = false;
+      }
+    }
+  }
+  met[t] = uint8_t((met[t] & ~1u) | ((ok || shortcut) ? 1u : 0u));
+  int64_t stamp = EVG_TIME_ZERO;
+  if (ok && !shortcut && e1 > e0) {
+    if (dep_fin)
+      for (int64_t e = e0; e < e1; e++) {
+        const int64_t fin = dep_fin[e];
+        if (fin != EVG_TIME_ZERO && fin != 0 && fin > stamp) stamp = fin;
+      }
+    if (stamp == EVG_TIME_ZERO || stamp == 0) stamp = now;
+  }
+  met_time[t] = stamp;
+}
+
+// The candidates' edges without those of EVG_FINDER_PIPELINE rows (whose DependsOn decodes empty): count, then (after a
+// scan into new_off) copy.  The kept rows of the other finders keep their edges for compose_tick to re-index.
+__global__ void __launch_bounds__(256) k_pl_edge_count(int64_t n, int32_t D, const int64_t* __restrict__ off, const uint8_t* __restrict__ finder,
+                                                       const int64_t* __restrict__ dep_off, int32_t* __restrict__ cnt) {
+  const int64_t t = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  const int d = block_find_distro(off, D, t, n);
+  if (d < 0) return;
+  cnt[t] = finder[d] == EVG_FINDER_PIPELINE ? 0 : int32_t(dep_off[t + 1] - dep_off[t]);
+}
+__global__ void __launch_bounds__(256) k_pl_edge_write(int64_t n, const int64_t* __restrict__ dep_off, const int32_t* __restrict__ dep_idx,
+                                                       const int64_t* __restrict__ new_off, int32_t* __restrict__ new_idx) {
+  const int64_t t = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (t >= n) return;
+  const int64_t w = new_off[t], k = new_off[t + 1] - w, e0 = dep_off[t];
+  for (int64_t j = 0; j < k; j++) new_idx[w + j] = dep_idx[e0 + j];
+}
 
 // Expected-duration statistics (model/task/expected_duration.go:36-96): the $match, then per key count / sum, then
 // the squared deviations from floor(mean) as an exact 128-bit integer, then one rounding per output.
@@ -900,6 +1122,10 @@ struct evg_ctx {
     TaskCols cand;       // evg_plan_from_finder: the candidates' columns
     DevBuf dep_off, dep_idx;  // and their edges
   } pf;
+  struct {  // the pipeline finder's tables (the first evg_find_runnable_ex / evg_plan_from_finder_ex with a pipeline allocates them)
+    DevBuf dep_status, task_status, ext_status, task_unatt, ext_unatt, project_raw;  // an evg_pipeline_in, staged
+    DevBuf edge_cnt, dep_off, dep_idx, scan_sum;  // the candidates' edges without those of EVG_FINDER_PIPELINE rows
+  } pl;
   // evg_edit_tasks: resident columns an edit may start from (evg_upload, evg_upload_with_deps, evg_plan_from_finder,
   // evg_edit_tasks; not borrowed columns, not what a one-shot call left)
   bool editable = false;
@@ -2185,8 +2411,10 @@ int evg_expected_durations_batch(evg_ctx* c, const evg_duration_rows* in, evg_du
 }
 
 // The finder tables of evg_find_runnable_batch and evg_plan_from_finder: checked, staged into pf.*, and k_runnable's view
-// of them (the caller sets r->met).  `any_deps`: some distro's finder reads the dependency verdicts.  n_distros > 0.
-static int stage_finder(evg_ctx* c, const evg_runnable_in* in, DRunnable* r, bool* any_deps) {
+// of them (the caller sets r->met).  `any_deps`: some distro's finder reads the dependency verdicts.  `pipe`: the pipeline
+// codes are allowed, `any_pipe` / `pipe_deps` report whether some distro uses one / EVG_FINDER_PIPELINE.  n_distros > 0.
+static int stage_finder(evg_ctx* c, const evg_runnable_in* in, DRunnable* r, bool* any_deps, const evg_pipeline_in* pipe = nullptr,
+                        bool* any_pipe = nullptr, bool* pipe_deps = nullptr) {
   const int64_t T = in->n_tasks;
   const int32_t D = in->n_distros, P = in->n_projects;
   if (!in->task_off || !in->valid_off || !in->finder) return fail(EVG_ERR_INVALID, "null distro arrays");
@@ -2194,13 +2422,26 @@ static int stage_finder(evg_ctx* c, const evg_runnable_in* in, DRunnable* r, boo
   if (P > 0 && !in->project_flags) return fail(EVG_ERR_INVALID, "null project_flags");
   if (in->task_off[0] != 0 || in->task_off[D] != T || in->valid_off[0] != 0) return fail(EVG_ERR_INVALID, "offsets do not span the tables");
   *any_deps = false;
+  const uint8_t max_code = pipe ? EVG_FINDER_PIPELINE_NO_DEPS : EVG_FINDER_ALTERNATE;
   for (int32_t d = 0; d < D; d++) {
     if (in->task_off[d + 1] < in->task_off[d] || in->valid_off[d + 1] < in->valid_off[d]) return fail(EVG_ERR_INVALID, "offsets of distro %d decrease", d);
-    if (in->finder[d] > EVG_FINDER_ALTERNATE) return fail(EVG_ERR_INVALID, "distro %d: unknown finder %d", d, int(in->finder[d]));
-    *any_deps = *any_deps || in->finder[d] != EVG_FINDER_NO_DEPS;
+    if (in->finder[d] > max_code)
+      return fail(EVG_ERR_INVALID, in->finder[d] <= EVG_FINDER_PIPELINE_NO_DEPS ? "distro %d: the pipeline finder (%d) needs an evg_pipeline_in"
+                                                                                 : "distro %d: unknown finder %d", d, int(in->finder[d]));
+    *any_deps = *any_deps || (in->finder[d] != EVG_FINDER_NO_DEPS && in->finder[d] != EVG_FINDER_PIPELINE_NO_DEPS);
+    if (any_pipe) *any_pipe = *any_pipe || in->finder[d] >= EVG_FINDER_PIPELINE;
+    if (pipe_deps) *pipe_deps = *pipe_deps || in->finder[d] == EVG_FINDER_PIPELINE;
   }
   const int64_t V = in->valid_off[D];
   if (V > 0 && !in->valid_idx) return fail(EVG_ERR_INVALID, "null valid_idx");
+  if (pipe_deps && *pipe_deps && in->n_tasks > 0) {  // what the host can check of the pipeline's dependency tables
+    const evg_deps_in* x = in->deps;
+    if (!x || x->n_tasks != in->n_tasks) return fail(EVG_ERR_INVALID, "the pipeline finder needs the candidates' dependency table");
+    if (pipe->n_status < 3) return fail(EVG_ERR_INVALID, "evg_pipeline_in: n_status %d < 3 (the reserved ids)", int(pipe->n_status));
+    if (!pipe->task_status || !pipe->task_unattainable || (x->n_deps > 0 && !pipe->dep_status) ||
+        (x->n_ext > 0 && (!pipe->ext_status || !pipe->ext_unattainable)))
+      return fail(EVG_ERR_INVALID, "evg_pipeline_in: null status column");
+  }
   CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   auto& pf = c->pf;
@@ -2217,10 +2458,46 @@ static int stage_finder(evg_ctx* c, const evg_runnable_in* in, DRunnable* r, boo
   r->task_off = pf.task_off.as<int64_t>(); r->sched = pf.sched.as<uint8_t>(); r->project = pf.project.as<int32_t>();
   r->project_flags = pf.project_flags.as<uint8_t>(); r->valid_off = pf.valid_off.as<int64_t>(); r->valid_idx = pf.valid_idx.as<int32_t>();
   r->finder = pf.finder.as<uint8_t>(); r->met = nullptr;
+  if (pipe && P > 0) {
+    if (!pipe->project_raw) return fail(EVG_ERR_INVALID, "null project_raw");
+    UP(s, c->pl.project_raw, pipe->project_raw, P, uint8_t);
+  }
   return EVG_OK;
 }
 
-int evg_find_runnable_batch(evg_ctx* c, const evg_runnable_in* in, int32_t* runnable, int64_t* count) {
+// The status columns of an evg_pipeline_in over the staged dependency table `x` (deps_to_device ran) and k_pl_deps,
+// which adds bit 2 to deps.met.  stage_finder checked the sizes; the ids are checked on the device.
+static int pipeline_deps(evg_ctx* c, const evg_deps_in* x, const evg_pipeline_in* pipe) {
+  const int64_t T = x->n_tasks, E = x->n_deps, X = x->n_ext;
+  cudaStream_t s = c->stream;
+  auto& p = c->pl;
+  UP(s, p.dep_status, pipe->dep_status, E, int32_t);
+  UP(s, p.task_status, pipe->task_status, T, int32_t);
+  UP(s, p.ext_status, pipe->ext_status, X, int32_t);
+  UP(s, p.task_unatt, pipe->task_unattainable, T, uint8_t);
+  UP(s, p.ext_unatt, pipe->ext_unattainable, X, uint8_t);
+  const auto& d = c->deps;
+  DDeps dd;
+  dd.n_tasks = T; dd.dep_off = d.off.as<int64_t>(); dd.dep_kind = d.kind.as<uint8_t>(); dd.dep_ref = d.ref.as<int32_t>();
+  dd.dep_want = d.want.as<uint8_t>(); dd.task_state = d.state.as<uint8_t>(); dd.task_pre = d.pre.as<uint8_t>();
+  dd.ext_state = d.ext.as<uint8_t>(); dd.n_ext = X;
+  DPipe dp;
+  dp.n_status = pipe->n_status; dp.dep_status = p.dep_status.as<int32_t>(); dp.task_status = p.task_status.as<int32_t>();
+  dp.ext_status = p.ext_status.as<int32_t>(); dp.task_unatt = p.task_unatt.as<uint8_t>(); dp.ext_unatt = p.ext_unatt.as<uint8_t>();
+  k_pl_deps<<<grid_for(T, 256), 256, 0, s>>>(dd, dp, c->deps.met.as<uint8_t>(), c->b_err.as<int>());
+  c->launches++;
+  CK(cudaGetLastError());
+  return EVG_OK;
+}
+
+// The device-side range checks of the finder pass, as one message (err bit 1: project row / dep_ref, bit 2: status id).
+static int finder_bad(int bad) {
+  if (bad & 2) return fail(EVG_ERR_INVALID, "a status id of the evg_pipeline_in is outside [0, n_status)");
+  return fail(EVG_ERR_INVALID, "a project row or dep_ref is out of range");
+}
+
+// evg_find_runnable_batch and evg_find_runnable_ex (pipe == NULL: the former)
+static int find_runnable(evg_ctx* c, const evg_runnable_in* in, const evg_pipeline_in* pipe, int32_t* runnable, int64_t* count) {
   if (!c || !in) return fail(EVG_ERR_INVALID, "evg_find_runnable_batch: null argument");
   LOCK(c);
   const int64_t T = in->n_tasks;
@@ -2229,8 +2506,8 @@ int evg_find_runnable_batch(evg_ctx* c, const evg_runnable_in* in, int32_t* runn
   if (D == 0) return T == 0 ? EVG_OK : fail(EVG_ERR_INVALID, "tasks without distros");
   if (!count || (T > 0 && !runnable)) return fail(EVG_ERR_INVALID, "null output");
   DRunnable r;
-  bool any_deps;
-  int rc = stage_finder(c, in, &r, &any_deps);
+  bool any_deps, any_pipe = false, pipe_deps = false;
+  int rc = stage_finder(c, in, &r, &any_deps, pipe, &any_pipe, &pipe_deps);
   if (rc != EVG_OK) return rc;
   if (any_deps && T > 0 && (!in->deps || in->deps->n_tasks != T)) return fail(EVG_ERR_INVALID, "a finder checks dependencies but deps is null or of another size");
   cudaStream_t s = c->stream;
@@ -2241,9 +2518,17 @@ int evg_find_runnable_batch(evg_ctx* c, const evg_runnable_in* in, int32_t* runn
   if (any_deps && T > 0) {
     rc = deps_to_device(c, in->deps, 1);
     if (rc != EVG_OK) return rc;
+    if (pipe_deps) {
+      rc = pipeline_deps(c, in->deps, pipe);
+      if (rc != EVG_OK) return rc;
+    }
     r.met = c->deps.met.as<uint8_t>();
   }
-  k_runnable<<<unsigned(D), 256, 0, s>>>(r, c->pf.kept.as<int32_t>(), c->pf.count.as<int64_t>(), c->b_err.as<int>());
+  if (any_pipe)
+    k_runnable_pipe<<<unsigned(D), 256, 0, s>>>(r, c->pl.project_raw.as<uint8_t>(), c->pf.kept.as<int32_t>(), c->pf.count.as<int64_t>(),
+                                                c->b_err.as<int>());
+  else
+    k_runnable<<<unsigned(D), 256, 0, s>>>(r, c->pf.kept.as<int32_t>(), c->pf.count.as<int64_t>(), c->b_err.as<int>());
   c->launches++;
   CK(cudaGetLastError());
   int bad = 0;
@@ -2251,8 +2536,14 @@ int evg_find_runnable_batch(evg_ctx* c, const evg_runnable_in* in, int32_t* runn
   CK(cudaMemcpyAsync(count, c->pf.count.p, sizeof(int64_t) * size_t(D), cudaMemcpyDeviceToHost, s));
   CK(cudaMemcpyAsync(&bad, c->b_err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
-  if (bad) return fail(EVG_ERR_INVALID, "a project row or dep_ref is out of range");
+  if (bad) return finder_bad(bad);
   return EVG_OK;
+}
+int evg_find_runnable_batch(evg_ctx* c, const evg_runnable_in* in, int32_t* runnable, int64_t* count) {
+  return find_runnable(c, in, nullptr, runnable, count);
+}
+int evg_find_runnable_ex(evg_ctx* c, const evg_runnable_in* in, const evg_pipeline_in* pipe, int32_t* runnable, int64_t* count) {
+  return find_runnable(c, in, pipe, runnable, count);
 }
 
 // --------------------------------------------------------------------------
@@ -2577,9 +2868,10 @@ static int compose_tick(evg_ctx* c, EdMap m, const DTasks& O, const DTasks& In, 
 // --------------------------------------------------------------------------
 // evg_plan_from_finder: finder -> dependency predicate -> compaction -> resident planner inputs, all on the device
 // --------------------------------------------------------------------------
-int evg_plan_from_finder(evg_ctx* c, const evg_runnable_in* in, const evg_task_soa* cand, const evg_distro_table* distros,
-                         const evg_host_soa* hosts, const int64_t* host_off, const evg_alloc_cfg* acfg, const int64_t* dep_finished_ns,
-                         int64_t now_ns, int32_t* runnable, int64_t* count) {
+// evg_plan_from_finder and evg_plan_from_finder_ex (pipe == NULL: the former)
+static int plan_from_finder(evg_ctx* c, const evg_runnable_in* in, const evg_pipeline_in* pipe, const evg_task_soa* cand,
+                            const evg_distro_table* distros, const evg_host_soa* hosts, const int64_t* host_off, const evg_alloc_cfg* acfg,
+                            const int64_t* dep_finished_ns, int64_t now_ns, int32_t* runnable, int64_t* count) {
   if (!c || !in || !cand || !distros) return fail(EVG_ERR_INVALID, "evg_plan_from_finder: null argument");
   LOCK(c);
   const int64_t T = in->n_tasks, E = cand->n_edges;
@@ -2602,8 +2894,8 @@ int evg_plan_from_finder(evg_ctx* c, const evg_runnable_in* in, const evg_task_s
   std::future<int64_t> dep_off_bad;
   if (E > 0 && T > 0) dep_off_bad = std::async(std::launch::async | std::launch::deferred, csr_bad_row, cand->dep_off, T, E);
   DRunnable r;
-  bool any_deps;
-  int rc = stage_finder(c, in, &r, &any_deps);
+  bool any_deps, any_pipe = false, pipe_deps = false;
+  int rc = stage_finder(c, in, &r, &any_deps, pipe, &any_pipe, &pipe_deps);
   if (rc != EVG_OK) return rc;
   for (int32_t d = 0; d <= D; d++)
     if (in->task_off[d] != distros->task_off[d]) return fail(EVG_ERR_INVALID, "the finder table and the distro table cut the candidates differently at distro %d", d);
@@ -2619,10 +2911,18 @@ int evg_plan_from_finder(evg_ctx* c, const evg_runnable_in* in, const evg_task_s
   // 1. Task.DependenciesMet / AllDependenciesSatisfied of every candidate, with the DependenciesMetTime stamps
   rc = deps_to_device(c, in->deps, 1, dep_finished_ns, now_ns, /*want_stamp=*/true);
   if (rc != EVG_OK) return rc;
+  if (pipe_deps) {
+    rc = pipeline_deps(c, in->deps, pipe);
+    if (rc != EVG_OK) return rc;
+  }
   // 2. the finders
   auto& pf = c->pf;
   r.met = c->deps.met.as<uint8_t>();
-  k_runnable<<<unsigned(D), 256, 0, s>>>(r, pf.kept.as<int32_t>(), pf.count.as<int64_t>(), c->b_err.as<int>());
+  if (any_pipe)
+    k_runnable_pipe<<<unsigned(D), 256, 0, s>>>(r, c->pl.project_raw.as<uint8_t>(), pf.kept.as<int32_t>(), pf.count.as<int64_t>(),
+                                                c->b_err.as<int>());
+  else
+    k_runnable<<<unsigned(D), 256, 0, s>>>(r, pf.kept.as<int32_t>(), pf.count.as<int64_t>(), c->b_err.as<int>());
   c->launches++;
   CK(cudaGetLastError());
   // 3. the only thing the host needs before the planner can be routed: how many tasks each distro kept
@@ -2631,7 +2931,7 @@ int evg_plan_from_finder(evg_ctx* c, const evg_runnable_in* in, const evg_task_s
   CK(cudaMemcpyAsync(&bad, c->b_err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
   if (runnable) CK(cudaMemcpyAsync(runnable, pf.kept.p, sizeof(int32_t) * size_t(T), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
-  if (bad) return fail(EVG_ERR_INVALID, "a project row or dep_ref is out of range");
+  if (bad) return finder_bad(bad);
   rc = dep_off_bad.valid() ? check_csr(dep_off_bad.get(), T, "evg_plan_from_finder: the candidate dep_off") : EVG_OK;
   if (rc != EVG_OK) return rc;
   std::vector<int64_t> new_off(size_t(D) + 1, 0);
@@ -2649,13 +2949,43 @@ int evg_plan_from_finder(evg_ctx* c, const evg_runnable_in* in, const evg_task_s
     UP(s, pf.dep_idx, cand->dep_idx, E, int32_t);
     O.n_edges = E; O.dep_off = pf.dep_off.as<int64_t>(); O.dep_idx = pf.dep_idx.as<int32_t>();
   }
-  k_apply_deps<<<grid_for(T, 256), 256, 0, s>>>(T, c->deps.met.as<uint8_t>(), c->deps.stamp.as<int64_t>(), pf.cand.flags.as<uint32_t>(),
-                                                pf.cand.wb.as<int64_t>());
   auto& e = c->ed;
   CK(e.keep.ensure(sizeof(int32_t) * size_t(T + 1)));
   CK(cudaMemsetAsync(e.keep.p, 0, sizeof(int32_t) * size_t(T), s));
   k_kept_mask<<<grid_for(T, 256), 256, 0, s>>>(T, D, pf.task_off.as<int64_t>(), pf.kept.as<int32_t>(), e.keep.as<int32_t>());
-  c->launches += 2;
+  c->launches++;
+  if (any_pipe) {
+    // what the pipeline distros' planner receives: their verdicts (k_pl_plan needs the keep mask), and no candidate
+    // edges for EVG_FINDER_PIPELINE rows (compose_tick then re-indexes the rest as for any finder)
+    const auto& d = c->deps;
+    DDeps dd;
+    dd.n_tasks = T; dd.dep_off = d.off.as<int64_t>(); dd.dep_kind = d.kind.as<uint8_t>(); dd.dep_ref = d.ref.as<int32_t>();
+    dd.dep_want = d.want.as<uint8_t>(); dd.task_state = d.state.as<uint8_t>(); dd.task_pre = d.pre.as<uint8_t>();
+    dd.ext_state = d.ext.as<uint8_t>(); dd.n_ext = in->deps->n_ext;
+    const int64_t* fin = dep_finished_ns && in->deps->n_deps > 0 ? d.fin.as<int64_t>() : nullptr;
+    k_pl_plan<<<grid_for(T, 256), 256, 0, s>>>(dd, D, pf.task_off.as<int64_t>(), pf.finder.as<uint8_t>(), e.keep.as<int32_t>(),
+                                               c->deps.met.as<uint8_t>(), fin, now_ns, c->deps.stamp.as<int64_t>());
+    c->launches++;
+    if (pipe_deps && E > 0) {
+      auto& p = c->pl;
+      CK(p.edge_cnt.ensure(sizeof(int32_t) * size_t(T + 1)));
+      CK(p.dep_off.ensure(sizeof(int64_t) * size_t(T + 1)));
+      CK(p.scan_sum.ensure(sizeof(int64_t) * size_t((T + 1023) / 1024 + 1)));
+      k_pl_edge_count<<<grid_for(T, 256), 256, 0, s>>>(T, D, pf.task_off.as<int64_t>(), pf.finder.as<uint8_t>(), pf.dep_off.as<int64_t>(),
+                                                       p.edge_cnt.as<int32_t>());
+      c->launches++;
+      scan_counts(c, p.edge_cnt.as<int32_t>(), T, p.dep_off.as<int64_t>(), p.scan_sum.as<int64_t>());
+      // the kept edges fit in the candidates' E: no count has to reach the host
+      CK(p.dep_idx.ensure(sizeof(int32_t) * size_t(E)));
+      k_pl_edge_write<<<grid_for(T, 256), 256, 0, s>>>(T, pf.dep_off.as<int64_t>(), pf.dep_idx.as<int32_t>(), p.dep_off.as<int64_t>(),
+                                                       p.dep_idx.as<int32_t>());
+      c->launches++;
+      O.dep_off = p.dep_off.as<int64_t>(); O.dep_idx = p.dep_idx.as<int32_t>();
+    }
+  }
+  k_apply_deps<<<grid_for(T, 256), 256, 0, s>>>(T, c->deps.met.as<uint8_t>(), c->deps.stamp.as<int64_t>(), pf.cand.flags.as<uint32_t>(),
+                                                pf.cand.wb.as<int64_t>());
+  c->launches++;
   CK(e.ins_off.ensure(sizeof(int64_t) * size_t(D + 1)));
   CK(cudaMemsetAsync(e.ins_off.p, 0, sizeof(int64_t) * size_t(D + 1), s));
   // 5. the kept candidates become the resident tick, in the context's own columns
@@ -2675,6 +3005,16 @@ int evg_plan_from_finder(evg_ctx* c, const evg_runnable_in* in, const evg_task_s
   CK(cudaStreamSynchronize(s));
   c->editable = true;
   return EVG_OK;
+}
+int evg_plan_from_finder(evg_ctx* c, const evg_runnable_in* in, const evg_task_soa* cand, const evg_distro_table* distros,
+                         const evg_host_soa* hosts, const int64_t* host_off, const evg_alloc_cfg* acfg, const int64_t* dep_finished_ns,
+                         int64_t now_ns, int32_t* runnable, int64_t* count) {
+  return plan_from_finder(c, in, nullptr, cand, distros, hosts, host_off, acfg, dep_finished_ns, now_ns, runnable, count);
+}
+int evg_plan_from_finder_ex(evg_ctx* c, const evg_runnable_in* in, const evg_pipeline_in* pipe, const evg_task_soa* cand,
+                            const evg_distro_table* distros, const evg_host_soa* hosts, const int64_t* host_off, const evg_alloc_cfg* acfg,
+                            const int64_t* dep_finished_ns, int64_t now_ns, int32_t* runnable, int64_t* count) {
+  return plan_from_finder(c, in, pipe, cand, distros, hosts, host_off, acfg, dep_finished_ns, now_ns, runnable, count);
 }
 
 // --------------------------------------------------------------------------

@@ -275,8 +275,12 @@ class Engine:
         runnable = self._out("runnable", table.n_tasks, np.int32)
         count = self._out("runnable_count", table.n_distros, np.int64)
         st, keep = table.struct()
-        L.check(self.lib.evg_find_runnable_batch(self.ctx, C.byref(st), L.ptr(runnable) if table.n_tasks else None,
-                                                 L.ptr(count) if table.n_distros else None))
+        outs = (L.ptr(runnable) if table.n_tasks else None, L.ptr(count) if table.n_distros else None)
+        if table.pipe is None:
+            L.check(self.lib.evg_find_runnable_batch(self.ctx, C.byref(st), *outs))
+        else:  # evg_find_runnable_ex: the pipeline finder's tables ride along
+            ps = table.pipe.struct()
+            L.check(self.lib.evg_find_runnable_ex(self.ctx, C.byref(st), C.byref(ps), *outs))
         del keep
         return runnable, count
 
@@ -295,9 +299,13 @@ class Engine:
         if hosts is not None:
             hs = hosts.struct()
             hargs = (C.byref(hs), L.ptr(hosts.host_off), L.ptr(hosts.cfg) if hosts.cfg.shape[0] else None)
-        L.check(self.lib.evg_plan_from_finder(self.ctx, C.byref(st), C.byref(ts), C.byref(ds), *hargs,
-                                              L.ptr(fin) if fin is not None and fin.shape[0] else None, int(now),
-                                              L.ptr(runnable) if table.n_tasks else None, L.ptr(count) if table.n_distros else None))
+        rest = (*hargs, L.ptr(fin) if fin is not None and fin.shape[0] else None, int(now),
+                L.ptr(runnable) if table.n_tasks else None, L.ptr(count) if table.n_distros else None)
+        if table.pipe is None:
+            L.check(self.lib.evg_plan_from_finder(self.ctx, C.byref(st), C.byref(ts), C.byref(ds), *rest))
+        else:  # evg_plan_from_finder_ex
+            ps = table.pipe.struct()
+            L.check(self.lib.evg_plan_from_finder_ex(self.ctx, C.byref(st), C.byref(ps), C.byref(ts), C.byref(ds), *rest))
         del keep
         self._n_tasks, self._n_distros, self._n_groups = int(count.sum()), distros.n_distros, distros.n_groups
         self._has_hosts = hosts is not None
@@ -712,9 +720,10 @@ def dependencies_met(batch: Sequence[Tuple[M.Distro, List[M.Task]]], *, engine: 
 def find_runnable_tasks(batch: Sequence[Tuple[M.Distro, List[M.Task]]], project_refs: Sequence[M.ProjectRef], *,
                         finder: str = "legacy", dependency_db: Optional[Dict[str, M.Task]] = None,
                         engine: Optional[Engine] = None) -> List[List[M.Task]]:
-    """LegacyFindRunnableTasks / AlternateTaskFinder / ParallelTaskFinder (scheduler/task_finder.go:40-317) for every
-    distro of the tick: `batch` holds each distro's candidates (the rows the tasks collection has for it), the result
-    the tasks each finder returns, in candidate order."""
+    """LegacyFindRunnableTasks / AlternateTaskFinder / ParallelTaskFinder (scheduler/task_finder.go:40-317) or
+    RunnableTasksPipeline (finder="pipeline", :34-36) for every distro of the tick: `batch` holds each distro's
+    candidates (the rows the tasks collection has for it), the result the tasks each finder returns, in candidate order.
+    The pipeline returns the candidates themselves here; pipeline_returned_tasks gives them as the aggregation decodes them."""
     eng = engine or default_engine()
     table = S.marshal_runnable(batch, project_refs, finder, dependency_db)
     runnable, count = eng.find_runnable_batch(table)
@@ -730,7 +739,8 @@ def plan_candidates(batch: Sequence[Tuple[M.Distro, List[M.Task]]], project_refs
                     engine: Optional[Engine] = None):
     """The finder -> checkDependenciesMet -> PrioritizeTasks hand-over of scheduler.PlanDistro (wrapper.go:60-118,
     scheduler.go:56-168) without the host in the middle: `batch` holds every distro's CANDIDATES; the device filters them,
-    evaluates their dependencies, compacts the planner's columns and plans (evg_plan_from_finder).  Returns, per distro,
+    evaluates their dependencies, compacts the planner's columns and plans (evg_plan_from_finder; finder="pipeline":
+    evg_plan_from_finder_ex, which plans the kept tasks as pipeline_returned_tasks gives them).  Returns, per distro,
     (ranked kept tasks with TotalValue stamped, DistroQueueInfo)."""
     eng = engine or default_engine()
     table = S.marshal_runnable(batch, project_refs, finder, dependency_db)
@@ -855,6 +865,39 @@ def LegacyFindRunnableTasks(d: M.Distro, candidates: List[M.Task], project_refs:
 def AlternateTaskFinder(d: M.Distro, candidates: List[M.Task], project_refs: Sequence[M.ProjectRef], **kw) -> List[M.Task]:
     """scheduler/task_finder.go:108-197 for one distro."""
     return find_runnable_tasks([(d, candidates)], project_refs, finder="alternate", **kw)[0]
+
+
+def ParallelTaskFinder(d: M.Distro, candidates: List[M.Task], project_refs: Sequence[M.ProjectRef], **kw) -> List[M.Task]:
+    """scheduler/task_finder.go:199-317 for one distro (it filters as AlternateTaskFinder does)."""
+    return find_runnable_tasks([(d, candidates)], project_refs, finder="parallel", **kw)[0]
+
+
+def RunnableTasksPipeline(d: M.Distro, candidates: List[M.Task], project_refs: Sequence[M.ProjectRef], **kw) -> List[M.Task]:
+    """scheduler/task_finder.go:34-36 (task.FindHostRunnable, model/task/db.go:887-1066) for one distro, the tasks as
+    the aggregation returns them (pipeline_returned_tasks).  `project_refs` are the raw project_ref documents; the
+    distro's ValidProjects must be those of its stored document ([] when there is none)."""
+    return pipeline_returned_tasks(d, find_runnable_tasks([(d, candidates)], project_refs, finder="pipeline", **kw)[0])
+
+
+def GetTaskFinder(version: str):
+    """scheduler/task_finder.go:19-32: the finder of FinderSettings.Version; an unknown name falls back to legacy."""
+    return {"parallel": ParallelTaskFinder, "legacy": LegacyFindRunnableTasks, "pipeline": RunnableTasksPipeline,
+            "alternate": AlternateTaskFinder}.get(version, LegacyFindRunnableTasks)
+
+
+def pipeline_returned_tasks(d: M.Distro, kept: Sequence[M.Task]) -> List[M.Task]:
+    """The pipeline finder's kept tasks as PlanDistro receives them (copies):
+    - with removeDeps (the distro is not revised-with-dependencies): DependsOn is empty.  $first: $$ROOT after
+      $unwind depends_on leaves one sub-document, which mgo skips when it decodes into []Dependency;
+    - otherwise: every DependsOn entry without Unattainable ($project of db.go:916-921)."""
+    import copy
+    out = []
+    remove_deps = d.dispatcher_settings.version != M.DISPATCHER_VERSION_REVISED_WITH_DEPENDENCIES
+    for t in kept:
+        c = copy.copy(t)
+        c.depends_on = [] if remove_deps else [M.Dependency(x.task_id, x.status, False, x.finished_at) for x in t.depends_on]
+        out.append(c)
+    return out
 
 
 def get_expected_durations_for_window(tasks: Sequence[M.Task], window_start: int, window_end: int, *,

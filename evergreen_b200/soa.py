@@ -646,6 +646,7 @@ class RunnableTable:
     valid_idx: np.ndarray
     finder: np.ndarray
     deps: Optional[DepsTable]
+    pipe: Optional["PipelineTable"] = None  # what the pipeline finder reads besides (evg_pipeline_in); None: no pipeline distro
 
     @property
     def n_tasks(self) -> int:
@@ -700,12 +701,72 @@ def project_bits(p: M.ProjectRef) -> int:
             (L.EVG_PF_PATCHING_DISABLED if p.patching_disabled else 0))
 
 
+@dataclass
+class PipelineTable:
+    """evg_pipeline_in: interned status strings of the candidates, of their dependency entries and of the external
+    dependency documents, the "has an unattainable depends_on entry" bits, and the raw project_ref bits."""
+    n_status: int
+    dep_status: np.ndarray         # int32 per evg_deps_in entry: Dependency.Status
+    task_status: np.ndarray        # int32 per candidate: Task.Status
+    ext_status: np.ndarray         # int32 per external row
+    task_unattainable: np.ndarray  # uint8 per candidate
+    ext_unattainable: np.ndarray   # uint8 per external row
+    project_raw: np.ndarray        # uint8 EVG_PR_* per project row
+
+    def struct(self) -> L.PipelineInStruct:
+        s = L.PipelineInStruct()
+        s.n_status = int(self.n_status)
+        nz = lambda a: L.ptr(a) if a.shape[0] else None  # noqa: E731
+        s.dep_status, s.task_status, s.ext_status = nz(self.dep_status), nz(self.task_status), nz(self.ext_status)
+        s.task_unattainable, s.ext_unattainable = nz(self.task_unattainable), nz(self.ext_unattainable)
+        s.project_raw = nz(self.project_raw)
+        return s
+
+
+def project_raw_bits(p: M.ProjectRef) -> int:
+    """EVG_PR_* of the project_ref DOCUMENT as stored (model/project_ref.go:52-59): enabled is bool,omitempty (stored only
+    when true), dispatching_disabled and patching_disabled are *bool,omitempty (stored only when set)."""
+    return ((L.EVG_PR_ENABLED if p.enabled else 0) | (L.EVG_PR_DISPATCHING_DISABLED if p.dispatching_disabled is True else 0) |
+            (L.EVG_PR_PATCHING_FALSE if p.patching_disabled is False else 0))
+
+
+def marshal_pipeline(batch: Sequence[tuple], project_refs: Sequence[M.ProjectRef],
+                     dependency_db: Optional[Dict[str, M.Task]] = None) -> PipelineTable:
+    """The evg_pipeline_in of a batch, in marshal_deps' order (its entries and external rows resolve the same way: the
+    distro's own candidates first, then `dependency_db`).  Status strings are interned with the reserved ids first."""
+    ids: Dict[str, int] = {M.TASK_SUCCEEDED: L.EVG_STATUS_SUCCESS, M.TASK_FAILED: L.EVG_STATUS_FAILED,
+                           M.ALL_STATUSES: L.EVG_STATUS_ANY}
+    intern = lambda x: ids.setdefault(x, len(ids))  # noqa: E731
+    unatt = lambda t: int(any(d.unattainable for d in t.depends_on))  # noqa: E731
+    db = dependency_db or {}
+    dep_status, task_status, task_un, ext_status, ext_un = [], [], [], [], []
+    ext_seen = set()
+    for _, tasks in batch:
+        index = {t.id for t in tasks}
+        for t in tasks:
+            task_status.append(intern(t.status))
+            task_un.append(unatt(t))
+            for d in t.depends_on:
+                dep_status.append(intern(d.status))
+                if d.task_id not in index and d.task_id in db and d.task_id not in ext_seen:
+                    ext_seen.add(d.task_id)
+                    ext_status.append(intern(db[d.task_id].status))
+                    ext_un.append(unatt(db[d.task_id]))
+    return PipelineTable(len(ids), np.array(dep_status, np.int32), np.array(task_status, np.int32),
+                         np.array(ext_status, np.int32), np.array(task_un, np.uint8), np.array(ext_un, np.uint8),
+                         np.array([project_raw_bits(p) for p in project_refs], np.uint8))
+
+
 def marshal_runnable(batch: Sequence[tuple], project_refs: Sequence[M.ProjectRef], finder: str = "legacy",
                      dependency_db: Optional[Dict[str, M.Task]] = None) -> RunnableTable:
     """[(Distro, [candidate Task])] + the project-ref cache (getProjectRefCache, task_finder.go:46) -> RunnableTable.
-    `finder`: "legacy" (LegacyFindRunnableTasks) or "alternate" (AlternateTaskFinder / ParallelTaskFinder)."""
+    `finder`: "legacy" (LegacyFindRunnableTasks), "alternate" (AlternateTaskFinder / ParallelTaskFinder) or "pipeline"
+    (RunnableTasksPipeline: `project_refs` are then the raw project_ref documents, and the table carries a
+    PipelineTable)."""
     prow = {p.id: i for i, p in enumerate(project_refs)}
-    flavour = {"legacy": L.EVG_FINDER_LEGACY, "alternate": L.EVG_FINDER_ALTERNATE, "parallel": L.EVG_FINDER_ALTERNATE}[finder]
+    flavour = {"legacy": L.EVG_FINDER_LEGACY, "alternate": L.EVG_FINDER_ALTERNATE, "parallel": L.EVG_FINDER_ALTERNATE,
+               "pipeline": L.EVG_FINDER_PIPELINE}[finder]
+    no_deps = L.EVG_FINDER_PIPELINE_NO_DEPS if finder == "pipeline" else L.EVG_FINDER_NO_DEPS
     task_off, valid_off, valid_idx, fnd, sched, proj = [0], [0], [], [], [], []
     for d, tasks in batch:
         for t in tasks:
@@ -714,12 +775,12 @@ def marshal_runnable(batch: Sequence[tuple], project_refs: Sequence[M.ProjectRef
         task_off.append(len(sched))
         valid_idx.extend(prow.get(name, -1) for name in d.valid_projects)
         valid_off.append(len(valid_idx))
-        fnd.append(L.EVG_FINDER_NO_DEPS
-                   if d.dispatcher_settings.version == M.DISPATCHER_VERSION_REVISED_WITH_DEPENDENCIES else flavour)
-    deps = marshal_deps(batch, dependency_db) if any(f != L.EVG_FINDER_NO_DEPS for f in fnd) else None
+        fnd.append(no_deps if d.dispatcher_settings.version == M.DISPATCHER_VERSION_REVISED_WITH_DEPENDENCIES else flavour)
+    deps = marshal_deps(batch, dependency_db) if any(f != no_deps for f in fnd) else None
+    pipe = marshal_pipeline(batch, project_refs, dependency_db) if finder == "pipeline" else None
     return RunnableTable(np.array(task_off, np.int64), np.array(sched, np.uint8), np.array(proj, np.int32),
                          np.array([project_bits(p) for p in project_refs], np.uint8), np.array(valid_off, np.int64),
-                         np.array(valid_idx, np.int32), np.array(fnd, np.uint8), deps)
+                         np.array(valid_idx, np.int32), np.array(fnd, np.uint8), deps, pipe)
 
 
 # ---------------------------------------------------------------------------

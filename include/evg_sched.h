@@ -458,6 +458,12 @@ int evg_download_deps(evg_ctx* ctx, uint8_t* met, int64_t* met_time_ns);
 #define EVG_FINDER_NO_DEPS 0    /* DispatcherSettings.Version == "revised-with-dependencies": dependencies are not filtered (task_finder.go:85) */
 #define EVG_FINDER_LEGACY 1     /* LegacyFindRunnableTasks: Task.DependenciesMet, with the HasDependenciesMet short-circuit */
 #define EVG_FINDER_ALTERNATE 2  /* AlternateTaskFinder / ParallelTaskFinder: Task.AllDependenciesSatisfied (task.go:795-821), no short-circuit */
+/* RunnableTasksPipeline (task.FindHostRunnable, model/task/db.go:887-1066): only through the *_ex entry points, which
+ * take an evg_pipeline_in.  Project gating reads the RAW project_ref document (evg_pipeline_in.project_raw), not the
+ * merged ref of project_flags: enabled stored true, dispatching_disabled not true, and a PatchRequesters task needs
+ * patching_disabled stored false (no hidden-project exemption). */
+#define EVG_FINDER_PIPELINE 3          /* removeDeps: the $graphLookup dependency filter (db.go:923-996) */
+#define EVG_FINDER_PIPELINE_NO_DEPS 4  /* DispatcherSettings.Version == "revised-with-dependencies" on the pipeline finder */
 
 /* Every candidate task of every distro (the rows task.FindHostSchedulable would be asked about), concatenated. */
 typedef struct {
@@ -499,6 +505,57 @@ int evg_find_runnable_batch(evg_ctx* ctx, const evg_runnable_in* in, int32_t* ru
 int evg_plan_from_finder(evg_ctx* ctx, const evg_runnable_in* in, const evg_task_soa* candidates, const evg_distro_table* distros,
                          const evg_host_soa* hosts, const int64_t* host_off, const evg_alloc_cfg* acfg,
                          const int64_t* dep_finished_ns, int64_t now_ns, int32_t* runnable, int64_t* count);
+
+/* ---- the pipeline finder (RunnableTasksPipeline, scheduler/task_finder.go:34-36) ---- */
+
+/* Status strings are interned by the shim; these ids are reserved. */
+#define EVG_STATUS_SUCCESS 0 /* "success" */
+#define EVG_STATUS_FAILED 1  /* "failed" */
+#define EVG_STATUS_ANY 2     /* "*" (a Dependency.Status only) */
+/* evg_pipeline_in.project_raw: the raw project_ref document the $lookup joins (db.go:998-1028) */
+#define EVG_PR_ENABLED 0x1u              /* enabled stored true */
+#define EVG_PR_DISPATCHING_DISABLED 0x2u /* dispatching_disabled stored true */
+#define EVG_PR_PATCHING_FALSE 0x4u       /* patching_disabled stored false (unset is NOT false: *bool,omitempty) */
+
+/* What the pipeline finder reads that evg_runnable_in cannot express.  The dependency documents are the entries of
+ * in->deps: an EVG_DEP_IN_QUEUE entry's document is candidate dep_ref, an EVG_DEP_EXTERNAL one ext row dep_ref (any
+ * document of the tasks collection, not only the queue's), and EVG_DEP_MISSING means no document has that id.
+ * in->deps->dep_want, task_state, task_pre and ext_state are not read by the pipeline's own filter. */
+typedef struct {
+  int32_t n_status;                 /* interned status strings: ids 0 .. n_status-1, n_status >= 3 */
+  int32_t _reserved;
+  const int32_t* dep_status;        /* deps->n_deps: Dependency.Status */
+  const int32_t* task_status;       /* n_tasks: Task.Status of each candidate */
+  const int32_t* ext_status;        /* deps->n_ext: Task.Status of each external document */
+  const uint8_t* task_unattainable; /* n_tasks: 1 when some entry of the candidate's own depends_on has unattainable: true */
+  const uint8_t* ext_unattainable;  /* deps->n_ext: the same for each external document */
+  const uint8_t* project_raw;       /* n_projects: EVG_PR_* of the raw project_ref document of each project row */
+} evg_pipeline_in;
+
+/* evg_find_runnable_batch with the pipeline finder available to any distro.  For an EVG_FINDER_PIPELINE distro a
+ * candidate passes schedulableHostTasksQuery and ValidProjects as the other finders, the raw project gating above, and
+ * the dependency filter: every DependsOn entry whose document EXISTS is satisfied -- its Status equals the document's
+ * Status exactly, or it is "*" and the document is "success" / "failed" or has an unattainable depends_on entry --
+ * entries without a document are ignored, a candidate whose entries ALL lack a document is dropped, one without
+ * DependsOn is kept; OverrideDependencies and DependenciesMetTime do not help.  EVG_FINDER_PIPELINE_NO_DEPS distros
+ * apply the gating without the dependency filter.  Output order: candidate order, as for the other finders.
+ * pipe == NULL behaves exactly like evg_find_runnable_batch.  EVG_ERR_INVALID: a pipeline code with pipe == NULL, a
+ * pipeline distro without in->deps, a status id outside [0, n_status), n_status < 3.  Host pointers. */
+int evg_find_runnable_ex(evg_ctx* ctx, const evg_runnable_in* in, const evg_pipeline_in* pipe, int32_t* runnable,
+                         int64_t* count);
+
+/* evg_plan_from_finder with the pipeline finder available (pipe == NULL: exactly evg_plan_from_finder).  What the
+ * planner receives is what PlanDistro hands PrioritizeTasks after the aggregation's decode:
+ *   - EVG_FINDER_PIPELINE: a kept task's DependsOn decodes empty ($unwind leaves one sub-document, which mgo skips), so
+ *     its in-queue edges are dropped and EVG_TF_DEPS_MET is set without a DependenciesMetTime stamp;
+ *   - EVG_FINDER_PIPELINE_NO_DEPS: DependenciesMet and its stamp are evaluated after the finder, with the Blocked()
+ *     state of a dependency that is a KEPT candidate of the same distro ignored ($project strips
+ *     depends_on.unattainable from the returned tasks, db.go:916-921, and they form the depCache, scheduler.go:61-64).
+ * Everything else as evg_plan_from_finder; the candidate edges of EVG_FINDER_PIPELINE rows are not read. */
+int evg_plan_from_finder_ex(evg_ctx* ctx, const evg_runnable_in* in, const evg_pipeline_in* pipe, const evg_task_soa* candidates,
+                            const evg_distro_table* distros, const evg_host_soa* hosts, const int64_t* host_off,
+                            const evg_alloc_cfg* acfg, const int64_t* dep_finished_ns, int64_t now_ns, int32_t* runnable,
+                            int64_t* count);
 
 /* ---- alias queues: the secondary queue of every distro (SURVEY.md §8 row A21) ---- */
 
