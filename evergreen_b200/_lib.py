@@ -159,6 +159,34 @@ class DurationRowsStruct(C.Structure):
 
 EVG_DR_COMPLETED, EVG_DR_TIMED_OUT = 0x1, 0x2
 DURATION_STAT_DTYPE = np.dtype([("count", np.int64), ("mean_ns", np.float64), ("stddev_ns", np.float64)])
+EVG_DK_NONE = -1
+
+
+def EVG_DK_PAIR(p: int) -> int:
+    return -2 - p
+
+
+EVG_DS_FRESH, EVG_DS_BACKFILL, EVG_DS_HISTORY, EVG_DS_PREVIOUS, EVG_DS_DEFAULT = 0, 1, 2, 3, 4
+DURATION_CACHE_COLUMNS = ("value_ns", "std_ns", "ttl_ns", "collected_ns", "expected_ns", "expected_std_ns")
+
+
+class DurationCacheStruct(C.Structure):
+    _fields_ = [("n_rows", C.c_int64), ("rows", C.c_void_p), ("value_ns", C.c_void_p), ("std_ns", C.c_void_p),
+                ("ttl_ns", C.c_void_p), ("collected_ns", C.c_void_p), ("expected_ns", C.c_void_p),
+                ("expected_std_ns", C.c_void_p), ("key", C.c_void_p)]
+
+
+class DurationInStruct(C.Structure):
+    _fields_ = [("history", C.POINTER(DurationRowsStruct)), ("n_pairs", C.c_int32), ("_reserved", C.c_int32),
+                ("pair_key_off", C.c_void_p), ("tasks", C.POINTER(DurationCacheStruct)),
+                ("hosts", C.POINTER(DurationCacheStruct))]
+
+
+DURATION_OUT_FIELDS = ("avg_ns", "std_ns", "value_ns", "pred_std_ns", "collected_ns", "source")
+
+
+class DurationOutStruct(C.Structure):
+    _fields_ = [(f, C.c_void_p) for f in DURATION_OUT_FIELDS]
 
 
 class LegacySoAStruct(C.Structure):
@@ -224,6 +252,8 @@ SYMBOLS = {
     "evg_find_runnable_batch": (C.c_int, [_P, _P, _P, _P]),
     "evg_find_runnable_ex": (C.c_int, [_P, _P, _P, _P, _P]),
     "evg_expected_durations_batch": (C.c_int, [_P, _P, _P]),
+    "evg_resolve_durations": (C.c_int, [_P, _P, C.c_int64]),
+    "evg_download_durations": (C.c_int, [_P, _P, _P]),
     "evg_prioritize_legacy_batch": (C.c_int, [_P, _P, _P, _P, C.c_int32, _P, _P, _P]),
     "evg_dag_rebuild_batch": (C.c_int, [_P, _P, _P, _P, C.c_int32, _P, _P, _P, _P, _P]),
     "evg_plan_distro": (C.c_int, [_P, _P, _P, C.c_int32, _P, C.c_int64, C.c_uint32, _P]),

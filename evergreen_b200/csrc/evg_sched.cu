@@ -25,6 +25,9 @@
 //   k_pl_deps             the pipeline's $graphLookup dependency filter (db.go:923-996)
 //   k_pl_plan, k_pl_edge_*  what the planner receives from a pipeline distro (evg_plan_from_finder_ex)
 //   k_dur_sum/dev/final   expected-duration statistics (model/task/expected_duration.go:36-96)
+//   k_dur_pair            the single matched key of a (project, build variant) pair (expected_duration.go:54-56)
+//   k_dur_resolve         Task.FetchExpectedDuration per listed row (model/task/task.go:3519-3590) into staging
+//   k_dur_commit          the resolved durations into the resident columns, unless the call found an error
 // No CPU fallback exists in this file: without a device every entry point fails.
 #include <cuda_runtime.h>
 #include <stdarg.h>
@@ -752,6 +755,90 @@ __global__ void __launch_bounds__(256) k_dur_final(DDur X, evg_duration_stat* ou
   out[k] = st;
 }
 
+// The duration cache of a resident tick (evg_resolve_durations).  Pair p's keys are pair_key_off[p] .. [p+1]: a task
+// with DisplayName "" queries the pair without a name filter and gets one document only when ONE of them matched.
+__global__ void __launch_bounds__(256) k_dur_pair(int32_t n_pairs, const int64_t* __restrict__ pair_key_off,
+                                                  const unsigned long long* __restrict__ cnt, int32_t* __restrict__ single) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= n_pairs) return;
+  int32_t k1 = -1;
+  int n = 0;
+  for (int64_t k = pair_key_off[p]; k < pair_key_off[p + 1] && n < 2; k++)
+    if (cnt[k] > 0) { k1 = int32_t(k); n++; }
+  single[p] = n == 1 ? k1 : -1;
+}
+
+// The listed rows of one call: tasks first (n_t), then hosts (n_h).  A NULL row list means rows 0 .. n-1.
+struct DDurRows {
+  int64_t n_t, n_h;
+  const int64_t* trows;
+  const int64_t* hrows;
+  const int64_t* value;
+  const int64_t* pstd;
+  const int64_t* ttl;
+  const int64_t* coll;
+  const int64_t* exp;
+  const int64_t* exp_std;
+  const int32_t* key;
+  int64_t *o_avg, *o_std, *o_value, *o_pstd, *o_coll;
+  uint8_t* o_src;
+};
+
+// One listed row: FetchExpectedDuration with CachedDurationValue.Get and the refresher (task.go:3519-3590,
+// cached_value.go:125-145) against the statistics of its key.  Out-of-range keys set bit 2 of *err.
+__global__ void __launch_bounds__(256) k_dur_resolve(DDurRows R, int32_t n_keys, int32_t n_pairs, const evg_duration_stat* __restrict__ stat,
+                                                     const int32_t* __restrict__ single, int64_t now, int* err) {
+  const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= R.n_t + R.n_h) return;
+  const int64_t value = R.value[i], pstd = R.pstd[i], coll = R.coll[i], e = R.exp[i];
+  const int64_t ttl = R.ttl[i] == 0 ? 8 * kHour : R.ttl[i];  // predictionTTL (task.go:67), unjittered
+  const int32_t key = R.key[i];
+  int32_t doc = -1;  // the key whose statistics the window query returns as its one document
+  if (key >= 0) {
+    if (key >= n_keys) { atomicOr(err, 2); return; }
+    if (stat[key].count > 0) doc = key;
+  } else if (key != EVG_DK_NONE) {
+    const int64_t p = -2 - int64_t(key);
+    if (p >= n_pairs) { atomicOr(err, 2); return; }
+    doc = single[p];
+  }
+  int64_t avg, sd, nv = value, ns = pstd, nc = coll;
+  uint8_t src;
+  if (value == 0 && e != 0) {  // backfill: Value and CollectedAt set, StdDev kept (task.go:3524-3538)
+    avg = e; sd = R.exp_std[i]; nv = e; nc = now - kMinute;
+    src = EVG_DS_BACKFILL;
+  } else if (since(now, coll) < ttl) {
+    avg = value; sd = pstd;
+    src = EVG_DS_FRESH;
+  } else {
+    if (doc < 0) {
+      src = value == 0 ? EVG_DS_DEFAULT : EVG_DS_PREVIOUS;
+      avg = value == 0 ? 10 * kMinute : value; sd = value == 0 ? 0 : pstd;
+    } else {
+      const int64_t a = __double2ll_rz(stat[doc].mean_ns);  // time.Duration(float64) truncates toward zero
+      src = a == 0 ? EVG_DS_DEFAULT : EVG_DS_HISTORY;
+      avg = a == 0 ? 10 * kMinute : a; sd = a == 0 ? 0 : __double2ll_rz(stat[doc].stddev_ns);
+    }
+    nv = avg; ns = sd; nc = now;
+  }
+  R.o_avg[i] = avg; R.o_std[i] = sd; R.o_value[i] = nv; R.o_pstd[i] = ns; R.o_coll[i] = nc; R.o_src[i] = src;
+}
+
+// The resolved rows into the resident columns -- only when the call found no error, so a rejected call leaves the
+// tick as it was without a host round trip in between.
+__global__ void __launch_bounds__(256) k_dur_commit(DDurRows R, const int* __restrict__ err, int64_t* __restrict__ texp,
+                                                    int64_t* __restrict__ hexp, int64_t* __restrict__ hstd) {
+  const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= R.n_t + R.n_h || *err) return;
+  if (i < R.n_t) {
+    texp[R.trows ? R.trows[i] : i] = R.o_avg[i];
+  } else {
+    const int64_t j = i - R.n_t, r = R.hrows ? R.hrows[j] : j;
+    hexp[r] = R.o_avg[i];
+    hstd[r] = R.o_std[i];
+  }
+}
+
 // The 13-field SortingValueBreakdown of the unit each ranked task was emitted
 // from (planner.go:472-476, model/task/task.go:3990-4038); both paths.
 __global__ void __launch_bounds__(256) k_breakdown(DTasks T, DDistros D, DWork W, const uint32_t* run_all, const URec* pay, int64_t now, int any_complex,
@@ -1147,6 +1234,15 @@ struct evg_ctx {
     DevBuf hk, hv, gslot, vslot, fg, fv, pg, pv;  // first-appearance ids of groups and versions per queue
     DevBuf qoff, samp, gout, srow, gsrc, err;  // queue offsets, per-distro samples, group slots, the alias map
   } al;
+  // evg_resolve_durations (the first call allocates these): the staged history, the per-key accumulators and statistics,
+  // the pairs' single keys, the listed rows (tasks, then hosts) and their results, which evg_download_durations returns
+  // while `valid` holds (upload_tasks clears it)
+  struct {
+    DevBuf key, taken, start, finish, flags, acc, stat, pair_off, single;
+    DevBuf rows, in, out, src, err;
+    int64_t n_t = 0, n_h = 0;
+    bool valid = false;
+  } dur;
   DevBuf b_err;
   DevBuf b_route, b_unitv, b_unita, b_unitn, b_unitmask;
   DevBuf b_punt, b_puntcnt;
@@ -1429,6 +1525,7 @@ int upload_tasks(evg_ctx* c, const evg_task_soa* t, const evg_distro_table* dt, 
   c->h_dtileoff.swap(dtile_off);
   c->have_tasks = true;
   c->alias_map = false;  // evg_plan_aliases sets it again after its upload
+  c->dur.valid = false;  // the resolved rows name rows of the previous table
   c->editable = false;  // the entry point that uploaded says whether evg_edit_tasks may follow
   c->alist_valid = false;  // upload_hosts lists the allocator's distros against THIS table
   c->have_hosts = false;
@@ -2407,6 +2504,145 @@ int evg_expected_durations_batch(evg_ctx* c, const evg_duration_rows* in, evg_du
   CK(cudaMemcpyAsync(&bad, c->b_err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   if (bad) return fail(EVG_ERR_INVALID, "a key is out of range");
+  return EVG_OK;
+}
+
+// The host's checks of one evg_duration_cache against a resident table of n rows.
+static int check_duration_cache(const evg_duration_cache* dc, int64_t n, const char* what) {
+  if (dc->n_rows < 0) return fail(EVG_ERR_INVALID, "evg_resolve_durations: negative %s n_rows", what);
+  if (!dc->rows && dc->n_rows != n)
+    return fail(EVG_ERR_INVALID, "evg_resolve_durations: %s rows == NULL but n_rows %lld != %lld resident rows", what,
+                (long long)dc->n_rows, (long long)n);
+  if (dc->n_rows > 0 && (!dc->value_ns || !dc->std_ns || !dc->ttl_ns || !dc->collected_ns || !dc->expected_ns ||
+                         !dc->expected_std_ns || !dc->key))
+    return fail(EVG_ERR_INVALID, "evg_resolve_durations: null %s column", what);
+  if (dc->rows)
+    for (int64_t i = 0; i < dc->n_rows; i++) {
+      const int64_t r = dc->rows[i];
+      if (r < 0 || r >= n || (i > 0 && r <= dc->rows[i - 1]))
+        return fail(EVG_ERR_INVALID, "evg_resolve_durations: %s rows[%lld] = %lld is out of range or not strictly ascending", what,
+                    (long long)i, (long long)r);
+    }
+  return EVG_OK;
+}
+
+int evg_resolve_durations(evg_ctx* c, const evg_duration_in* in, int64_t now_ns) {
+  if (!c) return fail(EVG_ERR_INVALID, "null context");
+  LOCK(c);
+  if (!in) return fail(EVG_ERR_INVALID, "evg_resolve_durations: null argument");
+  if (!c->have_tasks) return fail(EVG_ERR_STATE, "evg_resolve_durations without a resident tick");
+  if (!c->editable)  // the context's own columns: not borrowed ones, not the tick a one-shot call left
+    return fail(EVG_ERR_STATE, c->adopted ? "the resident columns are borrowed (evg_upload_device): resolve on the host instead"
+                                          : "evg_resolve_durations: the resident tick is what a one-shot call left");
+  if (in->hosts && !c->have_hosts) return fail(EVG_ERR_STATE, "evg_resolve_durations: hosts given but the resident tick has none");
+  const evg_duration_rows* h = in->history;
+  const int64_t R = h ? h->n_rows : 0;
+  const int32_t K = h ? h->n_keys : 0, P = in->n_pairs;
+  if (R < 0 || K < 0 || P < 0) return fail(EVG_ERR_INVALID, "evg_resolve_durations: negative sizes");
+  if (R > 0 && (!h->key || !h->time_taken_ns || !h->start_ns || !h->finish_ns || !h->flags))
+    return fail(EVG_ERR_INVALID, "evg_resolve_durations: null history column");
+  if (P > 0 && !in->pair_key_off) return fail(EVG_ERR_INVALID, "evg_resolve_durations: null pair_key_off");
+  if (in->pair_key_off) {
+    const int64_t* o = in->pair_key_off;
+    bool ok = o[0] == 0 && o[P] == K;
+    for (int32_t p = 0; ok && p < P; p++) ok = o[p + 1] >= o[p];
+    if (!ok) return fail(EVG_ERR_INVALID, "evg_resolve_durations: pair_key_off must start at 0, end at n_keys and never decrease");
+  }
+  int rc;
+  if (in->tasks && (rc = check_duration_cache(in->tasks, c->T, "tasks")) != EVG_OK) return rc;
+  if (in->hosts && (rc = check_duration_cache(in->hosts, c->H, "hosts")) != EVG_OK) return rc;
+  CK(cudaSetDevice(c->device));
+  cudaStream_t s = c->stream;
+  auto& d = c->dur;
+  d.valid = false;  // the staging below is overwritten whatever the outcome
+  const int64_t Nt = in->tasks ? in->tasks->n_rows : 0, Nh = in->hosts ? in->hosts->n_rows : 0, N = Nt + Nh;
+  // history -> per-key statistics, on the call's own buffers (evg_expected_durations_batch's scratch is not touched)
+  UP(s, d.key, h ? h->key : nullptr, R, int32_t);
+  UP(s, d.taken, h ? h->time_taken_ns : nullptr, R, int64_t);
+  UP(s, d.start, h ? h->start_ns : nullptr, R, int64_t);
+  UP(s, d.finish, h ? h->finish_ns : nullptr, R, int64_t);
+  UP(s, d.flags, h ? h->flags : nullptr, R, uint8_t);
+  CK(d.acc.ensure(sizeof(unsigned long long) * 4 * size_t(K)));
+  CK(d.stat.ensure(sizeof(evg_duration_stat) * size_t(K)));
+  UP(s, d.pair_off, in->pair_key_off, P > 0 ? P + 1 : 0, int64_t);
+  CK(d.single.ensure(sizeof(int32_t) * size_t(P)));
+  CK(d.err.ensure(sizeof(int)));
+  CK(cudaMemsetAsync(d.err.p, 0, sizeof(int), s));
+  if (K > 0) CK(cudaMemsetAsync(d.acc.p, 0, sizeof(unsigned long long) * 4 * size_t(K), s));
+  // the listed rows: six int64 columns and the key, tasks then hosts; the results: five int64 columns and the source
+  CK(d.rows.ensure(sizeof(int64_t) * size_t(N)));
+  CK(d.in.ensure((sizeof(int64_t) * 6 + sizeof(int32_t)) * size_t(N)));
+  CK(d.out.ensure(sizeof(int64_t) * 5 * size_t(N)));
+  CK(d.src.ensure(size_t(N)));
+  DDurRows X;
+  int64_t* col = d.in.as<int64_t>();
+  X.n_t = Nt; X.n_h = Nh;
+  X.value = col; X.pstd = col + N; X.ttl = col + 2 * N; X.coll = col + 3 * N; X.exp = col + 4 * N; X.exp_std = col + 5 * N;
+  X.key = reinterpret_cast<const int32_t*>(col + 6 * N);
+  int64_t* o = d.out.as<int64_t>();
+  X.o_avg = o; X.o_std = o + N; X.o_value = o + 2 * N; X.o_pstd = o + 3 * N; X.o_coll = o + 4 * N;
+  X.o_src = d.src.as<uint8_t>();
+  X.trows = (in->tasks && in->tasks->rows) ? d.rows.as<int64_t>() : nullptr;
+  X.hrows = (in->hosts && in->hosts->rows) ? d.rows.as<int64_t>() + Nt : nullptr;
+  const evg_duration_cache* seg[2] = {in->tasks, in->hosts};
+  const int64_t base[2] = {0, Nt};
+  for (int k = 0; k < 2; k++) {
+    const evg_duration_cache* dc = seg[k];
+    if (!dc || dc->n_rows == 0) continue;
+    const size_t n = size_t(dc->n_rows), b = size_t(base[k]);
+    if (dc->rows) CK(cudaMemcpyAsync(d.rows.as<int64_t>() + b, dc->rows, 8 * n, cudaMemcpyHostToDevice, s));
+    const int64_t* src[6] = {dc->value_ns, dc->std_ns, dc->ttl_ns, dc->collected_ns, dc->expected_ns, dc->expected_std_ns};
+    for (int j = 0; j < 6; j++) CK(cudaMemcpyAsync(col + size_t(j) * size_t(N) + b, src[j], 8 * n, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(const_cast<int32_t*>(X.key) + b, dc->key, 4 * n, cudaMemcpyHostToDevice, s));
+  }
+  DDur x;
+  x.n_rows = R; x.n_keys = K; x.key = d.key.as<int32_t>(); x.taken = d.taken.as<int64_t>(); x.start = d.start.as<int64_t>();
+  x.finish = d.finish.as<int64_t>(); x.flags = d.flags.as<uint8_t>();
+  x.w0 = h ? h->window_start_ns : 0; x.w1 = h ? h->window_end_ns : 0;
+  x.cnt = d.acc.as<unsigned long long>(); x.sum = x.cnt + K; x.sq_lo = x.sum + K; x.sq_hi = x.sq_lo + K;
+  if (R > 0) {
+    k_dur_sum<<<grid_for(R, 256), 256, 0, s>>>(x, d.err.as<int>());
+    k_dur_dev<<<grid_for(R, 256), 256, 0, s>>>(x);
+  }
+  if (K > 0) k_dur_final<<<grid_for(K, 256), 256, 0, s>>>(x, d.stat.as<evg_duration_stat>());
+  if (P > 0) k_dur_pair<<<grid_for(P, 256), 256, 0, s>>>(P, d.pair_off.as<int64_t>(), x.cnt, d.single.as<int32_t>());
+  if (N > 0) {
+    k_dur_resolve<<<grid_for(N, 256), 256, 0, s>>>(X, K, P, d.stat.as<evg_duration_stat>(), d.single.as<int32_t>(), now_ns, d.err.as<int>());
+    k_dur_commit<<<grid_for(N, 256), 256, 0, s>>>(X, d.err.as<int>(), c->tasks.exp.as<int64_t>(), c->b_hexp.as<int64_t>(),
+                                                   c->b_hstd.as<int64_t>());
+  }
+  CK(cudaGetLastError());
+  int bad = 0;
+  CK(cudaMemcpyAsync(&bad, d.err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));  // the caller's arrays are free again
+  if (bad & 1) return fail(EVG_ERR_INVALID, "evg_resolve_durations: a history key is outside [0, n_keys)");
+  if (bad) return fail(EVG_ERR_INVALID, "evg_resolve_durations: a row's key or pair is out of range");
+  d.n_t = Nt; d.n_h = Nh;
+  d.valid = true;
+  return EVG_OK;
+}
+
+int evg_download_durations(evg_ctx* c, evg_duration_out* tasks, evg_duration_out* hosts) {
+  if (!c) return fail(EVG_ERR_INVALID, "null context");
+  LOCK(c);
+  if (!c->have_tasks || !c->dur.valid) return fail(EVG_ERR_STATE, "evg_download_durations: no evg_resolve_durations on the resident tick's rows");
+  CK(cudaSetDevice(c->device));
+  cudaStream_t s = c->stream;
+  auto& d = c->dur;
+  const int64_t N = d.n_t + d.n_h;
+  const int64_t* o = d.out.as<int64_t>();
+  evg_duration_out* seg[2] = {tasks, hosts};
+  const int64_t base[2] = {0, d.n_t}, cnt[2] = {d.n_t, d.n_h};
+  for (int k = 0; k < 2; k++) {
+    evg_duration_out* q = seg[k];
+    if (!q || cnt[k] == 0) continue;
+    const size_t n = size_t(cnt[k]), b = size_t(base[k]);
+    int64_t* dst[5] = {q->avg_ns, q->std_ns, q->value_ns, q->pred_std_ns, q->collected_ns};
+    for (int j = 0; j < 5; j++)
+      if (dst[j]) CK(cudaMemcpyAsync(dst[j], o + size_t(j) * size_t(N) + b, 8 * n, cudaMemcpyDeviceToHost, s));
+    if (q->source) CK(cudaMemcpyAsync(q->source, d.src.as<uint8_t>() + b, n, cudaMemcpyDeviceToHost, s));
+  }
+  CK(cudaStreamSynchronize(s));
   return EVG_OK;
 }
 

@@ -57,6 +57,7 @@ class Engine:
         self.ctx = h
         self._n_tasks = self._n_distros = self._n_groups = 0
         self._has_hosts = False
+        self._n_dur = (0, 0)  # task and host rows of the last resolve_durations
         self._pinned = {}  # name -> (address, capacity in bytes): result buffers reused across ticks
 
     def close(self) -> None:
@@ -342,6 +343,40 @@ class Engine:
         L.check(self.lib.evg_expected_durations_batch(self.ctx, C.byref(st), L.ptr(out) if rows.n_keys else None))
         return out
 
+    def resolve_durations(self, history: Optional["S.DurationHistory"], now: int, tasks: Optional["S.DurationCache"] = None,
+                          hosts: Optional["S.DurationCache"] = None) -> None:
+        """evg_resolve_durations: Task.FetchExpectedDuration for the listed rows of the resident tick, against the
+        weekly statistics of `history`, written into the resident expected_ns (tasks) and expected_ns / std_ns (hosts)
+        on the device.  None leaves that side as uploaded."""
+        keep = []
+        din = L.DurationInStruct()
+        if history is not None:
+            hs = history.rows.struct()
+            keep.append(hs)
+            din.history = C.pointer(hs)
+            din.n_pairs = history.n_pairs
+            off = np.ascontiguousarray(history.pair_key_off, dtype=np.int64)
+            keep.append(off)
+            din.pair_key_off = L.ptr(off)
+        for name, cache in (("tasks", tasks), ("hosts", hosts)):
+            if cache is not None:
+                cs = cache.normalize().struct()
+                keep.append(cs)
+                setattr(din, name, C.pointer(cs))
+        L.check(self.lib.evg_resolve_durations(self.ctx, C.byref(din), int(now)))
+        self._n_dur = (tasks.n_rows if tasks is not None else 0, hosts.n_rows if hosts is not None else 0)
+        del keep
+
+    def download_durations(self):
+        """evg_download_durations -> (tasks, hosts): dicts of avg_ns, std_ns, value_ns, pred_std_ns, collected_ns and
+        source (EVG_DS_*) per listed row of the last resolve_durations."""
+        res = []
+        for side, n in zip(("tasks", "hosts"), self._n_dur):
+            res.append({f: self._out(f"dur_{side}_{f}", n, np.uint8 if f == "source" else np.int64) for f in L.DURATION_OUT_FIELDS})
+        outs = [L.DurationOutStruct(*[L.ptr(d[f]) if d[f].shape[0] else None for f in L.DURATION_OUT_FIELDS]) for d in res]
+        L.check(self.lib.evg_download_durations(self.ctx, C.byref(outs[0]), C.byref(outs[1])))
+        return res[0], res[1]
+
     def prioritize_legacy_batch(self, table: "S.LegacyTable"):
         """evg_prioritize_legacy_batch: (order, count, status) of CmpBasedTaskPrioritizer over every distro of the table."""
         T, D = table.n_tasks, table.n_distros
@@ -434,15 +469,41 @@ def _upload_with_device_deps(eng: Engine, batch, soa, table, hosts, now: int, de
             k += 1
 
 
+def _resolve_durations_on_device(eng: Engine, tasks: Sequence[M.Task], finished_tasks: Sequence[M.Task], now: int,
+                                 datas: Optional[Sequence[M.HostAllocatorData]] = None,
+                                 running_tasks: Optional[Dict[str, M.Task]] = None) -> None:
+    """PopulateCaches' FetchExpectedDuration for every task of the resident tick (and the running task of every host
+    that `running_tasks` holds) on the device, then the fields the reference leaves on those Task objects."""
+    docs = list(running_tasks.values()) if running_tasks is not None else []
+    hist, _ = S.marshal_duration_history(finished_tasks, (), now)
+    tcache = S.marshal_duration_cache(tasks, hist)
+    hcache, hdocs = (None, [])
+    if running_tasks is not None and datas is not None and docs:
+        hcache, hdocs = S.marshal_running_cache(datas, running_tasks, hist)
+    eng.resolve_durations(hist, now, tcache, hcache)
+    tout, hout = eng.download_durations()
+    S.write_back_durations(tasks, tout)
+    # a task several hosts run is resolved once per host, with the same inputs and result: write it back once
+    seen = set()
+    for i, t in enumerate(hdocs):
+        if id(t) not in seen:
+            seen.add(id(t))
+            S.write_back_durations([t], {f: hout[f][i:i + 1] for f in L.DURATION_OUT_FIELDS})
+
+
 def plan_distros(batch: Sequence[Tuple[M.Distro, List[M.Task]]], now: int, *, engine: Optional[Engine] = None,
                  dependency_db: Optional[Dict[str, M.Task]] = None, breakdown: bool = True,
-                 secondary: bool = False):
+                 secondary: bool = False, finished_tasks: Optional[Sequence[M.Task]] = None):
     """Batched runTunablePlanner minus persistence (scheduler/scheduler.go:34-51):
     returns, per distro, (ranked [Task] with SortingValueBreakdown stamped,
-    DistroQueueInfo)."""
+    DistroQueueInfo).  `finished_tasks`: the task history getExpectedDurationsForWindow reads; when given, every
+    task's expected duration is resolved on the device against it (evg_resolve_durations) instead of on the host, and
+    written back onto the Task objects as FetchExpectedDuration does."""
     eng = engine or default_engine()
-    soa, table, keys = S.marshal_tasks(batch, now, dependency_db)
+    soa, table, keys = S.marshal_tasks(batch, now, dependency_db, resolve_durations=finished_tasks is None)
     _upload_with_device_deps(eng, batch, soa, table, None, now, dependency_db)
+    if finished_tasks is not None:
+        _resolve_durations_on_device(eng, [t for _, ts in batch for t in ts], finished_tasks, now)
     return _ranked_results(eng, batch, table, keys, now, breakdown, secondary)
 
 
@@ -950,14 +1011,24 @@ def GetHostAllocator(name: str) -> HostAllocator:
 
 
 def plan_and_allocate(batch: Sequence[Tuple[M.Distro, List[M.Task], M.HostAllocatorData]], now: int, *,
-                      engine: Optional[Engine] = None, dependency_db: Optional[Dict[str, M.Task]] = None):
+                      engine: Optional[Engine] = None, dependency_db: Optional[Dict[str, M.Task]] = None,
+                      finished_tasks: Optional[Sequence[M.Task]] = None, running_tasks: Optional[Dict[str, M.Task]] = None):
     """The fused tick: distroSchedulerJob + hostAllocatorJob for every distro
     (units/scheduler.go:57-87, units/host_allocator.go:76-196) in one call; the
-    queue info stays on the device between the two halves."""
+    queue info stays on the device between the two halves.  `finished_tasks` as for plan_distros; `running_tasks`
+    (task id -> Task, the documents task.Find(ByIds) returns for the hosts' running tasks, allocator.go:337) have their
+    expected durations resolved on the device too (allocator.go:357-359) and written back.  Both need
+    finished_tasks; None keeps the host's resolution."""
+    if running_tasks is not None and finished_tasks is None:
+        raise ValueError("running_tasks are resolved against finished_tasks")
     eng = engine or default_engine()
-    soa, table, keys = S.marshal_tasks([(d, t) for d, t, _ in batch], now, dependency_db)
-    hosts = S.marshal_hosts([h for _, _, h in batch], [k.group_names for k in keys])
+    datas = [h for _, _, h in batch]
+    soa, table, keys = S.marshal_tasks([(d, t) for d, t, _ in batch], now, dependency_db,
+                                       resolve_durations=finished_tasks is None)
+    hosts = S.marshal_hosts(datas, [k.group_names for k in keys], running_tasks)
     _upload_with_device_deps(eng, batch, soa, table, hosts, now, dependency_db)
+    if finished_tasks is not None:
+        _resolve_durations_on_device(eng, [t for _, ts, _ in batch for t in ts], finished_tasks, now, datas, running_tasks)
     eng.run(now)
     po, ao = eng.download()
     out = []

@@ -343,10 +343,12 @@ class MarshalledDistro:
 
 
 def marshal_tasks(batch: Sequence[tuple], now: int, dependency_db: Optional[Dict[str, M.Task]] = None,
-                  duration_history: Optional[dict] = None, resolve_deps: bool = False):
+                  duration_history: Optional[dict] = None, resolve_deps: bool = False, resolve_durations: bool = True):
     """[(Distro, [Task])] -> (TaskSoA, DistroTable, [MarshalledDistro]).
 
-    Per task this resolves FetchExpectedDuration (PopulateCaches, setup_funcs.go:20-67).  Task.DependenciesMet
+    Per task this resolves FetchExpectedDuration (PopulateCaches, setup_funcs.go:20-67), which writes the task's
+    DurationPrediction back like the reference.  resolve_durations=False leaves the tasks untouched and uploads
+    Task.ExpectedDuration as it is, for callers that resolve the durations on the device (evg_resolve_durations).  Task.DependenciesMet
     (scheduler.go:161-168) is the DEVICE's job: the product path pairs these columns with marshal_deps() and
     Engine.upload_with_deps(), which sets the EVG_TF_DEPS_MET bit and the stamped wait basis on the GPU.
     resolve_deps=True evaluates it here instead (host restatement, kept for tests and for callers of the plain
@@ -364,8 +366,11 @@ def marshal_tasks(batch: Sequence[tuple], now: int, dependency_db: Optional[Dict
         versions: Dict[str, int] = {}
         md = MarshalledDistro()
         for t in tasks:
-            hist = None if duration_history is None else duration_history.get((t.project, t.build_variant, t.display_name))
-            avg, _ = M.fetch_expected_duration(t, now, hist)
+            if resolve_durations:
+                hist = None if duration_history is None else duration_history.get((t.project, t.build_variant, t.display_name))
+                avg, _ = M.fetch_expected_duration(t, now, hist)
+            else:
+                avg = t.expected_duration
             gid = -1
             if t.task_group != "":
                 name = t.get_task_group_string()
@@ -489,10 +494,14 @@ def alloc_cfg_row(data: M.HostAllocatorData) -> tuple:
             data.parent_distro_maximum_hosts if data.parent_distro_maximum_hosts is not None else 0)
 
 
-def marshal_hosts(datas: Sequence[M.HostAllocatorData], group_names: Sequence[Sequence[str]]) -> HostSoA:
+def marshal_hosts(datas: Sequence[M.HostAllocatorData], group_names: Sequence[Sequence[str]],
+                  running_tasks: Optional[Dict[str, M.Task]] = None) -> HostSoA:
     """[HostAllocatorData] -> HostSoA.  `group_names[d]` is the distro's group
     table (slot order of its TaskGroupInfos); hosts are bucketed like
-    groupByTaskGroup (utilization_based_host_allocator.go:223-260)."""
+    groupByTaskGroup (utilization_based_host_allocator.go:223-260).  `running_tasks` (task id -> Task): the documents
+    task.Find(ByIds) returned (allocator.go:337); a host whose running task is one of them is found, with its StartTime
+    and its ExpectedDuration / StdDev as stored (evg_resolve_durations replaces those on the device).  Other hosts
+    read HostAllocatorData.running_tasks."""
     fl, gid, exp, std, start, off, rows = [], [], [], [], [], [0], []
     for data, names in zip(datas, group_names):
         lookup = {n: i for i, n in enumerate(names)}
@@ -503,7 +512,9 @@ def marshal_hosts(datas: Sequence[M.HostAllocatorData], group_names: Sequence[Se
             st = M.ZERO_TIME
             if h.running_task != "":
                 f |= L.EVG_HF_RUNNING
-                rt = data.running_tasks.get(h.running_task)
+                doc = running_tasks.get(h.running_task) if running_tasks is not None else None
+                rt = data.running_tasks.get(h.running_task) if doc is None else \
+                    M.RunningTaskStats(True, doc.expected_duration, doc.expected_duration_std_dev, doc.start_time)
                 if rt is not None and rt.found:
                     f |= L.EVG_HF_RT_FOUND
                     e, s, st = rt.expected, rt.std_dev, rt.start_time
@@ -990,6 +1001,147 @@ def marshal_durations(tasks: Sequence[M.Task], window_start: int, window_end: in
     rows = DurationRows(np.array(key, np.int32), np.array(taken, np.int64), np.array(start, np.int64),
                         np.array(finish, np.int64), np.array(flags, np.uint8), len(index), window_start, window_end)
     return rows, list(index)
+
+
+@dataclass
+class DurationHistory:
+    """The history half of evg_duration_in: finished tasks whose keys are numbered pair-major -- the keys of
+    (project, build variant) pair p are pair_key_off[p] .. pair_key_off[p+1] -- and the key code of a task."""
+    rows: DurationRows
+    pair_key_off: np.ndarray
+    keys: List[tuple]          # (project, build_variant, display_name) of each key
+    pairs: Dict[tuple, int]    # (project, build_variant) -> pair index
+    index: Dict[tuple, int]    # (project, build_variant, display_name) -> key
+
+    @property
+    def n_pairs(self) -> int:
+        return int(self.pair_key_off.shape[0]) - 1
+
+    def code(self, project: str, build_variant: str, display_name: str) -> int:
+        """The evg_duration_cache.key of a task: its key; EVG_DK_PAIR(p) for DisplayName "" (the window query then has
+        no name filter, expected_duration.go:54-56); EVG_DK_NONE when no finished task has it."""
+        if display_name == "":
+            p = self.pairs.get((project, build_variant))
+            return L.EVG_DK_NONE if p is None else L.EVG_DK_PAIR(p)
+        return self.index.get((project, build_variant, display_name), L.EVG_DK_NONE)
+
+    def __call__(self, t: M.Task) -> int:
+        return self.code(t.project, t.build_variant, t.display_name)
+
+
+def marshal_duration_history(finished: Sequence[M.Task], tasks: Sequence[M.Task], now: int):
+    """Finished tasks -> (DurationHistory, key code of each of `tasks`).  The window is the reference's
+    (now - 1 week, now] (task.go:3543-3544).  Pairs are numbered in first-appearance order, a pair's names likewise."""
+    pairs: Dict[tuple, int] = {}
+    names: List[Dict[str, int]] = []
+    for t in finished:
+        p = pairs.setdefault((t.project, t.build_variant), len(pairs))
+        if p == len(names):
+            names.append({})
+        names[p].setdefault(t.display_name, len(names[p]))
+    off = np.zeros(len(pairs) + 1, np.int64)
+    if pairs:
+        np.cumsum([len(n) for n in names], out=off[1:])
+    keys: List[tuple] = []
+    for (proj, bv), p in pairs.items():
+        keys.extend((proj, bv, n) for n in names[p])
+    index = {k: i for i, k in enumerate(keys)}
+    key, taken, start, finish, flags = [], [], [], [], []
+    for t in finished:
+        key.append(index[(t.project, t.build_variant, t.display_name)])
+        taken.append(t.time_taken); start.append(t.start_time); finish.append(t.finish_time)
+        flags.append((L.EVG_DR_COMPLETED if t.status in M.TASK_COMPLETED_STATUSES else 0) |
+                     (L.EVG_DR_TIMED_OUT if t.timed_out else 0))
+    rows = DurationRows(np.array(key, np.int32), np.array(taken, np.int64), np.array(start, np.int64),
+                        np.array(finish, np.int64), np.array(flags, np.uint8), len(keys), now - 7 * 24 * M.HOUR, now)
+    hist = DurationHistory(rows, off, keys, pairs, index)
+    return hist, np.array([hist(t) for t in tasks], np.int32)
+
+
+@dataclass
+class DurationCache:
+    """evg_duration_cache: what FetchExpectedDuration reads of each listed row.  rows None = every resident row."""
+    value_ns: np.ndarray
+    std_ns: np.ndarray
+    ttl_ns: np.ndarray
+    collected_ns: np.ndarray
+    expected_ns: np.ndarray
+    expected_std_ns: np.ndarray
+    key: np.ndarray
+    rows: Optional[np.ndarray] = None
+
+    @property
+    def n_rows(self) -> int:
+        return int(self.key.shape[0])
+
+    def normalize(self) -> "DurationCache":
+        for f in L.DURATION_CACHE_COLUMNS:
+            setattr(self, f, np.ascontiguousarray(getattr(self, f), dtype=np.int64))
+        self.key = np.ascontiguousarray(self.key, dtype=np.int32)
+        if self.rows is not None:
+            self.rows = np.ascontiguousarray(self.rows, dtype=np.int64)
+        return self
+
+    def struct(self) -> L.DurationCacheStruct:
+        s = L.DurationCacheStruct()
+        s.n_rows = self.n_rows
+        # NULL means "every resident row": an explicit list keeps a pointer even when it lists nothing
+        self._rows_arg = None if self.rows is None else (self.rows if self.n_rows else np.zeros(1, np.int64))
+        s.rows = L.ptr(self._rows_arg)
+        for f in L.DURATION_CACHE_COLUMNS + ("key",):
+            setattr(s, f, L.ptr(getattr(self, f)) if self.n_rows else None)
+        return s
+
+    def nbytes(self) -> int:
+        return sum(getattr(self, f).nbytes for f in L.DURATION_CACHE_COLUMNS + ("key",)) + \
+            (self.rows.nbytes if self.rows is not None else 0)
+
+
+def _cache_of(tasks: Sequence[M.Task], codes, rows) -> DurationCache:
+    ps = [t.duration_prediction for t in tasks]
+    return DurationCache(np.array([p.value for p in ps], np.int64), np.array([p.std_dev for p in ps], np.int64),
+                         np.array([p.ttl for p in ps], np.int64), np.array([p.collected_at for p in ps], np.int64),
+                         np.array([t.expected_duration for t in tasks], np.int64),
+                         np.array([t.expected_duration_std_dev for t in tasks], np.int64),
+                         np.array(codes, np.int32), rows).normalize()
+
+
+def marshal_duration_cache(tasks: Sequence[M.Task], lookup, rows=None) -> DurationCache:
+    """The cache fields of the tick's tasks (resident order) for evg_resolve_durations; `lookup` maps a task to its key
+    code (a DurationHistory).  `rows` lists the resident rows to resolve (ascending), None = all.  Reads only: the
+    tasks are not touched."""
+    if rows is not None:
+        rows = np.ascontiguousarray(rows, dtype=np.int64)
+        tasks = [tasks[int(r)] for r in rows]
+    return _cache_of(tasks, [lookup(t) for t in tasks], rows)
+
+
+def marshal_running_cache(datas: Sequence[M.HostAllocatorData], running_tasks: Dict[str, M.Task], lookup):
+    """The host counterpart: the running task of every host (marshal_hosts order) that `running_tasks` holds ->
+    (DurationCache over those host rows, the Task of each listed row).  Hosts without such a task are not listed and
+    keep what marshal_hosts gave them."""
+    rows, docs = [], []
+    r = 0
+    for data in datas:
+        for h in data.existing_hosts:
+            t = running_tasks.get(h.running_task) if h.running_task != "" else None
+            if t is not None:
+                rows.append(r)
+                docs.append(t)
+            r += 1
+    return _cache_of(docs, [lookup(t) for t in docs], np.array(rows, np.int64)), docs
+
+
+def write_back_durations(tasks: Sequence[M.Task], out: dict) -> None:
+    """What FetchExpectedDuration leaves on each Task (task.go:3519-3590): ExpectedDuration / StdDev and the
+    DurationPrediction, from evg_download_durations' rows (`tasks` in listed-row order).  An unset TTL reads as
+    predictionTTL, as it does on the device."""
+    for i, t in enumerate(tasks):
+        p = t.duration_prediction
+        if p.ttl == 0:
+            p.ttl = M.PREDICTION_TTL
+        t.expected_duration, t.expected_duration_std_dev = int(out["avg_ns"][i]), int(out["std_ns"][i])
+        p.value, p.std_dev, p.collected_at = int(out["value_ns"][i]), int(out["pred_std_ns"][i]), int(out["collected_ns"][i])
 
 
 # ---------------------------------------------------------------------------------------------------------------

@@ -690,3 +690,65 @@ def config(k: int, scale: float = 1.0, *, each: bool = False) -> Workload:
                     unmet_dep_frac=0.03, met_dep_frac=0.01, group_versions_frac=0.2, includes_dependencies=True,
                     n_hosts=D // 2, providers=(0.6, 0.2, 0.2))
     raise ValueError(k)
+
+
+@dataclass
+class DurationWorkload:
+    """The duration cache of tick w (make_duration_cache): the finished-task history, pair-major, and the cache
+    fields of every task row and every host row."""
+    history: "DurationHistory"
+    tasks: "DurationCache"
+    hosts: Optional["DurationCache"]
+
+
+DURATION_SALT = 0x5DEECE66D
+
+
+def make_duration_cache(w: Workload, seed: int, *, n_rows: int = 100_000, n_keys: int = 1000, zipf_s: float = 1.1,
+                        pair_frac: float = 0.05, none_frac: float = 0.05) -> DurationWorkload:
+    """History rows with Zipf-skewed keys over n_keys (project, build variant, display name) keys, numbered pair-major
+    over about n_keys / 4 pairs of uneven size, and cache columns for every task and host of w that reach every EVG_DS_*
+    outcome: fresh and stale predictions (zero, past and future CollectedAt, unset and explicit TTL), backfill rows, keys
+    with and without matched rows, EVG_DK_NONE and EVG_DK_PAIR codes.  A key's TimeTaken values lie within 2^20 ns of
+    the key's own base (1 min .. 1 h) so exact integer restatements of its statistics stay within int64."""
+    from .soa import DurationCache, DurationHistory, DurationRows
+    rng = Rng(seed ^ DURATION_SALT)
+    now = w.now
+    K, R = int(n_keys), int(n_rows)
+    P = max(1, K // 4)
+    cuts = np.sort(rng.integers(P - 1, 0, K)) if P > 1 else np.zeros(0, np.int64)
+    pair_key_off = np.concatenate([[0], cuts, [K]]).astype(np.int64)
+    ranks = np.arange(1, K + 1, dtype=np.float64) ** (-zipf_s)
+    cdf = np.cumsum(ranks) / ranks.sum()
+    perm = np.argsort(rng.u64(K))  # hot keys spread over the pairs
+    key = perm[np.minimum(np.searchsorted(cdf, rng.uniform(R)), K - 1)].astype(np.int32)
+    base = rng.integers(K, M.MINUTE, 60 * M.MINUTE)
+    taken = base[key] + rng.integers(R, 0, (1 << 20) - 1)
+    # a quarter of the keys have no row inside the window; other rows fall outside it now and then
+    dead = rng.uniform(K) < 0.25
+    finish = now - rng.integers(R, 0, 6 * 24 * 60 * M.MINUTE)
+    out = (rng.uniform(R) < 0.05) | dead[key]
+    finish = np.where(out, now - 8 * 24 * 60 * M.MINUTE, finish)
+    flags = np.full(R, L.EVG_DR_COMPLETED, np.uint8)
+    flags[rng.uniform(R) < 0.03] = 0
+    flags[rng.uniform(R) < 0.03] |= L.EVG_DR_TIMED_OUT
+    rows = DurationRows(key, taken.astype(np.int64), (finish - taken).astype(np.int64), finish.astype(np.int64), flags, K,
+                        now - 7 * 24 * 60 * M.MINUTE, now)
+    hist = DurationHistory(rows, pair_key_off, [], {}, {})
+
+    def cache(n: int) -> DurationCache:
+        u = rng.uniform(n)
+        code = perm[np.minimum(np.searchsorted(cdf, rng.uniform(n)), K - 1)].astype(np.int32)
+        code = np.where(u < none_frac, L.EVG_DK_NONE, code)
+        code = np.where((u >= none_frac) & (u < none_frac + pair_frac), -2 - rng.integers(n, 0, P - 1), code).astype(np.int32)
+        value = np.where(rng.uniform(n) < 0.3, 0, rng.integers(n, 1, 120 * M.MINUTE))
+        std = np.where(rng.uniform(n) < 0.5, 0, rng.integers(n, 1, 10 * M.MINUTE))
+        ttl = np.where(rng.uniform(n) < 0.5, 0, rng.integers(n, M.MINUTE, 600 * M.MINUTE))
+        v = rng.uniform(n)
+        coll = np.where(v < 0.2, M.ZERO_TIME, now - rng.integers(n, 0, 720 * M.MINUTE))
+        coll = np.where(v > 0.9, now + rng.integers(n, 1, 60 * M.MINUTE), coll)
+        exp = np.where(rng.uniform(n) < 0.2, rng.integers(n, 1, 120 * M.MINUTE), 0)
+        exp_std = rng.integers(n, 0, 5 * M.MINUTE)
+        return DurationCache(value, std, ttl, coll, exp, exp_std, code).normalize()
+
+    return DurationWorkload(hist, cache(w.tasks.n_tasks), cache(w.hosts.n_hosts) if w.hosts is not None else None)

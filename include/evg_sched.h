@@ -689,6 +689,71 @@ typedef struct {
 /* getExpectedDurationsForWindow (model/task/expected_duration.go:36-96) for every key at once.  Host pointers. */
 int evg_expected_durations_batch(evg_ctx* ctx, const evg_duration_rows* in, evg_duration_stat* out);
 
+/* ---- the duration cache of a resident tick (SURVEY.md §8 rows A3/A4) ------- */
+
+/* evg_duration_cache.key: the history key of (Project, BuildVariant, DisplayName), or one of these */
+#define EVG_DK_NONE (-1)          /* no history row has the key: the window query returns no document */
+#define EVG_DK_PAIR(p) (-2 - (p)) /* DisplayName == "": no name filter, the rows of (Project, BuildVariant) pair p grouped by
+                                     name (expected_duration.go:54-56): one document exactly when ONE key of the pair matched */
+/* evg_duration_out.source: which branch of Task.FetchExpectedDuration decided the row; every source but FRESH is persisted */
+#define EVG_DS_FRESH 0     /* CachedDurationValue.Get: since(CollectedAt) < TTL, the cached value (cached_value.go:127-129) */
+#define EVG_DS_BACKFILL 1  /* Value == 0 && ExpectedDuration != 0 (task.go:3524-3538) */
+#define EVG_DS_HISTORY 2   /* stale, one document with a non-zero truncated $avg (task.go:3564-3569) */
+#define EVG_DS_PREVIOUS 3  /* stale, not exactly one document, previous Value != 0 (task.go:3556-3562) */
+#define EVG_DS_DEFAULT 4   /* stale: defaultTaskDuration (10 min, 0), no document and Value == 0 or a $avg truncating to 0 */
+
+/* What FetchExpectedDuration reads of one task, for the listed rows of a resident table.  Host pointers. */
+typedef struct {
+  int64_t n_rows;
+  const int64_t* rows;            /* strictly ascending resident rows (tasks or hosts); NULL = every row in order (a non-NULL list may be empty) */
+  const int64_t* value_ns;        /* DurationPrediction.Value */
+  const int64_t* std_ns;          /* DurationPrediction.StdDev */
+  const int64_t* ttl_ns;          /* DurationPrediction.TTL; 0 = predictionTTL (8 h) -- a shim that wants
+                                     utility.JitterInterval (task.go:3520-3522) passes its own draw instead */
+  const int64_t* collected_ns;    /* DurationPrediction.CollectedAt, EVG_TIME_ZERO = zero time */
+  const int64_t* expected_ns;     /* Task.ExpectedDuration */
+  const int64_t* expected_std_ns; /* Task.ExpectedDurationStdDev */
+  const int32_t* key;             /* history key, EVG_DK_NONE or EVG_DK_PAIR(p) */
+} evg_duration_cache;
+
+typedef struct {
+  const evg_duration_rows* history; /* finished tasks; keys numbered pair-major (the keys of pair p are
+                                       pair_key_off[p] .. pair_key_off[p+1]); window (now - 1 week, now]
+                                       (taskCompletionEstimateWindow, task.go:3543-3544); NULL = no rows */
+  int32_t n_pairs;
+  int32_t _reserved;
+  const int64_t* pair_key_off;      /* n_pairs + 1 */
+  const evg_duration_cache* tasks;  /* rows of the resident task table; NULL leaves expected_ns as uploaded */
+  const evg_duration_cache* hosts;  /* running tasks of the resident hosts; NULL leaves expected_ns / std_ns */
+} evg_duration_in;
+
+/* Per listed row, in listed-row order.  Any pointer may be NULL. */
+typedef struct {
+  int64_t* avg_ns;       /* the DurationStats returned = Task.ExpectedDuration afterwards */
+  int64_t* std_ns;       /* ... .StdDev = Task.ExpectedDurationStdDev afterwards */
+  int64_t* value_ns;     /* DurationPrediction after the call; persisted as ExpectedDuration (task.go:900) */
+  int64_t* pred_std_ns;  /* ... StdDev; persisted as ExpectedDurationStdDev (task.go:901), even for BACKFILL */
+  int64_t* collected_ns; /* ... CollectedAt */
+  uint8_t* source;       /* EVG_DS_* */
+} evg_duration_out;
+
+/* Task.FetchExpectedDuration (model/task/task.go:3519-3590 with CachedDurationValue.Get, util/cached_value.go:125-145,
+ * and getExpectedDurationsForWindow, expected_duration.go:36-96) for listed rows of the resident tick, the clock frozen
+ * at now_ns.  The statistics of every key are computed on the device, decided per row, and the result written into
+ * the resident planner column expected_ns (tasks) and the allocator columns expected_ns / std_ns (hosts); nothing
+ * goes back to the host but the error word.  Allowed whenever the context holds its own resident tick (after evg_upload,
+ * evg_upload_with_deps, evg_edit_tasks, evg_plan_from_finder(_ex) and evg_plan_aliases); the tick keeps everything else
+ * (dependency verdicts, the alias map, evg_update_tasks / evg_edit_tasks afterwards).  EVG_ERR_STATE: no tick, borrowed
+ * columns (evg_upload_device), the tick a one-shot call left, hosts != NULL on a tick without hosts.  EVG_ERR_INVALID with the tick untouched: rows out
+ * of range or not strictly ascending, n_rows != the resident count when rows == NULL, a pair_key_off that does not start
+ * at 0, end at n_keys and never decrease, null columns, and -- found on the device -- a key or pair out of range.
+ * Replaces: PopulateCaches -> Task.FetchExpectedDuration (scheduler/setup_funcs.go:20-67) and the running-task
+ * durations of the host allocator (utilization_based_host_allocator.go:357-359). */
+int evg_resolve_durations(evg_ctx* ctx, const evg_duration_in* in, int64_t now_ns);
+/* After evg_resolve_durations: its per-row results, listed-row order; either pointer may be NULL.  EVG_ERR_STATE once
+ * another call replaced the tick's rows. */
+int evg_download_durations(evg_ctx* ctx, evg_duration_out* tasks, evg_duration_out* hosts);
+
 /* ---- legacy comparator prioritiser (SURVEY.md §8 row L) ---------------------- */
 
 /* evg_legacy_soa.flags */
