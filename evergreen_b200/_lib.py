@@ -206,6 +206,13 @@ class DagInStruct(C.Structure):
                 ("group_id", C.c_void_p), ("group_index", C.c_void_p)]
 
 
+DISPATCH_OUT_FIELDS = ("item_off", "sorted", "n_sorted", "n_cycles", "group_off", "group_slot", "unit_items", "unit_off")
+
+
+class DispatchOutStruct(C.Structure):
+    _fields_ = [(f, C.c_void_p) for f in DISPATCH_OUT_FIELDS]
+
+
 class AllocOutStruct(C.Structure):
     _fields_ = [("result", C.c_void_p), ("status", C.c_void_p)]
 
@@ -256,6 +263,7 @@ SYMBOLS = {
     "evg_download_durations": (C.c_int, [_P, _P, _P]),
     "evg_prioritize_legacy_batch": (C.c_int, [_P, _P, _P, _P, C.c_int32, _P, _P, _P]),
     "evg_dag_rebuild_batch": (C.c_int, [_P, _P, _P, _P, C.c_int32, _P, _P, _P, _P, _P]),
+    "evg_rebuild_dispatchers": (C.c_int, [_P, C.c_int32, C.c_int64, C.c_int64, _P]),
     "evg_plan_distro": (C.c_int, [_P, _P, _P, C.c_int32, _P, C.c_int64, C.c_uint32, _P]),
     "evg_alloc_distro": (C.c_int, [_P, _P, _P, _P, _P, C.c_int32, C.c_int64, _P, _P]),
 }

@@ -1243,6 +1243,12 @@ struct evg_ctx {
     int64_t n_t = 0, n_h = 0;
     bool valid = false;
   } dur;
+  // evg_rebuild_dispatchers (the first call allocates these): the persisted queues' DAG input gathered from the tick,
+  // and the scratch and results of the k_dag_* kernels, so that the resident tick is only read
+  struct {
+    DevBuf item_off, rank_of, row, first, gslot_of, gindex, cnt, dep_off, dep_item, pos, group_off, group_slot, group_id, scan_sum;
+    DevBuf succ_off, succ, index, low, stack, cs_node, cs_pos, emit, on_stack, sorted, stats, buf[2], unit_off;
+  } dp;
   DevBuf b_err;
   DevBuf b_route, b_unitv, b_unita, b_unitn, b_unitmask;
   DevBuf b_punt, b_puntcnt;
@@ -3961,6 +3967,52 @@ int evg_prioritize_legacy_batch(evg_ctx* c, const evg_legacy_soa* in, const int6
   return EVG_OK;
 }
 
+// Where dag_run's kernels write: d.sorted, (n_sorted, n_cycles, grouped) at 0, D+1, 2(D+1), the two merge-sort buffers,
+// the groups' offsets (D+1, on the device) and the unit offsets.
+struct DagBufs {
+  int32_t* sorted;
+  int32_t* stats;
+  int32_t* buf[2];
+  const int64_t* group_off;
+  int32_t* unit_off;
+};
+// k_dag_topo, then the task-group buckets (k_dag_group_init / k_dag_group_pass / k_dag_units) over x, and the results
+// copied to the host.  item_off / group_off (D+1) are the host copies of x's offsets; max_n is the longest queue.
+static int dag_run(evg_ctx* c, const DDag& x, const DagBufs& b, int64_t max_n, const int64_t* item_off, const int64_t* group_off,
+                   int32_t* sorted, int32_t* n_sorted, int32_t* n_cycles, int32_t* unit_items, int32_t* unit_off) {
+  const int64_t N = x.n;
+  const int32_t D = x.n_distros;
+  const int64_t G = group_off[D];
+  cudaStream_t s = c->stream;
+  int32_t* d_nsorted = b.stats;
+  int32_t* d_ncycles = d_nsorted + (D + 1);
+  int32_t* d_grouped = d_ncycles + (D + 1);
+  LAUNCH(c, k_dag_topo, grid_for(int64_t(D) * 32, 64), 64, x, b.sorted, d_nsorted, d_ncycles);
+  std::vector<int32_t> grouped(size_t(D), 0);
+  int cur = 0;
+  if (N > 0) {
+    CK(cudaMemcpyAsync(sorted, b.sorted, sizeof(int32_t) * size_t(N), cudaMemcpyDeviceToHost, s));
+    // every item has a group or not: "no ungrouped item" leaves grouped[d] at the distro's length
+    for (int32_t d = 0; d < D; d++) grouped[size_t(d)] = int32_t(item_off[d + 1] - item_off[d]);
+    CK(cudaMemcpyAsync(d_grouped, grouped.data(), sizeof(int32_t) * size_t(D), cudaMemcpyHostToDevice, s));
+    LAUNCH(c, k_dag_group_init, grid_for(N, 256), 256, x, b.buf[0]);
+    for (int64_t L = 1; L < max_n; L <<= 1) {
+      LAUNCH(c, k_dag_group_pass, grid_for(N, 256), 256, x, b.buf[cur], b.buf[cur ^ 1], L);
+      cur ^= 1;
+    }
+    LAUNCH(c, k_dag_units, grid_for(N, 256), 256, x, b.buf[cur], b.group_off, b.unit_off, d_grouped);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(unit_items, b.buf[cur], sizeof(int32_t) * size_t(N), cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(unit_off, b.unit_off, sizeof(int32_t) * size_t(G + D), cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(grouped.data(), d_grouped, sizeof(int32_t) * size_t(D), cudaMemcpyDeviceToHost, s));
+  }
+  CK(cudaMemcpyAsync(n_sorted, d_nsorted, sizeof(int32_t) * size_t(D), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(n_cycles, d_ncycles, sizeof(int32_t) * size_t(D), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  for (int32_t d = 0; d < D; d++) unit_off[group_off[d + 1] + d] = grouped[size_t(d)];  // the closing entry of each distro
+  return EVG_OK;
+}
+
 int evg_dag_rebuild_batch(evg_ctx* c, const evg_dag_in* in, const int64_t* item_off, const int64_t* group_off, int32_t n_distros,
                           int32_t* sorted, int32_t* n_sorted, int32_t* n_cycles, int32_t* unit_items, int32_t* unit_off) {
   if (!c || !in) return fail(EVG_ERR_INVALID, "evg_dag_rebuild_batch: null argument");
@@ -4005,34 +4057,157 @@ int evg_dag_rebuild_batch(evg_ctx* c, const evg_dag_in* in, const int64_t* item_
   x.succ_off = c->tasks.prio.as<int32_t>(); x.succ = c->b_rn5.as<int32_t>(); x.index = c->tasks.nd.as<int32_t>(); x.low = c->tasks.vid.as<int32_t>();
   x.stack = c->tasks.flags.as<int32_t>(); x.cs_node = c->b_rn0.as<int32_t>(); x.cs_pos = c->b_rn1.as<int32_t>(); x.emit = c->b_rn2.as<int32_t>();
   x.on_stack = c->b_hasdep.as<uint8_t>();
-  int32_t* d_nsorted = c->b_rn6.as<int32_t>();
-  int32_t* d_ncycles = d_nsorted + (D + 1);
-  int32_t* d_grouped = d_ncycles + (D + 1);
-  LAUNCH(c, k_dag_topo, grid_for(int64_t(D) * 32, 64), 64, x, c->b_order.as<int32_t>(), d_nsorted, d_ncycles);
-  std::vector<int32_t> grouped(size_t(D), 0);
-  int32_t* buf[2] = {c->b_rn3.as<int32_t>(), c->b_rn4.as<int32_t>()};
-  int cur = 0;
-  if (N > 0) {
-    CK(cudaMemcpyAsync(sorted, c->b_order.p, sizeof(int32_t) * size_t(N), cudaMemcpyDeviceToHost, s));
-    // every item has a group or not: "no ungrouped item" leaves grouped[d] at the distro's length
-    for (int32_t d = 0; d < D; d++) grouped[size_t(d)] = int32_t(item_off[d + 1] - item_off[d]);
-    CK(cudaMemcpyAsync(d_grouped, grouped.data(), sizeof(int32_t) * size_t(D), cudaMemcpyHostToDevice, s));
-    LAUNCH(c, k_dag_group_init, grid_for(N, 256), 256, x, buf[0]);
-    for (int64_t L = 1; L < max_n; L <<= 1) {
-      LAUNCH(c, k_dag_group_pass, grid_for(N, 256), 256, x, buf[cur], buf[cur ^ 1], L);
-      cur ^= 1;
-    }
-    LAUNCH(c, k_dag_units, grid_for(N, 256), 256, x, buf[cur], c->b_groupoff.as<int64_t>(), c->b_rn7.as<int32_t>(), d_grouped);
-    CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(unit_items, buf[cur], sizeof(int32_t) * size_t(N), cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(unit_off, c->b_rn7.p, sizeof(int32_t) * size_t(G + D), cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(grouped.data(), d_grouped, sizeof(int32_t) * size_t(D), cudaMemcpyDeviceToHost, s));
+  DagBufs b{c->b_order.as<int32_t>(), c->b_rn6.as<int32_t>(), {c->b_rn3.as<int32_t>(), c->b_rn4.as<int32_t>()}, c->b_groupoff.as<int64_t>(),
+            c->b_rn7.as<int32_t>()};
+  return dag_run(c, x, b, max_n, item_off, group_off, sorted, n_sorted, n_cycles, unit_items, unit_off);
+}
+
+// The persisted queue of every distro of the resident tick as a DAG input (evg_rebuild_dispatchers).  Item j of distro d
+// is rank r = j - item_off[d], the task order[task_off[d] + r].
+struct DDisp {
+  int32_t D;
+  int64_t n;                   // items
+  const int64_t* task_off;     // [D+1] resident
+  const int64_t* group_off;    // [D+1] resident group slots
+  const int64_t* item_off;     // [D+1]
+  const int32_t* order;        // the resident rank order (distro-local tasks)
+  const int32_t* gid;          // resident group slot ids
+  const int32_t* tgo;          // resident TaskGroupOrder
+  const int64_t* dep_off;      // resident edges; NULL when the tick has none
+  const int32_t* dep_idx;
+  int32_t* rank_of;            // [T]: rank of a task below the cap, -1 otherwise (set to -1 before k_dp_gather)
+  int32_t* row;                // [n]: distro-local task of an item, -1 for an order entry outside the distro
+  int32_t* first;              // [G]: first rank of each group slot (INT32_MAX-like before k_dp_gather: never seen)
+};
+// per item: its task, rank_of, GroupIndex, group slot, edge count, and the slot's first rank
+__global__ void __launch_bounds__(256) k_dp_gather(DDisp X, int32_t* __restrict__ gslot_of, int32_t* __restrict__ gindex, int32_t* __restrict__ cnt) {
+  const int64_t j = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  const int d = block_find_distro(X.item_off, X.D, j, X.n);
+  if (d < 0) return;
+  const int64_t base = X.task_off[d];
+  const int32_t r = int32_t(j - X.item_off[d]);
+  const int32_t i = X.order[base + r];
+  if (i < 0 || i >= X.task_off[d + 1] - base) { X.row[j] = -1; gslot_of[j] = -1; gindex[j] = 0; cnt[j] = 0; return; }
+  const int64_t t = base + i;
+  X.row[j] = i;
+  X.rank_of[t] = r;
+  gindex[j] = X.tgo[t];
+  const int32_t g = X.gid[t];
+  gslot_of[j] = g;
+  if (g >= 0) atomicMin(X.first + X.group_off[d] + g, r);
+  cnt[j] = X.dep_off ? int32_t(X.dep_off[t + 1] - X.dep_off[t]) : 0;
+}
+// per item: its edges as ranks (-1 past the cap), in the resident order; and the flag of the item that first holds its slot
+__global__ void __launch_bounds__(256) k_dp_edges(DDisp X, const int64_t* __restrict__ e_off, int32_t* __restrict__ dep_item,
+                                                  const int32_t* __restrict__ gslot_of, int32_t* __restrict__ flag) {
+  const int64_t j = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  const int d = block_find_distro(X.item_off, X.D, j, X.n);
+  if (d < 0) return;
+  const int32_t g = gslot_of[j];
+  flag[j] = (g >= 0 && X.first[X.group_off[d] + g] == int32_t(j - X.item_off[d])) ? 1 : 0;
+  const int32_t i = X.row[j];
+  if (i < 0 || !X.dep_off) return;
+  const int64_t base = X.task_off[d], t = base + i;
+  int64_t w = e_off[j];
+  for (int64_t e = X.dep_off[t]; e < X.dep_off[t + 1]; e++) dep_item[w++] = X.rank_of[base + X.dep_idx[e]];
+}
+// pos = exclusive scan of the flags: the dense id of an item's group is the position of its slot's first item within
+// the distro; group_off[d] = pos[item_off[d]] (threads 0 .. D); group_slot[pos[j]] = the slot of a first item j
+__global__ void __launch_bounds__(256) k_dp_groups(DDisp X, const int64_t* __restrict__ pos, const int32_t* __restrict__ gslot_of,
+                                                   int32_t* __restrict__ group_id, int32_t* __restrict__ group_slot,
+                                                   int64_t* __restrict__ group_off) {
+  const int64_t j = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (j <= X.D) group_off[j] = pos[X.item_off[j]];
+  if (j >= X.n) return;
+  const int d = find_distro(X.item_off, 0, X.D - 1, j);
+  const int32_t g = gslot_of[j];
+  if (g < 0) { group_id[j] = -1; return; }
+  const int64_t head = X.item_off[d] + X.first[X.group_off[d] + g];
+  group_id[j] = int32_t(pos[head] - pos[X.item_off[d]]);
+  if (head == j) group_slot[pos[j]] = g;
+}
+
+int evg_rebuild_dispatchers(evg_ctx* c, int32_t cap, int64_t items_capacity, int64_t groups_capacity, evg_dispatch_out* out) {
+  if (!c || !out) return fail(EVG_ERR_INVALID, "evg_rebuild_dispatchers: null argument");
+  LOCK(c);
+  if (!c->have_tasks) return fail(EVG_ERR_STATE, "evg_rebuild_dispatchers without a resident tick");
+  if (cap < 0) return fail(EVG_ERR_INVALID, "evg_rebuild_dispatchers: negative cap");
+  if (cap == 0) cap = EVG_PERSISTED_QUEUE_CAP;
+  if (!out->item_off || !out->n_sorted || !out->n_cycles || !out->group_off || !out->unit_off)
+    return fail(EVG_ERR_INVALID, "evg_rebuild_dispatchers: null output");
+  const int32_t D = c->Dn;
+  int64_t* item_off = out->item_off;
+  item_off[0] = 0;
+  int64_t max_n = 0, g_need = 0;
+  for (int32_t d = 0; d < D; d++) {
+    const int64_t n = std::min<int64_t>(c->h_taskoff[d + 1] - c->h_taskoff[d], cap);
+    item_off[d + 1] = item_off[d] + n;
+    max_n = std::max(max_n, n);
+    g_need += std::min(c->h_groupoff[d + 1] - c->h_groupoff[d], n);
   }
-  CK(cudaMemcpyAsync(n_sorted, d_nsorted, sizeof(int32_t) * size_t(D), cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(n_cycles, d_ncycles, sizeof(int32_t) * size_t(D), cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  for (int32_t d = 0; d < D; d++) unit_off[group_off[d + 1] + d] = grouped[size_t(d)];  // the closing entry of each distro
-  return EVG_OK;
+  const int64_t N = item_off[D];
+  if (N > items_capacity || g_need > groups_capacity)
+    return fail(EVG_ERR_INVALID, "evg_rebuild_dispatchers: %lld items and %lld groups needed, capacities %lld and %lld", (long long)N,
+                (long long)g_need, (long long)items_capacity, (long long)groups_capacity);
+  if (N > 0 && (!out->sorted || !out->unit_items)) return fail(EVG_ERR_INVALID, "evg_rebuild_dispatchers: null item output");
+  if (g_need > 0 && !out->group_slot) return fail(EVG_ERR_INVALID, "evg_rebuild_dispatchers: null group_slot");
+  c->launches = 0;
+  if (N == 0) {  // every queue is empty: no items, no groups
+    for (int32_t d = 0; d < D; d++) out->n_sorted[d] = out->n_cycles[d] = out->unit_off[d] = 0;
+    for (int32_t d = 0; d <= D; d++) out->group_off[d] = 0;
+    return EVG_OK;
+  }
+  CK(cudaSetDevice(c->device));
+  cudaStream_t s = c->stream;
+  auto& p = c->dp;
+  const int64_t T = c->T, E = c->E, G = c->G;
+  UP(s, p.item_off, item_off, D + 1, int64_t);
+  CK(p.rank_of.ensure(sizeof(int32_t) * size_t(T + 1)));
+  CK(p.first.ensure(sizeof(int32_t) * size_t(G + 1)));
+  for (DevBuf* b : {&p.row, &p.gslot_of, &p.gindex, &p.cnt, &p.group_id, &p.index, &p.low, &p.stack, &p.cs_node, &p.cs_pos, &p.emit,
+                    &p.sorted, &p.buf[0], &p.buf[1]})
+    CK(b->ensure(sizeof(int32_t) * size_t(N + 1)));
+  CK(p.on_stack.ensure(size_t(N) + 16));
+  CK(p.dep_off.ensure(sizeof(int64_t) * size_t(N + 1)));
+  CK(p.pos.ensure(sizeof(int64_t) * size_t(N + 1)));
+  CK(p.scan_sum.ensure(sizeof(int64_t) * size_t((N + 1023) / 1024 + 2)));
+  CK(p.dep_item.ensure(sizeof(int32_t) * size_t(E + 1)));  // the persisted items hold at most every resident edge
+  CK(p.succ.ensure(sizeof(int32_t) * size_t(E + 1)));
+  CK(p.succ_off.ensure(sizeof(int32_t) * size_t(N + D + 1)));
+  CK(p.group_off.ensure(sizeof(int64_t) * size_t(D + 1)));
+  CK(p.group_slot.ensure(sizeof(int32_t) * size_t(g_need + 1)));
+  CK(p.unit_off.ensure(sizeof(int32_t) * size_t(g_need + D + 1)));
+  CK(p.stats.ensure(sizeof(int32_t) * 3 * size_t(D + 1)));
+  CK(cudaMemsetAsync(p.rank_of.p, 0xFF, sizeof(int32_t) * size_t(T), s));
+  if (G > 0) CK(cudaMemsetAsync(p.first.p, 0x7F, sizeof(int32_t) * size_t(G), s));
+  DDisp X;
+  X.D = D; X.n = N;
+  X.task_off = c->b_taskoff.as<int64_t>(); X.group_off = c->b_groupoff.as<int64_t>(); X.item_off = p.item_off.as<int64_t>();
+  X.order = c->b_order.as<int32_t>(); X.gid = c->tasks.gid.as<int32_t>(); X.tgo = c->tasks.tgo.as<int32_t>();
+  X.dep_off = E > 0 ? c->b_depoff.as<int64_t>() : nullptr; X.dep_idx = E > 0 ? c->b_depidx.as<int32_t>() : nullptr;
+  X.rank_of = p.rank_of.as<int32_t>(); X.row = p.row.as<int32_t>(); X.first = p.first.as<int32_t>();
+  int32_t* cnt = p.cnt.as<int32_t>();
+  LAUNCH(c, k_dp_gather, grid_for(N, 256), 256, X, p.gslot_of.as<int32_t>(), p.gindex.as<int32_t>(), cnt);
+  scan_counts(c, cnt, N, p.dep_off.as<int64_t>(), p.scan_sum.as<int64_t>());
+  LAUNCH(c, k_dp_edges, grid_for(N, 256), 256, X, p.dep_off.as<int64_t>(), p.dep_item.as<int32_t>(), p.gslot_of.as<int32_t>(), cnt);
+  scan_counts(c, cnt, N, p.pos.as<int64_t>(), p.scan_sum.as<int64_t>());
+  LAUNCH(c, k_dp_groups, grid_for(std::max<int64_t>(N, D + 1), 256), 256, X, p.pos.as<int64_t>(), p.gslot_of.as<int32_t>(),
+         p.group_id.as<int32_t>(), p.group_slot.as<int32_t>(), p.group_off.as<int64_t>());
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(out->group_off, p.group_off.p, sizeof(int64_t) * size_t(D + 1), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));  // group_off sizes the unit table and closes each distro's unit_off
+  const int64_t G2 = out->group_off[D];
+  if (G2 > 0) CK(cudaMemcpyAsync(out->group_slot, p.group_slot.p, sizeof(int32_t) * size_t(G2), cudaMemcpyDeviceToHost, s));
+  DDag x;
+  x.n = N; x.n_deps = E; x.n_distros = D;
+  x.item_off = p.item_off.as<int64_t>(); x.dep_off = p.dep_off.as<int64_t>(); x.dep_item = p.dep_item.as<int32_t>();
+  x.group_id = p.group_id.as<int32_t>(); x.group_index = p.gindex.as<int32_t>();
+  x.succ_off = p.succ_off.as<int32_t>(); x.succ = p.succ.as<int32_t>(); x.index = p.index.as<int32_t>(); x.low = p.low.as<int32_t>();
+  x.stack = p.stack.as<int32_t>(); x.cs_node = p.cs_node.as<int32_t>(); x.cs_pos = p.cs_pos.as<int32_t>(); x.emit = p.emit.as<int32_t>();
+  x.on_stack = p.on_stack.as<uint8_t>();
+  DagBufs b{p.sorted.as<int32_t>(), p.stats.as<int32_t>(), {p.buf[0].as<int32_t>(), p.buf[1].as<int32_t>()}, p.group_off.as<int64_t>(),
+            p.unit_off.as<int32_t>()};
+  return dag_run(c, x, b, max_n, item_off, out->group_off, out->sorted, out->n_sorted, out->n_cycles, out->unit_items, out->unit_off);
 }
 
 int evg_plan_distro(evg_ctx* c, const evg_task_soa* tasks, const evg_distro_cfg* cfg, int32_t n_groups,

@@ -401,6 +401,22 @@ class Engine:
                                                L.ptr(n_sorted), L.ptr(n_cycles), L.ptr(unit_items) if N else None, L.ptr(unit_off)))
         return sorted_[:N], n_sorted, n_cycles, unit_items[:N], unit_off
 
+    def rebuild_dispatchers(self, cap: int = 0):
+        """evg_rebuild_dispatchers: the DAG dispatcher of every distro's persisted queue (the first min(length, cap) ranks,
+        cap 0 = the reference's 10 000), built on the device from the resident tick after run().  -> dict of
+        L.DISPATCH_OUT_FIELDS: item_off, sorted, n_sorted, n_cycles, group_off, group_slot, unit_items, unit_off, laid
+        out as dag_rebuild_batch's results; group_slot maps each dense group back to the tick's group slot."""
+        T, D, G = self._n_tasks, self._n_distros, self._n_groups
+        o = {"item_off": self._out("disp_item_off", D + 1, np.int64), "group_off": self._out("disp_group_off", D + 1, np.int64)}
+        for f, n in (("sorted", T), ("unit_items", T), ("group_slot", G), ("unit_off", G + D), ("n_sorted", D), ("n_cycles", D)):
+            o[f] = self._out(f"disp_{f}", max(n, 1), np.int32)
+        st = L.DispatchOutStruct(*[L.ptr(o[f]) for f in L.DISPATCH_OUT_FIELDS])
+        L.check(self.lib.evg_rebuild_dispatchers(self.ctx, int(cap), max(T, 1), max(G, 1), C.byref(st)))
+        N, G2 = int(o["item_off"][D]), int(o["group_off"][D])
+        return {"item_off": o["item_off"], "sorted": o["sorted"][:N], "n_sorted": o["n_sorted"][:D], "n_cycles": o["n_cycles"][:D],
+                "group_off": o["group_off"], "group_slot": o["group_slot"][:G2], "unit_items": o["unit_items"][:N],
+                "unit_off": o["unit_off"][:G2 + D]}
+
     def alloc_batch(self, hosts: S.HostSoA, qinfo: np.ndarray, ginfo: np.ndarray, group_off: np.ndarray, now: int):
         D = int(qinfo.shape[0])
         ao = self._alloc_output(D)
@@ -552,6 +568,7 @@ class ResidentTick:
         self.row: Dict[str, int] = {}    # task id -> row of the resident table
         self.soa = self.table = self.keys = None
         self.last = None                 # (edit, update rows) of the last plan(), None when it uploaded
+        self.ranked: List[List[str]] = []  # per distro: task ids in the last plan()'s rank order
 
     def canonical(self, batch):
         """The batch in canonical order: survivors in their previous order, then arrivals in batch order."""
@@ -653,7 +670,14 @@ class ResidentTick:
                 eng.update_tasks(rows, values)
         self.last = None if change is None else change[:2]
         self.remember(canon, soa, table, keys)
-        return _ranked_results(eng, canon, table, keys, now, breakdown, secondary)
+        res = _ranked_results(eng, canon, table, keys, now, breakdown, secondary)
+        self.ranked = [[t.id for t in ranked] for ranked, _ in res]
+        return res
+
+    def dispatchers(self, cap: int = 0):
+        """The DAG dispatcher of every distro's persisted queue of the last plan(), built on the device from the tick
+        (dispatchers_from_tick): what rebuild_dag_dispatchers returns for the queues persist_task_queues would save."""
+        return dispatchers_from_tick(self.ranked, [k.group_names for k in self.keys], cap=cap, engine=self.engine)
 
     def remember(self, canon, soa: S.TaskSoA, table: S.DistroTable, keys) -> None:
         """Make the marshalled `canon` the resident tick the next diff starts from."""
@@ -1086,27 +1110,8 @@ def rebuild_dag_dispatchers(queues: Sequence[M.TaskQueue], *, engine: Optional[E
     153-252).  Per queue: (sorted item ids with None for each dependency cycle's placeholder, number of cycles,
     {composite group id: [item ids by GroupIndex]})."""
     eng = engine or default_engine()
-    item_off, group_off, dep_off, dep_item, group_id, group_index, names = [0], [0], [0], [], [], [], []
-    for q in queues:
-        pos = {it.id: k for k, it in enumerate(q.queue)}
-        groups: Dict[str, int] = {}
-        for it in q.queue:
-            for dep in it.dependencies:
-                dep_item.append(pos.get(dep, -1))
-            dep_off.append(len(dep_item))
-            if it.group:
-                gid = f"{it.group}_{it.build_variant}_{it.project}_{it.version}"  # compositeGroupID
-                group_id.append(groups.setdefault(gid, len(groups)))
-            else:
-                group_id.append(-1)
-            group_index.append(it.group_index)
-        names.append(list(groups))
-        item_off.append(item_off[-1] + len(q.queue))
-        group_off.append(group_off[-1] + len(groups))
-    a = lambda x, t: np.ascontiguousarray(np.array(x, dtype=t))  # noqa: E731
-    io, go = a(item_off, np.int64), a(group_off, np.int64)
-    srt, n_sorted, n_cycles, unit_items, unit_off = eng.dag_rebuild_batch(io, go, a(dep_off, np.int64), a(dep_item, np.int32),
-                                                                            a(group_id, np.int32), a(group_index, np.int32))
+    io, go, dep_off, dep_item, group_id, group_index, names = S.dag_input_from_queues(queues)
+    srt, n_sorted, n_cycles, unit_items, unit_off = eng.dag_rebuild_batch(io, go, dep_off, dep_item, group_id, group_index)
     out = []
     for d, q in enumerate(queues):
         b = int(io[d])
@@ -1116,3 +1121,38 @@ def rebuild_dag_dispatchers(queues: Sequence[M.TaskQueue], *, engine: Optional[E
                  for g, name in enumerate(names[d])}
         out.append((order, int(n_cycles[d]), units))
     return out
+
+
+def dispatchers_from_tick(ranked_ids: Sequence[Sequence[str]], group_names: Sequence[Sequence[str]], *, cap: int = 0,
+                          engine: Optional[Engine] = None):
+    """What rebuild_dag_dispatchers returns for the queues PersistTaskQueue would save from the engine's resident tick
+    (after run()), built on the device: the queues never cross PCIe (evg_rebuild_dispatchers).  `ranked_ids[d]` holds
+    distro d's task ids in rank order (at least its persisted head: what plan_distros / ResidentTick.plan /
+    plan_alias_queues return), `group_names[d]` the name of each of its group slots (marshal_tasks' keys[d].group_names:
+    Task.GetTaskGroupString has compositeGroupID's format)."""
+    eng = engine or default_engine()
+    r = eng.rebuild_dispatchers(cap)
+    io, go = r["item_off"], r["group_off"]
+    out = []
+    for d, (ids, names) in enumerate(zip(ranked_ids, group_names)):
+        b, u = int(io[d]), int(go[d]) + d
+        order = [None if int(i) < 0 else ids[int(i)] for i in r["sorted"][b:b + int(r["n_sorted"][d])]]
+        units = {names[int(r["group_slot"][int(go[d]) + g])]:
+                 [ids[int(i)] for i in r["unit_items"][b + int(r["unit_off"][u + g]):b + int(r["unit_off"][u + g + 1])]]
+                 for g in range(int(go[d + 1] - go[d]))}
+        out.append((order, int(r["n_cycles"][d]), units))
+    return out
+
+
+def alias_dispatchers(distros: Sequence[M.Distro], tasks: Sequence[M.Task], now: int, *, engine: Optional[Engine] = None,
+                      dependency_db: Optional[Dict[str, M.Task]] = None, cap: int = 0):
+    """The DAG dispatcher of every distro's alias queue: evg_plan_aliases, the run, then evg_rebuild_dispatchers on the
+    secondary queues persist_alias_task_queues would save.  Per distro what rebuild_dag_dispatchers returns for them."""
+    eng = engine or default_engine()
+    task_off, group_off, src, names = _plan_aliases(eng, distros, tasks, now, dependency_db)
+    eng.run(now)
+    po, _ = eng.download(want_alloc=False)
+    ranked = [[tasks[int(src[int(task_off[d]) + int(i)])].id for i in po.order[int(task_off[d]):int(task_off[d + 1])]]
+              for d in range(len(distros))]
+    return dispatchers_from_tick(ranked, [names[int(group_off[d]):int(group_off[d + 1])] for d in range(len(distros))],
+                                 cap=cap, engine=eng)

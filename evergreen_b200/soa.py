@@ -1254,3 +1254,72 @@ def marshal_legacy(batch: Sequence[tuple], now: Optional[int] = None) -> LegacyT
         task_off.append(task_off[-1] + len(tasks))
     return LegacyTable(**{name: np.array(cols[name], dtype=dt) for name, dt in LegacyTable.COLUMNS},
                        task_off=np.array(task_off, dtype=np.int64), list_mode=np.array(modes, dtype=np.uint8))
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# DAG dispatcher input (model/task_queue_service_dependency.go:153-252)
+def dag_input_from_queues(queues: Sequence[M.TaskQueue]):
+    """Persisted TaskQueue documents -> the evg_dag_in of evg_dag_rebuild_batch, as rebuild() reads them:
+    (item_off, group_off, dep_off, dep_item, group_id, group_index, per queue the compositeGroupID of each dense group).
+    A dependency id that is not in the queue becomes -1 (addEdge returns without a line, :118-150)."""
+    item_off, group_off, dep_off, dep_item, group_id, group_index, names = [0], [0], [0], [], [], [], []
+    for q in queues:
+        pos = {it.id: k for k, it in enumerate(q.queue)}
+        groups: Dict[str, int] = {}
+        for it in q.queue:
+            for dep in it.dependencies:
+                dep_item.append(pos.get(dep, -1))
+            dep_off.append(len(dep_item))
+            if it.group:
+                gid = f"{it.group}_{it.build_variant}_{it.project}_{it.version}"  # compositeGroupID
+                group_id.append(groups.setdefault(gid, len(groups)))
+            else:
+                group_id.append(-1)
+            group_index.append(it.group_index)
+        names.append(list(groups))
+        item_off.append(item_off[-1] + len(q.queue))
+        group_off.append(group_off[-1] + len(groups))
+    a = lambda x, t: np.ascontiguousarray(np.array(x, dtype=t))  # noqa: E731
+    return (a(item_off, np.int64), a(group_off, np.int64), a(dep_off, np.int64), a(dep_item, np.int32), a(group_id, np.int32),
+            a(group_index, np.int32), names)
+
+
+def persisted_dag_input(soa: TaskSoA, table: DistroTable, order: np.ndarray, cap: int = 0):
+    """Host restatement of what evg_rebuild_dispatchers builds on the device: the evg_dag_in of every distro's persisted
+    queue (the first min(length, cap) ranks, cap 0 = EVG_PERSISTED_QUEUE_CAP) from marshalled columns and the rank order
+    (order[task_off[d] + r] = distro-local task at rank r; only the persisted ranks are read).
+    -> (item_off, group_off, dep_off, dep_item, group_id, group_index, group_slot): item k of distro d is rank k; a
+    resident edge becomes the rank of its dependency, -1 past the cap; the group slots that occur are numbered densely in
+    order of first appearance, group_slot[group_off[d] + g] holding the slot of dense group g."""
+    cap = cap or L.EVG_PERSISTED_QUEUE_CAP
+    toff = np.asarray(table.task_off, dtype=np.int64)
+    D = table.n_distros
+    lens = np.minimum(np.diff(toff), cap)
+    item_off = np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
+    N = int(item_off[-1])
+    d_of = np.repeat(np.arange(D, dtype=np.int64), lens)
+    r = np.arange(N, dtype=np.int64) - item_off[d_of]
+    task = toff[d_of] + np.asarray(order, dtype=np.int64)[toff[d_of] + r]
+    rank_of = np.full(soa.n_tasks, -1, dtype=np.int32)
+    rank_of[task] = r
+    if soa.n_edges:
+        deg = soa.dep_off[task + 1] - soa.dep_off[task]
+        dep_off = np.concatenate([[0], np.cumsum(deg)]).astype(np.int64)
+        e = np.repeat(soa.dep_off[task] - dep_off[:-1], deg) + np.arange(int(dep_off[-1]), dtype=np.int64)
+        dep_item = rank_of[np.repeat(toff[d_of], deg) + soa.dep_idx[e]].astype(np.int32)
+    else:
+        dep_off, dep_item = np.zeros(N + 1, dtype=np.int64), np.zeros(0, dtype=np.int32)
+    slot = soa.group_id[task].astype(np.int64)
+    grouped = np.nonzero(slot >= 0)[0]
+    key = np.asarray(table.group_off, dtype=np.int64)[d_of[grouped]] + slot[grouped]
+    _, first_at, inv = np.unique(key, return_index=True, return_inverse=True)
+    head = grouped[first_at]                    # the item that first holds each occurring slot
+    flag = np.zeros(N + 1, dtype=np.int64)
+    flag[head] = 1
+    pos = np.concatenate([[0], np.cumsum(flag[:N])])
+    group_id = np.full(N, -1, dtype=np.int32)
+    group_id[grouped] = pos[head[inv.ravel()]] - pos[item_off[d_of[grouped]]]
+    group_off = pos[item_off].astype(np.int64)
+    group_slot = np.zeros(int(group_off[-1]), dtype=np.int32)
+    group_slot[pos[head]] = slot[head]
+    return (item_off, group_off, dep_off, dep_item, group_id, soa.task_group_order[task].astype(np.int32), group_slot)

@@ -822,6 +822,37 @@ typedef struct {
 int evg_dag_rebuild_batch(evg_ctx* ctx, const evg_dag_in* in, const int64_t* item_off, const int64_t* group_off, int32_t n_distros,
                           int32_t* sorted, int32_t* n_sorted, int32_t* n_cycles, int32_t* unit_items, int32_t* unit_off);
 
+/* What evg_rebuild_dispatchers writes.  Host pointers; the arrays are laid out as evg_dag_rebuild_batch's. */
+typedef struct {
+  int64_t* item_off;   /* n_distros + 1: items of distro d = min(length_d, cap), exactly evg_download_queue's item_off */
+  int32_t* sorted;     /* items_capacity: d.sorted as item (queue) indices, -1 per cyclic component, -2 tail */
+  int32_t* n_sorted;   /* n_distros */
+  int32_t* n_cycles;   /* n_distros */
+  int64_t* group_off;  /* n_distros + 1: the task groups that occur in each persisted queue */
+  int32_t* group_slot; /* groups_capacity: group_slot[group_off[d] + g] = the tick's distro-local group id of DAG group g
+                          of distro d (its name is the shim's string for that slot) */
+  int32_t* unit_items; /* items_capacity */
+  int32_t* unit_off;   /* groups_capacity + n_distros, over group_off above */
+} evg_dispatch_out;
+
+/* basicCachedDAGDispatcherImpl.rebuild (model/task_queue_service_dependency.go:153-252) over the queue PersistTaskQueue
+ * would save (scheduler/task_queue_persister.go:17-41, TaskQueue.Save model/task_queue.go:216-219) for every distro of
+ * the resident tick, built on the device from the tick itself.  Item k of distro d is rank k, the row
+ * evg_download_queue returns, for k < min(length_d, cap), cap = 0 meaning EVG_PERSISTED_QUEUE_CAP; same precondition as
+ * evg_download_queue (after evg_run_resident), on a tick from any entry point that leaves one.
+ *   - edges: a resident edge t -> j is a DAG edge when both rank below the cap (addEdge drops a dependency that is not in
+ *     the persisted queue, :118-150); parallel edges and self-edges as in evg_dag_rebuild_batch;
+ *   - groups: the tick's group slots of distro d that occur among its items, numbered densely in order of first
+ *     appearance (compositeGroupID, :700-702, has Task.GetTaskGroupString's format, model/task/task.go:417-419).
+ * Every output equals what evg_dag_rebuild_batch returns for that queue marshalled on the host.  The tick is left as it
+ * was (outputs, dependency verdicts, alias map, durations, evg_edit_tasks afterwards).
+ * EVG_ERR_INVALID with nothing launched: cap < 0, a null pointer the call needs, items_capacity below the items or
+ * groups_capacity below sum over d of min(group slots of d, items of d) (the tick's group slot count always suffices);
+ * evg_last_error reports both needed sizes.  EVG_ERR_STATE: no resident tick.
+ * Replaces: the evg_download_queue -> dependency-id resolution -> compositeGroupID interning -> evg_dag_rebuild_batch
+ * round trip a shim would make to hand FindNextTask d.sorted and d.taskGroups (:475-476, :527-543). */
+int evg_rebuild_dispatchers(evg_ctx* ctx, int32_t cap, int64_t items_capacity, int64_t groups_capacity, evg_dispatch_out* out);
+
 /* ---- single-distro wrappers: the per-job drop-in ------------------------- */
 
 /* One distro: PrioritizeTasks for `d` (scheduler/scheduler.go:27). */
