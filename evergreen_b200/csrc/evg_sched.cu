@@ -65,6 +65,24 @@ int fail(int code, const char* fmt, ...) {
   return code;
 }
 
+// The CSR offset tables of the C boundary are indexed directly, so each is checked before its first use: off[0 .. n] starts
+// at 0, never decreases, ends at `total` (< 0: its last entry is the count); the error names `who`, `name` and the bad row.
+int check_offsets(const int64_t* off, int64_t n, int64_t total, const char* who, const char* name) {
+  int64_t row = off[0] != 0 ? 0 : -1;
+  for (int64_t i = 0; row < 0 && i < n; i++)
+    if (off[i + 1] < off[i]) row = i + 1;
+  if (row < 0 && total >= 0 && off[n] != total) row = n;
+  if (row < 0) return EVG_OK;
+  return fail(EVG_ERR_INVALID, "%s: %s[%lld] = %lld breaks the offsets (they start at 0, never decrease and end at %s)", who, name,
+              (long long)row, (long long)off[row], total >= 0 ? std::to_string(total).c_str() : "the count");
+}
+
+// One of the nine planner columns of an evg_task_soa is null.
+bool task_cols_missing(const evg_task_soa* t) {
+  return !t->priority || !t->expected_ns || !t->queue_basis_ns || !t->wait_basis_ns || !t->num_dependents || !t->task_group_order ||
+         !t->group_id || !t->version_id || !t->flags;
+}
+
 #define CK(call)                                                                              \
   do {                                                                                        \
     cudaError_t e_ = (call);                                                                  \
@@ -314,7 +332,7 @@ __global__ void __launch_bounds__(256) k_validate(DTasks T, DDistros D, DWork W,
 
 // Task.DependenciesMet over direct dependencies (model/task/task.go:529-543,632-671).
 struct DDeps {
-  int64_t n_tasks;
+  int64_t n_tasks, n_deps;
   const int64_t* dep_off;
   const uint8_t* dep_kind;
   const int32_t* dep_ref;
@@ -324,6 +342,10 @@ struct DDeps {
   const uint8_t* ext_state;
   int64_t n_ext;
 };
+// deps->dep_off is checked by the first kernel that reads a row (k_deps_met, k_pl_deps): a row outside [0, n_deps] or
+// decreasing sets this bit of the error word and is not walked.  Bit 1 there: a dep_ref (or a finder's project row), 2: a status id.
+constexpr int kErrDepOff = 4;
+__device__ __forceinline__ bool deps_row_bad(const DDeps& X, int64_t e0, int64_t e1) { return e0 < 0 || e1 < e0 || e1 > X.n_deps; }
 // met[t] bit 0: Task.DependenciesMet (with the HasDependenciesMet short-circuit); with `both`, bit 1:
 // Task.AllDependenciesSatisfied (task.go:795-821: the same walk without the short-circuit).
 __global__ void __launch_bounds__(256) k_deps_met(DDeps X, uint8_t* met, int* err, int both, const int64_t* __restrict__ dep_fin,
@@ -331,9 +353,10 @@ __global__ void __launch_bounds__(256) k_deps_met(DDeps X, uint8_t* met, int* er
   const int64_t t = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
   if (t >= X.n_tasks) return;
   const int64_t e0 = X.dep_off[t], e1 = X.dep_off[t + 1];
-  bool ok = true;
+  bool ok = !deps_row_bad(X, e0, e1);  // a bad row is walked nowhere below
+  if (!ok) atomicOr(err, kErrDepOff);
   const bool shortcut = (X.task_pre[t] & (EVG_TP_OVERRIDE | EVG_TP_MET_TIME)) != 0;  // HasDependenciesMet task.go:3393
-  if (e1 > e0 && (both || !shortcut)) {
+  if (ok && e1 > e0 && (both || !shortcut)) {
     for (int64_t e = e0; e < e1 && ok; e++) {
       const uint8_t kind = X.dep_kind[e];
       const int32_t ref = X.dep_ref[e];
@@ -589,6 +612,7 @@ __global__ void __launch_bounds__(256) k_pl_deps(DDeps X, DPipe P, uint8_t* __re
   const int64_t t = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
   if (t >= X.n_tasks) return;
   const int64_t e0 = X.dep_off[t], e1 = X.dep_off[t + 1];
+  if (deps_row_bad(X, e0, e1)) { atomicOr(err, kErrDepOff); return; }
   const int32_t own = P.task_status[t];
   bool ok = true, paired = false;
   if (own < 0 || own >= P.n_status) { atomicOr(err, 2); ok = false; }
@@ -1304,7 +1328,7 @@ enum class Cols {
 // Route every distro of the tick, stage the small tables, size the work buffers.  Every mode but kChunked range-checks
 // the ids here (the pipelined call checks chunk by chunk).
 // `edge_off` (D+1, host) is dep_off sampled at the distro boundaries; NULL when the host can read t->dep_off itself.
-int upload_tasks(evg_ctx* c, const evg_task_soa* t, const evg_distro_table* dt, Cols cols = Cols::kCopy,
+int upload_tasks(evg_ctx* c, const char* who, const evg_task_soa* t, const evg_distro_table* dt, Cols cols = Cols::kCopy,
                  const int64_t* edge_off = nullptr) {
   const bool copy_columns = cols == Cols::kCopy, adopt = cols == Cols::kAdopt;
   if (!t || !dt) return fail(EVG_ERR_INVALID, "null task table / distro table");
@@ -1314,11 +1338,12 @@ int upload_tasks(evg_ctx* c, const evg_task_soa* t, const evg_distro_table* dt, 
   if (T >= (int64_t(1) << 31) - 2) return fail(EVG_ERR_INVALID, "n_tasks %lld exceeds 2^31-2 per call", (long long)T);
   if (2 * T + E >= int64_t(0xFFFFFFF0u)) return fail(EVG_ERR_INVALID, "2*n_tasks+n_edges exceeds the 32-bit pair id space");
   if (D > 0 && (!dt->task_off || !dt->group_off || !dt->cfg)) return fail(EVG_ERR_INVALID, "null distro arrays");
-  if (T > 0 && (!t->priority || !t->expected_ns || !t->queue_basis_ns || !t->wait_basis_ns || !t->num_dependents ||
-                !t->task_group_order || !t->group_id || !t->version_id || !t->flags))
-    return fail(EVG_ERR_INVALID, "null task column");
+  if (T > 0 && task_cols_missing(t)) return fail(EVG_ERR_INVALID, "null task column");
   if (E > 0 && (!t->dep_off || !t->dep_idx)) return fail(EVG_ERR_INVALID, "n_edges > 0 but dep_off/dep_idx null");
   if (D == 0 && T != 0) return fail(EVG_ERR_INVALID, "tasks without distros");
+  int rc = D > 0 ? check_offsets(dt->task_off, D, T, who, "task_off") : EVG_OK;
+  if (rc == EVG_OK && D > 0) rc = check_offsets(dt->group_off, D, -1, who, "group_off");
+  if (rc != EVG_OK) return rc;
   std::vector<int64_t> unit_base(size_t(D) + 1, 0), dtile_off(size_t(D) + 1, 0);
   std::vector<int32_t> tile_distro, list[kRoutes];
   std::vector<int64_t> tile_start;
@@ -1350,13 +1375,7 @@ int upload_tasks(evg_ctx* c, const evg_task_soa* t, const evg_distro_table* dt, 
   // tasks held the whole tick, then ~50 GroupVersions distros of 129-1024 tasks whose version units are walked member by
   // member).  The general path spreads every distro over all SMs, so sparse classes go there.
   int64_t n_class[kBigUnits + 1] = {};
-  for (int32_t d = 0; d < D; d++) {
-    const int64_t a = dt->task_off[d], b = dt->task_off[d + 1];
-    if (d == 0 && (a != 0 || dt->group_off[0] != 0)) return fail(EVG_ERR_INVALID, "offsets must start at 0");
-    if (b < a || dt->group_off[d + 1] < dt->group_off[d]) return fail(EVG_ERR_INVALID, "offsets of distro %d decrease", d);
-    if (b > T) return fail(EVG_ERR_INVALID, "task_off of distro %d exceeds n_tasks", d);
-    n_class[size_class(d)]++;
-  }
+  for (int32_t d = 0; d < D; d++) n_class[size_class(d)]++;
   const char* sparse_env = getenv("EVG_SPARSE_CLASS");  // tests set 0 to keep every class on its own kernel
   const int64_t sparse = sparse_env ? atoll(sparse_env) : kSparseClass;
   // The route of distro d: its size class, after the sparse-class rule (needs every class's size: the count above).
@@ -1389,7 +1408,6 @@ int upload_tasks(evg_ctx* c, const evg_task_soa* t, const evg_distro_table* dt, 
     }
     dtile_off[d + 1] = int64_t(tile_distro.size());
   }
-  if (D > 0 && dt->task_off[D] != T) return fail(EVG_ERR_INVALID, "task_off[n_distros] != n_tasks");
   const int64_t G = D > 0 ? dt->group_off[D] : 0;
   if (G > 0 && !dt->group_max_hosts) return fail(EVG_ERR_INVALID, "null group_max_hosts");
   const int64_t U = unit_base[D];
@@ -1548,15 +1566,14 @@ int upload_tasks(evg_ctx* c, const evg_task_soa* t, const evg_distro_table* dt, 
   return EVG_OK;
 }
 
-int upload_hosts(evg_ctx* c, const evg_host_soa* h, const int64_t* host_off, const evg_alloc_cfg* acfg, int32_t D) {
+int upload_hosts(evg_ctx* c, const char* who, const evg_host_soa* h, const int64_t* host_off, const evg_alloc_cfg* acfg, int32_t D) {
   if (!h || (D > 0 && !acfg)) return fail(EVG_ERR_INVALID, "null host table / allocator config");
   const int64_t H = h->n_hosts;
   if (H < 0) return fail(EVG_ERR_INVALID, "negative n_hosts");
   if (D > 0 && !host_off) return fail(EVG_ERR_INVALID, "null host_off");
   if (D == 0 && H != 0) return fail(EVG_ERR_INVALID, "hosts without distros");
-  for (int32_t d = 0; d < D; d++)
-    if (host_off[d + 1] < host_off[d] || (d == 0 && host_off[0] != 0)) return fail(EVG_ERR_INVALID, "bad host_off at distro %d", d);
-  if (D > 0 && host_off[D] != H) return fail(EVG_ERR_INVALID, "host_off[n_distros] != n_hosts");
+  const int rc = D > 0 ? check_offsets(host_off, D, H, who, "host_off") : EVG_OK;
+  if (rc != EVG_OK) return rc;
   if (H > 0 && (!h->flags || !h->group_id || !h->expected_ns || !h->std_ns || !h->start_ns)) return fail(EVG_ERR_INVALID, "null host column");
   cudaStream_t s = c->stream;
   UP(s, c->b_hflags, h->flags, H, uint32_t);
@@ -1944,20 +1961,25 @@ void evg_shutdown(evg_ctx* c) {
   delete c;  // its buffers free themselves, on the device selected above
 }
 
-int evg_upload(evg_ctx* c, const evg_task_soa* tasks, const evg_distro_table* distros, const evg_host_soa* hosts,
-               const int64_t* host_off, const evg_alloc_cfg* acfg) {
-  if (!c) return fail(EVG_ERR_INVALID, "null context");
-  LOCK(c);
+// evg_upload for the entry point `who` (the caller holds the context's lock)
+static int upload(evg_ctx* c, const char* who, const evg_task_soa* tasks, const evg_distro_table* distros, const evg_host_soa* hosts,
+                  const int64_t* host_off, const evg_alloc_cfg* acfg) {
   CK(cudaSetDevice(c->device));
-  int rc = upload_tasks(c, tasks, distros);
+  int rc = upload_tasks(c, who, tasks, distros);
   if (rc != EVG_OK) return rc;
   if (hosts) {
-    rc = upload_hosts(c, hosts, host_off, acfg, distros->n_distros);
+    rc = upload_hosts(c, who, hosts, host_off, acfg, distros->n_distros);
     if (rc != EVG_OK) return rc;
     CK(cudaStreamSynchronize(c->stream));
   }
   c->editable = true;
   return EVG_OK;
+}
+int evg_upload(evg_ctx* c, const evg_task_soa* tasks, const evg_distro_table* distros, const evg_host_soa* hosts,
+               const int64_t* host_off, const evg_alloc_cfg* acfg) {
+  if (!c) return fail(EVG_ERR_INVALID, "null context");
+  LOCK(c);
+  return upload(c, "evg_upload", tasks, distros, hosts, host_off, acfg);
 }
 
 __global__ void k_gather_i64(const int64_t* __restrict__ src, const int64_t* __restrict__ at, int64_t* __restrict__ out, int n) {
@@ -2040,10 +2062,10 @@ int evg_upload_device(evg_ctx* c, const evg_task_soa* tasks, const evg_distro_ta
     CK(cudaMemcpyAsync(edge_off.data(), c->b_rn1.p, sizeof(int64_t) * size_t(D + 1), cudaMemcpyDeviceToHost, c->stream));
     CK(cudaStreamSynchronize(c->stream));
   }
-  int rc = upload_tasks(c, tasks, distros, Cols::kAdopt, edge_off.empty() ? nullptr : edge_off.data());
+  int rc = upload_tasks(c, "evg_upload_device", tasks, distros, Cols::kAdopt, edge_off.empty() ? nullptr : edge_off.data());
   if (rc != EVG_OK) return rc;
   if (hosts) {
-    rc = upload_hosts(c, hosts, host_off, acfg, distros->n_distros);
+    rc = upload_hosts(c, "evg_upload_device", hosts, host_off, acfg, distros->n_distros);
     if (rc != EVG_OK) return rc;
     CK(cudaStreamSynchronize(c->stream));
   }
@@ -2195,7 +2217,7 @@ int evg_plan_batch(evg_ctx* c, const evg_task_soa* tasks, const evg_distro_table
                    evg_plan_out* out) {
   if (!c) return fail(EVG_ERR_INVALID, "null context");
   LOCK(c);
-  int rc = evg_upload(c, tasks, distros, nullptr, nullptr, nullptr);
+  int rc = upload(c, "evg_plan_batch", tasks, distros, nullptr, nullptr, nullptr);
   if (rc != EVG_OK) return rc;
   c->editable = false;  // a one-shot call's tick is not a resident one to edit
   rc = evg_run_resident(c, now_ns, opts);
@@ -2320,14 +2342,14 @@ int evg_plan_and_alloc_batch(evg_ctx* c, const evg_task_soa* tasks, const evg_di
   if (!(opts & EVG_OPT_BREAKDOWN) && tasks && distros && tasks->n_tasks >= (int64_t(1) << 21)) {
     // large tick: stage the small tables, then pipeline the columns chunk by chunk
     CK(cudaSetDevice(c->device));
-    int rc0 = upload_tasks(c, tasks, distros, Cols::kChunked);
+    int rc0 = upload_tasks(c, "evg_plan_and_alloc_batch", tasks, distros, Cols::kChunked);
     if (rc0 != EVG_OK) return rc0;
-    rc0 = upload_hosts(c, hosts, host_off, acfg, distros->n_distros);
+    rc0 = upload_hosts(c, "evg_plan_and_alloc_batch", hosts, host_off, acfg, distros->n_distros);
     if (rc0 != EVG_OK) return rc0;
     CK(cudaStreamSynchronize(c->stream));
     return plan_and_alloc_pipelined(c, tasks, distros, hosts, host_off, acfg, now_ns, plan_out, alloc_out);
   }
-  int rc = evg_upload(c, tasks, distros, hosts, host_off, acfg);
+  int rc = upload(c, "evg_plan_and_alloc_batch", tasks, distros, hosts, host_off, acfg);
   if (rc != EVG_OK) return rc;
   c->editable = false;  // a one-shot call's tick is not a resident one to edit
   rc = evg_run_resident(c, now_ns, opts);
@@ -2342,10 +2364,12 @@ int evg_alloc_batch(evg_ctx* c, const evg_host_soa* hosts, const int64_t* host_o
   LOCK(c);
   if (n_distros < 0 || (n_distros > 0 && (!info || !group_off || !out))) return fail(EVG_ERR_INVALID, "evg_alloc_batch: null argument");
   CK(cudaSetDevice(c->device));
+  int rc = n_distros > 0 ? check_offsets(group_off, n_distros, -1, "evg_alloc_batch", "group_off") : EVG_OK;
+  if (rc != EVG_OK) return rc;
   const int64_t G = n_distros > 0 ? group_off[n_distros] : 0;
   if (G > 0 && !groups) return fail(EVG_ERR_INVALID, "evg_alloc_batch: groups is null");
   c->have_tasks = false;  // the resident planner inputs no longer match the tables of this call (and upload_hosts must not list distros from them)
-  int rc = upload_hosts(c, hosts, host_off, cfg, n_distros);
+  rc = upload_hosts(c, "evg_alloc_batch", hosts, host_off, cfg, n_distros);
   if (rc != EVG_OK) return rc;
   cudaStream_t s = c->stream;
   CK(c->b_groupoff.ensure(sizeof(int64_t) * size_t(n_distros + 1)));
@@ -2371,16 +2395,28 @@ int evg_alloc_batch(evg_ctx* c, const evg_host_soa* hosts, const int64_t* host_o
   return EVG_OK;
 }
 
+// The device view of the dependency table deps_to_device staged from `in`.
+static DDeps ddeps(const evg_ctx* c, const evg_deps_in* in) {
+  const auto& x = c->deps;
+  DDeps d;
+  d.n_tasks = in->n_tasks; d.n_deps = in->n_deps; d.n_ext = in->n_ext;
+  d.dep_off = x.off.as<int64_t>(); d.dep_kind = x.kind.as<uint8_t>(); d.dep_ref = x.ref.as<int32_t>(); d.dep_want = x.want.as<uint8_t>();
+  d.task_state = x.state.as<uint8_t>(); d.task_pre = x.pre.as<uint8_t>(); d.ext_state = x.ext.as<uint8_t>();
+  return d;
+}
+
 // Stage an evg_deps_in table and run k_deps_met into deps.met (left on the device); `both` adds the no-short-circuit bit.
-static int deps_to_device(evg_ctx* c, const evg_deps_in* in, int both, const int64_t* dep_finished = nullptr, int64_t now = 0,
-                          bool want_stamp = false) {
+// The host checks the ends of dep_off; its rows, n_tasks of them, are checked by k_deps_met (kErrDepOff).
+static int deps_to_device(evg_ctx* c, const char* who, const evg_deps_in* in, int both, const int64_t* dep_finished = nullptr,
+                          int64_t now = 0, bool want_stamp = false) {
   const int64_t T = in->n_tasks, E = in->n_deps, X = in->n_ext;
   if (T < 0 || E < 0 || X < 0) return fail(EVG_ERR_INVALID, "negative sizes");
   if (T == 0) return EVG_OK;
   if (!in->dep_off || !in->task_state || !in->task_pre) return fail(EVG_ERR_INVALID, "null task arrays");
   if (E > 0 && (!in->dep_kind || !in->dep_ref || !in->dep_want)) return fail(EVG_ERR_INVALID, "null dependency arrays");
   if (X > 0 && !in->ext_state) return fail(EVG_ERR_INVALID, "null ext_state");
-  if (in->dep_off[0] != 0 || in->dep_off[T] != E) return fail(EVG_ERR_INVALID, "dep_off does not span n_deps");
+  if (in->dep_off[0] != 0 || in->dep_off[T] != E)
+    return fail(EVG_ERR_INVALID, "%s: deps->dep_off runs from %lld to %lld, not from 0 to n_deps", who, (long long)in->dep_off[0], (long long)in->dep_off[T]);
   cudaStream_t s = c->stream;
   auto& x = c->deps;
   UP(s, x.off, in->dep_off, T + 1, int64_t);
@@ -2401,14 +2437,17 @@ static int deps_to_device(evg_ctx* c, const evg_deps_in* in, int both, const int
       fin = x.fin.as<int64_t>();
     }
   }
-  DDeps d;
-  d.n_tasks = T; d.dep_off = x.off.as<int64_t>(); d.dep_kind = x.kind.as<uint8_t>(); d.dep_ref = x.ref.as<int32_t>();
-  d.dep_want = x.want.as<uint8_t>(); d.task_state = x.state.as<uint8_t>(); d.task_pre = x.pre.as<uint8_t>();
-  d.ext_state = x.ext.as<uint8_t>(); d.n_ext = X;
-  k_deps_met<<<grid_for(T, 256), 256, 0, s>>>(d, x.met.as<uint8_t>(), c->b_err.as<int>(), both, fin, now, stamp);
+  k_deps_met<<<grid_for(T, 256), 256, 0, s>>>(ddeps(c, in), x.met.as<uint8_t>(), c->b_err.as<int>(), both, fin, now, stamp);
   c->launches++;
   CK(cudaGetLastError());
   return EVG_OK;
+}
+
+// The device-side checks of the dependency and finder passes (c->b_err, bits as at kErrDepOff) as one message.
+static int deps_bad(const char* who, int bad) {
+  if (bad & kErrDepOff) return fail(EVG_ERR_INVALID, "%s: deps->dep_off decreases or leaves [0, n_deps] at some row", who);
+  if (bad & 2) return fail(EVG_ERR_INVALID, "%s: a status id of the evg_pipeline_in is outside [0, n_status)", who);
+  return fail(EVG_ERR_INVALID, "%s: a dep_ref or project row is out of range", who);
 }
 
 int evg_deps_met_batch(evg_ctx* c, const evg_deps_in* in, uint8_t* met) {
@@ -2421,13 +2460,13 @@ int evg_deps_met_batch(evg_ctx* c, const evg_deps_in* in, uint8_t* met) {
   CK(cudaMemsetAsync(c->b_err.p, 0, sizeof(int) * 4, s));
   c->launches = 0;
   c->deps_resident = false;  // deps_to_device overwrites the resident tick's verdicts and stamps
-  int rc = deps_to_device(c, in, 0);
+  int rc = deps_to_device(c, "evg_deps_met_batch", in, 0);
   if (rc != EVG_OK) return rc;
   int bad = 0;
   CK(cudaMemcpyAsync(met, c->deps.met.p, size_t(in->n_tasks), cudaMemcpyDeviceToHost, s));
   CK(cudaMemcpyAsync(&bad, c->b_err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
-  if (bad) return fail(EVG_ERR_INVALID, "a dep_ref is out of range");
+  if (bad) return deps_bad("evg_deps_met_batch", bad);
   return EVG_OK;
 }
 
@@ -2438,12 +2477,12 @@ int evg_upload_with_deps(evg_ctx* c, const evg_task_soa* tasks, const evg_distro
   LOCK(c);
   if (!tasks || !deps) return fail(EVG_ERR_INVALID, "evg_upload_with_deps: null argument");
   if (deps->n_tasks != tasks->n_tasks) return fail(EVG_ERR_INVALID, "deps covers %lld tasks, the task table %lld", (long long)deps->n_tasks, (long long)tasks->n_tasks);
-  int rc = evg_upload(c, tasks, distros, hosts, host_off, acfg);
+  int rc = upload(c, "evg_upload_with_deps", tasks, distros, hosts, host_off, acfg);
   if (rc != EVG_OK) return rc;
   const int64_t T = tasks->n_tasks;
   if (T == 0) return EVG_OK;
   cudaStream_t s = c->stream;
-  rc = deps_to_device(c, deps, 0, dep_finished_ns, now_ns, /*want_stamp=*/true);
+  rc = deps_to_device(c, "evg_upload_with_deps", deps, 0, dep_finished_ns, now_ns, /*want_stamp=*/true);
   if (rc != EVG_OK) { c->have_tasks = false; return rc; }
   k_apply_deps<<<grid_for(T, 256), 256, 0, s>>>(T, c->deps.met.as<uint8_t>(), c->deps.stamp.as<int64_t>(), c->tasks.flags.as<uint32_t>(),
                                                 c->tasks.wb.as<int64_t>());
@@ -2452,7 +2491,7 @@ int evg_upload_with_deps(evg_ctx* c, const evg_task_soa* tasks, const evg_distro
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(&bad, c->b_err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
-  if (bad) { c->have_tasks = false; return fail(EVG_ERR_INVALID, "a dep_ref is out of range"); }
+  if (bad) { c->have_tasks = false; return deps_bad("evg_upload_with_deps", bad); }
   c->deps_resident = true;
   return EVG_OK;
 }
@@ -2548,13 +2587,8 @@ int evg_resolve_durations(evg_ctx* c, const evg_duration_in* in, int64_t now_ns)
   if (R > 0 && (!h->key || !h->time_taken_ns || !h->start_ns || !h->finish_ns || !h->flags))
     return fail(EVG_ERR_INVALID, "evg_resolve_durations: null history column");
   if (P > 0 && !in->pair_key_off) return fail(EVG_ERR_INVALID, "evg_resolve_durations: null pair_key_off");
-  if (in->pair_key_off) {
-    const int64_t* o = in->pair_key_off;
-    bool ok = o[0] == 0 && o[P] == K;
-    for (int32_t p = 0; ok && p < P; p++) ok = o[p + 1] >= o[p];
-    if (!ok) return fail(EVG_ERR_INVALID, "evg_resolve_durations: pair_key_off must start at 0, end at n_keys and never decrease");
-  }
   int rc;
+  if (in->pair_key_off && (rc = check_offsets(in->pair_key_off, P, K, "evg_resolve_durations", "pair_key_off")) != EVG_OK) return rc;
   if (in->tasks && (rc = check_duration_cache(in->tasks, c->T, "tasks")) != EVG_OK) return rc;
   if (in->hosts && (rc = check_duration_cache(in->hosts, c->H, "hosts")) != EVG_OK) return rc;
   CK(cudaSetDevice(c->device));
@@ -2655,18 +2689,19 @@ int evg_download_durations(evg_ctx* c, evg_duration_out* tasks, evg_duration_out
 // The finder tables of evg_find_runnable_batch and evg_plan_from_finder: checked, staged into pf.*, and k_runnable's view
 // of them (the caller sets r->met).  `any_deps`: some distro's finder reads the dependency verdicts.  `pipe`: the pipeline
 // codes are allowed, `any_pipe` / `pipe_deps` report whether some distro uses one / EVG_FINDER_PIPELINE.  n_distros > 0.
-static int stage_finder(evg_ctx* c, const evg_runnable_in* in, DRunnable* r, bool* any_deps, const evg_pipeline_in* pipe = nullptr,
-                        bool* any_pipe = nullptr, bool* pipe_deps = nullptr) {
+static int stage_finder(evg_ctx* c, const char* who, const evg_runnable_in* in, DRunnable* r, bool* any_deps,
+                        const evg_pipeline_in* pipe = nullptr, bool* any_pipe = nullptr, bool* pipe_deps = nullptr) {
   const int64_t T = in->n_tasks;
   const int32_t D = in->n_distros, P = in->n_projects;
   if (!in->task_off || !in->valid_off || !in->finder) return fail(EVG_ERR_INVALID, "null distro arrays");
   if (T > 0 && (!in->sched || !in->project)) return fail(EVG_ERR_INVALID, "null task column");
   if (P > 0 && !in->project_flags) return fail(EVG_ERR_INVALID, "null project_flags");
-  if (in->task_off[0] != 0 || in->task_off[D] != T || in->valid_off[0] != 0) return fail(EVG_ERR_INVALID, "offsets do not span the tables");
+  int rc = check_offsets(in->task_off, D, T, who, "task_off");
+  if (rc == EVG_OK) rc = check_offsets(in->valid_off, D, -1, who, "valid_off");
+  if (rc != EVG_OK) return rc;
   *any_deps = false;
   const uint8_t max_code = pipe ? EVG_FINDER_PIPELINE_NO_DEPS : EVG_FINDER_ALTERNATE;
   for (int32_t d = 0; d < D; d++) {
-    if (in->task_off[d + 1] < in->task_off[d] || in->valid_off[d + 1] < in->valid_off[d]) return fail(EVG_ERR_INVALID, "offsets of distro %d decrease", d);
     if (in->finder[d] > max_code)
       return fail(EVG_ERR_INVALID, in->finder[d] <= EVG_FINDER_PIPELINE_NO_DEPS ? "distro %d: the pipeline finder (%d) needs an evg_pipeline_in"
                                                                                  : "distro %d: unknown finder %d", d, int(in->finder[d]));
@@ -2718,30 +2753,20 @@ static int pipeline_deps(evg_ctx* c, const evg_deps_in* x, const evg_pipeline_in
   UP(s, p.ext_status, pipe->ext_status, X, int32_t);
   UP(s, p.task_unatt, pipe->task_unattainable, T, uint8_t);
   UP(s, p.ext_unatt, pipe->ext_unattainable, X, uint8_t);
-  const auto& d = c->deps;
-  DDeps dd;
-  dd.n_tasks = T; dd.dep_off = d.off.as<int64_t>(); dd.dep_kind = d.kind.as<uint8_t>(); dd.dep_ref = d.ref.as<int32_t>();
-  dd.dep_want = d.want.as<uint8_t>(); dd.task_state = d.state.as<uint8_t>(); dd.task_pre = d.pre.as<uint8_t>();
-  dd.ext_state = d.ext.as<uint8_t>(); dd.n_ext = X;
   DPipe dp;
   dp.n_status = pipe->n_status; dp.dep_status = p.dep_status.as<int32_t>(); dp.task_status = p.task_status.as<int32_t>();
   dp.ext_status = p.ext_status.as<int32_t>(); dp.task_unatt = p.task_unatt.as<uint8_t>(); dp.ext_unatt = p.ext_unatt.as<uint8_t>();
-  k_pl_deps<<<grid_for(T, 256), 256, 0, s>>>(dd, dp, c->deps.met.as<uint8_t>(), c->b_err.as<int>());
+  k_pl_deps<<<grid_for(T, 256), 256, 0, s>>>(ddeps(c, x), dp, c->deps.met.as<uint8_t>(), c->b_err.as<int>());
   c->launches++;
   CK(cudaGetLastError());
   return EVG_OK;
-}
-
-// The device-side range checks of the finder pass, as one message (err bit 1: project row / dep_ref, bit 2: status id).
-static int finder_bad(int bad) {
-  if (bad & 2) return fail(EVG_ERR_INVALID, "a status id of the evg_pipeline_in is outside [0, n_status)");
-  return fail(EVG_ERR_INVALID, "a project row or dep_ref is out of range");
 }
 
 // evg_find_runnable_batch and evg_find_runnable_ex (pipe == NULL: the former)
 static int find_runnable(evg_ctx* c, const evg_runnable_in* in, const evg_pipeline_in* pipe, int32_t* runnable, int64_t* count) {
   if (!c || !in) return fail(EVG_ERR_INVALID, "evg_find_runnable_batch: null argument");
   LOCK(c);
+  const char* who = pipe ? "evg_find_runnable_ex" : "evg_find_runnable_batch";
   const int64_t T = in->n_tasks;
   const int32_t D = in->n_distros, P = in->n_projects;
   if (T < 0 || D < 0 || P < 0) return fail(EVG_ERR_INVALID, "negative sizes");
@@ -2749,7 +2774,7 @@ static int find_runnable(evg_ctx* c, const evg_runnable_in* in, const evg_pipeli
   if (!count || (T > 0 && !runnable)) return fail(EVG_ERR_INVALID, "null output");
   DRunnable r;
   bool any_deps, any_pipe = false, pipe_deps = false;
-  int rc = stage_finder(c, in, &r, &any_deps, pipe, &any_pipe, &pipe_deps);
+  int rc = stage_finder(c, who, in, &r, &any_deps, pipe, &any_pipe, &pipe_deps);
   if (rc != EVG_OK) return rc;
   if (any_deps && T > 0 && (!in->deps || in->deps->n_tasks != T)) return fail(EVG_ERR_INVALID, "a finder checks dependencies but deps is null or of another size");
   cudaStream_t s = c->stream;
@@ -2758,7 +2783,7 @@ static int find_runnable(evg_ctx* c, const evg_runnable_in* in, const evg_pipeli
   c->launches = 0;
   c->have_tasks = false;  // the tick's dependency verdicts and stamps are overwritten: a finder batch ends the resident tick
   if (any_deps && T > 0) {
-    rc = deps_to_device(c, in->deps, 1);
+    rc = deps_to_device(c, who, in->deps, 1);
     if (rc != EVG_OK) return rc;
     if (pipe_deps) {
       rc = pipeline_deps(c, in->deps, pipe);
@@ -2778,7 +2803,7 @@ static int find_runnable(evg_ctx* c, const evg_runnable_in* in, const evg_pipeli
   CK(cudaMemcpyAsync(count, c->pf.count.p, sizeof(int64_t) * size_t(D), cudaMemcpyDeviceToHost, s));
   CK(cudaMemcpyAsync(&bad, c->b_err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
-  if (bad) return finder_bad(bad);
+  if (bad) return deps_bad(who, bad);
   return EVG_OK;
 }
 int evg_find_runnable_batch(evg_ctx* c, const evg_runnable_in* in, int32_t* runnable, int64_t* count) {
@@ -2983,20 +3008,6 @@ __global__ void __launch_bounds__(256) k_kept_mask(int64_t n, int32_t D, const i
   if (k >= 0) keep[off[d] + k] = 1;
 }
 
-// A CSR offset array over n rows that spans `total` entries starts at 0, ends at total and never decreases: the first
-// row where `off` fails that (n: it does not start at 0 or end at total), -1 when it holds.
-static int64_t csr_bad_row(const int64_t* off, int64_t n, int64_t total) {
-  if (off[0] != 0 || off[n] != total) return n;
-  for (int64_t j = 0; j < n; j++)
-    if (off[j + 1] < off[j]) return j;
-  return -1;
-}
-static int check_csr(int64_t bad_row, int64_t n, const char* what) {
-  if (bad_row < 0) return EVG_OK;
-  if (bad_row == n) return fail(EVG_ERR_INVALID, "%s does not span n_edges", what);
-  return fail(EVG_ERR_INVALID, "%s decreases at row %lld", what, (long long)bad_row);
-}
-
 // Exclusive scan of n int32 counts into out[0 .. n] (int64; out[n] = the total); `sum` holds (n + 1023) / 1024 + 1 int64.
 static void scan_counts(evg_ctx* c, const int32_t* in, int64_t n, int64_t* out, int64_t* sum) {
   const int64_t nb = (n + 1023) / 1024;
@@ -3027,7 +3038,7 @@ static int shadow_cols(evg_ctx* c, int64_t Tn, EdDst* o) {
 
 // The composed table in the shadow set (Tn rows) and in ed.dep_off / ed.dep_idx (En edges; edge_off: dep_off at the
 // distro boundaries) becomes the resident one, routed, sized and range-checked like an upload.  An error leaves no tick.
-static int install_composed(evg_ctx* c, int64_t Tn, int64_t En, const int64_t* edge_off, const evg_distro_table* distros) {
+static int install_composed(evg_ctx* c, const char* who, int64_t Tn, int64_t En, const int64_t* edge_off, const evg_distro_table* distros) {
   auto& e = c->ed;
   c->tasks.swap(e.out);
   if (En > 0) { c->b_depoff.swap(e.dep_off); c->b_depidx.swap(e.dep_idx); }
@@ -3038,7 +3049,7 @@ static int install_composed(evg_ctx* c, int64_t Tn, int64_t En, const int64_t* e
   ts.group_id = c->tasks.gid.as<int32_t>(); ts.version_id = c->tasks.vid.as<int32_t>(); ts.flags = c->tasks.flags.as<uint32_t>();
   ts.expected_ns = c->tasks.exp.as<int64_t>(); ts.queue_basis_ns = c->tasks.qb.as<int64_t>(); ts.wait_basis_ns = c->tasks.wb.as<int64_t>();
   if (En > 0) { ts.dep_off = c->b_depoff.as<int64_t>(); ts.dep_idx = c->b_depidx.as<int32_t>(); }
-  int rc = upload_tasks(c, &ts, distros, Cols::kResident, En > 0 ? edge_off : nullptr);
+  int rc = upload_tasks(c, who, &ts, distros, Cols::kResident, En > 0 ? edge_off : nullptr);
   if (rc != EVG_OK) { c->have_tasks = false; return rc; }
   return EVG_OK;
 }
@@ -3046,7 +3057,7 @@ static int install_composed(evg_ctx* c, int64_t Tn, int64_t En, const int64_t* e
 // The rows of O that ed.keep marks (O.n entries, staged by the caller) survive in their order, distro d's inserted rows
 // m.ins_off[d] .. m.ins_off[d+1] of In follow them, and the composed table over `distros` becomes the resident tick.  The
 // caller fills m but for new_off, keep, pos and src.  A device-side error leaves no resident tick.
-static int compose_tick(evg_ctx* c, EdMap m, const DTasks& O, const DTasks& In, const evg_distro_table* distros) {
+static int compose_tick(evg_ctx* c, const char* who, EdMap m, const DTasks& O, const DTasks& In, const evg_distro_table* distros) {
   cudaStream_t s = c->stream;
   auto& e = c->ed;
   const int32_t D = m.D;
@@ -3104,7 +3115,7 @@ static int compose_tick(evg_ctx* c, EdMap m, const DTasks& O, const DTasks& In, 
     }
   }
   // ---- 4. the shadow set becomes the resident one
-  return install_composed(c, Tn, En, edge_off.data(), distros);
+  return install_composed(c, who, Tn, En, edge_off.data(), distros);
 }
 
 // --------------------------------------------------------------------------
@@ -3116,28 +3127,29 @@ static int plan_from_finder(evg_ctx* c, const evg_runnable_in* in, const evg_pip
                             const int64_t* dep_finished_ns, int64_t now_ns, int32_t* runnable, int64_t* count) {
   if (!c || !in || !cand || !distros) return fail(EVG_ERR_INVALID, "evg_plan_from_finder: null argument");
   LOCK(c);
+  const char* who = pipe ? "evg_plan_from_finder_ex" : "evg_plan_from_finder";
   const int64_t T = in->n_tasks, E = cand->n_edges;
   const int32_t D = in->n_distros, P = in->n_projects;
   if (T < 0 || D < 0 || P < 0 || E < 0) return fail(EVG_ERR_INVALID, "negative sizes");
   if (cand->n_tasks != T || distros->n_distros != D) return fail(EVG_ERR_INVALID, "the candidate table, the finder table and the distro table disagree on their sizes");
-  if (D == 0) return T == 0 ? evg_upload(c, cand, distros, hosts, host_off, acfg) : fail(EVG_ERR_INVALID, "tasks without distros");
+  if (D == 0) return T == 0 ? upload(c, who, cand, distros, hosts, host_off, acfg) : fail(EVG_ERR_INVALID, "tasks without distros");
   if (!count) return fail(EVG_ERR_INVALID, "null count");
   // a composed row's source row is 32-bit (compose_tick's src)
   if (T > (int64_t(1) << 31) - 2) return fail(EVG_ERR_INVALID, "evg_plan_from_finder: %lld candidates exceed 2^31-2", (long long)T);
   if (!distros->task_off) return fail(EVG_ERR_INVALID, "null distro arrays");
   if (T > 0 && (!in->deps || in->deps->n_tasks != T)) return fail(EVG_ERR_INVALID, "evg_plan_from_finder needs the candidates' dependency table (the planner's EVG_TF_DEPS_MET comes from it)");
-  if (T > 0 && (!cand->priority || !cand->expected_ns || !cand->queue_basis_ns || !cand->wait_basis_ns || !cand->num_dependents ||
-                !cand->task_group_order || !cand->group_id || !cand->version_id || !cand->flags))
-    return fail(EVG_ERR_INVALID, "null candidate column");
+  if (T > 0 && task_cols_missing(cand)) return fail(EVG_ERR_INVALID, "null candidate column");
   if (E > 0 && (!cand->dep_off || !cand->dep_idx)) return fail(EVG_ERR_INVALID, "null candidate dependency edges");
   // The candidates' dep_off (8 B per candidate, ~10 ms of host memory reads at 8e6 candidates) is checked on a second
   // host thread while this one stages the tables and the device runs the finders; it indexes nothing before step 4.
-  // (Where no thread can be started, the check runs at get().)
-  std::future<int64_t> dep_off_bad;
-  if (E > 0 && T > 0) dep_off_bad = std::async(std::launch::async | std::launch::deferred, csr_bad_row, cand->dep_off, T, E);
+  // (Where no thread can be started, the check runs at get().)  The thread hands back its message, empty when it passed.
+  std::future<std::string> dep_off_err;
+  if (E > 0 && T > 0)
+    dep_off_err = std::async(std::launch::async | std::launch::deferred,
+                             [=] { return check_offsets(cand->dep_off, T, E, who, "candidates->dep_off") == EVG_OK ? std::string() : g_err; });
   DRunnable r;
   bool any_deps, any_pipe = false, pipe_deps = false;
-  int rc = stage_finder(c, in, &r, &any_deps, pipe, &any_pipe, &pipe_deps);
+  int rc = stage_finder(c, who, in, &r, &any_deps, pipe, &any_pipe, &pipe_deps);
   if (rc != EVG_OK) return rc;
   for (int32_t d = 0; d <= D; d++)
     if (in->task_off[d] != distros->task_off[d]) return fail(EVG_ERR_INVALID, "the finder table and the distro table cut the candidates differently at distro %d", d);
@@ -3148,10 +3160,10 @@ static int plan_from_finder(evg_ctx* c, const evg_runnable_in* in, const evg_pip
   c->have_tasks = false;
   if (T == 0) {
     for (int32_t d = 0; d < D; d++) count[d] = 0;
-    return evg_upload(c, cand, distros, hosts, host_off, acfg);
+    return upload(c, who, cand, distros, hosts, host_off, acfg);
   }
   // 1. Task.DependenciesMet / AllDependenciesSatisfied of every candidate, with the DependenciesMetTime stamps
-  rc = deps_to_device(c, in->deps, 1, dep_finished_ns, now_ns, /*want_stamp=*/true);
+  rc = deps_to_device(c, who, in->deps, 1, dep_finished_ns, now_ns, /*want_stamp=*/true);
   if (rc != EVG_OK) return rc;
   if (pipe_deps) {
     rc = pipeline_deps(c, in->deps, pipe);
@@ -3173,9 +3185,9 @@ static int plan_from_finder(evg_ctx* c, const evg_runnable_in* in, const evg_pip
   CK(cudaMemcpyAsync(&bad, c->b_err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
   if (runnable) CK(cudaMemcpyAsync(runnable, pf.kept.p, sizeof(int32_t) * size_t(T), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
-  if (bad) return finder_bad(bad);
-  rc = dep_off_bad.valid() ? check_csr(dep_off_bad.get(), T, "evg_plan_from_finder: the candidate dep_off") : EVG_OK;
-  if (rc != EVG_OK) return rc;
+  if (bad) return deps_bad(who, bad);
+  const std::string dep_off_msg = dep_off_err.valid() ? dep_off_err.get() : std::string();
+  if (!dep_off_msg.empty()) return fail(EVG_ERR_INVALID, "%s", dep_off_msg.c_str());
   std::vector<int64_t> new_off(size_t(D) + 1, 0);
   for (int32_t d = 0; d < D; d++) {
     if (count[d] < 0 || count[d] > in->task_off[d + 1] - in->task_off[d]) return fail(EVG_ERR_CUDA, "finder count out of range");
@@ -3199,13 +3211,8 @@ static int plan_from_finder(evg_ctx* c, const evg_runnable_in* in, const evg_pip
   if (any_pipe) {
     // what the pipeline distros' planner receives: their verdicts (k_pl_plan needs the keep mask), and no candidate
     // edges for EVG_FINDER_PIPELINE rows (compose_tick then re-indexes the rest as for any finder)
-    const auto& d = c->deps;
-    DDeps dd;
-    dd.n_tasks = T; dd.dep_off = d.off.as<int64_t>(); dd.dep_kind = d.kind.as<uint8_t>(); dd.dep_ref = d.ref.as<int32_t>();
-    dd.dep_want = d.want.as<uint8_t>(); dd.task_state = d.state.as<uint8_t>(); dd.task_pre = d.pre.as<uint8_t>();
-    dd.ext_state = d.ext.as<uint8_t>(); dd.n_ext = in->deps->n_ext;
-    const int64_t* fin = dep_finished_ns && in->deps->n_deps > 0 ? d.fin.as<int64_t>() : nullptr;
-    k_pl_plan<<<grid_for(T, 256), 256, 0, s>>>(dd, D, pf.task_off.as<int64_t>(), pf.finder.as<uint8_t>(), e.keep.as<int32_t>(),
+    const int64_t* fin = dep_finished_ns && in->deps->n_deps > 0 ? c->deps.fin.as<int64_t>() : nullptr;
+    k_pl_plan<<<grid_for(T, 256), 256, 0, s>>>(ddeps(c, in->deps), D, pf.task_off.as<int64_t>(), pf.finder.as<uint8_t>(), e.keep.as<int32_t>(),
                                                c->deps.met.as<uint8_t>(), fin, now_ns, c->deps.stamp.as<int64_t>());
     c->launches++;
     if (pipe_deps && E > 0) {
@@ -3238,10 +3245,10 @@ static int plan_from_finder(evg_ctx* c, const evg_runnable_in* in, const evg_pip
   memset(&none, 0, sizeof(none));
   evg_distro_table dn = *distros;
   dn.task_off = new_off.data();
-  rc = compose_tick(c, m, O, none, &dn);
+  rc = compose_tick(c, who, m, O, none, &dn);
   if (rc != EVG_OK) return rc;
   if (hosts) {
-    rc = upload_hosts(c, hosts, host_off, acfg, D);
+    rc = upload_hosts(c, who, hosts, host_off, acfg, D);
     if (rc != EVG_OK) return rc;
   }
   CK(cudaStreamSynchronize(s));
@@ -3279,9 +3286,7 @@ int evg_edit_tasks(evg_ctx* c, const evg_task_edit* ed, const evg_distro_table* 
   if (distros->n_distros != D) return fail(EVG_ERR_INVALID, "evg_edit_tasks: n_distros %d, the resident tick has %d", distros->n_distros, D);
   if (R < 0 || I < 0 || EI < 0 || NA < 0) return fail(EVG_ERR_INVALID, "evg_edit_tasks: negative sizes");
   if (R > 0 && !ed->remove_rows) return fail(EVG_ERR_INVALID, "evg_edit_tasks: null remove_rows");
-  if (I > 0 && (!ed->insert_off || !ins->priority || !ins->expected_ns || !ins->queue_basis_ns || !ins->wait_basis_ns ||
-                !ins->num_dependents || !ins->task_group_order || !ins->group_id || !ins->version_id || !ins->flags))
-    return fail(EVG_ERR_INVALID, "evg_edit_tasks: null insert_off / inserted column");
+  if (I > 0 && (!ed->insert_off || task_cols_missing(ins))) return fail(EVG_ERR_INVALID, "evg_edit_tasks: null insert_off / inserted column");
   if (EI > 0 && (I == 0 || !ins->dep_off || !ins->dep_idx)) return fail(EVG_ERR_INVALID, "evg_edit_tasks: inserted edges without dep_off / dep_idx");
   if (NA > 0 && (!ed->add_edge_task || !ed->add_edge_dep)) return fail(EVG_ERR_INVALID, "evg_edit_tasks: null added edges");
   if (D > 0 && (!distros->task_off || !distros->group_off || !distros->cfg)) return fail(EVG_ERR_INVALID, "evg_edit_tasks: null distro arrays");
@@ -3293,18 +3298,13 @@ int evg_edit_tasks(evg_ctx* c, const evg_task_edit* ed, const evg_distro_table* 
       return fail(EVG_ERR_INVALID, "evg_edit_tasks: remove_rows[%lld] = %lld is not ascending inside [0, %lld)", (long long)k, (long long)r, (long long)T0);
     removed[size_t(std::upper_bound(c->h_taskoff.begin(), c->h_taskoff.end(), r) - c->h_taskoff.begin() - 1)]++;
   }
-  if (I > 0) {
-    if (ed->insert_off[0] != 0 || ed->insert_off[D] != I) return fail(EVG_ERR_INVALID, "evg_edit_tasks: insert_off does not span the inserted rows");
-    ins_off.assign(ed->insert_off, ed->insert_off + D + 1);
-  }
-  if (EI > 0) {
-    const int rc = check_csr(csr_bad_row(ins->dep_off, I, EI), I, "evg_edit_tasks: the inserted dep_off");
-    if (rc != EVG_OK) return rc;
-  }
-  if (D > 0 && (distros->task_off[0] != 0 || distros->group_off[0] != 0)) return fail(EVG_ERR_INVALID, "evg_edit_tasks: offsets must start at 0");
+  int rc = I > 0 ? check_offsets(ed->insert_off, D, I, "evg_edit_tasks", "insert_off") : EVG_OK;
+  if (rc == EVG_OK && EI > 0) rc = check_offsets(ins->dep_off, I, EI, "evg_edit_tasks", "insert->dep_off");
+  if (rc == EVG_OK && D > 0) rc = check_offsets(distros->task_off, D, -1, "evg_edit_tasks", "task_off");
+  if (rc == EVG_OK && D > 0) rc = check_offsets(distros->group_off, D, -1, "evg_edit_tasks", "group_off");
+  if (rc != EVG_OK) return rc;
+  if (I > 0) ins_off.assign(ed->insert_off, ed->insert_off + D + 1);
   for (int32_t d = 0; d < D; d++) {
-    if (ins_off[d + 1] < ins_off[d]) return fail(EVG_ERR_INVALID, "evg_edit_tasks: insert_off decreases at distro %d", d);
-    if (distros->group_off[d + 1] < distros->group_off[d]) return fail(EVG_ERR_INVALID, "evg_edit_tasks: group_off decreases at distro %d", d);
     const int64_t want = (c->h_taskoff[d + 1] - c->h_taskoff[d]) - removed[d] + (ins_off[d + 1] - ins_off[d]);
     if (distros->task_off[d + 1] - distros->task_off[d] != want)
       return fail(EVG_ERR_INVALID, "evg_edit_tasks: distro %d holds %lld tasks after the edit, task_off says %lld", d, (long long)want,
@@ -3327,10 +3327,7 @@ int evg_edit_tasks(evg_ctx* c, const evg_task_edit* ed, const evg_distro_table* 
   c->launches = 0;
   // ---- stage the edit
   UP(s, e.rm, ed->remove_rows, R, int64_t);
-  if (I > 0) {
-    int rc = e.ins.stage(ins, I, s);
-    if (rc != EVG_OK) return rc;
-  }
+  if (I > 0 && (rc = e.ins.stage(ins, I, s)) != EVG_OK) return rc;
   UP(s, e.ins_dep_off, EI > 0 ? ins->dep_off : nullptr, EI > 0 ? I + 1 : 0, int64_t);
   UP(s, e.ins_dep_idx, EI > 0 ? ins->dep_idx : nullptr, EI, int32_t);
   UP(s, e.add_task, ed->add_edge_task, NA, int64_t);
@@ -3356,10 +3353,10 @@ int evg_edit_tasks(evg_ctx* c, const evg_task_edit* ed, const evg_distro_table* 
   m.n_add = NA; m.add_task = e.add_task.as<int64_t>(); m.add_dep = e.add_dep.as<int32_t>();
   DTasks In = e.ins.view(I);
   In.n_edges = EI; In.dep_off = e.ins_dep_off.as<int64_t>(); In.dep_idx = e.ins_dep_idx.as<int32_t>();
-  int rc = compose_tick(c, m, dtasks(c), In, distros);
+  rc = compose_tick(c, "evg_edit_tasks", m, dtasks(c), In, distros);
   if (rc != EVG_OK) return rc;
   if (hosts) {
-    rc = upload_hosts(c, hosts, host_off, acfg, D);
+    rc = upload_hosts(c, "evg_edit_tasks", hosts, host_off, acfg, D);
     if (rc != EVG_OK) return rc;
     CK(cudaStreamSynchronize(s));
   }
@@ -3600,19 +3597,18 @@ int evg_plan_aliases(evg_ctx* c, const evg_alias_in* in, const evg_distro_cfg* c
   if (T > (int64_t(1) << 31) - 2) return fail(EVG_ERR_INVALID, "evg_plan_aliases: %lld rows exceed 2^31-2", (long long)T);
   if (!out->task_off || !out->group_off || (D > 0 && (!out->n_versions || !cfg))) return fail(EVG_ERR_INVALID, "evg_plan_aliases: null cfg / output");
   if (!in->secondary_off || !in->dest_off || (NG > 0 && !in->group_max_hosts)) return fail(EVG_ERR_INVALID, "evg_plan_aliases: null offsets / group_max_hosts");
-  if (T > 0 && (!t->priority || !t->expected_ns || !t->queue_basis_ns || !t->wait_basis_ns || !t->num_dependents ||
-                !t->task_group_order || !t->group_id || !t->version_id || !t->flags || !in->sched || !in->task_group_max_hosts ||
-                !in->primary || !dp->dep_off || !dp->task_state || !dp->task_pre))
+  if (T > 0 && (task_cols_missing(t) || !in->sched || !in->task_group_max_hosts || !in->primary || !dp->dep_off || !dp->task_state ||
+                !dp->task_pre))
     return fail(EVG_ERR_INVALID, "evg_plan_aliases: null task column");
   if (E > 0 && (!t->dep_off || !t->dep_idx)) return fail(EVG_ERR_INVALID, "evg_plan_aliases: null dep_off / dep_idx");
   if (dp->n_deps > 0 && (!dp->dep_kind || !dp->dep_ref || !dp->dep_want)) return fail(EVG_ERR_INVALID, "evg_plan_aliases: null dependency arrays");
   if (dp->n_ext > 0 && !dp->ext_state) return fail(EVG_ERR_INVALID, "evg_plan_aliases: null ext_state");
-  const int64_t NS = in->secondary_off[T], ND = in->dest_off[NN];
-  int rc = check_csr(csr_bad_row(in->secondary_off, T, NS), T, "evg_plan_aliases: secondary_off");
-  if (rc == EVG_OK) rc = check_csr(csr_bad_row(in->dest_off, NN, ND), NN, "evg_plan_aliases: dest_off");
-  if (rc == EVG_OK && E > 0) rc = check_csr(csr_bad_row(t->dep_off, T, E), T, "evg_plan_aliases: dep_off");
-  if (rc == EVG_OK && T > 0) rc = check_csr(csr_bad_row(dp->dep_off, T, dp->n_deps), T, "evg_plan_aliases: deps->dep_off");
+  // deps->dep_off is checked by deps_to_device and k_deps_met, like every evg_deps_in
+  int rc = check_offsets(in->secondary_off, T, -1, "evg_plan_aliases", "secondary_off");
+  if (rc == EVG_OK) rc = check_offsets(in->dest_off, NN, -1, "evg_plan_aliases", "dest_off");
+  if (rc == EVG_OK && E > 0) rc = check_offsets(t->dep_off, T, E, "evg_plan_aliases", "tasks.dep_off");
   if (rc != EVG_OK) return rc;
+  const int64_t NS = in->secondary_off[T], ND = in->dest_off[NN];
   if (NS > 0 && !in->secondary_idx) return fail(EVG_ERR_INVALID, "evg_plan_aliases: null secondary_idx");
   if (ND > 0 && !in->dest_idx) return fail(EVG_ERR_INVALID, "evg_plan_aliases: null dest_idx");
   for (int64_t k = 0; k < ND; k++)
@@ -3645,7 +3641,7 @@ int evg_plan_aliases(evg_ctx* c, const evg_alias_in* in, const evg_distro_cfg* c
   UP(s, a.doff, in->dest_off, NN + 1, int64_t);
   UP(s, a.didx, in->dest_idx, ND, int32_t);
   if (T > 0) {
-    rc = deps_to_device(c, dp, 0, in->dep_finished_ns, now_ns, /*want_stamp=*/true);
+    rc = deps_to_device(c, "evg_plan_aliases", dp, 0, in->dep_finished_ns, now_ns, /*want_stamp=*/true);
     if (rc != EVG_OK) return rc;
     k_apply_deps<<<grid_for(T, 256), 256, 0, s>>>(T, c->deps.met.as<uint8_t>(), c->deps.stamp.as<int64_t>(), a.src.flags.as<uint32_t>(),
                                                   a.src.wb.as<int64_t>());
@@ -3672,7 +3668,7 @@ int evg_plan_aliases(evg_ctx* c, const evg_alias_in* in, const evg_distro_cfg* c
   CK(cudaMemcpyAsync(&bad_ref, c->b_err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   CK(cudaGetLastError());
-  if (bad_ref) return fail(EVG_ERR_INVALID, "evg_plan_aliases: a dep_ref is out of range");
+  if (bad_ref) return deps_bad("evg_plan_aliases", bad_ref);
   if (bad) return fail(EVG_ERR_INVALID, "evg_plan_aliases: a secondary_idx, primary, group_id or version_id is out of range");
   if (P > (int64_t(1) << 31) - 2) return fail(EVG_ERR_INVALID, "evg_plan_aliases: %lld (queue, task) pairs exceed 2^31-2", (long long)P);
   // 3. the pairs, in source-row order, sorted by queue
@@ -3785,7 +3781,7 @@ int evg_plan_aliases(evg_ctx* c, const evg_alias_in* in, const evg_distro_cfg* c
   evg_distro_table dt;
   memset(&dt, 0, sizeof(dt));
   dt.n_distros = D; dt.task_off = out->task_off; dt.group_off = out->group_off; dt.cfg = cf.data(); dt.group_max_hosts = gmax.data();
-  rc = install_composed(c, P, En, edge_off, &dt);
+  rc = install_composed(c, "evg_plan_aliases", P, En, edge_off, &dt);
   if (rc != EVG_OK) return rc;
   c->editable = true;
   c->alias_map = true;
@@ -3814,7 +3810,8 @@ int evg_intern_columns(const evg_string_cols* in, evg_intern_out* out, int32_t t
   if (T < 0 || D < 0) return fail(EVG_ERR_INVALID, "negative sizes");
   if (!out->group_off || (D > 0 && (!in->task_off || !out->n_versions))) return fail(EVG_ERR_INVALID, "null distro arrays");
   if (D == 0) { out->group_off[0] = 0; return T == 0 ? EVG_OK : fail(EVG_ERR_INVALID, "tasks without distros"); }
-  if (in->task_off[0] != 0 || in->task_off[D] != T) return fail(EVG_ERR_INVALID, "task_off does not span n_tasks");
+  int rc = check_offsets(in->task_off, D, T, "evg_intern_columns", "task_off");
+  if (rc != EVG_OK) return rc;
   if (T > 0 && (!in->id.off || !in->version.off || !in->group_key.off || !in->group_max_hosts || !in->dep_off || !out->group_id ||
                 !out->version_id || !out->group_max_hosts || !out->group_first || !out->dep_off))
     return fail(EVG_ERR_INVALID, "null column");
@@ -3827,6 +3824,9 @@ int evg_intern_columns(const evg_string_cols* in, evg_intern_out* out, int32_t t
   std::vector<std::vector<int32_t>> edge_by_distro(static_cast<size_t>(D));
   std::atomic<int32_t> next{0};
   std::atomic<int64_t> bad_row{-1};
+  // dep_off, a row per task, is checked by the workers as they walk it (a serial scan before them would cost a visible
+  // share of the call): a row outside [0, E] or decreasing is not walked, and sends the table through check_offsets
+  std::atomic<bool> bad_dep{false};
   int nt = threads > 0 ? threads : int(std::thread::hardware_concurrency());
   nt = std::max(1, std::min(nt, int(D)));
   auto work = [&]() {
@@ -3835,7 +3835,6 @@ int evg_intern_columns(const evg_string_cols* in, evg_intern_out* out, int32_t t
       const int32_t d = next.fetch_add(1);
       if (d >= D) return;
       const int64_t a = in->task_off[d], b = in->task_off[d + 1];
-      if (b < a) { bad_row.store(a); return; }
       const int64_t n = b - a;
       groups.reset(n); versions.reset(n); ids.reset(n);
       int32_t ng = 0, nv = 0;
@@ -3859,7 +3858,9 @@ int evg_intern_columns(const evg_string_cols* in, evg_intern_out* out, int32_t t
       std::vector<int32_t>& ed = edge_by_distro[size_t(d)];
       for (int64_t t = a; t < b; t++) {
         int64_t kept = 0;
-        for (int64_t e = in->dep_off[t]; e < in->dep_off[t + 1]; e++) {
+        const int64_t e0 = in->dep_off[t], e1 = in->dep_off[t + 1];
+        if (e0 < 0 || e1 < e0 || e1 > E) { bad_dep.store(true); return; }
+        for (int64_t e = e0; e < e1; e++) {
           const int32_t j = ids.find(str_at(in->dep_id.bytes, in->dep_id.off, e), in->id.bytes, in->id.off);
           if (j >= 0) { ed.push_back(j); kept++; }
         }
@@ -3872,7 +3873,8 @@ int evg_intern_columns(const evg_string_cols* in, evg_intern_out* out, int32_t t
   for (int k = 1; k < nt; k++) pool.emplace_back(work);
   work();
   for (std::thread& th : pool) th.join();
-  if (bad_row.load() >= 0) return fail(EVG_ERR_INVALID, "task group of row %lld: TaskGroupMaxHosts differs between members (or offsets decrease)", (long long)bad_row.load());
+  if (bad_dep.load() || (T > 0 && in->dep_off[0] != 0)) return check_offsets(in->dep_off, T, -1, "evg_intern_columns", "dep_off");
+  if (bad_row.load() >= 0) return fail(EVG_ERR_INVALID, "task group of row %lld: TaskGroupMaxHosts differs between members", (long long)bad_row.load());
   // offsets, then the per-distro pieces move to their places
   out->group_off[0] = 0;
   for (int32_t d = 0; d < D; d++) out->group_off[d + 1] = out->group_off[d] + n_groups[size_t(d)];
@@ -3900,12 +3902,10 @@ int evg_prioritize_legacy_batch(evg_ctx* c, const evg_legacy_soa* in, const int6
   if (T > 0 && (!in->priority || !in->ingest_ns || !in->expected_ns || !in->num_dependents || !in->revision_order || !in->project_id ||
                 !in->tg_rank || !in->tg_pair_id || !in->task_group_order || !in->presort_rank || !in->flags))
     return fail(EVG_ERR_INVALID, "null task column");
-  if (task_off[0] != 0 || task_off[D] != T) return fail(EVG_ERR_INVALID, "task_off does not span n_tasks");
+  const int rc = check_offsets(task_off, D, T, "evg_prioritize_legacy_batch", "task_off");
+  if (rc != EVG_OK) return rc;
   int64_t max_n = 0;
-  for (int32_t d = 0; d < D; d++) {
-    if (task_off[d + 1] < task_off[d]) return fail(EVG_ERR_INVALID, "offsets of distro %d decrease", d);
-    max_n = std::max(max_n, task_off[d + 1] - task_off[d]);
-  }
+  for (int32_t d = 0; d < D; d++) max_n = std::max(max_n, task_off[d + 1] - task_off[d]);
   for (int64_t k = 0; k < 3 * int64_t(D); k++)
     if (list_mode[k] > EVG_LEGACY_MODE_LITERAL) return fail(EVG_ERR_INVALID, "unknown list mode %d", int(list_mode[k]));
   CK(cudaSetDevice(c->device));
@@ -4024,13 +4024,12 @@ int evg_dag_rebuild_batch(evg_ctx* c, const evg_dag_in* in, const int64_t* item_
   if (!item_off || !group_off || !n_sorted || !n_cycles || !unit_off || (N > 0 && (!sorted || !unit_items))) return fail(EVG_ERR_INVALID, "null argument");
   if (N > 0 && (!in->dep_off || !in->group_id || !in->group_index)) return fail(EVG_ERR_INVALID, "null item column");
   if (E > 0 && !in->dep_item) return fail(EVG_ERR_INVALID, "null dep_item");
-  if (item_off[0] != 0 || item_off[D] != N || group_off[0] != 0) return fail(EVG_ERR_INVALID, "offsets do not span the tables");
-  if (N > 0 && (in->dep_off[0] != 0 || in->dep_off[N] != E)) return fail(EVG_ERR_INVALID, "dep_off does not span n_deps");
+  int rc = check_offsets(item_off, D, N, "evg_dag_rebuild_batch", "item_off");
+  if (rc == EVG_OK) rc = check_offsets(group_off, D, -1, "evg_dag_rebuild_batch", "group_off");
+  if (rc == EVG_OK && N > 0) rc = check_offsets(in->dep_off, N, E, "evg_dag_rebuild_batch", "dep_off");
+  if (rc != EVG_OK) return rc;
   int64_t max_n = 0;
-  for (int32_t d = 0; d < D; d++) {
-    if (item_off[d + 1] < item_off[d] || group_off[d + 1] < group_off[d]) return fail(EVG_ERR_INVALID, "offsets of distro %d decrease", d);
-    max_n = std::max(max_n, item_off[d + 1] - item_off[d]);
-  }
+  for (int32_t d = 0; d < D; d++) max_n = std::max(max_n, item_off[d + 1] - item_off[d]);
   if (max_n >= (int64_t(1) << 31) - 1) return fail(EVG_ERR_INVALID, "a queue exceeds 2^31 items");
   const int64_t G = group_off[D];
   CK(cudaSetDevice(c->device));

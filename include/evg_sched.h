@@ -254,7 +254,8 @@ int evg_plan_batch(evg_ctx* ctx, const evg_task_soa* tasks, const evg_distro_tab
  * count_required are written like the reference mutates TaskGroupInfos.
  * Replaces: scheduler.UtilizationBasedHostAllocator
  * (scheduler/utilization_based_host_allocator.go:26-130) behind the
- * HostAllocator plug point (scheduler/host_allocator.go:15,25-32). */
+ * HostAllocator plug point (scheduler/host_allocator.go:15,25-32).
+ * EVG_ERR_INVALID for a group_off that does not start at 0 or decreases, or a host_off that also misses n_hosts. */
 int evg_alloc_batch(evg_ctx* ctx, const evg_host_soa* hosts, const int64_t* host_off,
                     const evg_alloc_cfg* cfg, const evg_queue_info* info, evg_group_info* groups,
                     const int64_t* group_off, int32_t n_distros, int64_t now_ns, evg_alloc_out* out);
@@ -419,7 +420,9 @@ typedef struct {
 
 /* met[t] = Task.DependenciesMet(ctx, depCache) for every task (model/task/task.go:632-671 with
  * SatisfiesDependency :529-543): the bit evg_task_soa.flags carries as EVG_TF_DEPS_MET and the predicate the
- * task finders filter on (scheduler/task_finder.go:40-197).  Host pointers in and out. */
+ * task finders filter on (scheduler/task_finder.go:40-197).  Host pointers in and out.
+ * EVG_ERR_INVALID for a dep_ref out of range or a dep_off that does not start at 0, end at n_deps and never decrease:
+ * the host checks its ends, k_deps_met every row before it reads the row's entries. */
 int evg_deps_met_batch(evg_ctx* ctx, const evg_deps_in* in, uint8_t* met);
 
 /* evg_upload with the dependency predicate evaluated ON THE DEVICE and wired into the planner's inputs: after the
@@ -430,7 +433,8 @@ int evg_deps_met_batch(evg_ctx* ctx, const evg_deps_in* in, uint8_t* met);
  *     NULL = unknown) of its dependencies, else now_ns; its resident wait basis becomes the later of the caller's
  *     wait_basis_ns (ScheduledTime) and that stamp (scheduler.go:119-122).
  * Neither the bit nor the stamp visits the host; evg_download_deps returns them for the write-back the reference does
- * (UpdateOne of DependenciesMetTime, task.go:659-666).
+ * (UpdateOne of DependenciesMetTime, task.go:659-666).  `deps` is checked as by evg_deps_met_batch; a table rejected on
+ * the device leaves no resident tick.
  * Replaces: checkDependenciesMet inside GetDistroQueueInfo (scheduler/scheduler.go:82-98,161-168). */
 int evg_upload_with_deps(evg_ctx* ctx, const evg_task_soa* tasks, const evg_distro_table* distros,
                          const evg_host_soa* hosts, const int64_t* host_off, const evg_alloc_cfg* acfg,
@@ -483,7 +487,9 @@ typedef struct {
 /* LegacyFindRunnableTasks / AlternateTaskFinder / ParallelTaskFinder (scheduler/task_finder.go:40-317) over all
  * distros at once: runnable[task_off[d] .. task_off[d] + count[d]) holds the distro-local indices of the tasks
  * the finder returns for distro d, in input order (the reference appends in query order); the rest of the
- * distro's slots are -1.  Host pointers. */
+ * distro's slots are -1.  Host pointers.  EVG_ERR_INVALID for a task_off that does not start at 0, end at n_tasks and
+ * never decrease, a valid_off that does not start at 0 or decreases, a project row out of range, or in->deps rejected
+ * as by evg_deps_met_batch. */
 int evg_find_runnable_batch(evg_ctx* ctx, const evg_runnable_in* in, int32_t* runnable, int64_t* count);
 
 /* The finder's output feeds the planner without leaving the device.  `in` describes every CANDIDATE task of every
@@ -498,8 +504,9 @@ int evg_find_runnable_batch(evg_ctx* ctx, const evg_runnable_in* in, int32_t* ru
  * call evg_run_resident / evg_download next (evg_update_tasks and evg_edit_tasks may follow, as after evg_upload); ranks
  * refer to the compacted queues, and `runnable` (n_tasks, may be NULL) / `count` (n_distros) map them back exactly as
  * evg_find_runnable_batch reports them.  The only values the host reads in between are the n_distros counts (the
- * routing needs queue lengths).  EVG_ERR_INVALID for a candidate dep_off that does not start at 0, end at n_edges and
- * never decrease, or a dep_idx outside its distro's candidates.
+ * routing needs queue lengths).  EVG_ERR_INVALID for `in` rejected as by evg_find_runnable_batch, a candidate dep_off
+ * that does not start at 0, end at n_edges and never decrease, a dep_idx outside its distro's candidates, or a
+ * distros->group_off / host_off rejected as by evg_upload.
  * Replaces: the finder + checkDependenciesMet + PrioritizeTasks hand-over inside scheduler.PlanDistro
  * (scheduler/wrapper.go:60-118, scheduler/scheduler.go:56-168), where the filtered []task.Task is rebuilt on the host. */
 int evg_plan_from_finder(evg_ctx* ctx, const evg_runnable_in* in, const evg_task_soa* candidates, const evg_distro_table* distros,
@@ -540,7 +547,8 @@ typedef struct {
  * DependsOn is kept; OverrideDependencies and DependenciesMetTime do not help.  EVG_FINDER_PIPELINE_NO_DEPS distros
  * apply the gating without the dependency filter.  Output order: candidate order, as for the other finders.
  * pipe == NULL behaves exactly like evg_find_runnable_batch.  EVG_ERR_INVALID: a pipeline code with pipe == NULL, a
- * pipeline distro without in->deps, a status id outside [0, n_status), n_status < 3.  Host pointers. */
+ * pipeline distro without in->deps, a status id outside [0, n_status), n_status < 3, and what evg_find_runnable_batch
+ * rejects (k_pl_deps checks the rows of in->deps->dep_off as k_deps_met does).  Host pointers. */
 int evg_find_runnable_ex(evg_ctx* ctx, const evg_runnable_in* in, const evg_pipeline_in* pipe, int32_t* runnable,
                          int64_t* count);
 
@@ -603,10 +611,10 @@ typedef struct {
  * group, version and edge offsets of every distro and the group_max_hosts of every alias group slot -- O(n_distros +
  * alias groups) values, nothing per task.
  * EVG_ERR_INVALID, previous tick still resident and runnable: negative sizes, null arrays, sizes that disagree, a CSR
- * (secondary_off, dest_off, dep_off, deps->dep_off) that does not start at 0, end at its entry count and never
- * decrease, a dest_idx outside [0, n_distros).  EVG_ERR_INVALID with no resident tick: an id found out of range on the
- * device (secondary_idx, primary, group_id, version_id, dep_idx, dep_ref), more than 2^31-2 (queue, task) pairs, or an
- * alias queue above 2^21-1 tasks.
+ * (secondary_off, dest_off, tasks.dep_off) that does not start at 0, end at its entry count and never decrease, a
+ * dest_idx outside [0, n_distros).  EVG_ERR_INVALID with no resident tick: deps rejected as by evg_deps_met_batch, an
+ * id found out of range on the device (secondary_idx, primary, group_id, version_id, dep_idx, dep_ref), more than
+ * 2^31-2 (queue, task) pairs, or an alias queue above 2^21-1 tasks.
  * Replaces: distroAliasSchedulerJob.Run for every distro (units/scheduler_alias.go:55-117): FindHostSchedulableForAlias
  * (model/task/task.go:3371-3386, model/distro/aliases.go:14-27) and PrioritizeTasks (scheduler/scheduler.go:27-51). */
 int evg_plan_aliases(evg_ctx* ctx, const evg_alias_in* in, const evg_distro_cfg* cfg, int32_t n_distros, int64_t now_ns,
@@ -652,7 +660,9 @@ typedef struct {
 /* String work of marshalling a tick (scheduler.PrioritizeTasks builds the same maps while it walks a queue:
  * planner.go:431-456 files units under exactly these strings): group keys and versions to dense ids, dependency ids
  * to queue indices, per distro, `threads` distros at a time (<= 0: hardware concurrency).  Host only: no context.
- * EVG_ERR_INVALID when members of one task group disagree on TaskGroupMaxHosts (evg_last_error names the row). */
+ * EVG_ERR_INVALID when members of one task group disagree on TaskGroupMaxHosts (evg_last_error names the row), for a
+ * task_off that does not start at 0, end at n_tasks and never decrease, and for a dep_off that does not start at 0 or
+ * decreases. */
 int evg_intern_columns(const evg_string_cols* in, evg_intern_out* out, int32_t threads);
 
 /* ---- expected-duration statistics (SURVEY.md §8f.2) ----------------------- */
@@ -818,7 +828,9 @@ typedef struct {
  * unit_items[item_off[d] ..] = the items that have a group, bucketed by group id and stably sorted by GroupIndex inside
  *   each bucket (d.taskGroups[...].tasks); group g of distro d is unit_items[item_off[d] + unit_off[u + g] ..
  *   item_off[d] + unit_off[u + g + 1]) with u = group_off[d] + d (each distro has one closing entry).
- * Host pointers.  group_off (n_distros + 1) counts the groups of each distro. */
+ * Host pointers.  group_off (n_distros + 1) counts the groups of each distro.  EVG_ERR_INVALID for an item_off or
+ * in->dep_off that does not start at 0, end at n_items / n_deps and never decrease, or a group_off that does not start
+ * at 0 or decreases. */
 int evg_dag_rebuild_batch(evg_ctx* ctx, const evg_dag_in* in, const int64_t* item_off, const int64_t* group_off, int32_t n_distros,
                           int32_t* sorted, int32_t* n_sorted, int32_t* n_cycles, int32_t* unit_items, int32_t* unit_off);
 

@@ -185,6 +185,24 @@ def test_intern_columns_equals_the_python_marshaller():
     with pytest.raises(L.EvgError):
         S.intern_columns(batch, 3)
     assert S.intern_columns([], 1)["group_off"].tolist() == [0]
+    # a dep_off that decreases is refused before any row is read (its rows would outrun the caller's dep_idx)
+    assert intern_raw(np.array([0, 2, 4]), np.array([0, 2, 2, 3, 3])) == L.EVG_OK
+    assert intern_raw(np.array([0, 2, 4]), np.array([0, 2, 1, 2, 3])) == L.EVG_ERR_INVALID
+    assert "evg_intern_columns" in L.last_error() and "dep_off" in L.last_error()
+
+
+def intern_raw(task_off, dep_off):
+    """evg_intern_columns over tasks t0, t1, ... cut by `task_off`, every dependency on t0, with `dep_off` as given."""
+    task_off, dep_off = task_off.astype(np.int64), dep_off.astype(np.int64)
+    T, D, E = len(dep_off) - 1, len(task_off) - 1, int(dep_off.max())
+    ids, blank, dep = S.pack_strings([f"t{i}" for i in range(T)]), S.pack_strings([""] * T), S.pack_strings(["t0"] * E)
+    col = lambda s: L.StrColStruct(L.ptr(s[0]) if s[0].shape[0] else None, L.ptr(s[1]))  # noqa: E731
+    gmax = np.zeros(T, np.int32)
+    ins = L.StringColsStruct(T, D, L.ptr(task_off), col(ids), col(ids), col(blank), L.ptr(gmax), L.ptr(dep_off), col(dep))
+    out = [np.zeros(n, dt) for n, dt in ((T, np.int32), (T, np.int32), (D + 1, np.int64), (D, np.int32), (T, np.int32),
+                                         (T, np.int64), (T + 1, np.int64), (E, np.int32))]
+    import ctypes as C
+    return L.load().evg_intern_columns(C.byref(ins), C.byref(L.InternOutStruct(*[L.ptr(o) for o in out])), 1)
 
 
 def test_take_distros_is_the_same_tick_per_distro():
