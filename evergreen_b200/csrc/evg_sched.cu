@@ -1188,6 +1188,10 @@ struct TaskCols {  // the nine planner columns of a task table
   }
 };
 
+// Whose columns the resident tick is: none; the context's own but no base for edits (what a one-shot call leaves, or a
+// call that failed after upload_tasks); caller-owned device memory (evg_upload_device); the context's own, editable.
+enum class Tick : uint8_t { kNone, kFixed, kBorrowed, kOwn };
+
 struct evg_ctx {
   int device = 0;
   int num_sms = 0;  // the device's multiprocessor count: grid cap of the grid-stride work-list kernels
@@ -1209,15 +1213,15 @@ struct evg_ctx {
   static constexpr int kAux = 6;
   cudaStream_t s_aux[kAux] = {};
   cudaEvent_t ev_fork = nullptr, ev_join[kAux] = {};
-  // resident inputs
-  bool have_tasks = false, have_hosts = false;
+  // The resident tick (need_tick checks it; upload_tasks and drop_tick replace it), and whether the allocator's tables,
+  // evg_upload_with_deps' verdicts (`deps`), evg_plan_aliases' map (`al`) and evg_resolve_durations' results (`dur`)
+  // belong to it.
+  struct { Tick kind = Tick::kNone; bool hosts = false, deps = false, aliases = false, durations = false; } tick;
   int64_t T = 0, E = 0, G = 0, H = 0, U = 0, NT = 0, t_pad = 0;
   int32_t Dn = 0;
   int any_complex = 0;
   int64_t launches = 0;
   bool timed = false;
-  bool adopted = false;  // task columns are caller-owned device memory (evg_upload_device)
-  bool deps_resident = false;  // evg_upload_with_deps left the verdicts and stamps of this tick in `deps`
   TaskCols tasks;  // the resident planner columns
   DevBuf b_depoff, b_depidx;
   DevBuf b_taskoff, b_groupoff, b_cfg, b_gmax, b_unitbase;
@@ -1237,9 +1241,6 @@ struct evg_ctx {
     DevBuf dep_status, task_status, ext_status, task_unatt, ext_unatt, project_raw;  // an evg_pipeline_in, staged
     DevBuf edge_cnt, dep_off, dep_idx, scan_sum;  // the candidates' edges without those of EVG_FINDER_PIPELINE rows
   } pl;
-  // evg_edit_tasks: resident columns an edit may start from (evg_upload, evg_upload_with_deps, evg_plan_from_finder,
-  // evg_edit_tasks; not borrowed columns, not what a one-shot call left)
-  bool editable = false;
   struct {  // compose_tick's buffers (the first evg_edit_tasks or evg_plan_from_finder allocates them) and the staged edit
     TaskCols out;            // the shadow set: the composed table is written here, then swapped with the resident columns
     DevBuf dep_off, dep_idx; // the composed edges (swapped too)
@@ -1249,8 +1250,7 @@ struct evg_ctx {
     DevBuf keep, pos, src, scan_sum, edge_cnt, err;
   } ed;
   // evg_plan_aliases (the first call allocates these): the staged source table, the (queue, task) pairs and the alias
-  // map evg_download_alias_map returns while `alias_map` holds (upload_tasks clears it)
-  bool alias_map = false;
+  // map evg_download_alias_map returns while tick.aliases holds
   struct {
     TaskCols src;
     DevBuf dep_off, dep_idx, gmax, sched, tgmax, primary, soff, sidx, doff, didx;  // the source table
@@ -1260,12 +1260,11 @@ struct evg_ctx {
   } al;
   // evg_resolve_durations (the first call allocates these): the staged history, the per-key accumulators and statistics,
   // the pairs' single keys, the listed rows (tasks, then hosts) and their results, which evg_download_durations returns
-  // while `valid` holds (upload_tasks clears it)
+  // while tick.durations holds
   struct {
     DevBuf key, taken, start, finish, flags, acc, stat, pair_off, single;
     DevBuf rows, in, out, src, err;
     int64_t n_t = 0, n_h = 0;
-    bool valid = false;
   } dur;
   // evg_rebuild_dispatchers (the first call allocates these): the persisted queues' DAG input gathered from the tick,
   // and the scratch and results of the k_dag_* kernels, so that the resident tick is only read
@@ -1316,6 +1315,27 @@ inline unsigned grid_for(int64_t n, int block) { return unsigned((n + block - 1)
 
 // Columns are padded so that 128-bit loads and TMA copies that start inside the table may run past its last row.
 constexpr int64_t kColPad = 8;
+
+// A call that writes the resident columns or the tables beside them (a new table, or scratch it shares with the
+// planner's inputs) drops the tick before its first such write: a call that fails partway must not leave the next
+// evg_run_resident a tick whose buffers it has half replaced.
+void drop_tick(evg_ctx* c) { c->tick = {}; }
+
+// What a call needs of the resident tick.  EVG_ERR_STATE names the call and the first unmet condition: a tick, then
+// its kind, then the state the call reads.
+enum class Need { kTick, kOwnColumns, kEditable, kHosts, kVerdicts, kAliasMap, kDurations };
+int need_tick(const evg_ctx* c, const char* who, Need what) {
+  const auto& t = c->tick;
+  const bool own = what == Need::kOwnColumns || what == Need::kEditable;
+  const char* unmet = t.kind == Tick::kNone                               ? "no resident tick"
+                      : own && t.kind == Tick::kBorrowed                  ? "the resident columns are borrowed (evg_upload_device)"
+                      : what == Need::kEditable && t.kind == Tick::kFixed ? "the resident tick is what a one-shot call left"
+                      : what == Need::kHosts && !t.hosts                  ? "the resident tick has no hosts"
+                      : what == Need::kVerdicts && !t.deps                ? "the resident tick was not uploaded with evg_upload_with_deps"
+                      : what == Need::kAliasMap && !t.aliases             ? "the resident tick was not built by evg_plan_aliases"
+                      : what == Need::kDurations && !t.durations          ? "no evg_resolve_durations on the resident tick's rows" : nullptr;
+  return unmet ? fail(EVG_ERR_STATE, "%s: %s", who, unmet) : EVG_OK;
+}
 
 // Where upload_tasks finds the task columns.
 enum class Cols {
@@ -1417,6 +1437,7 @@ int upload_tasks(evg_ctx* c, const char* who, const evg_task_soa* t, const evg_d
   const int64_t NT = int64_t(tile_distro.size());
   const int64_t P = 2 * T + E;
   cudaStream_t s = c->stream;
+  drop_tick(c);
 #define UPC(buf, ptr, count, type)                                                                    \
   do {                                                                                                \
     if (cols == Cols::kResident) break;                                                               \
@@ -1528,8 +1549,6 @@ int upload_tasks(evg_ctx* c, const char* who, const evg_task_soa* t, const evg_d
   CK(c->b_tv.ensure(sizeof(int64_t) * size_t(T + kColPad)));
   c->T = T; c->E = E; c->G = G; c->U = U; c->NT = NT; c->Dn = D;
   c->t_pad = (T + 3) & ~int64_t(3);
-  c->adopted = adopt;
-  c->deps_resident = false;
   c->Tgc = Tgc;
   c->max_groups = 0;
   for (int32_t d = 0; d < D; d++) c->max_groups = std::max(c->max_groups, dt->group_off[d + 1] - dt->group_off[d]);
@@ -1547,12 +1566,8 @@ int upload_tasks(evg_ctx* c, const char* who, const evg_task_soa* t, const evg_d
   for (int32_t d = 0; d < D; d++) c->h_nver[size_t(d)] = dt->cfg[d].n_versions;
   c->h_unitbase.swap(unit_base);
   c->h_dtileoff.swap(dtile_off);
-  c->have_tasks = true;
-  c->alias_map = false;  // evg_plan_aliases sets it again after its upload
-  c->dur.valid = false;  // the resolved rows name rows of the previous table
-  c->editable = false;  // the entry point that uploaded says whether evg_edit_tasks may follow
+  c->tick.kind = adopt ? Tick::kBorrowed : Tick::kFixed;  // the entry point that uploaded says whether evg_edit_tasks may follow
   c->alist_valid = false;  // upload_hosts lists the allocator's distros against THIS table
-  c->have_hosts = false;
   if (cols != Cols::kChunked && T > 0) {  // range-check the ids the kernels index with
     DTasks dtv = dtasks(c);
     DDistros ddv = ddistros(c);
@@ -1561,7 +1576,7 @@ int upload_tasks(evg_ctx* c, const char* who, const evg_task_soa* t, const evg_d
     int bad = 0;
     CK(cudaMemcpyAsync(&bad, c->b_err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
-    if (bad) { c->have_tasks = false; return fail(EVG_ERR_INVALID, "a group_id / version_id / dep_idx is out of range for its distro"); }
+    if (bad) { drop_tick(c); return fail(EVG_ERR_INVALID, "a group_id / version_id / dep_idx is out of range for its distro"); }
   }
   return EVG_OK;
 }
@@ -1585,7 +1600,7 @@ int upload_hosts(evg_ctx* c, const char* who, const evg_host_soa* h, const int64
   UP(s, c->b_acfg, acfg, D, evg_alloc_cfg);
   c->alist_valid = false;
   std::vector<int32_t> alist;
-  if (c->have_tasks && c->Dn == D && int64_t(c->h_groupoff.size()) == int64_t(D) + 1) {
+  if (c->tick.kind != Tick::kNone && c->Dn == D && int64_t(c->h_groupoff.size()) == int64_t(D) + 1) {
     for (int32_t d = 0; d < D; d++)
       if (c->h_groupoff[d + 1] != c->h_groupoff[d] || host_off[d + 1] - host_off[d] > kGrouplessHosts) alist.push_back(d);
     UP(s, c->b_alist, alist.data(), int64_t(alist.size()), int32_t);
@@ -1596,7 +1611,7 @@ int upload_hosts(evg_ctx* c, const char* who, const evg_host_soa* h, const int64
   CK(c->b_result.ensure(sizeof(evg_alloc_result) * size_t(D + 1)));
   CK(c->b_status.ensure(sizeof(int32_t) * size_t(D + 1)));
   c->H = H;
-  c->have_hosts = true;
+  c->tick.hosts = true;
   return EVG_OK;
 }
 
@@ -1961,25 +1976,27 @@ void evg_shutdown(evg_ctx* c) {
   delete c;  // its buffers free themselves, on the device selected above
 }
 
-// evg_upload for the entry point `who` (the caller holds the context's lock)
+// evg_upload for the entry point `who` (the caller holds the context's lock), leaving a tick of the given kind; `cols`
+// and `edge_off` as for upload_tasks
 static int upload(evg_ctx* c, const char* who, const evg_task_soa* tasks, const evg_distro_table* distros, const evg_host_soa* hosts,
-                  const int64_t* host_off, const evg_alloc_cfg* acfg) {
+                  const int64_t* host_off, const evg_alloc_cfg* acfg, Tick kind, Cols cols = Cols::kCopy,
+                  const int64_t* edge_off = nullptr) {
   CK(cudaSetDevice(c->device));
-  int rc = upload_tasks(c, who, tasks, distros);
+  int rc = upload_tasks(c, who, tasks, distros, cols, edge_off);
   if (rc != EVG_OK) return rc;
   if (hosts) {
     rc = upload_hosts(c, who, hosts, host_off, acfg, distros->n_distros);
     if (rc != EVG_OK) return rc;
     CK(cudaStreamSynchronize(c->stream));
   }
-  c->editable = true;
+  c->tick.kind = kind;
   return EVG_OK;
 }
 int evg_upload(evg_ctx* c, const evg_task_soa* tasks, const evg_distro_table* distros, const evg_host_soa* hosts,
                const int64_t* host_off, const evg_alloc_cfg* acfg) {
   if (!c) return fail(EVG_ERR_INVALID, "null context");
   LOCK(c);
-  return upload(c, "evg_upload", tasks, distros, hosts, host_off, acfg);
+  return upload(c, "evg_upload", tasks, distros, hosts, host_off, acfg, Tick::kOwn);
 }
 
 __global__ void k_gather_i64(const int64_t* __restrict__ src, const int64_t* __restrict__ at, int64_t* __restrict__ out, int n) {
@@ -2004,8 +2021,7 @@ __global__ void __launch_bounds__(256) k_update_rows(int64_t n, const int64_t* _
 int evg_update_tasks(evg_ctx* c, int64_t n_rows, const int64_t* rows, const evg_task_soa* v) {
   if (!c) return fail(EVG_ERR_INVALID, "null context");
   LOCK(c);
-  if (!c->have_tasks) return fail(EVG_ERR_STATE, "evg_update_tasks before evg_upload");
-  if (c->adopted) return fail(EVG_ERR_STATE, "the resident columns are borrowed (evg_upload_device): edit them in place instead");
+  if (const int rc = need_tick(c, "evg_update_tasks", Need::kOwnColumns); rc != EVG_OK) return rc;
   if (n_rows < 0) return fail(EVG_ERR_INVALID, "negative row count");
   if (n_rows == 0) return EVG_OK;
   if (!rows || !v || v->n_tasks != n_rows || !v->priority || !v->num_dependents || !v->task_group_order || !v->flags || !v->expected_ns ||
@@ -2040,7 +2056,7 @@ int evg_update_tasks(evg_ctx* c, int64_t n_rows, const int64_t* rows, const evg_
   CK(cudaMemcpyAsync(&h_bad, bad, sizeof(int), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));  // the caller's staging arrays are free again
   if (h_bad) return fail(EVG_ERR_INVALID, "evg_update_tasks: a row index is outside [0, n_tasks)");
-  c->deps_resident = false;  // flags / wait bases written by a device-side dependency evaluation may have been replaced
+  c->tick.deps = false;  // flags / wait bases written by a device-side dependency evaluation may have been replaced
   return EVG_OK;
 }
 
@@ -2062,20 +2078,14 @@ int evg_upload_device(evg_ctx* c, const evg_task_soa* tasks, const evg_distro_ta
     CK(cudaMemcpyAsync(edge_off.data(), c->b_rn1.p, sizeof(int64_t) * size_t(D + 1), cudaMemcpyDeviceToHost, c->stream));
     CK(cudaStreamSynchronize(c->stream));
   }
-  int rc = upload_tasks(c, "evg_upload_device", tasks, distros, Cols::kAdopt, edge_off.empty() ? nullptr : edge_off.data());
-  if (rc != EVG_OK) return rc;
-  if (hosts) {
-    rc = upload_hosts(c, "evg_upload_device", hosts, host_off, acfg, distros->n_distros);
-    if (rc != EVG_OK) return rc;
-    CK(cudaStreamSynchronize(c->stream));
-  }
-  return EVG_OK;
+  return upload(c, "evg_upload_device", tasks, distros, hosts, host_off, acfg, Tick::kBorrowed, Cols::kAdopt,
+                edge_off.empty() ? nullptr : edge_off.data());
 }
 
 int evg_run_resident(evg_ctx* c, int64_t now_ns, uint32_t opts) {
   if (!c) return fail(EVG_ERR_INVALID, "null context");
   LOCK(c);
-  if (!c->have_tasks) return fail(EVG_ERR_STATE, "evg_run_resident before evg_upload");
+  if (const int rc = need_tick(c, "evg_run_resident", Need::kTick); rc != EVG_OK) return rc;
   CK(cudaSetDevice(c->device));
   c->launches = 0;
   c->timed = true;
@@ -2083,7 +2093,7 @@ int evg_run_resident(evg_ctx* c, int64_t now_ns, uint32_t opts) {
   CK(cudaEventRecord(c->ev_begin, c->stream));
   int rc = run_plan(c, now_ns, opts);
   if (rc != EVG_OK) return rc;
-  if (c->have_hosts) {
+  if (c->tick.hosts) {
     rc = run_alloc(c, now_ns);
     if (rc != EVG_OK) return rc;
   }
@@ -2094,7 +2104,7 @@ int evg_run_resident(evg_ctx* c, int64_t now_ns, uint32_t opts) {
 int evg_download(evg_ctx* c, evg_plan_out* po, evg_alloc_out* ao) {
   if (!c) return fail(EVG_ERR_INVALID, "null context");
   LOCK(c);
-  if (!c->have_tasks) return fail(EVG_ERR_STATE, "evg_download before evg_upload");
+  if (const int rc = need_tick(c, "evg_download", Need::kTick); rc != EVG_OK) return rc;
   CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   if (po) {
@@ -2108,7 +2118,7 @@ int evg_download(evg_ctx* c, evg_plan_out* po, evg_alloc_out* ao) {
     if (po->group_info && c->G) CK(cudaMemcpyAsync(po->group_info, c->b_ginfo.p, sizeof(evg_group_info) * size_t(c->G), cudaMemcpyDeviceToHost, s));
   }
   if (ao) {
-    if (!c->have_hosts) return fail(EVG_ERR_STATE, "allocator results requested but no hosts were uploaded");
+    if (const int rc = need_tick(c, "evg_download", Need::kHosts); rc != EVG_OK) return rc;
     if (ao->result && c->Dn) CK(cudaMemcpyAsync(ao->result, c->result_ptr(), sizeof(evg_alloc_result) * size_t(c->Dn), cudaMemcpyDeviceToHost, s));
     if (ao->status && c->Dn) CK(cudaMemcpyAsync(ao->status, c->b_status.p, sizeof(int32_t) * size_t(c->Dn), cudaMemcpyDeviceToHost, s));
   }
@@ -2142,7 +2152,7 @@ __global__ void __launch_bounds__(256) k_project_queue(DTasks T, DDistros D, con
 int evg_download_queue(evg_ctx* c, int32_t cap, int64_t* item_off, evg_queue_item* items, int64_t items_capacity) {
   if (!c) return fail(EVG_ERR_INVALID, "null context");
   LOCK(c);
-  if (!c->have_tasks) return fail(EVG_ERR_STATE, "evg_download_queue before evg_upload");
+  if (const int rc = need_tick(c, "evg_download_queue", Need::kTick); rc != EVG_OK) return rc;
   if (cap < 0 || !item_off) return fail(EVG_ERR_INVALID, "evg_download_queue: bad argument");
   if (cap == 0) cap = EVG_PERSISTED_QUEUE_CAP;
   const int32_t D = c->Dn;
@@ -2217,9 +2227,8 @@ int evg_plan_batch(evg_ctx* c, const evg_task_soa* tasks, const evg_distro_table
                    evg_plan_out* out) {
   if (!c) return fail(EVG_ERR_INVALID, "null context");
   LOCK(c);
-  int rc = upload(c, "evg_plan_batch", tasks, distros, nullptr, nullptr, nullptr);
+  int rc = upload(c, "evg_plan_batch", tasks, distros, nullptr, nullptr, nullptr, Tick::kFixed);
   if (rc != EVG_OK) return rc;
-  c->editable = false;  // a one-shot call's tick is not a resident one to edit
   rc = evg_run_resident(c, now_ns, opts);
   if (rc != EVG_OK) return rc;
   return evg_download(c, out, nullptr);
@@ -2328,8 +2337,7 @@ static int plan_and_alloc_pipelined(evg_ctx* c, const evg_task_soa* t, const evg
   CK(cudaMemcpyAsync(&bad, c->b_err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(c->s_d2h));
   CK(cudaStreamSynchronize(s));
-  if (bad) { c->have_tasks = false; return fail(EVG_ERR_INVALID, "a group_id / version_id / dep_idx is out of range for its distro"); }
-  c->have_hosts = true;
+  if (bad) { drop_tick(c); return fail(EVG_ERR_INVALID, "a group_id / version_id / dep_idx is out of range for its distro"); }
   return EVG_OK;
 }
 
@@ -2341,17 +2349,12 @@ int evg_plan_and_alloc_batch(evg_ctx* c, const evg_task_soa* tasks, const evg_di
   if (!hosts || (!acfg && distros && distros->n_distros > 0)) return fail(EVG_ERR_INVALID, "evg_plan_and_alloc_batch needs hosts and allocator config");
   if (!(opts & EVG_OPT_BREAKDOWN) && tasks && distros && tasks->n_tasks >= (int64_t(1) << 21)) {
     // large tick: stage the small tables, then pipeline the columns chunk by chunk
-    CK(cudaSetDevice(c->device));
-    int rc0 = upload_tasks(c, "evg_plan_and_alloc_batch", tasks, distros, Cols::kChunked);
+    const int rc0 = upload(c, "evg_plan_and_alloc_batch", tasks, distros, hosts, host_off, acfg, Tick::kFixed, Cols::kChunked);
     if (rc0 != EVG_OK) return rc0;
-    rc0 = upload_hosts(c, "evg_plan_and_alloc_batch", hosts, host_off, acfg, distros->n_distros);
-    if (rc0 != EVG_OK) return rc0;
-    CK(cudaStreamSynchronize(c->stream));
     return plan_and_alloc_pipelined(c, tasks, distros, hosts, host_off, acfg, now_ns, plan_out, alloc_out);
   }
-  int rc = upload(c, "evg_plan_and_alloc_batch", tasks, distros, hosts, host_off, acfg);
+  int rc = upload(c, "evg_plan_and_alloc_batch", tasks, distros, hosts, host_off, acfg, Tick::kFixed);
   if (rc != EVG_OK) return rc;
-  c->editable = false;  // a one-shot call's tick is not a resident one to edit
   rc = evg_run_resident(c, now_ns, opts);
   if (rc != EVG_OK) return rc;
   return evg_download(c, plan_out, alloc_out);
@@ -2368,7 +2371,7 @@ int evg_alloc_batch(evg_ctx* c, const evg_host_soa* hosts, const int64_t* host_o
   if (rc != EVG_OK) return rc;
   const int64_t G = n_distros > 0 ? group_off[n_distros] : 0;
   if (G > 0 && !groups) return fail(EVG_ERR_INVALID, "evg_alloc_batch: groups is null");
-  c->have_tasks = false;  // the resident planner inputs no longer match the tables of this call (and upload_hosts must not list distros from them)
+  drop_tick(c);  // before upload_hosts, which must not list distros from the tick's tables
   rc = upload_hosts(c, "evg_alloc_batch", hosts, host_off, cfg, n_distros);
   if (rc != EVG_OK) return rc;
   cudaStream_t s = c->stream;
@@ -2384,7 +2387,6 @@ int evg_alloc_batch(evg_ctx* c, const evg_host_soa* hosts, const int64_t* host_o
   c->G = G;
   c->max_groups = 0;
   for (int32_t d = 0; d < n_distros; d++) c->max_groups = std::max(c->max_groups, group_off[d + 1] - group_off[d]);
-  c->have_tasks = false;  // the resident planner inputs no longer match these tables
   c->launches = 0;
   rc = run_alloc(c, now_ns);
   if (rc != EVG_OK) return rc;
@@ -2459,7 +2461,7 @@ int evg_deps_met_batch(evg_ctx* c, const evg_deps_in* in, uint8_t* met) {
   CK(c->b_err.ensure(sizeof(int) * 4));
   CK(cudaMemsetAsync(c->b_err.p, 0, sizeof(int) * 4, s));
   c->launches = 0;
-  c->deps_resident = false;  // deps_to_device overwrites the resident tick's verdicts and stamps
+  c->tick.deps = false;  // deps_to_device overwrites the resident tick's verdicts and stamps
   int rc = deps_to_device(c, "evg_deps_met_batch", in, 0);
   if (rc != EVG_OK) return rc;
   int bad = 0;
@@ -2477,13 +2479,13 @@ int evg_upload_with_deps(evg_ctx* c, const evg_task_soa* tasks, const evg_distro
   LOCK(c);
   if (!tasks || !deps) return fail(EVG_ERR_INVALID, "evg_upload_with_deps: null argument");
   if (deps->n_tasks != tasks->n_tasks) return fail(EVG_ERR_INVALID, "deps covers %lld tasks, the task table %lld", (long long)deps->n_tasks, (long long)tasks->n_tasks);
-  int rc = upload(c, "evg_upload_with_deps", tasks, distros, hosts, host_off, acfg);
+  int rc = upload(c, "evg_upload_with_deps", tasks, distros, hosts, host_off, acfg, Tick::kOwn);
   if (rc != EVG_OK) return rc;
   const int64_t T = tasks->n_tasks;
   if (T == 0) return EVG_OK;
   cudaStream_t s = c->stream;
   rc = deps_to_device(c, "evg_upload_with_deps", deps, 0, dep_finished_ns, now_ns, /*want_stamp=*/true);
-  if (rc != EVG_OK) { c->have_tasks = false; return rc; }
+  if (rc != EVG_OK) { drop_tick(c); return rc; }
   k_apply_deps<<<grid_for(T, 256), 256, 0, s>>>(T, c->deps.met.as<uint8_t>(), c->deps.stamp.as<int64_t>(), c->tasks.flags.as<uint32_t>(),
                                                 c->tasks.wb.as<int64_t>());
   c->launches++;
@@ -2491,18 +2493,18 @@ int evg_upload_with_deps(evg_ctx* c, const evg_task_soa* tasks, const evg_distro
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(&bad, c->b_err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
-  if (bad) { c->have_tasks = false; return deps_bad("evg_upload_with_deps", bad); }
-  c->deps_resident = true;
+  if (bad) { drop_tick(c); return deps_bad("evg_upload_with_deps", bad); }
+  c->tick.deps = true;
   return EVG_OK;
 }
 
 int evg_download_deps(evg_ctx* c, uint8_t* met, int64_t* met_time_ns) {
   if (!c) return fail(EVG_ERR_INVALID, "null context");
   LOCK(c);
-  if (!c->have_tasks) return fail(EVG_ERR_STATE, "evg_download_deps before evg_upload_with_deps");
+  if (const int rc = need_tick(c, "evg_download_deps", Need::kTick); rc != EVG_OK) return rc;
   CK(cudaSetDevice(c->device));
   if (c->T == 0) return EVG_OK;
-  if (!c->deps_resident) return fail(EVG_ERR_STATE, "the resident tick was not uploaded with evg_upload_with_deps");
+  if (const int rc = need_tick(c, "evg_download_deps", Need::kVerdicts); rc != EVG_OK) return rc;
   if (met) CK(cudaMemcpyAsync(met, c->deps.met.p, size_t(c->T), cudaMemcpyDeviceToHost, c->stream));
   if (met_time_ns) CK(cudaMemcpyAsync(met_time_ns, c->deps.stamp.p, sizeof(int64_t) * size_t(c->T), cudaMemcpyDeviceToHost, c->stream));
   CK(cudaStreamSynchronize(c->stream));
@@ -2521,7 +2523,7 @@ int evg_expected_durations_batch(evg_ctx* c, const evg_duration_rows* in, evg_du
   CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   c->launches = 0;
-  c->have_tasks = false;  // shares scratch buffers with the finder entry points
+  drop_tick(c);
   UP(s, c->b_rn0, in->key, R, int32_t);
   UP(s, c->b_rn1, in->time_taken_ns, R, int64_t);
   UP(s, c->b_rn2, in->start_ns, R, int64_t);
@@ -2575,11 +2577,9 @@ int evg_resolve_durations(evg_ctx* c, const evg_duration_in* in, int64_t now_ns)
   if (!c) return fail(EVG_ERR_INVALID, "null context");
   LOCK(c);
   if (!in) return fail(EVG_ERR_INVALID, "evg_resolve_durations: null argument");
-  if (!c->have_tasks) return fail(EVG_ERR_STATE, "evg_resolve_durations without a resident tick");
-  if (!c->editable)  // the context's own columns: not borrowed ones, not the tick a one-shot call left
-    return fail(EVG_ERR_STATE, c->adopted ? "the resident columns are borrowed (evg_upload_device): resolve on the host instead"
-                                          : "evg_resolve_durations: the resident tick is what a one-shot call left");
-  if (in->hosts && !c->have_hosts) return fail(EVG_ERR_STATE, "evg_resolve_durations: hosts given but the resident tick has none");
+  int rc;
+  if ((rc = need_tick(c, "evg_resolve_durations", Need::kEditable)) != EVG_OK) return rc;
+  if (in->hosts && (rc = need_tick(c, "evg_resolve_durations", Need::kHosts)) != EVG_OK) return rc;
   const evg_duration_rows* h = in->history;
   const int64_t R = h ? h->n_rows : 0;
   const int32_t K = h ? h->n_keys : 0, P = in->n_pairs;
@@ -2587,14 +2587,13 @@ int evg_resolve_durations(evg_ctx* c, const evg_duration_in* in, int64_t now_ns)
   if (R > 0 && (!h->key || !h->time_taken_ns || !h->start_ns || !h->finish_ns || !h->flags))
     return fail(EVG_ERR_INVALID, "evg_resolve_durations: null history column");
   if (P > 0 && !in->pair_key_off) return fail(EVG_ERR_INVALID, "evg_resolve_durations: null pair_key_off");
-  int rc;
   if (in->pair_key_off && (rc = check_offsets(in->pair_key_off, P, K, "evg_resolve_durations", "pair_key_off")) != EVG_OK) return rc;
   if (in->tasks && (rc = check_duration_cache(in->tasks, c->T, "tasks")) != EVG_OK) return rc;
   if (in->hosts && (rc = check_duration_cache(in->hosts, c->H, "hosts")) != EVG_OK) return rc;
   CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   auto& d = c->dur;
-  d.valid = false;  // the staging below is overwritten whatever the outcome
+  c->tick.durations = false;  // the staging below is overwritten whatever the outcome
   const int64_t Nt = in->tasks ? in->tasks->n_rows : 0, Nh = in->hosts ? in->hosts->n_rows : 0, N = Nt + Nh;
   // history -> per-key statistics, on the call's own buffers (evg_expected_durations_batch's scratch is not touched)
   UP(s, d.key, h ? h->key : nullptr, R, int32_t);
@@ -2658,14 +2657,14 @@ int evg_resolve_durations(evg_ctx* c, const evg_duration_in* in, int64_t now_ns)
   if (bad & 1) return fail(EVG_ERR_INVALID, "evg_resolve_durations: a history key is outside [0, n_keys)");
   if (bad) return fail(EVG_ERR_INVALID, "evg_resolve_durations: a row's key or pair is out of range");
   d.n_t = Nt; d.n_h = Nh;
-  d.valid = true;
+  c->tick.durations = true;
   return EVG_OK;
 }
 
 int evg_download_durations(evg_ctx* c, evg_duration_out* tasks, evg_duration_out* hosts) {
   if (!c) return fail(EVG_ERR_INVALID, "null context");
   LOCK(c);
-  if (!c->have_tasks || !c->dur.valid) return fail(EVG_ERR_STATE, "evg_download_durations: no evg_resolve_durations on the resident tick's rows");
+  if (const int rc = need_tick(c, "evg_download_durations", Need::kDurations); rc != EVG_OK) return rc;
   CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   auto& d = c->dur;
@@ -2781,7 +2780,7 @@ static int find_runnable(evg_ctx* c, const evg_runnable_in* in, const evg_pipeli
   CK(c->b_err.ensure(sizeof(int) * 4));
   CK(cudaMemsetAsync(c->b_err.p, 0, sizeof(int) * 4, s));
   c->launches = 0;
-  c->have_tasks = false;  // the tick's dependency verdicts and stamps are overwritten: a finder batch ends the resident tick
+  drop_tick(c);
   if (any_deps && T > 0) {
     rc = deps_to_device(c, who, in->deps, 1);
     if (rc != EVG_OK) return rc;
@@ -3040,6 +3039,7 @@ static int shadow_cols(evg_ctx* c, int64_t Tn, EdDst* o) {
 // distro boundaries) becomes the resident one, routed, sized and range-checked like an upload.  An error leaves no tick.
 static int install_composed(evg_ctx* c, const char* who, int64_t Tn, int64_t En, const int64_t* edge_off, const evg_distro_table* distros) {
   auto& e = c->ed;
+  drop_tick(c);
   c->tasks.swap(e.out);
   if (En > 0) { c->b_depoff.swap(e.dep_off); c->b_depidx.swap(e.dep_idx); }
   evg_task_soa ts;
@@ -3049,9 +3049,7 @@ static int install_composed(evg_ctx* c, const char* who, int64_t Tn, int64_t En,
   ts.group_id = c->tasks.gid.as<int32_t>(); ts.version_id = c->tasks.vid.as<int32_t>(); ts.flags = c->tasks.flags.as<uint32_t>();
   ts.expected_ns = c->tasks.exp.as<int64_t>(); ts.queue_basis_ns = c->tasks.qb.as<int64_t>(); ts.wait_basis_ns = c->tasks.wb.as<int64_t>();
   if (En > 0) { ts.dep_off = c->b_depoff.as<int64_t>(); ts.dep_idx = c->b_depidx.as<int32_t>(); }
-  int rc = upload_tasks(c, who, &ts, distros, Cols::kResident, En > 0 ? edge_off : nullptr);
-  if (rc != EVG_OK) { c->have_tasks = false; return rc; }
-  return EVG_OK;
+  return upload_tasks(c, who, &ts, distros, Cols::kResident, En > 0 ? edge_off : nullptr);
 }
 
 // The rows of O that ed.keep marks (O.n entries, staged by the caller) survive in their order, distro d's inserted rows
@@ -3103,8 +3101,9 @@ static int compose_tick(evg_ctx* c, const char* who, EdMap m, const DTasks& O, c
   CK(cudaMemcpyAsync(&bad, e.err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   CK(cudaGetLastError());
-  if (bad & 1) { c->have_tasks = false; return fail(EVG_ERR_INVALID, "group_remap maps the task group of a surviving task to -1"); }
-  if (bad & 2) { c->have_tasks = false; return fail(EVG_ERR_INVALID, "an in-queue dep_idx is outside its distro"); }
+  if (bad) drop_tick(c);
+  if (bad & 1) return fail(EVG_ERR_INVALID, "group_remap maps the task group of a surviving task to -1");
+  if (bad & 2) return fail(EVG_ERR_INVALID, "an in-queue dep_idx is outside its distro");
   if (edges) {
     En = edge_off[size_t(D)];
     CK(e.dep_idx.ensure(sizeof(int32_t) * size_t(En + kColPad)));
@@ -3132,7 +3131,7 @@ static int plan_from_finder(evg_ctx* c, const evg_runnable_in* in, const evg_pip
   const int32_t D = in->n_distros, P = in->n_projects;
   if (T < 0 || D < 0 || P < 0 || E < 0) return fail(EVG_ERR_INVALID, "negative sizes");
   if (cand->n_tasks != T || distros->n_distros != D) return fail(EVG_ERR_INVALID, "the candidate table, the finder table and the distro table disagree on their sizes");
-  if (D == 0) return T == 0 ? upload(c, who, cand, distros, hosts, host_off, acfg) : fail(EVG_ERR_INVALID, "tasks without distros");
+  if (D == 0) return T == 0 ? upload(c, who, cand, distros, hosts, host_off, acfg, Tick::kOwn) : fail(EVG_ERR_INVALID, "tasks without distros");
   if (!count) return fail(EVG_ERR_INVALID, "null count");
   // a composed row's source row is 32-bit (compose_tick's src)
   if (T > (int64_t(1) << 31) - 2) return fail(EVG_ERR_INVALID, "evg_plan_from_finder: %lld candidates exceed 2^31-2", (long long)T);
@@ -3157,10 +3156,10 @@ static int plan_from_finder(evg_ctx* c, const evg_runnable_in* in, const evg_pip
   CK(c->b_err.ensure(sizeof(int) * 4));
   CK(cudaMemsetAsync(c->b_err.p, 0, sizeof(int) * 4, s));
   c->launches = 0;
-  c->have_tasks = false;
+  drop_tick(c);
   if (T == 0) {
     for (int32_t d = 0; d < D; d++) count[d] = 0;
-    return upload(c, who, cand, distros, hosts, host_off, acfg);
+    return upload(c, who, cand, distros, hosts, host_off, acfg, Tick::kOwn);
   }
   // 1. Task.DependenciesMet / AllDependenciesSatisfied of every candidate, with the DependenciesMetTime stamps
   rc = deps_to_device(c, who, in->deps, 1, dep_finished_ns, now_ns, /*want_stamp=*/true);
@@ -3252,7 +3251,7 @@ static int plan_from_finder(evg_ctx* c, const evg_runnable_in* in, const evg_pip
     if (rc != EVG_OK) return rc;
   }
   CK(cudaStreamSynchronize(s));
-  c->editable = true;
+  c->tick.kind = Tick::kOwn;
   return EVG_OK;
 }
 int evg_plan_from_finder(evg_ctx* c, const evg_runnable_in* in, const evg_task_soa* cand, const evg_distro_table* distros,
@@ -3273,10 +3272,7 @@ int evg_edit_tasks(evg_ctx* c, const evg_task_edit* ed, const evg_distro_table* 
                    const int64_t* host_off, const evg_alloc_cfg* acfg) {
   if (!c) return fail(EVG_ERR_INVALID, "null context");
   LOCK(c);
-  if (!c->have_tasks) return fail(EVG_ERR_STATE, "evg_edit_tasks before evg_upload");
-  if (!c->editable)
-    return fail(EVG_ERR_STATE, c->adopted ? "the resident columns are borrowed (evg_upload_device): edit them in place instead"
-                                          : "the resident tick was left by a one-shot call: evg_upload it first");
+  if (const int rc = need_tick(c, "evg_edit_tasks", Need::kEditable); rc != EVG_OK) return rc;
   if (!ed || !distros) return fail(EVG_ERR_INVALID, "evg_edit_tasks: null edit / distro table");
   // ---- every check the host can make, before anything resident changes
   const int32_t D = c->Dn;
@@ -3360,7 +3356,7 @@ int evg_edit_tasks(evg_ctx* c, const evg_task_edit* ed, const evg_distro_table* 
     if (rc != EVG_OK) return rc;
     CK(cudaStreamSynchronize(s));
   }
-  c->editable = true;
+  c->tick.kind = Tick::kOwn;
   return EVG_OK;
 }
 
@@ -3618,7 +3614,7 @@ int evg_plan_aliases(evg_ctx* c, const evg_alias_in* in, const evg_distro_cfg* c
   CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   auto& a = c->al;
-  c->have_tasks = false;
+  drop_tick(c);
   c->launches = 0;
   CK(c->b_err.ensure(sizeof(int) * 4));
   CK(cudaMemsetAsync(c->b_err.p, 0, sizeof(int) * 4, s));
@@ -3783,15 +3779,15 @@ int evg_plan_aliases(evg_ctx* c, const evg_alias_in* in, const evg_distro_cfg* c
   dt.n_distros = D; dt.task_off = out->task_off; dt.group_off = out->group_off; dt.cfg = cf.data(); dt.group_max_hosts = gmax.data();
   rc = install_composed(c, "evg_plan_aliases", P, En, edge_off, &dt);
   if (rc != EVG_OK) return rc;
-  c->editable = true;
-  c->alias_map = true;
+  c->tick.kind = Tick::kOwn;
+  c->tick.aliases = true;
   return EVG_OK;
 }
 
 int evg_download_alias_map(evg_ctx* c, int32_t* source_row, int32_t* group_source) {
   if (!c) return fail(EVG_ERR_INVALID, "null context");
   LOCK(c);
-  if (!c->have_tasks || !c->alias_map) return fail(EVG_ERR_STATE, "evg_download_alias_map: the resident tick was not built by evg_plan_aliases");
+  if (const int rc = need_tick(c, "evg_download_alias_map", Need::kAliasMap); rc != EVG_OK) return rc;
   CK(cudaSetDevice(c->device));
   if (source_row && c->T) CK(cudaMemcpyAsync(source_row, c->al.srow.p, sizeof(int32_t) * size_t(c->T), cudaMemcpyDeviceToHost, c->stream));
   if (group_source && c->G) CK(cudaMemcpyAsync(group_source, c->al.gsrc.p, sizeof(int32_t) * size_t(c->G), cudaMemcpyDeviceToHost, c->stream));
@@ -3911,7 +3907,7 @@ int evg_prioritize_legacy_batch(evg_ctx* c, const evg_legacy_soa* in, const int6
   CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   c->launches = 0;
-  c->have_tasks = false;  // shares scratch buffers with the other entry points
+  drop_tick(c);
   UP(s, c->tasks.exp, in->priority, T, int64_t);
   UP(s, c->tasks.qb, in->ingest_ns, T, int64_t);
   UP(s, c->tasks.wb, in->expected_ns, T, int64_t);
@@ -4035,7 +4031,7 @@ int evg_dag_rebuild_batch(evg_ctx* c, const evg_dag_in* in, const int64_t* item_
   CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   c->launches = 0;
-  c->have_tasks = false;  // shares scratch buffers with the planner's resident inputs
+  drop_tick(c);
   UP(s, c->b_taskoff, item_off, D + 1, int64_t);
   UP(s, c->b_groupoff, group_off, D + 1, int64_t);
   UP(s, c->b_depoff, in->dep_off, N + 1, int64_t);
@@ -4129,7 +4125,7 @@ __global__ void __launch_bounds__(256) k_dp_groups(DDisp X, const int64_t* __res
 int evg_rebuild_dispatchers(evg_ctx* c, int32_t cap, int64_t items_capacity, int64_t groups_capacity, evg_dispatch_out* out) {
   if (!c || !out) return fail(EVG_ERR_INVALID, "evg_rebuild_dispatchers: null argument");
   LOCK(c);
-  if (!c->have_tasks) return fail(EVG_ERR_STATE, "evg_rebuild_dispatchers without a resident tick");
+  if (const int rc = need_tick(c, "evg_rebuild_dispatchers", Need::kTick); rc != EVG_OK) return rc;
   if (cap < 0) return fail(EVG_ERR_INVALID, "evg_rebuild_dispatchers: negative cap");
   if (cap == 0) cap = EVG_PERSISTED_QUEUE_CAP;
   if (!out->item_off || !out->n_sorted || !out->n_cycles || !out->group_off || !out->unit_off)

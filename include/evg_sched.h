@@ -45,7 +45,8 @@ enum {
   EVG_ERR_INVALID = -1, /* bad argument / inconsistent offsets */
   EVG_ERR_CUDA = -2,    /* no usable sm_90 device, or a CUDA call failed */
   EVG_ERR_NOMEM = -3,   /* device or pinned allocation failed */
-  EVG_ERR_STATE = -4    /* resident call without a prior evg_upload */
+  EVG_ERR_STATE = -4    /* the resident tick cannot serve the call: there is none, or it lacks what the call needs
+                           (its own columns, editability, hosts, dependency verdicts, alias map, resolved durations) */
 };
 
 /* per-distro allocator status: the data errors UtilizationBasedHostAllocator
@@ -275,13 +276,15 @@ int evg_plan_and_alloc_batch(evg_ctx* ctx, const evg_task_soa* tasks, const evg_
 int evg_upload(evg_ctx* ctx, const evg_task_soa* tasks, const evg_distro_table* distros,
                const evg_host_soa* hosts, const int64_t* host_off, const evg_alloc_cfg* acfg);
 /* Tick-to-tick update of the resident task table: row rows[i] (a task slot of the resident table, 0 <= rows[i] <
- * n_tasks: the table of evg_upload, evg_upload_with_deps or evg_edit_tasks, or the kept candidates of
- * evg_plan_from_finder) gets priority, num_dependents, task_group_order, flags, expected_ns, queue_basis_ns and wait_basis_ns of row i
+ * n_tasks) gets priority, num_dependents, task_group_order, flags, expected_ns, queue_basis_ns and wait_basis_ns of row i
  * of `values` (values->n_tasks == n_rows; its group / version / dependency columns are not read: a task keeps its
  * distro, its task group, its version and its in-queue dependency edges -- a tick that adds or removes tasks calls
- * evg_edit_tasks first).  48 bytes cross PCIe per changed row instead of the whole table.  Not available after evg_upload_device (the
- * caller owns those columns and edits them in place).  Replaces nothing in the reference: there the scheduler re-reads
- * every task document each tick (scheduler/task_finder.go:40-197). */
+ * evg_edit_tasks first).  48 bytes cross PCIe per changed row instead of the whole table.  Allowed on any tick in the
+ * context's own columns: after evg_upload, evg_upload_with_deps, evg_edit_tasks, evg_plan_from_finder(_ex),
+ * evg_plan_aliases, evg_plan_batch and evg_plan_and_alloc_batch; EVG_ERR_STATE without a tick or after
+ * evg_upload_device (the caller owns those columns and edits them in place).  Drops the dependency verdicts of
+ * evg_upload_with_deps.  Replaces nothing in the reference: there the scheduler re-reads every task document each tick
+ * (scheduler/task_finder.go:40-197). */
 int evg_update_tasks(evg_ctx* ctx, int64_t n_rows, const int64_t* rows, const evg_task_soa* values);
 
 /* A change in queue membership between two ticks: rows leave, rows join, surviving tasks gain in-queue dependencies.
@@ -314,8 +317,9 @@ typedef struct {
  * resident one.  A survivor cannot LOSE an in-queue dependency that stays in the queue (upload again for that), and
  * dependencies are not re-evaluated: pass EVG_TF_DEPS_MET for inserted rows and flip it for survivors with
  * evg_update_tasks.  Any device-side dependency state of evg_upload_with_deps is dropped.
- * Allowed after evg_upload, evg_upload_with_deps, evg_plan_from_finder and evg_edit_tasks; EVG_ERR_STATE otherwise
- * (no table, borrowed columns of evg_upload_device, the tick a one-shot call left).  EVG_ERR_INVALID for an edit the
+ * Allowed after evg_upload, evg_upload_with_deps, evg_plan_from_finder(_ex), evg_edit_tasks and evg_plan_aliases;
+ * EVG_ERR_STATE otherwise (no table, borrowed columns of evg_upload_device, the tick a one-shot call left).
+ * EVG_ERR_INVALID for an edit the
  * host can reject (remove rows not strictly ascending or out of range, counts that disagree, another n_distros, an
  * added edge on a task that is not a survivor) leaves the previous tick resident and runnable; an id found out of range
  * on the device (or a survivor whose task group maps to -1) leaves no resident tick, as for evg_upload.
@@ -439,7 +443,10 @@ int evg_deps_met_batch(evg_ctx* ctx, const evg_deps_in* in, uint8_t* met);
 int evg_upload_with_deps(evg_ctx* ctx, const evg_task_soa* tasks, const evg_distro_table* distros,
                          const evg_host_soa* hosts, const int64_t* host_off, const evg_alloc_cfg* acfg,
                          const evg_deps_in* deps, const int64_t* dep_finished_ns, int64_t now_ns);
-/* met[t] = Task.DependenciesMet; met_time_ns[t] = the stamp (EVG_TIME_ZERO when nothing was stamped).  Either may be NULL. */
+/* met[t] = Task.DependenciesMet; met_time_ns[t] = the stamp (EVG_TIME_ZERO when nothing was stamped).  Either may be NULL.
+ * EVG_ERR_STATE without a tick; EVG_OK for a tick of no rows; then EVG_ERR_STATE unless the tick's verdicts are
+ * evg_upload_with_deps' (evg_deps_met_batch and evg_update_tasks drop them; evg_resolve_durations and
+ * evg_rebuild_dispatchers keep them). */
 int evg_download_deps(evg_ctx* ctx, uint8_t* met, int64_t* met_time_ns);
 
 /* ---- runnable-task filter: the task finders (SURVEY.md §8f.1) ------------- */
@@ -619,7 +626,7 @@ typedef struct {
  * (model/task/task.go:3371-3386, model/distro/aliases.go:14-27) and PrioritizeTasks (scheduler/scheduler.go:27-51). */
 int evg_plan_aliases(evg_ctx* ctx, const evg_alias_in* in, const evg_distro_cfg* cfg, int32_t n_distros, int64_t now_ns,
                      evg_alias_out* out);
-/* After evg_plan_aliases (and evg_update_tasks): source_row[r] = the source row of resident row r (task_off[n_distros]
+/* After evg_plan_aliases (and evg_update_tasks, evg_resolve_durations, evg_rebuild_dispatchers): source_row[r] = the source row of resident row r (task_off[n_distros]
  * entries), group_source[s] = the global group id of alias group slot s (group_off[n_distros] entries).  Either may be
  * NULL.  EVG_ERR_STATE once another call replaced the tick's rows. */
 int evg_download_alias_map(evg_ctx* ctx, int32_t* source_row, int32_t* group_source);
@@ -761,7 +768,7 @@ typedef struct {
  * durations of the host allocator (utilization_based_host_allocator.go:357-359). */
 int evg_resolve_durations(evg_ctx* ctx, const evg_duration_in* in, int64_t now_ns);
 /* After evg_resolve_durations: its per-row results, listed-row order; either pointer may be NULL.  EVG_ERR_STATE once
- * another call replaced the tick's rows. */
+ * another call replaced the tick's rows, or when the last evg_resolve_durations was rejected on the device. */
 int evg_download_durations(evg_ctx* ctx, evg_duration_out* tasks, evg_duration_out* hosts);
 
 /* ---- legacy comparator prioritiser (SURVEY.md §8 row L) ---------------------- */
