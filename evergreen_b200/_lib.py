@@ -217,6 +217,20 @@ class AllocOutStruct(C.Structure):
     _fields_ = [("result", C.c_void_p), ("status", C.c_void_p)]
 
 
+HOST_JOB_CFG_DTYPE = np.dtype([("n_provisioning", "<i8"), ("single_task_distro", "<i4"),
+                               ("terminate_when_overallocated", "<i4"), ("hourly_billing", "<i4"), ("_reserved", "<i4")])
+HOST_REPORT_FIELDS = ("time_to_empty_ns", "time_to_empty_no_spawns_ns", "scheduled_duration_ns", "hosts_avail", "hosts_spawned",
+                      "overdue_in_groups", "free_in_groups", "required_in_groups", "new_cap_target", "killable_hosts",
+                      "host_queue_ratio", "no_spawns_ratio", "drawdown")
+HOST_REPORT_DTYPE = np.dtype([(f, "<i8") for f in HOST_REPORT_FIELDS[:10]] + [
+    ("host_queue_ratio", "<f4"), ("no_spawns_ratio", "<f4"), ("drawdown", "<i4"), ("_reserved", "<i4")])
+assert HOST_JOB_CFG_DTYPE.itemsize == 24 and HOST_REPORT_DTYPE.itemsize == 96
+
+
+class HostJobOutStruct(C.Structure):
+    _fields_ = [("n_hosts", C.c_void_p), ("n_hosts_free", C.c_void_p), ("status", C.c_void_p), ("report", C.c_void_p)]
+
+
 class EvgError(RuntimeError):
     def __init__(self, code: int, msg: str):
         super().__init__(f"libevgsched error {code}: {msg}")
@@ -264,6 +278,7 @@ SYMBOLS = {
     "evg_prioritize_legacy_batch": (C.c_int, [_P, _P, _P, _P, C.c_int32, _P, _P, _P]),
     "evg_dag_rebuild_batch": (C.c_int, [_P, _P, _P, _P, C.c_int32, _P, _P, _P, _P, _P]),
     "evg_rebuild_dispatchers": (C.c_int, [_P, C.c_int32, C.c_int64, C.c_int64, _P]),
+    "evg_host_job": (C.c_int, [_P, _P, _P, _P]),
     "evg_plan_distro": (C.c_int, [_P, _P, _P, C.c_int32, _P, C.c_int64, C.c_uint32, _P]),
     "evg_alloc_distro": (C.c_int, [_P, _P, _P, _P, _P, C.c_int32, C.c_int64, _P, _P]),
 }

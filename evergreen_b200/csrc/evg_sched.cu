@@ -28,6 +28,7 @@
 //   k_dur_pair            the single matched key of a (project, build variant) pair (expected_duration.go:54-56)
 //   k_dur_resolve         Task.FetchExpectedDuration per listed row (model/task/task.go:3519-3590) into staging
 //   k_dur_commit          the resolved durations into the resident columns, unless the call found an error
+//   k_host_job            hostAllocatorJob.Run past the allocator: single-task bypass, report, drawdown (units/host_allocator.go:180-425)
 // No CPU fallback exists in this file: without a device every entry point fails.
 #include <cuda_runtime.h>
 #include <stdarg.h>
@@ -1215,8 +1216,9 @@ struct evg_ctx {
   cudaEvent_t ev_fork = nullptr, ev_join[kAux] = {};
   // The resident tick (need_tick checks it; upload_tasks and drop_tick replace it), and whether the allocator's tables,
   // evg_upload_with_deps' verdicts (`deps`), evg_plan_aliases' map (`al`) and evg_resolve_durations' results (`dur`)
-  // belong to it.
-  struct { Tick kind = Tick::kNone; bool hosts = false, deps = false, aliases = false, durations = false; } tick;
+  // belong to it.  `allocated`: run state -- the allocator's results (queue and group infos, result rows, status) are
+  // from a run on this tick, into the result buffer bound now; evg_host_job reads them.
+  struct { Tick kind = Tick::kNone; bool hosts = false, deps = false, aliases = false, durations = false, allocated = false; } tick;
   int64_t T = 0, E = 0, G = 0, H = 0, U = 0, NT = 0, t_pad = 0;
   int32_t Dn = 0;
   int any_complex = 0;
@@ -1272,6 +1274,8 @@ struct evg_ctx {
     DevBuf item_off, rank_of, row, first, gslot_of, gindex, cnt, dep_off, dep_item, pos, group_off, group_slot, group_id, scan_sum;
     DevBuf succ_off, succ, index, low, stack, cs_node, cs_pos, emit, on_stack, sorted, stats, buf[2], unit_off;
   } dp;
+  // evg_host_job (the first call allocates these): the staged job settings and spawned counts, and the outputs
+  struct { DevBuf cfg, spawned, out; } hj;
   DevBuf b_err;
   DevBuf b_route, b_unitv, b_unita, b_unitn, b_unitmask;
   DevBuf b_punt, b_puntcnt;
@@ -1323,14 +1327,15 @@ void drop_tick(evg_ctx* c) { c->tick = {}; }
 
 // What a call needs of the resident tick.  EVG_ERR_STATE names the call and the first unmet condition: a tick, then
 // its kind, then the state the call reads.
-enum class Need { kTick, kOwnColumns, kEditable, kHosts, kVerdicts, kAliasMap, kDurations };
+enum class Need { kTick, kOwnColumns, kEditable, kHosts, kVerdicts, kAliasMap, kDurations, kAllocated };
 int need_tick(const evg_ctx* c, const char* who, Need what) {
   const auto& t = c->tick;
   const bool own = what == Need::kOwnColumns || what == Need::kEditable;
   const char* unmet = t.kind == Tick::kNone                               ? "no resident tick"
                       : own && t.kind == Tick::kBorrowed                  ? "the resident columns are borrowed (evg_upload_device)"
                       : what == Need::kEditable && t.kind == Tick::kFixed ? "the resident tick is what a one-shot call left"
-                      : what == Need::kHosts && !t.hosts                  ? "the resident tick has no hosts"
+                      : (what == Need::kHosts || what == Need::kAllocated) && !t.hosts ? "the resident tick has no hosts"
+                      : what == Need::kAllocated && !t.allocated          ? "no allocator run on the resident tick since it was set or a result buffer was bound"
                       : what == Need::kVerdicts && !t.deps                ? "the resident tick was not uploaded with evg_upload_with_deps"
                       : what == Need::kAliasMap && !t.aliases             ? "the resident tick was not built by evg_plan_aliases"
                       : what == Need::kDurations && !t.durations          ? "no evg_resolve_durations on the resident tick's rows" : nullptr;
@@ -2090,12 +2095,14 @@ int evg_run_resident(evg_ctx* c, int64_t now_ns, uint32_t opts) {
   c->launches = 0;
   c->timed = true;
   c->general_timed = false;
+  c->tick.allocated = false;
   CK(cudaEventRecord(c->ev_begin, c->stream));
   int rc = run_plan(c, now_ns, opts);
   if (rc != EVG_OK) return rc;
   if (c->tick.hosts) {
     rc = run_alloc(c, now_ns);
     if (rc != EVG_OK) return rc;
+    c->tick.allocated = true;
   }
   CK(cudaEventRecord(c->ev_end, c->stream));
   return EVG_OK;
@@ -2181,6 +2188,7 @@ int evg_bind_result_buffer(evg_ctx* c, void* device_ptr, int64_t capacity) {
   if (device_ptr && capacity < 0) return fail(EVG_ERR_INVALID, "negative capacity");
   c->ext_result = reinterpret_cast<evg_alloc_result*>(device_ptr);
   c->ext_capacity = device_ptr ? capacity : 0;
+  c->tick.allocated = false;  // the last run's result rows are not in the buffer bound now
   return EVG_OK;
 }
 int64_t evg_last_launch_count(evg_ctx* c) { return c ? c->launches : 0; }
@@ -2351,7 +2359,9 @@ int evg_plan_and_alloc_batch(evg_ctx* c, const evg_task_soa* tasks, const evg_di
     // large tick: stage the small tables, then pipeline the columns chunk by chunk
     const int rc0 = upload(c, "evg_plan_and_alloc_batch", tasks, distros, hosts, host_off, acfg, Tick::kFixed, Cols::kChunked);
     if (rc0 != EVG_OK) return rc0;
-    return plan_and_alloc_pipelined(c, tasks, distros, hosts, host_off, acfg, now_ns, plan_out, alloc_out);
+    const int rc1 = plan_and_alloc_pipelined(c, tasks, distros, hosts, host_off, acfg, now_ns, plan_out, alloc_out);
+    c->tick.allocated = rc1 == EVG_OK;
+    return rc1;
   }
   int rc = upload(c, "evg_plan_and_alloc_batch", tasks, distros, hosts, host_off, acfg, Tick::kFixed);
   if (rc != EVG_OK) return rc;
@@ -4203,6 +4213,141 @@ int evg_rebuild_dispatchers(evg_ctx* c, int32_t cap, int64_t items_capacity, int
   DagBufs b{p.sorted.as<int32_t>(), p.stats.as<int32_t>(), {p.buf[0].as<int32_t>(), p.buf[1].as<int32_t>()}, p.group_off.as<int64_t>(),
             p.unit_off.as<int32_t>()};
   return dag_run(c, x, b, max_n, item_off, out->group_off, out->sorted, out->n_sorted, out->n_cycles, out->unit_items, out->unit_off);
+}
+
+// The group sums of the job's report (units/host_allocator.go:271-280) over slots [g, g1) with stride `step`, in wrapping
+// int64.  A single-task distro's CountFree / CountRequired stay 0: the reference never runs the allocator for it.
+struct JobSums { uint64_t overdue, n_over, d_over, expected, free, required; };
+__device__ __forceinline__ JobSums job_group_sums(const evg_group_info* __restrict__ gi, int64_t g, int64_t g1, int step, bool single) {
+  JobSums s{0, 0, 0, 0, 0, 0};
+  for (; g < g1; g += step) {
+    const evg_group_info& x = gi[g];
+    s.overdue += uint64_t(x.count_wait_over_threshold);
+    s.n_over += uint64_t(x.count_duration_over_threshold);
+    s.d_over += uint64_t(x.duration_over_threshold);
+    s.expected += uint64_t(x.expected_duration);
+    if (!single) { s.free += uint64_t(x.count_free); s.required += uint64_t(x.count_required); }
+  }
+  return s;
+}
+
+constexpr int64_t kHostJobWarpGroups = 16;  // k_host_job: a distro with more group slots has them summed by its warp
+constexpr int64_t kMaxPossibleTime = int64_t(2532000) * 3600 * 1000000000;  // maxPossibleHours * time.Hour (:309)
+
+// hostAllocatorJob.Run past the allocator (units/host_allocator.go:180-196, 253-337, 394-425), one thread per distro.
+// A distro with few group slots sums them itself; the warp sums those of each distro with many, one distro at a time,
+// all lanes striding over its slots (the k_alloc_groupless / k_alloc split).  Only reads the tick.
+__global__ void __launch_bounds__(128) k_host_job(int32_t n_distros, const int64_t* __restrict__ group_off, const int64_t* __restrict__ host_off,
+                                                  const evg_queue_info* __restrict__ qinfo, const evg_group_info* __restrict__ ginfo,
+                                                  const evg_alloc_result* __restrict__ result, const int32_t* __restrict__ status,
+                                                  const evg_alloc_cfg* __restrict__ acfg, const evg_host_job_cfg* __restrict__ cfg,
+                                                  const int32_t* __restrict__ spawned, int64_t* __restrict__ n_hosts_out,
+                                                  int64_t* __restrict__ n_free_out, int32_t* __restrict__ status_out,
+                                                  evg_host_report* __restrict__ report) {
+  const unsigned full = 0xffffffffu;
+  const int d = int(blockIdx.x * blockDim.x + threadIdx.x), lane = int(threadIdx.x & 31);
+  const bool in = d < n_distros;  // lanes past the end still take part in the warp's sums
+  const int64_t g0 = in ? group_off[d] : 0, g1 = in ? group_off[d + 1] : 0;
+  const evg_host_job_cfg jc = in ? cfg[d] : evg_host_job_cfg{0, 0, 0, 0, 0};
+  const bool wide = g1 - g0 > kHostJobWarpGroups;
+  JobSums s = job_group_sums(ginfo, g0, wide ? g0 : g1, 1, jc.single_task_distro != 0);
+  for (unsigned todo = __ballot_sync(full, wide); todo; todo &= todo - 1u) {
+    const int j = __ffs(todo) - 1;
+    const int64_t a = __shfl_sync(full, g0, j), b = __shfl_sync(full, g1, j);
+    const JobSums w = job_group_sums(ginfo, a + lane, b, 32, __shfl_sync(full, jc.single_task_distro, j) != 0);
+    const JobSums r{uint64_t(warp_sum64(int64_t(w.overdue))), uint64_t(warp_sum64(int64_t(w.n_over))),
+                    uint64_t(warp_sum64(int64_t(w.d_over))), uint64_t(warp_sum64(int64_t(w.expected))),
+                    uint64_t(warp_sum64(int64_t(w.free))), uint64_t(warp_sum64(int64_t(w.required)))};
+    if (lane == j) s = r;
+  }
+  if (!in) return;
+  const evg_queue_info& q = qinfo[d];
+  int64_t n_hosts, n_free;
+  int32_t st = EVG_ALLOC_OK;
+  if (jc.single_task_distro) {  // :182-184
+    n_hosts = wsub(q.length_with_dependencies_met, jc.n_provisioning);
+    n_free = 0;
+  } else {  // :186-195
+    const evg_alloc_result r = result[d];
+    n_hosts = r.new_hosts;
+    n_free = r.free_hosts;
+    st = status[d];
+  }
+  evg_host_report o{};
+  if (st == EVG_ALLOC_OK) {
+    const int64_t n_spawned = spawned ? int64_t(spawned[d]) : (n_hosts > 0 ? n_hosts : 0);
+    const int64_t sched = wsub(wsub(q.expected_duration, int64_t(s.expected)), wsub(q.duration_over_threshold, int64_t(s.d_over)));  // :283-287
+    const int64_t over_no_groups = wsub(q.count_duration_over_threshold, int64_t(s.n_over));                                         // :289
+    const int64_t spawned_standalone = wsub(n_spawned, int64_t(s.required));                                                        // :292
+    const int64_t avail = wsub(wadd(wsub(n_free, int64_t(s.free)), spawned_standalone), over_no_groups);                            // :294
+    int64_t tte = 0, tte_ns = 0;
+    if (sched > 0) {  // :304-321
+      const int64_t avail_ns = wsub(avail, spawned_standalone);
+      tte = avail <= 0 ? kMaxPossibleTime : sched / avail;
+      tte_ns = avail <= 0 || avail_ns <= 0 ? kMaxPossibleTime : sched / avail_ns;
+    }
+    const float thr = __ll2float_rn(q.max_duration_threshold);
+    const float ratio = __fdiv_rn(__ll2float_rn(tte), thr), ratio_ns = __fdiv_rn(__ll2float_rn(tte_ns), thr);  // :324-326
+    const evg_alloc_cfg ac = acfg[d];
+    const int64_t n_up = host_off[d + 1] - host_off[d];
+    if (jc.terminate_when_overallocated && ac.provider != EVG_PROVIDER_STATIC && ratio < 0.25f && n_up > 0 && !jc.hourly_billing) {
+      // setTargetAndTerminate (:394-425); the float -> int conversion saturates
+      const int64_t killable = ratio == 0.0f ? n_up : __float2ll_rz(__fmul_rn(__ll2float_rn(n_up), __fsub_rn(1.0f, ratio)));
+      int64_t cap = ratio == 0.0f ? 0 : n_up - killable;
+      if (cap < ac.minimum_hosts) cap = ac.minimum_hosts;
+      o.killable_hosts = killable;
+      o.new_cap_target = cap;
+      o.drawdown = killable > 0;
+    }
+    o.time_to_empty_ns = tte;
+    o.time_to_empty_no_spawns_ns = tte_ns;
+    o.scheduled_duration_ns = sched;
+    o.hosts_avail = avail;
+    o.hosts_spawned = n_spawned;
+    o.overdue_in_groups = int64_t(s.overdue);
+    o.free_in_groups = int64_t(s.free);
+    o.required_in_groups = int64_t(s.required);
+    o.host_queue_ratio = ratio;
+    o.no_spawns_ratio = ratio_ns;
+  }
+  n_hosts_out[d] = n_hosts;
+  n_free_out[d] = n_free;
+  status_out[d] = st;
+  report[d] = o;
+}
+
+int evg_host_job(evg_ctx* c, const evg_host_job_cfg* cfg, const int32_t* spawned, evg_host_job_out* out) {
+  if (!c) return fail(EVG_ERR_INVALID, "null context");
+  LOCK(c);
+  if (!cfg || !out || !out->n_hosts || !out->n_hosts_free || !out->status || !out->report)
+    return fail(EVG_ERR_INVALID, "evg_host_job: null cfg or output");
+  if (const int rc = need_tick(c, "evg_host_job", Need::kAllocated); rc != EVG_OK) return rc;
+  const int32_t D = c->Dn;
+  for (int32_t d = 0; d < D; d++)
+    if (cfg[d].n_provisioning < 0) return fail(EVG_ERR_INVALID, "evg_host_job: cfg[%d].n_provisioning is negative", d);
+  c->launches = 0;
+  if (D == 0) return EVG_OK;
+  CK(cudaSetDevice(c->device));
+  cudaStream_t s = c->stream;
+  auto& h = c->hj;
+  UP(s, h.cfg, cfg, D, evg_host_job_cfg);
+  if (spawned) UP(s, h.spawned, spawned, D, int32_t);
+  // outputs: the reports, then n_hosts, n_hosts_free and status
+  CK(h.out.ensure((sizeof(evg_host_report) + 2 * sizeof(int64_t) + sizeof(int32_t)) * size_t(D)));
+  evg_host_report* rep = h.out.as<evg_host_report>();
+  int64_t* nh = reinterpret_cast<int64_t*>(rep + D);
+  int64_t* nf = nh + D;
+  int32_t* st = reinterpret_cast<int32_t*>(nf + D);
+  LAUNCH(c, k_host_job, grid_for(D, 128), 128, D, c->b_groupoff.as<int64_t>(), c->b_hostoff.as<int64_t>(), c->b_qinfo.as<evg_queue_info>(),
+         c->b_ginfo.as<evg_group_info>(), c->result_ptr(), c->b_status.as<int32_t>(), c->b_acfg.as<evg_alloc_cfg>(),
+         h.cfg.as<evg_host_job_cfg>(), spawned ? h.spawned.as<int32_t>() : nullptr, nh, nf, st, rep);
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(out->report, rep, sizeof(evg_host_report) * size_t(D), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(out->n_hosts, nh, sizeof(int64_t) * size_t(D), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(out->n_hosts_free, nf, sizeof(int64_t) * size_t(D), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(out->status, st, sizeof(int32_t) * size_t(D), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));  // the caller's cfg / spawned arrays are free again and the outputs are written
+  return EVG_OK;
 }
 
 int evg_plan_distro(evg_ctx* c, const evg_task_soa* tasks, const evg_distro_cfg* cfg, int32_t n_groups,

@@ -65,6 +65,7 @@ PROVIDER_DOCKER = "docker"
 PROVIDER_STATIC = "static"
 PROVIDER_MOCK = "mock"
 PROVIDER_SPAWNABLE = (PROVIDER_EC2_ONDEMAND, PROVIDER_EC2_FLEET, PROVIDER_MOCK, PROVIDER_DOCKER)  # globals.go:723-728
+HOSTS_OVERALLOCATED_TERMINATE = "terminate-hosts-when-overallocated"  # globals.go:317
 # model/task_queue.go:216-219
 PERSISTED_QUEUE_CAP = 10000
 # model/task_queue.go:17-20: the collections TaskQueue.Save writes to
@@ -229,6 +230,7 @@ class Distro:
     dispatcher_settings: DispatcherSettings = field(default_factory=lambda: DispatcherSettings(version=""))
     valid_projects: List[str] = field(default_factory=list)
     aliases: List[str] = field(default_factory=list)  # Distro.Aliases (FindApplicableDistroIDs, model/distro/aliases.go:14-27)
+    arch: str = ""  # Distro.Arch (cloud.UsesHourlyBilling reads it, cloud/ec2_util.go:256-268)
 
     def max_duration_per_host(self) -> int:  # distro.go:422-432
         if self.container_pool != "":
@@ -377,6 +379,32 @@ class HostAllocatorData:  # scheduler/host_allocator.go:17-23
     # resolved lookups the reference performs against MongoDB
     running_tasks: dict = field(default_factory=dict)         # task id -> RunningTaskStats
     parent_distro_maximum_hosts: Optional[int] = None         # distro.FindOneId(pool.Distro) (allocator.go:151-160)
+
+
+@dataclass
+class HostAllocatorJobReport:
+    """The distro-scheduler-report hostAllocatorJob.Run computes after spawning (units/host_allocator.go:257-326), with
+    the drawdown decision of setTargetAndTerminate (:328-337, 394-425).  Ratios are float32 values, as Go computes them;
+    new_cap_target and killable_hosts are 0 when setTargetAndTerminate is not called."""
+    time_to_empty: int = 0
+    time_to_empty_no_spawns: int = 0
+    scheduled_duration: int = 0
+    hosts_avail: int = 0
+    hosts_spawned: int = 0
+    overdue_in_groups: int = 0
+    free_in_groups: int = 0
+    required_in_groups: int = 0
+    host_queue_ratio: float = 0.0
+    no_spawns_ratio: float = 0.0
+    drawdown: bool = False
+    new_cap_target: int = 0
+    killable_hosts: int = 0
+
+
+@dataclass
+class DrawdownInfo:  # units/host_drawdown.go:33-36
+    distro_id: str = ""
+    new_cap_target: int = 0
 
 
 def fetch_expected_duration(t: Task, now: int, history=None):

@@ -417,6 +417,22 @@ class Engine:
                 "group_off": o["group_off"], "group_slot": o["group_slot"][:G2], "unit_items": o["unit_items"][:N],
                 "unit_off": o["unit_off"][:G2 + D]}
 
+    def host_job(self, cfg: np.ndarray, spawned: Optional[np.ndarray] = None) -> dict:
+        """evg_host_job: hostAllocatorJob.Run past the allocator for every distro of the resident tick after run(),
+        on the device.  `cfg`: HOST_JOB_CFG rows (soa.marshal_host_job); `spawned`: len(hostsSpawned) per distro, None
+        = max(n_hosts, 0).  -> dict of n_hosts, n_hosts_free, status (EVG_ALLOC_*) and report (HOST_REPORT rows)."""
+        D = self._n_distros
+        cfg = np.ascontiguousarray(cfg, dtype=L.HOST_JOB_CFG_DTYPE)
+        if cfg.shape[0] != D or (spawned is not None and len(spawned) != D):
+            raise ValueError("one job setting and spawned count per distro of the resident tick")
+        sp = None if spawned is None else np.ascontiguousarray(spawned, dtype=np.int32)
+        o = {"n_hosts": self._out("job_n_hosts", max(D, 1), np.int64), "n_hosts_free": self._out("job_n_free", max(D, 1), np.int64),
+             "status": self._out("job_status", max(D, 1), np.int32), "report": self._out("job_report", max(D, 1), L.HOST_REPORT_DTYPE)}
+        st = L.HostJobOutStruct(*[L.ptr(o[f]) for f in ("n_hosts", "n_hosts_free", "status", "report")])
+        cfg_arg = cfg if D else np.zeros(1, L.HOST_JOB_CFG_DTYPE)
+        L.check(self.lib.evg_host_job(self.ctx, L.ptr(cfg_arg), L.ptr(sp) if sp is not None and D else None, C.byref(st)))
+        return {k: v[:D] for k, v in o.items()}
+
     def alloc_batch(self, hosts: S.HostSoA, qinfo: np.ndarray, ginfo: np.ndarray, group_off: np.ndarray, now: int):
         D = int(qinfo.shape[0])
         ao = self._alloc_output(D)
@@ -755,6 +771,58 @@ def hosts_to_request(distro: M.Distro, info: M.DistroQueueInfo, n_provisioning_h
     if distro.single_task_distro:
         return info.length_with_dependencies_met - n_provisioning_hosts, 0
     return allocate()
+
+
+# cloud/ec2_util.go:63-67
+BY_THE_SECOND_BILLING_OS = ("linux", "windows")
+COMMERCIAL_LINUX_DISTROS = ("suse",)
+
+
+def uses_hourly_billing(d: M.Distro) -> bool:
+    """cloud.UsesHourlyBilling (cloud/ec2_util.go:256-268): billed by the hour unless the arch names a by-the-second OS,
+    and always for a commercial Linux distro."""
+    by_the_second = any(a in d.arch for a in BY_THE_SECOND_BILLING_OS)
+    commercial = any(c in d.id for c in COMMERCIAL_LINUX_DISTROS)
+    return not by_the_second or commercial
+
+
+def host_job_results(distros: Sequence[M.Distro], res: dict) -> list:
+    """Engine.host_job's arrays -> [(n_hosts, n_hosts_free, HostAllocatorJobReport | None, DrawdownInfo | None)]: the
+    report is None when the allocator's error ended the job (units/host_allocator.go:192-195)."""
+    out = []
+    for i, d in enumerate(distros):
+        n, f = int(res["n_hosts"][i]), int(res["n_hosts_free"][i])
+        if int(res["status"][i]) != L.EVG_ALLOC_OK:
+            out.append((n, f, None, None))
+            continue
+        r = res["report"][i]
+        rep = M.HostAllocatorJobReport(
+            time_to_empty=int(r["time_to_empty_ns"]), time_to_empty_no_spawns=int(r["time_to_empty_no_spawns_ns"]),
+            scheduled_duration=int(r["scheduled_duration_ns"]), hosts_avail=int(r["hosts_avail"]),
+            hosts_spawned=int(r["hosts_spawned"]), overdue_in_groups=int(r["overdue_in_groups"]),
+            free_in_groups=int(r["free_in_groups"]), required_in_groups=int(r["required_in_groups"]),
+            host_queue_ratio=float(r["host_queue_ratio"]), no_spawns_ratio=float(r["no_spawns_ratio"]),
+            drawdown=bool(r["drawdown"]), new_cap_target=int(r["new_cap_target"]), killable_hosts=int(r["killable_hosts"]))
+        out.append((n, f, rep, M.DrawdownInfo(d.id, rep.new_cap_target) if rep.drawdown else None))
+    return out
+
+
+def host_allocator_jobs(batch: Sequence[Tuple[M.Distro, List[M.Task], M.HostAllocatorData]], now: int, *,
+                        n_provisioning: Sequence[int], spawned: Optional[Sequence[int]] = None,
+                        engine: Optional[Engine] = None, dependency_db: Optional[Dict[str, M.Task]] = None) -> list:
+    """hostAllocatorJob.Run for every distro of one tick (units/host_allocator.go:152-337, 394-425): the planner and
+    the allocator as plan_and_allocate runs them, then the single-task bypass, the time-to-empty report and the
+    drawdown decision on the device.  `n_provisioning[d]` = len(ProvisioningHosts()); `spawned[d]` = len(hostsSpawned)
+    (None: what CreateIntentHosts creates without a container pool, max(n_hosts, 0)).  Returns, per distro,
+    (n_hosts, n_hosts_free, HostAllocatorJobReport or None when the allocator failed, DrawdownInfo or None)."""
+    eng = engine or default_engine()
+    datas = [h for _, _, h in batch]
+    soa, table, keys = S.marshal_tasks([(d, t) for d, t, _ in batch], now, dependency_db)
+    hosts = S.marshal_hosts(datas, [k.group_names for k in keys])
+    _upload_with_device_deps(eng, batch, soa, table, hosts, now, dependency_db)
+    eng.run(now)
+    res = eng.host_job(S.marshal_host_job(datas, n_provisioning), None if spawned is None else np.asarray(spawned))
+    return host_job_results([d for d, _, _ in batch], res)
 
 
 def PrioritizeTasks(d: M.Distro, tasks: List[M.Task], opts: Optional[TaskPlannerOptions] = None, *, now: int,

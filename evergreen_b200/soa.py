@@ -530,6 +530,22 @@ def marshal_hosts(datas: Sequence[M.HostAllocatorData], group_names: Sequence[Se
                    np.array(rows, dtype=L.ALLOC_CFG_DTYPE)).normalize()
 
 
+def marshal_host_job(datas: Sequence[M.HostAllocatorData], n_provisioning: Sequence[int]) -> np.ndarray:
+    """[HostAllocatorData] + len(ProvisioningHosts()) per distro -> HOST_JOB_CFG rows (evg_host_job_cfg): what
+    hostAllocatorJob.Run reads besides the allocator's inputs (units/host_allocator.go:169-184, 330-333).  The billing
+    rule reads the distro itself: the up hosts' embedded distro document is that distro."""
+    from .scheduler import uses_hourly_billing
+    if len(n_provisioning) != len(datas):
+        raise ValueError("one provisioning count per distro")
+    rows = np.zeros(len(datas), dtype=L.HOST_JOB_CFG_DTYPE)
+    for i, (data, n) in enumerate(zip(datas, n_provisioning)):
+        d = data.distro
+        rows[i] = (int(n), int(d.single_task_distro),
+                   int(d.host_allocator_settings.hosts_overallocated_rule == M.HOSTS_OVERALLOCATED_TERMINATE),
+                   int(uses_hourly_billing(d)), 0)
+    return rows
+
+
 def queue_info_rows(infos: Sequence[M.DistroQueueInfo]):
     """[DistroQueueInfo] -> (QUEUE_INFO rows, GROUP_INFO rows, group_off, names per distro).
     Later duplicates of a name win, like the map built at allocator.go:243-246."""

@@ -46,7 +46,8 @@ enum {
   EVG_ERR_CUDA = -2,    /* no usable sm_90 device, or a CUDA call failed */
   EVG_ERR_NOMEM = -3,   /* device or pinned allocation failed */
   EVG_ERR_STATE = -4    /* the resident tick cannot serve the call: there is none, or it lacks what the call needs
-                           (its own columns, editability, hosts, dependency verdicts, alias map, resolved durations) */
+                           (its own columns, editability, hosts, dependency verdicts, alias map, resolved durations,
+                           an allocator run since it was set) */
 };
 
 /* per-distro allocator status: the data errors UtilizationBasedHostAllocator
@@ -871,6 +872,73 @@ typedef struct {
  * Replaces: the evg_download_queue -> dependency-id resolution -> compositeGroupID interning -> evg_dag_rebuild_batch
  * round trip a shim would make to hand FindNextTask d.sorted and d.taskGroups (:475-476, :527-543). */
 int evg_rebuild_dispatchers(evg_ctx* ctx, int32_t cap, int64_t items_capacity, int64_t groups_capacity, evg_dispatch_out* out);
+
+/* ---- the host allocator job's decisions (SURVEY.md §8 row A21) ---------------- */
+
+/* What hostAllocatorJob.Run reads besides HostAllocatorData, per distro, resolved by the shim.  24 B. */
+typedef struct {
+  int64_t n_provisioning;               /* len(existingHosts.ProvisioningHosts()) (units/host_allocator.go:169); not in the host SoA */
+  int32_t single_task_distro;           /* Distro.SingleTaskDistro (:182) */
+  int32_t terminate_when_overallocated; /* resolved HostsOverallocatedRule == "terminate-hosts-when-overallocated" (:330) */
+  int32_t hourly_billing;               /* cloud.UsesHourlyBilling(&upHosts[0].Distro) (:333, cloud/ec2_util.go:256-268) */
+  int32_t _reserved;
+} evg_host_job_cfg;
+
+/* The distro-scheduler-report of one distro (units/host_allocator.go:257-337, 394-425).  96 B. */
+typedef struct {
+  int64_t time_to_empty_ns;           /* timeToEmpty (:304-321) */
+  int64_t time_to_empty_no_spawns_ns; /* timeToEmptyNoSpawns */
+  int64_t scheduled_duration_ns;      /* scheduledDuration (:287) */
+  int64_t hosts_avail;                /* hostsAvail (:294) */
+  int64_t hosts_spawned;              /* len(hostsSpawned) the report used (:233, :292) */
+  int64_t overdue_in_groups;          /* totalOverdueInTaskGroups (:273) */
+  int64_t free_in_groups;             /* freeInTaskGroups (:277) */
+  int64_t required_in_groups;         /* requiredInTaskGroups (:278) */
+  int64_t new_cap_target;             /* DrawdownInfo.NewCapTarget (:399-405); 0 when setTargetAndTerminate is not called */
+  int64_t killable_hosts;             /* killableHosts (:396-400); 0 when setTargetAndTerminate is not called */
+  float host_queue_ratio;             /* hostQueueRatio (:324), float32 as Go computes it */
+  float no_spawns_ratio;              /* noSpawnsRatio (:326) */
+  int32_t drawdown;                   /* 1: the job enqueues a host drawdown job (killableHosts > lowCountFloor, :408) */
+  int32_t _reserved;
+} evg_host_report;
+
+/* Host pointers, n_distros entries each. */
+typedef struct {
+  int64_t* n_hosts;         /* nHosts handed to CreateIntentHosts (:184, :191) */
+  int64_t* n_hosts_free;    /* nHostsFree (:191); 0 for a single-task distro */
+  int32_t* status;          /* EVG_ALLOC_*: the allocator's error ends the job (:192-195) */
+  evg_host_report* report;  /* all zero when status != EVG_ALLOC_OK */
+} evg_host_job_out;
+
+/* hostAllocatorJob.Run after the allocator (units/host_allocator.go:180-196, 253-337, 394-425) for every distro of the
+ * resident tick, on the device, from the queue infos, group infos and allocator results evg_run_resident left there
+ * (the result rows are read wherever evg_bind_result_buffer put them).  The tick is only read: calling it twice gives
+ * the same answer, and every call allowed before it stays allowed.
+ *   - single-task distro (:182-184): n_hosts = LengthWithDependenciesMet - n_provisioning (may be negative), n_hosts_free
+ *     = 0, status EVG_ALLOC_OK; its group slots count CountFree = CountRequired = 0 (the reference never runs the
+ *     allocator for it, whatever k_alloc wrote on the device);
+ *   - any other distro: new_hosts, free_hosts and status of the allocator run; a status other than EVG_ALLOC_OK ends the
+ *     job there (:192-195) and the report is zero;
+ *   - spawned[d] = len(hostsSpawned) (:233); spawned == NULL means max(n_hosts, 0), what CreateIntentHosts creates
+ *     without a container pool (scheduler/scheduler.go:172-215); a pool distro's shim calls again with the count
+ *     MakeContainersAndParents returned;
+ *   - report (:257-326): sums over the distro's group slots (its named TaskGroupInfos; the ungrouped info is excluded),
+ *     int64 arithmetic with wrap, timeToEmpty truncated toward zero, 2532000 h when its host count is <= 0, both times
+ *     0 when scheduledDuration <= 0; the ratios are float32(int64) rounded to nearest-even and divided IEEE-correctly
+ *     (MaxDurationThreshold 0 gives +Inf or NaN, as Go does);
+ *   - drawdown (:328-337, 394-425): when terminate_when_overallocated, the provider is not EVG_PROVIDER_STATIC
+ *     (evergreen.ProviderSpawnable), hostQueueRatio < 0.25f, the distro has up hosts (its hosts in the host SoA) and
+ *     !hourly_billing: killable = n_up when the ratio is 0, else int(float32(n_up) * (1 - ratio)) truncated (saturated
+ *     at the int64 range, which only a negative MaxDurationThreshold can reach; Go leaves that conversion
+ *     implementation-defined), new_cap_target = n_up - killable floored at MinimumHosts; drawdown = killable > 0.
+ * What the library does not model and the shim applies itself: a disabled distro returns before this phase (:144-146);
+ * the intent-host cap (:212-229) and a CreateIntentHosts error (:233-237) end the job before the report, so the shim
+ * discards that distro's report; choosing the hosts to decommission is the drawdown job's (units/host_drawdown.go).
+ * EVG_ERR_INVALID with nothing launched: null cfg or out (or a null array of out), a negative n_provisioning.
+ * EVG_ERR_STATE: no resident tick, a tick without hosts, or no evg_run_resident on it since it was set (the one-shot
+ * evg_plan_and_alloc_batch counts as one).  The first call allocates the call's own small buffers.
+ * Replaces: the single-task bypass, the time-to-empty report and the drawdown decision of hostAllocatorJob.Run. */
+int evg_host_job(evg_ctx* ctx, const evg_host_job_cfg* cfg, const int32_t* spawned, evg_host_job_out* out);
 
 /* ---- single-distro wrappers: the per-job drop-in ------------------------- */
 
