@@ -78,12 +78,6 @@ int check_offsets(const int64_t* off, int64_t n, int64_t total, const char* who,
               (long long)row, (long long)off[row], total >= 0 ? std::to_string(total).c_str() : "the count");
 }
 
-// One of the nine planner columns of an evg_task_soa is null.
-bool task_cols_missing(const evg_task_soa* t) {
-  return !t->priority || !t->expected_ns || !t->queue_basis_ns || !t->wait_basis_ns || !t->num_dependents || !t->task_group_order ||
-         !t->group_id || !t->version_id || !t->flags;
-}
-
 #define CK(call)                                                                              \
   do {                                                                                        \
     cudaError_t e_ = (call);                                                                  \
@@ -170,6 +164,8 @@ constexpr int kNT_C = 512, kNCapC = 10240, kNOccC = 2;
 constexpr uint32_t kInactive = 0xFFFFFFFFu;  // next[]: pair not linked / head[]: empty list
 constexpr uint32_t kEnd = 0xFFFFFFFEu;       // next[]: end of list
 constexpr uint32_t kNoAnchor = 0xFFFFFFFFu;
+// Columns are padded so that 128-bit loads and TMA copies that start inside the table may run past its last row.
+constexpr int64_t kColPad = 8;
 
 }  // namespace
 
@@ -189,6 +185,12 @@ struct DTasks {
   const uint32_t* flags;
   const int64_t* dep_off;
   const int32_t* dep_idx;
+};
+
+struct EdDst {  // the shadow column set the composed table is written to
+  int32_t *priority, *numdep, *tgo, *gid, *vid;
+  uint32_t* flags;
+  int64_t *expected, *qbasis, *wbasis;
 };
 
 struct DDistros {
@@ -1160,32 +1162,95 @@ __global__ void __launch_bounds__(128) k_alloc_groupless(DHosts H, int32_t d_beg
 // --------------------------------------------------------------------------
 // context
 // --------------------------------------------------------------------------
-struct TaskCols {  // the nine planner columns of a task table
+// The nine planner columns of a task table.  each() is the one list of them: every check, copy and view of the columns
+// goes through it, so a column is added or changed there alone.
+struct TaskCols {
   DevBuf prio, nd, tgo, gid, vid, flags, exp, qb, wb;
-  int stage(const evg_task_soa* t, int64_t n, cudaStream_t s) {  // copy the first n rows of t's columns
-    UP(s, prio, t->priority, n, int32_t);
-    UP(s, nd, t->num_dependents, n, int32_t);
-    UP(s, tgo, t->task_group_order, n, int32_t);
-    UP(s, gid, t->group_id, n, int32_t);
-    UP(s, vid, t->version_id, n, int32_t);
-    UP(s, flags, t->flags, n, uint32_t);
-    UP(s, exp, t->expected_ns, n, int64_t);
-    UP(s, qb, t->queue_basis_ns, n, int64_t);
-    UP(s, wb, t->wait_basis_ns, n, int64_t);
-    return EVG_OK;
+
+  // f(buffer, evg_task_soa field, field name) -> int for every column, the 8-byte ones first (evg_update_tasks packs
+  // them in this order); stops at the first f that does not return EVG_OK and returns its code.
+  template <class F>
+  static int each(F&& f) {
+    int rc = EVG_OK;
+    auto col = [&](DevBuf TaskCols::*b, auto field, const char* name) { if (rc == EVG_OK) rc = f(b, field, name); };
+    col(&TaskCols::exp, &evg_task_soa::expected_ns, "expected_ns");
+    col(&TaskCols::qb, &evg_task_soa::queue_basis_ns, "queue_basis_ns");
+    col(&TaskCols::wb, &evg_task_soa::wait_basis_ns, "wait_basis_ns");
+    col(&TaskCols::prio, &evg_task_soa::priority, "priority");
+    col(&TaskCols::nd, &evg_task_soa::num_dependents, "num_dependents");
+    col(&TaskCols::tgo, &evg_task_soa::task_group_order, "task_group_order");
+    col(&TaskCols::gid, &evg_task_soa::group_id, "group_id");
+    col(&TaskCols::vid, &evg_task_soa::version_id, "version_id");
+    col(&TaskCols::flags, &evg_task_soa::flags, "flags");
+    return rc;
   }
-  DTasks view(int64_t n) const {  // n rows, no edges
-    DTasks v;
-    memset(&v, 0, sizeof(v));
-    v.n = n;
+  template <class T>
+  static constexpr size_t elem(const T* evg_task_soa::*) { return sizeof(T); }
+  template <class T>
+  static void point(const T*& field, const void* p) { field = static_cast<const T*>(p); }
+  static bool is_id(DevBuf TaskCols::*b) { return b == &TaskCols::gid || b == &TaskCols::vid; }
+
+  // Some column of t is null; without `ids`, group_id and version_id are not looked at.
+  static bool missing(const evg_task_soa* t, bool ids = true) {
+    return each([&](auto b, auto f, const char*) { return t->*f || (!ids && is_id(b)) ? EVG_OK : EVG_ERR_INVALID; }) != EVG_OK;
+  }
+  // Every column grown to n rows and kColPad rows of padding; with `zero_pad`, the padding zeroed on s as an upload
+  // leaves it.
+  int size(int64_t n, cudaStream_t s = nullptr, bool zero_pad = false) {
+    return each([&](auto b, auto f, const char*) -> int {
+      CK((this->*b).ensure(elem(f) * size_t(n + kColPad)));
+      if (zero_pad) CK(cudaMemsetAsync(static_cast<char*>((this->*b).p) + elem(f) * n, 0, elem(f) * kColPad, s));
+      return EVG_OK;
+    });
+  }
+  // Rows [t0, t0 + n) of t's columns from host memory into the same rows here, on s.
+  int copy_rows(const evg_task_soa* t, int64_t t0, int64_t n, cudaStream_t s) {
+    return each([&](auto b, auto f, const char*) -> int {
+      if (n > 0) CK(cudaMemcpyAsync(static_cast<char*>((this->*b).p) + elem(f) * t0, t->*f + t0, elem(f) * n, cudaMemcpyHostToDevice, s));
+      return EVG_OK;
+    });
+  }
+  // The first n rows of t's columns, each grown to at least one row.
+  int stage(const evg_task_soa* t, int64_t n, cudaStream_t s) {
+    const int rc = each([&](auto b, auto f, const char*) -> int {
+      CK((this->*b).ensure(elem(f) * size_t(n > 0 ? n : 1)));
+      return EVG_OK;
+    });
+    return rc != EVG_OK ? rc : copy_rows(t, 0, n, s);
+  }
+  // t's columns are caller-owned device memory, borrowed as they are (evg_upload_device).
+  int adopt(const evg_task_soa* t) {
+    return each([&](auto b, auto f, const char* name) -> int {
+      if ((reinterpret_cast<uintptr_t>(t->*f) & 15u) != 0) return fail(EVG_ERR_INVALID, "device column t->%s is not 16-byte aligned", name);
+      (this->*b).adopt(const_cast<void*>(static_cast<const void*>(t->*f)));
+      return EVG_OK;
+    });
+  }
+  // The columns as an evg_task_soa of n rows without edges.
+  evg_task_soa soa(int64_t n) const {
+    evg_task_soa s;
+    memset(&s, 0, sizeof(s));
+    s.n_tasks = n;
+    each([&](auto b, auto f, const char*) -> int { point(s.*f, (this->*b).p); return EVG_OK; });
+    return s;
+  }
+  // The device views: DTasks of n rows without edges, and the EdDst a composed table is written to.
+  template <class V>
+  V fill(V v) const {
     v.priority = prio.as<int32_t>(); v.expected = exp.as<int64_t>(); v.qbasis = qb.as<int64_t>(); v.wbasis = wb.as<int64_t>();
     v.numdep = nd.as<int32_t>(); v.tgo = tgo.as<int32_t>(); v.gid = gid.as<int32_t>(); v.vid = vid.as<int32_t>();
     v.flags = flags.as<uint32_t>();
     return v;
   }
+  DTasks view(int64_t n) const {
+    DTasks v;
+    memset(&v, 0, sizeof(v));
+    v.n = n;
+    return fill(v);
+  }
+  EdDst dst() const { return fill(EdDst{}); }
   void swap(TaskCols& o) {
-    prio.swap(o.prio); nd.swap(o.nd); tgo.swap(o.tgo); gid.swap(o.gid); vid.swap(o.vid);
-    flags.swap(o.flags); exp.swap(o.exp); qb.swap(o.qb); wb.swap(o.wb);
+    each([&](auto b, auto, const char*) -> int { (this->*b).swap(o.*b); return EVG_OK; });
   }
 };
 
@@ -1317,8 +1382,22 @@ DWork dwork(const evg_ctx* c);
 DGen dgen(const evg_ctx* c);
 inline unsigned grid_for(int64_t n, int block) { return unsigned((n + block - 1) / block); }
 
-// Columns are padded so that 128-bit loads and TMA copies that start inside the table may run past its last row.
-constexpr int64_t kColPad = 8;
+// Every kernel of this file is launched here: an empty grid launches nothing, any other launch adds one to the count
+// evg_last_launch_count reports.  Launch errors are left to the caller's CK(cudaGetLastError()).
+template <class... P, class... A>
+void launch(evg_ctx* c, cudaStream_t st, void (*kernel)(P...), unsigned grid, unsigned block, size_t smem, A&&... args) {
+  if (grid == 0) return;
+  kernel<<<grid, block, smem, st>>>(std::forward<A>(args)...);
+  c->launches++;
+}
+
+// The start of every entry point that takes a context: it names the call once (`who`, for its later messages too), fails
+// a null context with that name, holds the context's lock for the rest of the call and selects the context's device.
+#define ENTER(c, name)                                                    \
+  const char* const who = (name);                                         \
+  if (!(c)) return fail(EVG_ERR_INVALID, "%s: null context", who);       \
+  std::lock_guard<std::recursive_mutex> lock_((c)->mu);                   \
+  CK(cudaSetDevice((c)->device))
 
 // A call that writes the resident columns or the tables beside them (a new table, or scratch it shares with the
 // planner's inputs) drops the tick before its first such write: a call that fails partway must not leave the next
@@ -1363,7 +1442,7 @@ int upload_tasks(evg_ctx* c, const char* who, const evg_task_soa* t, const evg_d
   if (T >= (int64_t(1) << 31) - 2) return fail(EVG_ERR_INVALID, "n_tasks %lld exceeds 2^31-2 per call", (long long)T);
   if (2 * T + E >= int64_t(0xFFFFFFF0u)) return fail(EVG_ERR_INVALID, "2*n_tasks+n_edges exceeds the 32-bit pair id space");
   if (D > 0 && (!dt->task_off || !dt->group_off || !dt->cfg)) return fail(EVG_ERR_INVALID, "null distro arrays");
-  if (T > 0 && task_cols_missing(t)) return fail(EVG_ERR_INVALID, "null task column");
+  if (T > 0 && TaskCols::missing(t)) return fail(EVG_ERR_INVALID, "null task column");
   if (E > 0 && (!t->dep_off || !t->dep_idx)) return fail(EVG_ERR_INVALID, "n_edges > 0 but dep_off/dep_idx null");
   if (D == 0 && T != 0) return fail(EVG_ERR_INVALID, "tasks without distros");
   int rc = D > 0 ? check_offsets(dt->task_off, D, T, who, "task_off") : EVG_OK;
@@ -1443,6 +1522,10 @@ int upload_tasks(evg_ctx* c, const char* who, const evg_task_soa* t, const evg_d
   const int64_t P = 2 * T + E;
   cudaStream_t s = c->stream;
   drop_tick(c);
+  if (adopt) rc = c->tasks.adopt(t);
+  else if (cols != Cols::kResident) rc = c->tasks.size(T);
+  if (rc == EVG_OK && copy_columns) rc = c->tasks.copy_rows(t, 0, T, s);
+  if (rc != EVG_OK) return rc;
 #define UPC(buf, ptr, count, type)                                                                    \
   do {                                                                                                \
     if (cols == Cols::kResident) break;                                                               \
@@ -1454,15 +1537,6 @@ int upload_tasks(evg_ctx* c, const char* who, const evg_task_soa* t, const evg_d
       if (copy_columns && (count) > 0) CK(cudaMemcpyAsync((buf).p, (ptr), sizeof(type) * size_t(count), cudaMemcpyHostToDevice, s)); \
     }                                                                                                 \
   } while (0)
-  UPC(c->tasks.prio, t->priority, T, int32_t);
-  UPC(c->tasks.exp, t->expected_ns, T, int64_t);
-  UPC(c->tasks.qb, t->queue_basis_ns, T, int64_t);
-  UPC(c->tasks.wb, t->wait_basis_ns, T, int64_t);
-  UPC(c->tasks.nd, t->num_dependents, T, int32_t);
-  UPC(c->tasks.tgo, t->task_group_order, T, int32_t);
-  UPC(c->tasks.gid, t->group_id, T, int32_t);
-  UPC(c->tasks.vid, t->version_id, T, int32_t);
-  UPC(c->tasks.flags, t->flags, T, uint32_t);
   if (E > 0) {
     UPC(c->b_depoff, t->dep_off, T + 1, int64_t);
     UPC(c->b_depidx, t->dep_idx, E, int32_t);
@@ -1574,10 +1648,7 @@ int upload_tasks(evg_ctx* c, const char* who, const evg_task_soa* t, const evg_d
   c->tick.kind = adopt ? Tick::kBorrowed : Tick::kFixed;  // the entry point that uploaded says whether evg_edit_tasks may follow
   c->alist_valid = false;  // upload_hosts lists the allocator's distros against THIS table
   if (cols != Cols::kChunked && T > 0) {  // range-check the ids the kernels index with
-    DTasks dtv = dtasks(c);
-    DDistros ddv = ddistros(c);
-    DWork wv = dwork(c);
-    k_validate<<<grid_for(T, 256), 256, 0, s>>>(dtv, ddv, wv, 0, T);
+    launch(c, s, k_validate, grid_for(T, 256), 256, 0, dtasks(c), ddistros(c), dwork(c), int64_t(0), T);
     int bad = 0;
     CK(cudaMemcpyAsync(&bad, c->b_err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
@@ -1677,15 +1748,6 @@ DGen dgen(const evg_ctx* c) {
   return g;
 }
 
-#define LOCK(c) std::lock_guard<std::recursive_mutex> lock_((c)->mu)
-#define LAUNCH_ON(c, st, kernel, grid, block, ...)                           \
-  do {                                                                       \
-    if ((grid) > 0) {                                                        \
-      kernel<<<(grid), (block), 0, (st)>>>(__VA_ARGS__);                     \
-      (c)->launches++;                                                       \
-    }                                                                        \
-  } while (0)
-#define LAUNCH(c, kernel, grid, block, ...) LAUNCH_ON(c, (c)->stream, kernel, grid, block, __VA_ARGS__)
 
 int run_alloc_range(evg_ctx* c, int64_t now, int32_t d0, int32_t d1) {
   DHosts h;
@@ -1702,14 +1764,14 @@ int run_alloc_range(evg_ctx* c, int64_t now, int32_t d0, int32_t d1) {
   const int32_t* al = listed ? c->b_alist.as<int32_t>() : nullptr;
   const int64_t teams = listed ? c->n_alist : int64_t(d1 - d0);
   if (c->max_groups > kWideAllocGroups)
-    LAUNCH(c, k_alloc<128>, unsigned(teams), 128, h, d0, d1, c->b_groupoff.as<int64_t>(), c->b_qinfo.as<evg_queue_info>(),
+    launch(c, c->stream, k_alloc<128>, unsigned(teams), 128, 0, h, d0, d1, c->b_groupoff.as<int64_t>(), c->b_qinfo.as<evg_queue_info>(),
            c->b_ginfo.as<evg_group_info>(), c->b_gs.as<GroupScratch>(), now, c->result_ptr(), c->b_status.as<int32_t>(), split, al, int32_t(c->n_alist));
   else
-    LAUNCH(c, k_alloc<32>, grid_for(teams, 4), 128, h, d0, d1, c->b_groupoff.as<int64_t>(), c->b_qinfo.as<evg_queue_info>(),
+    launch(c, c->stream, k_alloc<32>, grid_for(teams, 4), 128, 0, h, d0, d1, c->b_groupoff.as<int64_t>(), c->b_qinfo.as<evg_queue_info>(),
            c->b_ginfo.as<evg_group_info>(), c->b_gs.as<GroupScratch>(), now, c->result_ptr(), c->b_status.as<int32_t>(), split, al, int32_t(c->n_alist));
   if (split)
-    LAUNCH(c, k_alloc_groupless, grid_for(d1 - d0, 128), 128, h, d0, d1, c->b_groupoff.as<int64_t>(), c->b_qinfo.as<evg_queue_info>(), now,
-           c->result_ptr(), c->b_status.as<int32_t>());
+    launch(c, c->stream, k_alloc_groupless, grid_for(d1 - d0, 128), 128, 0, h, d0, d1, c->b_groupoff.as<int64_t>(), c->b_qinfo.as<evg_queue_info>(),
+           now, c->result_ptr(), c->b_status.as<int32_t>());
   CK(cudaGetLastError());
   return EVG_OK;
 }
@@ -1721,9 +1783,8 @@ int launch_smem(evg_ctx* c, cudaStream_t st, const DTasks& dt, const DDistros& d
   if (n <= 0) return EVG_OK;
   const size_t bytes = PlanSmem<THREADS, ITEMS>::kBytes;
   CK(cudaFuncSetAttribute(k_plan_smem<THREADS, ITEMS, MIN_CTAS>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(bytes)));
-  k_plan_smem<THREADS, ITEMS, MIN_CTAS><<<unsigned(n), THREADS, bytes, st>>>(dt, dd, w, list, list_count, now, lists_needed,
-                                                                          c->b_order.as<int32_t>(), c->b_tv.as<int64_t>());
-  c->launches++;
+  launch(c, st, k_plan_smem<THREADS, ITEMS, MIN_CTAS>, unsigned(n), THREADS, bytes, dt, dd, w, list, list_count, now, lists_needed,
+         c->b_order.as<int32_t>(), c->b_tv.as<int64_t>());
   return EVG_OK;
 }
 
@@ -1734,9 +1795,8 @@ int launch_cta(evg_ctx* c, cudaStream_t st, const DTasks& dt, const DDistros& dd
   if (n <= 0) return EVG_OK;
   const size_t bytes = PlanCta<THREADS, CAP>::kBytes;
   CK(cudaFuncSetAttribute(k_plan_cta<THREADS, CAP, OCC>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(bytes)));
-  k_plan_cta<THREADS, CAP, OCC><<<unsigned(n), THREADS, bytes, st>>>(dt, dd, w, list, now, c->t_pad, c->b_order.as<int32_t>(),
-                                                                  c->b_tv.as<int64_t>(), punt_list, punt_count);
-  c->launches++;
+  launch(c, st, k_plan_cta<THREADS, CAP, OCC>, unsigned(n), THREADS, bytes, dt, dd, w, list, now, c->t_pad, c->b_order.as<int32_t>(),
+         c->b_tv.as<int64_t>(), punt_list, punt_count);
   return EVG_OK;
 }
 
@@ -1744,10 +1804,8 @@ int launch_cta(evg_ctx* c, cudaStream_t st, const DTasks& dt, const DDistros& dd
 // sends them through the smallest on-chip class instead.
 int launch_tiny(evg_ctx* c, cudaStream_t st, const DTasks& dt, const DDistros& dd, const DWork& w, const int32_t* list, int32_t n,
                 int64_t now, int lists_needed) {
-  if (n <= 0) return EVG_OK;
   if (lists_needed) return launch_smem<128, 8, 8>(c, st, dt, dd, w, list, n, now, 1);
-  k_plan_warp<<<grid_for(int64_t(n) * 32, 256), 256, 0, st>>>(dt, dd, w, list, n, now, c->b_order.as<int32_t>(), c->b_tv.as<int64_t>());
-  c->launches++;
+  launch(c, st, k_plan_warp, grid_for(int64_t(n) * 32, 256), 256, 0, dt, dd, w, list, n, now, c->b_order.as<int32_t>(), c->b_tv.as<int64_t>());
   return EVG_OK;
 }
 
@@ -1779,37 +1837,37 @@ int run_general(evg_ctx* c, cudaStream_t st, const DTasks& dt, const DDistros& d
   g.tile0 = c->h_dtileoff[size_t(d_first)];
   const unsigned nt = unsigned(c->h_dtileoff[size_t(d_last) + 1] - g.tile0);
   const int32_t* gl = c->routes[kGeneral].b.as<int32_t>() + gfirst;
-  LAUNCH_ON(c, st, k_ginit, grid_for(gcount, 256), 256, g, gl, gcount);
-  if (gc && c->E > 0) LAUNCH_ON(c, st, k_gmark, nt, 256, dt, dd, w, g);
+  launch(c, st, k_ginit, grid_for(gcount, 256), 256, 0, g, gl, gcount);
+  if (gc && c->E > 0) launch(c, st, k_gmark, nt, 256, 0, dt, dd, w, g);
   if (c->timed) CK(cudaEventRecord(c->ev_gt0, st));
-  LAUNCH_ON(c, st, k_gtask, nt, 256, dt, dd, w, g, now, gc);
+  launch(c, st, k_gtask, nt, 256, 0, dt, dd, w, g, now, gc);
   if (c->timed) { CK(cudaEventRecord(c->ev_gt1, st)); c->general_timed = true; }
   const unsigned wl_grid = unsigned(std::min<int64_t>(std::max<int64_t>(1, (c->Tgc + 255) / 256), int64_t(c->num_sms) * 16));
   if (gc) {
-    LAUNCH_ON(c, st, k_glink, wl_grid, 256, dt, dd, w, g, now);
-    LAUNCH_ON(c, st, k_galloc, wl_grid, 256, dt, dd, w, g);
-    LAUNCH_ON(c, st, k_gfill, wl_grid, 256, dt, dd, w, g);
-    LAUNCH_ON(c, st, k_gunit, wl_grid, 256, dd, w, g, now);
-    LAUNCH_ON(c, st, k_grank, wl_grid, 256, w, g);
-    LAUNCH_ON(c, st, k_gbest, wl_grid, 256, dt, dd, w, g, c->bd_valid ? 1 : 0);
+    launch(c, st, k_glink, wl_grid, 256, 0, dt, dd, w, g, now);
+    launch(c, st, k_galloc, wl_grid, 256, 0, dt, dd, w, g);
+    launch(c, st, k_gfill, wl_grid, 256, 0, dt, dd, w, g);
+    launch(c, st, k_gunit, wl_grid, 256, 0, dd, w, g, now);
+    launch(c, st, k_grank, wl_grid, 256, 0, w, g);
+    launch(c, st, k_gbest, wl_grid, 256, 0, dt, dd, w, g, c->bd_valid ? 1 : 0);
   }
-  LAUNCH_ON(c, st, k_gsched, grid_for(gcount, 128), 128, g, gl, gcount);
+  launch(c, st, k_gsched, grid_for(gcount, 128), 128, 0, g, gl, gcount);
   if (gc) {
-    LAUNCH_ON(c, st, k_gsum, nt, 256, dd, g);
-    LAUNCH_ON(c, st, k_gscan, unsigned(gcount), 1024, g, gl);
+    launch(c, st, k_gsum, nt, 256, 0, dd, g);
+    launch(c, st, k_gscan, unsigned(gcount), 1024, 0, g, gl);
   }
-  LAUNCH_ON(c, st, k_gplace, nt, 256, dd, w, g, gc);
-  if (gc) LAUNCH_ON(c, st, k_gplace_disp, wl_grid, 256, dt, dd, w, g);
+  launch(c, st, k_gplace, nt, 256, 0, dd, w, g, gc);
+  if (gc) launch(c, st, k_gplace_disp, wl_grid, 256, 0, dt, dd, w, g);
   if (c->timed) CK(cudaEventRecord(c->ev_sort0, st));  // the general path's segmented sort
   for (int j = 0; j < 8; j++) {  // passes beyond the tick's longest key exit at once (*maxpass is device-side)
-    LAUNCH_ON(c, st, k_ghist, nt, 256, j, dd, g);
-    LAUNCH_ON(c, st, k_gdscan, unsigned(gcount), 1024, j, gl, g);
-    LAUNCH_ON(c, st, k_gscatter, nt, 256, j, dd, g);
+    launch(c, st, k_ghist, nt, 256, 0, j, dd, g);
+    launch(c, st, k_gdscan, unsigned(gcount), 1024, 0, j, gl, g);
+    launch(c, st, k_gscatter, nt, 256, 0, j, dd, g);
   }
   if (c->timed) CK(cudaEventRecord(c->ev_sort1, st));
-  LAUNCH_ON(c, st, k_gemit, nt, 256, dd, g, c->b_order.as<int32_t>(), c->b_tv.as<int64_t>());
+  launch(c, st, k_gemit, nt, 256, 0, dd, g, c->b_order.as<int32_t>(), c->b_tv.as<int64_t>());
   const int64_t g0 = c->h_groupoff[size_t(d_first)], g1 = c->h_groupoff[size_t(d_last) + 1];
-  LAUNCH_ON(c, st, k_finalize_info, grid_for(std::max<int64_t>(d_last + 1 - d_first, g1 - g0), 256), 256, dd, w, d_first, d_last + 1, g0, g1);
+  launch(c, st, k_finalize_info, grid_for(std::max<int64_t>(d_last + 1 - d_first, g1 - g0), 256), 256, 0, dd, w, d_first, d_last + 1, g0, g1);
   return EVG_OK;
 }
 
@@ -1925,7 +1983,7 @@ int run_plan(evg_ctx* c, int64_t now, uint32_t opts) {
       CK(cudaStreamWaitEvent(s, c->ev_join[k], 0));
     }
   }
-  if (bd) LAUNCH(c, k_breakdown, grid_for(T, 256), 256, dt, dd, w, c->b_run.as<uint32_t>(), c->b_pay.as<URec>(), now, c->any_complex, c->b_order.as<int32_t>(), bd);
+  if (bd) launch(c, c->stream, k_breakdown, grid_for(T, 256), 256, 0, dt, dd, w, c->b_run.as<uint32_t>(), c->b_pay.as<URec>(), now, c->any_complex, c->b_order.as<int32_t>(), bd);
   CK(cudaGetLastError());
   return EVG_OK;
 }
@@ -1986,7 +2044,6 @@ void evg_shutdown(evg_ctx* c) {
 static int upload(evg_ctx* c, const char* who, const evg_task_soa* tasks, const evg_distro_table* distros, const evg_host_soa* hosts,
                   const int64_t* host_off, const evg_alloc_cfg* acfg, Tick kind, Cols cols = Cols::kCopy,
                   const int64_t* edge_off = nullptr) {
-  CK(cudaSetDevice(c->device));
   int rc = upload_tasks(c, who, tasks, distros, cols, edge_off);
   if (rc != EVG_OK) return rc;
   if (hosts) {
@@ -1999,9 +2056,8 @@ static int upload(evg_ctx* c, const char* who, const evg_task_soa* tasks, const 
 }
 int evg_upload(evg_ctx* c, const evg_task_soa* tasks, const evg_distro_table* distros, const evg_host_soa* hosts,
                const int64_t* host_off, const evg_alloc_cfg* acfg) {
-  if (!c) return fail(EVG_ERR_INVALID, "null context");
-  LOCK(c);
-  return upload(c, "evg_upload", tasks, distros, hosts, host_off, acfg, Tick::kOwn);
+  ENTER(c, "evg_upload");
+  return upload(c, who, tasks, distros, hosts, host_off, acfg, Tick::kOwn);
 }
 
 __global__ void k_gather_i64(const int64_t* __restrict__ src, const int64_t* __restrict__ at, int64_t* __restrict__ out, int n) {
@@ -2024,38 +2080,35 @@ __global__ void __launch_bounds__(256) k_update_rows(int64_t n, const int64_t* _
 }
 
 int evg_update_tasks(evg_ctx* c, int64_t n_rows, const int64_t* rows, const evg_task_soa* v) {
-  if (!c) return fail(EVG_ERR_INVALID, "null context");
-  LOCK(c);
-  if (const int rc = need_tick(c, "evg_update_tasks", Need::kOwnColumns); rc != EVG_OK) return rc;
+  ENTER(c, "evg_update_tasks");
+  if (const int rc = need_tick(c, who, Need::kOwnColumns); rc != EVG_OK) return rc;
   if (n_rows < 0) return fail(EVG_ERR_INVALID, "negative row count");
   if (n_rows == 0) return EVG_OK;
-  if (!rows || !v || v->n_tasks != n_rows || !v->priority || !v->num_dependents || !v->task_group_order || !v->flags || !v->expected_ns ||
-      !v->queue_basis_ns || !v->wait_basis_ns)
+  if (!rows || !v || v->n_tasks != n_rows || TaskCols::missing(v, /*ids=*/false))
     return fail(EVG_ERR_INVALID, "evg_update_tasks: rows and a %lld-row value table (priority, num_dependents, task_group_order, flags, "
                                  "expected_ns, queue_basis_ns, wait_basis_ns) are required", (long long)n_rows);
-  CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   const size_t n = size_t(n_rows);
-  // staging: rows (8) + three 8-byte and four 4-byte columns = 48 B per changed row
+  // staging: rows (8) + the nine columns but group_id and version_id, the 8-byte ones first = 48 B per changed row
   CK(c->b_upd.ensure(n * 48 + 64));
-  unsigned char* base = c->b_upd.as<unsigned char>();
-  int64_t* d_rows = reinterpret_cast<int64_t*>(base);
-  int64_t* d_exp = d_rows + n; int64_t* d_qb = d_exp + n; int64_t* d_wb = d_qb + n;
-  int32_t* d_prio = reinterpret_cast<int32_t*>(d_wb + n); int32_t* d_nd = d_prio + n; int32_t* d_tgo = d_nd + n;
-  uint32_t* d_fl = reinterpret_cast<uint32_t*>(d_tgo + n);
-  CK(cudaMemcpyAsync(d_rows, rows, n * 8, cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(d_exp, v->expected_ns, n * 8, cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(d_qb, v->queue_basis_ns, n * 8, cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(d_wb, v->wait_basis_ns, n * 8, cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(d_prio, v->priority, n * 4, cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(d_nd, v->num_dependents, n * 4, cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(d_tgo, v->task_group_order, n * 4, cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(d_fl, v->flags, n * 4, cudaMemcpyHostToDevice, s));
-  int* bad = reinterpret_cast<int*>(base + n * 48);
+  unsigned char* at = c->b_upd.as<unsigned char>();
+  const int64_t* d_rows = reinterpret_cast<int64_t*>(at);
+  CK(cudaMemcpyAsync(at, rows, n * 8, cudaMemcpyHostToDevice, s));
+  at += n * 8;
+  evg_task_soa d{};  // the staged values
+  const int rc = TaskCols::each([&](auto b, auto f, const char*) -> int {
+    if (TaskCols::is_id(b)) return EVG_OK;
+    TaskCols::point(d.*f, at);
+    CK(cudaMemcpyAsync(at, v->*f, TaskCols::elem(f) * n, cudaMemcpyHostToDevice, s));
+    at += TaskCols::elem(f) * n;
+    return EVG_OK;
+  });
+  if (rc != EVG_OK) return rc;
+  int* bad = reinterpret_cast<int*>(at);
   CK(cudaMemsetAsync(bad, 0, sizeof(int), s));
-  k_update_rows<<<grid_for(n_rows, 256), 256, 0, s>>>(n_rows, d_rows, c->T, c->tasks.prio.as<int32_t>(), c->tasks.nd.as<int32_t>(), c->tasks.tgo.as<int32_t>(),
-                                                      c->tasks.flags.as<uint32_t>(), c->tasks.exp.as<int64_t>(), c->tasks.qb.as<int64_t>(), c->tasks.wb.as<int64_t>(),
-                                                      d_prio, d_nd, d_tgo, d_fl, d_exp, d_qb, d_wb, bad);
+  const EdDst o = c->tasks.dst();
+  launch(c, s, k_update_rows, grid_for(n_rows, 256), 256, 0, n_rows, d_rows, c->T, o.priority, o.numdep, o.tgo, o.flags, o.expected,
+         o.qbasis, o.wbasis, d.priority, d.num_dependents, d.task_group_order, d.flags, d.expected_ns, d.queue_basis_ns, d.wait_basis_ns, bad);
   CK(cudaGetLastError());
   int h_bad = 0;
   CK(cudaMemcpyAsync(&h_bad, bad, sizeof(int), cudaMemcpyDeviceToHost, s));
@@ -2067,10 +2120,8 @@ int evg_update_tasks(evg_ctx* c, int64_t n_rows, const int64_t* rows, const evg_
 
 int evg_upload_device(evg_ctx* c, const evg_task_soa* tasks, const evg_distro_table* distros, const evg_host_soa* hosts,
                       const int64_t* host_off, const evg_alloc_cfg* acfg) {
-  if (!c) return fail(EVG_ERR_INVALID, "null context");
-  LOCK(c);
+  ENTER(c, "evg_upload_device");
   if (!tasks || !distros) return fail(EVG_ERR_INVALID, "null task table / distro table");
-  CK(cudaSetDevice(c->device));
   std::vector<int64_t> edge_off;
   const int32_t D = distros->n_distros;
   if (tasks->n_edges > 0 && D > 0) {  // dep_off is device memory: sample it at the distro boundaries for the routing
@@ -2079,19 +2130,17 @@ int evg_upload_device(evg_ctx* c, const evg_task_soa* tasks, const evg_distro_ta
     CK(c->b_rn0.ensure(sizeof(int64_t) * size_t(D + 1)));
     CK(c->b_rn1.ensure(sizeof(int64_t) * size_t(D + 1)));
     CK(cudaMemcpyAsync(c->b_rn0.p, distros->task_off, sizeof(int64_t) * size_t(D + 1), cudaMemcpyHostToDevice, c->stream));
-    k_gather_i64<<<grid_for(D + 1, 256), 256, 0, c->stream>>>(tasks->dep_off, c->b_rn0.as<int64_t>(), c->b_rn1.as<int64_t>(), D + 1);
+    launch(c, c->stream, k_gather_i64, grid_for(D + 1, 256), 256, 0, tasks->dep_off, c->b_rn0.as<int64_t>(), c->b_rn1.as<int64_t>(), D + 1);
     CK(cudaMemcpyAsync(edge_off.data(), c->b_rn1.p, sizeof(int64_t) * size_t(D + 1), cudaMemcpyDeviceToHost, c->stream));
     CK(cudaStreamSynchronize(c->stream));
   }
-  return upload(c, "evg_upload_device", tasks, distros, hosts, host_off, acfg, Tick::kBorrowed, Cols::kAdopt,
+  return upload(c, who, tasks, distros, hosts, host_off, acfg, Tick::kBorrowed, Cols::kAdopt,
                 edge_off.empty() ? nullptr : edge_off.data());
 }
 
 int evg_run_resident(evg_ctx* c, int64_t now_ns, uint32_t opts) {
-  if (!c) return fail(EVG_ERR_INVALID, "null context");
-  LOCK(c);
-  if (const int rc = need_tick(c, "evg_run_resident", Need::kTick); rc != EVG_OK) return rc;
-  CK(cudaSetDevice(c->device));
+  ENTER(c, "evg_run_resident");
+  if (const int rc = need_tick(c, who, Need::kTick); rc != EVG_OK) return rc;
   c->launches = 0;
   c->timed = true;
   c->general_timed = false;
@@ -2109,10 +2158,8 @@ int evg_run_resident(evg_ctx* c, int64_t now_ns, uint32_t opts) {
 }
 
 int evg_download(evg_ctx* c, evg_plan_out* po, evg_alloc_out* ao) {
-  if (!c) return fail(EVG_ERR_INVALID, "null context");
-  LOCK(c);
-  if (const int rc = need_tick(c, "evg_download", Need::kTick); rc != EVG_OK) return rc;
-  CK(cudaSetDevice(c->device));
+  ENTER(c, "evg_download");
+  if (const int rc = need_tick(c, who, Need::kTick); rc != EVG_OK) return rc;
   cudaStream_t s = c->stream;
   if (po) {
     if (po->order && c->T) CK(cudaMemcpyAsync(po->order, c->b_order.p, sizeof(int32_t) * size_t(c->T), cudaMemcpyDeviceToHost, s));
@@ -2125,7 +2172,7 @@ int evg_download(evg_ctx* c, evg_plan_out* po, evg_alloc_out* ao) {
     if (po->group_info && c->G) CK(cudaMemcpyAsync(po->group_info, c->b_ginfo.p, sizeof(evg_group_info) * size_t(c->G), cudaMemcpyDeviceToHost, s));
   }
   if (ao) {
-    if (const int rc = need_tick(c, "evg_download", Need::kHosts); rc != EVG_OK) return rc;
+    if (const int rc = need_tick(c, who, Need::kHosts); rc != EVG_OK) return rc;
     if (ao->result && c->Dn) CK(cudaMemcpyAsync(ao->result, c->result_ptr(), sizeof(evg_alloc_result) * size_t(c->Dn), cudaMemcpyDeviceToHost, s));
     if (ao->status && c->Dn) CK(cudaMemcpyAsync(ao->status, c->b_status.p, sizeof(int32_t) * size_t(c->Dn), cudaMemcpyDeviceToHost, s));
   }
@@ -2157,9 +2204,8 @@ __global__ void __launch_bounds__(256) k_project_queue(DTasks T, DDistros D, con
 }
 
 int evg_download_queue(evg_ctx* c, int32_t cap, int64_t* item_off, evg_queue_item* items, int64_t items_capacity) {
-  if (!c) return fail(EVG_ERR_INVALID, "null context");
-  LOCK(c);
-  if (const int rc = need_tick(c, "evg_download_queue", Need::kTick); rc != EVG_OK) return rc;
+  ENTER(c, "evg_download_queue");
+  if (const int rc = need_tick(c, who, Need::kTick); rc != EVG_OK) return rc;
   if (cap < 0 || !item_off) return fail(EVG_ERR_INVALID, "evg_download_queue: bad argument");
   if (cap == 0) cap = EVG_PERSISTED_QUEUE_CAP;
   const int32_t D = c->Dn;
@@ -2168,35 +2214,40 @@ int evg_download_queue(evg_ctx* c, int32_t cap, int64_t* item_off, evg_queue_ite
   const int64_t n = item_off[D];
   if (n > items_capacity || (n > 0 && !items)) return fail(EVG_ERR_INVALID, "evg_download_queue: %lld rows needed, %lld available", (long long)n, (long long)items_capacity);
   if (n == 0) return EVG_OK;
-  CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   CK(c->b_rn0.ensure(sizeof(int64_t) * size_t(D + 1)));
   CK(c->b_rn1.ensure(sizeof(evg_queue_item) * size_t(n)));
   CK(cudaMemcpyAsync(c->b_rn0.p, item_off, sizeof(int64_t) * size_t(D + 1), cudaMemcpyHostToDevice, s));
-  k_project_queue<<<grid_for(n, 256), 256, 0, s>>>(dtasks(c), ddistros(c), c->b_rn0.as<int64_t>(), n, c->b_order.as<int32_t>(),
-                                                 c->b_tv.as<int64_t>(), c->b_rn1.as<evg_queue_item>());
+  launch(c, s, k_project_queue, grid_for(n, 256), 256, 0, dtasks(c), ddistros(c), c->b_rn0.as<int64_t>(), n, c->b_order.as<int32_t>(),
+         c->b_tv.as<int64_t>(), c->b_rn1.as<evg_queue_item>());
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(items, c->b_rn1.p, sizeof(evg_queue_item) * size_t(n), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   return EVG_OK;
 }
 
-void* evg_device_result_ptr(evg_ctx* c) { return c ? (void*)c->result_ptr() : nullptr; }
+// The two queries that return no status take the lock and leave the device alone.
+void* evg_device_result_ptr(evg_ctx* c) {
+  if (!c) return nullptr;
+  std::lock_guard<std::recursive_mutex> lock_(c->mu);
+  return c->result_ptr();
+}
+int64_t evg_last_launch_count(evg_ctx* c) {
+  if (!c) return 0;
+  std::lock_guard<std::recursive_mutex> lock_(c->mu);
+  return c->launches;
+}
 int evg_bind_result_buffer(evg_ctx* c, void* device_ptr, int64_t capacity) {
-  if (!c) return fail(EVG_ERR_INVALID, "null context");
-  LOCK(c);
+  ENTER(c, "evg_bind_result_buffer");
   if (device_ptr && capacity < 0) return fail(EVG_ERR_INVALID, "negative capacity");
   c->ext_result = reinterpret_cast<evg_alloc_result*>(device_ptr);
   c->ext_capacity = device_ptr ? capacity : 0;
   c->tick.allocated = false;  // the last run's result rows are not in the buffer bound now
   return EVG_OK;
 }
-int64_t evg_last_launch_count(evg_ctx* c) { return c ? c->launches : 0; }
-
 int evg_last_timing_ms(evg_ctx* c, float* total_ms, float* sort_ms) {
-  if (!c || !c->timed) return fail(EVG_ERR_STATE, "no timed run");
-  LOCK(c);
-  CK(cudaSetDevice(c->device));
+  ENTER(c, "evg_last_timing_ms");
+  if (!c->timed) return fail(EVG_ERR_STATE, "no timed run");
   CK(cudaEventSynchronize(c->ev_end));
   if (total_ms) CK(cudaEventElapsedTime(total_ms, c->ev_begin, c->ev_end));
   if (sort_ms) {
@@ -2208,10 +2259,8 @@ int evg_last_timing_ms(evg_ctx* c, float* total_ms, float* sort_ms) {
 }
 
 int evg_general_timing_ms(evg_ctx* c, float* task_pass_ms, float* sort_ms) {
-  if (!c) return fail(EVG_ERR_INVALID, "null context");
-  LOCK(c);
+  ENTER(c, "evg_general_timing_ms");
   if (!c->timed || !c->general_timed) return fail(EVG_ERR_STATE, "the last timed run had no general-path distro");
-  CK(cudaSetDevice(c->device));
   CK(cudaEventSynchronize(c->ev_end));
   if (task_pass_ms) CK(cudaEventElapsedTime(task_pass_ms, c->ev_gt0, c->ev_gt1));
   if (sort_ms) CK(cudaEventElapsedTime(sort_ms, c->ev_sort0, c->ev_sort1));
@@ -2219,10 +2268,9 @@ int evg_general_timing_ms(evg_ctx* c, float* task_pass_ms, float* sort_ms) {
 }
 
 int evg_kernel_timing_ms(evg_ctx* c, float* out_ms, int32_t n) {
-  if (!c || !out_ms || n < 0) return fail(EVG_ERR_INVALID, "evg_kernel_timing_ms: bad argument");
-  LOCK(c);
+  ENTER(c, "evg_kernel_timing_ms");
+  if (!out_ms || n < 0) return fail(EVG_ERR_INVALID, "%s: bad argument", who);
   if (n > evg_ctx::kRing || n > c->runs) return fail(EVG_ERR_STATE, "only %lld timed runs recorded (ring of %d)", (long long)c->runs, evg_ctx::kRing);
-  CK(cudaSetDevice(c->device));
   for (int32_t k = 0; k < n; k++) {
     const int slot = int((c->runs - n + k) % evg_ctx::kRing);
     CK(cudaEventSynchronize(c->ring1[slot]));
@@ -2233,9 +2281,8 @@ int evg_kernel_timing_ms(evg_ctx* c, float* out_ms, int32_t n) {
 
 int evg_plan_batch(evg_ctx* c, const evg_task_soa* tasks, const evg_distro_table* distros, int64_t now_ns, uint32_t opts,
                    evg_plan_out* out) {
-  if (!c) return fail(EVG_ERR_INVALID, "null context");
-  LOCK(c);
-  int rc = upload(c, "evg_plan_batch", tasks, distros, nullptr, nullptr, nullptr, Tick::kFixed);
+  ENTER(c, "evg_plan_batch");
+  int rc = upload(c, who, tasks, distros, nullptr, nullptr, nullptr, Tick::kFixed);
   if (rc != EVG_OK) return rc;
   rc = evg_run_resident(c, now_ns, opts);
   if (rc != EVG_OK) return rc;
@@ -2296,15 +2343,7 @@ static int plan_and_alloc_pipelined(evg_ctx* c, const evg_task_soa* t, const evg
     if (d1 <= d0) continue;
     const int64_t t0 = c->h_taskoff[d0], n = c->h_taskoff[d1] - t0;
     const int64_t g0 = c->h_groupoff[d0], ng = c->h_groupoff[d1] - g0;
-    H2D(c->tasks.prio, t->priority, t0, n, int32_t);
-    H2D(c->tasks.exp, t->expected_ns, t0, n, int64_t);
-    H2D(c->tasks.qb, t->queue_basis_ns, t0, n, int64_t);
-    H2D(c->tasks.wb, t->wait_basis_ns, t0, n, int64_t);
-    H2D(c->tasks.nd, t->num_dependents, t0, n, int32_t);
-    H2D(c->tasks.tgo, t->task_group_order, t0, n, int32_t);
-    H2D(c->tasks.gid, t->group_id, t0, n, int32_t);
-    H2D(c->tasks.vid, t->version_id, t0, n, int32_t);
-    H2D(c->tasks.flags, t->flags, t0, n, uint32_t);
+    if ((rc = c->tasks.copy_rows(t, t0, n, c->s_h2d)) != EVG_OK) return rc;
     if (E > 0) {
       const int64_t e0 = t->dep_off[t0], ne = t->dep_off[t0 + n] - e0;
       H2D(c->b_depoff, t->dep_off, t0, n + 1, int64_t);
@@ -2312,7 +2351,7 @@ static int plan_and_alloc_pipelined(evg_ctx* c, const evg_task_soa* t, const evg
     }
     CK(cudaEventRecord(c->ev_h[k], c->s_h2d));
     CK(cudaStreamWaitEvent(s, c->ev_h[k], 0));
-    k_validate<<<grid_for(n, 256), 256, 0, s>>>(dtk, dd, w, t0, t0 + n);
+    launch(c, s, k_validate, grid_for(n, 256), 256, 0, dtk, dd, w, t0, t0 + n);
     // the chunk's distros of each class; what k_plan_cta hands back is replanned by k_plan_smem right behind it, and the
     // general path runs restricted to the chunk's tiles
     int32_t* pl = c->b_punt.as<int32_t>() + d0;  // a chunk hands back at most its own d1 - d0 distros
@@ -2352,18 +2391,17 @@ static int plan_and_alloc_pipelined(evg_ctx* c, const evg_task_soa* t, const evg
 int evg_plan_and_alloc_batch(evg_ctx* c, const evg_task_soa* tasks, const evg_distro_table* distros,
                              const evg_host_soa* hosts, const int64_t* host_off, const evg_alloc_cfg* acfg, int64_t now_ns,
                              uint32_t opts, evg_plan_out* plan_out, evg_alloc_out* alloc_out) {
-  if (!c) return fail(EVG_ERR_INVALID, "null context");
-  LOCK(c);
+  ENTER(c, "evg_plan_and_alloc_batch");
   if (!hosts || (!acfg && distros && distros->n_distros > 0)) return fail(EVG_ERR_INVALID, "evg_plan_and_alloc_batch needs hosts and allocator config");
   if (!(opts & EVG_OPT_BREAKDOWN) && tasks && distros && tasks->n_tasks >= (int64_t(1) << 21)) {
     // large tick: stage the small tables, then pipeline the columns chunk by chunk
-    const int rc0 = upload(c, "evg_plan_and_alloc_batch", tasks, distros, hosts, host_off, acfg, Tick::kFixed, Cols::kChunked);
+    const int rc0 = upload(c, who, tasks, distros, hosts, host_off, acfg, Tick::kFixed, Cols::kChunked);
     if (rc0 != EVG_OK) return rc0;
     const int rc1 = plan_and_alloc_pipelined(c, tasks, distros, hosts, host_off, acfg, now_ns, plan_out, alloc_out);
     c->tick.allocated = rc1 == EVG_OK;
     return rc1;
   }
-  int rc = upload(c, "evg_plan_and_alloc_batch", tasks, distros, hosts, host_off, acfg, Tick::kFixed);
+  int rc = upload(c, who, tasks, distros, hosts, host_off, acfg, Tick::kFixed);
   if (rc != EVG_OK) return rc;
   rc = evg_run_resident(c, now_ns, opts);
   if (rc != EVG_OK) return rc;
@@ -2373,16 +2411,14 @@ int evg_plan_and_alloc_batch(evg_ctx* c, const evg_task_soa* tasks, const evg_di
 int evg_alloc_batch(evg_ctx* c, const evg_host_soa* hosts, const int64_t* host_off, const evg_alloc_cfg* cfg,
                     const evg_queue_info* info, evg_group_info* groups, const int64_t* group_off, int32_t n_distros,
                     int64_t now_ns, evg_alloc_out* out) {
-  if (!c) return fail(EVG_ERR_INVALID, "null context");
-  LOCK(c);
+  ENTER(c, "evg_alloc_batch");
   if (n_distros < 0 || (n_distros > 0 && (!info || !group_off || !out))) return fail(EVG_ERR_INVALID, "evg_alloc_batch: null argument");
-  CK(cudaSetDevice(c->device));
-  int rc = n_distros > 0 ? check_offsets(group_off, n_distros, -1, "evg_alloc_batch", "group_off") : EVG_OK;
+  int rc = n_distros > 0 ? check_offsets(group_off, n_distros, -1, who, "group_off") : EVG_OK;
   if (rc != EVG_OK) return rc;
   const int64_t G = n_distros > 0 ? group_off[n_distros] : 0;
   if (G > 0 && !groups) return fail(EVG_ERR_INVALID, "evg_alloc_batch: groups is null");
   drop_tick(c);  // before upload_hosts, which must not list distros from the tick's tables
-  rc = upload_hosts(c, "evg_alloc_batch", hosts, host_off, cfg, n_distros);
+  rc = upload_hosts(c, who, hosts, host_off, cfg, n_distros);
   if (rc != EVG_OK) return rc;
   cudaStream_t s = c->stream;
   CK(c->b_groupoff.ensure(sizeof(int64_t) * size_t(n_distros + 1)));
@@ -2449,8 +2485,7 @@ static int deps_to_device(evg_ctx* c, const char* who, const evg_deps_in* in, in
       fin = x.fin.as<int64_t>();
     }
   }
-  k_deps_met<<<grid_for(T, 256), 256, 0, s>>>(ddeps(c, in), x.met.as<uint8_t>(), c->b_err.as<int>(), both, fin, now, stamp);
-  c->launches++;
+  launch(c, s, k_deps_met, grid_for(T, 256), 256, 0, ddeps(c, in), x.met.as<uint8_t>(), c->b_err.as<int>(), both, fin, now, stamp);
   CK(cudaGetLastError());
   return EVG_OK;
 }
@@ -2463,58 +2498,53 @@ static int deps_bad(const char* who, int bad) {
 }
 
 int evg_deps_met_batch(evg_ctx* c, const evg_deps_in* in, uint8_t* met) {
-  if (!c || !in || (in->n_tasks > 0 && !met)) return fail(EVG_ERR_INVALID, "evg_deps_met_batch: null argument");
-  LOCK(c);
+  ENTER(c, "evg_deps_met_batch");
+  if (!in || (in->n_tasks > 0 && !met)) return fail(EVG_ERR_INVALID, "evg_deps_met_batch: null argument");
   if (in->n_tasks == 0) return EVG_OK;
-  CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   CK(c->b_err.ensure(sizeof(int) * 4));
   CK(cudaMemsetAsync(c->b_err.p, 0, sizeof(int) * 4, s));
   c->launches = 0;
   c->tick.deps = false;  // deps_to_device overwrites the resident tick's verdicts and stamps
-  int rc = deps_to_device(c, "evg_deps_met_batch", in, 0);
+  int rc = deps_to_device(c, who, in, 0);
   if (rc != EVG_OK) return rc;
   int bad = 0;
   CK(cudaMemcpyAsync(met, c->deps.met.p, size_t(in->n_tasks), cudaMemcpyDeviceToHost, s));
   CK(cudaMemcpyAsync(&bad, c->b_err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
-  if (bad) return deps_bad("evg_deps_met_batch", bad);
+  if (bad) return deps_bad(who, bad);
   return EVG_OK;
 }
 
 int evg_upload_with_deps(evg_ctx* c, const evg_task_soa* tasks, const evg_distro_table* distros, const evg_host_soa* hosts,
                          const int64_t* host_off, const evg_alloc_cfg* acfg, const evg_deps_in* deps, const int64_t* dep_finished_ns,
                          int64_t now_ns) {
-  if (!c) return fail(EVG_ERR_INVALID, "null context");
-  LOCK(c);
+  ENTER(c, "evg_upload_with_deps");
   if (!tasks || !deps) return fail(EVG_ERR_INVALID, "evg_upload_with_deps: null argument");
   if (deps->n_tasks != tasks->n_tasks) return fail(EVG_ERR_INVALID, "deps covers %lld tasks, the task table %lld", (long long)deps->n_tasks, (long long)tasks->n_tasks);
-  int rc = upload(c, "evg_upload_with_deps", tasks, distros, hosts, host_off, acfg, Tick::kOwn);
+  int rc = upload(c, who, tasks, distros, hosts, host_off, acfg, Tick::kOwn);
   if (rc != EVG_OK) return rc;
   const int64_t T = tasks->n_tasks;
   if (T == 0) return EVG_OK;
   cudaStream_t s = c->stream;
-  rc = deps_to_device(c, "evg_upload_with_deps", deps, 0, dep_finished_ns, now_ns, /*want_stamp=*/true);
+  rc = deps_to_device(c, who, deps, 0, dep_finished_ns, now_ns, /*want_stamp=*/true);
   if (rc != EVG_OK) { drop_tick(c); return rc; }
-  k_apply_deps<<<grid_for(T, 256), 256, 0, s>>>(T, c->deps.met.as<uint8_t>(), c->deps.stamp.as<int64_t>(), c->tasks.flags.as<uint32_t>(),
-                                                c->tasks.wb.as<int64_t>());
-  c->launches++;
+  launch(c, s, k_apply_deps, grid_for(T, 256), 256, 0, T, c->deps.met.as<uint8_t>(), c->deps.stamp.as<int64_t>(), c->tasks.flags.as<uint32_t>(),
+         c->tasks.wb.as<int64_t>());
   int bad = 0;
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(&bad, c->b_err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
-  if (bad) { drop_tick(c); return deps_bad("evg_upload_with_deps", bad); }
+  if (bad) { drop_tick(c); return deps_bad(who, bad); }
   c->tick.deps = true;
   return EVG_OK;
 }
 
 int evg_download_deps(evg_ctx* c, uint8_t* met, int64_t* met_time_ns) {
-  if (!c) return fail(EVG_ERR_INVALID, "null context");
-  LOCK(c);
-  if (const int rc = need_tick(c, "evg_download_deps", Need::kTick); rc != EVG_OK) return rc;
-  CK(cudaSetDevice(c->device));
+  ENTER(c, "evg_download_deps");
+  if (const int rc = need_tick(c, who, Need::kTick); rc != EVG_OK) return rc;
   if (c->T == 0) return EVG_OK;
-  if (const int rc = need_tick(c, "evg_download_deps", Need::kVerdicts); rc != EVG_OK) return rc;
+  if (const int rc = need_tick(c, who, Need::kVerdicts); rc != EVG_OK) return rc;
   if (met) CK(cudaMemcpyAsync(met, c->deps.met.p, size_t(c->T), cudaMemcpyDeviceToHost, c->stream));
   if (met_time_ns) CK(cudaMemcpyAsync(met_time_ns, c->deps.stamp.p, sizeof(int64_t) * size_t(c->T), cudaMemcpyDeviceToHost, c->stream));
   CK(cudaStreamSynchronize(c->stream));
@@ -2522,15 +2552,14 @@ int evg_download_deps(evg_ctx* c, uint8_t* met, int64_t* met_time_ns) {
 }
 
 int evg_expected_durations_batch(evg_ctx* c, const evg_duration_rows* in, evg_duration_stat* out) {
-  if (!c || !in) return fail(EVG_ERR_INVALID, "evg_expected_durations_batch: null argument");
-  LOCK(c);
+  ENTER(c, "evg_expected_durations_batch");
+  if (!in) return fail(EVG_ERR_INVALID, "evg_expected_durations_batch: null argument");
   const int64_t R = in->n_rows;
   const int32_t K = in->n_keys;
   if (R < 0 || K < 0) return fail(EVG_ERR_INVALID, "negative sizes");
   if (K == 0) return R == 0 ? EVG_OK : fail(EVG_ERR_INVALID, "rows without keys");
   if (!out) return fail(EVG_ERR_INVALID, "null output");
   if (R > 0 && (!in->key || !in->time_taken_ns || !in->start_ns || !in->finish_ns || !in->flags)) return fail(EVG_ERR_INVALID, "null row column");
-  CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   c->launches = 0;
   drop_tick(c);
@@ -2548,13 +2577,9 @@ int evg_expected_durations_batch(evg_ctx* c, const evg_duration_rows* in, evg_du
   x.n_rows = R; x.n_keys = K; x.key = c->b_rn0.as<int32_t>(); x.taken = c->b_rn1.as<int64_t>(); x.start = c->b_rn2.as<int64_t>();
   x.finish = c->b_rn3.as<int64_t>(); x.flags = c->b_rn4.as<uint8_t>(); x.w0 = in->window_start_ns; x.w1 = in->window_end_ns;
   x.cnt = c->b_rn5.as<unsigned long long>(); x.sum = x.cnt + K; x.sq_lo = x.sum + K; x.sq_hi = x.sq_lo + K;
-  if (R > 0) {
-    k_dur_sum<<<grid_for(R, 256), 256, 0, s>>>(x, c->b_err.as<int>());
-    k_dur_dev<<<grid_for(R, 256), 256, 0, s>>>(x);
-    c->launches += 2;
-  }
-  k_dur_final<<<grid_for(K, 256), 256, 0, s>>>(x, c->b_rn6.as<evg_duration_stat>());
-  c->launches++;
+  launch(c, s, k_dur_sum, grid_for(R, 256), 256, 0, x, c->b_err.as<int>());
+  launch(c, s, k_dur_dev, grid_for(R, 256), 256, 0, x);
+  launch(c, s, k_dur_final, grid_for(K, 256), 256, 0, x, c->b_rn6.as<evg_duration_stat>());
   CK(cudaGetLastError());
   int bad = 0;
   CK(cudaMemcpyAsync(out, c->b_rn6.p, sizeof(evg_duration_stat) * size_t(K), cudaMemcpyDeviceToHost, s));
@@ -2584,12 +2609,11 @@ static int check_duration_cache(const evg_duration_cache* dc, int64_t n, const c
 }
 
 int evg_resolve_durations(evg_ctx* c, const evg_duration_in* in, int64_t now_ns) {
-  if (!c) return fail(EVG_ERR_INVALID, "null context");
-  LOCK(c);
+  ENTER(c, "evg_resolve_durations");
   if (!in) return fail(EVG_ERR_INVALID, "evg_resolve_durations: null argument");
   int rc;
-  if ((rc = need_tick(c, "evg_resolve_durations", Need::kEditable)) != EVG_OK) return rc;
-  if (in->hosts && (rc = need_tick(c, "evg_resolve_durations", Need::kHosts)) != EVG_OK) return rc;
+  if ((rc = need_tick(c, who, Need::kEditable)) != EVG_OK) return rc;
+  if (in->hosts && (rc = need_tick(c, who, Need::kHosts)) != EVG_OK) return rc;
   const evg_duration_rows* h = in->history;
   const int64_t R = h ? h->n_rows : 0;
   const int32_t K = h ? h->n_keys : 0, P = in->n_pairs;
@@ -2597,10 +2621,9 @@ int evg_resolve_durations(evg_ctx* c, const evg_duration_in* in, int64_t now_ns)
   if (R > 0 && (!h->key || !h->time_taken_ns || !h->start_ns || !h->finish_ns || !h->flags))
     return fail(EVG_ERR_INVALID, "evg_resolve_durations: null history column");
   if (P > 0 && !in->pair_key_off) return fail(EVG_ERR_INVALID, "evg_resolve_durations: null pair_key_off");
-  if (in->pair_key_off && (rc = check_offsets(in->pair_key_off, P, K, "evg_resolve_durations", "pair_key_off")) != EVG_OK) return rc;
+  if (in->pair_key_off && (rc = check_offsets(in->pair_key_off, P, K, who, "pair_key_off")) != EVG_OK) return rc;
   if (in->tasks && (rc = check_duration_cache(in->tasks, c->T, "tasks")) != EVG_OK) return rc;
   if (in->hosts && (rc = check_duration_cache(in->hosts, c->H, "hosts")) != EVG_OK) return rc;
-  CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   auto& d = c->dur;
   c->tick.durations = false;  // the staging below is overwritten whatever the outcome
@@ -2649,17 +2672,13 @@ int evg_resolve_durations(evg_ctx* c, const evg_duration_in* in, int64_t now_ns)
   x.finish = d.finish.as<int64_t>(); x.flags = d.flags.as<uint8_t>();
   x.w0 = h ? h->window_start_ns : 0; x.w1 = h ? h->window_end_ns : 0;
   x.cnt = d.acc.as<unsigned long long>(); x.sum = x.cnt + K; x.sq_lo = x.sum + K; x.sq_hi = x.sq_lo + K;
-  if (R > 0) {
-    k_dur_sum<<<grid_for(R, 256), 256, 0, s>>>(x, d.err.as<int>());
-    k_dur_dev<<<grid_for(R, 256), 256, 0, s>>>(x);
-  }
-  if (K > 0) k_dur_final<<<grid_for(K, 256), 256, 0, s>>>(x, d.stat.as<evg_duration_stat>());
-  if (P > 0) k_dur_pair<<<grid_for(P, 256), 256, 0, s>>>(P, d.pair_off.as<int64_t>(), x.cnt, d.single.as<int32_t>());
-  if (N > 0) {
-    k_dur_resolve<<<grid_for(N, 256), 256, 0, s>>>(X, K, P, d.stat.as<evg_duration_stat>(), d.single.as<int32_t>(), now_ns, d.err.as<int>());
-    k_dur_commit<<<grid_for(N, 256), 256, 0, s>>>(X, d.err.as<int>(), c->tasks.exp.as<int64_t>(), c->b_hexp.as<int64_t>(),
-                                                   c->b_hstd.as<int64_t>());
-  }
+  launch(c, s, k_dur_sum, grid_for(R, 256), 256, 0, x, d.err.as<int>());
+  launch(c, s, k_dur_dev, grid_for(R, 256), 256, 0, x);
+  launch(c, s, k_dur_final, grid_for(K, 256), 256, 0, x, d.stat.as<evg_duration_stat>());
+  launch(c, s, k_dur_pair, grid_for(P, 256), 256, 0, P, d.pair_off.as<int64_t>(), x.cnt, d.single.as<int32_t>());
+  launch(c, s, k_dur_resolve, grid_for(N, 256), 256, 0, X, K, P, d.stat.as<evg_duration_stat>(), d.single.as<int32_t>(), now_ns, d.err.as<int>());
+  launch(c, s, k_dur_commit, grid_for(N, 256), 256, 0, X, d.err.as<int>(), c->tasks.exp.as<int64_t>(), c->b_hexp.as<int64_t>(),
+         c->b_hstd.as<int64_t>());
   CK(cudaGetLastError());
   int bad = 0;
   CK(cudaMemcpyAsync(&bad, d.err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
@@ -2672,10 +2691,8 @@ int evg_resolve_durations(evg_ctx* c, const evg_duration_in* in, int64_t now_ns)
 }
 
 int evg_download_durations(evg_ctx* c, evg_duration_out* tasks, evg_duration_out* hosts) {
-  if (!c) return fail(EVG_ERR_INVALID, "null context");
-  LOCK(c);
-  if (const int rc = need_tick(c, "evg_download_durations", Need::kDurations); rc != EVG_OK) return rc;
-  CK(cudaSetDevice(c->device));
+  ENTER(c, "evg_download_durations");
+  if (const int rc = need_tick(c, who, Need::kDurations); rc != EVG_OK) return rc;
   cudaStream_t s = c->stream;
   auto& d = c->dur;
   const int64_t N = d.n_t + d.n_h;
@@ -2728,7 +2745,6 @@ static int stage_finder(evg_ctx* c, const char* who, const evg_runnable_in* in, 
         (x->n_ext > 0 && (!pipe->ext_status || !pipe->ext_unattainable)))
       return fail(EVG_ERR_INVALID, "evg_pipeline_in: null status column");
   }
-  CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   auto& pf = c->pf;
   UP(s, pf.task_off, in->task_off, D + 1, int64_t);
@@ -2765,17 +2781,15 @@ static int pipeline_deps(evg_ctx* c, const evg_deps_in* x, const evg_pipeline_in
   DPipe dp;
   dp.n_status = pipe->n_status; dp.dep_status = p.dep_status.as<int32_t>(); dp.task_status = p.task_status.as<int32_t>();
   dp.ext_status = p.ext_status.as<int32_t>(); dp.task_unatt = p.task_unatt.as<uint8_t>(); dp.ext_unatt = p.ext_unatt.as<uint8_t>();
-  k_pl_deps<<<grid_for(T, 256), 256, 0, s>>>(ddeps(c, x), dp, c->deps.met.as<uint8_t>(), c->b_err.as<int>());
-  c->launches++;
+  launch(c, s, k_pl_deps, grid_for(T, 256), 256, 0, ddeps(c, x), dp, c->deps.met.as<uint8_t>(), c->b_err.as<int>());
   CK(cudaGetLastError());
   return EVG_OK;
 }
 
-// evg_find_runnable_batch and evg_find_runnable_ex (pipe == NULL: the former)
-static int find_runnable(evg_ctx* c, const evg_runnable_in* in, const evg_pipeline_in* pipe, int32_t* runnable, int64_t* count) {
-  if (!c || !in) return fail(EVG_ERR_INVALID, "evg_find_runnable_batch: null argument");
-  LOCK(c);
-  const char* who = pipe ? "evg_find_runnable_ex" : "evg_find_runnable_batch";
+// evg_find_runnable_batch and evg_find_runnable_ex (`name`; the former passes no pipe)
+static int find_runnable(const char* name, evg_ctx* c, const evg_runnable_in* in, const evg_pipeline_in* pipe, int32_t* runnable, int64_t* count) {
+  ENTER(c, name);
+  if (!in) return fail(EVG_ERR_INVALID, "%s: null argument", who);
   const int64_t T = in->n_tasks;
   const int32_t D = in->n_distros, P = in->n_projects;
   if (T < 0 || D < 0 || P < 0) return fail(EVG_ERR_INVALID, "negative sizes");
@@ -2801,11 +2815,10 @@ static int find_runnable(evg_ctx* c, const evg_runnable_in* in, const evg_pipeli
     r.met = c->deps.met.as<uint8_t>();
   }
   if (any_pipe)
-    k_runnable_pipe<<<unsigned(D), 256, 0, s>>>(r, c->pl.project_raw.as<uint8_t>(), c->pf.kept.as<int32_t>(), c->pf.count.as<int64_t>(),
-                                                c->b_err.as<int>());
+    launch(c, s, k_runnable_pipe, unsigned(D), 256, 0, r, c->pl.project_raw.as<uint8_t>(), c->pf.kept.as<int32_t>(), c->pf.count.as<int64_t>(),
+           c->b_err.as<int>());
   else
-    k_runnable<<<unsigned(D), 256, 0, s>>>(r, c->pf.kept.as<int32_t>(), c->pf.count.as<int64_t>(), c->b_err.as<int>());
-  c->launches++;
+    launch(c, s, k_runnable, unsigned(D), 256, 0, r, c->pf.kept.as<int32_t>(), c->pf.count.as<int64_t>(), c->b_err.as<int>());
   CK(cudaGetLastError());
   int bad = 0;
   if (T > 0) CK(cudaMemcpyAsync(runnable, c->pf.kept.p, sizeof(int32_t) * size_t(T), cudaMemcpyDeviceToHost, s));
@@ -2816,10 +2829,10 @@ static int find_runnable(evg_ctx* c, const evg_runnable_in* in, const evg_pipeli
   return EVG_OK;
 }
 int evg_find_runnable_batch(evg_ctx* c, const evg_runnable_in* in, int32_t* runnable, int64_t* count) {
-  return find_runnable(c, in, nullptr, runnable, count);
+  return find_runnable("evg_find_runnable_batch", c, in, nullptr, runnable, count);
 }
 int evg_find_runnable_ex(evg_ctx* c, const evg_runnable_in* in, const evg_pipeline_in* pipe, int32_t* runnable, int64_t* count) {
-  return find_runnable(c, in, pipe, runnable, count);
+  return find_runnable("evg_find_runnable_ex", c, in, pipe, runnable, count);
 }
 
 // --------------------------------------------------------------------------
@@ -2884,11 +2897,6 @@ __global__ void __launch_bounds__(1024) k_scan_add(int64_t* __restrict__ out, in
   if (i < n) out[i] += block_sum[blockIdx.x];
   if (i == 0) out[n] = block_sum[nb];
 }
-struct EdDst {  // the shadow column set the composed table is written to
-  int32_t *priority, *numdep, *tgo, *gid, *vid;
-  uint32_t* flags;
-  int64_t *expected, *qbasis, *wbasis;
-};
 // Where row i of the composed table comes from.  Distro d's composed rows are its survivors in their source order
 // (S_d of them), then its inserted rows ins_off[d] .. ins_off[d+1].  The source is the resident table (an edit) or the
 // candidates (the finder).
@@ -3020,29 +3028,9 @@ __global__ void __launch_bounds__(256) k_kept_mask(int64_t n, int32_t D, const i
 // Exclusive scan of n int32 counts into out[0 .. n] (int64; out[n] = the total); `sum` holds (n + 1023) / 1024 + 1 int64.
 static void scan_counts(evg_ctx* c, const int32_t* in, int64_t n, int64_t* out, int64_t* sum) {
   const int64_t nb = (n + 1023) / 1024;
-  k_scan_blocks<<<unsigned(nb), 1024, 0, c->stream>>>(in, n, out, sum);
-  k_scan_sums<<<1, 1024, 0, c->stream>>>(sum, nb);
-  k_scan_add<<<unsigned(nb), 1024, 0, c->stream>>>(out, n, sum, nb);
-  c->launches += 3;
-}
-
-// The shadow column set sized for Tn rows, its padding zeroed as an upload leaves it: where a composed table is written.
-static int shadow_cols(evg_ctx* c, int64_t Tn, EdDst* o) {
-  cudaStream_t s = c->stream;
-  auto& sh = c->ed.out;
-  const size_t np = size_t(Tn + kColPad);
-  for (DevBuf* b : {&sh.prio, &sh.nd, &sh.tgo, &sh.gid, &sh.vid, &sh.flags}) {
-    CK(b->ensure(4 * np));
-    CK(cudaMemsetAsync(b->as<int32_t>() + Tn, 0, 4 * kColPad, s));
-  }
-  for (DevBuf* b : {&sh.exp, &sh.qb, &sh.wb}) {
-    CK(b->ensure(8 * np));
-    CK(cudaMemsetAsync(b->as<int64_t>() + Tn, 0, 8 * kColPad, s));
-  }
-  o->priority = sh.prio.as<int32_t>(); o->numdep = sh.nd.as<int32_t>(); o->tgo = sh.tgo.as<int32_t>(); o->gid = sh.gid.as<int32_t>();
-  o->vid = sh.vid.as<int32_t>(); o->flags = sh.flags.as<uint32_t>(); o->expected = sh.exp.as<int64_t>(); o->qbasis = sh.qb.as<int64_t>();
-  o->wbasis = sh.wb.as<int64_t>();
-  return EVG_OK;
+  launch(c, c->stream, k_scan_blocks, unsigned(nb), 1024, 0, in, n, out, sum);
+  launch(c, c->stream, k_scan_sums, 1, 1024, 0, sum, nb);
+  launch(c, c->stream, k_scan_add, unsigned(nb), 1024, 0, out, n, sum, nb);
 }
 
 // The composed table in the shadow set (Tn rows) and in ed.dep_off / ed.dep_idx (En edges; edge_off: dep_off at the
@@ -3052,12 +3040,8 @@ static int install_composed(evg_ctx* c, const char* who, int64_t Tn, int64_t En,
   drop_tick(c);
   c->tasks.swap(e.out);
   if (En > 0) { c->b_depoff.swap(e.dep_off); c->b_depidx.swap(e.dep_idx); }
-  evg_task_soa ts;
-  memset(&ts, 0, sizeof(ts));
-  ts.n_tasks = Tn; ts.n_edges = En;
-  ts.priority = c->tasks.prio.as<int32_t>(); ts.num_dependents = c->tasks.nd.as<int32_t>(); ts.task_group_order = c->tasks.tgo.as<int32_t>();
-  ts.group_id = c->tasks.gid.as<int32_t>(); ts.version_id = c->tasks.vid.as<int32_t>(); ts.flags = c->tasks.flags.as<uint32_t>();
-  ts.expected_ns = c->tasks.exp.as<int64_t>(); ts.queue_basis_ns = c->tasks.qb.as<int64_t>(); ts.wait_basis_ns = c->tasks.wb.as<int64_t>();
+  evg_task_soa ts = c->tasks.soa(Tn);
+  ts.n_edges = En;
   if (En > 0) { ts.dep_off = c->b_depoff.as<int64_t>(); ts.dep_idx = c->b_depidx.as<int32_t>(); }
   return upload_tasks(c, who, &ts, distros, Cols::kResident, En > 0 ? edge_off : nullptr);
 }
@@ -3080,17 +3064,12 @@ static int compose_tick(evg_ctx* c, const char* who, EdMap m, const DTasks& O, c
   // ---- 1. survivors: the keep mask's scan (each survivor's place), composed row -> source row
   if (T0 > 0) {
     scan_counts(c, e.keep.as<int32_t>(), T0, e.pos.as<int64_t>(), e.scan_sum.as<int64_t>());
-    k_ed_src<<<grid_for(T0, 256), 256, 0, s>>>(T0, m, e.src.as<int32_t>());
-    c->launches++;
+    launch(c, s, k_ed_src, grid_for(T0, 256), 256, 0, T0, m, e.src.as<int32_t>());
   }
-  // ---- 2. the nine columns of the composed table into the shadow set
-  EdDst o;
-  int rc = shadow_cols(c, Tn, &o);
+  // ---- 2. the nine columns of the composed table into the shadow set, its padding zeroed as an upload leaves it
+  int rc = e.out.size(Tn, s, /*zero_pad=*/true);
   if (rc != EVG_OK) return rc;
-  if (Tn > 0) {
-    k_ed_gather<<<grid_for(Tn, 256), 256, 0, s>>>(Tn, m, O, In, o, e.err.as<int>());
-    c->launches++;
-  }
+  launch(c, s, k_ed_gather, grid_for(Tn, 256), 256, 0, Tn, m, O, In, e.out.dst(), e.err.as<int>());
   // ---- 3. edges: count (range-checking the source's), scan, dep_off at the distro boundaries for the routing (one D2H,
   // one sync), write
   int64_t En = 0;
@@ -3100,11 +3079,10 @@ static int compose_tick(evg_ctx* c, const char* who, EdMap m, const DTasks& O, c
   if (edges) {
     CK(e.edge_cnt.ensure(sizeof(int32_t) * size_t(Tn + 1)));
     CK(e.dep_off.ensure(sizeof(int64_t) * size_t(Tn + 1 + kColPad)));
-    k_ed_edge_count<<<grid_for(Tn, 256), 256, 0, s>>>(Tn, m, O, In, e.edge_cnt.as<int32_t>(), e.err.as<int>());
+    launch(c, s, k_ed_edge_count, grid_for(Tn, 256), 256, 0, Tn, m, O, In, e.edge_cnt.as<int32_t>(), e.err.as<int>());
     scan_counts(c, e.edge_cnt.as<int32_t>(), Tn, e.dep_off.as<int64_t>(), e.scan_sum.as<int64_t>());
     CK(e.edge_at.ensure(sizeof(int64_t) * size_t(D + 1)));
-    k_gather_i64<<<grid_for(D + 1, 256), 256, 0, s>>>(e.dep_off.as<int64_t>(), e.new_off.as<int64_t>(), e.edge_at.as<int64_t>(), D + 1);
-    c->launches += 2;
+    launch(c, s, k_gather_i64, grid_for(D + 1, 256), 256, 0, e.dep_off.as<int64_t>(), e.new_off.as<int64_t>(), e.edge_at.as<int64_t>(), D + 1);
     edge_off.resize(size_t(D) + 1);
     CK(cudaMemcpyAsync(edge_off.data(), e.edge_at.p, sizeof(int64_t) * size_t(D + 1), cudaMemcpyDeviceToHost, s));
   }
@@ -3118,8 +3096,7 @@ static int compose_tick(evg_ctx* c, const char* who, EdMap m, const DTasks& O, c
     En = edge_off[size_t(D)];
     CK(e.dep_idx.ensure(sizeof(int32_t) * size_t(En + kColPad)));
     if (En > 0) {
-      k_ed_edge_write<<<grid_for(Tn, 256), 256, 0, s>>>(Tn, m, O, In, e.dep_off.as<int64_t>(), e.dep_idx.as<int32_t>());
-      c->launches++;
+      launch(c, s, k_ed_edge_write, grid_for(Tn, 256), 256, 0, Tn, m, O, In, e.dep_off.as<int64_t>(), e.dep_idx.as<int32_t>());
       CK(cudaGetLastError());
     }
   }
@@ -3130,13 +3107,12 @@ static int compose_tick(evg_ctx* c, const char* who, EdMap m, const DTasks& O, c
 // --------------------------------------------------------------------------
 // evg_plan_from_finder: finder -> dependency predicate -> compaction -> resident planner inputs, all on the device
 // --------------------------------------------------------------------------
-// evg_plan_from_finder and evg_plan_from_finder_ex (pipe == NULL: the former)
-static int plan_from_finder(evg_ctx* c, const evg_runnable_in* in, const evg_pipeline_in* pipe, const evg_task_soa* cand,
+// evg_plan_from_finder and evg_plan_from_finder_ex (`name`; the former passes no pipe)
+static int plan_from_finder(const char* name, evg_ctx* c, const evg_runnable_in* in, const evg_pipeline_in* pipe, const evg_task_soa* cand,
                             const evg_distro_table* distros, const evg_host_soa* hosts, const int64_t* host_off, const evg_alloc_cfg* acfg,
                             const int64_t* dep_finished_ns, int64_t now_ns, int32_t* runnable, int64_t* count) {
-  if (!c || !in || !cand || !distros) return fail(EVG_ERR_INVALID, "evg_plan_from_finder: null argument");
-  LOCK(c);
-  const char* who = pipe ? "evg_plan_from_finder_ex" : "evg_plan_from_finder";
+  ENTER(c, name);
+  if (!in || !cand || !distros) return fail(EVG_ERR_INVALID, "%s: null argument", who);
   const int64_t T = in->n_tasks, E = cand->n_edges;
   const int32_t D = in->n_distros, P = in->n_projects;
   if (T < 0 || D < 0 || P < 0 || E < 0) return fail(EVG_ERR_INVALID, "negative sizes");
@@ -3147,7 +3123,7 @@ static int plan_from_finder(evg_ctx* c, const evg_runnable_in* in, const evg_pip
   if (T > (int64_t(1) << 31) - 2) return fail(EVG_ERR_INVALID, "evg_plan_from_finder: %lld candidates exceed 2^31-2", (long long)T);
   if (!distros->task_off) return fail(EVG_ERR_INVALID, "null distro arrays");
   if (T > 0 && (!in->deps || in->deps->n_tasks != T)) return fail(EVG_ERR_INVALID, "evg_plan_from_finder needs the candidates' dependency table (the planner's EVG_TF_DEPS_MET comes from it)");
-  if (T > 0 && task_cols_missing(cand)) return fail(EVG_ERR_INVALID, "null candidate column");
+  if (T > 0 && TaskCols::missing(cand)) return fail(EVG_ERR_INVALID, "null candidate column");
   if (E > 0 && (!cand->dep_off || !cand->dep_idx)) return fail(EVG_ERR_INVALID, "null candidate dependency edges");
   // The candidates' dep_off (8 B per candidate, ~10 ms of host memory reads at 8e6 candidates) is checked on a second
   // host thread while this one stages the tables and the device runs the finders; it indexes nothing before step 4.
@@ -3182,11 +3158,10 @@ static int plan_from_finder(evg_ctx* c, const evg_runnable_in* in, const evg_pip
   auto& pf = c->pf;
   r.met = c->deps.met.as<uint8_t>();
   if (any_pipe)
-    k_runnable_pipe<<<unsigned(D), 256, 0, s>>>(r, c->pl.project_raw.as<uint8_t>(), pf.kept.as<int32_t>(), pf.count.as<int64_t>(),
-                                                c->b_err.as<int>());
+    launch(c, s, k_runnable_pipe, unsigned(D), 256, 0, r, c->pl.project_raw.as<uint8_t>(), pf.kept.as<int32_t>(), pf.count.as<int64_t>(),
+           c->b_err.as<int>());
   else
-    k_runnable<<<unsigned(D), 256, 0, s>>>(r, pf.kept.as<int32_t>(), pf.count.as<int64_t>(), c->b_err.as<int>());
-  c->launches++;
+    launch(c, s, k_runnable, unsigned(D), 256, 0, r, pf.kept.as<int32_t>(), pf.count.as<int64_t>(), c->b_err.as<int>());
   CK(cudaGetLastError());
   // 3. the only thing the host needs before the planner can be routed: how many tasks each distro kept
   int bad = 0;
@@ -3215,35 +3190,30 @@ static int plan_from_finder(evg_ctx* c, const evg_runnable_in* in, const evg_pip
   auto& e = c->ed;
   CK(e.keep.ensure(sizeof(int32_t) * size_t(T + 1)));
   CK(cudaMemsetAsync(e.keep.p, 0, sizeof(int32_t) * size_t(T), s));
-  k_kept_mask<<<grid_for(T, 256), 256, 0, s>>>(T, D, pf.task_off.as<int64_t>(), pf.kept.as<int32_t>(), e.keep.as<int32_t>());
-  c->launches++;
+  launch(c, s, k_kept_mask, grid_for(T, 256), 256, 0, T, D, pf.task_off.as<int64_t>(), pf.kept.as<int32_t>(), e.keep.as<int32_t>());
   if (any_pipe) {
     // what the pipeline distros' planner receives: their verdicts (k_pl_plan needs the keep mask), and no candidate
     // edges for EVG_FINDER_PIPELINE rows (compose_tick then re-indexes the rest as for any finder)
     const int64_t* fin = dep_finished_ns && in->deps->n_deps > 0 ? c->deps.fin.as<int64_t>() : nullptr;
-    k_pl_plan<<<grid_for(T, 256), 256, 0, s>>>(ddeps(c, in->deps), D, pf.task_off.as<int64_t>(), pf.finder.as<uint8_t>(), e.keep.as<int32_t>(),
-                                               c->deps.met.as<uint8_t>(), fin, now_ns, c->deps.stamp.as<int64_t>());
-    c->launches++;
+    launch(c, s, k_pl_plan, grid_for(T, 256), 256, 0, ddeps(c, in->deps), D, pf.task_off.as<int64_t>(), pf.finder.as<uint8_t>(),
+           e.keep.as<int32_t>(), c->deps.met.as<uint8_t>(), fin, now_ns, c->deps.stamp.as<int64_t>());
     if (pipe_deps && E > 0) {
       auto& p = c->pl;
       CK(p.edge_cnt.ensure(sizeof(int32_t) * size_t(T + 1)));
       CK(p.dep_off.ensure(sizeof(int64_t) * size_t(T + 1)));
       CK(p.scan_sum.ensure(sizeof(int64_t) * size_t((T + 1023) / 1024 + 1)));
-      k_pl_edge_count<<<grid_for(T, 256), 256, 0, s>>>(T, D, pf.task_off.as<int64_t>(), pf.finder.as<uint8_t>(), pf.dep_off.as<int64_t>(),
-                                                       p.edge_cnt.as<int32_t>());
-      c->launches++;
+      launch(c, s, k_pl_edge_count, grid_for(T, 256), 256, 0, T, D, pf.task_off.as<int64_t>(), pf.finder.as<uint8_t>(), pf.dep_off.as<int64_t>(),
+             p.edge_cnt.as<int32_t>());
       scan_counts(c, p.edge_cnt.as<int32_t>(), T, p.dep_off.as<int64_t>(), p.scan_sum.as<int64_t>());
       // the kept edges fit in the candidates' E: no count has to reach the host
       CK(p.dep_idx.ensure(sizeof(int32_t) * size_t(E)));
-      k_pl_edge_write<<<grid_for(T, 256), 256, 0, s>>>(T, pf.dep_off.as<int64_t>(), pf.dep_idx.as<int32_t>(), p.dep_off.as<int64_t>(),
-                                                       p.dep_idx.as<int32_t>());
-      c->launches++;
+      launch(c, s, k_pl_edge_write, grid_for(T, 256), 256, 0, T, pf.dep_off.as<int64_t>(), pf.dep_idx.as<int32_t>(), p.dep_off.as<int64_t>(),
+             p.dep_idx.as<int32_t>());
       O.dep_off = p.dep_off.as<int64_t>(); O.dep_idx = p.dep_idx.as<int32_t>();
     }
   }
-  k_apply_deps<<<grid_for(T, 256), 256, 0, s>>>(T, c->deps.met.as<uint8_t>(), c->deps.stamp.as<int64_t>(), pf.cand.flags.as<uint32_t>(),
-                                                pf.cand.wb.as<int64_t>());
-  c->launches++;
+  launch(c, s, k_apply_deps, grid_for(T, 256), 256, 0, T, c->deps.met.as<uint8_t>(), c->deps.stamp.as<int64_t>(), pf.cand.flags.as<uint32_t>(),
+         pf.cand.wb.as<int64_t>());
   CK(e.ins_off.ensure(sizeof(int64_t) * size_t(D + 1)));
   CK(cudaMemsetAsync(e.ins_off.p, 0, sizeof(int64_t) * size_t(D + 1), s));
   // 5. the kept candidates become the resident tick, in the context's own columns
@@ -3267,12 +3237,12 @@ static int plan_from_finder(evg_ctx* c, const evg_runnable_in* in, const evg_pip
 int evg_plan_from_finder(evg_ctx* c, const evg_runnable_in* in, const evg_task_soa* cand, const evg_distro_table* distros,
                          const evg_host_soa* hosts, const int64_t* host_off, const evg_alloc_cfg* acfg, const int64_t* dep_finished_ns,
                          int64_t now_ns, int32_t* runnable, int64_t* count) {
-  return plan_from_finder(c, in, nullptr, cand, distros, hosts, host_off, acfg, dep_finished_ns, now_ns, runnable, count);
+  return plan_from_finder("evg_plan_from_finder", c, in, nullptr, cand, distros, hosts, host_off, acfg, dep_finished_ns, now_ns, runnable, count);
 }
 int evg_plan_from_finder_ex(evg_ctx* c, const evg_runnable_in* in, const evg_pipeline_in* pipe, const evg_task_soa* cand,
                             const evg_distro_table* distros, const evg_host_soa* hosts, const int64_t* host_off, const evg_alloc_cfg* acfg,
                             const int64_t* dep_finished_ns, int64_t now_ns, int32_t* runnable, int64_t* count) {
-  return plan_from_finder(c, in, pipe, cand, distros, hosts, host_off, acfg, dep_finished_ns, now_ns, runnable, count);
+  return plan_from_finder("evg_plan_from_finder_ex", c, in, pipe, cand, distros, hosts, host_off, acfg, dep_finished_ns, now_ns, runnable, count);
 }
 
 // --------------------------------------------------------------------------
@@ -3280,9 +3250,8 @@ int evg_plan_from_finder_ex(evg_ctx* c, const evg_runnable_in* in, const evg_pip
 // --------------------------------------------------------------------------
 int evg_edit_tasks(evg_ctx* c, const evg_task_edit* ed, const evg_distro_table* distros, const evg_host_soa* hosts,
                    const int64_t* host_off, const evg_alloc_cfg* acfg) {
-  if (!c) return fail(EVG_ERR_INVALID, "null context");
-  LOCK(c);
-  if (const int rc = need_tick(c, "evg_edit_tasks", Need::kEditable); rc != EVG_OK) return rc;
+  ENTER(c, "evg_edit_tasks");
+  if (const int rc = need_tick(c, who, Need::kEditable); rc != EVG_OK) return rc;
   if (!ed || !distros) return fail(EVG_ERR_INVALID, "evg_edit_tasks: null edit / distro table");
   // ---- every check the host can make, before anything resident changes
   const int32_t D = c->Dn;
@@ -3292,7 +3261,7 @@ int evg_edit_tasks(evg_ctx* c, const evg_task_edit* ed, const evg_distro_table* 
   if (distros->n_distros != D) return fail(EVG_ERR_INVALID, "evg_edit_tasks: n_distros %d, the resident tick has %d", distros->n_distros, D);
   if (R < 0 || I < 0 || EI < 0 || NA < 0) return fail(EVG_ERR_INVALID, "evg_edit_tasks: negative sizes");
   if (R > 0 && !ed->remove_rows) return fail(EVG_ERR_INVALID, "evg_edit_tasks: null remove_rows");
-  if (I > 0 && (!ed->insert_off || task_cols_missing(ins))) return fail(EVG_ERR_INVALID, "evg_edit_tasks: null insert_off / inserted column");
+  if (I > 0 && (!ed->insert_off || TaskCols::missing(ins))) return fail(EVG_ERR_INVALID, "evg_edit_tasks: null insert_off / inserted column");
   if (EI > 0 && (I == 0 || !ins->dep_off || !ins->dep_idx)) return fail(EVG_ERR_INVALID, "evg_edit_tasks: inserted edges without dep_off / dep_idx");
   if (NA > 0 && (!ed->add_edge_task || !ed->add_edge_dep)) return fail(EVG_ERR_INVALID, "evg_edit_tasks: null added edges");
   if (D > 0 && (!distros->task_off || !distros->group_off || !distros->cfg)) return fail(EVG_ERR_INVALID, "evg_edit_tasks: null distro arrays");
@@ -3304,10 +3273,10 @@ int evg_edit_tasks(evg_ctx* c, const evg_task_edit* ed, const evg_distro_table* 
       return fail(EVG_ERR_INVALID, "evg_edit_tasks: remove_rows[%lld] = %lld is not ascending inside [0, %lld)", (long long)k, (long long)r, (long long)T0);
     removed[size_t(std::upper_bound(c->h_taskoff.begin(), c->h_taskoff.end(), r) - c->h_taskoff.begin() - 1)]++;
   }
-  int rc = I > 0 ? check_offsets(ed->insert_off, D, I, "evg_edit_tasks", "insert_off") : EVG_OK;
-  if (rc == EVG_OK && EI > 0) rc = check_offsets(ins->dep_off, I, EI, "evg_edit_tasks", "insert->dep_off");
-  if (rc == EVG_OK && D > 0) rc = check_offsets(distros->task_off, D, -1, "evg_edit_tasks", "task_off");
-  if (rc == EVG_OK && D > 0) rc = check_offsets(distros->group_off, D, -1, "evg_edit_tasks", "group_off");
+  int rc = I > 0 ? check_offsets(ed->insert_off, D, I, who, "insert_off") : EVG_OK;
+  if (rc == EVG_OK && EI > 0) rc = check_offsets(ins->dep_off, I, EI, who, "insert->dep_off");
+  if (rc == EVG_OK && D > 0) rc = check_offsets(distros->task_off, D, -1, who, "task_off");
+  if (rc == EVG_OK && D > 0) rc = check_offsets(distros->group_off, D, -1, who, "group_off");
   if (rc != EVG_OK) return rc;
   if (I > 0) ins_off.assign(ed->insert_off, ed->insert_off + D + 1);
   for (int32_t d = 0; d < D; d++) {
@@ -3327,7 +3296,6 @@ int evg_edit_tasks(evg_ctx* c, const evg_task_edit* ed, const evg_distro_table* 
     if (row - distros->task_off[d] >= survivors)
       return fail(EVG_ERR_INVALID, "evg_edit_tasks: add_edge_task[%lld] = %lld is not a surviving task", (long long)k, (long long)row);
   }
-  CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   auto& e = c->ed;
   c->launches = 0;
@@ -3346,10 +3314,7 @@ int evg_edit_tasks(evg_ctx* c, const evg_task_edit* ed, const evg_distro_table* 
   UP(s, e.ins_off, ins_off.data(), D + 1, int64_t);
   UP(s, e.old_vbase, old_vbase.data(), D + 1, int64_t);
   CK(e.keep.ensure(sizeof(int32_t) * size_t(T0 + 1)));
-  if (T0 > 0) {
-    k_ed_keep<<<grid_for(T0, 256), 256, 0, s>>>(T0, e.rm.as<int64_t>(), R, e.keep.as<int32_t>());
-    c->launches++;
-  }
+  launch(c, s, k_ed_keep, grid_for(T0, 256), 256, 0, T0, e.rm.as<int64_t>(), R, e.keep.as<int32_t>());
   EdMap m;
   memset(&m, 0, sizeof(m));
   m.D = D; m.old_off = e.old_off.as<int64_t>(); m.ins_off = e.ins_off.as<int64_t>();
@@ -3359,10 +3324,10 @@ int evg_edit_tasks(evg_ctx* c, const evg_task_edit* ed, const evg_distro_table* 
   m.n_add = NA; m.add_task = e.add_task.as<int64_t>(); m.add_dep = e.add_dep.as<int32_t>();
   DTasks In = e.ins.view(I);
   In.n_edges = EI; In.dep_off = e.ins_dep_off.as<int64_t>(); In.dep_idx = e.ins_dep_idx.as<int32_t>();
-  rc = compose_tick(c, "evg_edit_tasks", m, dtasks(c), In, distros);
+  rc = compose_tick(c, who, m, dtasks(c), In, distros);
   if (rc != EVG_OK) return rc;
   if (hosts) {
-    rc = upload_hosts(c, "evg_edit_tasks", hosts, host_off, acfg, D);
+    rc = upload_hosts(c, who, hosts, host_off, acfg, D);
     if (rc != EVG_OK) return rc;
     CK(cudaStreamSynchronize(s));
   }
@@ -3589,8 +3554,7 @@ __global__ void __launch_bounds__(256) k_al_edge_write(int64_t n, const uint64_t
 }
 
 int evg_plan_aliases(evg_ctx* c, const evg_alias_in* in, const evg_distro_cfg* cfg, int32_t D, int64_t now_ns, evg_alias_out* out) {
-  if (!c) return fail(EVG_ERR_INVALID, "null context");
-  LOCK(c);
+  ENTER(c, "evg_plan_aliases");
   if (!in || !out || !in->deps) return fail(EVG_ERR_INVALID, "evg_plan_aliases: null argument");
   // ---- every check the host can make, before anything resident changes
   const evg_task_soa* t = &in->tasks;
@@ -3603,16 +3567,16 @@ int evg_plan_aliases(evg_ctx* c, const evg_alias_in* in, const evg_distro_cfg* c
   if (T > (int64_t(1) << 31) - 2) return fail(EVG_ERR_INVALID, "evg_plan_aliases: %lld rows exceed 2^31-2", (long long)T);
   if (!out->task_off || !out->group_off || (D > 0 && (!out->n_versions || !cfg))) return fail(EVG_ERR_INVALID, "evg_plan_aliases: null cfg / output");
   if (!in->secondary_off || !in->dest_off || (NG > 0 && !in->group_max_hosts)) return fail(EVG_ERR_INVALID, "evg_plan_aliases: null offsets / group_max_hosts");
-  if (T > 0 && (task_cols_missing(t) || !in->sched || !in->task_group_max_hosts || !in->primary || !dp->dep_off || !dp->task_state ||
+  if (T > 0 && (TaskCols::missing(t) || !in->sched || !in->task_group_max_hosts || !in->primary || !dp->dep_off || !dp->task_state ||
                 !dp->task_pre))
     return fail(EVG_ERR_INVALID, "evg_plan_aliases: null task column");
   if (E > 0 && (!t->dep_off || !t->dep_idx)) return fail(EVG_ERR_INVALID, "evg_plan_aliases: null dep_off / dep_idx");
   if (dp->n_deps > 0 && (!dp->dep_kind || !dp->dep_ref || !dp->dep_want)) return fail(EVG_ERR_INVALID, "evg_plan_aliases: null dependency arrays");
   if (dp->n_ext > 0 && !dp->ext_state) return fail(EVG_ERR_INVALID, "evg_plan_aliases: null ext_state");
   // deps->dep_off is checked by deps_to_device and k_deps_met, like every evg_deps_in
-  int rc = check_offsets(in->secondary_off, T, -1, "evg_plan_aliases", "secondary_off");
-  if (rc == EVG_OK) rc = check_offsets(in->dest_off, NN, -1, "evg_plan_aliases", "dest_off");
-  if (rc == EVG_OK && E > 0) rc = check_offsets(t->dep_off, T, E, "evg_plan_aliases", "tasks.dep_off");
+  int rc = check_offsets(in->secondary_off, T, -1, who, "secondary_off");
+  if (rc == EVG_OK) rc = check_offsets(in->dest_off, NN, -1, who, "dest_off");
+  if (rc == EVG_OK && E > 0) rc = check_offsets(t->dep_off, T, E, who, "tasks.dep_off");
   if (rc != EVG_OK) return rc;
   const int64_t NS = in->secondary_off[T], ND = in->dest_off[NN];
   if (NS > 0 && !in->secondary_idx) return fail(EVG_ERR_INVALID, "evg_plan_aliases: null secondary_idx");
@@ -3621,7 +3585,6 @@ int evg_plan_aliases(evg_ctx* c, const evg_alias_in* in, const evg_distro_cfg* c
     if (in->dest_idx[k] < 0 || in->dest_idx[k] >= D)
       return fail(EVG_ERR_INVALID, "evg_plan_aliases: dest_idx[%lld] = %d is outside [0, %d)", (long long)k, in->dest_idx[k], D);
   // ---- from here the previous tick is gone: the dependency state and the resident columns are replaced
-  CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   auto& a = c->al;
   drop_tick(c);
@@ -3647,11 +3610,10 @@ int evg_plan_aliases(evg_ctx* c, const evg_alias_in* in, const evg_distro_cfg* c
   UP(s, a.doff, in->dest_off, NN + 1, int64_t);
   UP(s, a.didx, in->dest_idx, ND, int32_t);
   if (T > 0) {
-    rc = deps_to_device(c, "evg_plan_aliases", dp, 0, in->dep_finished_ns, now_ns, /*want_stamp=*/true);
+    rc = deps_to_device(c, who, dp, 0, in->dep_finished_ns, now_ns, /*want_stamp=*/true);
     if (rc != EVG_OK) return rc;
-    k_apply_deps<<<grid_for(T, 256), 256, 0, s>>>(T, c->deps.met.as<uint8_t>(), c->deps.stamp.as<int64_t>(), a.src.flags.as<uint32_t>(),
-                                                  a.src.wb.as<int64_t>());
-    c->launches++;
+    launch(c, s, k_apply_deps, grid_for(T, 256), 256, 0, T, c->deps.met.as<uint8_t>(), c->deps.stamp.as<int64_t>(), a.src.flags.as<uint32_t>(),
+           a.src.wb.as<int64_t>());
   }
   // 2. per row: eligibility and its distinct alias queues; the pair offsets (one value crosses to the host)
   AlView v;
@@ -3664,8 +3626,7 @@ int evg_plan_aliases(evg_ctx* c, const evg_alias_in* in, const evg_distro_cfg* c
   int64_t P = 0;
   int bad = 0;
   if (T > 0) {
-    k_al_count<<<grid_for(T, 256), 256, 0, s>>>(v, S, a.cnt.as<int32_t>(), err);
-    c->launches++;
+    launch(c, s, k_al_count, grid_for(T, 256), 256, 0, v, S, a.cnt.as<int32_t>(), err);
     scan_counts(c, a.cnt.as<int32_t>(), T, a.poff.as<int64_t>(), c->ed.scan_sum.as<int64_t>());
     CK(cudaMemcpyAsync(&P, a.poff.as<int64_t>() + T, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
   }
@@ -3674,15 +3635,14 @@ int evg_plan_aliases(evg_ctx* c, const evg_alias_in* in, const evg_distro_cfg* c
   CK(cudaMemcpyAsync(&bad_ref, c->b_err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   CK(cudaGetLastError());
-  if (bad_ref) return deps_bad("evg_plan_aliases", bad_ref);
+  if (bad_ref) return deps_bad(who, bad_ref);
   if (bad) return fail(EVG_ERR_INVALID, "evg_plan_aliases: a secondary_idx, primary, group_id or version_id is out of range");
   if (P > (int64_t(1) << 31) - 2) return fail(EVG_ERR_INVALID, "evg_plan_aliases: %lld (queue, task) pairs exceed 2^31-2", (long long)P);
   // 3. the pairs, in source-row order, sorted by queue
   for (int k = 0; k < 2; k++) CK(a.keys[k].ensure(sizeof(uint64_t) * size_t(P + 1)));
   int cur = 0;
   if (P > 0) {
-    k_al_pairs<<<grid_for(T, 256), 256, 0, s>>>(v, a.poff.as<int64_t>(), a.keys[0].as<uint64_t>());
-    c->launches++;
+    launch(c, s, k_al_pairs, grid_for(T, 256), 256, 0, v, a.poff.as<int64_t>(), a.keys[0].as<uint64_t>());
     int bits = 0;
     while (bits < 31 && (int64_t(1) << bits) < D) bits++;
     const int64_t n_tiles = (P + kAlTile - 1) / kAlTile, nh = 256 * n_tiles;
@@ -3692,17 +3652,15 @@ int evg_plan_aliases(evg_ctx* c, const evg_alias_in* in, const evg_distro_cfg* c
       CK(c->ed.scan_sum.ensure(sizeof(int64_t) * size_t((nh + 1023) / 1024 + 1)));
     }
     for (int shift = 32; shift < 32 + bits; shift += 8, cur ^= 1) {
-      k_al_hist<<<unsigned(n_tiles), 256, 0, s>>>(a.keys[cur].as<uint64_t>(), P, shift, a.hist.as<int32_t>(), n_tiles);
+      launch(c, s, k_al_hist, unsigned(n_tiles), 256, 0, a.keys[cur].as<uint64_t>(), P, shift, a.hist.as<int32_t>(), n_tiles);
       scan_counts(c, a.hist.as<int32_t>(), nh, a.hoff.as<int64_t>(), c->ed.scan_sum.as<int64_t>());
-      k_al_scatter<<<unsigned(n_tiles), 256, 0, s>>>(a.keys[cur].as<uint64_t>(), a.keys[cur ^ 1].as<uint64_t>(), P, shift,
-                                                     a.hoff.as<int64_t>(), n_tiles);
-      c->launches += 2;
+      launch(c, s, k_al_scatter, unsigned(n_tiles), 256, 0, a.keys[cur].as<uint64_t>(), a.keys[cur ^ 1].as<uint64_t>(), P, shift,
+             a.hoff.as<int64_t>(), n_tiles);
     }
   }
   const uint64_t* keys = a.keys[cur].as<uint64_t>();
   CK(a.qoff.ensure(sizeof(int64_t) * size_t(D + 1)));
-  k_al_qoff<<<grid_for(D + 1, 256), 256, 0, s>>>(keys, P, D, a.qoff.as<int64_t>());
-  c->launches++;
+  launch(c, s, k_al_qoff, grid_for(D + 1, 256), 256, 0, keys, P, D, a.qoff.as<int64_t>());
   // 4. per queue, dense group and version ids in first-appearance order
   uint64_t cap = 64;
   while (cap < 4 * uint64_t(P)) cap <<= 1;  // at most 2P keys: load factor <= 1/2
@@ -3716,42 +3674,35 @@ int evg_plan_aliases(evg_ctx* c, const evg_alias_in* in, const evg_distro_cfg* c
     CK(a.hv.ensure(sizeof(uint32_t) * cap));
     CK(cudaMemsetAsync(a.hk.p, 0xFF, sizeof(uint64_t) * cap, s));
     CK(cudaMemsetAsync(a.hv.p, 0xFF, sizeof(uint32_t) * cap, s));
-    k_al_first<<<grid_for(P, 256), 256, 0, s>>>(P, keys, S, a.hk.as<uint64_t>(), a.hv.as<uint32_t>(), cap - 1, a.gslot.as<int64_t>(),
-                                                a.vslot.as<int64_t>());
-    k_al_flag<<<grid_for(P, 256), 256, 0, s>>>(P, a.gslot.as<int64_t>(), a.vslot.as<int64_t>(), a.hv.as<uint32_t>(), a.fg.as<int32_t>(),
-                                               a.fv.as<int32_t>());
-    c->launches += 2;
+    launch(c, s, k_al_first, grid_for(P, 256), 256, 0, P, keys, S, a.hk.as<uint64_t>(), a.hv.as<uint32_t>(), cap - 1, a.gslot.as<int64_t>(),
+           a.vslot.as<int64_t>());
+    launch(c, s, k_al_flag, grid_for(P, 256), 256, 0, P, a.gslot.as<int64_t>(), a.vslot.as<int64_t>(), a.hv.as<uint32_t>(), a.fg.as<int32_t>(),
+           a.fv.as<int32_t>());
     CK(c->ed.scan_sum.ensure(sizeof(int64_t) * size_t((P + 1023) / 1024 + 1)));
     scan_counts(c, a.fg.as<int32_t>(), P, a.pg.as<int64_t>(), c->ed.scan_sum.as<int64_t>());
     scan_counts(c, a.fv.as<int32_t>(), P, a.pv.as<int64_t>(), c->ed.scan_sum.as<int64_t>());
   }
-  // 5. the nine columns into the shadow set
-  EdDst o;
-  rc = shadow_cols(c, P, &o);
+  // 5. the nine columns into the shadow set, its padding zeroed as an upload leaves it
+  auto& e = c->ed;
+  rc = e.out.size(P, s, /*zero_pad=*/true);
   if (rc != EVG_OK) return rc;
   AlIds ids;
   ids.qoff = a.qoff.as<int64_t>(); ids.gslot = a.gslot.as<int64_t>(); ids.vslot = a.vslot.as<int64_t>();
   ids.pg = a.pg.as<int64_t>(); ids.pv = a.pv.as<int64_t>(); ids.hv = a.hv.as<uint32_t>();
-  if (P > 0) {
-    k_al_gather<<<grid_for(P, 256), 256, 0, s>>>(P, keys, ids, S, a.primary.as<int32_t>(), a.gmax.as<int32_t>(), o, a.srow.as<int32_t>(),
-                                                 a.gout.as<int32_t>(), a.gsrc.as<int32_t>());
-    c->launches++;
-  }
+  launch(c, s, k_al_gather, grid_for(P, 256), 256, 0, P, keys, ids, S, a.primary.as<int32_t>(), a.gmax.as<int32_t>(), e.out.dst(),
+         a.srow.as<int32_t>(), a.gout.as<int32_t>(), a.gsrc.as<int32_t>());
   // 6. edges: count, scan; the queue, group, version and edge offsets of every distro cross to the host (one sync)
-  auto& e = c->ed;
   const bool edges = P > 0 && E > 0;
   CK(a.samp.ensure(sizeof(int64_t) * 3 * size_t(D + 1)));
   int64_t* samp = a.samp.as<int64_t>();
-  k_gather_i64<<<grid_for(D + 1, 256), 256, 0, s>>>(a.pg.as<int64_t>(), a.qoff.as<int64_t>(), samp, D + 1);
-  k_gather_i64<<<grid_for(D + 1, 256), 256, 0, s>>>(a.pv.as<int64_t>(), a.qoff.as<int64_t>(), samp + (D + 1), D + 1);
-  c->launches += 2;
+  launch(c, s, k_gather_i64, grid_for(D + 1, 256), 256, 0, a.pg.as<int64_t>(), a.qoff.as<int64_t>(), samp, D + 1);
+  launch(c, s, k_gather_i64, grid_for(D + 1, 256), 256, 0, a.pv.as<int64_t>(), a.qoff.as<int64_t>(), samp + (D + 1), D + 1);
   if (edges) {
     CK(e.edge_cnt.ensure(sizeof(int32_t) * size_t(P + 1)));
     CK(e.dep_off.ensure(sizeof(int64_t) * size_t(P + 1 + kColPad)));
-    k_al_edge_count<<<grid_for(P, 256), 256, 0, s>>>(P, keys, a.qoff.as<int64_t>(), S, e.edge_cnt.as<int32_t>(), err);
+    launch(c, s, k_al_edge_count, grid_for(P, 256), 256, 0, P, keys, a.qoff.as<int64_t>(), S, e.edge_cnt.as<int32_t>(), err);
     scan_counts(c, e.edge_cnt.as<int32_t>(), P, e.dep_off.as<int64_t>(), c->ed.scan_sum.as<int64_t>());
-    k_gather_i64<<<grid_for(D + 1, 256), 256, 0, s>>>(e.dep_off.as<int64_t>(), a.qoff.as<int64_t>(), samp + 2 * (D + 1), D + 1);
-    c->launches += 2;
+    launch(c, s, k_gather_i64, grid_for(D + 1, 256), 256, 0, e.dep_off.as<int64_t>(), a.qoff.as<int64_t>(), samp + 2 * (D + 1), D + 1);
   }
   std::vector<int64_t> h(3 * size_t(D + 1), 0);
   CK(cudaMemcpyAsync(out->task_off, a.qoff.p, sizeof(int64_t) * size_t(D + 1), cudaMemcpyDeviceToHost, s));
@@ -3775,10 +3726,8 @@ int evg_plan_aliases(evg_ctx* c, const evg_alias_in* in, const evg_distro_cfg* c
   if (G > 0) CK(cudaMemcpyAsync(gmax.data(), a.gout.p, sizeof(int32_t) * size_t(G), cudaMemcpyDeviceToHost, s));
   if (edges) {
     CK(e.dep_idx.ensure(sizeof(int32_t) * size_t(En + kColPad)));
-    if (En > 0) {
-      k_al_edge_write<<<grid_for(P, 256), 256, 0, s>>>(P, keys, a.qoff.as<int64_t>(), S, e.dep_off.as<int64_t>(), e.dep_idx.as<int32_t>());
-      c->launches++;
-    }
+    if (En > 0)
+      launch(c, s, k_al_edge_write, grid_for(P, 256), 256, 0, P, keys, a.qoff.as<int64_t>(), S, e.dep_off.as<int64_t>(), e.dep_idx.as<int32_t>());
   }
   CK(cudaStreamSynchronize(s));
   CK(cudaGetLastError());
@@ -3787,7 +3736,7 @@ int evg_plan_aliases(evg_ctx* c, const evg_alias_in* in, const evg_distro_cfg* c
   evg_distro_table dt;
   memset(&dt, 0, sizeof(dt));
   dt.n_distros = D; dt.task_off = out->task_off; dt.group_off = out->group_off; dt.cfg = cf.data(); dt.group_max_hosts = gmax.data();
-  rc = install_composed(c, "evg_plan_aliases", P, En, edge_off, &dt);
+  rc = install_composed(c, who, P, En, edge_off, &dt);
   if (rc != EVG_OK) return rc;
   c->tick.kind = Tick::kOwn;
   c->tick.aliases = true;
@@ -3795,10 +3744,8 @@ int evg_plan_aliases(evg_ctx* c, const evg_alias_in* in, const evg_distro_cfg* c
 }
 
 int evg_download_alias_map(evg_ctx* c, int32_t* source_row, int32_t* group_source) {
-  if (!c) return fail(EVG_ERR_INVALID, "null context");
-  LOCK(c);
-  if (const int rc = need_tick(c, "evg_download_alias_map", Need::kAliasMap); rc != EVG_OK) return rc;
-  CK(cudaSetDevice(c->device));
+  ENTER(c, "evg_download_alias_map");
+  if (const int rc = need_tick(c, who, Need::kAliasMap); rc != EVG_OK) return rc;
   if (source_row && c->T) CK(cudaMemcpyAsync(source_row, c->al.srow.p, sizeof(int32_t) * size_t(c->T), cudaMemcpyDeviceToHost, c->stream));
   if (group_source && c->G) CK(cudaMemcpyAsync(group_source, c->al.gsrc.p, sizeof(int32_t) * size_t(c->G), cudaMemcpyDeviceToHost, c->stream));
   CK(cudaStreamSynchronize(c->stream));
@@ -3898,8 +3845,8 @@ int evg_intern_columns(const evg_string_cols* in, evg_intern_out* out, int32_t t
 
 int evg_prioritize_legacy_batch(evg_ctx* c, const evg_legacy_soa* in, const int64_t* task_off, const uint8_t* list_mode,
                                 int32_t n_distros, int32_t* order, int64_t* count, int32_t* status) {
-  if (!c || !in) return fail(EVG_ERR_INVALID, "evg_prioritize_legacy_batch: null argument");
-  LOCK(c);
+  ENTER(c, "evg_prioritize_legacy_batch");
+  if (!in) return fail(EVG_ERR_INVALID, "evg_prioritize_legacy_batch: null argument");
   const int64_t T = in->n_tasks;
   const int32_t D = n_distros;
   if (T < 0 || D < 0) return fail(EVG_ERR_INVALID, "negative sizes");
@@ -3908,13 +3855,12 @@ int evg_prioritize_legacy_batch(evg_ctx* c, const evg_legacy_soa* in, const int6
   if (T > 0 && (!in->priority || !in->ingest_ns || !in->expected_ns || !in->num_dependents || !in->revision_order || !in->project_id ||
                 !in->tg_rank || !in->tg_pair_id || !in->task_group_order || !in->presort_rank || !in->flags))
     return fail(EVG_ERR_INVALID, "null task column");
-  const int rc = check_offsets(task_off, D, T, "evg_prioritize_legacy_batch", "task_off");
+  const int rc = check_offsets(task_off, D, T, who, "task_off");
   if (rc != EVG_OK) return rc;
   int64_t max_n = 0;
   for (int32_t d = 0; d < D; d++) max_n = std::max(max_n, task_off[d + 1] - task_off[d]);
   for (int64_t k = 0; k < 3 * int64_t(D); k++)
     if (list_mode[k] > EVG_LEGACY_MODE_LITERAL) return fail(EVG_ERR_INVALID, "unknown list mode %d", int(list_mode[k]));
-  CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   c->launches = 0;
   drop_tick(c);
@@ -3947,12 +3893,12 @@ int evg_prioritize_legacy_batch(evg_ctx* c, const evg_legacy_soa* in, const int6
   int32_t* buf[2] = {c->b_rn3.as<int32_t>(), c->b_rn4.as<int32_t>()};
   int cur = 0;
   if (T > 0) {
-    LAUNCH(c, k_legacy_init, grid_for(T, 256), 256, x, buf[0], c->b_rn5.as<unsigned int>());
+    launch(c, c->stream, k_legacy_init, grid_for(T, 256), 256, 0, x, buf[0], c->b_rn5.as<unsigned int>());
     for (int64_t L = 1; L < max_n; L <<= 1) {
-      LAUNCH(c, k_legacy_merge_pass, grid_for(T, 256), 256, x, buf[cur], buf[cur ^ 1], L);
+      launch(c, c->stream, k_legacy_merge_pass, grid_for(T, 256), 256, 0, x, buf[cur], buf[cur ^ 1], L);
       cur ^= 1;
     }
-    LAUNCH(c, k_legacy_interleave, grid_for(T, 256), 256, x, buf[cur], c->b_rn5.as<unsigned int>(), c->b_order.as<int32_t>(),
+    launch(c, c->stream, k_legacy_interleave, grid_for(T, 256), 256, 0, x, buf[cur], c->b_rn5.as<unsigned int>(), c->b_order.as<int32_t>(),
            c->b_rn6.as<int64_t>(), c->b_status.as<int32_t>());
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(order, c->b_order.p, sizeof(int32_t) * size_t(T), cudaMemcpyDeviceToHost, s));
@@ -3993,7 +3939,7 @@ static int dag_run(evg_ctx* c, const DDag& x, const DagBufs& b, int64_t max_n, c
   int32_t* d_nsorted = b.stats;
   int32_t* d_ncycles = d_nsorted + (D + 1);
   int32_t* d_grouped = d_ncycles + (D + 1);
-  LAUNCH(c, k_dag_topo, grid_for(int64_t(D) * 32, 64), 64, x, b.sorted, d_nsorted, d_ncycles);
+  launch(c, c->stream, k_dag_topo, grid_for(int64_t(D) * 32, 64), 64, 0, x, b.sorted, d_nsorted, d_ncycles);
   std::vector<int32_t> grouped(size_t(D), 0);
   int cur = 0;
   if (N > 0) {
@@ -4001,12 +3947,12 @@ static int dag_run(evg_ctx* c, const DDag& x, const DagBufs& b, int64_t max_n, c
     // every item has a group or not: "no ungrouped item" leaves grouped[d] at the distro's length
     for (int32_t d = 0; d < D; d++) grouped[size_t(d)] = int32_t(item_off[d + 1] - item_off[d]);
     CK(cudaMemcpyAsync(d_grouped, grouped.data(), sizeof(int32_t) * size_t(D), cudaMemcpyHostToDevice, s));
-    LAUNCH(c, k_dag_group_init, grid_for(N, 256), 256, x, b.buf[0]);
+    launch(c, c->stream, k_dag_group_init, grid_for(N, 256), 256, 0, x, b.buf[0]);
     for (int64_t L = 1; L < max_n; L <<= 1) {
-      LAUNCH(c, k_dag_group_pass, grid_for(N, 256), 256, x, b.buf[cur], b.buf[cur ^ 1], L);
+      launch(c, c->stream, k_dag_group_pass, grid_for(N, 256), 256, 0, x, b.buf[cur], b.buf[cur ^ 1], L);
       cur ^= 1;
     }
-    LAUNCH(c, k_dag_units, grid_for(N, 256), 256, x, b.buf[cur], b.group_off, b.unit_off, d_grouped);
+    launch(c, c->stream, k_dag_units, grid_for(N, 256), 256, 0, x, b.buf[cur], b.group_off, b.unit_off, d_grouped);
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(unit_items, b.buf[cur], sizeof(int32_t) * size_t(N), cudaMemcpyDeviceToHost, s));
     CK(cudaMemcpyAsync(unit_off, b.unit_off, sizeof(int32_t) * size_t(G + D), cudaMemcpyDeviceToHost, s));
@@ -4021,8 +3967,8 @@ static int dag_run(evg_ctx* c, const DDag& x, const DagBufs& b, int64_t max_n, c
 
 int evg_dag_rebuild_batch(evg_ctx* c, const evg_dag_in* in, const int64_t* item_off, const int64_t* group_off, int32_t n_distros,
                           int32_t* sorted, int32_t* n_sorted, int32_t* n_cycles, int32_t* unit_items, int32_t* unit_off) {
-  if (!c || !in) return fail(EVG_ERR_INVALID, "evg_dag_rebuild_batch: null argument");
-  LOCK(c);
+  ENTER(c, "evg_dag_rebuild_batch");
+  if (!in) return fail(EVG_ERR_INVALID, "evg_dag_rebuild_batch: null argument");
   const int64_t N = in->n_items, E = in->n_deps;
   const int32_t D = n_distros;
   if (N < 0 || E < 0 || D < 0) return fail(EVG_ERR_INVALID, "negative sizes");
@@ -4030,15 +3976,14 @@ int evg_dag_rebuild_batch(evg_ctx* c, const evg_dag_in* in, const int64_t* item_
   if (!item_off || !group_off || !n_sorted || !n_cycles || !unit_off || (N > 0 && (!sorted || !unit_items))) return fail(EVG_ERR_INVALID, "null argument");
   if (N > 0 && (!in->dep_off || !in->group_id || !in->group_index)) return fail(EVG_ERR_INVALID, "null item column");
   if (E > 0 && !in->dep_item) return fail(EVG_ERR_INVALID, "null dep_item");
-  int rc = check_offsets(item_off, D, N, "evg_dag_rebuild_batch", "item_off");
-  if (rc == EVG_OK) rc = check_offsets(group_off, D, -1, "evg_dag_rebuild_batch", "group_off");
-  if (rc == EVG_OK && N > 0) rc = check_offsets(in->dep_off, N, E, "evg_dag_rebuild_batch", "dep_off");
+  int rc = check_offsets(item_off, D, N, who, "item_off");
+  if (rc == EVG_OK) rc = check_offsets(group_off, D, -1, who, "group_off");
+  if (rc == EVG_OK && N > 0) rc = check_offsets(in->dep_off, N, E, who, "dep_off");
   if (rc != EVG_OK) return rc;
   int64_t max_n = 0;
   for (int32_t d = 0; d < D; d++) max_n = std::max(max_n, item_off[d + 1] - item_off[d]);
   if (max_n >= (int64_t(1) << 31) - 1) return fail(EVG_ERR_INVALID, "a queue exceeds 2^31 items");
   const int64_t G = group_off[D];
-  CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   c->launches = 0;
   drop_tick(c);
@@ -4133,9 +4078,9 @@ __global__ void __launch_bounds__(256) k_dp_groups(DDisp X, const int64_t* __res
 }
 
 int evg_rebuild_dispatchers(evg_ctx* c, int32_t cap, int64_t items_capacity, int64_t groups_capacity, evg_dispatch_out* out) {
-  if (!c || !out) return fail(EVG_ERR_INVALID, "evg_rebuild_dispatchers: null argument");
-  LOCK(c);
-  if (const int rc = need_tick(c, "evg_rebuild_dispatchers", Need::kTick); rc != EVG_OK) return rc;
+  ENTER(c, "evg_rebuild_dispatchers");
+  if (!out) return fail(EVG_ERR_INVALID, "evg_rebuild_dispatchers: null argument");
+  if (const int rc = need_tick(c, who, Need::kTick); rc != EVG_OK) return rc;
   if (cap < 0) return fail(EVG_ERR_INVALID, "evg_rebuild_dispatchers: negative cap");
   if (cap == 0) cap = EVG_PERSISTED_QUEUE_CAP;
   if (!out->item_off || !out->n_sorted || !out->n_cycles || !out->group_off || !out->unit_off)
@@ -4162,7 +4107,6 @@ int evg_rebuild_dispatchers(evg_ctx* c, int32_t cap, int64_t items_capacity, int
     for (int32_t d = 0; d <= D; d++) out->group_off[d] = 0;
     return EVG_OK;
   }
-  CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   auto& p = c->dp;
   const int64_t T = c->T, E = c->E, G = c->G;
@@ -4192,11 +4136,11 @@ int evg_rebuild_dispatchers(evg_ctx* c, int32_t cap, int64_t items_capacity, int
   X.dep_off = E > 0 ? c->b_depoff.as<int64_t>() : nullptr; X.dep_idx = E > 0 ? c->b_depidx.as<int32_t>() : nullptr;
   X.rank_of = p.rank_of.as<int32_t>(); X.row = p.row.as<int32_t>(); X.first = p.first.as<int32_t>();
   int32_t* cnt = p.cnt.as<int32_t>();
-  LAUNCH(c, k_dp_gather, grid_for(N, 256), 256, X, p.gslot_of.as<int32_t>(), p.gindex.as<int32_t>(), cnt);
+  launch(c, c->stream, k_dp_gather, grid_for(N, 256), 256, 0, X, p.gslot_of.as<int32_t>(), p.gindex.as<int32_t>(), cnt);
   scan_counts(c, cnt, N, p.dep_off.as<int64_t>(), p.scan_sum.as<int64_t>());
-  LAUNCH(c, k_dp_edges, grid_for(N, 256), 256, X, p.dep_off.as<int64_t>(), p.dep_item.as<int32_t>(), p.gslot_of.as<int32_t>(), cnt);
+  launch(c, c->stream, k_dp_edges, grid_for(N, 256), 256, 0, X, p.dep_off.as<int64_t>(), p.dep_item.as<int32_t>(), p.gslot_of.as<int32_t>(), cnt);
   scan_counts(c, cnt, N, p.pos.as<int64_t>(), p.scan_sum.as<int64_t>());
-  LAUNCH(c, k_dp_groups, grid_for(std::max<int64_t>(N, D + 1), 256), 256, X, p.pos.as<int64_t>(), p.gslot_of.as<int32_t>(),
+  launch(c, c->stream, k_dp_groups, grid_for(std::max<int64_t>(N, D + 1), 256), 256, 0, X, p.pos.as<int64_t>(), p.gslot_of.as<int32_t>(),
          p.group_id.as<int32_t>(), p.group_slot.as<int32_t>(), p.group_off.as<int64_t>());
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(out->group_off, p.group_off.p, sizeof(int64_t) * size_t(D + 1), cudaMemcpyDeviceToHost, s));
@@ -4317,17 +4261,15 @@ __global__ void __launch_bounds__(128) k_host_job(int32_t n_distros, const int64
 }
 
 int evg_host_job(evg_ctx* c, const evg_host_job_cfg* cfg, const int32_t* spawned, evg_host_job_out* out) {
-  if (!c) return fail(EVG_ERR_INVALID, "null context");
-  LOCK(c);
+  ENTER(c, "evg_host_job");
   if (!cfg || !out || !out->n_hosts || !out->n_hosts_free || !out->status || !out->report)
     return fail(EVG_ERR_INVALID, "evg_host_job: null cfg or output");
-  if (const int rc = need_tick(c, "evg_host_job", Need::kAllocated); rc != EVG_OK) return rc;
+  if (const int rc = need_tick(c, who, Need::kAllocated); rc != EVG_OK) return rc;
   const int32_t D = c->Dn;
   for (int32_t d = 0; d < D; d++)
     if (cfg[d].n_provisioning < 0) return fail(EVG_ERR_INVALID, "evg_host_job: cfg[%d].n_provisioning is negative", d);
   c->launches = 0;
   if (D == 0) return EVG_OK;
-  CK(cudaSetDevice(c->device));
   cudaStream_t s = c->stream;
   auto& h = c->hj;
   UP(s, h.cfg, cfg, D, evg_host_job_cfg);
@@ -4338,7 +4280,7 @@ int evg_host_job(evg_ctx* c, const evg_host_job_cfg* cfg, const int32_t* spawned
   int64_t* nh = reinterpret_cast<int64_t*>(rep + D);
   int64_t* nf = nh + D;
   int32_t* st = reinterpret_cast<int32_t*>(nf + D);
-  LAUNCH(c, k_host_job, grid_for(D, 128), 128, D, c->b_groupoff.as<int64_t>(), c->b_hostoff.as<int64_t>(), c->b_qinfo.as<evg_queue_info>(),
+  launch(c, c->stream, k_host_job, grid_for(D, 128), 128, 0, D, c->b_groupoff.as<int64_t>(), c->b_hostoff.as<int64_t>(), c->b_qinfo.as<evg_queue_info>(),
          c->b_ginfo.as<evg_group_info>(), c->result_ptr(), c->b_status.as<int32_t>(), c->b_acfg.as<evg_alloc_cfg>(),
          h.cfg.as<evg_host_job_cfg>(), spawned ? h.spawned.as<int32_t>() : nullptr, nh, nf, st, rep);
   CK(cudaGetLastError());
@@ -4352,6 +4294,7 @@ int evg_host_job(evg_ctx* c, const evg_host_job_cfg* cfg, const int32_t* spawned
 
 int evg_plan_distro(evg_ctx* c, const evg_task_soa* tasks, const evg_distro_cfg* cfg, int32_t n_groups,
                     const int32_t* group_max_hosts, int64_t now_ns, uint32_t opts, evg_plan_out* out) {
+  ENTER(c, "evg_plan_distro");
   if (!tasks || !cfg) return fail(EVG_ERR_INVALID, "evg_plan_distro: null argument");
   int64_t task_off[2] = {0, tasks->n_tasks};
   int64_t group_off[2] = {0, n_groups};
@@ -4363,6 +4306,7 @@ int evg_plan_distro(evg_ctx* c, const evg_task_soa* tasks, const evg_distro_cfg*
 
 int evg_alloc_distro(evg_ctx* c, const evg_host_soa* hosts, const evg_alloc_cfg* cfg, const evg_queue_info* info,
                      evg_group_info* groups, int32_t n_groups, int64_t now_ns, evg_alloc_result* result, int32_t* status) {
+  ENTER(c, "evg_alloc_distro");
   if (!hosts || !cfg || !info) return fail(EVG_ERR_INVALID, "evg_alloc_distro: null argument");
   int64_t host_off[2] = {0, hosts->n_hosts};
   int64_t group_off[2] = {0, n_groups};

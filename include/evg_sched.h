@@ -374,7 +374,13 @@ void* evg_device_result_ptr(evg_ctx* ctx);
  * caller-owned DEVICE buffer (e.g. the NCCL send buffer of the all-gather),
  * `capacity` rows long; NULL restores the context-owned buffer. */
 int evg_bind_result_buffer(evg_ctx* ctx, void* device_ptr, int64_t capacity);
-/* Number of kernel launches issued by the last evg_run_resident. */
+/* Number of kernels the context launched since the last call that reset the count; 0 for a NULL ctx.  These calls
+ * reset it to 0 before their first launch: evg_run_resident (so evg_plan_batch, evg_plan_distro and the
+ * evg_plan_and_alloc_batch it runs), evg_plan_and_alloc_batch's pipelined large ticks, evg_alloc_batch / evg_alloc_distro,
+ * evg_deps_met_batch, evg_find_runnable_batch / _ex, evg_plan_from_finder / _ex, evg_edit_tasks, evg_plan_aliases,
+ * evg_expected_durations_batch, evg_prioritize_legacy_batch, evg_dag_rebuild_batch, evg_rebuild_dispatchers and
+ * evg_host_job.  Every other call adds the kernels it launches: the uploads (their range check), evg_update_tasks,
+ * evg_download_queue and evg_resolve_durations. */
 int64_t evg_last_launch_count(evg_ctx* ctx);
 /* Device time in ms of the last evg_run_resident, from CUDA events on the context
  * stream (valid after a sync / download): total_ms spans the whole tick; sort_ms is
