@@ -231,6 +231,36 @@ class HostJobOutStruct(C.Structure):
     _fields_ = [("n_hosts", C.c_void_p), ("n_hosts_free", C.c_void_p), ("status", C.c_void_p), ("report", C.c_void_p)]
 
 
+# the idle-host table of evg_host_drawdown / evg_idle_hosts
+(EVG_IH_RUNNING_TASK_GROUP, EVG_IH_LAST_TASK, EVG_IH_STATUS_RUNNING, EVG_IH_USER_DATA, EVG_IH_LEGACY_BOOTSTRAP,
+ EVG_IH_NEEDS_NEW_AGENT, EVG_IH_NEEDS_NEW_AGENT_MONITOR, EVG_IH_OUTDATED_AMI, EVG_IH_SINGLE_HOST_TASK_GROUP,
+ EVG_IH_TASK_LOOKUP_FAILED, EVG_IH_PAYMENT_NOT_DUE, EVG_IH_CLOUD_MANAGER_FAILED) = (1 << k for k in range(12))
+(EVG_HT_NOT_CHECKED, EVG_HT_KEPT, EVG_HT_EXEMPT_AGENT, EVG_HT_EXEMPT_PAYMENT, EVG_HT_ERR_CLOUD_MANAGER, EVG_HT_ERR_TASK_LOOKUP,
+ EVG_HT_DECOMMISSION, EVG_HT_TERM_OUTDATED_AMI, EVG_HT_TERM_COMMUNICATION, EVG_HT_TERM_IDLE, EVG_HT_TERM_TEARDOWN) = range(11)
+EVG_NO_DRAWDOWN = -(2 ** 63)
+IDLE_HOST_COLUMNS = ("creation_ns", "start_ns", "provision_ns", "agent_start_ns", "last_communication_ns",
+                     "last_task_completed_ns", "teardown_start_ns", "acceptable_idle_ns")
+HOST_VERDICT_DTYPE = np.dtype([("idle_ns", "<i8"), ("communication_ns", "<i8"), ("threshold_ns", "<i8"),
+                               ("since_teardown_ns", "<i8"), ("decision", "<i4"), ("_reserved", "<i4")])
+DRAWDOWN_DISTRO_DTYPE = np.dtype([("target", "<i8"), ("decommissioned", "<i8"), ("ran", "<i4"), ("_reserved", "<i4")])
+IDLE_CFG_DTYPE = np.dtype([("minimum_hosts", "<i8"), ("running_hosts_count", "<i8"), ("acceptable_idle_ns", "<i8")])
+IDLE_DISTRO_DTYPE = np.dtype([("min_evaluate", "<i8"), ("terminated", "<i8")])
+assert (HOST_VERDICT_DTYPE.itemsize, DRAWDOWN_DISTRO_DTYPE.itemsize, IDLE_CFG_DTYPE.itemsize, IDLE_DISTRO_DTYPE.itemsize) == (40, 24, 24, 16)
+
+
+class IdleHostSoAStruct(C.Structure):
+    _fields_ = [("n_hosts", C.c_int64), ("n_distros", C.c_int32), ("_reserved", C.c_int32)] + [
+        (f, C.c_void_p) for f in IDLE_HOST_COLUMNS + ("flags",)]
+
+
+class DrawdownInStruct(C.Structure):
+    _fields_ = [("existing_hosts", C.c_void_p), ("new_cap_target", C.c_void_p), ("queue_length_dm", C.c_void_p)]
+
+
+class HostTermOutStruct(C.Structure):  # evg_host_drawdown_out and evg_idle_hosts_out
+    _fields_ = [("hosts", C.c_void_p), ("distros", C.c_void_p)]
+
+
 class EvgError(RuntimeError):
     def __init__(self, code: int, msg: str):
         super().__init__(f"libevgsched error {code}: {msg}")
@@ -279,6 +309,8 @@ SYMBOLS = {
     "evg_dag_rebuild_batch": (C.c_int, [_P, _P, _P, _P, C.c_int32, _P, _P, _P, _P, _P]),
     "evg_rebuild_dispatchers": (C.c_int, [_P, C.c_int32, C.c_int64, C.c_int64, _P]),
     "evg_host_job": (C.c_int, [_P, _P, _P, _P]),
+    "evg_host_drawdown": (C.c_int, [_P, _P, _P, _P, C.c_int64, _P]),
+    "evg_idle_hosts": (C.c_int, [_P, _P, _P, _P, C.c_int64, _P]),
     "evg_plan_distro": (C.c_int, [_P, _P, _P, C.c_int32, _P, C.c_int64, C.c_uint32, _P]),
     "evg_alloc_distro": (C.c_int, [_P, _P, _P, _P, _P, C.c_int32, C.c_int64, _P, _P]),
 }

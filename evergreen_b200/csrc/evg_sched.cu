@@ -1282,8 +1282,9 @@ struct evg_ctx {
   // The resident tick (need_tick checks it; upload_tasks and drop_tick replace it), and whether the allocator's tables,
   // evg_upload_with_deps' verdicts (`deps`), evg_plan_aliases' map (`al`) and evg_resolve_durations' results (`dur`)
   // belong to it.  `allocated`: run state -- the allocator's results (queue and group infos, result rows, status) are
-  // from a run on this tick, into the result buffer bound now; evg_host_job reads them.
-  struct { Tick kind = Tick::kNone; bool hosts = false, deps = false, aliases = false, durations = false, allocated = false; } tick;
+  // from a run on this tick, into the result buffer bound now; evg_host_job reads them.  `host_job`: run state --
+  // evg_host_job's reports in hj.out are from the current run; a chained evg_host_drawdown reads them.
+  struct { Tick kind = Tick::kNone; bool hosts = false, deps = false, aliases = false, durations = false, allocated = false, host_job = false; } tick;
   int64_t T = 0, E = 0, G = 0, H = 0, U = 0, NT = 0, t_pad = 0;
   int32_t Dn = 0;
   int any_complex = 0;
@@ -1341,6 +1342,9 @@ struct evg_ctx {
   } dp;
   // evg_host_job (the first call allocates these): the staged job settings and spawned counts, and the outputs
   struct { DevBuf cfg, spawned, out; } hj;
+  // evg_host_drawdown / evg_idle_hosts (the first call allocates these): the staged idle-host table, its offsets and the
+  // per-distro inputs, the verdicts, the decided flags and their scan, and the per-distro outputs
+  struct { DevBuf cols, off, din, verdict, flag, pos, scan_sum, dout; } ih;
   DevBuf b_err;
   DevBuf b_route, b_unitv, b_unita, b_unitn, b_unitmask;
   DevBuf b_punt, b_puntcnt;
@@ -1406,7 +1410,7 @@ void drop_tick(evg_ctx* c) { c->tick = {}; }
 
 // What a call needs of the resident tick.  EVG_ERR_STATE names the call and the first unmet condition: a tick, then
 // its kind, then the state the call reads.
-enum class Need { kTick, kOwnColumns, kEditable, kHosts, kVerdicts, kAliasMap, kDurations, kAllocated };
+enum class Need { kTick, kOwnColumns, kEditable, kHosts, kVerdicts, kAliasMap, kDurations, kAllocated, kHostJob };
 int need_tick(const evg_ctx* c, const char* who, Need what) {
   const auto& t = c->tick;
   const bool own = what == Need::kOwnColumns || what == Need::kEditable;
@@ -1417,7 +1421,8 @@ int need_tick(const evg_ctx* c, const char* who, Need what) {
                       : what == Need::kAllocated && !t.allocated          ? "no allocator run on the resident tick since it was set or a result buffer was bound"
                       : what == Need::kVerdicts && !t.deps                ? "the resident tick was not uploaded with evg_upload_with_deps"
                       : what == Need::kAliasMap && !t.aliases             ? "the resident tick was not built by evg_plan_aliases"
-                      : what == Need::kDurations && !t.durations          ? "no evg_resolve_durations on the resident tick's rows" : nullptr;
+                      : what == Need::kDurations && !t.durations          ? "no evg_resolve_durations on the resident tick's rows"
+                      : what == Need::kHostJob && !t.host_job             ? "no evg_host_job on the resident tick's current run" : nullptr;
   return unmet ? fail(EVG_ERR_STATE, "%s: %s", who, unmet) : EVG_OK;
 }
 
@@ -2144,7 +2149,7 @@ int evg_run_resident(evg_ctx* c, int64_t now_ns, uint32_t opts) {
   c->launches = 0;
   c->timed = true;
   c->general_timed = false;
-  c->tick.allocated = false;
+  c->tick.allocated = c->tick.host_job = false;
   CK(cudaEventRecord(c->ev_begin, c->stream));
   int rc = run_plan(c, now_ns, opts);
   if (rc != EVG_OK) return rc;
@@ -2242,7 +2247,7 @@ int evg_bind_result_buffer(evg_ctx* c, void* device_ptr, int64_t capacity) {
   if (device_ptr && capacity < 0) return fail(EVG_ERR_INVALID, "negative capacity");
   c->ext_result = reinterpret_cast<evg_alloc_result*>(device_ptr);
   c->ext_capacity = device_ptr ? capacity : 0;
-  c->tick.allocated = false;  // the last run's result rows are not in the buffer bound now
+  c->tick.allocated = c->tick.host_job = false;  // the last run's result rows are not in the buffer bound now
   return EVG_OK;
 }
 int evg_last_timing_ms(evg_ctx* c, float* total_ms, float* sort_ms) {
@@ -4269,7 +4274,8 @@ int evg_host_job(evg_ctx* c, const evg_host_job_cfg* cfg, const int32_t* spawned
   for (int32_t d = 0; d < D; d++)
     if (cfg[d].n_provisioning < 0) return fail(EVG_ERR_INVALID, "evg_host_job: cfg[%d].n_provisioning is negative", d);
   c->launches = 0;
-  if (D == 0) return EVG_OK;
+  c->tick.host_job = false;  // until the reports below are written
+  if (D == 0) return c->tick.host_job = true, EVG_OK;
   cudaStream_t s = c->stream;
   auto& h = c->hj;
   UP(s, h.cfg, cfg, D, evg_host_job_cfg);
@@ -4289,7 +4295,290 @@ int evg_host_job(evg_ctx* c, const evg_host_job_cfg* cfg, const int32_t* spawned
   CK(cudaMemcpyAsync(out->n_hosts_free, nf, sizeof(int64_t) * size_t(D), cudaMemcpyDeviceToHost, s));
   CK(cudaMemcpyAsync(out->status, st, sizeof(int32_t) * size_t(D), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));  // the caller's cfg / spawned arrays are free again and the outputs are written
+  c->tick.host_job = true;
   return EVG_OK;
+}
+
+// ---- host termination: the drawdown job and the idle-host job over one idle-host table ----
+
+constexpr int64_t kMaxTeardownGroup = 4 * kMinute;   // evergreen.MaxTeardownGroupThreshold (globals.go:348)
+constexpr int64_t kAgentUnresponsive = 5 * kMinute;  // MaxAgentUnresponsiveInterval = MaxAgentMonitorUnresponsiveInterval (host.go:624, 634)
+constexpr int64_t kWaitingForAgentCutoff = 10 * kMinute;  // idleWaitingForAgentCutoff (host_monitoring_idle_termination.go:24)
+
+struct DIdleHosts {  // evg_idle_host_soa staged on the device
+  const int64_t *creation, *start, *provision, *agent_start, *last_comm, *last_done, *teardown, *acceptable;
+  const uint32_t* flags;
+};
+
+// The host predicates both jobs share, for a row without a running task, at the frozen `now`.
+struct IdleHostRow {
+  int64_t idle, comm, since_td;
+  uint32_t f;
+  bool tearing, td_exceeded;
+  int32_t exempt;  // checkTerminationExemptions' outcome: an EVG_HT_* code, EVG_HT_NOT_CHECKED when none applies
+};
+__device__ __forceinline__ IdleHostRow idle_host_row(const DIdleHosts& h, int64_t i, int64_t now) {
+  IdleHostRow r;
+  r.f = h.flags[i];
+  const int64_t td = h.teardown[i], lc = h.last_comm[i], ct = h.creation[i], st = h.start[i];
+  r.tearing = td != EVG_TIME_ZERO;  // IsTearingDown (model/host/host.go:219-221)
+  r.since_td = since(now, td);
+  r.td_exceeded = r.since_td > kMaxTeardownGroup;  // TeardownTimeExceededMax (:2241-2243)
+  if (r.tearing) r.idle = r.td_exceeded ? r.since_td : 0;  // IdleTime (:671-706)
+  else if (r.f & EVG_IH_LAST_TASK) r.idle = since(now, h.last_done[i]);
+  else if (r.f & EVG_IH_USER_DATA) r.idle = h.agent_start[i] > 0 ? since(now, h.agent_start[i]) : 0;  // After(Unix 0)
+  else r.idle = (r.f & EVG_IH_STATUS_RUNNING) ? since(now, h.provision[i]) : 0;
+  if (r.tearing) r.comm = 0;  // GetElapsedCommunicationTime (:2220-2238)
+  else if (lc > ct) r.comm = since(now, lc);
+  else if (st > ct) r.comm = since(now, st);
+  else if (lc != EVG_TIME_ZERO) r.comm = since(now, lc);
+  else r.comm = since(now, ct);
+  const bool legacy = r.f & EVG_IH_LEGACY_BOOTSTRAP;  // IsWaitingForAgent (:2006-2026)
+  const int64_t cutoff = now < kI64Min + kAgentUnresponsive ? kI64Min : now - kAgentUnresponsive;
+  const bool waiting = (legacy && (r.f & EVG_IH_NEEDS_NEW_AGENT)) || (!legacy && (r.f & EVG_IH_NEEDS_NEW_AGENT_MONITOR)) ||
+                       lc == EVG_TIME_ZERO || lc == 0 || lc < cutoff;
+  // checkTerminationExemptions (units/host_monitoring_idle_termination.go:287-338) past its !IsEphemeral branch
+  r.exempt = waiting && (r.comm < kWaitingForAgentCutoff || r.idle < kWaitingForAgentCutoff) ? EVG_HT_EXEMPT_AGENT
+             : (r.f & EVG_IH_CLOUD_MANAGER_FAILED)                                          ? EVG_HT_ERR_CLOUD_MANAGER
+             : (r.f & EVG_IH_PAYMENT_NOT_DUE)                                                ? EVG_HT_EXEMPT_PAYMENT
+                                                                                             : EVG_HT_NOT_CHECKED;
+  return r;
+}
+
+// The drawdown job's inputs for distro d: its NewCapTarget (EVG_NO_DRAWDOWN: no job) and LengthWithDependenciesMet,
+// from the last evg_host_job's report and the tick's queue infos (chained, `rep` given) or from the caller's arrays.
+struct DrawdownSrc {
+  const evg_host_report* rep;
+  const evg_queue_info* qinfo;
+  const int64_t *cap, *qlen, *existing;
+};
+__device__ __forceinline__ int64_t dd_cap(const DrawdownSrc& s, int d) {
+  return s.rep ? (s.rep[d].drawdown ? s.rep[d].new_cap_target : EVG_NO_DRAWDOWN) : s.cap[d];
+}
+
+__device__ __forceinline__ void put_verdict(evg_host_verdict* __restrict__ v, int64_t i, const IdleHostRow& r, int64_t thr, int32_t code) {
+  evg_host_verdict o;
+  o.idle_ns = r.idle; o.communication_ns = r.comm; o.threshold_ns = thr; o.since_teardown_ns = r.since_td;
+  o.decision = code; o._reserved = 0;
+  v[i] = o;
+}
+
+// checkAndDecommission (units/host_drawdown.go:127-159) for every row of a distro with a drawdown job, as if the target
+// were not yet reached; decom[i] = 1 when the row would be decommissioned.  k_hd_cap applies the target.
+__global__ void __launch_bounds__(256) k_hd_host(int64_t n, int32_t D, const int64_t* __restrict__ off, DIdleHosts h, DrawdownSrc s,
+                                                 int64_t now, evg_host_verdict* __restrict__ verdict, int32_t* __restrict__ decom) {
+  const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  const int d = block_find_distro(off, D, i, n);
+  if (d < 0) return;
+  decom[i] = 0;
+  if (dd_cap(s, d) == EVG_NO_DRAWDOWN) { verdict[i] = evg_host_verdict{}; return; }
+  const IdleHostRow r = idle_host_row(h, i, now);
+  int64_t thr = 0;
+  int32_t code;
+  if (r.exempt != EVG_HT_NOT_CHECKED) code = r.exempt;                       // :128-131
+  else if (r.tearing && !r.td_exceeded) code = EVG_HT_KEPT;                  // :134-136
+  else if (r.f & EVG_IH_TASK_LOOKUP_FAILED) code = EVG_HT_ERR_TASK_LOOKUP;   // :139-142
+  else if (r.f & EVG_IH_SINGLE_HOST_TASK_GROUP) code = EVG_HT_KEPT;          // :143-145
+  else {                                                                     // :147-158
+    const int64_t qlen = s.rep ? s.qinfo[d].length_with_dependencies_met : s.qlen[d];
+    thr = (r.f & EVG_IH_RUNNING_TASK_GROUP) ? 10 * kMinute : 5 * kSecond;
+    if (h.last_done[i] != EVG_TIME_ZERO && qlen > 0) thr = h.acceptable[i];
+    code = r.idle > thr ? EVG_HT_DECOMMISSION : EVG_HT_KEPT;
+  }
+  put_verdict(verdict, i, r, thr, code);
+  decom[i] = code == EVG_HT_DECOMMISSION;
+}
+
+// The loop stops before any row once the target is <= 0 and the target drops only on a decommission (:93-97, :149-151):
+// a row is checked iff fewer than `target` rows before it in its distro would be decommissioned (pos: their exclusive
+// scan over the whole table).  Rows past that point get no decision.
+__global__ void __launch_bounds__(256) k_hd_cap(int64_t n, int32_t D, const int64_t* __restrict__ off, DrawdownSrc s,
+                                                const int64_t* __restrict__ pos, evg_host_verdict* __restrict__ verdict) {
+  const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  const int d = block_find_distro(off, D, i, n);
+  if (d < 0) return;
+  const int64_t cap = dd_cap(s, d);
+  if (cap != EVG_NO_DRAWDOWN && pos[i] - pos[off[d]] >= wsub(s.existing[d], cap)) verdict[i] = evg_host_verdict{};
+}
+
+__global__ void __launch_bounds__(256) k_hd_distro(int32_t D, const int64_t* __restrict__ off, DrawdownSrc s, const int64_t* __restrict__ pos,
+                                                   evg_drawdown_distro* __restrict__ out) {
+  const int d = int(blockIdx.x * blockDim.x + threadIdx.x);
+  if (d >= D) return;
+  const int64_t cap = dd_cap(s, d);
+  evg_drawdown_distro o{};
+  if (cap != EVG_NO_DRAWDOWN) {
+    o.ran = 1;
+    o.target = wsub(s.existing[d], cap);  // :91
+    const int64_t would = pos ? pos[off[d + 1]] - pos[off[d]] : 0;
+    o.decommissioned = o.target <= 0 ? 0 : (would < o.target ? would : o.target);
+  }
+  out[d] = o;
+}
+
+// idleHostJob.Run's loop (units/host_monitoring_idle_termination.go:128-140), checkAndTerminateHost (:158-180),
+// getIdleInfo (:194-226) and getTerminationReason (:258-283) per row; term[i] = 1 when the row is terminated.
+__global__ void __launch_bounds__(256) k_idle_host(int64_t n, int32_t D, const int64_t* __restrict__ off, DIdleHosts h,
+                                                   const evg_idle_cfg* __restrict__ cfg, int64_t now,
+                                                   evg_host_verdict* __restrict__ verdict, int32_t* __restrict__ term) {
+  const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  const int d = block_find_distro(off, D, i, n);
+  if (d < 0) return;
+  term[i] = 0;
+  const evg_idle_cfg c = cfg[d];
+  const int64_t n_idle = off[d + 1] - off[d], room = c.running_hosts_count - c.minimum_hosts;
+  const int64_t min_eval = room <= 0 ? 0 : (room < n_idle ? room : n_idle);  // getMinNumHostsToEvaluate (:143-156)
+  const uint32_t f = h.flags[i];
+  if (i - off[d] >= min_eval && !(f & EVG_IH_OUTDATED_AMI)) { verdict[i] = evg_host_verdict{}; return; }
+  const IdleHostRow r = idle_host_row(h, i, now);
+  int64_t thr = 0;
+  int32_t code;
+  if (r.exempt != EVG_HT_NOT_CHECKED) code = r.exempt;                      // :160-163
+  else if (f & EVG_IH_TASK_LOOKUP_FAILED) code = EVG_HT_ERR_TASK_LOOKUP;    // :209-212
+  else {
+    const bool single = f & EVG_IH_SINGLE_HOST_TASK_GROUP;
+    thr = single ? 5 * kMinute : (f & EVG_IH_RUNNING_TASK_GROUP) ? wadd(c.acceptable_idle_ns, c.acceptable_idle_ns) : c.acceptable_idle_ns;
+    code = (f & EVG_IH_OUTDATED_AMI) && r.idle > 0 && !single ? EVG_HT_TERM_OUTDATED_AMI
+           : r.comm >= thr && !r.tearing                       ? EVG_HT_TERM_COMMUNICATION
+           : r.idle > 0 && r.idle >= thr                       ? EVG_HT_TERM_IDLE
+           : r.since_td > kMaxTeardownGroup && r.tearing       ? EVG_HT_TERM_TEARDOWN
+                                                               : EVG_HT_KEPT;
+  }
+  put_verdict(verdict, i, r, thr, code);
+  term[i] = code >= EVG_HT_TERM_OUTDATED_AMI;
+}
+
+__global__ void __launch_bounds__(256) k_idle_distro(int32_t D, const int64_t* __restrict__ off, const evg_idle_cfg* __restrict__ cfg,
+                                                     const int64_t* __restrict__ pos, evg_idle_distro* __restrict__ out) {
+  const int d = int(blockIdx.x * blockDim.x + threadIdx.x);
+  if (d >= D) return;
+  const int64_t n_idle = off[d + 1] - off[d], room = cfg[d].running_hosts_count - cfg[d].minimum_hosts;
+  evg_idle_distro o;
+  o.min_evaluate = room <= 0 ? 0 : (room < n_idle ? room : n_idle);
+  o.terminated = pos ? pos[off[d + 1]] - pos[off[d]] : 0;
+  out[d] = o;
+}
+
+// The idle-host table and its offsets, checked before anything is staged or launched.
+static int check_idle_hosts(const char* who, const evg_idle_host_soa* t, const int64_t* off) {
+  if (!t || !off) return fail(EVG_ERR_INVALID, "%s: null host table or idle_off", who);
+  if (t->n_hosts < 0 || t->n_distros < 0) return fail(EVG_ERR_INVALID, "%s: negative n_hosts or n_distros", who);
+  if (t->n_hosts > 0 && (!t->creation_ns || !t->start_ns || !t->provision_ns || !t->agent_start_ns || !t->last_communication_ns ||
+                         !t->last_task_completed_ns || !t->teardown_start_ns || !t->acceptable_idle_ns || !t->flags))
+    return fail(EVG_ERR_INVALID, "%s: null host column", who);
+  return check_offsets(off, t->n_distros, t->n_hosts, who, "idle_off");
+}
+
+// Stage the table's columns, its offsets and `per_distro_bytes` of per-distro input into ih, and size the outputs and
+// the scan.  Returns the device view in `v`.
+static int stage_idle_hosts(evg_ctx* c, const evg_idle_host_soa* t, const int64_t* off, const void* per_distro, size_t per_distro_bytes,
+                            DIdleHosts* v) {
+  auto& x = c->ih;
+  const int64_t H = t->n_hosts;
+  const int32_t D = t->n_distros;
+  cudaStream_t s = c->stream;
+  CK(x.cols.ensure((8 * sizeof(int64_t) + sizeof(uint32_t)) * size_t(H > 0 ? H : 1)));
+  const int64_t* src[8] = {t->creation_ns, t->start_ns, t->provision_ns, t->agent_start_ns, t->last_communication_ns,
+                           t->last_task_completed_ns, t->teardown_start_ns, t->acceptable_idle_ns};
+  int64_t* col = x.cols.as<int64_t>();
+  const int64_t* dcol[8];
+  for (int k = 0; k < 8; k++) {
+    dcol[k] = col + k * H;
+    if (H > 0) CK(cudaMemcpyAsync(col + k * H, src[k], sizeof(int64_t) * size_t(H), cudaMemcpyHostToDevice, s));
+  }
+  uint32_t* flags = reinterpret_cast<uint32_t*>(col + 8 * H);
+  if (H > 0) CK(cudaMemcpyAsync(flags, t->flags, sizeof(uint32_t) * size_t(H), cudaMemcpyHostToDevice, s));
+  UP(s, x.off, off, D + 1, int64_t);
+  CK(x.din.ensure(per_distro_bytes > 0 ? per_distro_bytes : 1));
+  if (per_distro_bytes > 0) CK(cudaMemcpyAsync(x.din.p, per_distro, per_distro_bytes, cudaMemcpyHostToDevice, s));
+  CK(x.verdict.ensure(sizeof(evg_host_verdict) * size_t(H > 0 ? H : 1)));
+  CK(x.flag.ensure(sizeof(int32_t) * size_t(H > 0 ? H : 1)));
+  CK(x.pos.ensure(sizeof(int64_t) * size_t(H + 1)));
+  CK(x.scan_sum.ensure(sizeof(int64_t) * size_t((H + 1023) / 1024 + 1)));
+  *v = DIdleHosts{dcol[0], dcol[1], dcol[2], dcol[3], dcol[4], dcol[5], dcol[6], dcol[7], flags};
+  return EVG_OK;
+}
+
+// Scan the decided flags (none: pos stays NULL), copy the verdicts and `dout_bytes` of per-distro output back, wait.
+static int finish_idle_hosts(evg_ctx* c, int64_t H, evg_host_verdict* verdicts, void* dout, size_t dout_bytes) {
+  auto& x = c->ih;
+  cudaStream_t s = c->stream;
+  CK(cudaGetLastError());
+  if (H > 0) CK(cudaMemcpyAsync(verdicts, x.verdict.p, sizeof(evg_host_verdict) * size_t(H), cudaMemcpyDeviceToHost, s));
+  if (dout_bytes > 0) CK(cudaMemcpyAsync(dout, x.dout.p, dout_bytes, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));  // the caller's arrays are free again and the outputs are written
+  return EVG_OK;
+}
+
+int evg_host_drawdown(evg_ctx* c, const evg_idle_host_soa* hosts, const int64_t* idle_off, const evg_drawdown_in* in, int64_t now_ns,
+                      evg_host_drawdown_out* out) {
+  ENTER(c, "evg_host_drawdown");
+  int rc = check_idle_hosts(who, hosts, idle_off);
+  if (rc != EVG_OK) return rc;
+  const int64_t H = hosts->n_hosts;
+  const int32_t D = hosts->n_distros;
+  if (!in || !in->existing_hosts || !out || (H > 0 && !out->hosts) || (D > 0 && !out->distros))
+    return fail(EVG_ERR_INVALID, "%s: null input or output", who);
+  if (!in->new_cap_target != !in->queue_length_dm)
+    return fail(EVG_ERR_INVALID, "%s: new_cap_target and queue_length_dm must be both NULL (chained) or both given", who);
+  const bool chained = !in->new_cap_target;
+  for (int32_t d = 0; d < D; d++)
+    if (in->existing_hosts[d] < 0 || (!chained && in->queue_length_dm[d] < 0))
+      return fail(EVG_ERR_INVALID, "%s: distro %d has a negative existing_hosts or queue_length_dm", who, d);
+  if (chained) {
+    if ((rc = need_tick(c, who, Need::kTick)) != EVG_OK || (rc = need_tick(c, who, Need::kHostJob)) != EVG_OK) return rc;
+    if (D != c->Dn) return fail(EVG_ERR_INVALID, "%s: chained on a tick of %d distros, the host table has %d", who, c->Dn, D);
+  }
+  c->launches = 0;
+  // per-distro input: existing_hosts, then (standalone) new_cap_target and queue_length_dm
+  std::vector<int64_t> din(size_t(D) * (chained ? 1 : 3));
+  std::copy(in->existing_hosts, in->existing_hosts + D, din.begin());
+  if (!chained) {
+    std::copy(in->new_cap_target, in->new_cap_target + D, din.begin() + D);
+    std::copy(in->queue_length_dm, in->queue_length_dm + D, din.begin() + 2 * D);
+  }
+  DIdleHosts v;
+  if ((rc = stage_idle_hosts(c, hosts, idle_off, din.data(), din.size() * sizeof(int64_t), &v)) != EVG_OK) return rc;
+  auto& x = c->ih;
+  CK(x.dout.ensure(sizeof(evg_drawdown_distro) * size_t(D > 0 ? D : 1)));
+  const int64_t* dd = x.din.as<int64_t>();
+  const DrawdownSrc src{chained ? c->hj.out.as<evg_host_report>() : nullptr, chained ? c->b_qinfo.as<evg_queue_info>() : nullptr,
+                        chained ? nullptr : dd + D, chained ? nullptr : dd + 2 * D, dd};
+  const int64_t* off = x.off.as<int64_t>();
+  int64_t* pos = H > 0 ? x.pos.as<int64_t>() : nullptr;
+  launch(c, c->stream, k_hd_host, grid_for(H, 256), 256, 0, H, D, off, v, src, now_ns, x.verdict.as<evg_host_verdict>(), x.flag.as<int32_t>());
+  if (H > 0) {
+    scan_counts(c, x.flag.as<int32_t>(), H, pos, x.scan_sum.as<int64_t>());
+    launch(c, c->stream, k_hd_cap, grid_for(H, 256), 256, 0, H, D, off, src, static_cast<const int64_t*>(pos), x.verdict.as<evg_host_verdict>());
+  }
+  launch(c, c->stream, k_hd_distro, grid_for(D, 256), 256, 0, D, off, src, static_cast<const int64_t*>(pos), x.dout.as<evg_drawdown_distro>());
+  return finish_idle_hosts(c, H, out->hosts, out->distros, sizeof(evg_drawdown_distro) * size_t(D));
+}
+
+int evg_idle_hosts(evg_ctx* c, const evg_idle_host_soa* hosts, const int64_t* idle_off, const evg_idle_cfg* cfg, int64_t now_ns,
+                   evg_idle_hosts_out* out) {
+  ENTER(c, "evg_idle_hosts");
+  int rc = check_idle_hosts(who, hosts, idle_off);
+  if (rc != EVG_OK) return rc;
+  const int64_t H = hosts->n_hosts;
+  const int32_t D = hosts->n_distros;
+  if ((D > 0 && !cfg) || !out || (H > 0 && !out->hosts) || (D > 0 && !out->distros))
+    return fail(EVG_ERR_INVALID, "%s: null cfg or output", who);
+  for (int32_t d = 0; d < D; d++)
+    if (cfg[d].minimum_hosts < 0 || cfg[d].running_hosts_count < 0)
+      return fail(EVG_ERR_INVALID, "%s: cfg[%d] has a negative minimum_hosts or running_hosts_count", who, d);
+  c->launches = 0;
+  DIdleHosts v;
+  if ((rc = stage_idle_hosts(c, hosts, idle_off, cfg, sizeof(evg_idle_cfg) * size_t(D), &v)) != EVG_OK) return rc;
+  auto& x = c->ih;
+  CK(x.dout.ensure(sizeof(evg_idle_distro) * size_t(D > 0 ? D : 1)));
+  const int64_t* off = x.off.as<int64_t>();
+  const evg_idle_cfg* dcfg = x.din.as<evg_idle_cfg>();
+  int64_t* pos = H > 0 ? x.pos.as<int64_t>() : nullptr;
+  launch(c, c->stream, k_idle_host, grid_for(H, 256), 256, 0, H, D, off, v, dcfg, now_ns, x.verdict.as<evg_host_verdict>(), x.flag.as<int32_t>());
+  if (H > 0) scan_counts(c, x.flag.as<int32_t>(), H, pos, x.scan_sum.as<int64_t>());
+  launch(c, c->stream, k_idle_distro, grid_for(D, 256), 256, 0, D, off, dcfg, static_cast<const int64_t*>(pos), x.dout.as<evg_idle_distro>());
+  return finish_idle_hosts(c, H, out->hosts, out->distros, sizeof(evg_idle_distro) * size_t(D));
 }
 
 int evg_plan_distro(evg_ctx* c, const evg_task_soa* tasks, const evg_distro_cfg* cfg, int32_t n_groups,

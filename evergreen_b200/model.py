@@ -14,7 +14,7 @@ zero ``time.Time`` (year 1).  Durations are int nanoseconds (``time.Duration``).
 from __future__ import annotations
 
 from dataclasses import dataclass, field
-from typing import List, Optional
+from typing import List, Optional, Tuple
 
 ZERO_TIME = -(2 ** 63)
 
@@ -72,6 +72,10 @@ PERSISTED_QUEUE_CAP = 10000
 TASK_QUEUES_COLLECTION = "task_queues"
 TASK_SECONDARY_QUEUES_COLLECTION = "task_alias_queues"
 DISABLED_TASK_PRIORITY = -1  # globals.go:187
+HOST_RUNNING = "running"  # globals.go:24
+# model/distro/distro.go:319-321
+BOOTSTRAP_METHOD_LEGACY_SSH = "legacy-ssh"
+BOOTSTRAP_METHOD_USER_DATA = "user-data"
 
 
 def is_github_merge_queue_requester(r: str) -> bool:  # globals.go:1195-1197
@@ -231,6 +235,7 @@ class Distro:
     valid_projects: List[str] = field(default_factory=list)
     aliases: List[str] = field(default_factory=list)  # Distro.Aliases (FindApplicableDistroIDs, model/distro/aliases.go:14-27)
     arch: str = ""  # Distro.Arch (cloud.UsesHourlyBilling reads it, cloud/ec2_util.go:256-268)
+    default_ami: str = ""  # Distro.GetDefaultAMI() (model/distro/distro.go:112-127)
 
     def max_duration_per_host(self) -> int:  # distro.go:422-432
         if self.container_pool != "":
@@ -255,6 +260,26 @@ class Host:  # model/host/host.go:38-...
     running_task_project: str = ""
     running_task_version: str = ""
     task_group_teardown_start_time: int = ZERO_TIME
+    # what the drawdown and idle-host jobs read (units/host_drawdown.go, units/host_monitoring_idle_termination.go)
+    status: str = ""
+    creation_time: int = ZERO_TIME
+    start_time: int = ZERO_TIME
+    provision_time: int = ZERO_TIME
+    agent_start_time: int = ZERO_TIME
+    last_communication_time: int = ZERO_TIME
+    last_task_completed_time: int = ZERO_TIME
+    last_task: str = ""
+    last_group: str = ""
+    needs_new_agent: bool = False
+    needs_new_agent_monitor: bool = False
+    bootstrap_method: str = ""           # h.Distro.BootstrapSettings.Method (the embedded distro document)
+    acceptable_host_idle_time: int = 0   # h.Distro.HostAllocatorSettings.AcceptableHostIdleTime
+    ami: str = ""                        # h.GetAMI()
+    # resolved lookups the jobs perform against MongoDB and the cloud provider
+    last_task_single_host_task_group: Optional[bool] = False  # the last task IsPartOfSingleHostTaskGroup and succeeded;
+                                                               # None: task.FindOneId failed or found nothing
+    time_til_next_payment: int = 0       # manager.TimeTilNextPayment(h)
+    cloud_manager_error: bool = False    # cloud.GetManagerOptions / GetManager returned an error
 
     def is_free(self) -> bool:  # host.go:214-221
         return self.running_task == "" and self.task_group_teardown_start_time == ZERO_TIME
@@ -405,6 +430,70 @@ class HostAllocatorJobReport:
 class DrawdownInfo:  # units/host_drawdown.go:33-36
     distro_id: str = ""
     new_cap_target: int = 0
+
+
+@dataclass
+class HostDrawdownJob:
+    """What hostDrawdownJob.Run does for one distro (units/host_drawdown.go:70-118): the hosts it decommissions, in
+    order, the errors it logs per host, and the counts of its closing log line."""
+    distro_id: str = ""
+    new_cap_target: int = 0
+    existing_host_count: int = 0
+    num_idle_hosts: int = 0
+    drawdown_target: int = 0
+    decommissioned_hosts: List[str] = field(default_factory=list)
+    errors: List[Tuple[str, str]] = field(default_factory=list)  # (host id, what failed)
+
+    @property
+    def decommissioned(self) -> int:
+        return len(self.decommissioned_hosts)
+
+
+@dataclass
+class IdleHostJob:
+    """What idleHostJob.Run does for one distro (units/host_monitoring_idle_termination.go:128-140): the hosts it
+    terminates with getTerminationReason's reason, in order, the errors it adds per host, and its counts."""
+    distro_id: str = ""
+    num_idle_hosts: int = 0
+    min_hosts_to_evaluate: int = 0
+    terminated_hosts: List[str] = field(default_factory=list)
+    reasons: List[str] = field(default_factory=list)
+    errors: List[Tuple[str, str]] = field(default_factory=list)
+
+    @property
+    def terminated(self) -> int:
+        return len(self.terminated_hosts)
+
+
+def _frac(u: int, prec: int) -> Tuple[int, str]:  # time.fmtFrac
+    q, r = divmod(u, 10 ** prec)
+    digits = f"{r:0{prec}d}".rstrip("0") if prec else ""
+    return q, "." + digits if digits else ""
+
+
+def go_duration_string(d: int) -> str:
+    """time.Duration.String (go/src/time/time.go): "72h3m0.5s", "1.5µs", "0s"."""
+    u = -d if d < 0 else d
+    if u == 0:
+        return "0s"
+    if u < SECOND:
+        if u < MICROSECOND:
+            prec, unit = 0, "ns"
+        elif u < MILLISECOND:
+            prec, unit = 3, "µs"
+        else:
+            prec, unit = 6, "ms"
+        q, frac = _frac(u, prec)
+        text = f"{q}{frac}{unit}"
+    else:
+        secs, frac = _frac(u, 9)
+        text = f"{secs % 60}{frac}s"
+        mins = secs // 60
+        if mins > 0:
+            text = f"{mins % 60}m" + text
+            if mins // 60 > 0:
+                text = f"{mins // 60}h" + text
+    return "-" + text if d < 0 else text
 
 
 def fetch_expected_duration(t: Task, now: int, history=None):

@@ -433,6 +433,36 @@ class Engine:
         L.check(self.lib.evg_host_job(self.ctx, L.ptr(cfg_arg), L.ptr(sp) if sp is not None and D else None, C.byref(st)))
         return {k: v[:D] for k, v in o.items()}
 
+    def host_drawdown(self, table: S.IdleHostTable, existing_hosts, now: int, new_cap_target=None, queue_length_dm=None) -> dict:
+        """evg_host_drawdown: hostDrawdownJob.Run for every distro of `table`, on the device.  `new_cap_target` (int64,
+        EVG_NO_DRAWDOWN = no job) and `queue_length_dm` both None: chained on the resident tick's last host_job, whose
+        distros are the table's.  -> dict of hosts (HOST_VERDICT rows) and distros (DRAWDOWN_DISTRO rows)."""
+        D, H = table.n_distros, table.n_hosts
+        if (new_cap_target is None) != (queue_length_dm is None):
+            raise ValueError("new_cap_target and queue_length_dm: both or neither")
+        arrs = [None if a is None else np.ascontiguousarray(a, dtype=np.int64) for a in (existing_hosts, new_cap_target, queue_length_dm)]
+        if any(a is not None and a.shape != (D,) for a in arrs):
+            raise ValueError("one existing count, cap and queue length per distro of the table")
+        arrs = [None if a is None else (a if D else np.zeros(1, np.int64)) for a in arrs]
+        o = {"hosts": np.zeros(max(H, 1), L.HOST_VERDICT_DTYPE), "distros": np.zeros(max(D, 1), L.DRAWDOWN_DISTRO_DTYPE)}
+        ins = L.DrawdownInStruct(*[L.ptr(a) for a in arrs])
+        st = L.HostTermOutStruct(L.ptr(o["hosts"]), L.ptr(o["distros"]))
+        L.check(self.lib.evg_host_drawdown(self.ctx, C.byref(table.struct()), L.ptr(table.idle_off), C.byref(ins), int(now), C.byref(st)))
+        return {"hosts": o["hosts"][:H], "distros": o["distros"][:D]}
+
+    def idle_hosts(self, table: S.IdleHostTable, cfg: np.ndarray, now: int) -> dict:
+        """evg_idle_hosts: idleHostJob.Run for every distro of `table`, on the device.  `cfg`: IDLE_CFG rows.
+        -> dict of hosts (HOST_VERDICT rows) and distros (IDLE_DISTRO rows)."""
+        D, H = table.n_distros, table.n_hosts
+        cfg = np.ascontiguousarray(cfg, dtype=L.IDLE_CFG_DTYPE)
+        if cfg.shape != (D,):
+            raise ValueError("one setting per distro of the table")
+        o = {"hosts": np.zeros(max(H, 1), L.HOST_VERDICT_DTYPE), "distros": np.zeros(max(D, 1), L.IDLE_DISTRO_DTYPE)}
+        st = L.HostTermOutStruct(L.ptr(o["hosts"]), L.ptr(o["distros"]))
+        L.check(self.lib.evg_idle_hosts(self.ctx, C.byref(table.struct()), L.ptr(table.idle_off),
+                                        L.ptr(cfg if D else np.zeros(1, L.IDLE_CFG_DTYPE)), int(now), C.byref(st)))
+        return {"hosts": o["hosts"][:H], "distros": o["distros"][:D]}
+
     def alloc_batch(self, hosts: S.HostSoA, qinfo: np.ndarray, ginfo: np.ndarray, group_off: np.ndarray, now: int):
         D = int(qinfo.shape[0])
         ao = self._alloc_output(D)
@@ -823,6 +853,100 @@ def host_allocator_jobs(batch: Sequence[Tuple[M.Distro, List[M.Task], M.HostAllo
     eng.run(now)
     res = eng.host_job(S.marshal_host_job(datas, n_provisioning), None if spawned is None else np.asarray(spawned))
     return host_job_results([d for d, _, _ in batch], res)
+
+
+MAX_TEARDOWN_GROUP_THRESHOLD = 4 * M.MINUTE  # evergreen.MaxTeardownGroupThreshold (globals.go:348)
+
+
+def termination_reason(v) -> str:
+    """getTerminationReason's text (units/host_monitoring_idle_termination.go:258-283) for an EVG_HT_TERM_* verdict."""
+    ds = M.go_duration_string
+    code = int(v["decision"])
+    if code == L.EVG_HT_TERM_OUTDATED_AMI:
+        return "host has an outdated AMI"
+    if code == L.EVG_HT_TERM_COMMUNICATION:
+        return (f"host is idle or unreachable, communication time {ds(int(v['communication_ns']))} is over threshold time "
+                f"{ds(int(v['threshold_ns']))}")
+    if code == L.EVG_HT_TERM_IDLE:
+        return f"host is idle or unreachable, idle time {ds(int(v['idle_ns']))} is over threshold time {ds(int(v['threshold_ns']))}"
+    assert code == L.EVG_HT_TERM_TEARDOWN, code
+    return (f"time since the host's task group teardown start time {ds(int(v['since_teardown_ns']))} has exceeded the maximum "
+            f"teardown threshold {ds(MAX_TEARDOWN_GROUP_THRESHOLD)}")
+
+
+_HT_ERRORS = {L.EVG_HT_ERR_CLOUD_MANAGER: "getting cloud manager for host",  # what each job wraps its errors in
+              L.EVG_HT_ERR_TASK_LOOKUP: "checking if host is running single host task group"}  # host_drawdown.go:140
+_IDLE_ERRORS = dict(_HT_ERRORS)
+_IDLE_ERRORS[L.EVG_HT_ERR_TASK_LOOKUP] = "getting information on idle host"  # host_monitoring_idle_termination.go:170
+
+
+def host_drawdown_jobs(distro_ids: Sequence[str], idle_hosts: Sequence[Sequence[M.Host]], existing_host_counts: Sequence[int],
+                       now: int, *, drawdown: Optional[Sequence[Optional[M.DrawdownInfo]]] = None,
+                       queue_lengths: Optional[Sequence[int]] = None, engine: Optional[Engine] = None) -> list:
+    """hostDrawdownJob.Run (units/host_drawdown.go:70-159) for every distro on the device.  `idle_hosts[d]`: the
+    distro's IdleHostsWithDistroID, in order; `existing_host_counts[d]`: CountHostsCanOrWillRunTasksInDistro.
+    Standalone: `drawdown[d]` is the job's DrawdownInfo (None: no job) and `queue_lengths[d]` the distro's
+    LengthWithDependenciesMet.  Chained (both None): the drawdowns the engine's last host_allocator_jobs / host_job
+    decided, with the tick's queue lengths.  Returns a HostDrawdownJob per distro, None where no job ran."""
+    eng = engine or default_engine()
+    table = S.marshal_idle_hosts(idle_hosts)
+    cap = qlen = None
+    if drawdown is not None or queue_lengths is not None:
+        if drawdown is None or queue_lengths is None:
+            raise ValueError("drawdown and queue_lengths: both or neither")
+        cap = [L.EVG_NO_DRAWDOWN if x is None else int(x.new_cap_target) for x in drawdown]
+        qlen = list(queue_lengths)
+    res = eng.host_drawdown(table, existing_host_counts, now, cap, qlen)
+    out, v = [], res["hosts"]
+    for d, did in enumerate(distro_ids):
+        r = res["distros"][d]
+        if not r["ran"]:
+            out.append(None)
+            continue
+        a, b = int(table.idle_off[d]), int(table.idle_off[d + 1])
+        existing = int(existing_host_counts[d])
+        job = M.HostDrawdownJob(did, existing - int(r["target"]), existing, b - a, int(r["target"]))
+        for i in range(a, b):
+            code = int(v[i]["decision"])
+            if code == L.EVG_HT_DECOMMISSION:
+                job.decommissioned_hosts.append(table.ids[i])
+            elif code in _HT_ERRORS:
+                job.errors.append((table.ids[i], _HT_ERRORS[code]))
+        assert job.decommissioned == int(r["decommissioned"])
+        out.append(job)
+    return out
+
+
+def idle_host_jobs(distros: Sequence[Optional[M.Distro]], idle_hosts: Sequence[Sequence[M.Host]], running_hosts_counts: Sequence[int],
+                   now: int, *, acceptable_host_idle_time_seconds: int = 0, engine: Optional[Engine] = None) -> list:
+    """idleHostJob.Run (units/host_monitoring_idle_termination.go:64-140) for every distro on the device.
+    `distros[d]`: the distro document, None when it is missing from the collection (evaluated as the zero distro);
+    `idle_hosts[d]`: its IdleEphemeralGroupedByDistroID hosts by ascending CreationTime; `running_hosts_counts[d]`: the
+    aggregation's RunningHostsCount.  Returns an IdleHostJob per distro."""
+    eng = engine or default_engine()
+    zero = M.Distro()
+    ds = [zero if d is None else d for d in distros]
+    table = S.marshal_idle_hosts(idle_hosts, [d.default_ami for d in ds])
+    cfg = np.zeros(len(ds), L.IDLE_CFG_DTYPE)
+    for i, (d, n) in enumerate(zip(ds, running_hosts_counts)):
+        idle = d.host_allocator_settings.acceptable_host_idle_time
+        cfg[i] = (d.host_allocator_settings.minimum_hosts, int(n),
+                  idle if idle != 0 else int(acceptable_host_idle_time_seconds) * M.SECOND)  # getIdleInfo (:197-200)
+    res = eng.idle_hosts(table, cfg, now)
+    out, v = [], res["hosts"]
+    for d, did in enumerate(distros):
+        a, b = int(table.idle_off[d]), int(table.idle_off[d + 1])
+        job = M.IdleHostJob("" if did is None else did.id, b - a, int(res["distros"][d]["min_evaluate"]))
+        for i in range(a, b):
+            code = int(v[i]["decision"])
+            if code >= L.EVG_HT_TERM_OUTDATED_AMI:
+                job.terminated_hosts.append(table.ids[i])
+                job.reasons.append(termination_reason(v[i]))
+            elif code in _IDLE_ERRORS:
+                job.errors.append((table.ids[i], _IDLE_ERRORS[code]))
+        assert job.terminated == int(res["distros"][d]["terminated"])
+        out.append(job)
+    return out
 
 
 def PrioritizeTasks(d: M.Distro, tasks: List[M.Task], opts: Optional[TaskPlannerOptions] = None, *, now: int,

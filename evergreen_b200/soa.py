@@ -546,6 +546,78 @@ def marshal_host_job(datas: Sequence[M.HostAllocatorData], n_provisioning: Seque
     return rows
 
 
+@dataclass
+class IdleHostTable:
+    """evg_idle_host_soa + idle_off: the idle hosts of every distro, grouped by distro in the job's query order.
+    ``ids`` keeps each row's host id for the shim's follow-up (SetDecommissioned / a termination job)."""
+    cols: Dict[str, np.ndarray]   # L.IDLE_HOST_COLUMNS, int64
+    flags: np.ndarray             # uint32 EVG_IH_*
+    idle_off: np.ndarray          # int64, n_distros + 1
+    ids: List[str] = field(default_factory=list)
+
+    @property
+    def n_hosts(self) -> int:
+        return int(self.flags.shape[0])
+
+    @property
+    def n_distros(self) -> int:
+        return int(self.idle_off.shape[0]) - 1
+
+    def struct(self) -> L.IdleHostSoAStruct:
+        s = L.IdleHostSoAStruct()
+        s.n_hosts, s.n_distros = self.n_hosts, self.n_distros
+        for name in L.IDLE_HOST_COLUMNS:
+            setattr(s, name, L.ptr(self.cols[name]) if self.n_hosts else None)
+        s.flags = L.ptr(self.flags) if self.n_hosts else None
+        return s
+
+
+def idle_host_flags(h: M.Host, default_ami: Optional[str] = None) -> int:
+    """The EVG_IH_* bits of one host, resolved from the host document and its lookups.  ``default_ami``: the distro
+    document's GetDefaultAMI() (the idle-host job); None leaves EVG_IH_OUTDATED_AMI clear (the drawdown job)."""
+    m = h.bootstrap_method
+    f = ((L.EVG_IH_RUNNING_TASK_GROUP if h.running_task_group else 0) | (L.EVG_IH_LAST_TASK if h.last_task else 0)
+         | (L.EVG_IH_STATUS_RUNNING if h.status == M.HOST_RUNNING else 0)
+         | (L.EVG_IH_USER_DATA if m == M.BOOTSTRAP_METHOD_USER_DATA else 0)
+         | (L.EVG_IH_LEGACY_BOOTSTRAP if m in ("", M.BOOTSTRAP_METHOD_LEGACY_SSH) else 0)  # LegacyBootstrap (distro.go:842-844)
+         | (L.EVG_IH_NEEDS_NEW_AGENT if h.needs_new_agent else 0)
+         | (L.EVG_IH_NEEDS_NEW_AGENT_MONITOR if h.needs_new_agent_monitor else 0)
+         | (L.EVG_IH_OUTDATED_AMI if default_ami is not None and h.ami != default_ami else 0)
+         | (L.EVG_IH_PAYMENT_NOT_DUE if h.time_til_next_payment > 5 * M.MINUTE else 0)  # maxTimeTilNextPayment
+         | (L.EVG_IH_CLOUD_MANAGER_FAILED if h.cloud_manager_error else 0))
+    if h.last_group:  # isAssignedSingleHostTaskGroup's LastGroup branch (units/host_monitoring_idle_termination.go:239-251)
+        f |= L.EVG_IH_TASK_LOOKUP_FAILED if h.last_task_single_host_task_group is None else (
+            L.EVG_IH_SINGLE_HOST_TASK_GROUP if h.last_task_single_host_task_group else 0)
+    return f
+
+
+_IDLE_HOST_TIMES = (("creation_ns", "creation_time"), ("start_ns", "start_time"), ("provision_ns", "provision_time"),
+                    ("agent_start_ns", "agent_start_time"), ("last_communication_ns", "last_communication_time"),
+                    ("last_task_completed_ns", "last_task_completed_time"),
+                    ("teardown_start_ns", "task_group_teardown_start_time"), ("acceptable_idle_ns", "acceptable_host_idle_time"))
+
+
+def marshal_idle_hosts(groups: Sequence[Sequence[M.Host]], default_amis: Optional[Sequence[str]] = None) -> IdleHostTable:
+    """Idle hosts per distro, in the query's order -> the idle-host table.  ``default_amis``: each distro's
+    GetDefaultAMI() for the idle-host job, None for the drawdown job.  A time outside the int64 nanosecond range is
+    rejected, not clamped: the device would compare a different instant."""
+    if default_amis is not None and len(default_amis) != len(groups):
+        raise ValueError("one default AMI per distro")
+    hosts = [h for g in groups for h in g]
+    cols = {}
+    for col, attr in _IDLE_HOST_TIMES:
+        vals = [getattr(h, attr) for h in hosts]
+        for h, v in zip(hosts, vals):
+            if not -(2 ** 63) <= v < 2 ** 63:
+                raise ValueError(f"host {h.id!r}: {attr} = {v} is outside the int64 nanosecond range")
+        cols[col] = np.array(vals, dtype=np.int64)
+    flags = np.array([idle_host_flags(h, None if default_amis is None else default_amis[d])
+                      for d, g in enumerate(groups) for h in g], dtype=np.uint32)
+    off = np.zeros(len(groups) + 1, np.int64)
+    off[1:] = np.cumsum([len(g) for g in groups])
+    return IdleHostTable(cols, flags, off, [h.id for h in hosts])
+
+
 def queue_info_rows(infos: Sequence[M.DistroQueueInfo]):
     """[DistroQueueInfo] -> (QUEUE_INFO rows, GROUP_INFO rows, group_off, names per distro).
     Later duplicates of a name win, like the map built at allocator.go:243-246."""

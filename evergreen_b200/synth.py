@@ -752,3 +752,74 @@ def make_duration_cache(w: Workload, seed: int, *, n_rows: int = 100_000, n_keys
         return DurationCache(value, std, ttl, coll, exp, exp_std, code).normalize()
 
     return DurationWorkload(hist, cache(w.tasks.n_tasks), cache(w.hosts.n_hosts) if w.hosts is not None else None)
+
+
+@dataclass
+class IdleHostWorkload:
+    """Inputs of the drawdown and idle-host jobs over one set of distros (make_idle_hosts)."""
+    now: int
+    groups: list            # [[Host]] per distro, in the query's order
+    distros: list           # [Distro | None]: None = missing from the distro collection
+    existing: np.ndarray    # CountHostsCanOrWillRunTasksInDistro
+    drawdown: list          # [DrawdownInfo | None]
+    queue_lengths: np.ndarray
+    running_counts: np.ndarray
+    sched_idle_seconds: int
+
+
+def make_idle_hosts(sizes, seed: int, *, now: int = NOW_NS) -> IdleHostWorkload:
+    """Idle hosts for the C4/C5 shapes: sizes[d] idle hosts in distro d.  The times sit at, and 1 ns around, every
+    threshold the two jobs compare against (5 s, 4, 5, 8 and 10 min, the distro's idle time), and include Go's zero
+    time, the Unix epoch and the int64 extremes; the flags and per-distro settings cover every branch, and the
+    drawdown caps give targets <= 0, below and above the eligible count.  A generator of its own (seeded `seed` with
+    its own salt): the streams of every other generator here are untouched."""
+    sizes = np.asarray(sizes, dtype=np.int64)
+    D, H = len(sizes), int(sizes.sum())
+    rng = Rng(seed ^ 0x1D1E0057)
+    pivots = np.array([0, 5 * M.SECOND, 90 * M.SECOND, 4 * M.MINUTE, 5 * M.MINUTE, 8 * M.MINUTE, 10 * M.MINUTE, 20 * M.MINUTE,
+                       M.HOUR], dtype=np.int64)
+
+    def times(n):
+        k = rng.integers(n, 0, 99)
+        near = now - pivots[rng.integers(n, 0, len(pivots) - 1)] + rng.integers(n, -1, 1)
+        wide = now - rng.integers(n, -M.HOUR, 48 * M.HOUR)
+        out = np.where(k < 55, near, wide)
+        out = np.where(k >= 92, M.ZERO_TIME, out)
+        out = np.where(k == 91, 0, out)
+        out = np.where(k == 90, -(2 ** 63) + 1, out)
+        return np.where(k == 89, 2 ** 63 - 1, out)
+
+    cols = {f: times(H) for f in ("creation_time", "start_time", "provision_time", "agent_start_time", "last_communication_time",
+                                  "last_task_completed_time")}
+    cols["task_group_teardown_start_time"] = np.where(rng.uniform(H) < 0.7, M.ZERO_TIME, times(H))
+    idle_choice = np.array([0, 5 * M.SECOND, 90 * M.SECOND, 4 * M.MINUTE, 10 * M.MINUTE, 2 ** 62], dtype=np.int64)
+    cols["acceptable_host_idle_time"] = idle_choice[rng.integers(H, 0, len(idle_choice) - 1)]
+    u = [rng.uniform(H) for _ in range(12)]
+    methods = np.array(["", M.BOOTSTRAP_METHOD_LEGACY_SSH, M.BOOTSTRAP_METHOD_USER_DATA, "ssh"])[rng.integers(H, 0, 3)]
+    single = np.where(u[9] < 0.1, 2, np.where(u[8] < 0.5, 1, 0))  # 2: the lookup fails
+    hosts = []
+    for i in range(H):
+        hosts.append(M.Host(
+            id=f"ih{i}", status=M.HOST_RUNNING if u[0][i] < 0.8 else "provisioning",
+            running_task_group="g" if u[1][i] < 0.2 else "", last_task="t" if u[2][i] < 0.6 else "",
+            last_group="g" if u[3][i] < 0.25 else "", needs_new_agent=bool(u[4][i] < 0.05),
+            needs_new_agent_monitor=bool(u[5][i] < 0.05), ami="old" if u[6][i] < 0.1 else "",
+            bootstrap_method=str(methods[i]), last_task_single_host_task_group=None if single[i] == 2 else bool(single[i]),
+            time_til_next_payment=int(5 * M.MINUTE + (1 if u[10][i] < 0.05 else 0)), cloud_manager_error=bool(u[11][i] < 0.03),
+            **{f: int(v[i]) for f, v in cols.items()}))
+    off = np.concatenate([[0], np.cumsum(sizes)])
+    groups = [hosts[off[d]:off[d + 1]] for d in range(D)]
+    minimum = rng.integers(D, 0, 40)
+    d_idle = idle_choice[rng.integers(D, 0, len(idle_choice) - 1)]
+    distros = [None if x < 0.02 else M.Distro(id=f"d{d}", default_ami="old" if y < 0.05 else "",
+                                              host_allocator_settings=M.HostAllocatorSettings(minimum_hosts=int(minimum[d]),
+                                                                                              acceptable_host_idle_time=int(d_idle[d])))
+               for d, (x, y) in enumerate(zip(rng.uniform(D), rng.uniform(D)))]
+    running = sizes + rng.integers(D, 0, 50)
+    existing = sizes + rng.integers(D, 0, 50)
+    # the cap: no job, a target <= 0, or a target anywhere from 1 to past the distro's idle hosts
+    kind, target = rng.uniform(D), rng.integers(D, 1, 1 << 20) % (sizes + 2) + 1
+    cap = existing - np.where(kind < 0.3, -rng.integers(D, 0, 3), target)
+    drawdown = [None if k < 0.1 else M.DrawdownInfo(f"d{d}", int(c)) for d, (k, c) in enumerate(zip(kind, cap))]
+    qlen = np.where(rng.uniform(D) < 0.5, 0, rng.integers(D, 1, 100))
+    return IdleHostWorkload(now, groups, distros, existing, drawdown, qlen, running, 120)

@@ -47,7 +47,7 @@ enum {
   EVG_ERR_NOMEM = -3,   /* device or pinned allocation failed */
   EVG_ERR_STATE = -4    /* the resident tick cannot serve the call: there is none, or it lacks what the call needs
                            (its own columns, editability, hosts, dependency verdicts, alias map, resolved durations,
-                           an allocator run since it was set) */
+                           an allocator run since it was set, an evg_host_job on its current run) */
 };
 
 /* per-distro allocator status: the data errors UtilizationBasedHostAllocator
@@ -379,7 +379,7 @@ int evg_bind_result_buffer(evg_ctx* ctx, void* device_ptr, int64_t capacity);
  * evg_plan_and_alloc_batch it runs), evg_plan_and_alloc_batch's pipelined large ticks, evg_alloc_batch / evg_alloc_distro,
  * evg_deps_met_batch, evg_find_runnable_batch / _ex, evg_plan_from_finder / _ex, evg_edit_tasks, evg_plan_aliases,
  * evg_expected_durations_batch, evg_prioritize_legacy_batch, evg_dag_rebuild_batch, evg_rebuild_dispatchers and
- * evg_host_job.  Every other call adds the kernels it launches: the uploads (their range check), evg_update_tasks,
+ * evg_host_job, evg_host_drawdown and evg_idle_hosts.  Every other call adds the kernels it launches: the uploads (their range check), evg_update_tasks,
  * evg_download_queue and evg_resolve_durations. */
 int64_t evg_last_launch_count(evg_ctx* ctx);
 /* Device time in ms of the last evg_run_resident, from CUDA events on the context
@@ -939,12 +939,163 @@ typedef struct {
  *     implementation-defined), new_cap_target = n_up - killable floored at MinimumHosts; drawdown = killable > 0.
  * What the library does not model and the shim applies itself: a disabled distro returns before this phase (:144-146);
  * the intent-host cap (:212-229) and a CreateIntentHosts error (:233-237) end the job before the report, so the shim
- * discards that distro's report; choosing the hosts to decommission is the drawdown job's (units/host_drawdown.go).
+ * discards that distro's report; choosing the hosts to decommission is the drawdown job's (units/host_drawdown.go,
+ * evg_host_drawdown below, which can read this call's reports where they are).
  * EVG_ERR_INVALID with nothing launched: null cfg or out (or a null array of out), a negative n_provisioning.
  * EVG_ERR_STATE: no resident tick, a tick without hosts, or no evg_run_resident on it since it was set (the one-shot
  * evg_plan_and_alloc_batch counts as one).  The first call allocates the call's own small buffers.
  * Replaces: the single-task bypass, the time-to-empty report and the drawdown decision of hostAllocatorJob.Run. */
 int evg_host_job(evg_ctx* ctx, const evg_host_job_cfg* cfg, const int32_t* spawned, evg_host_job_out* out);
+
+/* ---- host termination: the drawdown job and the idle-host job ------------- */
+
+/* One idle-host table serves both jobs.  Rows are grouped by distro through an idle_off CSR (n_distros + 1 entries);
+ * within a distro they come in the order the job's query returned them: IdleHostsWithDistroID's natural order for the
+ * drawdown job (model/host/db.go:274-286, 373-381), IdleEphemeralGroupedByDistroID's ascending CreationTime for the
+ * idle-host job (db.go:211-255).  Both queries return only ephemeral hosts with no running task that are not container
+ * parents, so IdleTime's running-task branch, the running-task branch of isAssignedSingleHostTaskGroup and the
+ * !IsEphemeral exemption of checkTerminationExemptions cannot be reached and are not modelled.
+ * Times are int64 ns since the Unix epoch, EVG_TIME_ZERO for Go's zero time. */
+enum {
+  EVG_IH_RUNNING_TASK_GROUP = 1 << 0,      /* RunningTaskGroup != "" */
+  EVG_IH_LAST_TASK = 1 << 1,               /* LastTask != "" */
+  EVG_IH_STATUS_RUNNING = 1 << 2,          /* Status == evergreen.HostRunning */
+  EVG_IH_USER_DATA = 1 << 3,               /* the embedded distro's bootstrap method is user-data */
+  EVG_IH_LEGACY_BOOTSTRAP = 1 << 4,        /* the embedded distro's LegacyBootstrap() */
+  EVG_IH_NEEDS_NEW_AGENT = 1 << 5,         /* NeedsNewAgent */
+  EVG_IH_NEEDS_NEW_AGENT_MONITOR = 1 << 6, /* NeedsNewAgentMonitor */
+  EVG_IH_OUTDATED_AMI = 1 << 7,            /* h.GetAMI() != d.GetDefaultAMI() against the distro document (idle job only) */
+  EVG_IH_SINGLE_HOST_TASK_GROUP = 1 << 8,  /* isAssignedSingleHostTaskGroup through LastGroup: the last task is
+                                              IsPartOfSingleHostTaskGroup and succeeded */
+  EVG_IH_TASK_LOOKUP_FAILED = 1 << 9,      /* LastGroup != "" and the last task was not found, or the lookup failed */
+  EVG_IH_PAYMENT_NOT_DUE = 1 << 10,        /* TimeTilNextPayment(h) > maxTimeTilNextPayment (5 min) */
+  EVG_IH_CLOUD_MANAGER_FAILED = 1 << 11    /* GetManagerOptions or GetManager returned an error */
+};
+
+typedef struct {
+  int64_t n_hosts;
+  int32_t n_distros;
+  int32_t _reserved;
+  const int64_t* creation_ns;
+  const int64_t* start_ns;
+  const int64_t* provision_ns;
+  const int64_t* agent_start_ns;
+  const int64_t* last_communication_ns;
+  const int64_t* last_task_completed_ns;
+  const int64_t* teardown_start_ns;    /* TaskGroupTeardownStartTime */
+  const int64_t* acceptable_idle_ns;   /* the host's embedded Distro.HostAllocatorSettings.AcceptableHostIdleTime */
+  const uint32_t* flags;               /* EVG_IH_* */
+} evg_idle_host_soa;
+
+/* What the job decided for one row.  EVG_HT_NOT_CHECKED: past its distro's drawdown target, a distro without a drawdown,
+ * or not among the idle job's evaluated hosts; nothing else of the row is written then (all zero). */
+enum {
+  EVG_HT_NOT_CHECKED = 0,
+  EVG_HT_KEPT = 1,                 /* checked, no action */
+  EVG_HT_EXEMPT_AGENT = 2,         /* checkTerminationExemptions: waiting for an agent */
+  EVG_HT_EXEMPT_PAYMENT = 3,       /* checkTerminationExemptions: the next payment is more than 5 min away */
+  EVG_HT_ERR_CLOUD_MANAGER = 4,    /* checkTerminationExemptions' error: the job reports it and leaves the host */
+  EVG_HT_ERR_TASK_LOOKUP = 5,      /* isAssignedSingleHostTaskGroup's error: the job reports it and leaves the host */
+  EVG_HT_DECOMMISSION = 6,         /* the drawdown job decommissions the host */
+  EVG_HT_TERM_OUTDATED_AMI = 7,    /* the idle job terminates it, one code per reason of getTerminationReason, in its order */
+  EVG_HT_TERM_COMMUNICATION = 8,
+  EVG_HT_TERM_IDLE = 9,
+  EVG_HT_TERM_TEARDOWN = 10
+};
+
+/* One row's verdict and the durations the job's messages print.  40 B. */
+typedef struct {
+  int64_t idle_ns;            /* IdleTime() */
+  int64_t communication_ns;   /* GetElapsedCommunicationTime() */
+  int64_t threshold_ns;       /* the idle threshold the job compares against (drawdown: 5 s, 10 min or the embedded
+                                 distro's value; idle job: the distro's, 5 min or doubled); 0 when the job decided
+                                 before it got to one (an exemption, a lookup error, a teardown or single-host task group
+                                 that keeps a host from the drawdown) */
+  int64_t since_teardown_ns;  /* time.Since(TaskGroupTeardownStartTime), INT64_MAX for Go's zero time */
+  int32_t decision;           /* EVG_HT_* */
+  int32_t _reserved;
+} evg_host_verdict;
+
+#define EVG_NO_DRAWDOWN INT64_MIN /* new_cap_target: no drawdown job for this distro */
+
+/* evg_host_drawdown's per-distro inputs (n_distros entries each).  new_cap_target and queue_length_dm are both NULL
+ * (chained) or both given (standalone). */
+typedef struct {
+  const int64_t* existing_hosts;   /* CountHostsCanOrWillRunTasksInDistro (units/host_drawdown.go:77) */
+  const int64_t* new_cap_target;   /* DrawdownInfo.NewCapTarget, EVG_NO_DRAWDOWN = no job */
+  const int64_t* queue_length_dm;  /* the distro's DistroQueueInfo.LengthWithDependenciesMet (:87, :141) */
+} evg_drawdown_in;
+
+/* Per distro.  24 B. */
+typedef struct {
+  int64_t target;          /* drawdownTarget = existing - NewCapTarget (:91), possibly <= 0; 0 when the job did not run */
+  int64_t decommissioned;  /* j.Decommissioned */
+  int32_t ran;             /* 1: the distro had a drawdown job */
+  int32_t _reserved;
+} evg_drawdown_distro;
+
+typedef struct {
+  evg_host_verdict* hosts;        /* n_hosts entries */
+  evg_drawdown_distro* distros;   /* n_distros entries */
+} evg_host_drawdown_out;
+
+/* hostDrawdownJob.Run / checkAndDecommission (units/host_drawdown.go:70-159) for every distro, on the device, at a
+ * frozen now_ns.  Per checked host, in order: checkTerminationExemptions (waiting for an agent with communication or
+ * idle time < 10 min: exempt; a cloud manager error; the next payment more than 5 min away: exempt); tearing down and
+ * not past 4 min: kept; a single-host task group: kept (a lookup error is reported and the host kept); then the
+ * threshold is 5 s, 10 min in a running task group, the embedded distro's acceptable_idle_ns when LastTaskCompletedTime
+ * is not zero and queue_length_dm > 0; IdleTime > threshold decommissions.  The loop stops before any host once the
+ * target is <= 0 and the target drops only on a decommission, so a row is checked iff fewer than `target` rows before
+ * it in its distro would be decommissioned; later rows are EVG_HT_NOT_CHECKED and report no error.
+ *   - chained (new_cap_target and queue_length_dm NULL): the distros the last evg_host_job on the resident tick's run
+ *     flagged drawdown = 1, with its new_cap_target and the tick's LengthWithDependenciesMet, none of which leaves the
+ *     device; hosts->n_distros must be the tick's.
+ *   - standalone: explicit values, as a separate drawdown job fed a DrawdownInfo; needs no tick and touches none.
+ * The tick is only read.  EVG_ERR_INVALID with nothing launched: a null hosts, idle_off, in, existing_hosts or out (or a
+ * null array of out or of hosts with n_hosts > 0), a bad idle_off, a negative n_hosts, n_distros, existing_hosts or
+ * queue_length_dm, new_cap_target and queue_length_dm not both NULL or both given, or a chained call whose n_distros is
+ * not the tick's.  EVG_ERR_STATE (chained only): no resident tick, or no evg_host_job on its current run.  The first
+ * call allocates the call's own buffers.
+ * Replaces: the per-host loop of hostDrawdownJob (the shim calls SetDecommissioned for each EVG_HT_DECOMMISSION row). */
+int evg_host_drawdown(evg_ctx* ctx, const evg_idle_host_soa* hosts, const int64_t* idle_off, const evg_drawdown_in* in,
+                      int64_t now_ns, evg_host_drawdown_out* out);
+
+/* evg_idle_hosts' per-distro settings.  24 B. */
+typedef struct {
+  int64_t minimum_hosts;        /* Distro.HostAllocatorSettings.MinimumHosts; 0 for a distro missing from the collection */
+  int64_t running_hosts_count;  /* IdleHostsByDistroID.RunningHostsCount */
+  int64_t acceptable_idle_ns;   /* the distro's AcceptableHostIdleTime, or SchedulerConfig.AcceptableHostIdleTimeSeconds
+                                   when that is 0 (units/host_monitoring_idle_termination.go:197-200) */
+} evg_idle_cfg;
+
+/* Per distro.  16 B. */
+typedef struct {
+  int64_t min_evaluate;  /* getMinNumHostsToEvaluate (:143-156) */
+  int64_t terminated;    /* j.Terminated for the distro */
+} evg_idle_distro;
+
+typedef struct {
+  evg_host_verdict* hosts;     /* n_hosts entries */
+  evg_idle_distro* distros;    /* n_distros entries */
+} evg_idle_hosts_out;
+
+/* idleHostJob.Run / checkAndTerminateHost / getIdleInfo / getTerminationReason
+ * (units/host_monitoring_idle_termination.go:64-283) for every distro, on the device, at a frozen now_ns.  Row i of a
+ * distro is evaluated iff i < min_evaluate = clamp(running_hosts_count - minimum_hosts, 0, n_idle) or it has an
+ * outdated AMI.  An evaluated host: the exemptions (as evg_host_drawdown; a cloud manager error is reported), then a
+ * task lookup error (reported, not terminated), then the threshold: acceptable_idle_ns, 5 min in a single-host task
+ * group, else doubled (int64 wrap) in a running task group; then the first reason that holds: an outdated AMI with
+ * IdleTime > 0 outside a single-host task group; communication time >= threshold and not tearing down; IdleTime > 0 and
+ * >= threshold; more than 4 min since the teardown start while tearing down.  No reason: EVG_HT_KEPT.
+ * A distro missing from the distro collection is decommissioned by the shim (:92-110); its idle rows are still
+ * evaluated, as the Go loop does, with a zero-value distro: minimum_hosts 0, the scheduler config's idle time and
+ * EVG_IH_OUTDATED_AMI set iff the host's AMI is not "".
+ * Needs no tick and leaves any tick as it was.  EVG_ERR_INVALID with nothing launched: a null hosts, idle_off, cfg or
+ * out (or a null array of out or of hosts with n_hosts > 0), a bad idle_off, a negative n_hosts, n_distros,
+ * minimum_hosts or running_hosts_count.  The first call allocates the call's own buffers.
+ * Replaces: the per-host loop of idleHostJob (the shim enqueues a termination job for each EVG_HT_TERM_* row). */
+int evg_idle_hosts(evg_ctx* ctx, const evg_idle_host_soa* hosts, const int64_t* idle_off, const evg_idle_cfg* cfg,
+                   int64_t now_ns, evg_idle_hosts_out* out);
 
 /* ---- single-distro wrappers: the per-job drop-in ------------------------- */
 
