@@ -213,6 +213,43 @@ class DispatchOutStruct(C.Structure):
     _fields_ = [(f, C.c_void_p) for f in DISPATCH_OUT_FIELDS]
 
 
+# FindNextTask (evg_find_next_batch / evg_find_next_tasks)
+(EVG_ND_FOUND, EVG_ND_STARTED, EVG_ND_STARTED_GROUP, EVG_ND_FINISHED_NOT_SUCCEEDED, EVG_ND_VERSION_FOUND, EVG_ND_VERSION_S3,
+ EVG_ND_DEPS_MET_NOW, EVG_ND_DEPS_ERR) = (1 << k for k in range(8))
+EVG_NEXT_NONE, EVG_NEXT_FOUND, EVG_NEXT_GAVE_UP = 0, 1, 2
+EVG_NS_NODE, EVG_NS_UNIT = 1, 2
+
+
+class NextDbStruct(C.Structure):
+    _fields_ = [("n_items", C.c_int64), ("n_groups", C.c_int64), ("flags", C.c_void_p), ("est_generated", C.c_void_p),
+                ("ingest_ns", C.c_void_p), ("running_hosts", C.c_void_p), ("generate_limit", C.c_int32),
+                ("pending_generate", C.c_int32), ("max_large_parser", C.c_int32), ("num_large_parser", C.c_int32)]
+
+
+class NextReqStruct(C.Structure):
+    _fields_ = [("n_requests", C.c_int64), ("req_off", C.c_void_p), ("group", C.c_void_p), ("ami_updated_ns", C.c_void_p)]
+
+
+class NextOutStruct(C.Structure):
+    _fields_ = [("item", C.c_void_p), ("outcome", C.c_void_p)]
+
+
+class NextStateStruct(C.Structure):
+    _fields_ = [("item_bits", C.c_void_p), ("group_deleted", C.c_void_p), ("group_running", C.c_void_p)]
+
+
+NEXT_DISPATCHER_FIELDS = ("item_off", "group_off", "sorted", "n_sorted", "unit_items", "unit_off", "group_id", "group_max_hosts",
+                          "dependencies_met")
+
+
+class NextDispatchersStruct(C.Structure):
+    _fields_ = [("n_distros", C.c_int32), ("_reserved", C.c_int32)] + [(f, C.c_void_p) for f in NEXT_DISPATCHER_FIELDS]
+
+
+assert (C.sizeof(NextDbStruct), C.sizeof(NextReqStruct), C.sizeof(NextOutStruct), C.sizeof(NextStateStruct),
+        C.sizeof(NextDispatchersStruct)) == (64, 32, 16, 24, 80)
+
+
 class AllocOutStruct(C.Structure):
     _fields_ = [("result", C.c_void_p), ("status", C.c_void_p)]
 
@@ -308,6 +345,9 @@ SYMBOLS = {
     "evg_prioritize_legacy_batch": (C.c_int, [_P, _P, _P, _P, C.c_int32, _P, _P, _P]),
     "evg_dag_rebuild_batch": (C.c_int, [_P, _P, _P, _P, C.c_int32, _P, _P, _P, _P, _P]),
     "evg_rebuild_dispatchers": (C.c_int, [_P, C.c_int32, C.c_int64, C.c_int64, _P]),
+    "evg_find_next_batch": (C.c_int, [_P, _P, _P, _P, _P, _P, _P]),
+    "evg_find_next_tasks": (C.c_int, [_P, _P, _P, _P]),
+    "evg_download_dispatch_state": (C.c_int, [_P, _P]),
     "evg_host_job": (C.c_int, [_P, _P, _P, _P]),
     "evg_host_drawdown": (C.c_int, [_P, _P, _P, _P, C.c_int64, _P]),
     "evg_idle_hosts": (C.c_int, [_P, _P, _P, _P, C.c_int64, _P]),

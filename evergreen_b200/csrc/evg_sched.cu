@@ -29,6 +29,7 @@
 //   k_dur_resolve         Task.FetchExpectedDuration per listed row (model/task/task.go:3519-3590) into staging
 //   k_dur_commit          the resolved durations into the resident columns, unless the call found an error
 //   k_host_job            hostAllocatorJob.Run past the allocator: single-task bypass, report, drawdown (units/host_allocator.go:180-425)
+//   k_next_verdict/serve  the DAG dispatcher's FindNextTask, a warp per distro (model/task_queue_service_dependency.go:258-692)
 // No CPU fallback exists in this file: without a device every entry point fails.
 #include <cuda_runtime.h>
 #include <stdarg.h>
@@ -309,6 +310,7 @@ __device__ __forceinline__ uint32_t pair_task(const DTasks& T, const DWork& W, u
 #include "evg_plan_general.cuh"
 #include "evg_legacy.cuh"
 #include "evg_dag.cuh"
+#include "evg_next.cuh"
 
 // --------------------------------------------------------------------------
 // kernels (general path: any distro size)
@@ -1283,8 +1285,12 @@ struct evg_ctx {
   // evg_upload_with_deps' verdicts (`deps`), evg_plan_aliases' map (`al`) and evg_resolve_durations' results (`dur`)
   // belong to it.  `allocated`: run state -- the allocator's results (queue and group infos, result rows, status) are
   // from a run on this tick, into the result buffer bound now; evg_host_job reads them.  `host_job`: run state --
-  // evg_host_job's reports in hj.out are from the current run; a chained evg_host_drawdown reads them.
-  struct { Tick kind = Tick::kNone; bool hosts = false, deps = false, aliases = false, durations = false, allocated = false, host_job = false; } tick;
+  // evg_host_job's reports in hj.out are from the current run; a chained evg_host_drawdown reads them.  `dispatchers`:
+  // run state -- evg_rebuild_dispatchers built dp and nx from the current run; evg_find_next_tasks serves from them.
+  struct {
+    Tick kind = Tick::kNone;
+    bool hosts = false, deps = false, aliases = false, durations = false, allocated = false, host_job = false, dispatchers = false;
+  } tick;
   int64_t T = 0, E = 0, G = 0, H = 0, U = 0, NT = 0, t_pad = 0;
   int32_t Dn = 0;
   int any_complex = 0;
@@ -1342,6 +1348,16 @@ struct evg_ctx {
   } dp;
   // evg_host_job (the first call allocates these): the staged job settings and spawned counts, and the outputs
   struct { DevBuf cfg, spawned, out; } hj;
+  // FindNextTask: the per-item fields and per-group tables of the dispatchers being served (evg_rebuild_dispatchers
+  // gathers them, evg_find_next_batch stages them with the dispatchers themselves), their state, the staged snapshot
+  // and requests of a call, and the host copies of the offsets the requests are checked against
+  struct {
+    DevBuf gmh, deps_met, gfirst, unit_max, verdict, bits, deleted, running, inert;
+    DevBuf flags, est, ingest, running_db, req_off, req_group, req_ami, list, out_item, out_outcome;
+    DevBuf item_off, group_off, sorted, n_sorted, unit_items, unit_off, group_id;  // evg_find_next_batch's dispatchers
+    DNext x{};  // the chained dispatchers
+    std::vector<int64_t> h_item_off, h_group_off;
+  } nx;
   // evg_host_drawdown / evg_idle_hosts (the first call allocates these): the staged idle-host table, its offsets and the
   // per-distro inputs, the verdicts, the decided flags and their scan, and the per-distro outputs
   struct { DevBuf cols, off, din, verdict, flag, pos, scan_sum, dout; } ih;
@@ -1410,7 +1426,7 @@ void drop_tick(evg_ctx* c) { c->tick = {}; }
 
 // What a call needs of the resident tick.  EVG_ERR_STATE names the call and the first unmet condition: a tick, then
 // its kind, then the state the call reads.
-enum class Need { kTick, kOwnColumns, kEditable, kHosts, kVerdicts, kAliasMap, kDurations, kAllocated, kHostJob };
+enum class Need { kTick, kOwnColumns, kEditable, kHosts, kVerdicts, kAliasMap, kDurations, kAllocated, kHostJob, kDispatchers };
 int need_tick(const evg_ctx* c, const char* who, Need what) {
   const auto& t = c->tick;
   const bool own = what == Need::kOwnColumns || what == Need::kEditable;
@@ -1422,7 +1438,8 @@ int need_tick(const evg_ctx* c, const char* who, Need what) {
                       : what == Need::kVerdicts && !t.deps                ? "the resident tick was not uploaded with evg_upload_with_deps"
                       : what == Need::kAliasMap && !t.aliases             ? "the resident tick was not built by evg_plan_aliases"
                       : what == Need::kDurations && !t.durations          ? "no evg_resolve_durations on the resident tick's rows"
-                      : what == Need::kHostJob && !t.host_job             ? "no evg_host_job on the resident tick's current run" : nullptr;
+                      : what == Need::kHostJob && !t.host_job             ? "no evg_host_job on the resident tick's current run"
+                      : what == Need::kDispatchers && !t.dispatchers      ? "no evg_rebuild_dispatchers on the resident tick's current run" : nullptr;
   return unmet ? fail(EVG_ERR_STATE, "%s: %s", who, unmet) : EVG_OK;
 }
 
@@ -2149,7 +2166,7 @@ int evg_run_resident(evg_ctx* c, int64_t now_ns, uint32_t opts) {
   c->launches = 0;
   c->timed = true;
   c->general_timed = false;
-  c->tick.allocated = c->tick.host_job = false;
+  c->tick.allocated = c->tick.host_job = c->tick.dispatchers = false;
   CK(cudaEventRecord(c->ev_begin, c->stream));
   int rc = run_plan(c, now_ns, opts);
   if (rc != EVG_OK) return rc;
@@ -3936,7 +3953,8 @@ struct DagBufs {
 // k_dag_topo, then the task-group buckets (k_dag_group_init / k_dag_group_pass / k_dag_units) over x, and the results
 // copied to the host.  item_off / group_off (D+1) are the host copies of x's offsets; max_n is the longest queue.
 static int dag_run(evg_ctx* c, const DDag& x, const DagBufs& b, int64_t max_n, const int64_t* item_off, const int64_t* group_off,
-                   int32_t* sorted, int32_t* n_sorted, int32_t* n_cycles, int32_t* unit_items, int32_t* unit_off) {
+                   int32_t* sorted, int32_t* n_sorted, int32_t* n_cycles, int32_t* unit_items, int32_t* unit_off,
+                   const int32_t** d_unit_items = nullptr) {
   const int64_t N = x.n;
   const int32_t D = x.n_distros;
   const int64_t G = group_off[D];
@@ -3967,6 +3985,7 @@ static int dag_run(evg_ctx* c, const DDag& x, const DagBufs& b, int64_t max_n, c
   CK(cudaMemcpyAsync(n_cycles, d_ncycles, sizeof(int32_t) * size_t(D), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   for (int32_t d = 0; d < D; d++) unit_off[group_off[d + 1] + d] = grouped[size_t(d)];  // the closing entry of each distro
+  if (d_unit_items) *d_unit_items = b.buf[cur];
   return EVG_OK;
 }
 
@@ -4015,6 +4034,211 @@ int evg_dag_rebuild_batch(evg_ctx* c, const evg_dag_in* in, const int64_t* item_
   DagBufs b{c->b_order.as<int32_t>(), c->b_rn6.as<int32_t>(), {c->b_rn3.as<int32_t>(), c->b_rn4.as<int32_t>()}, c->b_groupoff.as<int64_t>(),
             c->b_rn7.as<int32_t>()};
   return dag_run(c, x, b, max_n, item_off, group_off, sorted, n_sorted, n_cycles, unit_items, unit_off);
+}
+
+// ---- FindNextTask over dispatchers on the device (evg_next.cuh) ----
+
+// The tables derived from the dispatchers x describes (each unit's maxHosts) and their state: `st` (host) or, NULL, the
+// state a rebuild leaves.  Fills x's derived and state pointers.
+static int next_reset(evg_ctx* c, DNext& x, int32_t D, int64_t G, const evg_next_state* st) {
+  auto& q = c->nx;
+  cudaStream_t s = c->stream;
+  const int64_t N = x.n;
+  CK(q.verdict.ensure(sizeof(uint16_t) * size_t(N + 1)));
+  CK(q.bits.ensure(size_t(N + 1)));
+  for (DevBuf* b : {&q.gfirst, &q.unit_max, &q.running}) CK(b->ensure(sizeof(int32_t) * size_t(G + 1)));
+  for (DevBuf* b : {&q.deleted, &q.inert}) CK(b->ensure(size_t(G + 1)));
+  x.gfirst = q.gfirst.as<int32_t>(); x.unit_max = q.unit_max.as<int32_t>(); x.verdict = q.verdict.as<uint16_t>();
+  x.bits = q.bits.as<uint8_t>(); x.deleted = q.deleted.as<uint8_t>(); x.running = q.running.as<int32_t>(); x.inert = q.inert.as<uint8_t>();
+  if (st && st->item_bits && N > 0) CK(cudaMemcpyAsync(x.bits, st->item_bits, size_t(N), cudaMemcpyHostToDevice, s));
+  else CK(cudaMemsetAsync(x.bits, 0, size_t(N + 1), s));
+  if (st && st->group_deleted && G > 0) CK(cudaMemcpyAsync(x.deleted, st->group_deleted, size_t(G), cudaMemcpyHostToDevice, s));
+  else CK(cudaMemsetAsync(x.deleted, 0, size_t(G + 1), s));
+  if (st && st->group_running && G > 0) CK(cudaMemcpyAsync(x.running, st->group_running, sizeof(int32_t) * size_t(G), cudaMemcpyHostToDevice, s));
+  else CK(cudaMemsetAsync(x.running, 0, sizeof(int32_t) * size_t(G + 1), s));
+  if (G > 0) {
+    CK(cudaMemsetAsync(x.gfirst, 0x7F, sizeof(int32_t) * size_t(G), s));
+    CK(cudaMemsetAsync(x.unit_max, 0, sizeof(int32_t) * size_t(G), s));
+    launch(c, s, k_next_first, grid_for(N, 256), 256, 0, x, D);
+    launch(c, s, k_next_unit_max, grid_for(N, 256), 256, 0, x, D);
+    CK(cudaGetLastError());
+  }
+  return EVG_OK;
+}
+
+// evg_rebuild_dispatchers' last step: the dispatchers in c->dp become the ones evg_find_next_tasks serves.  GroupMaxHosts
+// and DependenciesMet of every item are gathered from the tick now, so that later changes to the tick do not reach them.
+static int next_adopt(evg_ctx* c, const int32_t* d_unit_items, const evg_dispatch_out* out) {
+  auto& q = c->nx;
+  auto& p = c->dp;
+  const int32_t D = c->Dn;
+  q.h_item_off.assign(out->item_off, out->item_off + D + 1);
+  q.h_group_off.assign(out->group_off, out->group_off + D + 1);
+  const int64_t N = out->item_off[D], G = out->group_off[D];
+  DNext x{};
+  x.n = N;
+  if (N > 0) {
+    cudaStream_t s = c->stream;
+    CK(q.gmh.ensure(sizeof(int32_t) * size_t(N)));
+    CK(q.deps_met.ensure(size_t(N)));
+    int32_t* stats = p.stats.as<int32_t>();
+    launch(c, s, k_next_gather, grid_for(N, 256), 256, 0, D, N, p.item_off.as<int64_t>(), c->b_taskoff.as<int64_t>(), c->b_groupoff.as<int64_t>(),
+           p.row.as<int32_t>(), c->tasks.gid.as<int32_t>(), c->b_gmax.as<int32_t>(), c->tasks.flags.as<uint32_t>(), q.gmh.as<int32_t>(),
+           q.deps_met.as<uint8_t>());
+    launch(c, s, k_next_close, grid_for(D, 256), 256, 0, D, p.group_off.as<int64_t>(), stats + 2 * (D + 1), p.unit_off.as<int32_t>());
+    x.item_off = p.item_off.as<int64_t>(); x.group_off = p.group_off.as<int64_t>(); x.sorted = p.sorted.as<int32_t>();
+    x.n_sorted = stats; x.unit_items = d_unit_items; x.unit_off = p.unit_off.as<int32_t>(); x.group_id = p.group_id.as<int32_t>();
+    x.gmh = q.gmh.as<int32_t>(); x.deps_met = q.deps_met.as<uint8_t>();
+    if (const int rc = next_reset(c, x, D, G, nullptr); rc != EVG_OK) return rc;
+    CK(cudaStreamSynchronize(s));
+  }
+  q.x = x;
+  c->tick.dispatchers = true;
+  return EVG_OK;
+}
+
+// What a serving call checks of its snapshot, requests and outputs against the dispatchers' offsets (host copies).
+static int next_check(const char* who, const int64_t* item_off, const int64_t* group_off, int32_t D, const evg_next_db* db,
+                      const evg_next_req* req, const evg_next_out* out) {
+  if (!db || !req || !out) return fail(EVG_ERR_INVALID, "%s: null argument", who);
+  const int64_t N = item_off[D], G = group_off[D], R = req->n_requests;
+  if (db->n_items != N || db->n_groups != G)
+    return fail(EVG_ERR_INVALID, "%s: the snapshot has %lld items and %lld groups, the dispatchers %lld and %lld", who, (long long)db->n_items,
+                (long long)db->n_groups, (long long)N, (long long)G);
+  if (R < 0) return fail(EVG_ERR_INVALID, "%s: negative n_requests", who);
+  if (!req->req_off) return fail(EVG_ERR_INVALID, "%s: null req_off", who);
+  if (const int rc = check_offsets(req->req_off, D, R, who, "req_off"); rc != EVG_OK) return rc;
+  if (R > 0 && (!req->group || !req->ami_updated_ns || !out->item || !out->outcome)) return fail(EVG_ERR_INVALID, "%s: null request column or output", who);
+  if ((N > 0 && (!db->flags || !db->est_generated || !db->ingest_ns)) || (G > 0 && !db->running_hosts))
+    return fail(EVG_ERR_INVALID, "%s: null snapshot column", who);
+  if (db->pending_generate < -1 || db->num_large_parser < -1)
+    return fail(EVG_ERR_INVALID, "%s: pending_generate / num_large_parser below -1", who);
+  for (int64_t j = 0; j < N; j++)
+    if (db->est_generated[j] < 0) return fail(EVG_ERR_INVALID, "%s: est_generated[%lld] is negative", who, (long long)j);
+  for (int64_t g = 0; g < G; g++)
+    if (db->running_hosts[g] < -1) return fail(EVG_ERR_INVALID, "%s: running_hosts[%lld] is below -1", who, (long long)g);
+  for (int32_t d = 0; d < D; d++) {
+    const int64_t ng = group_off[d + 1] - group_off[d];
+    for (int64_t r = req->req_off[d]; r < req->req_off[d + 1]; r++)
+      if (req->group[r] < -1 || req->group[r] >= ng)
+        return fail(EVG_ERR_INVALID, "%s: request %lld asks for group %d of distro %d, which has %lld", who, (long long)r, req->group[r], d, (long long)ng);
+  }
+  return EVG_OK;
+}
+
+// One call's snapshot and requests (checked) staged, k_next_verdict over the items, k_next_serve over the distros that
+// have requests, and the rows copied out.
+static int next_serve(evg_ctx* c, const DNext& x, const int64_t* item_off, const int64_t* group_off, int32_t D, const evg_next_db* db,
+                      const evg_next_req* req, evg_next_out* out) {
+  auto& q = c->nx;
+  cudaStream_t s = c->stream;
+  const int64_t N = item_off[D], G = group_off[D], R = req->n_requests;
+  if (R == 0) return EVG_OK;
+  if (N == 0) {  // every queue is empty (no dispatcher buffers exist): each walk ends at once (:468)
+    for (int64_t r = 0; r < R; r++) { out->item[r] = -1; out->outcome[r] = EVG_NEXT_NONE; }
+    return EVG_OK;
+  }
+  std::vector<int32_t> list;
+  for (int32_t d = 0; d < D; d++)
+    if (req->req_off[d + 1] > req->req_off[d]) list.push_back(d);
+  UP(s, q.flags, db->flags, N, uint8_t);
+  UP(s, q.est, db->est_generated, N, int32_t);
+  UP(s, q.ingest, db->ingest_ns, N, int64_t);
+  UP(s, q.running_db, db->running_hosts, G, int32_t);
+  UP(s, q.req_off, req->req_off, D + 1, int64_t);
+  UP(s, q.req_group, req->group, R, int32_t);
+  UP(s, q.req_ami, req->ami_updated_ns, R, int64_t);
+  UP(s, q.list, list.data(), int64_t(list.size()), int32_t);
+  CK(q.out_item.ensure(sizeof(int32_t) * size_t(R)));
+  CK(q.out_outcome.ensure(sizeof(int32_t) * size_t(R)));
+  CK(cudaMemsetAsync(x.inert, 0, size_t(G + 1), s));
+  DNextDb B{q.flags.as<uint8_t>(), q.est.as<int32_t>(), db->generate_limit, db->pending_generate, db->max_large_parser, db->num_large_parser};
+  launch(c, s, k_next_verdict, grid_for(N, 256), 256, 0, x, B);
+  DNextReq Q{q.list.as<int32_t>(), int32_t(list.size()), q.req_off.as<int64_t>(), q.req_group.as<int32_t>(), q.req_ami.as<int64_t>(),
+             q.ingest.as<int64_t>(), q.running_db.as<int32_t>(), q.out_item.as<int32_t>(), q.out_outcome.as<int32_t>()};
+  launch(c, s, k_next_serve, grid_for(int64_t(list.size()) * 32, 128), 128, 0, x, Q);
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(out->item, q.out_item.p, sizeof(int32_t) * size_t(R), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(out->outcome, q.out_outcome.p, sizeof(int32_t) * size_t(R), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  return EVG_OK;
+}
+
+static int next_download_state(evg_ctx* c, const DNext& x, int64_t G, const evg_next_state* st) {
+  cudaStream_t s = c->stream;
+  if (st->item_bits && x.n > 0) CK(cudaMemcpyAsync(st->item_bits, x.bits, size_t(x.n), cudaMemcpyDeviceToHost, s));
+  if (st->group_deleted && G > 0) CK(cudaMemcpyAsync(st->group_deleted, x.deleted, size_t(G), cudaMemcpyDeviceToHost, s));
+  if (st->group_running && G > 0) CK(cudaMemcpyAsync(st->group_running, x.running, sizeof(int32_t) * size_t(G), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  return EVG_OK;
+}
+
+int evg_find_next_tasks(evg_ctx* c, const evg_next_db* db, const evg_next_req* req, evg_next_out* out) {
+  ENTER(c, "evg_find_next_tasks");
+  int rc;
+  if ((rc = need_tick(c, who, Need::kTick)) != EVG_OK || (rc = need_tick(c, who, Need::kDispatchers)) != EVG_OK) return rc;
+  auto& q = c->nx;
+  const int32_t D = c->Dn;
+  if ((rc = next_check(who, q.h_item_off.data(), q.h_group_off.data(), D, db, req, out)) != EVG_OK) return rc;
+  c->launches = 0;
+  return next_serve(c, q.x, q.h_item_off.data(), q.h_group_off.data(), D, db, req, out);
+}
+
+int evg_download_dispatch_state(evg_ctx* c, evg_next_state* state) {
+  ENTER(c, "evg_download_dispatch_state");
+  if (!state) return fail(EVG_ERR_INVALID, "evg_download_dispatch_state: null argument");
+  int rc;
+  if ((rc = need_tick(c, who, Need::kTick)) != EVG_OK || (rc = need_tick(c, who, Need::kDispatchers)) != EVG_OK) return rc;
+  return next_download_state(c, c->nx.x, c->nx.h_group_off[size_t(c->Dn)], state);
+}
+
+int evg_find_next_batch(evg_ctx* c, const evg_next_dispatchers* disp, const evg_next_db* db, const evg_next_req* req,
+                        const evg_next_state* state_in, evg_next_state* state_out, evg_next_out* out) {
+  ENTER(c, "evg_find_next_batch");
+  if (!disp) return fail(EVG_ERR_INVALID, "evg_find_next_batch: null argument");
+  const int32_t D = disp->n_distros;
+  if (D < 0) return fail(EVG_ERR_INVALID, "evg_find_next_batch: negative n_distros");
+  if (!disp->item_off || !disp->group_off) return fail(EVG_ERR_INVALID, "evg_find_next_batch: null offsets");
+  int rc = check_offsets(disp->item_off, D, -1, who, "item_off");
+  if (rc == EVG_OK) rc = check_offsets(disp->group_off, D, -1, who, "group_off");
+  if (rc != EVG_OK) return rc;
+  const int64_t N = disp->item_off[D], G = disp->group_off[D];
+  if ((D > 0 && (!disp->n_sorted || !disp->unit_off)) ||
+      (N > 0 && (!disp->sorted || !disp->unit_items || !disp->group_id || !disp->group_max_hosts || !disp->dependencies_met)))
+    return fail(EVG_ERR_INVALID, "evg_find_next_batch: null dispatcher column");
+  // the kernels index with these: every entry inside its distro
+  for (int32_t d = 0; d < D; d++) {
+    const int64_t b = disp->item_off[d], n = disp->item_off[d + 1] - b, g0 = disp->group_off[d], ng = disp->group_off[d + 1] - g0;
+    bool ok = n < (int64_t(1) << 31) - 1 && ng <= n && disp->n_sorted[d] >= 0 && disp->n_sorted[d] <= n;
+    for (int64_t k = 0; ok && k < n; k++)
+      ok = disp->sorted[b + k] >= -2 && disp->sorted[b + k] < n && disp->group_id[b + k] >= -1 && disp->group_id[b + k] < ng &&
+           disp->unit_items[b + k] >= 0 && disp->unit_items[b + k] < n;
+    const int32_t* uo = disp->unit_off + g0 + d;
+    for (int64_t g = 0; ok && g < ng; g++) ok = uo[g] >= 0 && uo[g] <= uo[g + 1] && uo[g + 1] <= n;
+    if (!ok) return fail(EVG_ERR_INVALID, "evg_find_next_batch: distro %d's dispatcher holds an entry outside the distro", d);
+  }
+  if ((rc = next_check(who, disp->item_off, disp->group_off, D, db, req, out)) != EVG_OK) return rc;
+  c->launches = 0;
+  drop_tick(c);  // the dispatcher buffers below are the ones a chained evg_find_next_tasks serves from
+  auto& q = c->nx;
+  cudaStream_t s = c->stream;
+  UP(s, q.item_off, disp->item_off, D + 1, int64_t);
+  UP(s, q.group_off, disp->group_off, D + 1, int64_t);
+  UP(s, q.sorted, disp->sorted, N, int32_t);
+  UP(s, q.n_sorted, disp->n_sorted, D, int32_t);
+  UP(s, q.unit_items, disp->unit_items, N, int32_t);
+  UP(s, q.unit_off, disp->unit_off, G + D, int32_t);
+  UP(s, q.group_id, disp->group_id, N, int32_t);
+  UP(s, q.gmh, disp->group_max_hosts, N, int32_t);
+  UP(s, q.deps_met, disp->dependencies_met, N, uint8_t);
+  DNext x{};
+  x.n = N;
+  x.item_off = q.item_off.as<int64_t>(); x.group_off = q.group_off.as<int64_t>(); x.sorted = q.sorted.as<int32_t>();
+  x.n_sorted = q.n_sorted.as<int32_t>(); x.unit_items = q.unit_items.as<int32_t>(); x.unit_off = q.unit_off.as<int32_t>();
+  x.group_id = q.group_id.as<int32_t>(); x.gmh = q.gmh.as<int32_t>(); x.deps_met = q.deps_met.as<uint8_t>();
+  if ((rc = next_reset(c, x, D, G, state_in)) != EVG_OK) return rc;
+  if ((rc = next_serve(c, x, disp->item_off, disp->group_off, D, db, req, out)) != EVG_OK) return rc;
+  return state_out ? next_download_state(c, x, G, state_out) : EVG_OK;
 }
 
 // The persisted queue of every distro of the resident tick as a DAG input (evg_rebuild_dispatchers).  Item j of distro d
@@ -4107,10 +4331,11 @@ int evg_rebuild_dispatchers(evg_ctx* c, int32_t cap, int64_t items_capacity, int
   if (N > 0 && (!out->sorted || !out->unit_items)) return fail(EVG_ERR_INVALID, "evg_rebuild_dispatchers: null item output");
   if (g_need > 0 && !out->group_slot) return fail(EVG_ERR_INVALID, "evg_rebuild_dispatchers: null group_slot");
   c->launches = 0;
+  c->tick.dispatchers = false;  // until the dispatchers below are built and their state reset
   if (N == 0) {  // every queue is empty: no items, no groups
     for (int32_t d = 0; d < D; d++) out->n_sorted[d] = out->n_cycles[d] = out->unit_off[d] = 0;
     for (int32_t d = 0; d <= D; d++) out->group_off[d] = 0;
-    return EVG_OK;
+    return next_adopt(c, nullptr, out);
   }
   cudaStream_t s = c->stream;
   auto& p = c->dp;
@@ -4161,7 +4386,10 @@ int evg_rebuild_dispatchers(evg_ctx* c, int32_t cap, int64_t items_capacity, int
   x.on_stack = p.on_stack.as<uint8_t>();
   DagBufs b{p.sorted.as<int32_t>(), p.stats.as<int32_t>(), {p.buf[0].as<int32_t>(), p.buf[1].as<int32_t>()}, p.group_off.as<int64_t>(),
             p.unit_off.as<int32_t>()};
-  return dag_run(c, x, b, max_n, item_off, out->group_off, out->sorted, out->n_sorted, out->n_cycles, out->unit_items, out->unit_off);
+  const int32_t* d_unit_items = nullptr;
+  if (const int rc = dag_run(c, x, b, max_n, item_off, out->group_off, out->sorted, out->n_sorted, out->n_cycles, out->unit_items,
+                             out->unit_off, &d_unit_items); rc != EVG_OK) return rc;
+  return next_adopt(c, d_unit_items, out);
 }
 
 // The group sums of the job's report (units/host_allocator.go:271-280) over slots [g, g1) with stride `step`, in wrapping

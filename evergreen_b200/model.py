@@ -341,6 +341,18 @@ class TaskQueueItem:  # model/task_queue.go:131-153
 
 
 @dataclass
+class TaskSpec:  # model/task_queue.go:184-190: the task group the host last ran, as FindNextTask receives it
+    group: str = ""
+    build_variant: str = ""
+    project: str = ""
+    version: str = ""
+    group_max_hosts: int = 0
+
+    def composite_group_id(self) -> str:  # compositeGroupID, model/task_queue_service_dependency.go:700-702
+        return f"{self.group}_{self.build_variant}_{self.project}_{self.version}"
+
+
+@dataclass
 class TaskQueue:  # model/task_queue.go:117-123
     distro: str = ""
     generated_at: int = ZERO_TIME

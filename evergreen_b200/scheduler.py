@@ -56,6 +56,7 @@ class Engine:
         L.check(self.lib.evg_init(int(device), C.c_void_p(stream) if stream else None, C.byref(h)))
         self.ctx = h
         self._n_tasks = self._n_distros = self._n_groups = 0
+        self._n_disp = (0, 0)  # items and groups of the last rebuild_dispatchers()
         self._has_hosts = False
         self._n_dur = (0, 0)  # task and host rows of the last resolve_durations
         self._pinned = {}  # name -> (address, capacity in bytes): result buffers reused across ticks
@@ -413,9 +414,64 @@ class Engine:
         st = L.DispatchOutStruct(*[L.ptr(o[f]) for f in L.DISPATCH_OUT_FIELDS])
         L.check(self.lib.evg_rebuild_dispatchers(self.ctx, int(cap), max(T, 1), max(G, 1), C.byref(st)))
         N, G2 = int(o["item_off"][D]), int(o["group_off"][D])
+        self._n_disp = (N, G2)
         return {"item_off": o["item_off"], "sorted": o["sorted"][:N], "n_sorted": o["n_sorted"][:D], "n_cycles": o["n_cycles"][:D],
                 "group_off": o["group_off"], "group_slot": o["group_slot"][:G2], "unit_items": o["unit_items"][:N],
                 "unit_off": o["unit_off"][:G2 + D]}
+
+    @staticmethod
+    def _next_args(db: dict, req, n_items: int, n_groups: int):
+        """The evg_next_db / evg_next_req / evg_next_out of one call (soa.marshal_next_db, soa.marshal_next_requests)."""
+        req_off, group, ami = (np.ascontiguousarray(a, dtype=t) for a, t in zip(req, (np.int64, np.int32, np.int64)))
+        R = int(group.shape[0])
+        cols = {f: np.ascontiguousarray(db[f]) for f in ("flags", "est_generated", "ingest_ns", "running_hosts")}
+        dbs = L.NextDbStruct(n_items, n_groups, *[L.ptr(cols[f]) if cols[f].shape[0] else None
+                                                  for f in ("flags", "est_generated", "ingest_ns", "running_hosts")],
+                             db["generate_limit"], db["pending_generate"], db["max_large_parser"], db["num_large_parser"])
+        rs = L.NextReqStruct(R, L.ptr(req_off), L.ptr(group) if R else None, L.ptr(ami) if R else None)
+        item, outcome = np.full(R, -1, np.int32), np.zeros(R, np.int32)
+        os_ = L.NextOutStruct(L.ptr(item) if R else None, L.ptr(outcome) if R else None)
+        return dbs, rs, os_, item, outcome, (req_off, group, ami, cols)
+
+    @staticmethod
+    def _next_state(n_items: int, n_groups: int, state: Optional[dict] = None):
+        st = {"item_bits": np.zeros(max(n_items, 1), np.uint8), "group_deleted": np.zeros(max(n_groups, 1), np.uint8),
+              "group_running": np.zeros(max(n_groups, 1), np.int32)}
+        if state is not None:
+            for k in st:
+                st[k][:state[k].shape[0]] = state[k]
+        return st, L.NextStateStruct(*[L.ptr(st[k]) for k in ("item_bits", "group_deleted", "group_running")])
+
+    def find_next_batch(self, disp: dict, db: dict, req, state: Optional[dict] = None):
+        """evg_find_next_batch: FindNextTask for every request of every distro over host-marshalled dispatchers (`disp`:
+        arrays named L.NEXT_DISPATCHER_FIELDS).  `state`: dict of item_bits / group_deleted / group_running, None = what a
+        rebuild leaves.  -> (item per request, outcome per request, the state after the call)."""
+        D = int(disp["item_off"].shape[0]) - 1
+        N, G = int(disp["item_off"][-1]), int(disp["group_off"][-1])
+        arrs = {f: np.ascontiguousarray(disp[f]) for f in L.NEXT_DISPATCHER_FIELDS}
+        ds = L.NextDispatchersStruct(D, 0, *[L.ptr(arrs[f]) if arrs[f].shape[0] else None for f in L.NEXT_DISPATCHER_FIELDS])
+        dbs, rs, os_, item, outcome, keep = self._next_args(db, req, N, G)
+        st_in, si = self._next_state(N, G, state)
+        st_out, so = self._next_state(N, G)
+        L.check(self.lib.evg_find_next_batch(self.ctx, C.byref(ds), C.byref(dbs), C.byref(rs), C.byref(si), C.byref(so), C.byref(os_)))
+        del keep
+        return item, outcome, {"item_bits": st_out["item_bits"][:N], "group_deleted": st_out["group_deleted"][:G],
+                               "group_running": st_out["group_running"][:G]}
+
+    def find_next_tasks(self, db: dict, req):
+        """evg_find_next_tasks: the same on the dispatchers the last rebuild_dispatchers() built, whose state stays on
+        the device.  -> (item per request: the rank evg_download_queue returns, outcome per request)."""
+        dbs, rs, os_, item, outcome, keep = self._next_args(db, req, *self._n_disp)
+        L.check(self.lib.evg_find_next_tasks(self.ctx, C.byref(dbs), C.byref(rs), C.byref(os_)))
+        del keep
+        return item, outcome
+
+    def download_dispatch_state(self) -> dict:
+        """evg_download_dispatch_state: item_bits (EVG_NS_*), group_deleted and group_running of the chained dispatchers."""
+        N, G = self._n_disp
+        st, ss = self._next_state(N, G)
+        L.check(self.lib.evg_download_dispatch_state(self.ctx, C.byref(ss)))
+        return {"item_bits": st["item_bits"][:N], "group_deleted": st["group_deleted"][:G], "group_running": st["group_running"][:G]}
 
     def host_job(self, cfg: np.ndarray, spawned: Optional[np.ndarray] = None) -> dict:
         """evg_host_job: hostAllocatorJob.Run past the allocator for every distro of the resident tick after run(),
@@ -615,6 +671,7 @@ class ResidentTick:
         self.soa = self.table = self.keys = None
         self.last = None                 # (edit, update rows) of the last plan(), None when it uploaded
         self.ranked: List[List[str]] = []  # per distro: task ids in the last plan()'s rank order
+        self._disp = None                # (item_off, group names per dense group) of the dispatchers being served
 
     def canonical(self, batch):
         """The batch in canonical order: survivors in their previous order, then arrivals in batch order."""
@@ -718,12 +775,30 @@ class ResidentTick:
         self.remember(canon, soa, table, keys)
         res = _ranked_results(eng, canon, table, keys, now, breakdown, secondary)
         self.ranked = [[t.id for t in ranked] for ranked, _ in res]
+        self._disp = None  # the run ended the last dispatchers
         return res
 
     def dispatchers(self, cap: int = 0):
         """The DAG dispatcher of every distro's persisted queue of the last plan(), built on the device from the tick
         (dispatchers_from_tick): what rebuild_dag_dispatchers returns for the queues persist_task_queues would save."""
         return dispatchers_from_tick(self.ranked, [k.group_names for k in self.keys], cap=cap, engine=self.engine)
+
+    def find_next_tasks(self, requests, db: dict, cap: int = 0, rebuild: bool = False):
+        """FindNextTask for `requests[d]` = distro d's (TaskSpec or None, amiUpdatedTime) in serving order, on the
+        dispatchers of the last plan()'s persisted queues (evg_find_next_tasks).  The first call after a plan(), or
+        rebuild=True, builds them (evg_rebuild_dispatchers, which starts from IsDispatched == false); later calls serve
+        against the state the earlier ones left on the device.  -> per distro the task id (None for nil) and EVG_NEXT_*
+        outcome of each request."""
+        eng = self.engine
+        if rebuild or self._disp is None:
+            r = eng.rebuild_dispatchers(cap)
+            io, go = r["item_off"].copy(), r["group_off"].copy()
+            self._disp = (io, [[self.keys[d].group_names[int(g)] for g in r["group_slot"][int(go[d]):int(go[d + 1])]]
+                               for d in range(len(self.ranked))])
+        io, names = self._disp
+        ids = [self.ranked[d][:int(io[d + 1] - io[d])] for d in range(len(self.ranked))]
+        item, outcome = eng.find_next_tasks(S.marshal_next_db(ids, names, db), S.marshal_next_requests(names, requests))
+        return _next_results(ids, requests, item, outcome)
 
     def remember(self, canon, soa: S.TaskSoA, table: S.DistroTable, keys) -> None:
         """Make the marshalled `canon` the resident tick the next diff starts from."""
@@ -1348,3 +1423,64 @@ def alias_dispatchers(distros: Sequence[M.Distro], tasks: Sequence[M.Task], now:
               for d in range(len(distros))]
     return dispatchers_from_tick(ranked, [names[int(group_off[d]):int(group_off[d + 1])] for d in range(len(distros))],
                                  cap=cap, engine=eng)
+
+
+# ---------------------------------------------------------------------------------------------------------------
+def _next_results(ids, requests, item, outcome):
+    out, r = [], 0
+    for d, reqs in enumerate(requests):
+        out.append([(ids[d][int(item[r + k])] if item[r + k] >= 0 else None, int(outcome[r + k])) for k in range(len(reqs))])
+        r += len(reqs)
+    return out
+
+
+def next_dispatchers(queues: Sequence[M.TaskQueue], *, engine: Optional[Engine] = None):
+    """The evg_next_dispatchers of a batch of persisted queues: evg_dag_rebuild_batch's arrays plus GroupMaxHosts,
+    DependenciesMet and the dense group id of every item.  -> (disp, compositeGroupID of each dense group per queue,
+    the state a rebuild leaves: both IsDispatched copies from the persisted IsDispatched)."""
+    eng = engine or default_engine()
+    io, go, dep_off, dep_item, group_id, group_index, names = S.dag_input_from_queues(queues)
+    srt, n_sorted, n_cycles, unit_items, unit_off = eng.dag_rebuild_batch(io, go, dep_off, dep_item, group_id, group_index)
+    items = [it for q in queues for it in q.queue]
+    disp = {"item_off": io, "group_off": go, "sorted": srt.copy(), "n_sorted": n_sorted.copy(), "unit_items": unit_items.copy(),
+            "unit_off": unit_off.copy(), "group_id": group_id,
+            "group_max_hosts": np.array([it.group_max_hosts for it in items], dtype=np.int32),
+            "dependencies_met": np.array([it.dependencies_met for it in items], dtype=np.uint8)}
+    # a persisted IsDispatched sets the node's bit and, for an item rebuild copies into a unit, the copy's
+    state = {"item_bits": np.array([(L.EVG_NS_NODE | (L.EVG_NS_UNIT if g >= 0 else 0)) if it.is_dispatched else 0
+                                    for it, g in zip(items, group_id)], dtype=np.uint8),
+             "group_deleted": np.zeros(int(go[-1]), np.uint8), "group_running": np.zeros(int(go[-1]), np.int32)}
+    return disp, names, state
+
+
+def find_next_tasks(queues: Sequence[M.TaskQueue], requests, db: dict, *, engine: Optional[Engine] = None, built=None):
+    """basicCachedDAGDispatcherImpl.FindNextTask (model/task_queue_service_dependency.go:258-469) for a batch of
+    persisted queues: `requests[d]` = queue d's (TaskSpec or None, amiUpdatedTime) in serving order, against one frozen
+    database snapshot `db` (soa.marshal_next_db).  `built`: (disp, names, state) from next_dispatchers or an earlier call,
+    None = rebuild from the queues.  -> (per queue the (task id or None, EVG_NEXT_* outcome) of each request, `built`
+    with the state the call left)."""
+    eng = engine or default_engine()
+    disp, names, state = built or next_dispatchers(queues, engine=eng)
+    ids = [[it.id for it in q.queue] for q in queues]
+    item, outcome, state = eng.find_next_batch(disp, S.marshal_next_db(ids, names, db), S.marshal_next_requests(names, requests), state)
+    return _next_results(ids, requests, item, outcome), (disp, names, state)
+
+
+class DAGDispatchService:
+    """One distro's basicCachedDAGDispatcherImpl on the GPU: built from its persisted TaskQueue, FindNextTask(spec,
+    amiUpdatedTime, db) serves one request per call like the reference, rebuild() starts over (Refresh's TTL is the
+    caller's, :75-94).  last_outcome is the EVG_NEXT_* code of the last request."""
+
+    def __init__(self, queue: M.TaskQueue, engine: Optional[Engine] = None):
+        self.engine = engine
+        self.rebuild(queue)
+
+    def rebuild(self, queue: M.TaskQueue) -> None:
+        self.queue = queue
+        self.built = next_dispatchers([queue], engine=self.engine or default_engine())
+        self.last_outcome = L.EVG_NEXT_NONE
+
+    def FindNextTask(self, spec: Optional[M.TaskSpec], ami_updated_time: int, db: dict) -> Optional[M.TaskQueueItem]:
+        res, self.built = find_next_tasks([self.queue], [[(spec, ami_updated_time)]], db, engine=self.engine, built=self.built)
+        (tid, self.last_outcome), = res[0]
+        return None if tid is None else next(it for it in self.queue.queue if it.id == tid)

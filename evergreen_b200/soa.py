@@ -1411,3 +1411,60 @@ def persisted_dag_input(soa: TaskSoA, table: DistroTable, order: np.ndarray, cap
     group_slot = np.zeros(int(group_off[-1]), dtype=np.int32)
     group_slot[pos[head]] = slot[head]
     return (item_off, group_off, dep_off, dep_item, group_id, soa.task_group_order[task].astype(np.int32), group_slot)
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# FindNextTask's inputs (model/task_queue_service_dependency.go:258-469): evg_next_db and evg_next_req
+def marshal_next_db(item_ids: Sequence[Sequence[str]], group_names: Sequence[Sequence[str]], db: dict) -> dict:
+    """A database snapshot -> the columns of evg_next_db over the dispatchers' items (`item_ids[d]`: distro d's item ids
+    in queue order) and groups (`group_names[d]`: the compositeGroupID of each dense group).  `db`:
+      tasks: {id: {"start", "finish", "ingest": ns (M.ZERO_TIME = Go's zero time), "status", "version",
+                   "est_generated": int or None, "deps_met": True / False / None for an error}}; a missing id = no document
+      versions: {id: ProjectStorageMethod}; running_hosts: {compositeGroupID: count, -1 = error}, missing = 0
+      generate_limit, pending_generate, max_large_parser, num_large_parser: ints, -1 = the query failed.
+    The two start-time bits are evaluated as the reference writes them: !utility.IsZeroTime(StartTime) (:334) and
+    StartTime != utility.ZeroTime, a comparison with time.Unix(0, 0) that Go's zero time fails (:657)."""
+    flags, est, ingest = [], [], []
+    tasks, versions = db.get("tasks", {}), db.get("versions", {})
+    for ids in item_ids:
+        for i in ids:
+            doc = tasks.get(i)
+            f = 0
+            if doc is not None:
+                f |= L.EVG_ND_FOUND
+                if not M.is_zero_time(doc.get("start", 0)):
+                    f |= L.EVG_ND_STARTED
+                if doc.get("start", 0) != 0:
+                    f |= L.EVG_ND_STARTED_GROUP
+                if not M.is_zero_time(doc.get("finish", 0)) and doc.get("status", "") != M.TASK_SUCCEEDED:
+                    f |= L.EVG_ND_FINISHED_NOT_SUCCEEDED
+                if doc.get("version", "") in versions:
+                    f |= L.EVG_ND_VERSION_FOUND
+                    if versions[doc.get("version", "")] == "s3":
+                        f |= L.EVG_ND_VERSION_S3
+                met = doc.get("deps_met", True)
+                f |= L.EVG_ND_DEPS_ERR if met is None else (L.EVG_ND_DEPS_MET_NOW if met else 0)
+            flags.append(f)
+            est.append(int((doc or {}).get("est_generated") or 0))
+            t = (doc or {}).get("ingest", 0)
+            ingest.append(0 if t == M.ZERO_TIME else t)  # only compared with After(amiUpdatedTime), itself after the epoch
+    hosts = db.get("running_hosts", {})
+    return {"flags": np.array(flags, dtype=np.uint8), "est_generated": np.array(est, dtype=np.int32),
+            "ingest_ns": np.array(ingest, dtype=np.int64),
+            "running_hosts": np.array([hosts.get(n, 0) for names in group_names for n in names], dtype=np.int32),
+            "generate_limit": int(db.get("generate_limit", 0)), "pending_generate": int(db.get("pending_generate", 0)),
+            "max_large_parser": int(db.get("max_large_parser", 0)), "num_large_parser": int(db.get("num_large_parser", 0))}
+
+
+def marshal_next_requests(group_names: Sequence[Sequence[str]], requests):
+    """`requests[d]`: distro d's (TaskSpec or None, amiUpdatedTime) in serving order -> (req_off, group, ami_updated_ns):
+    the spec's compositeGroupID resolved to the dispatcher's dense group id, -1 for spec.Group == "" or an id that is
+    none of the dispatcher's groups (:268-274); a zero amiUpdatedTime becomes 0."""
+    req_off, group, ami = [0], [], []
+    for names, reqs in zip(group_names, requests):
+        dense = {n: g for g, n in enumerate(names)}
+        for spec, t in reqs:
+            group.append(dense.get(spec.composite_group_id(), -1) if spec is not None and spec.group else -1)
+            ami.append(0 if M.is_zero_time(t) else t)
+        req_off.append(len(group))
+    return np.array(req_off, dtype=np.int64), np.array(group, dtype=np.int32), np.array(ami, dtype=np.int64)

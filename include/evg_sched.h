@@ -378,8 +378,8 @@ int evg_bind_result_buffer(evg_ctx* ctx, void* device_ptr, int64_t capacity);
  * reset it to 0 before their first launch: evg_run_resident (so evg_plan_batch, evg_plan_distro and the
  * evg_plan_and_alloc_batch it runs), evg_plan_and_alloc_batch's pipelined large ticks, evg_alloc_batch / evg_alloc_distro,
  * evg_deps_met_batch, evg_find_runnable_batch / _ex, evg_plan_from_finder / _ex, evg_edit_tasks, evg_plan_aliases,
- * evg_expected_durations_batch, evg_prioritize_legacy_batch, evg_dag_rebuild_batch, evg_rebuild_dispatchers and
- * evg_host_job, evg_host_drawdown and evg_idle_hosts.  Every other call adds the kernels it launches: the uploads (their range check), evg_update_tasks,
+ * evg_expected_durations_batch, evg_prioritize_legacy_batch, evg_dag_rebuild_batch, evg_rebuild_dispatchers,
+ * evg_host_job, evg_host_drawdown, evg_idle_hosts, evg_find_next_batch and evg_find_next_tasks.  Every other call adds the kernels it launches: the uploads (their range check), evg_update_tasks,
  * evg_download_queue and evg_resolve_durations. */
 int64_t evg_last_launch_count(evg_ctx* ctx);
 /* Device time in ms of the last evg_run_resident, from CUDA events on the context
@@ -878,6 +878,109 @@ typedef struct {
  * Replaces: the evg_download_queue -> dependency-id resolution -> compositeGroupID interning -> evg_dag_rebuild_batch
  * round trip a shim would make to hand FindNextTask d.sorted and d.taskGroups (:475-476, :527-543). */
 int evg_rebuild_dispatchers(evg_ctx* ctx, int32_t cap, int64_t items_capacity, int64_t groups_capacity, evg_dispatch_out* out);
+
+/* ---- DAG dispatcher: FindNextTask (SURVEY.md §8 f.3) ------------------------- */
+
+/* evg_next_db.flags: what FindNextTask reads of an item's task document and version, resolved by the shim */
+#define EVG_ND_FOUND 0x01u         /* task.FindOneId returned a document (:312, :433, :630); error or nil: clear */
+#define EVG_ND_STARTED 0x02u       /* !utility.IsZeroTime(StartTime) (:334): false for Go's zero time and the Unix epoch */
+#define EVG_ND_STARTED_GROUP 0x04u /* StartTime != utility.ZeroTime (:657): a struct comparison with time.Unix(0, 0) */
+#define EVG_ND_FINISHED_NOT_SUCCEEDED 0x08u /* !IsZeroTime(FinishTime) && Status != "success" (:696-698) */
+#define EVG_ND_VERSION_FOUND 0x10u /* VersionFindOne returned a document (:554-576) */
+#define EVG_ND_VERSION_S3 0x20u    /* its ProjectStorageMethod is S3 (:578) */
+#define EVG_ND_DEPS_MET_NOW 0x40u  /* nextTaskFromDB.DependenciesMet (:373, :662), e.g. from evg_deps_met_batch */
+#define EVG_ND_DEPS_ERR 0x80u      /* ... returned an error: the item is skipped */
+
+/* One frozen snapshot of the database for one call.  Per-item columns run over the concatenated items of every
+ * dispatcher (item_off), running_hosts over their groups (group_off).  64 B. */
+typedef struct {
+  int64_t n_items;
+  int64_t n_groups;
+  const uint8_t* flags;          /* n_items: EVG_ND_* */
+  const int32_t* est_generated;  /* n_items: EstimatedNumGeneratedTasks, 0 for nil (:340) */
+  const int64_t* ingest_ns;      /* n_items: IngestTime (:392) */
+  const int32_t* running_hosts;  /* n_groups: host.NumHostsByTaskSpec (:412, model/host/db.go:521-533); -1: error, which
+                                    includes an empty variant / project / version */
+  int32_t generate_limit;        /* TaskLimits.MaxPendingGeneratedTasks (:339) */
+  int32_t pending_generate;      /* task.GetPendingGenerateTasks (:342); -1: the query failed */
+  int32_t max_large_parser;      /* getMaxConcurrentLargeParserProjTasks, degraded mode resolved (:605-612); <= 0: no rule */
+  int32_t num_large_parser;      /* task.CountLargeParserProjectTasks (:579); -1: the count failed */
+} evg_next_db;
+
+/* The requests of one call: distro d's are req_off[d] .. req_off[d+1], served in that order.  32 B. */
+typedef struct {
+  int64_t n_requests;
+  const int64_t* req_off;        /* n_distros + 1 */
+  const int32_t* group;          /* per request: the dense group id compositeGroupID(spec) resolves to in its distro (:268-274);
+                                    -1 when spec.Group == "" or the id is none of the dispatcher's groups */
+  const int64_t* ami_updated_ns; /* per request: amiUpdatedTime, 0 for a zero time (:392) */
+} evg_next_req;
+
+#define EVG_NEXT_NONE 0    /* the walk over d.sorted ended: FindNextTask returned nil at :468 */
+#define EVG_NEXT_FOUND 1   /* item = the queue index (rank, the row evg_download_queue returns) of the TaskQueueItem */
+#define EVG_NEXT_GAVE_UP 2 /* nil on a database miss: no task document, no version, a failed host count */
+typedef struct {
+  int32_t* item;    /* per request; -1 for nil */
+  int32_t* outcome; /* per request: EVG_NEXT_* */
+} evg_next_out;
+
+/* Dispatcher state.  item_bits: the two IsDispatched copies the reference keeps per item. */
+#define EVG_NS_NODE 0x1u /* the node's item (d.nodeItemMap; set at :496 and :515) */
+#define EVG_NS_UNIT 0x2u /* the copy in schedulableUnit.tasks (:172-183; set at :681; all getTaskGroup and nextTaskGroupTask read) */
+typedef struct {
+  uint8_t* item_bits;      /* n_items */
+  uint8_t* group_deleted;  /* n_groups: the unit left d.taskGroups (:653, :685) */
+  int32_t* group_running;  /* n_groups: the unit's cached runningHosts (:411-427); 0 after a rebuild */
+} evg_next_state;
+
+/* A batch of dispatchers as evg_dag_rebuild_batch returns them, plus what FindNextTask reads of each item.  80 B. */
+typedef struct {
+  int32_t n_distros;
+  int32_t _reserved;
+  const int64_t* item_off;         /* n_distros + 1 */
+  const int64_t* group_off;        /* n_distros + 1 */
+  const int32_t* sorted;           /* evg_dag_rebuild_batch's outputs ... */
+  const int32_t* n_sorted;
+  const int32_t* unit_items;
+  const int32_t* unit_off;
+  const int32_t* group_id;         /* n_items: as evg_dag_in.group_id */
+  const int32_t* group_max_hosts;  /* n_items: TaskQueueItem.GroupMaxHosts */
+  const uint8_t* dependencies_met; /* n_items: TaskQueueItem.DependenciesMet */
+} evg_next_dispatchers;
+
+/* basicCachedDAGDispatcherImpl.FindNextTask (model/task_queue_service_dependency.go:258-469, with tryMarkItemDispatched
+ * :486-498, tryMarkNextTaskGroupTaskDispatched :500-519, getTaskGroup :524-538, checkMaxConcurrentLargeParserProjectTasks
+ * :549-603, nextTaskGroupTask :614-692, isBlockedSingleHostTaskGroup :696-698) for every request of every distro.
+ *
+ * The snapshot is frozen for the call.  The requests of one distro are served in the order given, each against the
+ * state the earlier ones left.  With one request per distro this is the reference exactly; with several it is the
+ * reference under requests that arrive before the database writes of the earlier ones land, which the reference accepts
+ * ("a best-effort attempt ... not a foolproof operation", :428-430).  Nothing raises running_hosts inside a call.  Within a call state only
+ * accumulates (bits get set, units get deleted, a cached runningHosts stops moving once it reaches maxHosts), and the
+ * serving kernel relies on it: a unit found unable to yield under the snapshot is not scanned again in that call.  A
+ * caller that clears bits does so between calls (state_in, or a rebuild), never between the requests of one call.
+ *
+ * Stateless form, host pointers: state_in (NULL: every bit clear, nothing deleted, runningHosts 0; an item persisted with
+ * IsDispatched has both bits set) is not changed; state_out receives the state after the last request.  Ends the
+ * resident tick (it stages into the dispatcher buffers evg_find_next_tasks serves from).
+ * EVG_ERR_INVALID with nothing launched: a null pointer the call needs, offsets check_offsets rejects (item_off, group_off,
+ * req_off), db sizes that differ from item_off / group_off, a request group outside [-1, groups of its distro), a
+ * negative est_generated, a snapshot scalar below -1 (generate_limit and max_large_parser may be any value <= 0). */
+int evg_find_next_batch(evg_ctx* ctx, const evg_next_dispatchers* disp, const evg_next_db* db, const evg_next_req* req,
+                        const evg_next_state* state_in, evg_next_state* state_out, evg_next_out* out);
+
+/* The same on the dispatchers the last successful evg_rebuild_dispatchers built from the resident tick; their state
+ * stays on the device between calls and starts from IsDispatched == false at every rebuild.  GroupMaxHosts,
+ * DependenciesMet and the dense group id of every item were gathered into the dispatchers' own buffers by the rebuild, as
+ * the Go dispatcher holds the items as persisted: evg_update_tasks or evg_resolve_durations in between do not reach them.
+ * Only reads the tick.  db->n_items / n_groups and req_off are over that rebuild's item_off / group_off.
+ * EVG_ERR_STATE: no resident tick, or no evg_rebuild_dispatchers on it since the last evg_run_resident.
+ * Replaces: copying sorted / unit_items back per distro and walking them in Go for the agents' next-task endpoint
+ * (rest/route/host_agent.go:350-368). */
+int evg_find_next_tasks(evg_ctx* ctx, const evg_next_db* db, const evg_next_req* req, evg_next_out* out);
+
+/* The chained dispatchers' state (same precondition as evg_find_next_tasks); any pointer may be NULL. */
+int evg_download_dispatch_state(evg_ctx* ctx, evg_next_state* state);
 
 /* ---- the host allocator job's decisions (SURVEY.md §8 row A21) ---------------- */
 
