@@ -11,8 +11,8 @@
 //     after the block-wide counter scan -- 6 B/task of sort state instead of 12.
 //   * digits are up to 10 bits wide (16 warps x 1024 u16 counters): a 20-bit value range sorts in 2 passes.
 //   * task columns arrive by TMA: one thread issues cp.async.bulk (UBLKCP) copies of the seven columns of a
-//     THREADS-task tile into a two-stage shared-memory ring guarded by mbarriers; the other threads never compute
-//     a global address in the task pass.
+//     2*THREADS-task tile into one shared-memory stage guarded by a full and an empty mbarrier; the other threads
+//     never compute a global address in the task pass.
 //   * scoring runs in 32-bit arithmetic wherever the distro's factors and the task allow it (single_task_value32).
 // Handles distros without GroupVersions and without in-queue dependency edges (task groups allowed); the host routes
 // everything else to k_plan_smem.  Runtime punts: a value outside u32, work-list overflow, TaskGroupOrder >= 64 or
@@ -20,8 +20,8 @@
 //
 // Shared memory (bytes), CAP = tasks, T = THREADS, W = warps:
 //   key   4*CAP            u32 TotalValue per task (phase 2b parks (group, order) of task-group tasks here)
-//   idx   2*CAP            u16 permutation                 | task pass: TMA stage 0 (+ start of stage 1)
-//   cnt   W*2^bits*2       u16 per-warp digit counters     | task pass: TMA stage 1; group phases: per-group
+//   idx   2*CAP            u16 permutation                 | task pass: the TMA stage (80*THREADS bytes, from here on)
+//   cnt   W*2^bits*2       u16 per-warp digit counters     | task pass: rest of the TMA stage; group phases: per-group
 //                                                          |   accumulators (with idx); pre-arrangement: e[] histogram
 //   list  6*CAP/4          u16 work list: task, anchor, rank (one stretch per warp)
 //
@@ -33,26 +33,13 @@ struct CtaDigit {
   static constexpr int kBits = THREADS >= 512 ? 10 : (THREADS >= 256 ? 9 : (THREADS >= 128 ? 8 : 7));  // 2^bits == 2*THREADS: one u32 counter pair per thread in the scan
 };
 
-// Tasks per thread and tile of the task pass.  2: one 2*THREADS-task stage, refilled as soon as every thread has its two
-// tasks in registers -- per-tile overhead (barrier wait, refill, list append) amortised over two tasks and two
-// independent scoring chains per thread; 1: two THREADS-task stages.
-#ifndef EVG_CTA_TPT
-#define EVG_CTA_TPT 2
-#endif
-// Tiles whose columns are pulled into L2 (cp.async.bulk.prefetch.L2) ahead of the one being staged; 0 = none.
-#ifndef EVG_CTA_PF
-#define EVG_CTA_PF 0
-#endif
-// ns a waiter may sleep inside mbarrier.try_wait before it re-polls; 0 = the default (short) suspend
-#ifndef EVG_CTA_WAITHINT
-#define EVG_CTA_WAITHINT 0
-#endif
-
 template <int THREADS, int CAP>
 struct PlanCta {
-  static constexpr int kTpt = EVG_CTA_TPT;
+  // Tasks per thread and tile of the task pass: one 2*THREADS-task stage, refilled as soon as every thread has its two
+  // tasks in registers -- per-tile overhead (barrier wait, refill, list append) amortised over two tasks and two
+  // independent scoring chains per thread.
+  static constexpr int kTpt = 2;
   static constexpr int kTile = kTpt * THREADS;
-  static constexpr int kStages = kTpt == 1 ? 2 : 1;
   static constexpr int kWarps = THREADS / 32;
   static constexpr int kItems = CAP / THREADS;
   static constexpr int kDigitBits = CtaDigit<THREADS>::kBits;
@@ -62,7 +49,7 @@ struct PlanCta {
   static constexpr size_t kIdxBytes = size_t(2) * CAP;
   static constexpr size_t kStageBytes = size_t(40) * kTile;
   static constexpr size_t kCntNeed = size_t(kWarps) * kDigitWords * 4;
-  static constexpr size_t kMultiBytes = (kIdxBytes + kCntNeed) > kStages * kStageBytes ? (kIdxBytes + kCntNeed) : kStages * kStageBytes;  // idx + cnt, contiguous
+  static constexpr size_t kMultiBytes = (kIdxBytes + kCntNeed) > kStageBytes ? (kIdxBytes + kCntNeed) : kStageBytes;  // idx + cnt, contiguous
   static constexpr size_t kListBytes = size_t(6) * kListCap;
   static constexpr size_t kOffKey = 0;
   static constexpr size_t kOffIdx = kKeyBytes;
@@ -102,43 +89,12 @@ __device__ __forceinline__ void mbar_fence_init() { asm volatile("fence.mbarrier
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  while (!mbar_try_wait(bar, parity)) {}
-}
-// the same on precomputed shared-window addresses: the task-pass loop issues them every tile
+// arrive and wait on precomputed shared-window addresses: the task-pass loop issues them every tile
 __device__ __forceinline__ void mbar_arrive_a(uint32_t bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory"); }
 __device__ __forceinline__ void mbar_wait_a(uint32_t bar, uint32_t parity) {
-#if EVG_CTA_WAITHINT > 0
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tWAIT_%=:\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1, %2;\n\t@!p bra WAIT_%=;\n\t}" ::"r"(bar), "r"(parity),
-      "r"(uint32_t(EVG_CTA_WAITHINT))
-      : "memory");
-#else
   asm volatile(
       "{\n\t.reg .pred p;\n\tWAIT_%=:\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t@!p bra WAIT_%=;\n\t}" ::"r"(bar), "r"(parity)
       : "memory");
-#endif
-}
-__device__ __forceinline__ void l2_prefetch_1d(const void* gmem_src, uint32_t bytes) {
-  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(gmem_src), "r"(bytes) : "memory");
-}
-// one lane's shared-memory add with the old value back (inline PTX: the compiler does not wrap it in its own warp aggregation)
-__device__ __forceinline__ uint32_t atom_add_shared(uint32_t addr, uint32_t v) {
-  uint32_t old;
-  asm volatile("atom.shared.add.u32 %0, [%1], %2;" : "=r"(old) : "r"(addr), "r"(v) : "memory");
-  return old;
 }
 // TMA, non-tensor form: one contiguous run global -> shared, completion counted in bytes on an mbarrier (SASS: UBLKCP)
 __device__ __forceinline__ void tma_load_1d(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar) {
@@ -173,10 +129,10 @@ k_plan_cta(DTasks T, DDistros D, DWork W, const int32_t* __restrict__ list, int6
   uint16_t* sLR = sLA + kListCap;                                            // its rank inside the unit
   uint32_t* sDisp = reinterpret_cast<uint32_t*>(smem_raw + L::kOffDisp);    // [CAP/32] task leaves its input position
   uint32_t* sScan = reinterpret_cast<uint32_t*>(smem_raw + L::kOffScan);    // [32] block-scan scratch
-  uint64_t* sBar = reinterpret_cast<uint64_t*>(smem_raw + L::kOffBar);      // full[2], empty[2]
+  uint64_t* sBar = reinterpret_cast<uint64_t*>(smem_raw + L::kOffBar);      // full[2], empty[2]; the one stage uses [0] of each
   CtaShared* S = reinterpret_cast<CtaShared*>(smem_raw + L::kOffShared);
   uint32_t* sNd = reinterpret_cast<uint32_t*>(smem_raw + L::kOffNd);
-  unsigned char* sStage = smem_raw + L::kOffIdx;                             // two stages of 40*THREADS bytes
+  unsigned char* sStage = smem_raw + L::kOffIdx;                             // the task pass's stage: 40*kTile bytes
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const unsigned full = 0xffffffffu;
@@ -210,38 +166,26 @@ k_plan_cta(DTasks T, DDistros D, DWork W, const int32_t* __restrict__ list, int6
   const evg_distro_cfg cfg = D.cfg[d];
 
   // ---- phase 2: one pass over the task columns ----
-  // Tile k holds tasks [a0 + k*THREADS, +THREADS) of the concatenated table, a0 = base rounded down to a multiple of
-  // four tasks so that every copy starts 16-byte aligned; slot `tid` of a stage is this thread's task.
+  // Tile k holds tasks [a0 + k*TILE, +TILE) of the concatenated table, a0 = base rounded down to a multiple of four
+  // tasks so that every copy starts 16-byte aligned; slots `tid` and `tid + THREADS` of the stage are this thread's tasks.
   const int64_t a0 = base - off0;
-  constexpr int TPT = L::kTpt, TILE = L::kTile, NST = L::kStages;
+  constexpr int TPT = L::kTpt, TILE = L::kTile;
   const int n_tiles = (off0 + tn + TILE - 1) / TILE;
   auto issue = [&](int k) {  // thread 0 only
-    const int s = k % NST;
     const int64_t start = a0 + int64_t(k) * TILE;
     const int64_t left = t_pad - start;
     const uint32_t cnt = uint32_t(left < int64_t(TILE) ? left : int64_t(TILE));  // multiple of 4, > 0
-    unsigned char* st = sStage + size_t(s) * L::kStageBytes;
-    uint64_t* bar = &sBar[s];
+    uint64_t* bar = &sBar[0];
     mbar_arrive_expect_tx(bar, cnt * 40u);
-    tma_load_1d(st + 0 * TILE * 4, T.priority + start, cnt * 4u, bar);
-    tma_load_1d(st + 1 * TILE * 4, T.numdep + start, cnt * 4u, bar);
-    tma_load_1d(st + 2 * TILE * 4, T.gid + start, cnt * 4u, bar);
-    tma_load_1d(st + 3 * TILE * 4, T.flags + start, cnt * 4u, bar);
-    tma_load_1d(st + 16 * TILE + 0 * TILE * 8, T.expected + start, cnt * 8u, bar);
-    tma_load_1d(st + 16 * TILE + 1 * TILE * 8, T.qbasis + start, cnt * 8u, bar);
-    tma_load_1d(st + 16 * TILE + 2 * TILE * 8, T.wbasis + start, cnt * 8u, bar);
-#if EVG_CTA_PF > 0
-    if (k + EVG_CTA_PF < n_tiles) {  // a later tile's columns start their trip from HBM to L2 now
-      const int64_t ps = start + int64_t(EVG_CTA_PF) * TILE;
-      const int64_t pl = t_pad - ps;
-      const uint32_t pc = uint32_t(pl < int64_t(TILE) ? pl : int64_t(TILE));
-      l2_prefetch_1d(T.priority + ps, pc * 4u); l2_prefetch_1d(T.numdep + ps, pc * 4u); l2_prefetch_1d(T.gid + ps, pc * 4u);
-      l2_prefetch_1d(T.flags + ps, pc * 4u); l2_prefetch_1d(T.expected + ps, pc * 8u); l2_prefetch_1d(T.qbasis + ps, pc * 8u);
-      l2_prefetch_1d(T.wbasis + ps, pc * 8u);
-    }
-#endif
+    tma_load_1d(sStage + 0 * TILE * 4, T.priority + start, cnt * 4u, bar);
+    tma_load_1d(sStage + 1 * TILE * 4, T.numdep + start, cnt * 4u, bar);
+    tma_load_1d(sStage + 2 * TILE * 4, T.gid + start, cnt * 4u, bar);
+    tma_load_1d(sStage + 3 * TILE * 4, T.flags + start, cnt * 4u, bar);
+    tma_load_1d(sStage + 16 * TILE + 0 * TILE * 8, T.expected + start, cnt * 8u, bar);
+    tma_load_1d(sStage + 16 * TILE + 1 * TILE * 8, T.qbasis + start, cnt * 8u, bar);
+    tma_load_1d(sStage + 16 * TILE + 2 * TILE * 8, T.wbasis + start, cnt * 8u, bar);
   };
-  if (tid == 0) { issue(0); if (NST > 1 && n_tiles > 1) issue(1); }
+  if (tid == 0) issue(0);
 
   unsigned int c_dm = 0, c_mq = 0, c_over = 0, c_wait = 0, c_sec = 0, c_cnt = 0;
   int64_t s_exp = 0, s_over = 0;
@@ -262,7 +206,7 @@ k_plan_cta(DTasks T, DDistros D, DWork W, const int32_t* __restrict__ list, int6
   }
   __syncthreads();
 
-  const uint32_t a_full0 = smem_u32(&sBar[0]), a_empty0 = smem_u32(&sBar[2]);
+  const uint32_t a_full = smem_u32(&sBar[0]), a_empty = smem_u32(&sBar[2]);
   const uint32_t opaque_zero = uint32_t(t_pad) & 3u;  // 0 at run time, unknown at compile time
   // Work list of task-group tasks: warp w owns entries [w*kSeg, (w+1)*kSeg) through every later phase.  Tile slots are dealt
   // to warps 32 tasks at a time, so the stretches fill evenly; one that overflows hands the distro to k_plan_smem.
@@ -270,14 +214,11 @@ k_plan_cta(DTasks T, DDistros D, DWork W, const int32_t* __restrict__ list, int6
   const int wl0 = warp * kSeg;
   const unsigned lt_mask = (1u << lane) - 1u;
   unsigned int wl_n = 0;
-  const uint32_t* st32_0 = reinterpret_cast<const uint32_t*>(sStage) + tid;
-  const int64_t* st64_0 = reinterpret_cast<const int64_t*>(sStage + 16 * TILE) + tid;
+  const uint32_t* st32 = reinterpret_cast<const uint32_t*>(sStage) + tid;
+  const int64_t* st64 = reinterpret_cast<const int64_t*>(sStage + 16 * TILE) + tid;
   for (int k = 0; k < n_tiles; k++) {
-    const int s = k % NST;
-    const uint32_t ph = uint32_t(k / NST) & 1u;
-    mbar_wait_a(a_full0 + 8u * s, ph);  // the tile's bytes have landed
-    const uint32_t* st32 = st32_0 + s * (L::kStageBytes / 4);
-    const int64_t* st64 = st64_0 + s * (L::kStageBytes / 8);
+    const uint32_t ph = uint32_t(k) & 1u;
+    mbar_wait_a(a_full, ph);  // the tile's bytes have landed
     int32_t prio[TPT], nd[TPT], gid[TPT];
     uint32_t fl[TPT];
     int64_t exp_ns[TPT], qb[TPT], wb[TPT];
@@ -292,17 +233,15 @@ k_plan_cta(DTasks T, DDistros D, DWork W, const int32_t* __restrict__ list, int6
     // back until the loads have actually read shared memory (without this, a rare warp scored the NEXT tile's bytes).
     // So the arrive's address is made data-dependent on every loaded register -- an AND with a zero the
     // compiler cannot prove (t_pad is a multiple of four) -- which waits on the loads' scoreboard and nothing else.
-#ifndef EVG_CTA_LATE_ARRIVE
     {
       uint32_t acc = 0;
 #pragma unroll
       for (int u = 0; u < TPT; u++)
         acc ^= uint32_t(prio[u]) ^ uint32_t(nd[u]) ^ uint32_t(gid[u]) ^ fl[u] ^ uint32_t(uint64_t(exp_ns[u])) ^ uint32_t(uint64_t(exp_ns[u]) >> 32) ^
                uint32_t(uint64_t(qb[u])) ^ uint32_t(uint64_t(qb[u]) >> 32) ^ uint32_t(uint64_t(wb[u])) ^ uint32_t(uint64_t(wb[u]) >> 32);
-      mbar_arrive_a(a_empty0 + 8u * s + (acc & opaque_zero));
+      mbar_arrive_a(a_empty + (acc & opaque_zero));
     }
-    if (tid == 0 && k + NST < n_tiles) { mbar_wait_a(a_empty0 + 8u * s, ph); issue(k + NST); }
-#endif
+    if (tid == 0 && k + 1 < n_tiles) { mbar_wait_a(a_empty, ph); issue(k + 1); }
     int idx[TPT];
     bool complex_task[TPT], scores[TPT];
     uint32_t nd_term[TPT];
@@ -358,10 +297,6 @@ k_plan_cta(DTasks T, DDistros D, DWork W, const int32_t* __restrict__ list, int6
         wl_n += __popc(m);
       }
     }
-#ifdef EVG_CTA_LATE_ARRIVE
-    mbar_arrive_a(a_empty0 + 8u * s);
-    if (tid == 0 && k + NST < n_tiles) { mbar_wait_a(a_empty0 + 8u * s, ph); issue(k + NST); }
-#endif
   }
   // fold the queue-info partials: warp shuffle, then shared atomics
   {
@@ -633,11 +568,7 @@ k_plan_cta(DTasks T, DDistros D, DWork W, const int32_t* __restrict__ list, int6
     const int seg = ((tn + NW - 1) / NW + 31) & ~31;
     const int seg0 = warp * seg;
     const int seg1 = min(seg0 + seg, tn);
-#ifdef EVG_CTA_NOFULL
-    const bool full_seg = false;
-#else
     const bool full_seg = seg1 - seg0 == ITEMS * 32;  // warp-uniform: every lane of every chunk holds an element
-#endif
     const unsigned lt = (1u << lane) - 1u;
     const int npass = (bits + MAXBITS - 1) / MAXBITS;
     const int wbase = npass ? bits / npass : 0, wrem = npass ? bits % npass : 0;
@@ -669,11 +600,7 @@ k_plan_cta(DTasks T, DDistros D, DWork W, const int32_t* __restrict__ list, int6
         // atomics execute in order, so chunk j+1's returned count includes chunk j's add), then their shuffles.  The
         // returns are first needed by the shuffles, so RB atomic round trips overlap instead of queueing behind each other
         // (the single-chunk form waits on that one dependent chain per chunk).
-#ifdef EVG_CTA_RB
-        constexpr int RB = EVG_CTA_RB;
-#else
         constexpr int RB = 1;  // one chunk per trip: with more, the extra live registers spill
-#endif
 #pragma unroll
         for (int j0 = 0; j0 < ITEMS; j0 += RB) {
           unsigned peers[RB];

@@ -24,27 +24,6 @@
 // Reference: scheduler/planner.go:209-481, scheduler/scheduler.go:56-159.
 #pragma once
 
-// minimum resident blocks of the work-list kernels (latency-bound: one thread per task or unit, scattered sectors)
-#ifndef EVG_OCC_GLINK
-#define EVG_OCC_GLINK 4
-#endif
-#ifndef EVG_OCC_GALLOC
-#define EVG_OCC_GALLOC 4
-#endif
-#ifndef EVG_OCC_GFILL
-#define EVG_OCC_GFILL 4
-#endif
-#ifndef EVG_OCC_GUNIT
-#define EVG_OCC_GUNIT 4
-#endif
-#ifndef EVG_OCC_GBEST
-#define EVG_OCC_GBEST 4
-#endif
-#ifndef EVG_GTASK_OCC
-// 2 blocks of 256 per SM: k_gtask fits its registers without spilling on sm_90a (at 3 it spills ~200 B a thread);
-// on H100 that took the kernel from 0.17 to 0.135 ms on 48 distros x 100 000 tasks of configs[2]'s mix
-#define EVG_GTASK_OCC 2
-#endif
 constexpr int kGTile = 2048;  // tasks per tile; tiles start at multiples of 4 tasks (16-byte aligned vector loads)
 
 struct DGen {
@@ -144,7 +123,10 @@ struct TileFold {  // queue-info partials of one tile (scheduler.go:66-138)
 
 // Per tile: queue info, single-task scores, unit links.  256 threads x 8 tasks: thread q of group u owns the four
 // consecutive task slots tile_start + 4*(u*256 + q) .. +3, so every column is read with 128-bit loads.
-__global__ void __launch_bounds__(256, EVG_GTASK_OCC) k_gtask(DTasks T, DDistros D, DWork W, DGen G, int64_t now, int any_complex) {
+// 2 blocks of 256 per SM: k_gtask fits its registers without spilling on sm_90a (at 3 it spills ~200 B a thread);
+// on H100 that took the kernel from 0.17 to 0.135 ms on 48 distros x 100 000 tasks of configs[2]'s mix
+constexpr int kGTaskOcc = 2;
+__global__ void __launch_bounds__(256, kGTaskOcc) k_gtask(DTasks T, DDistros D, DWork W, DGen G, int64_t now, int any_complex) {
   if (*W.err) return;
   __shared__ TileFold F;
   __shared__ evg_distro_cfg s_cfg;
@@ -422,7 +404,11 @@ __device__ __forceinline__ void wl_pairs(const DTasks& T, const DGen& G, const W
     }
 }
 
-__global__ void __launch_bounds__(256, EVG_OCC_GLINK) k_glink(DTasks T, DDistros D, DWork W, DGen G, int64_t now) {
+// minimum resident blocks of the unit-table kernels k_glink .. k_gbest (latency-bound: one thread per task or unit,
+// scattered sectors)
+constexpr int kUnitTableOcc = 4;
+
+__global__ void __launch_bounds__(256, kUnitTableOcc) k_glink(DTasks T, DDistros D, DWork W, DGen G, int64_t now) {
   if (*W.err) return;
   const unsigned int n = *G.ccount;
   for (unsigned int k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x) {
@@ -475,7 +461,7 @@ __global__ void __launch_bounds__(256, EVG_OCC_GLINK) k_glink(DTasks T, DDistros
 
 // Runs are reserved block by block: a block scan of the records its threads need, ONE atomic on the bump counter per
 // block and trip (an atomic per unit serialises ~10^5 units of a tick on one L2 address).
-__global__ void __launch_bounds__(256, EVG_OCC_GALLOC) k_galloc(DTasks T, DDistros D, DWork W, DGen G) {
+__global__ void __launch_bounds__(256, kUnitTableOcc) k_galloc(DTasks T, DDistros D, DWork W, DGen G) {
   if (*W.err) return;
   __shared__ uint32_t s_wsum[8], s_wcnt[8];
   __shared__ uint32_t s_base, s_hbase;
@@ -515,7 +501,7 @@ __global__ void __launch_bounds__(256, EVG_OCC_GALLOC) k_galloc(DTasks T, DDistr
   }
 }
 
-__global__ void __launch_bounds__(256, EVG_OCC_GFILL) k_gfill(DTasks T, DDistros D, DWork W, DGen G) {
+__global__ void __launch_bounds__(256, kUnitTableOcc) k_gfill(DTasks T, DDistros D, DWork W, DGen G) {
   if (*W.err) return;
   const unsigned int n = *G.ccount;
   for (unsigned int k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x) {
@@ -538,7 +524,7 @@ constexpr uint32_t kRankOne = 8;
 constexpr int kRankKey = 6;  // tgo, nd, prio, expected (two words), index
 
 // One thread per multi-member unit (dense warps: the unit list, not the work list).
-__global__ void __launch_bounds__(256, EVG_OCC_GUNIT) k_gunit(DDistros D, DWork W, DGen G, int64_t now) {
+__global__ void __launch_bounds__(256, kUnitTableOcc) k_gunit(DDistros D, DWork W, DGen G, int64_t now) {
   if (*W.err) return;
   const unsigned int n = *G.hcount;
   __shared__ uint32_t s_key[kRankOne * kRankKey][256];  // this thread's column: the rank keys of a small unit's members
@@ -589,7 +575,7 @@ __global__ void __launch_bounds__(256, EVG_OCC_GUNIT) k_gunit(DDistros D, DWork 
 // Ranks of the units above kRankOne members: a warp per 32 members (lane = member), the whole run streamed past them 32
 // records at a time (coalesced) and broadcast with shuffles.  n members cost n comparisons per lane, in parallel over
 // the ceil(n / 32) warps of the unit.
-__global__ void __launch_bounds__(256, EVG_OCC_GUNIT) k_grank(DWork W, DGen G) {
+__global__ void __launch_bounds__(256, kUnitTableOcc) k_grank(DWork W, DGen G) {
   if (*W.err) return;
   const unsigned int n = *G.bcount;
   const unsigned full = 0xffffffffu;
@@ -620,7 +606,7 @@ __global__ void __launch_bounds__(256, EVG_OCC_GUNIT) k_grank(DWork W, DGen G) {
   }
 }
 
-__global__ void __launch_bounds__(256, EVG_OCC_GBEST) k_gbest(DTasks T, DDistros D, DWork W, DGen G, int want_best_pair) {
+__global__ void __launch_bounds__(256, kUnitTableOcc) k_gbest(DTasks T, DDistros D, DWork W, DGen G, int want_best_pair) {
   if (*W.err) return;
   const unsigned int n = *G.ccount;
   const unsigned full = 0xffffffffu;

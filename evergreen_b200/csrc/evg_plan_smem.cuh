@@ -39,12 +39,6 @@ struct PlanShared {
 };
 
 // cp.async (LDGSTS): global -> shared without a register round trip
-__device__ __forceinline__ void cp_async4(void* smem_dst, const void* gmem_src) {
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(uint32_t(__cvta_generic_to_shared(smem_dst))), "l"(gmem_src) : "memory");
-}
-__device__ __forceinline__ void cp_async8(void* smem_dst, const void* gmem_src) {
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(uint32_t(__cvta_generic_to_shared(smem_dst))), "l"(gmem_src) : "memory");
-}
 __device__ __forceinline__ void cp_async4_s(uint32_t smem_addr, const void* gmem_src) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_addr), "l"(gmem_src) : "memory");
 }
@@ -64,7 +58,6 @@ __device__ __forceinline__ void smem_add64(unsigned long long* addr, unsigned lo
 }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void cp_async_wait_but_newest() { asm volatile("cp.async.wait_group 1;" ::: "memory"); }
 
 // (A vote-based replacement for MATCH.ANY -- 9 ballots per chunk -- issues more instructions per chunk.)
 __device__ __forceinline__ unsigned long long ord_i64(int64_t v) { return uint64_t(v) ^ 0x8000000000000000ULL; }
@@ -173,20 +166,19 @@ k_plan_smem(DTasks T, DDistros D, DWork W, const int32_t* __restrict__ list, con
   const bool sane_clock = threshold >= 0 && now >= threshold;
   const int64_t wait_cutoff = wsub(now, threshold);
   const bool fast_clock = now >= 0 && pf.nd_int != 0;  // single_task_value_fast's distro-wide preconditions
-  // The seven columns of the next EVG_STAGES iterations are staged with cp.async while this one computes
-  // (4 x 4 B + 3 x 8 B per thread and stage; each thread reads back only what it copied itself).  Stage 0 lives
-  // in the index region, stage 1 in the anchor/rank region -- both idle until phase 3.
+  // The seven columns of the next iteration are staged with cp.async while this one computes (4 x 4 B + 3 x 8 B per
+  // thread; each thread reads back only what it copied itself).  One stage in flight: the loop is issue-bound, a
+  // second stage does not shorten it.  The index region (b = 0) and the anchor/rank region (b = 1) are both idle until
+  // phase 3; the stage lives in the index region.
   constexpr bool kStage = size_t(4) * CAP >= size_t(THREADS) * 40;
-  // per stage: [4][THREADS] priority, num_dependents, group_id, flags, then [3][THREADS] expected, queue_basis, wait_basis
+  // [4][THREADS] priority, num_dependents, group_id, flags, then [3][THREADS] expected, queue_basis, wait_basis
   auto stage32 = [&](int b) { return reinterpret_cast<uint32_t*>(b ? sA : sIdx); };
   auto stage64 = [&](int b) { return reinterpret_cast<int64_t*>(stage32(b) + 4 * THREADS); };
-  const uint32_t st32_s0 = uint32_t(__cvta_generic_to_shared(stage32(0) + tid)), st32_s1 = uint32_t(__cvta_generic_to_shared(stage32(1) + tid));
-  const uint32_t st64_s0 = uint32_t(__cvta_generic_to_shared(stage64(0) + tid)), st64_s1 = uint32_t(__cvta_generic_to_shared(stage64(1) + tid));
-  auto prefetch = [&](int i0, int b) {  // always closes a copy group (possibly empty) so wait_group counts iterations
+  const uint32_t a32 = uint32_t(__cvta_generic_to_shared(stage32(0) + tid)), a64 = uint32_t(__cvta_generic_to_shared(stage64(0) + tid));
+  auto prefetch = [&](int i0) {  // always closes a copy group (possibly empty)
     const int i = i0 + tid;
     if (i < tn) {
       const int64_t t = base + i;
-      const uint32_t a32 = b ? st32_s1 : st32_s0, a64 = b ? st64_s1 : st64_s0;
       cp_async4_s(a32 + 0 * THREADS * 4, T.priority + t);
       cp_async4_s(a32 + 1 * THREADS * 4, T.numdep + t);
       cp_async4_s(a32 + 2 * THREADS * 4, T.gid + t);
@@ -197,28 +189,23 @@ k_plan_smem(DTasks T, DDistros D, DWork W, const int32_t* __restrict__ list, con
     }
     cp_async_commit();
   };
-#ifndef EVG_STAGES
-#define EVG_STAGES 1  // one stage in flight: the loop is issue-bound, a second stage does not shorten it
-#endif
-  if (kStage) { prefetch(0, 0); if (EVG_STAGES == 2) prefetch(THREADS, 1); }
-  int stage = 0;
-  for (int i0 = 0; i0 < tn; i0 += THREADS, stage ^= (EVG_STAGES == 2 ? 1 : 0)) {
+  if (kStage) prefetch(0);
+  for (int i0 = 0; i0 < tn; i0 += THREADS) {
     const int i = i0 + tid;
     bool complex_task = false, scores = false;
     int32_t prio = 0, nd = 0, gid = -1;
     int64_t exp_ns = 0, qb = 0, wb = 0;
     uint32_t fl = 0;
     if (kStage) {
-      if (EVG_STAGES == 2) cp_async_wait_but_newest();  // this iteration's stage has landed; the next one may still be in flight
-      else cp_async_wait_all();
+      cp_async_wait_all();
       if (i < tn) {
-        const uint32_t* st32 = stage32(stage);
-        const int64_t* st64 = stage64(stage);
+        const uint32_t* st32 = stage32(0);
+        const int64_t* st64 = stage64(0);
         prio = int32_t(st32[0 * THREADS + tid]); nd = int32_t(st32[1 * THREADS + tid]);
         gid = int32_t(st32[2 * THREADS + tid]); fl = st32[3 * THREADS + tid];
         exp_ns = st64[0 * THREADS + tid]; qb = st64[1 * THREADS + tid]; wb = st64[2 * THREADS + tid];
       }
-      prefetch(i0 + EVG_STAGES * THREADS, stage);  // refill the stage just consumed
+      prefetch(i0 + THREADS);  // refill the stage just consumed
     } else if (i < tn) {
       const int64_t t = base + i;
       prio = T.priority[t]; nd = T.numdep[t]; gid = T.gid[t]; fl = T.flags[t];

@@ -22,11 +22,10 @@ __device__ __forceinline__ int64_t shfl64(int64_t v, int src) {
   return int64_t((uint64_t(hi) << 32) | lo);
 }
 
-#ifndef EVG_WARP_OCC
-#define EVG_WARP_OCC 4  // blocks of 8 distros per SM: 64 registers (sm_90a: 16 B spill stores, 56 B spill loads) keep more
-                        // distros in flight than 3 (no spill), which was slower on H100 for configs[2] total and configs[4]
-#endif
-__global__ void __launch_bounds__(256, EVG_WARP_OCC) k_plan_warp(DTasks T, DDistros D, DWork W, const int32_t* __restrict__ list,
+// 4 blocks of 8 distros per SM: 64 registers (sm_90a: 16 B spill stores, 56 B spill loads) keep more distros in flight
+// than 3 (no spill), which was slower on H100 for configs[2] total and configs[4]
+constexpr int kWarpOcc = 4;
+__global__ void __launch_bounds__(256, kWarpOcc) k_plan_warp(DTasks T, DDistros D, DWork W, const int32_t* __restrict__ list,
                                                    int n_list, int64_t now, int32_t* __restrict__ order,
                                                    int64_t* __restrict__ total_value) {
   if (*W.err) return;

@@ -145,11 +145,8 @@ constexpr bool largest_first(int r) { return r != kWarp && r != kGeneral; }
 constexpr int kRouteStream[kRoutes + 1] = {4, 5, 3, 2, 1, 0, 0, 0, 0};
 
 // on-chip planner classes <THREADS, ITEMS>: capacity = THREADS*ITEMS tasks per distro
-#ifndef EVG_C_THREADS  // shape of the largest on-chip class (threads x tasks per thread = 12288 tasks in 218 KB)
-#define EVG_C_THREADS 1024
-#define EVG_C_ITEMS 12
-#endif
-constexpr int kCapA = 128 * 8, kCapB = 256 * 16, kCapC = EVG_C_THREADS * EVG_C_ITEMS;
+constexpr int kThreadsC = 1024, kItemsC = 12;  // the largest class: 12288 tasks in 218 KB
+constexpr int kCapA = 128 * 8, kCapB = 256 * 16, kCapC = kThreadsC * kItemsC;
 constexpr int64_t kWideAllocGroups = 1024;  // k_alloc<128> (a block per distro) once some distro has more task groups
 constexpr int kCapW = 32;  // k_plan_warp: one warp per distro
 constexpr int64_t kGrouplessHosts = 64;  // k_alloc_groupless walks a distro's hosts with one thread: only short walks
@@ -270,16 +267,6 @@ __device__ __forceinline__ int64_t warp_sum64(int64_t v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
-}
-__device__ __forceinline__ uint64_t warp_or64(uint64_t v) {
-  uint32_t lo = __reduce_or_sync(0xffffffffu, uint32_t(v));
-  uint32_t hi = __reduce_or_sync(0xffffffffu, uint32_t(v >> 32));
-  return (uint64_t(hi) << 32) | lo;
-}
-__device__ __forceinline__ uint64_t warp_and64(uint64_t v) {
-  uint32_t lo = __reduce_and_sync(0xffffffffu, uint32_t(v));
-  uint32_t hi = __reduce_and_sync(0xffffffffu, uint32_t(v >> 32));
-  return (uint64_t(hi) << 32) | lo;
 }
 __device__ __forceinline__ void atomic_add64(int64_t* p, int64_t v) {
   if (v != 0) atomicAdd(reinterpret_cast<unsigned long long*>(p), (unsigned long long)v);
@@ -1917,7 +1904,7 @@ int plan_route(evg_ctx* c, int r, Mode mode, cudaStream_t st, const DTasks& dt, 
   const int32_t* list = punt;
   if (r != kPunted) list = (mode != Mode::kPipelined && largest_first(r) ? c->routes[r].lpt : c->routes[r].b).as<int32_t>() + first;
   // breakdown needs the unit lists: every k_plan_cta distro goes through k_plan_smem (its largest class holds them all)
-  if (bd && is_cta(r)) return launch_smem<EVG_C_THREADS, EVG_C_ITEMS, 1>(c, st, dt, dd, w, list, n, now, 1);
+  if (bd && is_cta(r)) return launch_smem<kThreadsC, kItemsC, 1>(c, st, dt, dd, w, list, n, now, 1);
   int rc;
   switch (r) {
     case kCtaC: return launch_cta<kNT_C, kNCapC, kNOccC>(c, st, dt, dd, w, list, n, now, punt, punt_count);
@@ -1934,8 +1921,8 @@ int plan_route(evg_ctx* c, int r, Mode mode, cudaStream_t st, const DTasks& dt, 
       // 1024-thread CTAs are not free); the pipelined call always takes the largest
       if (mode == Mode::kResident && c->max_cta_tasks <= kCapA) return launch_smem<128, 8, 8>(c, st, dt, dd, w, list, n, now, 0, punt_count);
       if (mode == Mode::kResident && c->max_cta_tasks <= kCapB) return launch_smem<256, 16, 3>(c, st, dt, dd, w, list, n, now, 0, punt_count);
-      return launch_smem<EVG_C_THREADS, EVG_C_ITEMS, 1>(c, st, dt, dd, w, list, n, now, 0, punt_count);
-    case kSmemC: return launch_smem<EVG_C_THREADS, EVG_C_ITEMS, 1>(c, st, dt, dd, w, list, n, now, bd);
+      return launch_smem<kThreadsC, kItemsC, 1>(c, st, dt, dd, w, list, n, now, 0, punt_count);
+    case kSmemC: return launch_smem<kThreadsC, kItemsC, 1>(c, st, dt, dd, w, list, n, now, bd);
     case kSmemB: return launch_smem<256, 16, 3>(c, st, dt, dd, w, list, n, now, bd);
     case kSmemA: return launch_smem<128, 8, 8>(c, st, dt, dd, w, list, n, now, bd);
     case kWarp: return launch_tiny(c, st, dt, dd, w, list, n, now, bd);

@@ -1,5 +1,5 @@
 """Diagnostic: per-step device time of the resident configs[1] tick over a long run (clock ramp check).
-usage: python profiles/ab_test.py [path/to/libevgsched.so] [iterations]"""
+usage: python profiles/ab_build.py [path/to/libevgsched.so] [iterations]"""
 import sys, os, time, ctypes as C
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np

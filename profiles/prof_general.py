@@ -6,7 +6,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import ctypes as C
 import numpy as np
 from evergreen_b200 import _lib as L
-if len(sys.argv) > 3:  # another build of the library (profiles/ab_variants.py build ...)
+if len(sys.argv) > 3:  # another build of the library, e.g. another commit's, to compare the two
     lib = C.CDLL(sys.argv[3])
     for name, (res, args) in L.SYMBOLS.items():
         if hasattr(lib, name):

@@ -17,7 +17,7 @@ import numpy as np  # noqa: E402
 
 from evergreen_b200 import _lib as L  # noqa: E402
 
-if len(sys.argv) > 3:  # another build of the library (profiles/ab_variants.py build ...)
+if len(sys.argv) > 3:  # another build of the library, e.g. another commit's, to compare the two
     lib = C.CDLL(sys.argv[3])
     for name, (res, args) in L.SYMBOLS.items():
         if hasattr(lib, name):
