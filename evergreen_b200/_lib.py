@@ -298,6 +298,18 @@ class HostTermOutStruct(C.Structure):  # evg_host_drawdown_out and evg_idle_host
     _fields_ = [("hosts", C.c_void_p), ("distros", C.c_void_p)]
 
 
+# the start-time estimator's host table (evg_estimate_start_times / evg_estimate_start_batch)
+EVG_EH_UNINITIALIZED, EVG_EH_STARTING, EVG_EH_PROVISIONING, EVG_EH_FREE, EVG_EH_RUNNING, EVG_EH_IGNORED = range(6)
+EVG_EST_ONCHIP_HOSTS = 1024
+
+
+class EstHostSoAStruct(C.Structure):
+    _fields_ = [("n_hosts", C.c_int64), ("kind", C.c_void_p), ("expected_ns", C.c_void_p), ("dispatch_ns", C.c_void_p)]
+
+
+assert C.sizeof(EstHostSoAStruct) == 32
+
+
 class EvgError(RuntimeError):
     def __init__(self, code: int, msg: str):
         super().__init__(f"libevgsched error {code}: {msg}")
@@ -351,6 +363,8 @@ SYMBOLS = {
     "evg_host_job": (C.c_int, [_P, _P, _P, _P]),
     "evg_host_drawdown": (C.c_int, [_P, _P, _P, _P, C.c_int64, _P]),
     "evg_idle_hosts": (C.c_int, [_P, _P, _P, _P, C.c_int64, _P]),
+    "evg_estimate_start_times": (C.c_int, [_P, C.c_int32, _P, _P, C.c_int64, _P, _P, C.c_int64, _P]),
+    "evg_estimate_start_batch": (C.c_int, [_P, _P, _P, C.c_int32, _P, _P, C.c_int64, _P, _P]),
     "evg_plan_distro": (C.c_int, [_P, _P, _P, C.c_int32, _P, C.c_int64, C.c_uint32, _P]),
     "evg_alloc_distro": (C.c_int, [_P, _P, _P, _P, _P, C.c_int32, C.c_int64, _P, _P]),
 }

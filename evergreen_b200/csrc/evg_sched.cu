@@ -298,6 +298,7 @@ __device__ __forceinline__ uint32_t pair_task(const DTasks& T, const DWork& W, u
 #include "evg_legacy.cuh"
 #include "evg_dag.cuh"
 #include "evg_next.cuh"
+#include "evg_estimate.cuh"
 
 // --------------------------------------------------------------------------
 // kernels (general path: any distro size)
@@ -1348,6 +1349,10 @@ struct evg_ctx {
   // evg_host_drawdown / evg_idle_hosts (the first call allocates these): the staged idle-host table, its offsets and the
   // per-distro inputs, the verdicts, the decided flags and their scan, and the per-distro outputs
   struct { DevBuf cols, off, din, verdict, flag, pos, scan_sum, dout; } ih;
+  // evg_estimate_start_times / evg_estimate_start_batch (the first call allocates these): the staged host table, each
+  // row's timeToCompletion and whether it counts, their scan, the packed pools (two copies: the merge sort's), the
+  // queues' offsets and durations, the launch list and the outputs
+  struct { DevBuf kind, expected, dispatch, host_off, ttc, used, pos, scan_sum, pool[2], pool_off, item_off, dur, list, start, hosts_used; } es;
   DevBuf b_err;
   DevBuf b_route, b_unitv, b_unita, b_unitn, b_unitmask;
   DevBuf b_punt, b_puntcnt;
@@ -2212,15 +2217,21 @@ __global__ void __launch_bounds__(256) k_project_queue(DTasks T, DDistros D, con
   items[j] = q;
 }
 
+// The persisted head of every queue of the resident tick: item_off[d + 1] - item_off[d] = min(length, cap) (cap > 0).
+// Returns the rows in all.
+static int64_t persisted_item_off(const evg_ctx* c, int32_t cap, int64_t* item_off) {
+  item_off[0] = 0;
+  for (int32_t d = 0; d < c->Dn; d++) item_off[d + 1] = item_off[d] + std::min<int64_t>(c->h_taskoff[d + 1] - c->h_taskoff[d], cap);
+  return item_off[c->Dn];
+}
+
 int evg_download_queue(evg_ctx* c, int32_t cap, int64_t* item_off, evg_queue_item* items, int64_t items_capacity) {
   ENTER(c, "evg_download_queue");
   if (const int rc = need_tick(c, who, Need::kTick); rc != EVG_OK) return rc;
   if (cap < 0 || !item_off) return fail(EVG_ERR_INVALID, "evg_download_queue: bad argument");
   if (cap == 0) cap = EVG_PERSISTED_QUEUE_CAP;
   const int32_t D = c->Dn;
-  item_off[0] = 0;
-  for (int32_t d = 0; d < D; d++) item_off[d + 1] = item_off[d] + std::min<int64_t>(c->h_taskoff[d + 1] - c->h_taskoff[d], cap);
-  const int64_t n = item_off[D];
+  const int64_t n = persisted_item_off(c, cap, item_off);
   if (n > items_capacity || (n > 0 && !items)) return fail(EVG_ERR_INVALID, "evg_download_queue: %lld rows needed, %lld available", (long long)n, (long long)items_capacity);
   if (n == 0) return EVG_OK;
   cudaStream_t s = c->stream;
@@ -4794,6 +4805,113 @@ int evg_idle_hosts(evg_ctx* c, const evg_idle_host_soa* hosts, const int64_t* id
   if (H > 0) scan_counts(c, x.flag.as<int32_t>(), H, pos, x.scan_sum.as<int64_t>());
   launch(c, c->stream, k_idle_distro, grid_for(D, 256), 256, 0, D, off, dcfg, static_cast<const int64_t*>(pos), x.dout.as<evg_idle_distro>());
   return finish_idle_hosts(c, H, out->hosts, out->distros, sizeof(evg_idle_distro) * size_t(D));
+}
+
+// The host table and its offsets, checked before anything is staged or launched.
+static int check_est_hosts(const char* who, const evg_est_host_soa* h, const int64_t* off, int32_t D) {
+  if (!h || !off) return fail(EVG_ERR_INVALID, "%s: null host table or est_host_off", who);
+  if (h->n_hosts < 0) return fail(EVG_ERR_INVALID, "%s: negative n_hosts", who);
+  if (h->n_hosts > 0 && (!h->kind || !h->expected_ns || !h->dispatch_ns)) return fail(EVG_ERR_INVALID, "%s: null host column", who);
+  if (const int rc = check_offsets(off, D, h->n_hosts, who, "est_host_off"); rc != EVG_OK) return rc;
+  for (int64_t i = 0; i < h->n_hosts; i++)
+    if (h->kind[i] > EVG_EH_IGNORED) return fail(EVG_ERR_INVALID, "%s: host row %lld has kind %d", who, (long long)i, int(h->kind[i]));
+  return EVG_OK;
+}
+
+// What the two estimate entry points share: the queues' offsets and durations are in es.item_off / es.dur (item_off is
+// the host copy); the pools are built, sorted and simulated, and the estimates and pool sizes copied out.
+static int estimate_run(evg_ctx* c, int32_t D, const evg_est_host_soa* h, const int64_t* host_off, int64_t now, const int64_t* item_off,
+                        int64_t* start_ns, int32_t* hosts_used) {
+  const int64_t H = h->n_hosts, N = item_off[D];
+  if (H == 0) {  // len(s.hosts) == 0 everywhere (:54-56): answered here, as evg_find_next_tasks answers empty queues
+    std::fill(start_ns, start_ns + N, int64_t(-1));
+    std::fill(hosts_used, hosts_used + D, 0);
+    return EVG_OK;
+  }
+  auto& x = c->es;
+  cudaStream_t s = c->stream;
+  UP(s, x.kind, h->kind, H, uint8_t);
+  UP(s, x.expected, h->expected_ns, H, int64_t);
+  UP(s, x.dispatch, h->dispatch_ns, H, int64_t);
+  UP(s, x.host_off, host_off, D + 1, int64_t);
+  for (DevBuf* b : {&x.ttc, &x.pool[0], &x.pool[1]}) CK(b->ensure(sizeof(int64_t) * size_t(H)));
+  CK(x.used.ensure(sizeof(int32_t) * size_t(H)));
+  CK(x.pos.ensure(sizeof(int64_t) * size_t(H + 1)));
+  CK(x.scan_sum.ensure(sizeof(int64_t) * size_t((H + 1023) / 1024 + 1)));
+  CK(x.pool_off.ensure(sizeof(int64_t) * size_t(D + 1)));
+  CK(x.hosts_used.ensure(sizeof(int32_t) * size_t(D)));
+  launch(c, s, k_es_host, grid_for(H, 256), 256, 0, H, x.kind.as<uint8_t>(), x.expected.as<int64_t>(), x.dispatch.as<int64_t>(), now,
+         x.ttc.as<int64_t>(), x.used.as<int32_t>());
+  scan_counts(c, x.used.as<int32_t>(), H, x.pos.as<int64_t>(), x.scan_sum.as<int64_t>());
+  launch(c, s, k_es_compact, grid_for(H, 256), 256, 0, H, x.ttc.as<int64_t>(), x.used.as<int32_t>(), x.pos.as<int64_t>(), x.pool[0].as<int64_t>());
+  launch(c, s, k_es_pool_off, grid_for(D + 1, 256), 256, 0, D, x.host_off.as<int64_t>(), x.pos.as<int64_t>(), x.pool_off.as<int64_t>(),
+         x.hosts_used.as<int32_t>());
+  // one warp per distro that has host rows and items, the largest items x hosts first
+  std::vector<int32_t> list;
+  int64_t max_hosts = 0;
+  for (int32_t d = 0; d < D; d++)
+    if (host_off[d + 1] > host_off[d] && item_off[d + 1] > item_off[d]) {
+      list.push_back(d);
+      max_hosts = std::max(max_hosts, host_off[d + 1] - host_off[d]);
+    }
+  if (!list.empty()) {
+    const auto work = [&](int32_t d) { return double(host_off[d + 1] - host_off[d]) * double(item_off[d + 1] - item_off[d]); };
+    std::stable_sort(list.begin(), list.end(), [&](int32_t a, int32_t b) { return work(a) > work(b); });
+    UP(s, x.list, list.data(), int64_t(list.size()), int32_t);
+    CK(x.start.ensure(sizeof(int64_t) * size_t(N)));
+    int cur = 0;
+    for (int64_t L = 1; L < max_hosts; L <<= 1, cur ^= 1)
+      launch(c, s, k_es_sort_pass, grid_for(H, 256), 256, 0, D, x.pool_off.as<int64_t>(), x.pool[cur].as<int64_t>(), x.pool[cur ^ 1].as<int64_t>(), L);
+    CK(cudaMemsetAsync(x.start.p, 0xFF, sizeof(int64_t) * size_t(N), s));  // -1: no estimate
+    const DEst X{x.list.as<int32_t>(), int32_t(list.size()), x.pool_off.as<int64_t>(), x.item_off.as<int64_t>(), x.dur.as<int64_t>(),
+                 x.pool[cur].as<int64_t>(), x.start.as<int64_t>()};
+    launch(c, s, k_es_sim, grid_for(int64_t(list.size()), kEsWarps), 32 * kEsWarps, 0, X);
+  }
+  CK(cudaGetLastError());
+  if (list.empty()) std::fill(start_ns, start_ns + N, int64_t(-1));  // the distros with items have no host rows
+  else CK(cudaMemcpyAsync(start_ns, x.start.p, sizeof(int64_t) * size_t(N), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(hosts_used, x.hosts_used.p, sizeof(int32_t) * size_t(D), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  return EVG_OK;
+}
+
+int evg_estimate_start_times(evg_ctx* c, int32_t cap, const evg_est_host_soa* hosts, const int64_t* est_host_off, int64_t now_ns,
+                             int64_t* item_off, int64_t* start_ns, int64_t items_capacity, int32_t* hosts_used) {
+  ENTER(c, "evg_estimate_start_times");
+  int rc = need_tick(c, who, Need::kTick);
+  if (rc != EVG_OK) return rc;
+  const int32_t D = c->Dn;
+  if (cap < 0 || !item_off || (D > 0 && !hosts_used)) return fail(EVG_ERR_INVALID, "%s: negative cap, or null item_off or hosts_used", who);
+  if ((rc = check_est_hosts(who, hosts, est_host_off, D)) != EVG_OK) return rc;
+  const int64_t N = persisted_item_off(c, cap == 0 ? EVG_PERSISTED_QUEUE_CAP : cap, item_off);
+  if (N > items_capacity || (N > 0 && !start_ns))
+    return fail(EVG_ERR_INVALID, "%s: %lld rows needed, %lld available", who, (long long)N, (long long)items_capacity);
+  c->launches = 0;
+  if (N > 0 && hosts->n_hosts > 0) {
+    auto& x = c->es;
+    UP(c->stream, x.item_off, item_off, D + 1, int64_t);
+    CK(x.dur.ensure(sizeof(int64_t) * size_t(N)));
+    launch(c, c->stream, k_es_gather, grid_for(N, 256), 256, 0, D, N, x.item_off.as<int64_t>(), c->b_taskoff.as<int64_t>(),
+           c->b_order.as<int32_t>(), dtasks(c).expected, x.dur.as<int64_t>());
+  }
+  return estimate_run(c, D, hosts, est_host_off, now_ns, item_off, start_ns, hosts_used);
+}
+
+int evg_estimate_start_batch(evg_ctx* c, const int64_t* durations, const int64_t* item_off, int32_t D, const evg_est_host_soa* hosts,
+                             const int64_t* est_host_off, int64_t now_ns, int64_t* start_ns, int32_t* hosts_used) {
+  ENTER(c, "evg_estimate_start_batch");
+  if (D < 0 || !item_off || (D > 0 && !hosts_used)) return fail(EVG_ERR_INVALID, "%s: negative n_distros, or null item_off or hosts_used", who);
+  int rc = check_offsets(item_off, D, -1, who, "item_off");
+  if (rc != EVG_OK) return rc;
+  const int64_t N = item_off[D];
+  if (N > 0 && (!durations || !start_ns)) return fail(EVG_ERR_INVALID, "%s: null durations or start_ns", who);
+  if ((rc = check_est_hosts(who, hosts, est_host_off, D)) != EVG_OK) return rc;
+  c->launches = 0;
+  if (N > 0 && hosts->n_hosts > 0) {
+    UP(c->stream, c->es.item_off, item_off, D + 1, int64_t);
+    UP(c->stream, c->es.dur, durations, N, int64_t);
+  }
+  return estimate_run(c, D, hosts, est_host_off, now_ns, item_off, start_ns, hosts_used);
 }
 
 int evg_plan_distro(evg_ctx* c, const evg_task_soa* tasks, const evg_distro_cfg* cfg, int32_t n_groups,

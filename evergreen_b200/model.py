@@ -73,6 +73,11 @@ TASK_QUEUES_COLLECTION = "task_queues"
 TASK_SECONDARY_QUEUES_COLLECTION = "task_alias_queues"
 DISABLED_TASK_PRIORITY = -1  # globals.go:187
 HOST_RUNNING = "running"  # globals.go:24
+HOST_UNINITIALIZED = "initializing"  # globals.go:26
+HOST_STARTING = "starting"  # globals.go:35
+HOST_PROVISIONING = "provisioning"  # globals.go:36
+# globals.go:975-984: the statuses host.ByDistroIDs returns (model/host/db.go:628-635)
+UP_HOST_STATUS = (HOST_RUNNING, HOST_UNINITIALIZED, "building", HOST_STARTING, HOST_PROVISIONING, "provision failed", "stopping", "stopped")
 # model/distro/distro.go:319-321
 BOOTSTRAP_METHOD_LEGACY_SSH = "legacy-ssh"
 BOOTSTRAP_METHOD_USER_DATA = "user-data"
@@ -132,6 +137,7 @@ class Task:
     scheduled_time: int = ZERO_TIME
     dependencies_met_time: int = ZERO_TIME
     start_time: int = ZERO_TIME
+    dispatch_time: int = ZERO_TIME   # the start-time estimator reads it of a host's running task (task_start_estimation.go:156)
     distro_id: str = ""
     secondary_distros: List[str] = field(default_factory=list)  # Task.SecondaryDistros: the alias queues it may join
     status: str = TASK_UNDISPATCHED

@@ -519,6 +519,37 @@ class Engine:
                                         L.ptr(cfg if D else np.zeros(1, L.IDLE_CFG_DTYPE)), int(now), C.byref(st)))
         return {"hosts": o["hosts"][:H], "distros": o["distros"][:D]}
 
+    def estimate_start_times(self, table: S.EstHostTable, now: int, cap: int = 0, task_off=None):
+        """evg_estimate_start_times: GetEstimatedStartTime for every persisted rank of every distro of the resident tick
+        after run(), on the device.  `table`: soa.marshal_estimate_hosts over the tick's distros; `cap`, `task_off` as
+        download_queue.  -> (item_off, start_ns, hosts_used): start_ns[item_off[d] + r] is the estimate of rank r of
+        distro d (-1: no hosts), hosts_used[d] the size of its host pool."""
+        D = self._n_distros
+        if table.n_distros != D:
+            raise ValueError("one host list per distro of the resident tick")
+        item_off = self._out("est_item_off", D + 1, np.int64)
+        n = self._n_tasks if task_off is None else int(np.minimum(np.diff(task_off), cap or L.EVG_PERSISTED_QUEUE_CAP).sum())
+        start = self._out("est_start", max(n, 1), np.int64)
+        used = self._out("est_hosts_used", max(D, 1), np.int32)
+        L.check(self.lib.evg_estimate_start_times(self.ctx, int(cap), C.byref(table.struct()), L.ptr(table.est_host_off), int(now),
+                                                  L.ptr(item_off), L.ptr(start), int(max(n, 1)), L.ptr(used)))
+        return item_off, start[: int(item_off[D])], used[:D]
+
+    def estimate_start_batch(self, durations, item_off, table: S.EstHostTable, now: int):
+        """evg_estimate_start_batch: the same for caller-supplied queues -- durations[item_off[d] .. item_off[d+1]) are
+        the ExpectedDuration of distro d's queue items in order.  Needs no tick.  -> (start_ns, hosts_used)."""
+        item_off = np.ascontiguousarray(item_off, dtype=np.int64)
+        durations = np.ascontiguousarray(durations, dtype=np.int64)
+        D = item_off.shape[0] - 1
+        if table.n_distros != D or D < 0:
+            raise ValueError("one host list per queue")
+        n = int(durations.shape[0])
+        start = np.zeros(max(n, 1), np.int64)
+        used = np.zeros(max(D, 1), np.int32)
+        L.check(self.lib.evg_estimate_start_batch(self.ctx, L.ptr(durations) if n else None, L.ptr(item_off), D, C.byref(table.struct()),
+                                                  L.ptr(table.est_host_off), int(now), L.ptr(start), L.ptr(used)))
+        return start[:n], used[:D]
+
     def alloc_batch(self, hosts: S.HostSoA, qinfo: np.ndarray, ginfo: np.ndarray, group_off: np.ndarray, now: int):
         D = int(qinfo.shape[0])
         ao = self._alloc_output(D)
@@ -799,6 +830,14 @@ class ResidentTick:
         ids = [self.ranked[d][:int(io[d + 1] - io[d])] for d in range(len(self.ranked))]
         item, outcome = eng.find_next_tasks(S.marshal_next_db(ids, names, db), S.marshal_next_requests(names, requests))
         return _next_results(ids, requests, item, outcome)
+
+    def estimated_start_times(self, hosts_by_distro: Sequence[Sequence[M.Host]], running_tasks: Dict[str, object], now: int, cap: int = 0):
+        """GetEstimatedStartTime for every persisted task of the last plan(), chained on the tick (evg_estimate_start_times):
+        hosts_by_distro[d] are the up hosts of distro d in query order, running_tasks as soa.marshal_estimate_hosts takes
+        them.  -> per distro {task id: estimate in ns} over its persisted ranks (-1: the distro has no hosts); a task
+        that is not there is not queued, for which the reference returns -1."""
+        io, start, _ = self.engine.estimate_start_times(S.marshal_estimate_hosts(hosts_by_distro, running_tasks), now, cap, self.table.task_off)
+        return [dict(zip(ids, start[int(io[d]):int(io[d + 1])].tolist())) for d, ids in enumerate(self.ranked)]
 
     def remember(self, canon, soa: S.TaskSoA, table: S.DistroTable, keys) -> None:
         """Make the marshalled `canon` the resident tick the next diff starts from."""
@@ -1372,6 +1411,34 @@ class CmpBasedTaskPrioritizer:
 
 
 # ---------------------------------------------------------------------------------------------------------------
+def estimated_start_times(queues: Sequence[Optional[M.TaskQueue]], hosts_by_distro: Sequence[Sequence[M.Host]],
+                          running_tasks: Dict[str, object], now: int, *, engine: Optional[Engine] = None) -> List[List[int]]:
+    """model.GetEstimatedStartTime (model/task_start_estimation.go:99-122) for every item of every queue in one call
+    (evg_estimate_start_batch): queues[d] is a distro's TaskQueue document (None: there is none), hosts_by_distro[d] its
+    up hosts in query order; running_tasks as soa.marshal_estimate_hosts takes them.  -> per queue the estimate in ns of
+    each item, -1 without hosts."""
+    eng = engine or default_engine()
+    durations = [[it.expected_duration for it in q.queue] if q is not None else [] for q in queues]
+    off = np.zeros(len(queues) + 1, np.int64)
+    off[1:] = np.cumsum([len(x) for x in durations])
+    start, _ = eng.estimate_start_batch(np.array([v for x in durations for v in x], dtype=np.int64), off,
+                                        S.marshal_estimate_hosts(hosts_by_distro, running_tasks), now)
+    return [start[int(off[d]):int(off[d + 1])].tolist() for d in range(len(queues))]
+
+
+def get_estimated_start_time(task: M.Task, queue: Optional[M.TaskQueue], hosts: Sequence[M.Host], running_tasks: Dict[str, object],
+                             now: int, *, engine: Optional[Engine] = None) -> int:
+    """model.GetEstimatedStartTime for one task: `queue` is the task's distro's queue (None: no document), `hosts` the
+    distro's up hosts.  -1 when there is no queue or the task is not in it (:104-116), neither of which reaches the
+    device."""
+    if queue is None:
+        return -1
+    pos = next((i for i, it in enumerate(queue.queue) if it.id == task.id), -1)
+    if pos == -1:
+        return -1
+    return estimated_start_times([queue], [hosts], running_tasks, now, engine=engine)[0][pos]
+
+
 def rebuild_dag_dispatchers(queues: Sequence[M.TaskQueue], *, engine: Optional[Engine] = None):
     """basicCachedDAGDispatcherImpl.rebuild for a batch of persisted queues (model/task_queue_service_dependency.go:
     153-252).  Per queue: (sorted item ids with None for each dependency cycle's placeholder, number of cycles,

@@ -618,6 +618,58 @@ def marshal_idle_hosts(groups: Sequence[Sequence[M.Host]], default_amis: Optiona
     return IdleHostTable(cols, flags, off, [h.id for h in hosts])
 
 
+@dataclass
+class EstHostTable:
+    """evg_est_host_soa + est_host_off: the start-time estimator's hosts of every distro, in query order."""
+    kind: np.ndarray          # uint8 EVG_EH_*
+    expected_ns: np.ndarray   # int64
+    dispatch_ns: np.ndarray   # int64
+    est_host_off: np.ndarray  # int64, n_distros + 1
+
+    @property
+    def n_hosts(self) -> int:
+        return int(self.kind.shape[0])
+
+    @property
+    def n_distros(self) -> int:
+        return int(self.est_host_off.shape[0]) - 1
+
+    def struct(self) -> L.EstHostSoAStruct:
+        n = self.n_hosts
+        return L.EstHostSoAStruct(n, *[L.ptr(a) if n else None for a in (self.kind, self.expected_ns, self.dispatch_ns)])
+
+
+TASK_LOOKUP_ERROR = object()  # a running_tasks value: task.FindOneIdAndExecution returned an error
+_EST_KIND = {M.HOST_UNINITIALIZED: L.EVG_EH_UNINITIALIZED, M.HOST_STARTING: L.EVG_EH_STARTING, M.HOST_PROVISIONING: L.EVG_EH_PROVISIONING}
+
+
+def marshal_estimate_hosts(hosts_by_distro: Sequence[Sequence[M.Host]], running_tasks: Dict[str, object]) -> EstHostTable:
+    """The hosts host.Find(ByDistroIDs(d)) returned for each distro, in query order -> the estimator's host table, as
+    createSimulatorModel reads them (model/task_start_estimation.go:129-159).  running_tasks[h.running_task] is the
+    running task's document (expected_duration, dispatch_time); absent or None: no document, the host is
+    EVG_EH_IGNORED; TASK_LOOKUP_ERROR: the distro's rows end before that host."""
+    kind, exp, disp, off = [], [], [], [0]
+    for hosts in hosts_by_distro:
+        for h in hosts:
+            k, e, t = _EST_KIND.get(h.status, L.EVG_EH_IGNORED), 0, M.ZERO_TIME
+            if h.status == M.HOST_RUNNING:
+                k = L.EVG_EH_FREE
+                if h.running_task != "":
+                    doc = running_tasks.get(h.running_task)
+                    if doc is TASK_LOOKUP_ERROR:
+                        break
+                    if doc is None:
+                        k = L.EVG_EH_IGNORED
+                    else:
+                        k, e, t = L.EVG_EH_RUNNING, doc.expected_duration, doc.dispatch_time
+            kind.append(k)
+            exp.append(e)
+            disp.append(t)
+        off.append(len(kind))
+    return EstHostTable(np.array(kind, dtype=np.uint8), np.array(exp, dtype=np.int64), np.array(disp, dtype=np.int64),
+                        np.array(off, dtype=np.int64))
+
+
 def queue_info_rows(infos: Sequence[M.DistroQueueInfo]):
     """[DistroQueueInfo] -> (QUEUE_INFO rows, GROUP_INFO rows, group_off, names per distro).
     Later duplicates of a name win, like the map built at allocator.go:243-246."""

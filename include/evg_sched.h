@@ -379,7 +379,7 @@ int evg_bind_result_buffer(evg_ctx* ctx, void* device_ptr, int64_t capacity);
  * evg_plan_and_alloc_batch it runs), evg_plan_and_alloc_batch's pipelined large ticks, evg_alloc_batch / evg_alloc_distro,
  * evg_deps_met_batch, evg_find_runnable_batch / _ex, evg_plan_from_finder / _ex, evg_edit_tasks, evg_plan_aliases,
  * evg_expected_durations_batch, evg_prioritize_legacy_batch, evg_dag_rebuild_batch, evg_rebuild_dispatchers,
- * evg_host_job, evg_host_drawdown, evg_idle_hosts, evg_find_next_batch and evg_find_next_tasks.  Every other call adds the kernels it launches: the uploads (their range check), evg_update_tasks,
+ * evg_host_job, evg_host_drawdown, evg_idle_hosts, evg_find_next_batch, evg_find_next_tasks, evg_estimate_start_times and evg_estimate_start_batch.  Every other call adds the kernels it launches: the uploads (their range check), evg_update_tasks,
  * evg_download_queue and evg_resolve_durations. */
 int64_t evg_last_launch_count(evg_ctx* ctx);
 /* Device time in ms of the last evg_run_resident, from CUDA events on the context
@@ -1199,6 +1199,61 @@ typedef struct {
  * Replaces: the per-host loop of idleHostJob (the shim enqueues a termination job for each EVG_HT_TERM_* row). */
 int evg_idle_hosts(evg_ctx* ctx, const evg_idle_host_soa* hosts, const int64_t* idle_off, const evg_idle_cfg* cfg,
                    int64_t now_ns, evg_idle_hosts_out* out);
+
+/* ---- task start-time estimates (model/task_start_estimation.go) ----------- */
+
+/* evg_est_host_soa.kind: what createSimulatorModel makes of a host (model/task_start_estimation.go:129-159) */
+enum {
+  EVG_EH_UNINITIALIZED = 0, /* Status == evergreen.HostUninitialized: timeToCompletion 4 min (:131-132) */
+  EVG_EH_STARTING = 1,      /* HostStarting: 3 min (:133-134) */
+  EVG_EH_PROVISIONING = 2,  /* HostProvisioning: 1 min (:135-136) */
+  EVG_EH_FREE = 3,          /* HostRunning with RunningTask == "": 0 (:138-139) */
+  EVG_EH_RUNNING = 4,       /* HostRunning with a task: ExpectedDuration - time.Since(DispatchTime) (:156-157) */
+  EVG_EH_IGNORED = 5        /* contributes no host: any other status, or the running task has no document (:148-154) */
+};
+/* A pool of at most this many hosts is simulated in shared memory, a larger one in global memory; same results. */
+#define EVG_EST_ONCHIP_HOSTS 1024
+
+/* The hosts host.Find(ByDistroIDs(distro)) returns (model/task_start_estimation.go:117, model/host/db.go:628-635), per
+ * distro in query order, SoA; replaces the []host.Host and the task.FindOneIdAndExecution of each running host
+ * (:141).  A lookup ERROR makes the reference return the pool built so far (:142-147): the shim ends the distro's rows
+ * before that host.  32 B. */
+typedef struct {
+  int64_t n_hosts;
+  const uint8_t* kind;        /* EVG_EH_* */
+  const int64_t* expected_ns; /* EVG_EH_RUNNING: the running task's stored ExpectedDuration field (:157); else not read */
+  const int64_t* dispatch_ns; /* EVG_EH_RUNNING: its DispatchTime, EVG_TIME_ZERO for Go's zero time; else not read */
+} evg_est_host_soa;
+
+/* GetEstimatedStartTime (model/task_start_estimation.go:99-122) for EVERY persisted position of every distro of the
+ * resident tick, after evg_run_resident: createSimulatorModel (:124-163) on the device, the pool sorted once (:60), then
+ * one run of dispatchNextTask (:69-96) per distro, whose state after position p is what a fresh simulate(p) returns
+ * (:53-67).  `cap` and `item_off` (n_distros + 1, written) are evg_download_queue's, so start_ns[k] is the estimate of
+ * the queue item evg_download_queue returns as items[k]: the queue is the resident expected_ns column read through the
+ * rank order, which never leaves the device.  est_host_off (n_distros + 1) is the CSR of `hosts` over the tick's
+ * distros.  time.Since is taken at now_ns and saturates; everything else is int64 arithmetic that wraps, as in Go.
+ * A distro without items has no estimates; one without hosts (none given, or all EVG_EH_IGNORED) gets -1 for every item
+ * (:54-59).  -1 is also a value a run can reach, so hosts_used[d] (n_distros) reports the pool size of each distro.
+ * Only reads the tick: every call allowed before it stays allowed, the dispatchers of evg_rebuild_dispatchers included,
+ * and calling it again (another now_ns, other hosts) recomputes from the same queue.  The first call allocates its own
+ * buffers.  EVG_ERR_INVALID with nothing launched and the tick still runnable: a null pointer the call needs, a negative
+ * cap or n_hosts, an est_host_off check_offsets rejects, a kind above EVG_EH_IGNORED (evg_last_error names the row),
+ * items_capacity below the rows needed (with the count in evg_last_error, item_off already written).  EVG_ERR_STATE:
+ * no resident tick.
+ * Replaces: LoadTaskQueue, the position scan's simulator set-up and the O(position x hosts) replay per task asked about
+ * (graphql/task_resolver.go:360-371 calls it once per task); the id-to-position lookup stays with the shim. */
+int evg_estimate_start_times(evg_ctx* ctx, int32_t cap, const evg_est_host_soa* hosts, const int64_t* est_host_off,
+                             int64_t now_ns, int64_t* item_off, int64_t* start_ns, int64_t items_capacity,
+                             int32_t* hosts_used);
+
+/* The same for caller-supplied queues (a queue loaded from the task_queues collection, a secondary queue):
+ * durations[item_off[d] .. item_off[d+1]) are TaskQueueItem.ExpectedDuration of distro d's items in queue order (:126-128).
+ * Host pointers.  Needs no tick and leaves any tick as it was.  EVG_ERR_INVALID with nothing launched: as above, a
+ * negative n_distros, an item_off check_offsets rejects.
+ * Replaces: createSimulatorModel(...).simulate(pos) (:121) for every pos of every queue. */
+int evg_estimate_start_batch(evg_ctx* ctx, const int64_t* durations, const int64_t* item_off, int32_t n_distros,
+                             const evg_est_host_soa* hosts, const int64_t* est_host_off, int64_t now_ns, int64_t* start_ns,
+                             int32_t* hosts_used);
 
 /* ---- single-distro wrappers: the per-job drop-in ------------------------- */
 
