@@ -42,26 +42,26 @@ struct DGen {
   uint32_t* tile_hist;         // [NT*256]
   uint4* wl;                   // work list, one entry per task that touches a multi-member unit: x = global task index,
                                //     y = distro, z = global slot of its own-key unit (kInactive: not a member of it),
-                               //     w = global slot of its version unit (kInactive: none)
+                               //     w = global slot of its version unit (kInactive: none); k_gfill replaces both slots
+                               //     with the units' ids
   struct URec* pay;            // [work list] the entry's member payload (what k_gunit and k_gbest ask of a member)
   unsigned int* ccount;        // [1] work-list entries
   uint4* tie;                  // [work list] x = anchor of the unit the task is emitted from, y = rank inside it,
-                               //     z = that unit's slot (kInactive: its own single-task unit)
+                               //     z = that unit's id (kInactive: its own single-task unit)
   int32_t* maxpass;            // [1]
   uint32_t* run;               // unit table: the members of every multi-member unit as work-list entry ids (bit 31: an
                                //     own-key membership), one contiguous run per unit
   uint32_t* pown;              // [work list] place of the entry's own-key membership in its unit's run
   uint32_t* pver;              // [work list] place of its version membership
   uint32_t* pedge;             // [E] place of the edge's dependency membership
-  uint32_t* sedge;             // [E] unit slot of that membership (kInactive: the task already joined that unit)
+  uint32_t* sedge;             // [E] unit slot of that membership (kInactive: the task already joined that unit); k_gfill
+                               //     replaces it with the unit's id
   uint32_t* rank;              // [run positions] the member's rank inside its unit (TaskList.Less)
   unsigned int* rcount;        // [1] run positions reserved
-  uint2* blist;                // units above kRankOne members, in 32-member chunks: x = slot, y = chunk (k_grank ranks them)
+  uint2* blist;                // units above kRankOne members, in 32-member chunks: x = id, y = chunk (k_grank ranks them)
   unsigned int* bcount;        // [1]
-  uint4* usum;                 // [unit slots] what k_gbest asks of a candidate unit, in one 16-byte load: x|y<<32 = TotalValue, z = anchor
-                               //     (kNoAnchor: never exported), w = members
-  uint2* hlist;                // multi-member units of the tick: x = slot, y = distro (k_galloc lists them, k_gunit folds them)
-  unsigned int* hcount;        // [1]
+  struct GUnit* unit;          // [units] the multi-member units of the tick by dense id (k_galloc numbers them)
+  unsigned int* hcount;        // [1] units numbered
   int64_t* tv;                 // [T] TotalValue by task (the output buffer, reused)
 };
 
@@ -94,6 +94,33 @@ __device__ __forceinline__ void rec_store(URec* p, const URec& r) {
   reinterpret_cast<uint4*>(p)[0] = make_uint4(uint32_t(r.prio), uint32_t(r.nd), uint32_t(uint64_t(r.exp_ns)), uint32_t(uint64_t(r.exp_ns) >> 32));
   reinterpret_cast<uint4*>(p)[1] = make_uint4(uint32_t(uint64_t(r.qb)), uint32_t(uint64_t(r.qb) >> 32), uint32_t(r.tgo), r.lif);
 }
+
+// A multi-member unit: everything the kernels after k_gfill ask of it, in one sector.  Units are numbered densely: the
+// ~10 000 units of a 100 000-task distro take ~0.3 MB of L2, where fields indexed by its ~100 000 unit slots spread over
+// megabytes and fell out of L2 between the blocks of one grid-wide kernel.
+struct __align__(16) GUnit {
+  int64_t value;            // TotalValue (k_gunit)
+  uint32_t anchor;          // kNoAnchor: the unit never got a distro, it is not exported (planner.go:81-83) (k_gunit)
+  uint32_t n;               // members (k_galloc)
+  uint32_t start;           // its run: run[start .. start + n) (k_galloc)
+  int32_t d;                // distro (k_galloc)
+  unsigned long long mask;  // ranks emitted from the unit, units of <= 64 members (k_gunit clears it, k_gbest ORs them in)
+};
+static_assert(sizeof(GUnit) == 32, "one L2 sector per unit");
+__device__ __forceinline__ GUnit unit_load(const GUnit* p) {  // two 128-bit loads of one sector
+  const uint4 a = reinterpret_cast<const uint4*>(p)[0], b = reinterpret_cast<const uint4*>(p)[1];
+  GUnit u;
+  u.value = int64_t((unsigned long long)a.x | ((unsigned long long)a.y << 32)); u.anchor = a.z; u.n = a.w;
+  u.start = b.x; u.d = int32_t(b.y); u.mask = (unsigned long long)b.z | ((unsigned long long)b.w << 32);
+  return u;
+}
+__device__ __forceinline__ void unit_store(GUnit* p, const GUnit& u) {
+  reinterpret_cast<uint4*>(p)[0] = make_uint4(uint32_t(uint64_t(u.value)), uint32_t(uint64_t(u.value) >> 32), u.anchor, u.n);
+  reinterpret_cast<uint4*>(p)[1] = make_uint4(u.start, uint32_t(u.d), uint32_t(u.mask), uint32_t(u.mask >> 32));
+}
+// The slot map of the general path: k_galloc files a unit's id and run start under its slot, in the on-chip planners'
+// unit_v (no general-path slot is an on-chip one), so that k_gfill finds both with one load.
+__device__ __forceinline__ int64_t slot_unit(uint32_t id, uint32_t start) { return int64_t(uint64_t(id) | (uint64_t(start) << 32)); }
 
 __global__ void k_ginit(DGen G, const int32_t* __restrict__ general_list, int n) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
@@ -366,17 +393,19 @@ __global__ void __launch_bounds__(256, kGTaskOcc) k_gtask(DTasks T, DDistros D, 
 // entry ids, each naming the 32-byte payload k_gtask wrote for the task:
 //   k_glink   per pair: k = atomicAdd(unit_n[slot], 1) -- its place in the run (any order: everything computed from a
 //             run is order-free); TaskGroupInfo sums of task-group tasks, from the payload
-//   k_galloc  the pair that drew k == 0 reserves unit_n[slot] run positions: head[slot] = start of the run
-//   k_gfill   every pair writes its entry id at head[slot] + k
-//   k_gunit   per unit: the run folded into Unit.info (planner.go:302-337), value (planner.go:209-300), anchor; the
-//             members' ranks (TaskList.Less, planner.go:387-405) for units of up to kRankOne members
+//   k_galloc  the pair that drew k == 0 reserves unit_n[slot] run positions and numbers the unit: unit_v[slot] = its id
+//             and run start, unit[id] = {members, run start, distro}
+//   k_gfill   every pair writes its entry id at run start + k, and replaces its slot with the unit's id
+//   k_gunit   per unit, in id order: the run folded into Unit.info (planner.go:302-337), value (planner.go:209-300),
+//             anchor; the members' ranks (TaskList.Less, planner.go:387-405) for units of up to kRankOne members
 //   k_grank   the ranks of the larger units, a warp per 32 members
 //   k_gbest   per task: the first unit it is emitted from among its memberships (TaskPlan.Export, planner.go:467-477)
-//             and its rank there, one load
+//             and its rank there, one record load per membership
 // A membership's place in its run is kept next to the membership, so every access is coalesced: by work-list entry for
 // the own-key (pown) and version (pver) memberships, by edge for dependency memberships (pedge, with the edge's unit slot
-// in sedge).  The on-chip planner's next[] / pair_slot[], indexed by pair id over 2T+E entries of which the general path
-// would touch about a quarter (a sector per access), are not used here.
+// in sedge).  After k_gfill the slot space (one slot per task and group, ~10x the units) is not touched again: what the
+// later kernels ask of a unit is its 32-byte record, by id.  The on-chip planner's next[] / pair_slot[], indexed by pair
+// id over 2T+E entries of which the general path would touch about a quarter (a sector per access), are not used here.
 
 // what a work-list task is filed under: one 16-byte entry k_gtask wrote (the same answers in every kernel below)
 struct WlTask {
@@ -391,8 +420,9 @@ __device__ __forceinline__ WlTask wl_task(const DDistros& D, const DGen& G, unsi
   x.own_complex = x.s_own != kInactive;
   return x;
 }
-// f(place, slot, own) for every membership of work-list entry k: `place` points at its place in the unit's run, `own`
-// marks the own-key membership (after k_glink: the places and sedge are final)
+// f(place, unit, own) for every membership of work-list entry k: `place` points at its place in the unit's run, `unit`
+// is the unit's slot (up to k_gfill) or id (after it), `own` marks the own-key membership (after k_glink: the places
+// are final)
 template <typename F>
 __device__ __forceinline__ void wl_pairs(const DTasks& T, const DGen& G, const WlTask& x, unsigned int k, F&& f) {
   if (x.own_complex) f(G.pown + k, x.s_own, true);
@@ -494,21 +524,58 @@ __global__ void __launch_bounds__(256, kUnitTableOcc) k_galloc(DTasks T, DDistro
     if (heads) {
       uint32_t pos = s_base + before + inc - need, hp = s_hbase + hbefore + hinc - heads;
       wl_pairs(T, G, x, k, [&](const uint32_t* place, uint32_t slot, bool) {
-        if (*place == 0u) { W.head[slot] = pos; pos += W.unit_n[slot]; G.hlist[hp++] = make_uint2(slot, uint32_t(x.d)); }
+        if (*place != 0u) return;
+        GUnit u;
+        u.value = 0; u.anchor = kNoAnchor; u.n = W.unit_n[slot]; u.start = pos; u.d = x.d; u.mask = 0ull;
+        unit_store(G.unit + hp, u);
+        W.unit_v[slot] = slot_unit(hp++, pos);
+        pos += u.n;
       });
     }
     __syncthreads();  // the shared scratch is rewritten by the next trip
   }
 }
 
+// Two entries per trip, all their loads before any store: a store to the run could alias the next entry's loads, so one
+// entry at a time would wait on every load in turn.
+constexpr int kFillEntries = 2;
 __global__ void __launch_bounds__(256, kUnitTableOcc) k_gfill(DTasks T, DDistros D, DWork W, DGen G) {
   if (*W.err) return;
-  const unsigned int n = *G.ccount;
-  for (unsigned int k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x) {
-    const WlTask x = wl_task(D, G, k);
-    wl_pairs(T, G, x, k, [&](const uint32_t* place, uint32_t slot, bool own) {
-      G.run[W.head[slot] + *place] = k | (own ? kRunOwn : 0u);  // own-key members are the SetDistro members (planner.go:446)
-    });
+  const unsigned int n = *G.ccount, stride = gridDim.x * blockDim.x;
+  for (unsigned int k0 = blockIdx.x * blockDim.x + threadIdx.x; k0 < n; k0 += kFillEntries * stride) {
+    WlTask x[kFillEntries];
+    uint32_t place[kFillEntries][2], id[kFillEntries][2], start[kFillEntries][2];
+#pragma unroll
+    for (int j = 0; j < kFillEntries; j++) {
+      const unsigned int k = k0 + j * stride;
+      x[j].s_own = x[j].s_ver = kInactive;
+      if (k < n) x[j] = wl_task(D, G, k);
+      const uint32_t sl[2] = {x[j].s_own, x[j].s_ver};
+#pragma unroll
+      for (int m = 0; m < 2; m++) {
+        place[j][m] = sl[m] != kInactive ? (m ? G.pver : G.pown)[k] : 0u;
+        const uint64_t su = sl[m] != kInactive ? uint64_t(W.unit_v[sl[m]]) : ~0ull;  // the last read of the slot space
+        id[j][m] = uint32_t(su);
+        start[j][m] = uint32_t(su >> 32);
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < kFillEntries; j++) {
+      const unsigned int k = k0 + j * stride;
+      if (k >= n) continue;
+      // own-key members are the SetDistro members (planner.go:446)
+      if (id[j][0] != kInactive) G.run[start[j][0] + place[j][0]] = k | kRunOwn;
+      if (id[j][1] != kInactive) G.run[start[j][1] + place[j][1]] = k;
+      G.wl[k] = make_uint4(x[j].t, uint32_t(x[j].d), id[j][0], id[j][1]);  // the units' ids replace their slots
+      if (T.n_edges > 0)
+        for (int64_t e = T.dep_off[x[j].t]; e < T.dep_off[x[j].t + 1]; e++) {
+          const uint32_t sl = G.sedge[e];
+          if (sl == kInactive) continue;
+          const uint64_t su = uint64_t(W.unit_v[sl]);
+          G.run[uint32_t(su >> 32) + G.pedge[e]] = k;
+          G.sedge[e] = uint32_t(su);
+        }
+    }
   }
 }
 
@@ -523,14 +590,14 @@ __device__ __forceinline__ bool rec_less(const URec& x, const URec& y) {  // Tas
 constexpr uint32_t kRankOne = 8;
 constexpr int kRankKey = 6;  // tgo, nd, prio, expected (two words), index
 
-// One thread per multi-member unit (dense warps: the unit list, not the work list).
+// One thread per multi-member unit, in id order (dense warps: the unit records, not the work list).
 __global__ void __launch_bounds__(256, kUnitTableOcc) k_gunit(DDistros D, DWork W, DGen G, int64_t now) {
   if (*W.err) return;
   const unsigned int n = *G.hcount;
   __shared__ uint32_t s_key[kRankOne * kRankKey][256];  // this thread's column: the rank keys of a small unit's members
   for (unsigned int k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x) {  // the host cannot know n: fixed grid
-    const uint2 u = G.hlist[k];
-    const uint32_t cnt = W.unit_n[u.x], h = W.head[u.x];
+    GUnit u = unit_load(G.unit + k);
+    const uint32_t cnt = u.n, h = u.start;
     const uint32_t* run = G.run + h;
     UnitAcc a;
     acc_init(a);
@@ -547,9 +614,10 @@ __global__ void __launch_bounds__(256, kUnitTableOcc) k_gunit(DDistros D, DWork 
         kx[768] = uint32_t(uint64_t(r.exp_ns)); kx[1024] = uint32_t(uint64_t(r.exp_ns) >> 32); kx[1280] = rec_li(r);
       }
     }
-    const unsigned long long v = (unsigned long long)unit_value(a, D.cfg[u.y], nullptr);
-    G.usum[u.x] = make_uint4(uint32_t(v), uint32_t(v >> 32), anchor, cnt);  // kNoAnchor: the unit never got a distro -> not exported (planner.go:81-83)
-    W.unit_mask[u.x] = 0ull;  // k_gbest ORs the emitted ranks in (cleared here, unit by unit, instead of a slot-wide memset)
+    u.value = unit_value(a, D.cfg[u.d], nullptr);
+    u.anchor = anchor;
+    u.mask = 0ull;  // k_gbest ORs the emitted ranks in (cleared here, unit by unit, instead of a memset)
+    unit_store(G.unit + k, u);
     // every member's rank in the unit: a count over the member set, so the order of the run does not matter
     if (small) {
       auto key = [&](uint32_t i, URec& r) {
@@ -567,7 +635,7 @@ __global__ void __launch_bounds__(256, kUnitTableOcc) k_gunit(DDistros D, DWork 
     } else {
       const uint32_t nch = (cnt + 31) >> 5;
       const uint32_t b = atomicAdd(G.bcount, nch);
-      for (uint32_t c = 0; c < nch; c++) G.blist[b + c] = make_uint2(u.x, c);
+      for (uint32_t c = 0; c < nch; c++) G.blist[b + c] = make_uint2(k, c);
     }
   }
 }
@@ -583,7 +651,8 @@ __global__ void __launch_bounds__(256, kUnitTableOcc) k_grank(DWork W, DGen G) {
   const unsigned int nw = gridDim.x * (blockDim.x >> 5);
   for (unsigned int c = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); c < n; c += nw) {  // warp-uniform
     const uint2 ch = G.blist[c];
-    const uint32_t cnt = W.unit_n[ch.x], h = W.head[ch.x];
+    const GUnit u = unit_load(G.unit + ch.x);
+    const uint32_t cnt = u.n, h = u.start;
     const uint32_t* run = G.run + h;
     const uint32_t i = ch.y * 32u + uint32_t(lane);
     URec me;
@@ -623,23 +692,23 @@ __global__ void __launch_bounds__(256, kUnitTableOcc) k_gbest(DTasks T, DDistros
       d = x.d;
       bool have = false;
       int64_t bv = 0;
-      uint32_t ba = 0, brk = 0, bslot = kInactive, bn = 1, bkx = 0;
+      uint32_t ba = 0, brk = 0, bid = kInactive, bn = 1, bpos = 0;
       if (!x.own_complex) { have = true; bv = G.tv[t]; ba = li; }  // its own single-task unit, scored by k_gtask
-      wl_pairs(T, G, x, k, [&](const uint32_t* place, uint32_t slot, bool) {
-        const uint4 u = G.usum[slot];
-        const uint32_t kx = *place;  // this task's place in that unit's run (requested together with the summary)
-        const uint32_t a = u.z;
-        if (a == kNoAnchor) return;
-        const int64_t v = int64_t((unsigned long long)u.x | ((unsigned long long)u.y << 32));
-        if (!have || v > bv || (v == bv && a < ba)) { have = true; bv = v; ba = a; bslot = slot; bn = u.w; bkx = kx; }
+      wl_pairs(T, G, x, k, [&](const uint32_t* place, uint32_t id, bool) {
+        const GUnit u = unit_load(G.unit + id);
+        const uint32_t kx = *place;  // this task's place in that unit's run (requested together with the record)
+        if (u.anchor == kNoAnchor) return;
+        if (!have || u.value > bv || (u.value == bv && u.anchor < ba)) {
+          have = true; bv = u.value; ba = u.anchor; bid = id; bn = u.n; bpos = u.start + kx;
+        }
       });
-      if (bslot != kInactive) {  // its rank among ALL members of the chosen unit, as k_gunit / k_grank counted it
-        brk = G.rank[W.head[bslot] + bkx];
-        if (bn <= 64) atomicOr(&W.unit_mask[bslot], 1ull << brk);  // ranks emitted from the unit: k_gplace_disp counts below its own
+      if (bid != kInactive) {  // its rank among ALL members of the chosen unit, as k_gunit / k_grank counted it
+        brk = G.rank[bpos];
+        if (bn <= 64) atomicOr(&G.unit[bid].mask, 1ull << brk);  // ranks emitted from the unit: k_gplace_disp counts below its own
       }
       G.tv[t] = bv;
-      G.tie[k] = make_uint4(ba, brk, bslot, 0u);
-      if (want_best_pair) W.best_pair[t] = bslot;  // k_breakdown's way back to the unit (general path: its slot)
+      G.tie[k] = make_uint4(ba, brk, bid, 0u);
+      if (want_best_pair) W.best_pair[t] = bid;  // k_breakdown's way back to the unit (general path: its id)
       const bool displaced = !(ba == li && brk == 0);
       if (displaced) W.has_dep[t] |= 2;  // only this thread touches the byte now (k_gmark and k_gtask are done)
       atomicAdd(G.e + x.base + ba, 1u);
@@ -875,16 +944,16 @@ __global__ void __launch_bounds__(256) k_gplace_disp(DTasks T, DDistros D, DWork
   const int d = int(ent.y);
   const int64_t base = D.task_off[d];
   const uint4 tie = G.tie[k];
-  const uint32_t a = tie.x, myrk = tie.y, slot = tie.z;
+  const uint32_t a = tie.x, myrk = tie.y, id = tie.z;
   uint32_t pos = G.e[base + a];
-  const uint32_t cnt = W.unit_n[slot];
-  if (cnt <= 64) {
-    pos += __popcll(W.unit_mask[slot] & ((1ull << myrk) - 1ull));
+  const GUnit u = unit_load(G.unit + id);
+  if (u.n <= 64) {
+    pos += __popcll(u.mask & ((1ull << myrk) - 1ull));
   } else {
-    const uint32_t* run = G.run + W.head[slot];
-    for (uint32_t i = 0; i < cnt; i++) {
+    const uint32_t* run = G.run + u.start;
+    for (uint32_t i = 0; i < u.n; i++) {
       const uint4 tq = G.tie[run[i] & kRunEntry];
-      if (tq.z == slot && tq.y < myrk) pos++;
+      if (tq.z == id && tq.y < myrk) pos++;
     }
   }
   gen_put(G, base, pos, G.vmm[2 * d], gen_bits(G, d) > 32, G.tv[t], uint32_t(int64_t(t) - base));

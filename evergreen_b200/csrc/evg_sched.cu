@@ -213,7 +213,7 @@ struct DWork {
   uint8_t* edge_live;    // [E] on-chip path: 1 = edge pair linked (not a duplicate membership)
   const uint8_t* route;  // [D] 1 = distro planned by k_plan_smem (general kernels skip it)
   int* err;              // [1] set by k_validate when a distro-local id is out of range; planners then do nothing
-  int64_t* unit_v;       // [unit slots] on-chip path: TotalValue of the unit
+  int64_t* unit_v;       // [unit slots] on-chip path: TotalValue of the unit; general path: id | run start << 32 (slot_unit)
   uint32_t* unit_a;      // [unit slots] anchor
   uint32_t* unit_n;      // [unit slots] member count
   unsigned long long* unit_mask;  // [unit slots] ranks emitted from the unit (units of <= 64 members)
@@ -858,8 +858,8 @@ __global__ void __launch_bounds__(256) k_dur_commit(DDurRows R, const int* __res
 
 // The 13-field SortingValueBreakdown of the unit each ranked task was emitted
 // from (planner.go:472-476, model/task/task.go:3990-4038); both paths.
-__global__ void __launch_bounds__(256) k_breakdown(DTasks T, DDistros D, DWork W, const uint32_t* run_all, const URec* pay, int64_t now, int any_complex,
-                                                   const int32_t* order, int64_t* breakdown) {
+__global__ void __launch_bounds__(256) k_breakdown(DTasks T, DDistros D, DWork W, const uint32_t* run_all, const URec* pay, const GUnit* units,
+                                                   int64_t now, int any_complex, const int32_t* order, int64_t* breakdown) {
   if (*W.err) return;
   const int64_t t = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
   const int d = block_find_distro(D.task_off, D.n, t, T.n);
@@ -876,11 +876,10 @@ __global__ void __launch_bounds__(256) k_breakdown(DTasks T, DDistros D, DWork W
       const uint32_t tq = pair_task(T, W, q);
       acc_add(a, now, T.priority[tq], T.expected[tq], T.qbasis[tq], T.numdep[tq], T.gid[tq], T.flags[tq]);
     }
-  } else {  // general path: the unit table (k_gbest stored the chosen unit's slot)
-    const uint32_t slot = bp;
-    const uint32_t* run = run_all + W.head[slot];
-    const uint32_t cnt = W.unit_n[slot];
-    for (uint32_t i = 0; i < cnt; i++) rec_acc(a, now, rec_load(pay + (run[i] & kRunEntry)));
+  } else {  // general path: the unit table (k_gbest stored the chosen unit's id)
+    const GUnit u = unit_load(units + bp);
+    const uint32_t* run = run_all + u.start;
+    for (uint32_t i = 0; i < u.n; i++) rec_acc(a, now, rec_load(pay + (run[i] & kRunEntry)));
   }
   int64_t bd[EVG_BD_N];
   unit_value(a, D.cfg[d], bd);
@@ -1377,7 +1376,7 @@ struct evg_ctx {
   int general_complex = 0;
   int64_t Tgc = 0;  // tasks in general-path distros that can hold multi-member units (work-list capacity)
   DevBuf b_kv, b_vmm, b_klo[2], b_khi[2], b_ix[2], b_e, b_tilesum, b_gmisc;
-  DevBuf b_tiledistro, b_tilestart, b_dtileoff, b_tilehist, b_wl, b_pay, b_place, b_eplace, b_run, b_rank, b_blist, b_tie, b_hlist, b_usum, b_upd;
+  DevBuf b_tiledistro, b_tilestart, b_dtileoff, b_tilehist, b_wl, b_pay, b_place, b_eplace, b_run, b_rank, b_blist, b_tie, b_unit, b_upd;
   DevBuf b_qinfo, b_ginfo, b_order, b_tv, b_bd;
   DevBuf b_hflags, b_hgid, b_hexp, b_hstd, b_hstart, b_hostoff, b_acfg, b_gs, b_result, b_status;
   bool bd_valid = false;
@@ -1468,7 +1467,7 @@ int upload_tasks(evg_ctx* c, const char* who, const evg_task_soa* t, const evg_d
   std::vector<uint8_t> route(size_t(D) + 1, 0);
   int general_complex = 0;
   int any_complex = E > 0 ? 1 : 0;
-  int64_t Tgc = 0, Prec = 0;
+  int64_t Tgc = 0, Prec = 0, Urec = 0;
   constexpr int kGA = PlanCta<kNT_A, kNCapA>::kGroupCap, kGB = PlanCta<kNT_B, kNCapB>::kGroupCap, kGC = PlanCta<kNT_C, kNCapC>::kGroupCap;
   // Size class of distro d by its own shape (no side effects).  kBigUnits: a GroupVersions distro of k_plan_smem's
   // smallest class above kBigUnitTasks tasks, whose version units of dozens of tasks are walked member by member.
@@ -1520,6 +1519,8 @@ int upload_tasks(evg_ctx* c, const char* who, const evg_task_soa* t, const evg_d
         general_complex = 1;
         Tgc += n;
         Prec += n + ((cf.group_versions && gb > ga) ? n : 0) + de;  // own-key, version and dependency memberships at most
+        // units: every unit has an own-key member (a dependency joins its target's own-key unit) or is a version unit
+        Urec += n + ((cf.group_versions && gb > ga) ? std::min<int64_t>(cf.n_versions, n) : 0);
       }
       const int64_t a0 = a & ~int64_t(3);  // tiles start 16-byte aligned in every column
       for (int64_t s = a0; s < b; s += kGTile) { tile_distro.push_back(d); tile_start.push_back(s); }
@@ -1630,8 +1631,7 @@ int upload_tasks(evg_ctx* c, const char* who, const evg_task_soa* t, const evg_d
       CK(c->b_run.ensure(sizeof(uint32_t) * size_t(Prec + 1)));
       CK(c->b_rank.ensure(sizeof(uint32_t) * size_t(Prec + 1)));
       CK(c->b_blist.ensure(sizeof(uint2) * size_t(Prec / kRankOne + 1)));  // a unit of n > kRankOne members: ceil(n/32) <= n/kRankOne chunks
-      CK(c->b_hlist.ensure(sizeof(uint2) * size_t(Prec + 1)));
-      CK(c->b_usum.ensure(sizeof(uint4) * size_t(U + 1)));
+      CK(c->b_unit.ensure(sizeof(GUnit) * size_t(Urec + 1)));
     }
   }
   CK(c->b_punt.ensure(sizeof(int32_t) * size_t(D + 1)));
@@ -1754,8 +1754,7 @@ DGen dgen(const evg_ctx* c) {
   g.bcount = c->b_gmisc.as<unsigned int>() + 4;
   g.blist = c->b_blist.as<uint2>();
   g.rank = c->b_rank.as<uint32_t>();
-  g.hlist = c->b_hlist.as<uint2>();
-  g.usum = c->b_usum.as<uint4>();
+  g.unit = c->b_unit.as<GUnit>();
   g.run = c->b_run.as<uint32_t>();
   g.tie = c->b_tie.as<uint4>();
   g.tv = c->b_tv.as<int64_t>();
@@ -1997,7 +1996,7 @@ int run_plan(evg_ctx* c, int64_t now, uint32_t opts) {
       CK(cudaStreamWaitEvent(s, c->ev_join[k], 0));
     }
   }
-  if (bd) launch(c, c->stream, k_breakdown, grid_for(T, 256), 256, 0, dt, dd, w, c->b_run.as<uint32_t>(), c->b_pay.as<URec>(), now, c->any_complex, c->b_order.as<int32_t>(), bd);
+  if (bd) launch(c, c->stream, k_breakdown, grid_for(T, 256), 256, 0, dt, dd, w, c->b_run.as<uint32_t>(), c->b_pay.as<URec>(), c->b_unit.as<GUnit>(), now, c->any_complex, c->b_order.as<int32_t>(), bd);
   CK(cudaGetLastError());
   return EVG_OK;
 }
