@@ -10,10 +10,12 @@
 //   k_gunit/k_grank  per unit: Unit.info / value / anchor, and every member's rank in the unit, once
 //   k_gbest        per work-list task: its first-occurrence choice (planner.go:467-477) and that unit's rank of it;
 //                  anchor histogram e[]
-//   k_gsum/k_gscan/k_gplace(+_disp)
+//   k_gsum/k_gscan/k_gplace/k_gplace_unit
 //                  canonical pre-arrangement by COUNTING instead of sorting tie bytes: an exclusive scan of e[] over
 //                  the distro gives every anchor's run start; tasks are written to (key, index) buffers in
-//                  (anchor, rank-in-unit) order.  Distros without multi-member units skip the scan (identity).
+//                  (anchor, rank-in-unit) order: k_gplace the tasks emitted from their own single-task unit, k_gplace_unit
+//                  every multi-member unit's emitted tasks, from the unit.  Distros without multi-member units skip the
+//                  scan (identity).
 //   k_ghist/k_gdscan/k_gscatter
 //                  stable LSD radix sort on key = Vmax - V only: 32-bit keys, ceil(bits(Vmax-Vmin)/8) passes (3 for
 //                  a 20-bit range), 8 B/task each way per pass; a distro whose range exceeds 32 bits carries a
@@ -46,8 +48,6 @@ struct DGen {
                                //     with the units' ids
   struct URec* pay;            // [work list] the entry's member payload (what k_gunit and k_gbest ask of a member)
   unsigned int* ccount;        // [1] work-list entries
-  uint4* tie;                  // [work list] x = anchor of the unit the task is emitted from, y = rank inside it,
-                               //     z = that unit's id (kInactive: its own single-task unit)
   int32_t* maxpass;            // [1]
   uint32_t* run;               // unit table: the members of every multi-member unit as work-list entry ids (bit 31: an
                                //     own-key membership), one contiguous run per unit
@@ -57,6 +57,8 @@ struct DGen {
   uint32_t* sedge;             // [E] unit slot of that membership (kInactive: the task already joined that unit); k_gfill
                                //     replaces it with the unit's id
   uint32_t* rank;              // [run positions] the member's rank inside its unit (TaskList.Less)
+  uint32_t* emit;              // [run positions] by rank: emit[start + r] = distro-local index of the unit's rank-r member
+                               //     if the unit emits it (k_gbest), else kInactive (k_gunit / k_grank reset it per tick)
   unsigned int* rcount;        // [1] run positions reserved
   uint2* blist;                // units above kRankOne members, in 32-member chunks: x = id, y = chunk (k_grank ranks them)
   unsigned int* bcount;        // [1]
@@ -99,24 +101,24 @@ __device__ __forceinline__ void rec_store(URec* p, const URec& r) {
 // ~10 000 units of a 100 000-task distro take ~0.3 MB of L2, where fields indexed by its ~100 000 unit slots spread over
 // megabytes and fell out of L2 between the blocks of one grid-wide kernel.
 struct __align__(16) GUnit {
-  int64_t value;            // TotalValue (k_gunit)
-  uint32_t anchor;          // kNoAnchor: the unit never got a distro, it is not exported (planner.go:81-83) (k_gunit)
-  uint32_t n;               // members (k_galloc)
-  uint32_t start;           // its run: run[start .. start + n) (k_galloc)
-  int32_t d;                // distro (k_galloc)
-  unsigned long long mask;  // ranks emitted from the unit, units of <= 64 members (k_gunit clears it, k_gbest ORs them in)
+  int64_t value;    // TotalValue (k_gunit)
+  uint32_t anchor;  // kNoAnchor: the unit never got a distro, it is not exported (planner.go:81-83) (k_gunit)
+  uint32_t n;       // members (k_galloc)
+  uint32_t start;   // its run: run[start .. start + n), and its ranks: emit[start .. start + n) (k_galloc)
+  int32_t d;        // distro (k_galloc)
+  uint32_t spare[2];  // unused: keeps the record one sector (written as zero)
 };
 static_assert(sizeof(GUnit) == 32, "one L2 sector per unit");
 __device__ __forceinline__ GUnit unit_load(const GUnit* p) {  // two 128-bit loads of one sector
   const uint4 a = reinterpret_cast<const uint4*>(p)[0], b = reinterpret_cast<const uint4*>(p)[1];
   GUnit u;
   u.value = int64_t((unsigned long long)a.x | ((unsigned long long)a.y << 32)); u.anchor = a.z; u.n = a.w;
-  u.start = b.x; u.d = int32_t(b.y); u.mask = (unsigned long long)b.z | ((unsigned long long)b.w << 32);
+  u.start = b.x; u.d = int32_t(b.y); u.spare[0] = u.spare[1] = 0u;
   return u;
 }
 __device__ __forceinline__ void unit_store(GUnit* p, const GUnit& u) {
   reinterpret_cast<uint4*>(p)[0] = make_uint4(uint32_t(uint64_t(u.value)), uint32_t(uint64_t(u.value) >> 32), u.anchor, u.n);
-  reinterpret_cast<uint4*>(p)[1] = make_uint4(u.start, uint32_t(u.d), uint32_t(u.mask), uint32_t(u.mask >> 32));
+  reinterpret_cast<uint4*>(p)[1] = make_uint4(u.start, uint32_t(u.d), 0u, 0u);
 }
 // The slot map of the general path: k_galloc files a unit's id and run start under its slot, in the on-chip planners'
 // unit_v (no general-path slot is an on-chip one), so that k_gfill finds both with one load.
@@ -400,7 +402,8 @@ __global__ void __launch_bounds__(256, kGTaskOcc) k_gtask(DTasks T, DDistros D, 
 //             anchor; the members' ranks (TaskList.Less, planner.go:387-405) for units of up to kRankOne members
 //   k_grank   the ranks of the larger units, a warp per 32 members
 //   k_gbest   per task: the first unit it is emitted from among its memberships (TaskPlan.Export, planner.go:467-477)
-//             and its rank there, one record load per membership
+//             and its rank there, one record load per membership; the task is filed under that rank in the unit's
+//             emitted-by-rank slots, emit[start + rank], from which k_gplace_unit writes the unit's tasks in order
 // A membership's place in its run is kept next to the membership, so every access is coalesced: by work-list entry for
 // the own-key (pown) and version (pver) memberships, by edge for dependency memberships (pedge, with the edge's unit slot
 // in sedge).  After k_gfill the slot space (one slot per task and group, ~10x the units) is not touched again: what the
@@ -526,7 +529,7 @@ __global__ void __launch_bounds__(256, kUnitTableOcc) k_galloc(DTasks T, DDistro
       wl_pairs(T, G, x, k, [&](const uint32_t* place, uint32_t slot, bool) {
         if (*place != 0u) return;
         GUnit u;
-        u.value = 0; u.anchor = kNoAnchor; u.n = W.unit_n[slot]; u.start = pos; u.d = x.d; u.mask = 0ull;
+        u.value = 0; u.anchor = kNoAnchor; u.n = W.unit_n[slot]; u.start = pos; u.d = x.d;
         unit_store(G.unit + hp, u);
         W.unit_v[slot] = slot_unit(hp++, pos);
         pos += u.n;
@@ -616,9 +619,9 @@ __global__ void __launch_bounds__(256, kUnitTableOcc) k_gunit(DDistros D, DWork 
     }
     u.value = unit_value(a, D.cfg[u.d], nullptr);
     u.anchor = anchor;
-    u.mask = 0ull;  // k_gbest ORs the emitted ranks in (cleared here, unit by unit, instead of a memset)
     unit_store(G.unit + k, u);
-    // every member's rank in the unit: a count over the member set, so the order of the run does not matter
+    // every member's rank in the unit: a count over the member set, so the order of the run does not matter.  The
+    // emitted-by-rank slots are cleared with the ranks, unit by unit (no memset; nothing of an earlier tick survives).
     if (small) {
       auto key = [&](uint32_t i, URec& r) {
         const uint32_t* kx = &s_key[i * kRankKey][threadIdx.x];
@@ -631,6 +634,7 @@ __global__ void __launch_bounds__(256, kUnitTableOcc) k_gunit(DDistros D, DWork 
         uint32_t rk = 0;
         for (uint32_t j = 0; j < cnt; j++) { key(j, o); rk += rec_less(o, me) ? 1u : 0u; }
         G.rank[h + i] = rk;
+        G.emit[h + i] = kInactive;
       }
     } else {
       const uint32_t nch = (cnt + 31) >> 5;
@@ -671,7 +675,7 @@ __global__ void __launch_bounds__(256, kUnitTableOcc) k_grank(DWork W, DGen G) {
         rk += (i < cnt && rec_less(y, me)) ? 1u : 0u;
       }
     }
-    if (i < cnt) G.rank[h + i] = rk;
+    if (i < cnt) { G.rank[h + i] = rk; G.emit[h + i] = kInactive; }
   }
 }
 
@@ -692,25 +696,24 @@ __global__ void __launch_bounds__(256, kUnitTableOcc) k_gbest(DTasks T, DDistros
       d = x.d;
       bool have = false;
       int64_t bv = 0;
-      uint32_t ba = 0, brk = 0, bid = kInactive, bn = 1, bpos = 0;
+      uint32_t ba = 0, bid = kInactive, bstart = 0, bpos = 0;
       if (!x.own_complex) { have = true; bv = G.tv[t]; ba = li; }  // its own single-task unit, scored by k_gtask
       wl_pairs(T, G, x, k, [&](const uint32_t* place, uint32_t id, bool) {
         const GUnit u = unit_load(G.unit + id);
         const uint32_t kx = *place;  // this task's place in that unit's run (requested together with the record)
         if (u.anchor == kNoAnchor) return;
         if (!have || u.value > bv || (u.value == bv && u.anchor < ba)) {
-          have = true; bv = u.value; ba = u.anchor; bid = id; bn = u.n; bpos = u.start + kx;
+          have = true; bv = u.value; ba = u.anchor; bid = id; bstart = u.start; bpos = u.start + kx;
         }
       });
-      if (bid != kInactive) {  // its rank among ALL members of the chosen unit, as k_gunit / k_grank counted it
-        brk = G.rank[bpos];
-        if (bn <= 64) atomicOr(&G.unit[bid].mask, 1ull << brk);  // ranks emitted from the unit: k_gplace_disp counts below its own
+      // Emitted from a multi-member unit: filed under its rank among ALL members of the unit, as k_gunit / k_grank
+      // counted it (ranks are unique inside a unit: a plain store), and k_gplace_unit writes it with the unit's value.
+      // Emitted from its own single-task unit: k_gplace writes it with the value k_gtask left in tv.
+      if (bid != kInactive) {
+        G.emit[bstart + G.rank[bpos]] = li;
+        W.has_dep[t] |= 2;  // only this thread touches the byte now (k_gmark and k_gtask are done)
       }
-      G.tv[t] = bv;
-      G.tie[k] = make_uint4(ba, brk, bid, 0u);
       if (want_best_pair) W.best_pair[t] = bid;  // k_breakdown's way back to the unit (general path: its id)
-      const bool displaced = !(ba == li && brk == 0);
-      if (displaced) W.has_dep[t] |= 2;  // only this thread touches the byte now (k_gmark and k_gtask are done)
       atomicAdd(G.e + x.base + ba, 1u);
       kk = ord_i64(bv);
     }
@@ -793,16 +796,18 @@ __global__ void __launch_bounds__(1024) k_gscan(DGen G, const int32_t* __restric
   }
 }
 
-__device__ __forceinline__ void gen_put(const DGen& G, int64_t base, uint32_t pos, unsigned long long vmax_ord, bool wide,
-                                        int64_t v, uint32_t li) {
-  const unsigned long long key = vmax_ord - ord_i64(v);
+__device__ __forceinline__ void gen_put_key(const DGen& G, int64_t base, uint32_t pos, unsigned long long key, bool wide, uint32_t li) {
   G.key_lo[0][base + pos] = uint32_t(key);
   if (wide) G.key_hi[0][base + pos] = uint32_t(key >> 32);
   G.idx[0][base + pos] = li;
 }
+__device__ __forceinline__ void gen_put(const DGen& G, int64_t base, uint32_t pos, unsigned long long vmax_ord, bool wide,
+                                        int64_t v, uint32_t li) {
+  gen_put_key(G, base, pos, vmax_ord - ord_i64(v), wide, li);
+}
 
 // Per tile: exclusive scan of e[] (thread q owns 8 consecutive slots) on top of the tile's offset = the run start of
-// every anchor; tasks that keep their own anchor with rank 0 are written to their sort position.  use_e == 0 (no
+// every anchor; tasks emitted from their own single-task unit are written to their sort position.  use_e == 0 (no
 // multi-member unit in any general-path distro): positions are the input order.
 __global__ void __launch_bounds__(256) k_gplace(DDistros D, DWork W, DGen G, int use_e) {
   const int tile = int(blockIdx.x + G.tile0);
@@ -841,7 +846,7 @@ __global__ void __launch_bounds__(256) k_gplace(DDistros D, DWork W, DGen G, int
     run = G.tile_sum[tile] + before + inc - sum;
   }
   int64_t vv[8];
-  uint32_t dsp = 0;  // bit m: task t8+m leaves its own anchor's first slot (placed by k_gplace_disp)
+  uint32_t dsp = 0;  // bit m: task t8+m is emitted from a multi-member unit (placed by k_gplace_unit)
   if (interior) {
 #pragma unroll
     for (int m = 0; m < 8; m += 2) {
@@ -863,10 +868,10 @@ __global__ void __launch_bounds__(256) k_gplace(DDistros D, DWork W, DGen G, int
     }
   }
   if (use_e) {
-    // The tile's own-anchor tasks land in ONE contiguous stretch of the distro's segment, [tile_sum[tile], + sum of e over
-    // the tile), with holes where displaced tasks will be put by k_gplace_disp.  They are staged in shared memory and
-    // the stretch is written out whole (holes included: k_gplace_disp runs later and fills them): 4-byte stores
-    // straight from registers cost a sector each, several times the sectors of the payload.
+    // The tile's single-task-unit tasks land in ONE contiguous stretch of the distro's segment, [tile_sum[tile], + sum of
+    // e over the tile), with holes where the multi-member units' tasks will be put by k_gplace_unit.  They are staged in
+    // shared memory and the stretch is written out whole (holes included: k_gplace_unit runs later and fills them):
+    // 4-byte stores straight from registers cost a sector each, several times the sectors of the payload.
     constexpr int kStage = 3072;
     __shared__ uint32_t st_lo[kStage], st_ix[kStage], st_hi[kStage];
     __shared__ uint32_t s_total;
@@ -934,29 +939,50 @@ __global__ void __launch_bounds__(256) k_gplace(DDistros D, DWork W, DGen G, int
   }
 }
 
-// Displaced work-list tasks: position = run start of the anchor + number of tasks emitted from the same unit with a smaller rank.
-__global__ void __launch_bounds__(256) k_gplace_disp(DTasks T, DDistros D, DWork W, DGen G) {
-  const unsigned int n = *G.ccount;
+// The tasks a multi-member unit emits, written by the unit: they share one key, Vmax - unit value, and one stretch of the
+// pre-arrangement, from its anchor's run start (e[] holds exclusive positions by now) in rank order.  The unit walks its
+// emitted-by-rank slots, so no member is placed by a loop over the others.  Units of up to kRankOne members: a thread per
+// unit, in id order (coalesced records); larger ones: a warp per unit (its chunk-0 entry in blist), 32 ranks per step, a
+// ballot giving every lane its place after the running count.
+__global__ void __launch_bounds__(256, kUnitTableOcc) k_gplace_unit(DDistros D, DWork W, DGen G) {
+  if (*W.err) return;
+  const unsigned int n = *G.hcount;
   for (unsigned int k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x) {
-  const uint4 ent = G.wl[k];
-  const uint32_t t = ent.x;
-  if (!(W.has_dep[t] & 2)) continue;
-  const int d = int(ent.y);
-  const int64_t base = D.task_off[d];
-  const uint4 tie = G.tie[k];
-  const uint32_t a = tie.x, myrk = tie.y, id = tie.z;
-  uint32_t pos = G.e[base + a];
-  const GUnit u = unit_load(G.unit + id);
-  if (u.n <= 64) {
-    pos += __popcll(u.mask & ((1ull << myrk) - 1ull));
-  } else {
-    const uint32_t* run = G.run + u.start;
-    for (uint32_t i = 0; i < u.n; i++) {
-      const uint4 tq = G.tie[run[i] & kRunEntry];
-      if (tq.z == id && tq.y < myrk) pos++;
-    }
+    const GUnit u = unit_load(G.unit + k);
+    if (u.anchor == kNoAnchor || u.n > kRankOne) continue;
+    // every load of the unit before its first store: a store may alias a later emit load, so a walk that stored as it
+    // loaded would wait a memory round trip per member
+    uint32_t li[kRankOne];
+#pragma unroll
+    for (uint32_t i = 0; i < kRankOne; i++) li[i] = i < u.n ? G.emit[u.start + i] : kInactive;
+    const int64_t base = D.task_off[u.d];
+    const unsigned long long key = G.vmm[2 * u.d] - ord_i64(u.value);
+    const bool wide = gen_bits(G, u.d) > 32;
+    uint32_t pos = G.e[base + u.anchor];
+#pragma unroll
+    for (uint32_t i = 0; i < kRankOne; i++)
+      if (li[i] != kInactive) gen_put_key(G, base, pos++, key, wide, li[i]);
   }
-  gen_put(G, base, pos, G.vmm[2 * d], gen_bits(G, d) > 32, G.tv[t], uint32_t(int64_t(t) - base));
+  const unsigned int nb = *G.bcount;
+  const unsigned full = 0xffffffffu;
+  const int lane = threadIdx.x & 31;
+  const unsigned lt = (1u << lane) - 1u;
+  const unsigned int nw = gridDim.x * (blockDim.x >> 5);
+  for (unsigned int c = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); c < nb; c += nw) {  // warp-uniform
+    const uint2 ch = G.blist[c];
+    if (ch.y != 0u) continue;  // one warp per unit
+    const GUnit u = unit_load(G.unit + ch.x);
+    if (u.anchor == kNoAnchor) continue;
+    const int64_t base = D.task_off[u.d];
+    const unsigned long long key = G.vmm[2 * u.d] - ord_i64(u.value);
+    const bool wide = gen_bits(G, u.d) > 32;
+    uint32_t pos = G.e[base + u.anchor];
+    for (uint32_t r0 = 0; r0 < u.n; r0 += 32) {
+      const uint32_t li = r0 + lane < u.n ? G.emit[u.start + r0 + lane] : kInactive;
+      const unsigned b = __ballot_sync(full, li != kInactive);
+      if (li != kInactive) gen_put_key(G, base, pos + uint32_t(__popc(b & lt)), key, wide, li);
+      pos += uint32_t(__popc(b));
+    }
   }
 }
 

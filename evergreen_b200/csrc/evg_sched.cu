@@ -1376,7 +1376,7 @@ struct evg_ctx {
   int general_complex = 0;
   int64_t Tgc = 0;  // tasks in general-path distros that can hold multi-member units (work-list capacity)
   DevBuf b_kv, b_vmm, b_klo[2], b_khi[2], b_ix[2], b_e, b_tilesum, b_gmisc;
-  DevBuf b_tiledistro, b_tilestart, b_dtileoff, b_tilehist, b_wl, b_pay, b_place, b_eplace, b_run, b_rank, b_blist, b_tie, b_unit, b_upd;
+  DevBuf b_tiledistro, b_tilestart, b_dtileoff, b_tilehist, b_wl, b_pay, b_place, b_eplace, b_run, b_rank, b_emit, b_blist, b_unit, b_upd;
   DevBuf b_qinfo, b_ginfo, b_order, b_tv, b_bd;
   DevBuf b_hflags, b_hgid, b_hexp, b_hstd, b_hstart, b_hostoff, b_acfg, b_gs, b_result, b_status;
   bool bd_valid = false;
@@ -1625,11 +1625,11 @@ int upload_tasks(evg_ctx* c, const char* who, const evg_task_soa* t, const evg_d
       CK(c->b_e.ensure(sizeof(uint32_t) * size_t(T + kColPad)));
       CK(c->b_wl.ensure(sizeof(uint4) * size_t(Tgc + 1)));
       CK(c->b_pay.ensure(sizeof(URec) * size_t(Tgc + 1)));
-      CK(c->b_tie.ensure(sizeof(uint4) * size_t(Tgc + 1)));
       CK(c->b_place.ensure(sizeof(uint32_t) * 2 * size_t(Tgc + 1)));
       CK(c->b_eplace.ensure(sizeof(uint32_t) * 2 * size_t(E + 1)));
       CK(c->b_run.ensure(sizeof(uint32_t) * size_t(Prec + 1)));
       CK(c->b_rank.ensure(sizeof(uint32_t) * size_t(Prec + 1)));
+      CK(c->b_emit.ensure(sizeof(uint32_t) * size_t(Prec + 1)));
       CK(c->b_blist.ensure(sizeof(uint2) * size_t(Prec / kRankOne + 1)));  // a unit of n > kRankOne members: ceil(n/32) <= n/kRankOne chunks
       CK(c->b_unit.ensure(sizeof(GUnit) * size_t(Urec + 1)));
     }
@@ -1754,9 +1754,9 @@ DGen dgen(const evg_ctx* c) {
   g.bcount = c->b_gmisc.as<unsigned int>() + 4;
   g.blist = c->b_blist.as<uint2>();
   g.rank = c->b_rank.as<uint32_t>();
+  g.emit = c->b_emit.as<uint32_t>();
   g.unit = c->b_unit.as<GUnit>();
   g.run = c->b_run.as<uint32_t>();
-  g.tie = c->b_tie.as<uint4>();
   g.tv = c->b_tv.as<int64_t>();
   return g;
 }
@@ -1870,7 +1870,7 @@ int run_general(evg_ctx* c, cudaStream_t st, const DTasks& dt, const DDistros& d
     launch(c, st, k_gscan, unsigned(gcount), 1024, 0, g, gl);
   }
   launch(c, st, k_gplace, nt, 256, 0, dd, w, g, gc);
-  if (gc) launch(c, st, k_gplace_disp, wl_grid, 256, 0, dt, dd, w, g);
+  if (gc) launch(c, st, k_gplace_unit, wl_grid, 256, 0, dd, w, g);
   if (c->timed) CK(cudaEventRecord(c->ev_sort0, st));  // the general path's segmented sort
   for (int j = 0; j < 8; j++) {  // passes beyond the tick's longest key exit at once (*maxpass is device-side)
     launch(c, st, k_ghist, nt, 256, 0, j, dd, g);
