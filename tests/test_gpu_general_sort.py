@@ -70,8 +70,9 @@ def digits(v, j) -> np.ndarray:
     return ((sort_keys(v) >> np.uint64(8 * j)) & np.uint64(255)).astype(np.int64)
 
 
-def craft(n, b, rng, shape="dense"):
-    """(priority, rank) of n lone tasks whose values span width b:
+def craft(n, b, rng, shape="dense", offset=0):
+    """(priority, rank) of n lone tasks whose values span width b (offset: added to every rank of a priority-0 draw, so
+    the values move without the width changing):
       dense    values spread over the whole range, the minimum and the maximum both present;
       levels3  three distinct values (the extremes and one between), dealt to the tasks at random: ties across tiles;
       all256   priority 0 and rank deltas (i mod 256) + 256 * r: every pass-0 digit in any 256 consecutive tasks;
@@ -81,7 +82,7 @@ def craft(n, b, rng, shape="dense"):
       top      values k * 2^56 + 1 for k = 1 .. 256 in turn: keys that differ only in the top digit of the high word."""
     idx = np.arange(n)
     if b == 0:
-        return np.zeros(n, np.int64), np.full(n, RANK_MIN, np.int64)
+        return np.zeros(n, np.int64), np.full(n, RANK_MIN + offset, np.int64)
     if shape == "top":  # (1 + 2^30 - 1) * (k * 2^26) + 1
         return np.full(n, 2 ** 30 - 1, np.int64), (1 + rng.permutation(n) % 256) << 26
     if shape == "stride32":  # (1 + p) * 2^32 + 1, 1 + p < 3 * 2^(b - 34)
@@ -101,7 +102,7 @@ def craft(n, b, rng, shape="dense"):
         if shape == "levels3":
             delta = np.array([0, top, top // 3])[rng.integers(0, 3, n)]
             delta[:3] = (0, top, top // 3)
-        return np.zeros(n, np.int64), RANK_MIN + delta
+        return np.zeros(n, np.int64), RANK_MIN + offset + delta
     # wider: 1 + priority < 2^pb times rank <= R, R * 2^pb = 3 * 2^(b - 2); b = 64 wraps
     pb = min(PRIO_BITS, b - EXACT_BITS + 1)
     R = (3 << (b - 2)) >> pb
@@ -116,20 +117,23 @@ def craft(n, b, rng, shape="dense"):
     return p, r
 
 
-def craft_checked(n, b, rng, shape="dense"):
-    p, r = craft(n, b, rng, shape)
+def craft_checked(n, b, rng, shape="dense", offset=0):
+    p, r = craft(n, b, rng, shape, offset)
     perm = np.arange(n) if shape == "all256" else rng.permutation(n)  # the extremes anywhere (all256 keeps its order)
     p, r = p[perm], r[perm]
     assert width(lone_value(p, r)) == b, (b, shape, width(lone_value(p, r)))
     return p, r
 
 
-def lone_tick(parts, seed, *, units=False):
+def lone_tick(parts, seed, *, units=False, edges=True, n_hosts=0):
     """One tick whose distro d takes the (priority, rank) columns parts[d] (synth.make draws the rest).  units: task
-    groups and in-queue dependency edges as synth.make places them (values of multi-member units are the oracle's)."""
+    groups and in-queue dependency edges as synth.make places them (values of multi-member units are the oracle's);
+    edges=False keeps the task groups only.  n_hosts: hosts for the allocator, as synth.make spreads them."""
     sizes = np.array([len(p) for p, _ in parts], np.int64)
-    w = synth.make(sizes, seed, tg_frac=0.1 if units else 0.0, met_dep_frac=0.03 if units else 0.0,
-                   unmet_dep_frac=0.01 if units else 0.0, includes_dependencies=units, custom_factor_frac=0.0)
+    deps = units and edges
+    w = synth.make(sizes, seed, tg_frac=0.1 if units else 0.0, met_dep_frac=0.03 if deps else 0.0,
+                   unmet_dep_frac=0.01 if deps else 0.0, includes_dependencies=deps, custom_factor_frac=0.0,
+                   n_hosts=n_hosts)
     set_values(w.tasks, np.arange(w.n_tasks), np.concatenate([p for p, _ in parts]), np.concatenate([r for _, r in parts]),
                keep_deps_met=units)
     for f, x in PLANNER.items():
@@ -157,20 +161,22 @@ def tick_values(w):
                                          + RUNTIME_FACTOR * (w.tasks.expected_ns // M.MINUTE)))
 
 
-def place(specs, seed):
-    """Distros from specs (n, start residue mod 4 or None, width, shape), in order; a filler distro of 1-3 tasks
-    (width 0, k_plan_warp) goes before a spec whose start would not have its residue.  -> (tick, spec distro ids)."""
+def place(specs, seed, *, units=False, edges=True, n_hosts=0):
+    """Distros from specs (n, start residue mod 4 or None, width, shape) -- or (n, residue, (priority, rank)) for columns
+    crafted elsewhere -- in order; a filler distro of 1-3 tasks (width 0, k_plan_warp) goes before a spec whose start
+    would not have its residue.  units, edges, n_hosts: as lone_tick.  -> (tick, spec distro ids)."""
     rng = np.random.default_rng(seed)
     parts, ids, base = [], [], 0
-    for n, res, b, shape in specs:
+    for n, res, *what in specs:
         if res is not None and base % 4 != res:
             k = (res - base) % 4
             parts.append(craft(k, 0, rng))
             base += k
         ids.append(len(parts))
-        parts.append(craft_checked(n, b, rng, shape))
+        parts.append(what[0] if len(what) == 1 else craft_checked(n, what[0], rng, what[1]))
+        assert len(parts[-1][0]) == n
         base += n
-    return lone_tick(parts, seed), ids
+    return lone_tick(parts, seed, units=units, edges=edges, n_hosts=n_hosts), ids
 
 
 def size_for(tiles, res, last):
