@@ -19,9 +19,10 @@
 //   k_ghist/k_gdscan/k_gscatter
 //                  stable LSD radix sort on key = Vmax - V only: 32-bit keys, ceil(bits(Vmax-Vmin)/8) passes (3 for
 //                  a 20-bit range), 8 B/task each way per pass; a distro whose range exceeds 32 bits carries a
-//                  second key word and up to 8 passes (per-distro branch, same kernels)
-//   k_gemit        ranked queue + TotalValue
-// TotalValue per task is parked in the total_value OUTPUT buffer between k_gtask and k_gplace (no 8 B/task scratch).
+//                  second key word and up to 8 passes (per-distro branch, same kernels); a distro's last pass writes
+//                  the ranked queue and TotalValue instead of keys
+// TotalValue per task is parked in the total_value OUTPUT buffer between k_gtask and k_gplace (no 8 B/task scratch); the
+// last radix pass overwrites it with TotalValue by rank.
 //
 // Reference: scheduler/planner.go:209-481, scheduler/scheduler.go:56-159.
 #pragma once
@@ -71,7 +72,8 @@ __device__ __forceinline__ int gen_bits(const DGen& G, int d) {  // significant 
   const unsigned long long r = G.vmm[2 * d] - G.vmm[2 * d + 1];
   return r == 0 ? 0 : 64 - __clzll((long long)r);
 }
-__device__ __forceinline__ int gen_npass(int bits) { return (bits + 7) >> 3; }
+// at least one: the last pass writes the ranked queue, so a distro of width 0 takes one pass too
+__device__ __forceinline__ int gen_npass(int bits) { return bits ? (bits + 7) >> 3 : 1; }
 
 // A work-list entry's member payload: the fields Unit.info, the in-unit order and TaskGroupInfo need.
 struct __align__(16) URec {
@@ -744,8 +746,7 @@ __global__ void __launch_bounds__(256, kUnitTableOcc) k_gbest(DTasks T, DDistros
 __global__ void k_gsched(DGen G, const int32_t* __restrict__ general_list, int n) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n) return;
-  const int np = gen_npass(gen_bits(G, general_list[k]));
-  if (np > 0) atomicMax(G.maxpass, np);
+  atomicMax(G.maxpass, gen_npass(gen_bits(G, general_list[k])));
 }
 
 // sum of e[] over each tile
@@ -987,10 +988,11 @@ __global__ void __launch_bounds__(256, kUnitTableOcc) k_gplace_unit(DDistros D, 
 }
 
 __device__ __forceinline__ bool gen_tile(const DDistros& D, const DGen& G, int tile, int j, int* d_out, int64_t* seg, int64_t* lo,
-                                         int* cnt, bool* wide) {
+                                         int* cnt, bool* wide, bool* last) {
   const int d = G.tile_distro[tile];
-  const int bits = gen_bits(G, d);
-  if (j >= gen_npass(bits)) return false;
+  const int bits = gen_bits(G, d), np = gen_npass(bits);
+  if (j >= np) return false;
+  *last = j == np - 1;
   const int64_t base = D.task_off[d], end = D.task_off[d + 1];
   const int64_t a = max(G.tile_start[tile], base), b = min(G.tile_start[tile] + kGTile, end);
   *d_out = d; *seg = base; *lo = a; *cnt = int(b - a); *wide = bits > 32;
@@ -999,9 +1001,9 @@ __device__ __forceinline__ bool gen_tile(const DDistros& D, const DGen& G, int t
 
 __global__ void __launch_bounds__(256) k_ghist(int j, DDistros D, DGen G) {
   if (j >= *G.maxpass) return;
-  int d, cnt; int64_t seg, lo; bool wide;
+  int d, cnt; int64_t seg, lo; bool wide, last;
   const int tile = int(blockIdx.x + G.tile0);
-  if (!gen_tile(D, G, tile, j, &d, &seg, &lo, &cnt, &wide)) return;
+  if (!gen_tile(D, G, tile, j, &d, &seg, &lo, &cnt, &wide, &last)) return;
   const uint32_t* src = (j < 4 ? G.key_lo[j & 1] : G.key_hi[j & 1]) + lo;
   const int shift = 8 * (j & 3);
   __shared__ uint32_t h[256];
@@ -1064,9 +1066,11 @@ __global__ void __launch_bounds__(1024) k_gdscan(int j, const int32_t* __restric
 // the group size to the warp's digit counter and gets back the count of equal digits in the warp's earlier chunks (as in
 // k_plan_cta).  The tile is then sorted by digit IN SHARED MEMORY and written out in that order: consecutive threads
 // write consecutive addresses inside a digit's run, so a run costs its sectors once -- scattering straight from
-// registers puts nearly every 4-byte store in a sector of its own (L2-write bound).
+// registers puts nearly every 4-byte store in a sector of its own (L2-write bound).  A distro's last pass writes order[]
+// and TotalValue per rank (planner.go:467-477) instead of the key / index pair.
 template <bool WIDE>
-__device__ __forceinline__ void gscatter_tile(int j, const DGen& G, int tile, int64_t seg, int64_t lo, int cnt, uint32_t (*wcnt)[256],
+__device__ __forceinline__ void gscatter_tile(int j, const DGen& G, int tile, int d, int64_t seg, int64_t lo, int cnt, bool last,
+                                              int32_t* __restrict__ order, int64_t* __restrict__ total_value, uint32_t (*wcnt)[256],
                                               uint32_t* s_lo, uint32_t* s_ix, uint32_t* s_hi, int32_t* s_delta, uint32_t* s_wsum) {
   constexpr bool wide = WIDE;
   const int sb = j & 1, db = sb ^ 1;
@@ -1135,6 +1139,18 @@ __device__ __forceinline__ void gscatter_tile(int j, const DGen& G, int tile, in
     }
   }
   __syncthreads();
+  if (last) {
+    const unsigned long long vmax_ord = G.vmm[2 * d];
+    int32_t* dst_o = order + seg;
+    int64_t* dst_v = total_value + seg;
+    for (int i = tid; i < cnt; i += 256) {
+      const uint32_t a = s_lo[i], h = wide ? s_hi[i] : 0u;
+      const int64_t pos = int64_t(s_delta[((use_hi ? h : a) >> shift) & 255u]) + i;
+      dst_o[pos] = int32_t(s_ix[i]);
+      dst_v[pos] = unord_i64(vmax_ord - (((unsigned long long)h << 32) | a));
+    }
+    return;
+  }
   uint32_t* dst_lo = G.key_lo[db] + seg;
   uint32_t* dst_hi = G.key_hi[db] + seg;
   uint32_t* dst_ix = G.idx[db] + seg;
@@ -1150,33 +1166,16 @@ __device__ __forceinline__ void gscatter_tile(int j, const DGen& G, int tile, in
 
 // The key's high word travels only for distros whose value range exceeds 32 bits (a handful of registers and 8 KB of
 // shared memory the common case does not pay for).
-__global__ void __launch_bounds__(256, 4) k_gscatter(int j, DDistros D, DGen G) {
+__global__ void __launch_bounds__(256, 4) k_gscatter(int j, DDistros D, DGen G, int32_t* __restrict__ order,
+                                                     int64_t* __restrict__ total_value) {
   if (j >= *G.maxpass) return;
-  int d, cnt; int64_t seg, lo; bool wide;
+  int d, cnt; int64_t seg, lo; bool wide, last;
   const int tile = int(blockIdx.x + G.tile0);
-  if (!gen_tile(D, G, tile, j, &d, &seg, &lo, &cnt, &wide)) return;
+  if (!gen_tile(D, G, tile, j, &d, &seg, &lo, &cnt, &wide, &last)) return;
   __shared__ uint32_t wcnt[8][256];   // per-warp digit counters, then local positions
   __shared__ uint32_t s_lo[kGTile], s_ix[kGTile], s_hi[kGTile];
   __shared__ int32_t s_delta[256];    // digit -> (offset of the digit's run in the distro) - (its offset in the sorted tile)
   __shared__ uint32_t s_wsum[8];
-  if (wide) gscatter_tile<true>(j, G, tile, seg, lo, cnt, wcnt, s_lo, s_ix, s_hi, s_delta, s_wsum);
-  else gscatter_tile<false>(j, G, tile, seg, lo, cnt, wcnt, s_lo, s_ix, s_hi, s_delta, s_wsum);
-}
-
-// Ranked queue out: order[] and TotalValue per rank (planner.go:467-477).
-__global__ void __launch_bounds__(256) k_gemit(DDistros D, DGen G, int32_t* __restrict__ order, int64_t* __restrict__ total_value) {
-  const int tile = int(blockIdx.x + G.tile0);
-  const int d = G.tile_distro[tile];
-  const int64_t base = D.task_off[d], end = D.task_off[d + 1];
-  const int64_t lo = max(G.tile_start[tile], base), hi = min(G.tile_start[tile] + kGTile, end);
-  const int bits = gen_bits(G, d);
-  const int fin = gen_npass(bits) & 1;
-  const bool wide = bits > 32;
-  const unsigned long long vmax_ord = G.vmm[2 * d];
-  for (int64_t p = lo + threadIdx.x; p < hi; p += 256) {
-    unsigned long long key = G.key_lo[fin][p];
-    if (wide) key |= (unsigned long long)G.key_hi[fin][p] << 32;
-    order[p] = int32_t(G.idx[fin][p]);
-    total_value[p] = unord_i64(vmax_ord - key);
-  }
+  if (wide) gscatter_tile<true>(j, G, tile, d, seg, lo, cnt, last, order, total_value, wcnt, s_lo, s_ix, s_hi, s_delta, s_wsum);
+  else gscatter_tile<false>(j, G, tile, d, seg, lo, cnt, last, order, total_value, wcnt, s_lo, s_ix, s_hi, s_delta, s_wsum);
 }

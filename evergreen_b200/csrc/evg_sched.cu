@@ -11,8 +11,8 @@
 //   larger           the general path (evg_plan_general.cuh), any size up to 2^21-1 tasks:
 //     k_gmark/k_gtask/k_gunit/k_gbest  dependents, per-task pass, multi-member units
 //     k_gsum/k_gscan/k_gplace*     canonical pre-arrangement by counting
-//     k_ghist/k_gdscan/k_gscatter  segmented stable LSD radix sort of 32-bit keys
-//     k_gemit                      ranked queue + TotalValue
+//     k_ghist/k_gdscan/k_gscatter  segmented stable LSD radix sort of 32-bit keys; the last pass writes the ranked
+//                                  queue + TotalValue
 //     k_finalize_info              DistroQueueInfo / TaskGroupInfo scalars (scheduler.go:144-158)
 // Both:
 //   k_breakdown           the 13-field SortingValueBreakdown per ranked task (EVG_OPT_BREAKDOWN)
@@ -1875,10 +1875,9 @@ int run_general(evg_ctx* c, cudaStream_t st, const DTasks& dt, const DDistros& d
   for (int j = 0; j < 8; j++) {  // passes beyond the tick's longest key exit at once (*maxpass is device-side)
     launch(c, st, k_ghist, nt, 256, 0, j, dd, g);
     launch(c, st, k_gdscan, unsigned(gcount), 1024, 0, j, gl, g);
-    launch(c, st, k_gscatter, nt, 256, 0, j, dd, g);
+    launch(c, st, k_gscatter, nt, 256, 0, j, dd, g, c->b_order.as<int32_t>(), c->b_tv.as<int64_t>());
   }
   if (c->timed) CK(cudaEventRecord(c->ev_sort1, st));
-  launch(c, st, k_gemit, nt, 256, 0, dd, g, c->b_order.as<int32_t>(), c->b_tv.as<int64_t>());
   const int64_t g0 = c->h_groupoff[size_t(d_first)], g1 = c->h_groupoff[size_t(d_last) + 1];
   launch(c, st, k_finalize_info, grid_for(std::max<int64_t>(d_last + 1 - d_first, g1 - g0), 256), 256, 0, dd, w, d_first, d_last + 1, g0, g1);
   return EVG_OK;
