@@ -102,34 +102,22 @@ __device__ __forceinline__ unsigned long long dag_group_key(const DDag& X, int64
   if (gid < 0) return ~0ull;
   return ((unsigned long long)uint32_t(gid) << 32) | (unsigned long long)(uint32_t(X.group_index[g]) ^ 0x80000000u);
 }
+// k_seg_merge_pass's order of a distro's item indices (distro-local) by dag_group_key
+struct DagGroupOrder {
+  using Elem = int32_t;
+  DDag X;
+  struct Pivot {
+    DDag X; int64_t base; unsigned long long key;
+    __device__ bool before(int32_t x) const { return dag_group_key(X, base + x) < key; }
+    __device__ bool after(int32_t x) const { return dag_group_key(X, base + x) > key; }
+  };
+  __device__ Pivot pivot(int, int64_t base, int32_t me) const { return {X, base, dag_group_key(X, base + me)}; }
+};
 __global__ void __launch_bounds__(256) k_dag_group_init(DDag X, int32_t* __restrict__ idx) {
   const int64_t p = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
   if (p >= X.n) return;
   const int d = find_distro(X.item_off, 0, X.n_distros - 1, p);
   idx[p] = int32_t(p - X.item_off[d]);
-}
-// one pass of a segmented STABLE merge sort (runs of length L inside each distro's items)
-__global__ void __launch_bounds__(256) k_dag_group_pass(DDag X, const int32_t* __restrict__ src, int32_t* __restrict__ dst, int64_t L) {
-  const int64_t p = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (p >= X.n) return;
-  const int d = find_distro(X.item_off, 0, X.n_distros - 1, p);
-  const int64_t base = X.item_off[d], n = X.item_off[d + 1] - base;
-  const int64_t q = p - base;
-  const int32_t me = src[p];
-  if (L >= n) { dst[p] = me; return; }
-  const int64_t r = q / L, own0 = r * L;
-  int64_t s0, s1;
-  if ((r & 1) == 0) { s0 = own0 + L; s1 = min(s0 + L, n); } else { s0 = own0 - L; s1 = own0; }
-  if (s0 >= n) { dst[p] = me; return; }
-  const unsigned long long km = dag_group_key(X, base + me);
-  int64_t lo = s0, hi = s1;
-  if ((r & 1) == 0) {  // left run: sibling elements strictly smaller go first
-    while (lo < hi) { const int64_t m = (lo + hi) >> 1; if (dag_group_key(X, base + src[base + m]) < km) lo = m + 1; else hi = m; }
-    dst[base + own0 + (q - own0) + (lo - s0)] = me;
-  } else {             // right run: sibling elements smaller or equal go first (stability)
-    while (lo < hi) { const int64_t m = (lo + hi) >> 1; if (dag_group_key(X, base + src[base + m]) <= km) lo = m + 1; else hi = m; }
-    dst[base + s0 + (lo - s0) + (q - own0)] = me;
-  }
 }
 // bucket boundaries: unit_off[group_off[d] + g] = first position (distro-local) of group g in the sorted items;
 // the entry after a distro's last group is written by the host from grouped[d] (items that have a group)

@@ -52,30 +52,17 @@ __global__ void __launch_bounds__(256) k_es_pool_off(int32_t n_distros, const in
   if (d < n_distros) hosts_used[d] = int32_t(pos[host_off[d + 1]] - p);
 }
 
-// sort.Sort(s.hosts) (:60) for every distro: one pass of a segmented merge sort of signed int64 values (runs of length
-// L inside each distro's pool), one thread per value.  Pools of any size; equal values are interchangeable.
-__global__ void __launch_bounds__(256) k_es_sort_pass(int32_t n_distros, const int64_t* __restrict__ pool_off,
-                                                      const int64_t* __restrict__ src, int64_t* __restrict__ dst, int64_t L) {
-  const int64_t p = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
-  const int d = block_find_distro(pool_off, n_distros, p, pool_off[n_distros]);
-  if (d < 0) return;
-  const int64_t base = pool_off[d], n = pool_off[d + 1] - base;
-  const int64_t q = p - base;
-  const int64_t me = src[p];
-  if (L >= n) { dst[p] = me; return; }
-  const int64_t r = q / L, own0 = r * L;
-  int64_t s0, s1;
-  if ((r & 1) == 0) { s0 = own0 + L; s1 = min(s0 + L, n); } else { s0 = own0 - L; s1 = own0; }
-  if (s0 >= n) { dst[p] = me; return; }
-  int64_t lo = s0, hi = s1;
-  if ((r & 1) == 0) {  // left run: the sibling's strictly smaller values go first
-    while (lo < hi) { const int64_t m = (lo + hi) >> 1; if (src[base + m] < me) lo = m + 1; else hi = m; }
-    dst[base + q + (lo - s0)] = me;
-  } else {             // right run: the sibling's smaller or equal values go first
-    while (lo < hi) { const int64_t m = (lo + hi) >> 1; if (src[base + m] <= me) lo = m + 1; else hi = m; }
-    dst[base + lo + (q - own0)] = me;
-  }
-}
+// sort.Sort(s.hosts) (:60) for every distro: k_seg_merge_pass's order of the pool values, signed int64 ascending.
+// Pools of any size; equal values are interchangeable.
+struct EsValueOrder {
+  using Elem = int64_t;
+  struct Pivot {
+    int64_t me;
+    __device__ bool before(int64_t x) const { return x < me; }
+    __device__ bool after(int64_t x) const { return x > me; }
+  };
+  __device__ Pivot pivot(int, int64_t, int64_t me) const { return {me}; }
+};
 
 // The chained call's queue: TaskQueueItem.ExpectedDuration of every persisted rank, the column and rank order
 // k_project_queue reads.

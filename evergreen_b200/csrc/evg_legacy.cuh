@@ -90,32 +90,17 @@ __global__ void __launch_bounds__(256) k_legacy_init(DLegacy X, int32_t* idx, un
   atomicAdd(&counts[d * 4 + legacy_list(X, t)], 1u);
 }
 
-// One pass of a segmented merge sort: runs of length L inside each distro's segment are merged pairwise; every element
-// finds its destination with one binary search in the sibling run.
-__global__ void __launch_bounds__(256) k_legacy_merge_pass(DLegacy X, const int32_t* __restrict__ src, int32_t* __restrict__ dst, int64_t L) {
-  const int64_t p = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (p >= X.n) return;
-  const int d = find_distro(X.task_off, 0, X.n_distros - 1, p);
-  const int64_t base = X.task_off[d], n = X.task_off[d + 1] - base;
-  const int64_t q = p - base;
-  const int32_t me = src[p];
-  if (L >= n) { dst[p] = me; return; }
-  const int64_t r = q / L;
-  const int64_t own0 = r * L;
-  int64_t s0, s1;
-  if ((r & 1) == 0) { s0 = own0 + L; s1 = min(s0 + L, n); }
-  else { s0 = own0 - L; s1 = own0; }
-  if (s0 >= n) { dst[p] = me; return; }  // no sibling: the run is copied
-  const int64_t gm = base + me;
-  int64_t lo = s0, hi = s1;
-  if ((r & 1) == 0) {  // left run: count sibling elements strictly before me
-    while (lo < hi) { const int64_t m = (lo + hi) >> 1; if (legacy_less(X, d, base + src[base + m], gm)) lo = m + 1; else hi = m; }
-    dst[base + own0 + (q - own0) + (lo - s0)] = me;
-  } else {             // right run: count sibling elements not after me
-    while (lo < hi) { const int64_t m = (lo + hi) >> 1; if (!legacy_less(X, d, gm, base + src[base + m])) lo = m + 1; else hi = m; }
-    dst[base + s0 + (lo - s0) + (q - own0)] = me;
-  }
-}
+// k_seg_merge_pass's order of a distro's task indices (distro-local) by legacy_less
+struct LegacyOrder {
+  using Elem = int32_t;
+  DLegacy X;
+  struct Pivot {
+    DLegacy X; int d; int64_t base, gm;
+    __device__ bool before(int32_t x) const { return legacy_less(X, d, base + x, gm); }
+    __device__ bool after(int32_t x) const { return legacy_less(X, d, gm, base + x); }
+  };
+  __device__ Pivot pivot(int d, int64_t base, int32_t me) const { return {X, d, base, base + me}; }
+};
 
 // mergeTasks (task_prioritizer.go:251-278): high-priority tasks, then patch / repotracker alternately (patch first)
 // until one list runs out, then the rest of the other; dropped tasks leave -1 slots at the end.

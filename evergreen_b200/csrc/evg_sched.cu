@@ -263,6 +263,36 @@ __device__ __forceinline__ int block_find_distro(const int64_t* __restrict__ off
   return find_distro(off, s_lo, s_hi, t);
 }
 
+// One pass of a segmented stable merge sort, one thread per element: inside each segment [off[d], off[d+1]) of src,
+// runs of length L are merged pairwise into dst.  An element of a left run goes after the sibling run's elements that
+// sort strictly before it, one of a right run after those that do not sort after it: equal elements keep their order.
+// The total off[n_segs] is read here, so the grid may be sized by any bound above it.  Order::pivot(d, base, me) reads
+// what it needs of `me` once and answers before(x) ("x sorts strictly before me") and after(x) ("strictly after").
+template <class Order>
+__global__ void __launch_bounds__(256) k_seg_merge_pass(Order order, const int64_t* __restrict__ off, int32_t n_segs,
+                                                        const typename Order::Elem* __restrict__ src,
+                                                        typename Order::Elem* __restrict__ dst, int64_t L) {
+  const int64_t p = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  const int d = block_find_distro(off, n_segs, p, off[n_segs]);
+  if (d < 0) return;
+  const int64_t base = off[d], n = off[d + 1] - base, q = p - base;
+  const typename Order::Elem me = src[p];
+  if (L >= n) { dst[p] = me; return; }
+  const int64_t r = q / L, own0 = r * L;
+  const bool left = (r & 1) == 0;
+  const int64_t s0 = left ? own0 + L : own0 - L, s1 = left ? min(s0 + L, n) : own0;  // the sibling run
+  if (s0 >= n) { dst[p] = me; return; }  // a last left run without a sibling is copied
+  const auto pv = order.pivot(d, base, me);
+  int64_t lo = s0, hi = s1;
+  if (left) {  // the merged pair starts at own0: q - own0 of the own run and lo - s0 of the sibling's go first
+    while (lo < hi) { const int64_t m = (lo + hi) >> 1; if (pv.before(src[base + m])) lo = m + 1; else hi = m; }
+    dst[base + q + (lo - s0)] = me;
+  } else {     // the merged pair starts at s0: lo - s0 of the sibling's and q - own0 of the own run go first
+    while (lo < hi) { const int64_t m = (lo + hi) >> 1; if (!pv.after(src[base + m])) lo = m + 1; else hi = m; }
+    dst[base + lo + (q - own0)] = me;
+  }
+}
+
 __device__ __forceinline__ int64_t warp_sum64(int64_t v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -1400,6 +1430,18 @@ void launch(evg_ctx* c, cudaStream_t st, void (*kernel)(P...), unsigned grid, un
   if (grid == 0) return;
   kernel<<<grid, block, smem, st>>>(std::forward<A>(args)...);
   c->launches++;
+}
+
+// Sorts every segment of buf[0] that off (on the device, n_segs + 1 entries) delimits: ceil(log2 max_len) passes of
+// k_seg_merge_pass over n_threads threads, max_len and n_threads bounding the longest segment and the element total.
+// Returns the buffer that holds the result: buf[0] when max_len <= 1 and no pass runs.
+template <class Order>
+typename Order::Elem* seg_merge_sort(evg_ctx* c, cudaStream_t s, const Order& order, const int64_t* off, int32_t n_segs,
+                                     int64_t n_threads, int64_t max_len, typename Order::Elem* const buf[2]) {
+  int cur = 0;
+  for (int64_t L = 1; L < max_len; L <<= 1, cur ^= 1)
+    launch(c, s, k_seg_merge_pass<Order>, grid_for(n_threads, 256), 256, 0, order, off, n_segs, buf[cur], buf[cur ^ 1], L);
+  return buf[cur];
 }
 
 // The start of every entry point that takes a context: it names the call once (`who`, for its later messages too), fails
@@ -3909,14 +3951,10 @@ int evg_prioritize_legacy_batch(evg_ctx* c, const evg_legacy_soa* in, const int6
   x.presort = c->b_rn1.as<int32_t>(); x.flags = c->tasks.flags.as<uint32_t>(); x.list_mode = c->b_rn2.as<uint8_t>();
   x.task_off = c->b_taskoff.as<int64_t>(); x.n_distros = D;
   int32_t* buf[2] = {c->b_rn3.as<int32_t>(), c->b_rn4.as<int32_t>()};
-  int cur = 0;
   if (T > 0) {
     launch(c, c->stream, k_legacy_init, grid_for(T, 256), 256, 0, x, buf[0], c->b_rn5.as<unsigned int>());
-    for (int64_t L = 1; L < max_n; L <<= 1) {
-      launch(c, c->stream, k_legacy_merge_pass, grid_for(T, 256), 256, 0, x, buf[cur], buf[cur ^ 1], L);
-      cur ^= 1;
-    }
-    launch(c, c->stream, k_legacy_interleave, grid_for(T, 256), 256, 0, x, buf[cur], c->b_rn5.as<unsigned int>(), c->b_order.as<int32_t>(),
+    const int32_t* sorted = seg_merge_sort(c, c->stream, LegacyOrder{x}, x.task_off, D, T, max_n, buf);
+    launch(c, c->stream, k_legacy_interleave, grid_for(T, 256), 256, 0, x, sorted, c->b_rn5.as<unsigned int>(), c->b_order.as<int32_t>(),
            c->b_rn6.as<int64_t>(), c->b_status.as<int32_t>());
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(order, c->b_order.p, sizeof(int32_t) * size_t(T), cudaMemcpyDeviceToHost, s));
@@ -3946,7 +3984,7 @@ struct DagBufs {
   const int64_t* group_off;
   int32_t* unit_off;
 };
-// k_dag_topo, then the task-group buckets (k_dag_group_init / k_dag_group_pass / k_dag_units) over x, and the results
+// k_dag_topo, then the task-group buckets (k_dag_group_init / seg_merge_sort / k_dag_units) over x, and the results
 // copied to the host.  item_off / group_off (D+1) are the host copies of x's offsets; max_n is the longest queue.
 static int dag_run(evg_ctx* c, const DDag& x, const DagBufs& b, int64_t max_n, const int64_t* item_off, const int64_t* group_off,
                    int32_t* sorted, int32_t* n_sorted, int32_t* n_cycles, int32_t* unit_items, int32_t* unit_off,
@@ -3960,20 +3998,17 @@ static int dag_run(evg_ctx* c, const DDag& x, const DagBufs& b, int64_t max_n, c
   int32_t* d_grouped = d_ncycles + (D + 1);
   launch(c, c->stream, k_dag_topo, grid_for(int64_t(D) * 32, 64), 64, 0, x, b.sorted, d_nsorted, d_ncycles);
   std::vector<int32_t> grouped(size_t(D), 0);
-  int cur = 0;
+  int32_t* items = b.buf[0];
   if (N > 0) {
     CK(cudaMemcpyAsync(sorted, b.sorted, sizeof(int32_t) * size_t(N), cudaMemcpyDeviceToHost, s));
     // every item has a group or not: "no ungrouped item" leaves grouped[d] at the distro's length
     for (int32_t d = 0; d < D; d++) grouped[size_t(d)] = int32_t(item_off[d + 1] - item_off[d]);
     CK(cudaMemcpyAsync(d_grouped, grouped.data(), sizeof(int32_t) * size_t(D), cudaMemcpyHostToDevice, s));
     launch(c, c->stream, k_dag_group_init, grid_for(N, 256), 256, 0, x, b.buf[0]);
-    for (int64_t L = 1; L < max_n; L <<= 1) {
-      launch(c, c->stream, k_dag_group_pass, grid_for(N, 256), 256, 0, x, b.buf[cur], b.buf[cur ^ 1], L);
-      cur ^= 1;
-    }
-    launch(c, c->stream, k_dag_units, grid_for(N, 256), 256, 0, x, b.buf[cur], b.group_off, b.unit_off, d_grouped);
+    items = seg_merge_sort(c, c->stream, DagGroupOrder{x}, x.item_off, D, N, max_n, b.buf);
+    launch(c, c->stream, k_dag_units, grid_for(N, 256), 256, 0, x, items, b.group_off, b.unit_off, d_grouped);
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(unit_items, b.buf[cur], sizeof(int32_t) * size_t(N), cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(unit_items, items, sizeof(int32_t) * size_t(N), cudaMemcpyDeviceToHost, s));
     CK(cudaMemcpyAsync(unit_off, b.unit_off, sizeof(int32_t) * size_t(G + D), cudaMemcpyDeviceToHost, s));
     CK(cudaMemcpyAsync(grouped.data(), d_grouped, sizeof(int32_t) * size_t(D), cudaMemcpyDeviceToHost, s));
   }
@@ -3981,7 +4016,7 @@ static int dag_run(evg_ctx* c, const DDag& x, const DagBufs& b, int64_t max_n, c
   CK(cudaMemcpyAsync(n_cycles, d_ncycles, sizeof(int32_t) * size_t(D), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   for (int32_t d = 0; d < D; d++) unit_off[group_off[d + 1] + d] = grouped[size_t(d)];  // the closing entry of each distro
-  if (d_unit_items) *d_unit_items = b.buf[cur];
+  if (d_unit_items) *d_unit_items = items;
   return EVG_OK;
 }
 
@@ -4857,12 +4892,11 @@ static int estimate_run(evg_ctx* c, int32_t D, const evg_est_host_soa* h, const 
     std::stable_sort(list.begin(), list.end(), [&](int32_t a, int32_t b) { return work(a) > work(b); });
     UP(s, x.list, list.data(), int64_t(list.size()), int32_t);
     CK(x.start.ensure(sizeof(int64_t) * size_t(N)));
-    int cur = 0;
-    for (int64_t L = 1; L < max_hosts; L <<= 1, cur ^= 1)
-      launch(c, s, k_es_sort_pass, grid_for(H, 256), 256, 0, D, x.pool_off.as<int64_t>(), x.pool[cur].as<int64_t>(), x.pool[cur ^ 1].as<int64_t>(), L);
+    int64_t* const pools[2] = {x.pool[0].as<int64_t>(), x.pool[1].as<int64_t>()};
+    int64_t* pool = seg_merge_sort(c, s, EsValueOrder{}, x.pool_off.as<int64_t>(), D, H, max_hosts, pools);
     CK(cudaMemsetAsync(x.start.p, 0xFF, sizeof(int64_t) * size_t(N), s));  // -1: no estimate
     const DEst X{x.list.as<int32_t>(), int32_t(list.size()), x.pool_off.as<int64_t>(), x.item_off.as<int64_t>(), x.dur.as<int64_t>(),
-                 x.pool[cur].as<int64_t>(), x.start.as<int64_t>()};
+                 pool, x.start.as<int64_t>()};
     launch(c, s, k_es_sim, grid_for(int64_t(list.size()), kEsWarps), 32 * kEsWarps, 0, X);
   }
   CK(cudaGetLastError());

@@ -7,9 +7,9 @@
 Shapes: the flagship (--distros distros x --tasks tasks in configs[2]'s mix, a generated block of --block distros tiled
 as bench.py tiles it; persisted heads of 10 000 items) and configs[4] (100 000 ragged distros).  Both calls end in a
 stream synchronise, so the host clock around each spans its copies and kernels.  Per shape: warm-up, --reps alternating
-pairs, the launch count, the bytes each route moves over PCIe (computed from the shapes), torch.profiler's k_dag_* and
-k_dp_* kernel times of one device call, and an equality check of every output array.  Prints one JSON line with the
-card's name and power limit."""
+pairs, the launch count, the bytes each route moves over PCIe (computed from the shapes), torch.profiler's k_dag_*,
+k_seg_merge_pass and k_dp_* kernel times of one device call, and an equality check of every output array.  Prints one
+JSON line with the card's name and power limit."""
 import argparse
 import json
 import os
@@ -71,7 +71,7 @@ def profile_device(eng):
     kern = {}
     for e in prof.events():
         if e.device_type == torch.autograd.DeviceType.CUDA:
-            name = next((n for n in ("k_dag_topo", "k_dag_group_init", "k_dag_group_pass", "k_dag_units", "k_dp_gather",
+            name = next((n for n in ("k_dag_topo", "k_dag_group_init", "k_seg_merge_pass", "k_dag_units", "k_dp_gather",
                                      "k_dp_edges", "k_dp_groups", "k_scan_") if n in e.name), None)
             if name:
                 us = e.device_time if hasattr(e, "device_time") else e.cuda_time

@@ -19,13 +19,13 @@ once at more than 1 048 576 pairs, where scan_counts' block sums take k_scan_sum
 The fourth pass (shift 56) is not reached.  It needs D > 2^24, i.e. 16.8 M distro cfg rows and about 1.5 GB of host
 cfg.  It is the same kernel at a higher shift, and passes two and three already show that the shift advances.
 
-The segmented merge sorts (k_legacy_merge_pass, k_dag_group_pass, k_es_sort_pass) share one pass structure.  Runs of
-length L = 1, 2, 4, ... below the longest segment are merged pairwise, each element placed by one binary search in
-its sibling run: a left run counts the sibling's elements that sort strictly before it, a right run those that do not
-sort after it.  Edge branches: L >= n copies the segment, a run with no sibling (s0 >= n) is copied, and
-s1 = min(s0 + L, n) shortens the last sibling.  The pass count comes from the longest segment, so one shape set (the
-segments of SHAPE, with the longest one first, then last, and a call of many empty segments between tiny ones) runs
-through all three:
+The segmented merge sorts (k_seg_merge_pass<LegacyOrder / DagGroupOrder / EsValueOrder>) are one kernel template with
+three orders.  Runs of length L = 1, 2, 4, ... below the longest segment are merged pairwise, each element placed by
+one binary search in its sibling run: a left run counts the sibling's elements that sort strictly before it, a right
+run those that do not sort after it.  Edge branches: L >= n copies the segment, a run with no sibling (s0 >= n) is
+copied, and s1 = min(s0 + L, n) shortens the last sibling.  The pass count comes from the longest segment, so one
+shape set (the segments of SHAPE, with the longest one first, then last, and a call of many empty segments between
+tiny ones) runs through all three:
   legacy      a numpy lexsort of the comparator chain per list, then mergeTasks' interleave (oracle_legacy)
   DAG groups  oracle_dag.rebuild
   estimates   the numpy restatement of test_gpu_start_estimate (fresh / expect)
