@@ -197,7 +197,7 @@ class LegacySoAStruct(C.Structure):
 
 
 EVG_LF_REQ_SYSTEM, EVG_LF_REQ_PATCH, EVG_LF_REQ_OTHER, EVG_LF_GENERATE, EVG_LF_MERGE_QUEUE_VERSION = 0, 1, 2, 0x4, 0x8
-EVG_LEGACY_MODE_INGEST, EVG_LEGACY_MODE_REVISION, EVG_LEGACY_MODE_LITERAL = 0, 1, 2
+EVG_LEGACY_MODE_INGEST, EVG_LEGACY_MODE_REVISION, EVG_LEGACY_MODE_LITERAL, EVG_LEGACY_MODE_GO_STABLE = 0, 1, 2, 3
 EVG_LEGACY_OK, EVG_LEGACY_NOT_DECOMPOSABLE = 0, 1
 
 

@@ -162,6 +162,8 @@ constexpr int kNT_C = 512, kNCapC = 10240, kNOccC = 2;
 constexpr uint32_t kInactive = 0xFFFFFFFFu;  // next[]: pair not linked / head[]: empty list
 constexpr uint32_t kEnd = 0xFFFFFFFEu;       // next[]: end of list
 constexpr uint32_t kNoAnchor = 0xFFFFFFFFu;
+// k_gs_wave: a wave whose largest symMerge call spans more tasks than this rotates with a CTA per call, otherwise a warp
+constexpr int64_t kGsWarpRotation = 1024;
 // Columns are padded so that 128-bit loads and TMA copies that start inside the table may run past its last row.
 constexpr int64_t kColPad = 8;
 
@@ -3919,8 +3921,11 @@ int evg_prioritize_legacy_batch(evg_ctx* c, const evg_legacy_soa* in, const int6
   if (rc != EVG_OK) return rc;
   int64_t max_n = 0;
   for (int32_t d = 0; d < D; d++) max_n = std::max(max_n, task_off[d + 1] - task_off[d]);
-  for (int64_t k = 0; k < 3 * int64_t(D); k++)
-    if (list_mode[k] > EVG_LEGACY_MODE_LITERAL) return fail(EVG_ERR_INVALID, "unknown list mode %d", int(list_mode[k]));
+  int64_t max_gs = 0;  // the longest distro with a GO_STABLE list: a bound on that list's length
+  for (int64_t k = 0; k < 3 * int64_t(D); k++) {
+    if (list_mode[k] > EVG_LEGACY_MODE_GO_STABLE) return fail(EVG_ERR_INVALID, "unknown list mode %d", int(list_mode[k]));
+    if (list_mode[k] == EVG_LEGACY_MODE_GO_STABLE) max_gs = std::max(max_gs, task_off[k / 3 + 1] - task_off[k / 3]);
+  }
   cudaStream_t s = c->stream;
   c->launches = 0;
   drop_tick(c);
@@ -3951,9 +3956,42 @@ int evg_prioritize_legacy_batch(evg_ctx* c, const evg_legacy_soa* in, const int6
   x.presort = c->b_rn1.as<int32_t>(); x.flags = c->tasks.flags.as<uint32_t>(); x.list_mode = c->b_rn2.as<uint8_t>();
   x.task_off = c->b_taskoff.as<int64_t>(); x.n_distros = D;
   int32_t* buf[2] = {c->b_rn3.as<int32_t>(), c->b_rn4.as<int32_t>()};
+  int gs_err = 0;
+  int* d_gs_err = nullptr;
   if (T > 0) {
+    const unsigned int* counts = c->b_rn5.as<unsigned int>();
     launch(c, c->stream, k_legacy_init, grid_for(T, 256), 256, 0, x, buf[0], c->b_rn5.as<unsigned int>());
-    const int32_t* sorted = seg_merge_sort(c, c->stream, LegacyOrder{x}, x.task_off, D, T, max_n, buf);
+    int32_t* sorted = seg_merge_sort(c, c->stream, LegacyOrder{x}, x.task_off, D, T, max_n, buf);
+    if (max_gs > 1) {  // sort.Stable on the GO_STABLE lists, now in presort order; the other buffer is the rotations' scratch
+      int32_t* scratch = sorted == buf[0] ? buf[1] : buf[0];
+      const auto waves_of = [](int64_t size) { return 64 - __builtin_clzll(uint64_t(size - 1)); };  // ceil(log2 size), size >= 2
+      int64_t n_waves = 0;
+      for (int64_t block = 20; block < max_gs; block *= 2) n_waves += waves_of(std::min(2 * block, max_gs));
+      // [n_waves + 1] task counts, the error flag, then two task queues: a wave's calls own disjoint ranges of >= 2 tasks
+      const int64_t cap = T / 2 + 1, head = (sizeof(unsigned int) * (n_waves + 2) + 15) / 16 * 16;
+      CK(c->b_rn7.ensure(size_t(head) + 2 * sizeof(GsTask) * size_t(cap)));
+      CK(cudaMemsetAsync(c->b_rn7.p, 0, size_t(head), s));
+      unsigned int* n_tasks = c->b_rn7.as<unsigned int>();
+      d_gs_err = reinterpret_cast<int*>(n_tasks + n_waves + 1);
+      GsTask* queue[2] = {reinterpret_cast<GsTask*>(c->b_rn7.as<char>() + head), reinterpret_cast<GsTask*>(c->b_rn7.as<char>() + head) + cap};
+      const unsigned int grid_cta = unsigned(std::min<int64_t>(cap, int64_t(c->num_sms) * 8)), grid_warp = unsigned(std::min<int64_t>((cap + 7) / 8, int64_t(c->num_sms) * 8));
+      launch(c, s, k_gs_insertion, grid_for(T, 256), 256, 0, x, counts, sorted);
+      int64_t w = 0;
+      for (int64_t block = 20; block < max_gs; block *= 2) {
+        const int64_t size = std::min(2 * block, max_gs), level_waves = waves_of(size);
+        launch(c, s, k_gs_seed, grid_for(T, 256), 256, 0, x, counts, block, queue[w & 1], n_tasks + w);
+        for (int64_t k = 0; k < level_waves; k++, w++) {
+          const bool last = k == level_waves - 1;
+          GsTask* out = last ? nullptr : queue[(w + 1) & 1];
+          unsigned int* out_n = last ? nullptr : n_tasks + w + 1;
+          if (((size - 1) >> k) + 1 > kGsWarpRotation)  // the wave's largest call: a CTA rotates it
+            launch(c, s, k_gs_wave<256>, grid_cta, 256, 0, x, sorted, scratch, queue[w & 1], n_tasks + w, out, out_n, d_gs_err);
+          else
+            launch(c, s, k_gs_wave<32>, grid_warp, 256, 0, x, sorted, scratch, queue[w & 1], n_tasks + w, out, out_n, d_gs_err);
+        }
+      }
+      CK(cudaMemcpyAsync(&gs_err, d_gs_err, sizeof(int), cudaMemcpyDeviceToHost, s));
+    }
     launch(c, c->stream, k_legacy_interleave, grid_for(T, 256), 256, 0, x, sorted, c->b_rn5.as<unsigned int>(), c->b_order.as<int32_t>(),
            c->b_rn6.as<int64_t>(), c->b_status.as<int32_t>());
     CK(cudaGetLastError());
@@ -3967,6 +4005,7 @@ int evg_prioritize_legacy_batch(evg_ctx* c, const evg_legacy_soa* in, const int6
     CK(cudaMemcpyAsync(st.data(), c->b_status.p, sizeof(int32_t) * size_t(D), cudaMemcpyDeviceToHost, s));
   }
   CK(cudaStreamSynchronize(s));
+  if (gs_err) return fail(EVG_ERR_CUDA, "%s: a symMerge call outlived its level's wave bound", who);
   for (int32_t d = 0; d < D; d++) {
     const bool empty = task_off[d + 1] == task_off[d];
     count[d] = empty ? 0 : cnt[d];

@@ -1374,8 +1374,10 @@ def plan_and_allocate(batch: Sequence[Tuple[M.Distro, List[M.Task], M.HostAlloca
 # ---------------------------------------------------------------------------------------------------------------
 class NotDecomposableError(Exception):
     """The legacy comparator chain is not a strict weak order on some list of the distro (commit builds of several
-    projects in one list, zero and non-zero expected durations mixed): the reference's result then depends on the exact
-    steps of Go's sort.Stable, which this library does not reproduce.  The order it did compute is attached."""
+    projects in one list, zero and non-zero expected durations mixed, two task groups whose "BuildId-TaskGroup"
+    strings are equal): the reference's result then depends on the exact steps of Go's sort.Stable, which the default
+    prioritiser does not reproduce.  The order it did compute is attached.  CmpBasedTaskPrioritizer(exact=True)
+    replays sort.Stable on such lists and never raises this."""
 
     def __init__(self, distro_id: str, tasks):
         super().__init__(f"distro {distro_id!r}: the comparator chain is not a strict weak order on this queue")
@@ -1385,17 +1387,21 @@ class NotDecomposableError(Exception):
 class CmpBasedTaskPrioritizer:
     """scheduler.TaskPrioritizer (scheduler/task_prioritizer.go:20-25) implemented by the legacy comparator
     prioritiser on the GPU.  PrioritizeTasks returns (tasks in run order, orderingLogic, error) like the reference;
-    orderingLogic -- the reference's map of per-comparison reason strings -- is always empty here."""
+    orderingLogic -- the reference's map of per-comparison reason strings -- is always empty here.
+    exact=True: lists on which the chain is not a strict weak order are sorted by a replay of Go's sort.Stable
+    (EVG_LEGACY_MODE_GO_STABLE), so every queue gets the reference's order and PrioritizeTasks never returns
+    NotDecomposableError."""
 
-    def __init__(self, runtime_id: str = "", engine: Optional[Engine] = None, now: Optional[int] = None):
+    def __init__(self, runtime_id: str = "", engine: Optional[Engine] = None, now: Optional[int] = None, exact: bool = False):
         self.runtime_id = runtime_id
         self.engine = engine
         self.now = now
+        self.exact = exact
 
     def prioritize_batch(self, batch):
         """(distro_id, tasks, versions) per distro -> list of (sorted tasks, status)."""
         eng = self.engine or default_engine()
-        table = S.marshal_legacy(batch, self.now)
+        table = S.marshal_legacy(batch, self.now, exact=self.exact)
         order, count, status = eng.prioritize_legacy_batch(table)
         out = []
         for d, (_, tasks, _) in enumerate(batch):

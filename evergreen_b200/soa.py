@@ -1349,9 +1349,12 @@ def legacy_list_mode(tasks: Sequence[M.Task], expected: Sequence[int]) -> int:
     return L.EVG_LEGACY_MODE_LITERAL
 
 
-def marshal_legacy(batch: Sequence[tuple], now: Optional[int] = None) -> LegacyTable:
+def marshal_legacy(batch: Sequence[tuple], now: Optional[int] = None, exact: bool = False) -> LegacyTable:
     """batch: (distro_id, tasks, versions) per distro; `versions` maps a version id to its Requester (what byCommitQueue
-    reads of model.Version).  Resolves FetchExpectedDuration, interns the strings, decides each list's mode."""
+    reads of model.Version).  Resolves FetchExpectedDuration, interns the strings, decides each list's mode.
+    exact=True marks a list that would be EVG_LEGACY_MODE_LITERAL (a format collision included) GO_STABLE instead, so
+    the device replays Go's sort.Stable on it; INGEST and REVISION lists keep their key sort, which gives the same order
+    for less."""
     cols = {name: [] for name, _ in LegacyTable.COLUMNS}
     task_off, modes = [0], []
     for _, tasks, versions in batch:
@@ -1390,7 +1393,8 @@ def marshal_legacy(batch: Sequence[tuple], now: Optional[int] = None) -> LegacyT
         for lst in (0, 1, 2):
             sel = [k for k in range(len(tasks)) if lists[k] == lst]
             m = legacy_list_mode([tasks[k] for k in sel], [expected[k] for k in sel])
-            modes.append(L.EVG_LEGACY_MODE_LITERAL if collision else m)
+            m = L.EVG_LEGACY_MODE_LITERAL if collision else m
+            modes.append(L.EVG_LEGACY_MODE_GO_STABLE if exact and m == L.EVG_LEGACY_MODE_LITERAL else m)
         task_off.append(task_off[-1] + len(tasks))
     return LegacyTable(**{name: np.array(cols[name], dtype=dt) for name, dt in LegacyTable.COLUMNS},
                        task_off=np.array(task_off, dtype=np.int64), list_mode=np.array(modes, dtype=np.uint8))

@@ -792,11 +792,16 @@ int evg_download_durations(evg_ctx* ctx, evg_duration_out* tasks, evg_duration_o
 #define EVG_LEGACY_MODE_REVISION 1  /* every non-group task is a commit build of ONE project: RevisionOrderNumber descending */
 #define EVG_LEGACY_MODE_LITERAL 2   /* neither (or zero and non-zero expected durations mixed, or two (TaskGroup, BuildId)
                                        pairs format to one string): the chain is not a strict weak order on this list */
+#define EVG_LEGACY_MODE_GO_STABLE 3 /* any list: sorted exactly as Go's sort.Stable sorts it -- from the groupTaskGroups
+                                       presort, with the literal first-definitive chain, the same insertion sorts of
+                                       20-blocks, symMerge probes and rotations -- so the result is the reference's order on
+                                       any input.  Costs more than INGEST / REVISION, which give the same order where they apply */
 /* per-distro status */
 #define EVG_LEGACY_OK 0
 #define EVG_LEGACY_NOT_DECOMPOSABLE 1 /* some list was EVG_LEGACY_MODE_LITERAL: no order is common to all stable sorts there;
                                          the list was sorted by the nearest transitive key (byAge by IngestTime only),
-                                         which need not be the order Go's sort.Stable produces */
+                                         which need not be the order Go's sort.Stable produces.  A distro whose lists
+                                         are all INGEST, REVISION or GO_STABLE is EVG_LEGACY_OK */
 
 /* What CmpBasedTaskPrioritizer reads of []task.Task and map[string]model.Version, SoA over the concatenated distros
  * (scheduler/task_prioritizer.go:80-278, task_priority_cmp.go:25-208, setup_funcs.go:72-87).  Strings are interned
