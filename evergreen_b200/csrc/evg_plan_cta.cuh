@@ -517,20 +517,7 @@ k_plan_cta(DTasks T, DDistros D, DWork W, const int32_t* __restrict__ list, int6
       loc[k] = w & 0xFFFFu; loc[k + 1] = w >> 16;
       sum += loc[k] + loc[k + 1];
     }
-    uint32_t inc = sum;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const uint32_t x = __shfl_up_sync(full, inc, o); if (lane >= o) inc += x; }
-    if (lane == 31) sScan[warp] = inc;
-    __syncthreads();
-    if (warp == 0) {
-      const uint32_t w = lane < NW ? sScan[lane] : 0u;
-      uint32_t winc = w;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { const uint32_t x = __shfl_up_sync(full, winc, o); if (lane >= o) winc += x; }
-      if (lane < NW) sScan[lane] = winc - w;
-    }
-    __syncthreads();
-    uint32_t run = sScan[warp] + inc - sum;
+    uint32_t run = block_scan_excl<NW>(sum, sScan);
 #pragma unroll
     for (int k = 0; k < ITEMS; k += 2) {
       const int j = j0 + k;
@@ -634,21 +621,7 @@ k_plan_cta(DTasks T, DDistros D, DWork W, const int32_t* __restrict__ list, int6
           for (int w = 0; w < NW; w++) tot += sCnt[w * DW + tid];  // packed halves never carry: totals <= CAP
         }
         const uint32_t t0 = tot & 0xFFFFu, t1 = tot >> 16;
-        const uint32_t sum = t0 + t1;
-        uint32_t inc = sum;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(full, inc, o); if (lane >= o) inc += y; }
-        if (lane == 31) sScan[warp] = inc;
-        __syncthreads();
-        if (warp == 0) {
-          const uint32_t w = lane < NW ? sScan[lane] : 0u;
-          uint32_t winc = w;
-#pragma unroll
-          for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(full, winc, o); if (lane >= o) winc += y; }
-          if (lane < NW) sScan[lane] = winc - w;
-        }
-        __syncthreads();
-        const uint32_t ex = sScan[warp] + inc - sum;
+        const uint32_t ex = block_scan_excl<NW>(t0 + t1, sScan);
         uint32_t run = ex | ((ex + t0) << 16);
         if (act) {
 #pragma unroll

@@ -312,19 +312,12 @@ __global__ void __launch_bounds__(256, kGTaskOcc) k_gtask(DTasks T, DDistros D, 
     if (dcomplex) {  // block-uniform
       __shared__ uint32_t s_wsum[8];
       __shared__ uint32_t s_lbase;
-      const uint32_t mine = __popc(cmask);
-      uint32_t inc = mine;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { const uint32_t x = __shfl_up_sync(full, inc, o); if (lane >= o) inc += x; }
-      if (lane == 31) s_wsum[tid >> 5] = inc;
-      __syncthreads();
-      uint32_t before = 0, total = 0;
-#pragma unroll
-      for (int w = 0; w < 8; w++) { const uint32_t x = s_wsum[w]; before += w < (tid >> 5) ? x : 0u; total += x; }
+      uint32_t total;
+      const uint32_t before = block_scan_excl<8>(uint32_t(__popc(cmask)), s_wsum, &total);
       if (total) {  // block-uniform
         if (tid == 0) s_lbase = atomicAdd(G.ccount, total);
         __syncthreads();
-        uint32_t pos = s_lbase + before + inc - mine;
+        uint32_t pos = s_lbase + before;
         const int32_t vid_[4] = {vid4.x, vid4.y, vid4.z, vid4.w}, tgo_[4] = {tgo4.x, tgo4.y, tgo4.z, tgo4.w};
 #pragma unroll
         for (int m = 0; m < 4; m++) {
@@ -498,10 +491,9 @@ __global__ void __launch_bounds__(256, kUnitTableOcc) k_glink(DTasks T, DDistros
 // block and trip (an atomic per unit serialises ~10^5 units of a tick on one L2 address).
 __global__ void __launch_bounds__(256, kUnitTableOcc) k_galloc(DTasks T, DDistros D, DWork W, DGen G) {
   if (*W.err) return;
-  __shared__ uint32_t s_wsum[8], s_wcnt[8];
+  __shared__ uint64_t s_wsum[8];
   __shared__ uint32_t s_base, s_hbase;
   const unsigned int n = *G.ccount;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   for (unsigned int k0 = blockIdx.x * blockDim.x; k0 < n; k0 += gridDim.x * blockDim.x) {  // block-uniform trip count
     const unsigned int k = k0 + threadIdx.x;
     WlTask x;
@@ -510,24 +502,15 @@ __global__ void __launch_bounds__(256, kUnitTableOcc) k_galloc(DTasks T, DDistro
       x = wl_task(D, G, k);
       wl_pairs(T, G, x, k, [&](const uint32_t* place, uint32_t slot, bool) { if (*place == 0u) { need += W.unit_n[slot]; heads++; } });
     }
-    uint32_t inc = need, hinc = heads;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const uint32_t y = __shfl_up_sync(0xffffffffu, inc, o), z = __shfl_up_sync(0xffffffffu, hinc, o);
-      if (lane >= o) { inc += y; hinc += z; }
-    }
-    if (lane == 31) { s_wsum[warp] = inc; s_wcnt[warp] = hinc; }
-    __syncthreads();
-    uint32_t before = 0, total = 0, hbefore = 0, htotal = 0;
-#pragma unroll
-    for (int w = 0; w < 8; w++) {
-      const uint32_t y = s_wsum[w], z = s_wcnt[w];
-      before += w < warp ? y : 0u; total += y; hbefore += w < warp ? z : 0u; htotal += z;
-    }
+    // both counts in one scan, records in the low half: they never carry into the units, as the tick's record total
+    // is below 2^32 (upload_tasks)
+    uint64_t both;
+    const uint64_t ex = block_scan_excl<8>(uint64_t(need) | (uint64_t(heads) << 32), s_wsum, &both);
+    const uint32_t total = uint32_t(both), htotal = uint32_t(both >> 32);
     if (threadIdx.x == 0 && htotal) { s_base = atomicAdd(G.rcount, total); s_hbase = atomicAdd(G.hcount, htotal); }
     __syncthreads();
     if (heads) {
-      uint32_t pos = s_base + before + inc - need, hp = s_hbase + hbefore + hinc - heads;
+      uint32_t pos = s_base + uint32_t(ex), hp = s_hbase + uint32_t(ex >> 32);
       wl_pairs(T, G, x, k, [&](const uint32_t* place, uint32_t slot, bool) {
         if (*place != 0u) return;
         GUnit u;
@@ -767,34 +750,8 @@ __global__ void __launch_bounds__(256) k_gsum(DDistros D, DGen G) {
 // exclusive scan of the tile sums of one distro (<= 1025 tiles), one block per general-path distro
 __global__ void __launch_bounds__(1024) k_gscan(DGen G, const int32_t* __restrict__ general_list) {
   const int d = general_list[blockIdx.x];
-  const int64_t t0 = G.dtile_off[d], nt = G.dtile_off[d + 1] - t0;
-  __shared__ uint32_t sw[32];
-  __shared__ uint32_t carry;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (threadIdx.x == 0) carry = 0;
-  __syncthreads();
-  for (int64_t c0 = 0; c0 < nt; c0 += 1024) {
-    const int64_t i = c0 + threadIdx.x;
-    const uint32_t v = i < nt ? G.tile_sum[t0 + i] : 0u;
-    uint32_t inc = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const uint32_t x = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += x; }
-    if (lane == 31) sw[warp] = inc;
-    __syncthreads();
-    if (warp == 0) {
-      const uint32_t w = sw[lane];
-      uint32_t winc = w;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { const uint32_t x = __shfl_up_sync(0xffffffffu, winc, o); if (lane >= o) winc += x; }
-      sw[lane] = winc - w;
-    }
-    __syncthreads();
-    const uint32_t ex = carry + sw[warp] + inc - v;
-    if (i < nt) G.tile_sum[t0 + i] = ex;
-    __syncthreads();
-    if (threadIdx.x == 1023) carry = ex + v;
-    __syncthreads();
-  }
+  const int64_t t0 = G.dtile_off[d];
+  block_scan_segment(G.tile_sum + t0, G.dtile_off[d + 1] - t0);
 }
 
 __device__ __forceinline__ void gen_put_key(const DGen& G, int64_t base, uint32_t pos, unsigned long long key, bool wide, uint32_t li) {
@@ -817,7 +774,7 @@ __global__ void __launch_bounds__(256) k_gplace(DDistros D, DWork W, DGen G, int
   const int64_t ts = G.tile_start[tile];
   const unsigned long long vmax_ord = G.vmm[2 * d];
   const bool wide = gen_bits(G, d) > 32;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const int64_t t8 = ts + 8 * int64_t(tid);  // multiple of 4
   const bool interior = t8 >= base && t8 + 7 < end;  // the common case: 128-bit loads
   uint32_t ev[8];
@@ -836,15 +793,7 @@ __global__ void __launch_bounds__(256) k_gplace(DDistros D, DWork W, DGen G, int
   uint32_t run = 0;
   if (use_e) {
     __shared__ uint32_t sw[8];
-    uint32_t inc = sum;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const uint32_t x = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += x; }
-    if (lane == 31) sw[warp] = inc;
-    __syncthreads();
-    uint32_t before = 0;
-#pragma unroll
-    for (int w = 0; w < 8; w++) if (w < warp) before += sw[w];
-    run = G.tile_sum[tile] + before + inc - sum;
+    run = G.tile_sum[tile] + block_scan_excl<8>(sum, sw);
   }
   int64_t vv[8];
   uint32_t dsp = 0;  // bit m: task t8+m is emitted from a multi-member unit (placed by k_gplace_unit)
@@ -1040,16 +989,13 @@ __global__ void __launch_bounds__(1024) k_gdscan(int j, const int32_t* __restric
   part[grp][dg] = sum;
   __syncthreads();
   const uint32_t total = part[0][dg] + part[1][dg] + part[2][dg] + part[3][dg];
-  if (grp == 0) s[dg] = total;
+  // group 0 (threads 0 .. 255, one per digit) holds the digit totals, so their block scan is the scan over the digits;
+  // s passes it to the other groups
+  const uint32_t before = block_scan_excl<32>(grp == 0 ? total : 0u, s);
   __syncthreads();
-  for (int o = 1; o < 256; o <<= 1) {
-    uint32_t v = 0;
-    if (grp == 0 && dg >= o) v = s[dg - o];
-    __syncthreads();
-    if (grp == 0) s[dg] += v;
-    __syncthreads();
-  }
-  uint32_t run = s[dg] - total;
+  if (grp == 0) s[dg] = before;
+  __syncthreads();
+  uint32_t run = s[dg];
   for (int g = 0; g < grp; g++) run += part[g][dg];
   tile = a;
   for (; tile + 8 <= b; tile += 8) {
@@ -1114,15 +1060,7 @@ __device__ __forceinline__ void gscatter_tile(int j, const DGen& G, int tile, in
     uint32_t x[8], tot = 0;
 #pragma unroll
     for (int w = 0; w < 8; w++) { x[w] = wcnt[w][tid]; tot += x[w]; }
-    uint32_t inc = tot;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += y; }
-    if (lane == 31) s_wsum[warp] = inc;
-    __syncthreads();
-    uint32_t before = 0;
-#pragma unroll
-    for (int w = 0; w < 8; w++) before += w < warp ? s_wsum[w] : 0u;
-    const uint32_t lbase = before + inc - tot;  // where digit `tid` starts in the sorted tile
+    const uint32_t lbase = block_scan_excl<8>(tot, s_wsum);  // where digit `tid` starts in the sorted tile
     s_delta[tid] = int32_t(G.tile_hist[int64_t(tile) * 256 + tid]) - int32_t(lbase);
     uint32_t run = lbase;
 #pragma unroll

@@ -580,19 +580,7 @@ k_plan_smem(DTasks T, DDistros D, DWork W, const int32_t* __restrict__ list, con
     uint32_t sum = 0;
 #pragma unroll
     for (int k = 0; k < ITEMS; k++) { loc[k] = sE[tid * ITEMS + k]; sum += loc[k]; }
-    uint32_t inc = sum;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { uint32_t v = __shfl_up_sync(full, inc, o); if (lane >= o) inc += v; }
-    if (lane == 31) sScan[warp] = inc;
-    __syncthreads();
-    if (warp == 0) {
-      uint32_t w = lane < NW ? sScan[lane] : 0, winc = w;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { uint32_t v = __shfl_up_sync(full, winc, o); if (lane >= o) winc += v; }
-      if (lane < NW) sScan[lane] = winc - w;
-    }
-    __syncthreads();
-    uint32_t run = sScan[warp] + inc - sum;
+    uint32_t run = block_scan_excl<NW>(sum, sScan);
 #pragma unroll
     for (int k = 0; k < ITEMS; k++) { sE[tid * ITEMS + k] = uint16_t(run); run += loc[k]; }
     __syncthreads();
@@ -708,10 +696,7 @@ k_plan_smem(DTasks T, DDistros D, DWork W, const int32_t* __restrict__ list, con
         v[k] = tot;
         sum += tot;
       }
-      uint32_t inc = sum;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { uint32_t x = __shfl_up_sync(full, inc, o); if (lane >= o) inc += x; }
-      uint32_t run = inc - sum;
+      uint32_t run = warp_scan_incl(sum) - sum;
 #pragma unroll
       for (int k = 0; k < 8; k++) { sTot[lane * 8 + k] = run; run += v[k]; }
     }

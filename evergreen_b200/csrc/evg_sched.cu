@@ -300,6 +300,69 @@ __device__ __forceinline__ int64_t warp_sum64(int64_t v) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
+
+// Inclusive prefix sum of v over the lanes of a full warp (T: uint32_t, int64_t or uint64_t).
+template <class T>
+__device__ __forceinline__ T warp_scan_incl(T v) {
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const T y = __shfl_up_sync(0xffffffffu, v, o);
+    if (lane >= o) v += y;
+  }
+  return v;
+}
+
+__device__ __forceinline__ uint32_t warp_add(uint32_t v) { return __reduce_add_sync(0xffffffffu, v); }
+__device__ __forceinline__ uint64_t warp_add(uint64_t v) { return uint64_t(warp_sum64(int64_t(v))); }
+
+// Exclusive prefix sum of v over a block of NW full warps, and the block's total in *total when asked.  Every thread of
+// the block calls it.  s_warp is NW entries of shared memory the caller owns: the helper writes it before its first
+// barrier and reads it after its last, so a __syncthreads() must separate this call from any earlier read of s_warp
+// and from any later write to it (another scan included).  Up to 8 warps one barrier suffices: lane w reads warp w's
+// total and each warp adds up those of the warps before it (one load a thread, where reading all NW in turn costs the
+// on-chip planners spills); above that warp 0 scans the totals and a second barrier publishes them.
+template <int NW, class T>
+__device__ __forceinline__ T block_scan_excl(T v, T* s_warp, T* total = nullptr) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const T inc = warp_scan_incl(v);
+  if (lane == 31) s_warp[warp] = inc;
+  __syncthreads();
+  T before = 0;
+  if constexpr (NW <= 8) {
+    const T x = lane < NW ? s_warp[lane] : T(0);
+    before = warp_add(lane < warp ? x : T(0));
+    if (total) *total = warp_add(x);
+  } else {
+    if (warp == 0) {  // s_warp[w] becomes the total of warps 0 .. w
+      const T x = warp_scan_incl(lane < NW ? s_warp[lane] : T(0));
+      if (lane < NW) s_warp[lane] = x;
+    }
+    __syncthreads();
+    if (warp > 0) before = s_warp[warp - 1];
+    if (total) *total = s_warp[NW - 1];
+  }
+  return before + inc - v;
+}
+
+// One block of 1024 threads scans a[0 .. n) in place (exclusive), 1024 entries at a time with a carry, and returns the
+// total.
+template <class T>
+__device__ T block_scan_segment(T* a, int64_t n) {
+  __shared__ T s_warp[32];
+  T carry = 0;
+  for (int64_t c0 = 0; c0 < n; c0 += 1024) {
+    const int64_t i = c0 + threadIdx.x;
+    const T v = i < n ? a[i] : T(0);
+    T chunk;
+    const T ex = block_scan_excl<32>(v, s_warp, &chunk);
+    if (i < n) a[i] = carry + ex;
+    carry += chunk;
+    __syncthreads();  // s_warp is rewritten by the next chunk
+  }
+  return carry;
+}
+
 __device__ __forceinline__ void atomic_add64(int64_t* p, int64_t v) {
   if (v != 0) atomicAdd(reinterpret_cast<unsigned long long*>(p), (unsigned long long)v);
 }
@@ -1332,7 +1395,7 @@ struct evg_ctx {
   } pf;
   struct {  // the pipeline finder's tables (the first evg_find_runnable_ex / evg_plan_from_finder_ex with a pipeline allocates them)
     DevBuf dep_status, task_status, ext_status, task_unatt, ext_unatt, project_raw;  // an evg_pipeline_in, staged
-    DevBuf edge_cnt, dep_off, dep_idx, scan_sum;  // the candidates' edges without those of EVG_FINDER_PIPELINE rows
+    DevBuf edge_cnt, dep_off, dep_idx;  // the candidates' edges without those of EVG_FINDER_PIPELINE rows
   } pl;
   struct {  // compose_tick's buffers (the first evg_edit_tasks or evg_plan_from_finder allocates them) and the staged edit
     TaskCols out;            // the shadow set: the composed table is written here, then swapped with the resident columns
@@ -1340,7 +1403,7 @@ struct evg_ctx {
     TaskCols ins;            // the inserted rows, staged
     DevBuf ins_dep_off, ins_dep_idx, rm, add_task, add_dep, gremap, vremap;
     DevBuf new_off, old_off, old_goff, ins_off, old_vbase, edge_at;  // D+1 tables
-    DevBuf keep, pos, src, scan_sum, edge_cnt, err;
+    DevBuf keep, pos, src, edge_cnt, err;
   } ed;
   // evg_plan_aliases (the first call allocates these): the staged source table, the (queue, task) pairs and the alias
   // map evg_download_alias_map returns while tick.aliases holds
@@ -1362,7 +1425,7 @@ struct evg_ctx {
   // evg_rebuild_dispatchers (the first call allocates these): the persisted queues' DAG input gathered from the tick,
   // and the scratch and results of the k_dag_* kernels, so that the resident tick is only read
   struct {
-    DevBuf item_off, rank_of, row, first, gslot_of, gindex, cnt, dep_off, dep_item, pos, group_off, group_slot, group_id, scan_sum;
+    DevBuf item_off, rank_of, row, first, gslot_of, gindex, cnt, dep_off, dep_item, pos, group_off, group_slot, group_id;
     DevBuf succ_off, succ, index, low, stack, cs_node, cs_pos, emit, on_stack, sorted, stats, buf[2], unit_off;
   } dp;
   // evg_host_job (the first call allocates these): the staged job settings and spawned counts, and the outputs
@@ -1379,12 +1442,13 @@ struct evg_ctx {
   } nx;
   // evg_host_drawdown / evg_idle_hosts (the first call allocates these): the staged idle-host table, its offsets and the
   // per-distro inputs, the verdicts, the decided flags and their scan, and the per-distro outputs
-  struct { DevBuf cols, off, din, verdict, flag, pos, scan_sum, dout; } ih;
+  struct { DevBuf cols, off, din, verdict, flag, pos, dout; } ih;
   // evg_estimate_start_times / evg_estimate_start_batch (the first call allocates these): the staged host table, each
   // row's timeToCompletion and whether it counts, their scan, the packed pools (two copies: the merge sort's), the
   // queues' offsets and durations, the launch list and the outputs
-  struct { DevBuf kind, expected, dispatch, host_off, ttc, used, pos, scan_sum, pool[2], pool_off, item_off, dur, list, start, hosts_used; } es;
+  struct { DevBuf kind, expected, dispatch, host_off, ttc, used, pos, pool[2], pool_off, item_off, dur, list, start, hosts_used; } es;
   DevBuf b_err;
+  DevBuf b_scansum;  // scan_counts' per-block sums
   DevBuf b_route, b_unitv, b_unita, b_unitn, b_unitmask;
   DevBuf b_punt, b_puntcnt;
   // The distros of each size class: ascending ids on the host and the device (the pipelined call cuts them by distro
@@ -2906,53 +2970,14 @@ int evg_find_runnable_ex(evg_ctx* c, const evg_runnable_in* in, const evg_pipeli
 __global__ void __launch_bounds__(1024) k_scan_blocks(const int32_t* __restrict__ in, int64_t n, int64_t* __restrict__ out, int64_t* __restrict__ block_sum) {
   __shared__ int64_t sw[32];
   const int64_t i = int64_t(blockIdx.x) * 1024 + threadIdx.x;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int64_t v = i < n ? in[i] : 0;
-  int64_t inc = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) { const int64_t y = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += y; }
-  if (lane == 31) sw[warp] = inc;
-  __syncthreads();
-  if (warp == 0) {
-    const int64_t w = sw[lane];
-    int64_t winc = w;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const int64_t y = __shfl_up_sync(0xffffffffu, winc, o); if (lane >= o) winc += y; }
-    sw[lane] = winc - w;
-    if (lane == 31) block_sum[blockIdx.x] = winc;
-  }
-  __syncthreads();
-  if (i < n) out[i] = sw[warp] + inc - v;
+  int64_t total;
+  const int64_t ex = block_scan_excl<32>(i < n ? int64_t(in[i]) : int64_t(0), sw, &total);
+  if (i < n) out[i] = ex;
+  if (threadIdx.x == 0) block_sum[blockIdx.x] = total;
 }
 __global__ void __launch_bounds__(1024) k_scan_sums(int64_t* __restrict__ block_sum, int64_t nb) {  // one block
-  __shared__ int64_t sw[32];
-  __shared__ int64_t carry;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (threadIdx.x == 0) carry = 0;
-  __syncthreads();
-  for (int64_t c0 = 0; c0 < nb; c0 += 1024) {
-    const int64_t i = c0 + threadIdx.x;
-    const int64_t v = i < nb ? block_sum[i] : 0;
-    int64_t inc = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const int64_t y = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += y; }
-    if (lane == 31) sw[warp] = inc;
-    __syncthreads();
-    if (warp == 0) {
-      const int64_t w = sw[lane];
-      int64_t winc = w;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { const int64_t y = __shfl_up_sync(0xffffffffu, winc, o); if (lane >= o) winc += y; }
-      sw[lane] = winc - w;
-    }
-    __syncthreads();
-    const int64_t ex = carry + sw[warp] + inc - v;
-    if (i < nb) block_sum[i] = ex;
-    __syncthreads();
-    if (threadIdx.x == 1023) carry = ex + v;
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) block_sum[nb] = carry;  // the grand total
+  const int64_t total = block_scan_segment(block_sum, nb);
+  if (threadIdx.x == 0) block_sum[nb] = total;  // the grand total
 }
 __global__ void __launch_bounds__(1024) k_scan_add(int64_t* __restrict__ out, int64_t n, const int64_t* __restrict__ block_sum, int64_t nb) {
   const int64_t i = int64_t(blockIdx.x) * 1024 + threadIdx.x;
@@ -3087,12 +3112,17 @@ __global__ void __launch_bounds__(256) k_kept_mask(int64_t n, int32_t D, const i
   if (k >= 0) keep[off[d] + k] = 1;
 }
 
-// Exclusive scan of n int32 counts into out[0 .. n] (int64; out[n] = the total); `sum` holds (n + 1023) / 1024 + 1 int64.
-static void scan_counts(evg_ctx* c, const int32_t* in, int64_t n, int64_t* out, int64_t* sum) {
+// Exclusive scan of n int32 counts into out[0 .. n] (int64; out[n] = the total) on c->stream, the per-block sums in
+// c->b_scansum.
+static cudaError_t scan_counts(evg_ctx* c, const int32_t* in, int64_t n, int64_t* out) {
   const int64_t nb = (n + 1023) / 1024;
+  const cudaError_t e = c->b_scansum.ensure(sizeof(int64_t) * size_t(nb + 1));
+  if (e != cudaSuccess) return e;
+  int64_t* sum = c->b_scansum.as<int64_t>();
   launch(c, c->stream, k_scan_blocks, unsigned(nb), 1024, 0, in, n, out, sum);
   launch(c, c->stream, k_scan_sums, 1, 1024, 0, sum, nb);
   launch(c, c->stream, k_scan_add, unsigned(nb), 1024, 0, out, n, sum, nb);
+  return cudaSuccess;
 }
 
 // The composed table in the shadow set (Tn rows) and in ed.dep_off / ed.dep_idx (En edges; edge_off: dep_off at the
@@ -3119,13 +3149,12 @@ static int compose_tick(evg_ctx* c, const char* who, EdMap m, const DTasks& O, c
   UP(s, e.new_off, distros->task_off, D + 1, int64_t);
   CK(e.pos.ensure(sizeof(int64_t) * size_t(T0 + 1)));
   CK(e.src.ensure(sizeof(int32_t) * size_t(Tn + 1)));
-  CK(e.scan_sum.ensure(sizeof(int64_t) * size_t((std::max(T0, Tn) + 1023) / 1024 + 1)));  // both scans' block sums
   CK(e.err.ensure(sizeof(int)));
   CK(cudaMemsetAsync(e.err.p, 0, sizeof(int), s));
   m.new_off = e.new_off.as<int64_t>(); m.keep = e.keep.as<int32_t>(); m.pos = e.pos.as<int64_t>(); m.src = e.src.as<int32_t>();
   // ---- 1. survivors: the keep mask's scan (each survivor's place), composed row -> source row
   if (T0 > 0) {
-    scan_counts(c, e.keep.as<int32_t>(), T0, e.pos.as<int64_t>(), e.scan_sum.as<int64_t>());
+    CK(scan_counts(c, e.keep.as<int32_t>(), T0, e.pos.as<int64_t>()));
     launch(c, s, k_ed_src, grid_for(T0, 256), 256, 0, T0, m, e.src.as<int32_t>());
   }
   // ---- 2. the nine columns of the composed table into the shadow set, its padding zeroed as an upload leaves it
@@ -3142,7 +3171,7 @@ static int compose_tick(evg_ctx* c, const char* who, EdMap m, const DTasks& O, c
     CK(e.edge_cnt.ensure(sizeof(int32_t) * size_t(Tn + 1)));
     CK(e.dep_off.ensure(sizeof(int64_t) * size_t(Tn + 1 + kColPad)));
     launch(c, s, k_ed_edge_count, grid_for(Tn, 256), 256, 0, Tn, m, O, In, e.edge_cnt.as<int32_t>(), e.err.as<int>());
-    scan_counts(c, e.edge_cnt.as<int32_t>(), Tn, e.dep_off.as<int64_t>(), e.scan_sum.as<int64_t>());
+    CK(scan_counts(c, e.edge_cnt.as<int32_t>(), Tn, e.dep_off.as<int64_t>()));
     CK(e.edge_at.ensure(sizeof(int64_t) * size_t(D + 1)));
     launch(c, s, k_gather_i64, grid_for(D + 1, 256), 256, 0, e.dep_off.as<int64_t>(), e.new_off.as<int64_t>(), e.edge_at.as<int64_t>(), D + 1);
     edge_off.resize(size_t(D) + 1);
@@ -3263,10 +3292,9 @@ static int plan_from_finder(const char* name, evg_ctx* c, const evg_runnable_in*
       auto& p = c->pl;
       CK(p.edge_cnt.ensure(sizeof(int32_t) * size_t(T + 1)));
       CK(p.dep_off.ensure(sizeof(int64_t) * size_t(T + 1)));
-      CK(p.scan_sum.ensure(sizeof(int64_t) * size_t((T + 1023) / 1024 + 1)));
       launch(c, s, k_pl_edge_count, grid_for(T, 256), 256, 0, T, D, pf.task_off.as<int64_t>(), pf.finder.as<uint8_t>(), pf.dep_off.as<int64_t>(),
              p.edge_cnt.as<int32_t>());
-      scan_counts(c, p.edge_cnt.as<int32_t>(), T, p.dep_off.as<int64_t>(), p.scan_sum.as<int64_t>());
+      CK(scan_counts(c, p.edge_cnt.as<int32_t>(), T, p.dep_off.as<int64_t>()));
       // the kept edges fit in the candidates' E: no count has to reach the host
       CK(p.dep_idx.ensure(sizeof(int32_t) * size_t(E)));
       launch(c, s, k_pl_edge_write, grid_for(T, 256), 256, 0, T, pf.dep_off.as<int64_t>(), pf.dep_idx.as<int32_t>(), p.dep_off.as<int64_t>(),
@@ -3684,12 +3712,11 @@ int evg_plan_aliases(evg_ctx* c, const evg_alias_in* in, const evg_distro_cfg* c
   v.soff = a.soff.as<int64_t>(); v.sidx = a.sidx.as<int32_t>(); v.doff = a.doff.as<int64_t>(); v.didx = a.didx.as<int32_t>();
   CK(a.cnt.ensure(sizeof(int32_t) * size_t(T + 1)));
   CK(a.poff.ensure(sizeof(int64_t) * size_t(T + 1)));
-  CK(c->ed.scan_sum.ensure(sizeof(int64_t) * size_t((T + 1023) / 1024 + 1)));
   int64_t P = 0;
   int bad = 0;
   if (T > 0) {
     launch(c, s, k_al_count, grid_for(T, 256), 256, 0, v, S, a.cnt.as<int32_t>(), err);
-    scan_counts(c, a.cnt.as<int32_t>(), T, a.poff.as<int64_t>(), c->ed.scan_sum.as<int64_t>());
+    CK(scan_counts(c, a.cnt.as<int32_t>(), T, a.poff.as<int64_t>()));
     CK(cudaMemcpyAsync(&P, a.poff.as<int64_t>() + T, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
   }
   CK(cudaMemcpyAsync(&bad, err, sizeof(int), cudaMemcpyDeviceToHost, s));
@@ -3711,11 +3738,10 @@ int evg_plan_aliases(evg_ctx* c, const evg_alias_in* in, const evg_distro_cfg* c
     if (bits > 0) {
       CK(a.hist.ensure(sizeof(int32_t) * size_t(nh)));
       CK(a.hoff.ensure(sizeof(int64_t) * size_t(nh + 1)));
-      CK(c->ed.scan_sum.ensure(sizeof(int64_t) * size_t((nh + 1023) / 1024 + 1)));
     }
     for (int shift = 32; shift < 32 + bits; shift += 8, cur ^= 1) {
       launch(c, s, k_al_hist, unsigned(n_tiles), 256, 0, a.keys[cur].as<uint64_t>(), P, shift, a.hist.as<int32_t>(), n_tiles);
-      scan_counts(c, a.hist.as<int32_t>(), nh, a.hoff.as<int64_t>(), c->ed.scan_sum.as<int64_t>());
+      CK(scan_counts(c, a.hist.as<int32_t>(), nh, a.hoff.as<int64_t>()));
       launch(c, s, k_al_scatter, unsigned(n_tiles), 256, 0, a.keys[cur].as<uint64_t>(), a.keys[cur ^ 1].as<uint64_t>(), P, shift,
              a.hoff.as<int64_t>(), n_tiles);
     }
@@ -3740,9 +3766,8 @@ int evg_plan_aliases(evg_ctx* c, const evg_alias_in* in, const evg_distro_cfg* c
            a.vslot.as<int64_t>());
     launch(c, s, k_al_flag, grid_for(P, 256), 256, 0, P, a.gslot.as<int64_t>(), a.vslot.as<int64_t>(), a.hv.as<uint32_t>(), a.fg.as<int32_t>(),
            a.fv.as<int32_t>());
-    CK(c->ed.scan_sum.ensure(sizeof(int64_t) * size_t((P + 1023) / 1024 + 1)));
-    scan_counts(c, a.fg.as<int32_t>(), P, a.pg.as<int64_t>(), c->ed.scan_sum.as<int64_t>());
-    scan_counts(c, a.fv.as<int32_t>(), P, a.pv.as<int64_t>(), c->ed.scan_sum.as<int64_t>());
+    CK(scan_counts(c, a.fg.as<int32_t>(), P, a.pg.as<int64_t>()));
+    CK(scan_counts(c, a.fv.as<int32_t>(), P, a.pv.as<int64_t>()));
   }
   // 5. the nine columns into the shadow set, its padding zeroed as an upload leaves it
   auto& e = c->ed;
@@ -3763,7 +3788,7 @@ int evg_plan_aliases(evg_ctx* c, const evg_alias_in* in, const evg_distro_cfg* c
     CK(e.edge_cnt.ensure(sizeof(int32_t) * size_t(P + 1)));
     CK(e.dep_off.ensure(sizeof(int64_t) * size_t(P + 1 + kColPad)));
     launch(c, s, k_al_edge_count, grid_for(P, 256), 256, 0, P, keys, a.qoff.as<int64_t>(), S, e.edge_cnt.as<int32_t>(), err);
-    scan_counts(c, e.edge_cnt.as<int32_t>(), P, e.dep_off.as<int64_t>(), c->ed.scan_sum.as<int64_t>());
+    CK(scan_counts(c, e.edge_cnt.as<int32_t>(), P, e.dep_off.as<int64_t>()));
     launch(c, s, k_gather_i64, grid_for(D + 1, 256), 256, 0, e.dep_off.as<int64_t>(), a.qoff.as<int64_t>(), samp + 2 * (D + 1), D + 1);
   }
   std::vector<int64_t> h(3 * size_t(D + 1), 0);
@@ -4419,7 +4444,6 @@ int evg_rebuild_dispatchers(evg_ctx* c, int32_t cap, int64_t items_capacity, int
   CK(p.on_stack.ensure(size_t(N) + 16));
   CK(p.dep_off.ensure(sizeof(int64_t) * size_t(N + 1)));
   CK(p.pos.ensure(sizeof(int64_t) * size_t(N + 1)));
-  CK(p.scan_sum.ensure(sizeof(int64_t) * size_t((N + 1023) / 1024 + 2)));
   CK(p.dep_item.ensure(sizeof(int32_t) * size_t(E + 1)));  // the persisted items hold at most every resident edge
   CK(p.succ.ensure(sizeof(int32_t) * size_t(E + 1)));
   CK(p.succ_off.ensure(sizeof(int32_t) * size_t(N + D + 1)));
@@ -4437,9 +4461,9 @@ int evg_rebuild_dispatchers(evg_ctx* c, int32_t cap, int64_t items_capacity, int
   X.rank_of = p.rank_of.as<int32_t>(); X.row = p.row.as<int32_t>(); X.first = p.first.as<int32_t>();
   int32_t* cnt = p.cnt.as<int32_t>();
   launch(c, c->stream, k_dp_gather, grid_for(N, 256), 256, 0, X, p.gslot_of.as<int32_t>(), p.gindex.as<int32_t>(), cnt);
-  scan_counts(c, cnt, N, p.dep_off.as<int64_t>(), p.scan_sum.as<int64_t>());
+  CK(scan_counts(c, cnt, N, p.dep_off.as<int64_t>()));
   launch(c, c->stream, k_dp_edges, grid_for(N, 256), 256, 0, X, p.dep_off.as<int64_t>(), p.dep_item.as<int32_t>(), p.gslot_of.as<int32_t>(), cnt);
-  scan_counts(c, cnt, N, p.pos.as<int64_t>(), p.scan_sum.as<int64_t>());
+  CK(scan_counts(c, cnt, N, p.pos.as<int64_t>()));
   launch(c, c->stream, k_dp_groups, grid_for(std::max<int64_t>(N, D + 1), 256), 256, 0, X, p.pos.as<int64_t>(), p.gslot_of.as<int32_t>(),
          p.group_id.as<int32_t>(), p.group_slot.as<int32_t>(), p.group_off.as<int64_t>());
   CK(cudaGetLastError());
@@ -4792,7 +4816,6 @@ static int stage_idle_hosts(evg_ctx* c, const evg_idle_host_soa* t, const int64_
   CK(x.verdict.ensure(sizeof(evg_host_verdict) * size_t(H > 0 ? H : 1)));
   CK(x.flag.ensure(sizeof(int32_t) * size_t(H > 0 ? H : 1)));
   CK(x.pos.ensure(sizeof(int64_t) * size_t(H + 1)));
-  CK(x.scan_sum.ensure(sizeof(int64_t) * size_t((H + 1023) / 1024 + 1)));
   *v = DIdleHosts{dcol[0], dcol[1], dcol[2], dcol[3], dcol[4], dcol[5], dcol[6], dcol[7], flags};
   return EVG_OK;
 }
@@ -4846,7 +4869,7 @@ int evg_host_drawdown(evg_ctx* c, const evg_idle_host_soa* hosts, const int64_t*
   int64_t* pos = H > 0 ? x.pos.as<int64_t>() : nullptr;
   launch(c, c->stream, k_hd_host, grid_for(H, 256), 256, 0, H, D, off, v, src, now_ns, x.verdict.as<evg_host_verdict>(), x.flag.as<int32_t>());
   if (H > 0) {
-    scan_counts(c, x.flag.as<int32_t>(), H, pos, x.scan_sum.as<int64_t>());
+    CK(scan_counts(c, x.flag.as<int32_t>(), H, pos));
     launch(c, c->stream, k_hd_cap, grid_for(H, 256), 256, 0, H, D, off, src, static_cast<const int64_t*>(pos), x.verdict.as<evg_host_verdict>());
   }
   launch(c, c->stream, k_hd_distro, grid_for(D, 256), 256, 0, D, off, src, static_cast<const int64_t*>(pos), x.dout.as<evg_drawdown_distro>());
@@ -4874,7 +4897,7 @@ int evg_idle_hosts(evg_ctx* c, const evg_idle_host_soa* hosts, const int64_t* id
   const evg_idle_cfg* dcfg = x.din.as<evg_idle_cfg>();
   int64_t* pos = H > 0 ? x.pos.as<int64_t>() : nullptr;
   launch(c, c->stream, k_idle_host, grid_for(H, 256), 256, 0, H, D, off, v, dcfg, now_ns, x.verdict.as<evg_host_verdict>(), x.flag.as<int32_t>());
-  if (H > 0) scan_counts(c, x.flag.as<int32_t>(), H, pos, x.scan_sum.as<int64_t>());
+  if (H > 0) CK(scan_counts(c, x.flag.as<int32_t>(), H, pos));
   launch(c, c->stream, k_idle_distro, grid_for(D, 256), 256, 0, D, off, dcfg, static_cast<const int64_t*>(pos), x.dout.as<evg_idle_distro>());
   return finish_idle_hosts(c, H, out->hosts, out->distros, sizeof(evg_idle_distro) * size_t(D));
 }
@@ -4909,12 +4932,11 @@ static int estimate_run(evg_ctx* c, int32_t D, const evg_est_host_soa* h, const 
   for (DevBuf* b : {&x.ttc, &x.pool[0], &x.pool[1]}) CK(b->ensure(sizeof(int64_t) * size_t(H)));
   CK(x.used.ensure(sizeof(int32_t) * size_t(H)));
   CK(x.pos.ensure(sizeof(int64_t) * size_t(H + 1)));
-  CK(x.scan_sum.ensure(sizeof(int64_t) * size_t((H + 1023) / 1024 + 1)));
   CK(x.pool_off.ensure(sizeof(int64_t) * size_t(D + 1)));
   CK(x.hosts_used.ensure(sizeof(int32_t) * size_t(D)));
   launch(c, s, k_es_host, grid_for(H, 256), 256, 0, H, x.kind.as<uint8_t>(), x.expected.as<int64_t>(), x.dispatch.as<int64_t>(), now,
          x.ttc.as<int64_t>(), x.used.as<int32_t>());
-  scan_counts(c, x.used.as<int32_t>(), H, x.pos.as<int64_t>(), x.scan_sum.as<int64_t>());
+  CK(scan_counts(c, x.used.as<int32_t>(), H, x.pos.as<int64_t>()));
   launch(c, s, k_es_compact, grid_for(H, 256), 256, 0, H, x.ttc.as<int64_t>(), x.used.as<int32_t>(), x.pos.as<int64_t>(), x.pool[0].as<int64_t>());
   launch(c, s, k_es_pool_off, grid_for(D + 1, 256), 256, 0, D, x.host_off.as<int64_t>(), x.pos.as<int64_t>(), x.pool_off.as<int64_t>(),
          x.hosts_used.as<int32_t>());
