@@ -1015,7 +1015,10 @@ __device__ int eval_group(const evg_alloc_cfg& c, const evg_group_info& info, in
     if (!c.parent_found) return EVG_ALLOC_ERR_PARENT_MISSING;
     max_hosts = int64_t(c.parent_maximum_hosts) * int64_t(c.pool_max_containers);
   }
-  if (c.future_host_fraction > 1.0) return EVG_ALLOC_ERR_FUTURE_FRACTION;
+  // allocator.go:302-304 rejects a fraction above 1; a NaN or negative one is rejected too, so that every soon-to-be-free
+  // term lies in [0, 1] or is NaN (threshold 0, whose floor is 0 by DESIGN.md §3 (iv)) and free_hosts fits its int32
+  // field (evg_sched.h)
+  if (!(c.future_host_fraction >= 0.0 && c.future_host_fraction <= 1.0)) return EVG_ALLOC_ERR_FUTURE_FRACTION;
   const int64_t exp_free = n_free + d2i_floor(soon);  // allocator.go:317
   const int64_t overdue = c.waits_over_thresh_feedback ? info.count_wait_over_threshold : 0;
   const int64_t short_ns = wsub(info.expected_duration, info.duration_over_threshold);
@@ -1169,6 +1172,9 @@ __global__ void __launch_bounds__(128, TPD == 32 ? 6 : 4) k_alloc(DHosts H, int3
     } else {
       n_new = 0;  // (0, len(freeHosts), err) allocator.go:99-101
       n_free_out = n_free_all;
+      // the reference stops at the first failing group of a randomised map walk: which groups it had written is not
+      // defined, so an error leaves every group of the distro at 0 (evg_sched.h)
+      for (int64_t g = g0 + tt; g < g1; g += TPD) { ginfo[g].count_free = 0; ginfo[g].count_required = 0; }
     }
   }
   if (tt == 0) {

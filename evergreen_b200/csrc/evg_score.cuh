@@ -69,18 +69,27 @@ EVG_HD int64_t d2i_trunc(double x) {  // Go int64(x)
   return int64_t(x);
 #endif
 }
+// Go leaves int64(x) of a NaN or of a value outside the int64 range implementation-defined; d2i_floor and d2i_ceil
+// follow DESIGN.md §3: NaN gives 0 and a value beyond the range saturates at its end.  cvt.rmi / cvt.rpi saturate on
+// their own; the NaN case is spelled out.
+EVG_HD int64_t d2i_sat(double x) {  // x already integral
+  if (x != x) return 0;
+  if (x >= 9223372036854775808.0) return kI64Max;
+  if (x < -9223372036854775808.0) return kI64Min;
+  return int64_t(x);
+}
 EVG_HD int64_t d2i_floor(double x) {  // Go int64(math.Floor(x))
 #if defined(__CUDA_ARCH__)
-  return __double2ll_rd(x);
+  return x != x ? 0 : __double2ll_rd(x);
 #else
-  return int64_t(std::floor(x));
+  return d2i_sat(std::floor(x));
 #endif
 }
 EVG_HD int64_t d2i_ceil(double x) {  // Go int(math.Ceil(x))
 #if defined(__CUDA_ARCH__)
-  return __double2ll_ru(x);
+  return x != x ? 0 : __double2ll_ru(x);
 #else
-  return int64_t(std::ceil(x));
+  return d2i_sat(std::ceil(x));
 #endif
 }
 
@@ -422,7 +431,7 @@ EVG_HD double soon_free_term(int64_t now, int64_t expected, int64_t stddev, int6
 
 // isMaxHostsCapacity (allocator.go:397-409)
 EVG_HD bool is_max_hosts_capacity(int64_t max_hosts, bool pool, int64_t pool_max, int64_t n_new, int64_t n_existing) {
-  if (pool && n_new > max_hosts * pool_max - n_existing) return true;
+  if (pool && n_new > wsub(wmul(max_hosts, pool_max), n_existing)) return true;  // Go int: wraps
   return n_new + n_existing > max_hosts;
 }
 

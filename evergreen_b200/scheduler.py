@@ -34,7 +34,7 @@ HOST_ALLOCATOR_GPU_UTILIZATION = "gpu-utilization"
 class AllocatorError(Exception):
     """The `error` UtilizationBasedHostAllocator returns for data problems."""
     MESSAGES = {
-        L.EVG_ALLOC_ERR_FUTURE_FRACTION: "future host factor cannot be greater than 1",   # allocator.go:302-304
+        L.EVG_ALLOC_ERR_FUTURE_FRACTION: "future host factor must be between 0 and 1",   # allocator.go:302-304, NaN and < 0 too
         L.EVG_ALLOC_ERR_POOL_SIZE: "unable to plan hosts for distro due to pool size",     # allocator.go:200-202
         L.EVG_ALLOC_ERR_PARENT_MISSING: "error finding parent distros",                    # allocator.go:151-158
     }

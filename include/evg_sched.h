@@ -54,7 +54,7 @@ enum {
  * returns as `error` (utilization_based_host_allocator.go:151-160,200-202,302-304) */
 enum {
   EVG_ALLOC_OK = 0,
-  EVG_ALLOC_ERR_FUTURE_FRACTION = 1, /* "future host factor cannot be greater than 1" */
+  EVG_ALLOC_ERR_FUTURE_FRACTION = 1, /* future_host_fraction above 1 ("future host factor cannot be greater than 1"), below 0 or NaN */
   EVG_ALLOC_ERR_POOL_SIZE = 2,       /* "unable to plan hosts ... due to pool size" (maxHosts < 1) */
   EVG_ALLOC_ERR_PARENT_MISSING = 3   /* container pool parent distro not found */
 };
@@ -120,8 +120,8 @@ typedef struct {
  * of slot group_off[d]+g is the shim's string for group id g. 72 B. */
 typedef struct {
   int64_t count;
-  int64_t count_free;      /* written by the allocator (allocator.go:107-110) */
-  int64_t count_required;  /* written by the allocator */
+  int64_t count_free;      /* written by the allocator (allocator.go:107-110); 0 when the distro's status is an error */
+  int64_t count_required;  /* written by the allocator; 0 when the distro's status is an error */
   int64_t max_hosts;
   int64_t expected_duration;
   int64_t count_duration_over_threshold;
@@ -193,7 +193,7 @@ enum { EVG_PROVIDER_STATIC = 0, /* not in evergreen.ProviderSpawnable (globals.g
 /* distro.HostAllocatorSettings + the rest of HostAllocatorData that is not
  * hosts or queue info (model/distro/distro.go:267-280, host_allocator.go:17-23) */
 typedef struct {
-  double future_host_fraction;
+  double future_host_fraction;       /* outside [0, 1] (NaN included): EVG_ALLOC_ERR_FUTURE_FRACTION */
   int32_t provider;                   /* EVG_PROVIDER_* */
   int32_t disabled;                   /* Distro.Disabled */
   int32_t minimum_hosts;
@@ -208,11 +208,15 @@ typedef struct {
 
 /* Allocator outputs (replaces the (int, int, error) of HostAllocator,
  * host_allocator.go:15).  `result` is the same data packed for the
- * multi-GPU all-gather: 16 B per distro. */
+ * multi-GPU all-gather: 16 B per distro.  Both counts fit their int32 fields:
+ * new_hosts <= max(length_with_dependencies_met, minimum_hosts) and
+ * 0 <= free_hosts <= the distro's host count.  The fraction is rejected
+ * outside [0, 1], so every soon-to-be-free term lies in [0, 1] or, with a
+ * threshold of 0, is NaN; a NaN sum floors to 0 (DESIGN.md §3 (iv)). */
 typedef struct {
   int32_t new_hosts;   /* numNewHostsToRequest */
   int32_t free_hosts;  /* numFreeApprox (or len(freeHosts) on the early returns) */
-  int64_t deficit_ns;  /* auxiliary: max(0, expected_duration - free_hosts*threshold), host-time the free pool cannot absorb */
+  int64_t deficit_ns;  /* auxiliary: max(0, expected_duration - free_hosts*threshold), int64 with wrap: host-time the free pool cannot absorb */
 } evg_alloc_result;
 
 typedef struct {

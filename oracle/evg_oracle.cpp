@@ -36,6 +36,7 @@ inline std::string_view sv(const evo_strcol& c, int64_t i) {
 // Go: time.Duration arithmetic wraps (two's complement); do it unsigned.
 inline int64_t wadd(int64_t a, int64_t b) { return int64_t(uint64_t(a) + uint64_t(b)); }
 inline int64_t wmul(int64_t a, int64_t b) { return int64_t(uint64_t(a) * uint64_t(b)); }
+inline int64_t wsub(int64_t a, int64_t b) { return int64_t(uint64_t(a) - uint64_t(b)); }  // no negation: b may be INT64_MIN
 
 // Go time.Time.Sub / time.Since: saturating (time/time.go Sub).
 inline int64_t since(int64_t now, int64_t t) {
@@ -437,12 +438,21 @@ std::string host_group_name(const HView& hv, int64_t i) {  // allocator.go:226-2
   return s;
 }
 
+// int64(x) for an integral double x (DESIGN.md §3): NaN gives 0, a value beyond the int64 range saturates at its end.
+// Go leaves both implementation-defined, and a plain C++ cast of them is undefined.
+int64_t d2i_sat(double x) {
+  if (std::isnan(x)) return 0;
+  if (x >= 9223372036854775808.0) return INT64_MAX;
+  if (x < -9223372036854775808.0) return INT64_MIN;
+  return int64_t(x);
+}
+
 int64_t calc_new_hosts_needed(int64_t short_ns, int64_t threshold, int64_t exp_free, int64_t n_long,
                               int64_t n_overdue, int64_t n_mq, bool round_down) {  // :268-296
   double turn = double(short_ns) / double(threshold);
   double x = turn - double(exp_free) + double(n_long) + double(n_overdue) + double(n_mq);
   if (exp_free < 1 && x > 0 && x < 1) return 1;
-  int64_t n = round_down ? int64_t(std::floor(x)) : int64_t(std::ceil(x));
+  int64_t n = d2i_sat(round_down ? std::floor(x) : std::ceil(x));
   return n < 0 ? 0 : n;
 }
 
@@ -456,10 +466,10 @@ double soon_to_be_free(const HView& hv, const std::vector<int64_t>& hosts, doubl
     if (!(h.rt_found && h.rt_found[gi])) continue;  // task.Find returned no document for it
     int64_t expected = h.rt_expected_ns[gi], stddev = h.rt_std_ns[gi];
     int64_t elapsed = since(now, h.rt_start_time[gi]);
-    int64_t left = wadd(expected, -elapsed);
+    int64_t left = wsub(expected, elapsed);
     double f;
     if (elapsed > kMaxDurationPerDistroHost && stddev > 0 && elapsed > wadd(expected, wmul(3, stddev))) f = 0;
-    else f = double(wadd(threshold, -left)) / double(threshold);
+    else f = double(wsub(threshold, left)) / double(threshold);
     if (f < 0) f = 0;
     if (f > 1) f = 1;
     sum += frac * f;
@@ -470,15 +480,15 @@ double soon_to_be_free(const HView& hv, const std::vector<int64_t>& hosts, doubl
 int32_t calc_existing_free_hosts(const HView& hv, const std::vector<int64_t>& hosts, double frac,
                                  int64_t threshold, int64_t now, int64_t* out) {  // :300-318
   *out = 0;
-  if (frac > 1) return EVO_ERR_FUTURE_FRACTION;
+  if (!(frac >= 0 && frac <= 1)) return EVO_ERR_FUTURE_FRACTION;  // :302-304 rejects > 1; NaN and < 0 too (evg_sched.h)
   int64_t n_free = 0;
   for (int64_t i : hosts) if (host_is_free(hv, i)) n_free++;
-  *out = n_free + int64_t(std::floor(soon_to_be_free(hv, hosts, frac, threshold, now)));
+  *out = n_free + d2i_sat(std::floor(soon_to_be_free(hv, hosts, frac, threshold, now)));
   return EVO_OK;
 }
 
 bool is_max_hosts_capacity(int64_t max_hosts, bool pool, int64_t pool_max, int64_t n_new, int64_t n_existing) {  // :397-409
-  if (pool && n_new > max_hosts * pool_max - n_existing) return true;
+  if (pool && n_new > wsub(wmul(max_hosts, pool_max), n_existing)) return true;  // Go int: wraps
   return n_new + n_existing > max_hosts;
 }
 
@@ -502,7 +512,7 @@ int32_t eval_host_utilization(const HView& hv, const evo_alloc_settings& a, cons
   bool round_down = std::string_view(a.rounding_rule ? a.rounding_rule : "") != "round-up";
   int64_t overdue = std::string_view(a.feedback_rule ? a.feedback_rule : "") == "waits-over-thresh-feedback"
                         ? info.count_wait_over_threshold : 0;
-  int64_t short_ns = wadd(info.expected_duration, -info.duration_over_threshold);
+  int64_t short_ns = wsub(info.expected_duration, info.duration_over_threshold);
   int64_t n = calc_new_hosts_needed(short_ns, threshold, exp_free, info.count_duration_over_threshold, overdue,
                                     info.count_dep_filled_merge_queue_tasks, round_down);
   if (n > info.count) n = info.count;
@@ -547,7 +557,11 @@ int32_t allocate(const HView& hv, const evo_alloc_settings& a, const evo_queue_i
     }
     int64_t n = 0, f = 0;
     int32_t st = eval_host_utilization(hv, a, kv.second.hosts, gi, info.max_duration_threshold, max_hosts, now, &n, &f);
-    if (st != EVO_OK) { *out_new = 0; *out_free = n_free; return st; }
+    if (st != EVO_OK) {  // the groups written so far depend on Go's map order: an error leaves them all at 0
+      for (auto& g : info_by_name) groups[g.second].count_free = groups[g.second].count_required = 0;
+      *out_new = 0; *out_free = n_free;
+      return st;
+    }
     required += n;
     free_approx += f;
     if (!name.empty()) {
@@ -684,8 +698,9 @@ void evo_job_batch(const evo_tasks* t, const int64_t* task_off, const evo_hosts*
         out_total_value[task_off[d] + k] = r.units[r.unit_of_rank[k]].bd[EVO_BD_TOTAL_VALUE];
         if (out_bd) std::memcpy(out_bd + (task_off[d] + int64_t(k)) * EVO_BD_N, r.units[r.unit_of_rank[k]].bd, sizeof(int64_t) * EVO_BD_N);
       }
+      // evg_distro_cfg.target_time_ns is resolved already: 0 stays 0 (a threshold the C ABI accepts)
       QueueInfo q = queue_info(v, r.order.data(), int64_t(r.order.size()), distro_ids ? distro_ids[d] : "",
-                               target_time(ps[d]), ps[d].includes_dependencies != 0, now);
+                               ps[d].target_time_ns, ps[d].includes_dependencies != 0, now);
       out_info[d] = q.info;
       if (h && as) {
         HView hv{h, host_off[d], host_off[d + 1] - host_off[d]};

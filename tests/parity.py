@@ -18,7 +18,7 @@ def first_diff(a, b):
 
 def check_against_oracle(w, po, ao, distros=None, threads=8, check_groups=True):
     """Bit-exact: ranked order, TotalValue per rank, every DistroQueueInfo /
-    TaskGroupInfo scalar, (new_hosts, free_hosts, status)."""
+    TaskGroupInfo scalar, (new_hosts, free_hosts, status) and deficit_ns."""
     job = O.SoAJob(w.tasks, w.distros, w.hosts, distros)
     ref = job.run(w.now, threads)
     toff = w.distros.task_off
@@ -46,14 +46,22 @@ def check_against_oracle(w, po, ao, distros=None, threads=8, check_groups=True):
                     if g < 0 and f == "max_hosts":
                         continue  # the "" bucket's MaxHosts is never read (allocator.go:80-82)
                     assert int(mine[f]) == int(row[f]), (d, g, f, int(mine[f]), int(row[f]))
-                if ao is not None and g >= 0 and int(ref["status"][j]) == 0:
+                if ao is not None and g >= 0:  # an error status leaves them at 0 on both sides (evg_sched.h)
                     for f in ("count_free", "count_required"):
                         assert int(mine[f]) == int(row[f]), (d, g, f, int(mine[f]), int(row[f]))
         if ao is not None:
             got = (int(ao.result[d]["new_hosts"]), int(ao.result[d]["free_hosts"]), int(ao.status[d]))
             want = (int(ref["new_hosts"][j]), int(ref["free_hosts"][j]), int(ref["status"][j]))
             assert got == want, (d, got, want)
+            # max(0, ExpectedDuration - free_hosts * MaxDurationThreshold), int64 with wrap (evg_sched.h)
+            deficit = max(0, _wrap64(int(ref["info"][j]["expected_duration"]) -
+                                     _wrap64(int(ref["free_hosts"][j]) * int(ref["info"][j]["max_duration_threshold"]))))
+            assert int(ao.result[d]["deficit_ns"]) == deficit, (d, int(ao.result[d]["deficit_ns"]), deficit)
     return ref
+
+
+def _wrap64(x: int) -> int:
+    return (x + 2 ** 63) % 2 ** 64 - 2 ** 63
 
 
 def _sel_gid(w, job):
