@@ -10,12 +10,13 @@
 //   k_gunit/k_grank  per unit: Unit.info / value / anchor, and every member's rank in the unit, once
 //   k_gbest        per work-list task: its first-occurrence choice (planner.go:467-477) and that unit's rank of it;
 //                  anchor histogram e[]
-//   k_gsum/k_gscan/k_gplace/k_gplace_unit
-//                  canonical pre-arrangement by COUNTING instead of sorting tie bytes: an exclusive scan of e[] over
-//                  the distro gives every anchor's run start; tasks are written to (key, index) buffers in
-//                  (anchor, rank-in-unit) order: k_gplace the tasks emitted from their own single-task unit, k_gplace_unit
-//                  every multi-member unit's emitted tasks, from the unit.  Distros without multi-member units skip the
-//                  scan (identity).
+//   k_gsum/k_gscan/k_gplace
+//                  canonical pre-arrangement by COUNTING instead of sorting tie bytes: an exclusive scan of e[] per tile
+//                  (k_gsum) and of the tile totals per distro (k_gscan) gives every anchor's run start; tasks are
+//                  written to (key, index) buffers in (anchor, rank-in-unit) order by one kernel, k_gplace, a block per
+//                  tile: the tile's tasks emitted from their own single-task unit and the tasks of the small units
+//                  anchored in it, then a share of the large units, a warp each.  The writers touch disjoint slots and
+//                  write only those.  Distros without multi-member units skip the scans (identity).
 //   k_ghist/k_gdscan/k_gscatter
 //                  stable LSD radix sort on key = Vmax - V only: 32-bit keys, ceil(bits(Vmax-Vmin)/8) passes (3 for
 //                  a 20-bit range), 8 B/task each way per pass; a distro whose range exceeds 32 bits carries a
@@ -40,7 +41,8 @@ struct DGen {
   uint32_t* key_lo[2];         // [T] low word of Vmax - V, in sort position
   uint32_t* key_hi[2];         // [T] high word (distros with a range above 32 bits only)
   uint32_t* idx[2];            // [T] distro-local task index, in sort position
-  uint32_t* e;                 // [T] anchor histogram, then exclusive positions
+  uint32_t* e;                 // [T] anchor histogram, then (k_gsum) the offset of the anchor's run inside its tile's
+                               //     stretch; the run starts at tile_sum[tile] + e in the distro (gen_run_start)
   uint32_t* tile_sum;          // [NT] sum of e over the tile, then the tile's exclusive offset inside its distro
   uint32_t* tile_hist;         // [NT*256]
   uint4* wl;                   // work list, one entry per task that touches a multi-member unit: x = global task index,
@@ -123,7 +125,8 @@ __device__ __forceinline__ void unit_store(GUnit* p, const GUnit& u) {
   reinterpret_cast<uint4*>(p)[1] = make_uint4(u.start, uint32_t(u.d), 0u, 0u);
 }
 // The slot map of the general path: k_galloc files a unit's id and run start under its slot, in the on-chip planners'
-// unit_v (no general-path slot is an on-chip one), so that k_gfill finds both with one load.
+// unit_v (no general-path slot is an on-chip one), so that k_gfill finds both with one load (and k_gplace the id of the
+// unit a task anchors, under its own-key slot).
 __device__ __forceinline__ int64_t slot_unit(uint32_t id, uint32_t start) { return int64_t(uint64_t(id) | (uint64_t(start) << 32)); }
 
 __global__ void k_ginit(DGen G, const int32_t* __restrict__ general_list, int n) {
@@ -398,12 +401,13 @@ __global__ void __launch_bounds__(256, kGTaskOcc) k_gtask(DTasks T, DDistros D, 
 //   k_grank   the ranks of the larger units, a warp per 32 members
 //   k_gbest   per task: the first unit it is emitted from among its memberships (TaskPlan.Export, planner.go:467-477)
 //             and its rank there, one record load per membership; the task is filed under that rank in the unit's
-//             emitted-by-rank slots, emit[start + rank], from which k_gplace_unit writes the unit's tasks in order
+//             emitted-by-rank slots, emit[start + rank], from which k_gplace writes the unit's tasks in order
 // A membership's place in its run is kept next to the membership, so every access is coalesced: by work-list entry for
 // the own-key (pown) and version (pver) memberships, by edge for dependency memberships (pedge, with the edge's unit slot
-// in sedge).  After k_gfill the slot space (one slot per task and group, ~10x the units) is not touched again: what the
-// later kernels ask of a unit is its 32-byte record, by id.  The on-chip planner's next[] / pair_slot[], indexed by pair
-// id over 2T+E entries of which the general path would touch about a quarter (a sector per access), are not used here.
+// in sedge).  After k_gfill the slot space (one slot per task and group, ~10x the units) is read once more, by k_gplace,
+// for the unit each anchor task anchors; what the other later kernels ask of a unit is its 32-byte record, by id.  The
+// on-chip planner's next[] / pair_slot[], indexed by pair id over 2T+E entries of which the general path would touch
+// about a quarter (a sector per access), are not used here.
 
 // what a work-list task is filed under: one 16-byte entry k_gtask wrote (the same answers in every kernel below)
 struct WlTask {
@@ -542,7 +546,7 @@ __global__ void __launch_bounds__(256, kUnitTableOcc) k_gfill(DTasks T, DDistros
 #pragma unroll
       for (int m = 0; m < 2; m++) {
         place[j][m] = sl[m] != kInactive ? (m ? G.pver : G.pown)[k] : 0u;
-        const uint64_t su = sl[m] != kInactive ? uint64_t(W.unit_v[sl[m]]) : ~0ull;  // the last read of the slot space
+        const uint64_t su = sl[m] != kInactive ? uint64_t(W.unit_v[sl[m]]) : ~0ull;
         id[j][m] = uint32_t(su);
         start[j][m] = uint32_t(su >> 32);
       }
@@ -692,7 +696,7 @@ __global__ void __launch_bounds__(256, kUnitTableOcc) k_gbest(DTasks T, DDistros
         }
       });
       // Emitted from a multi-member unit: filed under its rank among ALL members of the unit, as k_gunit / k_grank
-      // counted it (ranks are unique inside a unit: a plain store), and k_gplace_unit writes it with the unit's value.
+      // counted it (ranks are unique inside a unit: a plain store), and k_gplace writes it with the unit's value.
       // Emitted from its own single-task unit: k_gplace writes it with the value k_gtask left in tv.
       if (bid != kInactive) {
         G.emit[bstart + G.rank[bpos]] = li;
@@ -732,19 +736,53 @@ __global__ void k_gsched(DGen G, const int32_t* __restrict__ general_list, int n
   atomicMax(G.maxpass, gen_npass(gen_bits(G, general_list[k])));
 }
 
-// sum of e[] over each tile
+// e[] of the eight task slots t8 .. t8+7 of a tile (t8 a multiple of 4): 128-bit accesses inside the distro, slot by
+// slot at its edges (slots outside it read as 0 and are not written)
+__device__ __forceinline__ void gen_e_load8(const DGen& G, int64_t t8, int64_t base, int64_t end, uint32_t (&ev)[8]) {
+  if (t8 >= base && t8 + 7 < end) {
+    const uint4 a = *reinterpret_cast<const uint4*>(G.e + t8), b = *reinterpret_cast<const uint4*>(G.e + t8 + 4);
+    ev[0] = a.x; ev[1] = a.y; ev[2] = a.z; ev[3] = a.w; ev[4] = b.x; ev[5] = b.y; ev[6] = b.z; ev[7] = b.w;
+  } else {
+#pragma unroll
+    for (int m = 0; m < 8; m++) { const int64_t t = t8 + m; ev[m] = (t >= base && t < end) ? G.e[t] : 0u; }
+  }
+}
+
+// Per tile: exclusive scan of e[] (thread q owns 8 consecutive slots).  Every task's e becomes the offset of its anchor's
+// run inside the tile's stretch, and tile_sum the tile's total (k_gscan turns the totals into the tiles' offsets in the
+// distro).  The offsets are final before k_gplace starts, so a unit placed by any block finds its anchor's run start
+// without waiting for the block that places the anchor's tile.
 __global__ void __launch_bounds__(256) k_gsum(DDistros D, DGen G) {
   const int tile = int(blockIdx.x + G.tile0);
   const int d = G.tile_distro[tile];
   const int64_t base = D.task_off[d], end = D.task_off[d + 1];
-  const int64_t lo = max(G.tile_start[tile], base), hi = min(G.tile_start[tile] + kGTile, end);
+  const int64_t t8 = G.tile_start[tile] + 8 * int64_t(threadIdx.x);  // multiple of 4
+  uint32_t ev[8];
+  gen_e_load8(G, t8, base, end, ev);
   uint32_t sum = 0;
-  for (int64_t t = lo + threadIdx.x; t < hi; t += 256) sum += G.e[t];
-  sum = __reduce_add_sync(0xffffffffu, sum);
+#pragma unroll
+  for (int m = 0; m < 8; m++) sum += ev[m];
   __shared__ uint32_t sw[8];
-  if ((threadIdx.x & 31) == 0) sw[threadIdx.x >> 5] = sum;
-  __syncthreads();
-  if (threadIdx.x == 0) G.tile_sum[tile] = sw[0] + sw[1] + sw[2] + sw[3] + sw[4] + sw[5] + sw[6] + sw[7];
+  uint32_t total;
+  uint32_t run = block_scan_excl<8>(sum, sw, &total);
+#pragma unroll
+  for (int m = 0; m < 8; m++) { const uint32_t x = ev[m]; ev[m] = run; run += x; }
+  if (t8 >= base && t8 + 7 < end) {
+    *reinterpret_cast<uint4*>(G.e + t8) = make_uint4(ev[0], ev[1], ev[2], ev[3]);
+    *reinterpret_cast<uint4*>(G.e + t8 + 4) = make_uint4(ev[4], ev[5], ev[6], ev[7]);
+  } else {
+#pragma unroll
+    for (int m = 0; m < 8; m++) { const int64_t t = t8 + m; if (t >= base && t < end) G.e[t] = ev[m]; }
+  }
+  if (threadIdx.x == 0) G.tile_sum[tile] = total;
+}
+
+// Where the run of the distro-local task `anchor` starts in its distro's pre-arrangement (after k_gsum and k_gscan): its
+// tile's offset plus its offset inside the tile.  Tiles of a distro start at (base & ~3) + k * kGTile.
+__device__ __forceinline__ uint32_t gen_run_start(const DDistros& D, const DGen& G, int d, uint32_t anchor) {
+  const int64_t base = D.task_off[d];
+  const int64_t tile = G.dtile_off[d] + ((int64_t(anchor) + (base & 3)) / kGTile);
+  return G.tile_sum[tile] + G.e[base + anchor];
 }
 
 // exclusive scan of the tile sums of one distro (<= 1025 tiles), one block per general-path distro
@@ -764,11 +802,19 @@ __device__ __forceinline__ void gen_put(const DGen& G, int64_t base, uint32_t po
   gen_put_key(G, base, pos, vmax_ord - ord_i64(v), wide, li);
 }
 
-// Per tile: exclusive scan of e[] (thread q owns 8 consecutive slots) on top of the tile's offset = the run start of
-// every anchor; tasks emitted from their own single-task unit are written to their sort position.  use_e == 0 (no
-// multi-member unit in any general-path distro): positions are the input order.
-__global__ void __launch_bounds__(256) k_gplace(DDistros D, DWork W, DGen G, int use_e) {
-  const int tile = int(blockIdx.x + G.tile0);
+// Placement: the (Vmax - V, index) pairs go to key_lo[0] / key_hi[0] / idx[0] in (anchor, rank-in-unit) order, by one
+// kernel, a block per tile.  The block writes its tile's stretch: the tasks emitted from their own single-task unit, and
+// the tasks of every unit of up to kRankOne members anchored in the tile.  Then it takes its share of blist: the larger
+// units, a warp each, wherever they are anchored.
+//
+// Every writer writes only the slots it fills, and the writers touch disjoint slots: a task emitted from its own unit
+// has a run of one slot (it anchors no multi-member unit, whose anchor is an own-key member), and a unit writes only
+// inside its anchor's run.  So no slot is written twice, none is left with an earlier tick's data, and the order of the
+// writers does not reach the result.  Placing a small unit from the block that holds its anchor puts the unit's bytes
+// into the same sectors as the tile's, while they are in L2 (in the stage, when the stretch fits it).  Walked in id
+// order, the units reach a stretch long after its tile has left L2 (k_galloc hands out ids in waves of resident
+// blocks, not in work-list order), and every sector a unit shares with a tile costs a DRAM read and a write.
+__device__ __forceinline__ void gplace_tile(const DTasks& T, const DDistros& D, const DWork& W, const DGen& G, int tile, int use_e) {
   const int d = G.tile_distro[tile];
   const int64_t base = D.task_off[d], end = D.task_off[d + 1];
   const int64_t ts = G.tile_start[tile];
@@ -777,26 +823,24 @@ __global__ void __launch_bounds__(256) k_gplace(DDistros D, DWork W, DGen G, int
   const int tid = threadIdx.x;
   const int64_t t8 = ts + 8 * int64_t(tid);  // multiple of 4
   const bool interior = t8 >= base && t8 + 7 < end;  // the common case: 128-bit loads
-  uint32_t ev[8];
-  uint32_t sum = 0;
+  // use_e: the tile's tasks land in ONE contiguous stretch of the distro's segment, [tile_sum[tile], + the tile's total),
+  // at the offsets k_gsum left in e.  The block's tasks are staged in shared memory and copied out slot by slot,
+  // skipping the slots of the warp-walked units (kInactive in st_ix): 4-byte stores straight from registers cost a
+  // sector each, several times the sectors of the payload.  A stretch above kStage slots is written from registers.
+  constexpr int kStage = 3072;
+  __shared__ uint32_t st_lo[kStage], st_ix[kStage], st_hi[kStage];
+  uint32_t p_tile = 0, total = 0;
   if (use_e) {
-    if (interior) {
-      const uint4 a = *reinterpret_cast<const uint4*>(G.e + t8), b = *reinterpret_cast<const uint4*>(G.e + t8 + 4);
-      ev[0] = a.x; ev[1] = a.y; ev[2] = a.z; ev[3] = a.w; ev[4] = b.x; ev[5] = b.y; ev[6] = b.z; ev[7] = b.w;
-    } else {
-#pragma unroll
-      for (int m = 0; m < 8; m++) { const int64_t t = t8 + m; ev[m] = (t >= base && t < end) ? G.e[t] : 0u; }
-    }
-#pragma unroll
-    for (int m = 0; m < 8; m++) sum += ev[m];
+    p_tile = G.tile_sum[tile];
+    // every task of the distro is emitted once, so the distro's stretches add up to its task count
+    const uint32_t p_next = tile + 1 < G.dtile_off[d + 1] ? G.tile_sum[tile + 1] : uint32_t(end - base);
+    total = p_next - p_tile;
+    if (total <= uint32_t(kStage))  // the barrier before the stage is filled publishes this
+      for (uint32_t q = tid; q < total; q += 256) st_ix[q] = kInactive;
   }
-  uint32_t run = 0;
-  if (use_e) {
-    __shared__ uint32_t sw[8];
-    run = G.tile_sum[tile] + block_scan_excl<8>(sum, sw);
-  }
+  const bool staged = total <= uint32_t(kStage);  // block-uniform
   int64_t vv[8];
-  uint32_t dsp = 0;  // bit m: task t8+m is emitted from a multi-member unit (placed by k_gplace_unit)
+  uint32_t dsp = 0;  // bit m: task t8+m is emitted from a multi-member unit (placed with that unit)
   if (interior) {
 #pragma unroll
     for (int m = 0; m < 8; m += 2) {
@@ -818,41 +862,68 @@ __global__ void __launch_bounds__(256) k_gplace(DDistros D, DWork W, DGen G, int
     }
   }
   if (use_e) {
-    // The tile's single-task-unit tasks land in ONE contiguous stretch of the distro's segment, [tile_sum[tile], + sum of
-    // e over the tile), with holes where the multi-member units' tasks will be put by k_gplace_unit.  They are staged in
-    // shared memory and the stretch is written out whole (holes included: k_gplace_unit runs later and fills them):
-    // 4-byte stores straight from registers cost a sector each, several times the sectors of the payload.
-    constexpr int kStage = 3072;
-    __shared__ uint32_t st_lo[kStage], st_ix[kStage], st_hi[kStage];
-    __shared__ uint32_t s_total;
-    const uint32_t p_tile = G.tile_sum[tile];
-    if (tid == 255) s_total = run + sum - p_tile;  // `run` is this thread's exclusive offset: the last thread knows the tile's total
     uint32_t ps[8];
-#pragma unroll
-    for (int m = 0; m < 8; m++) { ps[m] = run; run += ev[m]; }
-    if (interior) {
-      *reinterpret_cast<uint4*>(G.e + t8) = make_uint4(ps[0], ps[1], ps[2], ps[3]);
-      *reinterpret_cast<uint4*>(G.e + t8 + 4) = make_uint4(ps[4], ps[5], ps[6], ps[7]);
-    } else {
-#pragma unroll
-      for (int m = 0; m < 8; m++) { const int64_t t = t8 + m; if (t >= base && t < end) G.e[t] = ps[m]; }
-    }
+    gen_e_load8(G, t8, base, end, ps);
+    // the run length of every slot: the next slot's offset (the next thread's first, across warps through s_first)
+    __shared__ uint32_t s_first[8];
+    const int lane = tid & 31, warp = tid >> 5;
+    if (lane == 0) s_first[warp] = ps[0];
     __syncthreads();
-    const uint32_t total = s_total;
-    const bool staged = total <= uint32_t(kStage);  // block-uniform
+    uint32_t nx = __shfl_down_sync(0xffffffffu, ps[0], 1);
+    if (lane == 31) nx = warp < 7 ? s_first[warp + 1] : total;
 #pragma unroll
     for (int m = 0; m < 8; m++) {
       const int64_t t = t8 + m;
       if (t >= base && t < end && !((dsp >> m) & 1u)) {
         if (staged) {
           const unsigned long long key = vmax_ord - ord_i64(vv[m]);
-          const uint32_t q = ps[m] - p_tile;
-          st_lo[q] = uint32_t(key); st_ix[q] = uint32_t(t - base);
-          if (wide) st_hi[q] = uint32_t(key >> 32);
+          st_lo[ps[m]] = uint32_t(key); st_ix[ps[m]] = uint32_t(t - base);
+          if (wide) st_hi[ps[m]] = uint32_t(key >> 32);
         } else {
-          gen_put(G, base, ps[m], vmax_ord, wide, vv[m], uint32_t(t - base));
+          gen_put(G, base, p_tile + ps[m], vmax_ord, wide, vv[m], uint32_t(t - base));
         }
       }
+    }
+    // the small units anchored in this tile: a task emitted from a multi-member unit that has a run anchors the unit
+    // filed under its own key (an anchor is an own-key member), whose id k_galloc left in that slot.  The unit's
+    // emitted tasks fill the run in rank order.
+    uint32_t amask = 0;
+#pragma unroll
+    for (int m = 0; m < 8; m++) {
+      const int64_t t = t8 + m;
+      // the distro's last task runs to the end of the stretch: the slots past the distro read as 0
+      const uint32_t run_end = t + 1 < end ? (m < 7 ? ps[m + 1] : nx) : total;
+      amask |= ((t >= base && t < end && ((dsp >> m) & 1u) && run_end != ps[m]) ? 1u : 0u) << m;
+    }
+    if (amask) {
+      const uint32_t ub = uint32_t(D.unit_base[d]), ng = uint32_t(D.group_off[d + 1] - D.group_off[d]);
+      const bool gv = D.cfg[d].group_versions != 0;
+      do {
+        const int m = __ffs(amask) - 1;
+        amask &= amask - 1u;
+        uint32_t q = 0;
+#pragma unroll
+        for (int j = 0; j < 8; j++) q = j == m ? ps[j] : q;
+        const int64_t t = t8 + m;
+        const uint32_t id = uint32_t(W.unit_v[ub + own_slot_local(T.gid[t], T.vid[t], uint32_t(t - base), ng, gv)]);
+        const GUnit u = unit_load(G.unit + id);
+        if (u.n > kRankOne) continue;  // a warp's job (gplace_big_units)
+        uint32_t li[kRankOne];
+#pragma unroll
+        for (uint32_t i = 0; i < kRankOne; i++) li[i] = i < u.n ? G.emit[u.start + i] : kInactive;
+        const unsigned long long key = vmax_ord - ord_i64(u.value);
+#pragma unroll
+        for (uint32_t i = 0; i < kRankOne; i++) {
+          if (li[i] == kInactive) continue;
+          if (staged) {
+            st_lo[q] = uint32_t(key); st_ix[q] = li[i];
+            if (wide) st_hi[q] = uint32_t(key >> 32);
+          } else {
+            gen_put_key(G, base, p_tile + q, key, wide, li[i]);
+          }
+          q++;
+        }
+      } while (amask);
     }
     if (staged) {
       __syncthreads();
@@ -860,7 +931,9 @@ __global__ void __launch_bounds__(256) k_gplace(DDistros D, DWork W, DGen G, int
       uint32_t* dix = G.idx[0] + base + p_tile;
       uint32_t* dhi = G.key_hi[0] + base + p_tile;
       for (uint32_t q = tid; q < total; q += 256) {
-        dlo[q] = st_lo[q]; dix[q] = st_ix[q];
+        const uint32_t ix = st_ix[q];
+        if (ix == kInactive) continue;
+        dlo[q] = st_lo[q]; dix[q] = ix;
         if (wide) dhi[q] = st_hi[q];
       }
     }
@@ -889,36 +962,17 @@ __global__ void __launch_bounds__(256) k_gplace(DDistros D, DWork W, DGen G, int
   }
 }
 
-// The tasks a multi-member unit emits, written by the unit: they share one key, Vmax - unit value, and one stretch of the
-// pre-arrangement, from its anchor's run start (e[] holds exclusive positions by now) in rank order.  The unit walks its
-// emitted-by-rank slots, so no member is placed by a loop over the others.  Units of up to kRankOne members: a thread per
-// unit, in id order (coalesced records); larger ones: a warp per unit (its chunk-0 entry in blist), 32 ranks per step, a
-// ballot giving every lane its place after the running count.
-__global__ void __launch_bounds__(256, kUnitTableOcc) k_gplace_unit(DDistros D, DWork W, DGen G) {
-  if (*W.err) return;
-  const unsigned int n = *G.hcount;
-  for (unsigned int k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += gridDim.x * blockDim.x) {
-    const GUnit u = unit_load(G.unit + k);
-    if (u.anchor == kNoAnchor || u.n > kRankOne) continue;
-    // every load of the unit before its first store: a store may alias a later emit load, so a walk that stored as it
-    // loaded would wait a memory round trip per member
-    uint32_t li[kRankOne];
-#pragma unroll
-    for (uint32_t i = 0; i < kRankOne; i++) li[i] = i < u.n ? G.emit[u.start + i] : kInactive;
-    const int64_t base = D.task_off[u.d];
-    const unsigned long long key = G.vmm[2 * u.d] - ord_i64(u.value);
-    const bool wide = gen_bits(G, u.d) > 32;
-    uint32_t pos = G.e[base + u.anchor];
-#pragma unroll
-    for (uint32_t i = 0; i < kRankOne; i++)
-      if (li[i] != kInactive) gen_put_key(G, base, pos++, key, wide, li[i]);
-  }
-  const unsigned int nb = *G.bcount;
+// The tasks a unit emits share one key, Vmax - unit value, and one stretch of the pre-arrangement, from its anchor's run
+// start in rank order: the unit walks its emitted-by-rank slots, so no member is placed by a loop over the others.  Units
+// above kRankOne members: a warp per unit (its chunk-0 entry in blist), 32 ranks per step, a ballot giving every lane its
+// place after the running count.  Block `item` of n_items takes that share of blist.
+__device__ __forceinline__ void gplace_big_units(const DDistros& D, const DGen& G, unsigned int item, unsigned int n_items) {
+  const unsigned long long nb = *G.bcount;
   const unsigned full = 0xffffffffu;
   const int lane = threadIdx.x & 31;
   const unsigned lt = (1u << lane) - 1u;
-  const unsigned int nw = gridDim.x * (blockDim.x >> 5);
-  for (unsigned int c = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); c < nb; c += nw) {  // warp-uniform
+  const unsigned int c1 = unsigned(nb * (item + 1) / n_items);
+  for (unsigned int c = unsigned(nb * item / n_items) + (threadIdx.x >> 5); c < c1; c += blockDim.x >> 5) {  // warp-uniform
     const uint2 ch = G.blist[c];
     if (ch.y != 0u) continue;  // one warp per unit
     const GUnit u = unit_load(G.unit + ch.x);
@@ -926,7 +980,7 @@ __global__ void __launch_bounds__(256, kUnitTableOcc) k_gplace_unit(DDistros D, 
     const int64_t base = D.task_off[u.d];
     const unsigned long long key = G.vmm[2 * u.d] - ord_i64(u.value);
     const bool wide = gen_bits(G, u.d) > 32;
-    uint32_t pos = G.e[base + u.anchor];
+    uint32_t pos = gen_run_start(D, G, u.d, u.anchor);
     for (uint32_t r0 = 0; r0 < u.n; r0 += 32) {
       const uint32_t li = r0 + lane < u.n ? G.emit[u.start + r0 + lane] : kInactive;
       const unsigned b = __ballot_sync(full, li != kInactive);
@@ -934,6 +988,13 @@ __global__ void __launch_bounds__(256, kUnitTableOcc) k_gplace_unit(DDistros D, 
       pos += uint32_t(__popc(b));
     }
   }
+}
+
+// use_e == 0 (no multi-member unit in any general-path distro): positions are the input order, and there are no units.
+// 48 registers (5 blocks of 256 per SM); at the 40 of 6 blocks, the bound the stage allows, the kernel was no faster
+__global__ void __launch_bounds__(256) k_gplace(DTasks T, DDistros D, DWork W, DGen G, int use_e) {
+  gplace_tile(T, D, W, G, int(G.tile0 + blockIdx.x), use_e);
+  if (use_e && !*W.err) gplace_big_units(D, G, blockIdx.x, gridDim.x);
 }
 
 __device__ __forceinline__ bool gen_tile(const DDistros& D, const DGen& G, int tile, int j, int* d_out, int64_t* seg, int64_t* lo,

@@ -10,7 +10,7 @@
 //   <= 12288 tasks   k_plan_smem<THREADS,ITEMS> (evg_plan_smem.cuh): one CTA per distro, any unit structure
 //   larger           the general path (evg_plan_general.cuh), any size up to 2^21-1 tasks:
 //     k_gmark/k_gtask/k_gunit/k_gbest  dependents, per-task pass, multi-member units
-//     k_gsum/k_gscan/k_gplace*     canonical pre-arrangement by counting
+//     k_gsum/k_gscan/k_gplace      canonical pre-arrangement by counting
 //     k_ghist/k_gdscan/k_gscatter  segmented stable LSD radix sort of 32-bit keys; the last pass writes the ranked
 //                                  queue + TotalValue
 //     k_finalize_info              DistroQueueInfo / TaskGroupInfo scalars (scheduler.go:144-158)
@@ -1983,8 +1983,7 @@ int run_general(evg_ctx* c, cudaStream_t st, const DTasks& dt, const DDistros& d
     launch(c, st, k_gsum, nt, 256, 0, dd, g);
     launch(c, st, k_gscan, unsigned(gcount), 1024, 0, g, gl);
   }
-  launch(c, st, k_gplace, nt, 256, 0, dd, w, g, gc);
-  if (gc) launch(c, st, k_gplace_unit, wl_grid, 256, 0, dd, w, g);
+  launch(c, st, k_gplace, nt, 256, 0, dt, dd, w, g, gc);
   if (c->timed) CK(cudaEventRecord(c->ev_sort0, st));  // the general path's segmented sort
   for (int j = 0; j < 8; j++) {  // passes beyond the tick's longest key exit at once (*maxpass is device-side)
     launch(c, st, k_ghist, nt, 256, 0, j, dd, g);
