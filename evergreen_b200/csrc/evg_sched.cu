@@ -800,8 +800,10 @@ __global__ void __launch_bounds__(256) k_pl_edge_write(int64_t n, const int64_t*
   for (int64_t j = 0; j < k; j++) new_idx[w + j] = dep_idx[e0 + j];
 }
 
-// Expected-duration statistics (model/task/expected_duration.go:36-96): the $match, then per key count / sum, then
-// the squared deviations from floor(mean) as an exact 128-bit integer, then one rounding per output.
+// Expected-duration statistics (model/task/expected_duration.go:36-96): the $match, then per key the count and the
+// exact sum S (signed 128 bits), then S2 = sum (x - floor(S/n))^2 as an exact 192-bit integer (one term is below 2^128
+// and there are fewer than 2^64 of them), then one round-to-nearest-even conversion of S and of S2 to double.  The
+// accumulators are 6 words per key, every word zeroed by the caller: cnt, S as lo / hi, S2 as words 0 / 1 / 2.
 struct DDur {
   int64_t n_rows;
   int32_t n_keys;
@@ -811,14 +813,56 @@ struct DDur {
   const int64_t* finish;
   const uint8_t* flags;
   int64_t w0, w1;
-  unsigned long long* cnt;  // [n_keys]
-  unsigned long long* sum;  // [n_keys] two's complement
-  unsigned long long* sq_lo;
-  unsigned long long* sq_hi;
+  unsigned long long* cnt;     // [n_keys]
+  unsigned long long* sum_lo;  // [n_keys] S, two's complement over sum_hi:sum_lo
+  unsigned long long* sum_hi;
+  unsigned long long* sq0;     // [n_keys] S2 = sq2:sq1:sq0
+  unsigned long long* sq1;
+  unsigned long long* sq2;
 };
+static void dur_accumulators(DDur& x, unsigned long long* acc, int32_t K) {
+  x.cnt = acc; x.sum_lo = acc + K; x.sum_hi = acc + 2 * size_t(K);
+  x.sq0 = acc + 3 * size_t(K); x.sq1 = acc + 4 * size_t(K); x.sq2 = acc + 5 * size_t(K);
+}
 __device__ __forceinline__ bool dur_row_matches(const DDur& X, int64_t r) {
   const uint32_t f = X.flags[r];
   return (f & EVG_DR_COMPLETED) && !(f & EVG_DR_TIMED_OUT) && X.start[r] > X.w0 && X.finish[r] <= X.w1;
+}
+// floor(S / n) and S - n * floor(S / n) for the 128-bit S = hi:lo and n >= 1: the floor lies between the smallest
+// and the largest summand, so it fits int64, and the remainder lies in [0, n).  A sum that fits int64 divides in 64 bits.
+__device__ __forceinline__ int64_t dur_floor_mean(unsigned long long lo, unsigned long long hi, int64_t n, int64_t& rem) {
+  if (hi == (int64_t(lo) < 0 ? ~0ull : 0ull)) {
+    const int64_t s = int64_t(lo);
+    int64_t m = s / n, r = s % n;
+    if (r < 0) { m -= 1; r += n; }
+    rem = r;
+    return m;
+  }
+  const __int128 s = (__int128)(((unsigned __int128)hi << 64) | lo);
+  __int128 m = s / n, r = s % n;
+  if (r < 0) { m -= 1; r += n; }
+  rem = int64_t(r);
+  return int64_t(m);
+}
+// The unsigned integer w2:w1:w0 rounded once to nearest-even: its leading 64 bits, with every bit below them ORed into
+// the lowest one (that sticky bit lies under the rounding position of a 53-bit significand, so halfway stays halfway
+// only when everything below is zero), one __ull2double_rn, then an exact scaling by 2^e.
+__device__ __forceinline__ double dur_u192_to_double_rn(unsigned long long w2, unsigned long long w1, unsigned long long w0) {
+  if (!w2 && !w1) return __ull2double_rn(w0);
+  unsigned long long top, below;
+  int e;
+  if (w2) {
+    const int z = __clzll(w2);
+    top = z ? (w2 << z) | (w1 >> (64 - z)) : w2;
+    below = (w1 << z) | w0;
+    e = 128 - z;
+  } else {
+    const int z = __clzll(w1);
+    top = z ? (w1 << z) | (w0 >> (64 - z)) : w1;
+    below = w0 << z;
+    e = 64 - z;
+  }
+  return __dmul_rn(__ull2double_rn(top | (below != 0 ? 1ull : 0ull)), __longlong_as_double((long long)(1023 + e) << 52));
 }
 __global__ void __launch_bounds__(256) k_dur_sum(DDur X, int* err) {
   const int64_t r = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -827,22 +871,29 @@ __global__ void __launch_bounds__(256) k_dur_sum(DDur X, int* err) {
   if (k < 0 || k >= X.n_keys) { atomicOr(err, 1); return; }
   if (!dur_row_matches(X, r)) return;
   atomicAdd(X.cnt + k, 1ull);
-  atomicAdd(X.sum + k, (unsigned long long)X.taken[r]);
+  // x sign-extended to 128 bits: the low word's carry and the sign word go to the high word, which only a carry
+  // or a negative x touches
+  const int64_t x = X.taken[r];
+  const unsigned long long lo = (unsigned long long)x, old = atomicAdd(X.sum_lo + k, lo);
+  const unsigned long long hi = (x < 0 ? ~0ull : 0ull) + (old + lo < old ? 1ull : 0ull);
+  if (hi) atomicAdd(X.sum_hi + k, hi);
 }
 __global__ void __launch_bounds__(256) k_dur_dev(DDur X) {
   const int64_t r = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
   if (r >= X.n_rows) return;
   const int32_t k = X.key[r];
   if (k < 0 || k >= X.n_keys || !dur_row_matches(X, r)) return;
-  const int64_t n = int64_t(X.cnt[k]), s = int64_t(X.sum[k]);
-  int64_t m0 = s / n;
-  if ((s % n) < 0) m0 -= 1;  // floor
-  const int64_t dv = X.taken[r] - m0;
-  const unsigned long long a = dv < 0 ? (unsigned long long)(-dv) : (unsigned long long)dv;
-  const unsigned long long lo = a * a, hi = __umul64hi(a, a);
-  const unsigned long long old = atomicAdd(X.sq_lo + k, lo);
-  const unsigned long long carry = (old + lo < old) ? 1ull : 0ull;
-  if (hi + carry) atomicAdd(X.sq_hi + k, hi + carry);
+  int64_t rem;
+  const int64_t m0 = dur_floor_mean(X.sum_lo[k], X.sum_hi[k], int64_t(X.cnt[k]), rem);
+  // |x - m0| as an unsigned magnitude: the difference of two int64 is below 2^64 in absolute value
+  const int64_t x = X.taken[r];
+  const unsigned long long a = x >= m0 ? (unsigned long long)x - (unsigned long long)m0 : (unsigned long long)m0 - (unsigned long long)x;
+  const unsigned long long lo = a * a, hi = __umul64hi(a, a);  // hi <= 2^64 - 2: hi + carry does not wrap
+  const unsigned long long old0 = atomicAdd(X.sq0 + k, lo);
+  const unsigned long long h = hi + (old0 + lo < old0 ? 1ull : 0ull);
+  if (!h) return;
+  const unsigned long long old1 = atomicAdd(X.sq1 + k, h);
+  if (old1 + h < old1) atomicAdd(X.sq2 + k, 1ull);
 }
 __global__ void __launch_bounds__(256) k_dur_final(DDur X, evg_duration_stat* out) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
@@ -852,13 +903,17 @@ __global__ void __launch_bounds__(256) k_dur_final(DDur X, evg_duration_stat* ou
   st.mean_ns = 0.0;
   st.stddev_ns = 0.0;
   if (st.count > 0) {
-    const int64_t n = st.count, s = int64_t(X.sum[k]);
-    int64_t m0 = s / n, rem = s % n;
-    if (rem < 0) { m0 -= 1; rem += n; }
+    const int64_t n = st.count;
+    const unsigned long long lo = X.sum_lo[k], hi = X.sum_hi[k];
+    int64_t rem;
+    dur_floor_mean(lo, hi, n, rem);
+    // |S| = the two's complement of a negative S, then the sign back on the rounded magnitude
+    const bool neg = int64_t(hi) < 0;
+    const double s = dur_u192_to_double_rn(0, neg ? ~hi + (lo == 0 ? 1ull : 0ull) : hi, neg ? ~lo + 1ull : lo);
     const double dn = __ll2double_rn(n);
-    st.mean_ns = __ddiv_rn(__ll2double_rn(s), dn);
-    // variance = S2/n - (rem/n)^2 with S2 = sum (x - floor(mean))^2 held exactly in 128 bits
-    const double s2 = __dadd_rn(__dmul_rn(__ull2double_rn(X.sq_hi[k]), 18446744073709551616.0), __ull2double_rn(X.sq_lo[k]));
+    st.mean_ns = __ddiv_rn(neg ? -s : s, dn);
+    // variance = S2/n - (rem/n)^2
+    const double s2 = dur_u192_to_double_rn(X.sq2[k], X.sq1[k], X.sq0[k]);
     const double fr = __ddiv_rn(__ll2double_rn(rem), dn);
     double var = __dadd_rn(__ddiv_rn(s2, dn), -__dmul_rn(fr, fr));
     if (var < 0.0) var = 0.0;
@@ -927,7 +982,8 @@ __global__ void __launch_bounds__(256) k_dur_resolve(DDurRows R, int32_t n_keys,
       src = value == 0 ? EVG_DS_DEFAULT : EVG_DS_PREVIOUS;
       avg = value == 0 ? 10 * kMinute : value; sd = value == 0 ? 0 : pstd;
     } else {
-      const int64_t a = __double2ll_rz(stat[doc].mean_ns);  // time.Duration(float64) truncates toward zero
+      // time.Duration(float64) truncates toward zero; beyond the int64 range cvt.rzi saturates (DESIGN.md §3 (iv))
+      const int64_t a = __double2ll_rz(stat[doc].mean_ns);
       src = a == 0 ? EVG_DS_DEFAULT : EVG_DS_HISTORY;
       avg = a == 0 ? 10 * kMinute : a; sd = a == 0 ? 0 : __double2ll_rz(stat[doc].stddev_ns);
     }
@@ -2699,15 +2755,15 @@ int evg_expected_durations_batch(evg_ctx* c, const evg_duration_rows* in, evg_du
   UP(s, c->b_rn2, in->start_ns, R, int64_t);
   UP(s, c->b_rn3, in->finish_ns, R, int64_t);
   UP(s, c->b_rn4, in->flags, R, uint8_t);
-  CK(c->b_rn5.ensure(sizeof(unsigned long long) * 4 * size_t(K)));
+  CK(c->b_rn5.ensure(sizeof(unsigned long long) * 6 * size_t(K)));
   CK(c->b_rn6.ensure(sizeof(evg_duration_stat) * size_t(K)));
   CK(c->b_err.ensure(sizeof(int) * 4));
   CK(cudaMemsetAsync(c->b_err.p, 0, sizeof(int) * 4, s));
-  CK(cudaMemsetAsync(c->b_rn5.p, 0, sizeof(unsigned long long) * 4 * size_t(K), s));
+  CK(cudaMemsetAsync(c->b_rn5.p, 0, sizeof(unsigned long long) * 6 * size_t(K), s));
   DDur x;
   x.n_rows = R; x.n_keys = K; x.key = c->b_rn0.as<int32_t>(); x.taken = c->b_rn1.as<int64_t>(); x.start = c->b_rn2.as<int64_t>();
   x.finish = c->b_rn3.as<int64_t>(); x.flags = c->b_rn4.as<uint8_t>(); x.w0 = in->window_start_ns; x.w1 = in->window_end_ns;
-  x.cnt = c->b_rn5.as<unsigned long long>(); x.sum = x.cnt + K; x.sq_lo = x.sum + K; x.sq_hi = x.sq_lo + K;
+  dur_accumulators(x, c->b_rn5.as<unsigned long long>(), K);
   launch(c, s, k_dur_sum, grid_for(R, 256), 256, 0, x, c->b_err.as<int>());
   launch(c, s, k_dur_dev, grid_for(R, 256), 256, 0, x);
   launch(c, s, k_dur_final, grid_for(K, 256), 256, 0, x, c->b_rn6.as<evg_duration_stat>());
@@ -2765,13 +2821,13 @@ int evg_resolve_durations(evg_ctx* c, const evg_duration_in* in, int64_t now_ns)
   UP(s, d.start, h ? h->start_ns : nullptr, R, int64_t);
   UP(s, d.finish, h ? h->finish_ns : nullptr, R, int64_t);
   UP(s, d.flags, h ? h->flags : nullptr, R, uint8_t);
-  CK(d.acc.ensure(sizeof(unsigned long long) * 4 * size_t(K)));
+  CK(d.acc.ensure(sizeof(unsigned long long) * 6 * size_t(K)));
   CK(d.stat.ensure(sizeof(evg_duration_stat) * size_t(K)));
   UP(s, d.pair_off, in->pair_key_off, P > 0 ? P + 1 : 0, int64_t);
   CK(d.single.ensure(sizeof(int32_t) * size_t(P)));
   CK(d.err.ensure(sizeof(int)));
   CK(cudaMemsetAsync(d.err.p, 0, sizeof(int), s));
-  if (K > 0) CK(cudaMemsetAsync(d.acc.p, 0, sizeof(unsigned long long) * 4 * size_t(K), s));
+  if (K > 0) CK(cudaMemsetAsync(d.acc.p, 0, sizeof(unsigned long long) * 6 * size_t(K), s));
   // the listed rows: six int64 columns and the key, tasks then hosts; the results: five int64 columns and the source
   CK(d.rows.ensure(sizeof(int64_t) * size_t(N)));
   CK(d.in.ensure((sizeof(int64_t) * 6 + sizeof(int32_t)) * size_t(N)));
@@ -2802,7 +2858,7 @@ int evg_resolve_durations(evg_ctx* c, const evg_duration_in* in, int64_t now_ns)
   x.n_rows = R; x.n_keys = K; x.key = d.key.as<int32_t>(); x.taken = d.taken.as<int64_t>(); x.start = d.start.as<int64_t>();
   x.finish = d.finish.as<int64_t>(); x.flags = d.flags.as<uint8_t>();
   x.w0 = h ? h->window_start_ns : 0; x.w1 = h ? h->window_end_ns : 0;
-  x.cnt = d.acc.as<unsigned long long>(); x.sum = x.cnt + K; x.sq_lo = x.sum + K; x.sq_hi = x.sq_lo + K;
+  dur_accumulators(x, d.acc.as<unsigned long long>(), K);
   launch(c, s, k_dur_sum, grid_for(R, 256), 256, 0, x, d.err.as<int>());
   launch(c, s, k_dur_dev, grid_for(R, 256), 256, 0, x);
   launch(c, s, k_dur_final, grid_for(K, 256), 256, 0, x, d.stat.as<evg_duration_stat>());

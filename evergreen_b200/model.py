@@ -514,6 +514,18 @@ def go_duration_string(d: int) -> str:
     return "-" + text if d < 0 else text
 
 
+def duration_from_float(x: float) -> int:
+    """time.Duration(float64) under DESIGN.md §3 (iv): truncation toward zero, a value beyond the int64 range saturated
+    at its end, NaN -> 0 (the device's __double2ll_rz).  Go leaves the out-of-range conversion implementation-defined."""
+    if x != x:
+        return 0
+    if x >= 2.0 ** 63:
+        return 2 ** 63 - 1
+    if x < -2.0 ** 63:
+        return -2 ** 63
+    return int(x)
+
+
 def fetch_expected_duration(t: Task, now: int, history=None):
     """Decision logic of Task.FetchExpectedDuration (model/task/task.go:3519-3590)
     with CachedDurationValue.Get (util/cached_value.go:125-145).  ``history`` is
@@ -533,10 +545,10 @@ def fetch_expected_duration(t: Task, now: int, history=None):
     else:
         if history is None:
             avg, std = (DEFAULT_TASK_DURATION, 0) if p.value == 0 else (p.value, p.std_dev)
-        elif int(history[0]) == 0:
+        elif duration_from_float(history[0]) == 0:
             avg, std = DEFAULT_TASK_DURATION, 0
         else:
-            avg, std = int(history[0]), int(history[1])
+            avg, std = duration_from_float(history[0]), duration_from_float(history[1])
         p.value, p.std_dev, p.collected_at = avg, std, now
     t.expected_duration, t.expected_duration_std_dev = avg, std
     return avg, std

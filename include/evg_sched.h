@@ -705,9 +705,12 @@ typedef struct {
 } evg_duration_rows;
 
 /* One group of the $group stage (expected_duration.go:66-76): {$avg, $stdDevPop} of TimeTaken.  count == 0 means the
- * aggregation returns no document for the key.  mean_ns = double(sum) / double(count); stddev_ns = sqrt(variance)
- * with the variance accumulated EXACTLY in integers around floor(mean) and rounded once at the end (MongoDB's
- * streaming Welford update differs from it in the last few ulps; the reference's own test allows 0.01 minutes). */
+ * aggregation returns no document for the key.  The sum S of the matched TimeTaken is exact (128 bits, so it never
+ * wraps) and so is S2 = sum (x - floor(S/count))^2 (192 bits); each is rounded once to nearest-even into a double.
+ * mean_ns = double(S) / double(count); stddev_ns = sqrt(max(double(S2) / count - (rem / count)^2, 0)) with
+ * rem = S - count * floor(S/count) (MongoDB's streaming Welford update differs from it in the last few ulps; the
+ * reference's own test allows 0.01 minutes).  Either value may lie beyond the int64 range (a mean of [INT64_MAX] is
+ * 2^63): evg_resolve_durations saturates it there (DESIGN.md §3 (iv)). */
 typedef struct {
   int64_t count;
   double mean_ns;

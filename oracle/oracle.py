@@ -132,7 +132,8 @@ def fetch_expected_duration(t: M.Task, now: int, history=None):
     p = t.duration_prediction
     lib().evo_fetch_expected_duration(p.value, p.std_dev, p.ttl, p.collected_at, t.expected_duration,
                                       t.expected_duration_std_dev, now, int(history is not None),
-                                      int(history[0]) if history else 0, int(history[1]) if history else 0,
+                                      M.duration_from_float(history[0]) if history else 0,
+                                      M.duration_from_float(history[1]) if history else 0,
                                       C.addressof(a), C.addressof(s))
     return a.value, s.value
 
@@ -334,11 +335,11 @@ def expected_durations_for_window(tasks: Sequence[M.Task], window_start: int, wi
         m0 = s // n  # floor
         rem = s - n * m0
         s2 = sum((x - m0) ** 2 for x in xs)
-        # the canonical roundings of include/evg_sched.h: double(s)/double(n); S2 as hi*2^64+lo, /n, minus (rem/n)^2
+        # the canonical roundings of include/evg_sched.h: double(s)/double(n); double(S2)/n minus (rem/n)^2, where
+        # Python's int -> float conversions are the one round-to-nearest-even of the exact integers
         mean = float(s) / float(n)
-        s2f = float(s2 >> 64) * 18446744073709551616.0 + float(s2 & ((1 << 64) - 1))
         fr = float(rem) / float(n)
-        var = max(s2f / float(n) - fr * fr, 0.0)
+        var = max(float(s2) / float(n) - fr * fr, 0.0)
         exact_std = math.sqrt(Fraction(n * sum(x * x for x in xs) - s * s, n * n))  # reference value, for the tolerance test
         out[k] = (n, mean, math.sqrt(var), exact_std)
     return out

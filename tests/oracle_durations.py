@@ -42,12 +42,17 @@ def window_documents(finished: Sequence[M.Task], name: str, project: str, build_
     for n, xs in groups.items():
         k, s = len(xs), sum(xs)
         m0 = s // k
-        rem = s - k * m0
         s2 = sum((x - m0) ** 2 for x in xs)
-        s2f = float(s2 >> 64) * 18446744073709551616.0 + float(s2 & ((1 << 64) - 1))
-        fr = float(rem) / float(k)
-        out.append((n, float(s) / float(k), math.sqrt(max(s2f / float(k) - fr * fr, 0.0))))
+        out.append((n,) + canonical_stats(k, s, s2))
     return out
+
+
+def canonical_stats(n: int, s: int, s2: int):
+    """($avg, $stdDevPop) of a key from its exact count n, sum s and S2 = sum (x - floor(s/n))^2, with the roundings
+    of include/evg_sched.h: float(s) and float(s2) are each one round-to-nearest-even of the exact integer."""
+    rem = s - n * (s // n)
+    fr = float(rem) / float(n)
+    return float(s) / float(n), math.sqrt(max(float(s2) / float(n) - fr * fr, 0.0))
 
 
 def fetch_expected_duration(t: M.Task, now: int, finished: Sequence[M.Task]) -> dict:
@@ -66,9 +71,9 @@ def fetch_expected_duration(t: M.Task, now: int, finished: Sequence[M.Task]) -> 
             source = DEFAULT if value == 0 else PREVIOUS
             avg, std = (M.DEFAULT_TASK_DURATION, 0) if value == 0 else (value, pstd)
         else:
-            a = int(docs[0][1])  # time.Duration(float64): truncation toward zero
+            a = M.duration_from_float(docs[0][1])  # time.Duration(float64): truncation toward zero, saturated
             source = DEFAULT if a == 0 else HISTORY
-            avg, std = (M.DEFAULT_TASK_DURATION, 0) if a == 0 else (a, int(docs[0][2]))
+            avg, std = (M.DEFAULT_TASK_DURATION, 0) if a == 0 else (a, M.duration_from_float(docs[0][2]))
         value, pstd, coll = avg, std, now  # cached_value.go:139-142
     return dict(avg=avg, std=std, value=value, pred_std=pstd, collected=coll, ttl=ttl, source=source,
                 persisted=source != FRESH)
@@ -120,6 +125,18 @@ def key_stats_np(rows):
     return cnt, np.where(has, mean, 0.0), np.where(has, std, 0.0)
 
 
+def duration_from_float_np(x):
+    """model.duration_from_float over an array (numpy's astype of a value beyond the int64 range is undefined)."""
+    import numpy as np
+    x = np.asarray(x, np.float64)
+    out = np.zeros(x.shape, np.int64)
+    inside = (x >= -2.0 ** 63) & (x < 2.0 ** 63)
+    out[inside] = np.trunc(x[inside]).astype(np.int64)
+    out[x >= 2.0 ** 63] = I64_MAX
+    out[x < -2.0 ** 63] = -I64_MAX - 1
+    return out
+
+
 def resolve_np(rows, pair_key_off, cache, now: int):
     """evg_resolve_durations' per-row results for a DurationCache -> dict of avg_ns, std_ns, value_ns, pred_std_ns,
     collected_ns, source (listed-row order)."""
@@ -148,8 +165,8 @@ def resolve_np(rows, pair_key_off, cache, now: int):
     backfill = (value == 0) & (e != 0)
     fresh = ~backfill & (age < ttl)
     stale = ~backfill & ~fresh
-    a = np.where(doc >= 0, np.trunc(mean[np.maximum(doc, 0)]), 0).astype(np.int64) if mean.shape[0] else np.zeros_like(key)
-    sd = np.where(doc >= 0, np.trunc(std[np.maximum(doc, 0)]), 0).astype(np.int64) if std.shape[0] else np.zeros_like(key)
+    a = np.where(doc >= 0, duration_from_float_np(mean[np.maximum(doc, 0)]), 0) if mean.shape[0] else np.zeros_like(key)
+    sd = np.where(doc >= 0, duration_from_float_np(std[np.maximum(doc, 0)]), 0) if std.shape[0] else np.zeros_like(key)
     src = np.where(backfill, BACKFILL, FRESH)
     src = np.where(stale & (doc < 0), np.where(value == 0, DEFAULT, PREVIOUS), src)
     src = np.where(stale & (doc >= 0), np.where(a == 0, DEFAULT, HISTORY), src)
