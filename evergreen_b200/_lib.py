@@ -337,6 +337,8 @@ SYMBOLS = {
     "evg_plan_aliases": (C.c_int, [_P, _P, _P, C.c_int32, C.c_int64, _P]),
     "evg_download_alias_map": (C.c_int, [_P, _P, _P]),
     "evg_intern_columns": (C.c_int, [_P, _P, C.c_int32]),
+    "evg_intern_batch": (C.c_int, [_P, _P, _P]),
+    "evg_upload_strings": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P]),
     "evg_run_resident": (C.c_int, [_P, C.c_int64, C.c_uint32]),
     "evg_download": (C.c_int, [_P, _P, _P]),
     "evg_download_queue": (C.c_int, [_P, C.c_int32, _P, _P, C.c_int64]),

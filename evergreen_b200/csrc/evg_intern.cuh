@@ -1,0 +1,168 @@
+// evg_intern.cuh -- evg_intern_columns on the device (evg_intern_batch, evg_upload_strings): task-group keys, versions
+// and task ids to dense first-appearance ids per distro, dependency ids to queue indices.
+//
+// One warp per string.  The lanes read 32 consecutive bytes of the column a step (one or two sectors) and fold each
+// (position, byte) through a 64-bit mix; the terms are summed, so a string's hash is one warp reduction.  Each key
+// column has an open-addressing table in global memory whose slot is one 64-bit word, hash << 32 | the row that
+// claimed it, published by one CAS.  A prober whose hash matches compares its bytes with that row's (the warp again),
+// so equal hashes never decide equality and no lane waits on a half-written slot.  The distro is mixed into the hash
+// and a claimant must lie in the prober's distro, so one table serves every distro.  atomicMin gives each distinct key
+// the first row that carries it: which row claimed a slot depends on atomic order, the first row does not.
+#pragma once
+
+struct DStr {  // an evg_str_col staged on the device; n_bytes = off[n], the bytes staged
+  const uint8_t* bytes;
+  const int64_t* off;
+  int64_t n_bytes;
+};
+
+struct InView {
+  int64_t T, E;
+  int32_t D;
+  const int64_t* task_off;
+  DStr grp, ver, id, dep;  // group keys, versions, task ids (rows), dependency ids (edges)
+  const int64_t* dep_off;
+  const int32_t* gmh;      // Task.TaskGroupMaxHosts per row
+  uint32_t hmask;          // EVG_INTERN_HASH_BITS: the hash is masked to this many bits
+  uint64_t cap;            // slots per key column (a power of two, at least twice the rows)
+  unsigned long long* key; // three regions of cap slots: group keys, versions, task ids
+  uint32_t* first;         // per slot: the first row whose key is there
+};
+enum : int { kInGroup = 0, kInVersion = 1, kInId = 2 };
+// k_in_keys / k_in_deps error bits: a dep_off row, then a bad string row of each column
+constexpr int kInErrDepOff = 1, kInErrGroupOff = 2, kInErrVersionOff = 4, kInErrIdOff = 8, kInErrDepIdOff = 16;
+constexpr unsigned long long kInEmpty = ~0ull;
+
+__device__ __forceinline__ uint64_t in_mix(uint64_t x) {  // MurmurHash3's 64-bit finaliser
+  x ^= x >> 33;
+  x *= 0xFF51AFD7ED558CCDull;
+  x ^= x >> 33;
+  x *= 0xC4CEB9FE1A85EC53ull;
+  return x ^ (x >> 33);
+}
+__device__ __forceinline__ bool in_row_bad(const DStr& s, int64_t o0, int64_t o1) { return o0 < 0 || o1 < o0 || o1 > s.n_bytes; }
+
+// Hash of bytes [o0, o0 + n) of s in distro d, the same on every lane.
+__device__ __forceinline__ uint32_t in_hash(const DStr& s, int64_t o0, int64_t n, int d, uint32_t hmask, int lane) {
+  uint64_t acc = 0;
+  for (int64_t i = lane; i < n; i += 32) acc += in_mix(((uint64_t(i) << 8) | s.bytes[o0 + i]) + 0x9E3779B97F4A7C15ull);
+  for (int k = 16; k > 0; k >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, k);
+  return uint32_t(in_mix(acc ^ (uint64_t(n) * 0xD6E8FEB86659FD93ull) ^ (uint64_t(uint32_t(d)) << 40)) >> 32) & hmask;
+}
+
+// Bytes [a0, a0 + n) of s equal bytes [b0, b0 + n) of k, the same on every lane.
+__device__ __forceinline__ bool in_same(const DStr& s, int64_t a0, const DStr& k, int64_t b0, int64_t n, int lane) {
+  for (int64_t i = lane; i - lane < n; i += 32)
+    if (__any_sync(0xffffffffu, i < n && s.bytes[a0 + i] != k.bytes[b0 + i])) return false;
+  return true;
+}
+
+// Slot (an index of v.key / v.first) of the key bytes [o0, o0 + n) of s, hash h, in column r among the rows [a, b) of
+// its distro.  With `row` >= 0 an absent key is inserted, claimed by `row`; otherwise absent is -1.  Warp-uniform.
+__device__ int64_t in_probe(const InView& v, int r, const DStr& s, int64_t o0, int64_t n, uint32_t h, int64_t row, int64_t a,
+                            int64_t b, int lane) {
+  const DStr& k = r == kInGroup ? v.grp : r == kInVersion ? v.ver : v.id;
+  unsigned long long* key = v.key + uint64_t(r) * v.cap;
+  const unsigned long long mine = (uint64_t(h) << 32) | uint64_t(row);
+  for (uint64_t slot = h & (v.cap - 1);; slot = (slot + 1) & (v.cap - 1)) {
+    unsigned long long w = 0;
+    if (lane == 0) {
+      w = key[slot];
+      if (w == kInEmpty && row >= 0) w = atomicCAS(key + slot, kInEmpty, mine);  // kInEmpty back: this row claimed it
+    }
+    w = __shfl_sync(0xffffffffu, w, 0);
+    if (w == kInEmpty) return row >= 0 ? int64_t(uint64_t(r) * v.cap + slot) : -1;
+    if (uint32_t(w >> 32) != h) continue;
+    const int64_t q = int64_t(uint32_t(w));  // the claimant: its row passed in_row_bad before it claimed
+    if (q < a || q >= b) continue;
+    const int64_t q0 = k.off[q];
+    if (k.off[q + 1] - q0 == n && in_same(s, o0, k, q0, n, lane)) return int64_t(uint64_t(r) * v.cap + slot);
+  }
+}
+
+// A warp per row: its group key (none when empty), version and task id into their tables; the row's group and version
+// slots.  A string row outside its byte column raises its column's error bit and gets no slot.
+__global__ void __launch_bounds__(256) k_in_keys(InView v, int64_t* __restrict__ gslot, int64_t* __restrict__ vslot, int* err) {
+  const int64_t t = (int64_t(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (t >= v.T) return;
+  const int d = find_distro(v.task_off, 0, v.D - 1, t);
+  const int64_t a = v.task_off[d], b = v.task_off[d + 1];
+  for (int r = kInGroup; r <= kInId; r++) {
+    const DStr& s = r == kInGroup ? v.grp : r == kInVersion ? v.ver : v.id;
+    const int64_t o0 = s.off[t], o1 = s.off[t + 1];
+    int64_t slot = -1;
+    if (in_row_bad(s, o0, o1)) {
+      if (lane == 0) atomicOr(err, kInErrGroupOff << r);
+    } else if (r != kInGroup || o1 > o0) {
+      slot = in_probe(v, r, s, o0, o1 - o0, in_hash(s, o0, o1 - o0, d, v.hmask, lane), t, a, b, lane);
+      if (lane == 0) atomicMin(v.first + slot, uint32_t(t));
+    }
+    if (lane == 0 && r == kInGroup) gslot[t] = slot;
+    if (lane == 0 && r == kInVersion) vslot[t] = slot;
+  }
+}
+
+// A warp per row: each DependsOn id looked up among the task ids of the row's distro; res[e] = the distro-local index of
+// the first task with that id, -1 when none; cnt[t] = the row's resolved edges.  The row of dep_off is checked here.
+__global__ void __launch_bounds__(256) k_in_deps(InView v, int32_t* __restrict__ res, int32_t* __restrict__ cnt, int* err) {
+  const int64_t t = (int64_t(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (t >= v.T) return;
+  const int64_t e0 = v.dep_off[t], e1 = v.dep_off[t + 1];
+  int32_t kept = 0;
+  if (e0 < 0 || e1 < e0 || e1 > v.E) {
+    if (lane == 0) atomicOr(err, kInErrDepOff);
+  } else if (e1 > e0) {
+    const int d = find_distro(v.task_off, 0, v.D - 1, t);
+    const int64_t a = v.task_off[d], b = v.task_off[d + 1];
+    for (int64_t e = e0; e < e1; e++) {
+      const int64_t o0 = v.dep.off[e], o1 = v.dep.off[e + 1];
+      int32_t j = -1;
+      if (in_row_bad(v.dep, o0, o1)) {
+        if (lane == 0) atomicOr(err, kInErrDepIdOff);
+      } else {
+        const int64_t slot = in_probe(v, kInId, v.dep, o0, o1 - o0, in_hash(v.dep, o0, o1 - o0, d, v.hmask, lane), -1, a, b, lane);
+        if (slot >= 0) j = int32_t(int64_t(v.first[slot]) - a);
+      }
+      if (lane == 0) res[e] = j;
+      kept += j >= 0;
+    }
+  }
+  if (lane == 0) cnt[t] = kept;
+}
+
+// Per row, after k_al_flag and the scans of its flags (pg, pv): the dense group and version ids, the group tables from
+// each group's first member, and the lowest row whose TaskGroupMaxHosts differs from its group's first member's.
+__global__ void __launch_bounds__(256) k_in_ids(InView v, const int64_t* __restrict__ gslot, const int64_t* __restrict__ vslot,
+                                                const int64_t* __restrict__ pg, const int64_t* __restrict__ pv, int32_t* __restrict__ gid,
+                                                int32_t* __restrict__ vid, int32_t* __restrict__ gmax, int64_t* __restrict__ gfirst,
+                                                unsigned long long* bad_row) {
+  const int64_t t = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  const int d = block_find_distro(v.task_off, v.D, t, v.T);
+  if (d < 0) return;
+  const int64_t a = v.task_off[d];
+  int32_t g = -1;
+  if (gslot[t] >= 0) {
+    const int64_t f = v.first[gslot[t]];
+    g = int32_t(pg[f] - pg[a]);
+    if (f == t) {
+      gmax[pg[t]] = v.gmh[t];
+      gfirst[pg[t]] = t;
+    } else if (v.gmh[t] != v.gmh[f]) {
+      atomicMin(bad_row, (unsigned long long)t);
+    }
+  }
+  gid[t] = g;
+  vid[t] = int32_t(pv[v.first[vslot[t]]] - pv[a]);
+}
+
+// Per row: its resolved dependencies, in DependsOn order, at dep_off_out[t].
+__global__ void __launch_bounds__(256) k_in_edges(InView v, const int32_t* __restrict__ res, const int64_t* __restrict__ dep_off_out,
+                                                  int32_t* __restrict__ dep_idx) {
+  const int64_t t = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (t >= v.T) return;
+  int64_t w = dep_off_out[t];
+  for (int64_t e = v.dep_off[t]; e < v.dep_off[t + 1]; e++)
+    if (res[e] >= 0) dep_idx[w++] = res[e];
+}

@@ -30,6 +30,7 @@
 //   k_dur_commit          the resolved durations into the resident columns, unless the call found an error
 //   k_host_job            hostAllocatorJob.Run past the allocator: single-task bypass, report, drawdown (units/host_allocator.go:180-425)
 //   k_next_verdict/serve  the DAG dispatcher's FindNextTask, a warp per distro (model/task_queue_service_dependency.go:258-692)
+//   k_in_*                evg_intern_columns on the device: string keys to dense ids, dependency ids to queue indices
 // No CPU fallback exists in this file: without a device every entry point fails.
 #include <cuda_runtime.h>
 #include <stdarg.h>
@@ -394,6 +395,7 @@ __device__ __forceinline__ uint32_t pair_task(const DTasks& T, const DWork& W, u
 #include "evg_dag.cuh"
 #include "evg_next.cuh"
 #include "evg_estimate.cuh"
+#include "evg_intern.cuh"
 
 // --------------------------------------------------------------------------
 // kernels (general path: any distro size)
@@ -1349,10 +1351,11 @@ struct TaskCols {
       return EVG_OK;
     });
   }
-  // Rows [t0, t0 + n) of t's columns from host memory into the same rows here, on s.
-  int copy_rows(const evg_task_soa* t, int64_t t0, int64_t n, cudaStream_t s) {
+  // Rows [t0, t0 + n) of t's columns from host memory into the same rows here, on s; without `ids`, group_id and
+  // version_id are not copied.
+  int copy_rows(const evg_task_soa* t, int64_t t0, int64_t n, cudaStream_t s, bool ids = true) {
     return each([&](auto b, auto f, const char*) -> int {
-      if (n > 0) CK(cudaMemcpyAsync(static_cast<char*>((this->*b).p) + elem(f) * t0, t->*f + t0, elem(f) * n, cudaMemcpyHostToDevice, s));
+      if (n > 0 && (ids || !is_id(b))) CK(cudaMemcpyAsync(static_cast<char*>((this->*b).p) + elem(f) * t0, t->*f + t0, elem(f) * n, cudaMemcpyHostToDevice, s));
       return EVG_OK;
     });
   }
@@ -1509,6 +1512,13 @@ struct evg_ctx {
   // row's timeToCompletion and whether it counts, their scan, the packed pools (two copies: the merge sort's), the
   // queues' offsets and durations, the launch list and the outputs
   struct { DevBuf kind, expected, dispatch, host_off, ttc, used, pos, pool[2], pool_off, item_off, dur, list, start, hosts_used; } es;
+  // evg_intern_batch / evg_upload_strings (the first call allocates these): the staged string columns, the key tables,
+  // each row's group and version slots, their first-appearance flags and scans, the resolved dependencies and their
+  // counts, the per-distro samples and the error words; then evg_intern_batch's outputs
+  struct {
+    DevBuf task_off, gmh, dep_off, bytes[4], off[4], key, first, gslot, vslot, fg, fv, pg, pv, res, cnt, samp, err;
+    DevBuf gid, vid, gmax, gfirst, out_dep_off, out_dep_idx;
+  } in;
   DevBuf b_err;
   DevBuf b_scansum;  // scan_counts' per-block sums
   DevBuf b_route, b_unitv, b_unita, b_unitn, b_unitmask;
@@ -3990,6 +4000,264 @@ int evg_intern_columns(const evg_string_cols* in, evg_intern_out* out, int32_t t
   }
   return EVG_OK;
 }
+
+// --------------------------------------------------------------------------
+// evg_intern_batch / evg_upload_strings: evg_intern_columns on the device (evg_intern.cuh)
+// --------------------------------------------------------------------------
+// The string columns in InView order (group keys, versions, task ids, dependency ids) and their names in messages.
+static const char* const kInColName[4] = {"group_key.off", "version.off", "id.off", "dep_id.off"};
+static void intern_cols(const evg_string_cols* in, const evg_str_col* cols[4], int64_t rows[4]) {
+  const int64_t T = in->n_tasks;
+  cols[0] = &in->group_key; cols[1] = &in->version; cols[2] = &in->id; cols[3] = &in->dep_id;
+  rows[0] = rows[1] = rows[2] = T;
+  rows[3] = T > 0 ? in->dep_off[T] : 0;
+}
+
+// What the host checks of `in` before any device work: what evg_intern_columns checks, plus what staging needs -- each
+// byte column is staged up to its last offset (the kernels check every row against it) and rows fit 31 bits.
+static int intern_check(const char* who, const evg_string_cols* in) {
+  const int64_t T = in->n_tasks;
+  const int32_t D = in->n_distros;
+  if (T < 0 || D < 0) return fail(EVG_ERR_INVALID, "%s: negative sizes", who);
+  if (D == 0) return T == 0 ? EVG_OK : fail(EVG_ERR_INVALID, "%s: tasks without distros", who);
+  if (!in->task_off) return fail(EVG_ERR_INVALID, "%s: null task_off", who);
+  const int rc = check_offsets(in->task_off, D, T, who, "task_off");
+  if (rc != EVG_OK || T == 0) return rc;
+  if (T > (int64_t(1) << 31) - 2) return fail(EVG_ERR_INVALID, "%s: %lld tasks exceed 2^31-2", who, (long long)T);
+  if (!in->id.off || !in->version.off || !in->group_key.off || !in->group_max_hosts || !in->dep_off)
+    return fail(EVG_ERR_INVALID, "%s: null column", who);
+  if (in->dep_off[0] != 0 || in->dep_off[T] < 0) return check_offsets(in->dep_off, T, -1, who, "dep_off");
+  const evg_str_col* cols[4];
+  int64_t rows[4];
+  intern_cols(in, cols, rows);
+  if (rows[3] > 0 && !in->dep_id.off) return fail(EVG_ERR_INVALID, "%s: null dependency columns", who);
+  for (int k = 0; k < 4; k++) {
+    if (rows[k] == 0) continue;
+    const int64_t nb = cols[k]->off[rows[k]];
+    if (nb < 0) return check_offsets(cols[k]->off, rows[k], -1, who, kInColName[k]);
+    if (nb > 0 && !cols[k]->bytes) return fail(EVG_ERR_INVALID, "%s: null bytes for %s", who, kInColName[k]);
+  }
+  return EVG_OK;
+}
+
+// What the host reads back of an interned tick: O(n_distros) values.
+struct InternSizes {
+  std::vector<int64_t> group_off;  // D + 1
+  std::vector<int32_t> n_versions; // D
+  std::vector<int64_t> edge_off;   // D + 1: the in-queue dep_off at the distro boundaries
+};
+
+// The strings of `in` (passed by intern_check, n_tasks > 0) interned on c->stream: group and version ids into gid / vid,
+// the in-queue edges into dep_off / dep_idx, the group tables into c->in.gmax / c->in.gfirst (one entry per group slot),
+// the per-distro sizes into *z.  Every buffer is sized before the first launch, so a tick too large for the device
+// fails with EVG_ERR_NOMEM before any work and leaves the context usable.  Three syncs: the row checks, the sizes, the end.
+static int intern_strings(evg_ctx* c, const char* who, const evg_string_cols* in, DevBuf& gid, DevBuf& vid, DevBuf& dep_off,
+                          DevBuf& dep_idx, InternSizes* z) {
+  cudaStream_t s = c->stream;
+  auto& b = c->in;
+  const int64_t T = in->n_tasks;
+  const int32_t D = in->n_distros;
+  const evg_str_col* cols[4];
+  int64_t rows[4], nb[4];
+  intern_cols(in, cols, rows);
+  const int64_t E = rows[3];
+  for (int k = 0; k < 4; k++) nb[k] = rows[k] > 0 ? cols[k]->off[rows[k]] : 0;
+  uint64_t cap = 64;
+  while (cap < 2 * uint64_t(T)) cap <<= 1;  // at most T keys a column: load factor <= 1/2
+  {
+    cudaError_t e = cudaSuccess;
+    auto need = [&](DevBuf& x, int64_t bytes) { if (e == cudaSuccess) e = x.ensure(size_t(std::max<int64_t>(bytes, 1))); };
+    need(b.task_off, 8 * (D + 1)); need(b.gmh, 4 * T); need(b.dep_off, 8 * (T + 1));
+    for (int k = 0; k < 4; k++) { need(b.off[k], 8 * (rows[k] + 1)); need(b.bytes[k], nb[k]); }
+    need(b.key, 8 * 3 * int64_t(cap)); need(b.first, 4 * 3 * int64_t(cap));
+    need(b.gslot, 8 * T); need(b.vslot, 8 * T); need(b.fg, 4 * T); need(b.fv, 4 * T); need(b.pg, 8 * (T + 1)); need(b.pv, 8 * (T + 1));
+    need(b.res, 4 * E); need(b.cnt, 4 * T); need(b.samp, 8 * 3 * (D + 1)); need(b.err, 16);
+    need(b.gmax, 4 * T); need(b.gfirst, 8 * T); need(c->b_scansum, 8 * ((T + 1023) / 1024 + 1));
+    need(gid, 4 * (T + kColPad)); need(vid, 4 * (T + kColPad)); need(dep_off, 8 * (T + 1 + kColPad)); need(dep_idx, 4 * (E + kColPad));
+    if (e != cudaSuccess) {
+      cudaGetLastError();  // a failed allocation is not sticky: clear it so that the next call starts clean
+      return fail(e == cudaErrorMemoryAllocation ? EVG_ERR_NOMEM : EVG_ERR_CUDA, "%s: %s while sizing %lld tasks", who,
+                  cudaGetErrorString(e), (long long)T);
+    }
+  }
+  // ---- stage the columns; the tables empty
+  CK(cudaMemcpyAsync(b.task_off.p, in->task_off, sizeof(int64_t) * size_t(D + 1), cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(b.gmh.p, in->group_max_hosts, sizeof(int32_t) * size_t(T), cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(b.dep_off.p, in->dep_off, sizeof(int64_t) * size_t(T + 1), cudaMemcpyHostToDevice, s));
+  for (int k = 0; k < 4; k++) {
+    if (rows[k] > 0) CK(cudaMemcpyAsync(b.off[k].p, cols[k]->off, sizeof(int64_t) * size_t(rows[k] + 1), cudaMemcpyHostToDevice, s));
+    if (nb[k] > 0) CK(cudaMemcpyAsync(b.bytes[k].p, cols[k]->bytes, size_t(nb[k]), cudaMemcpyHostToDevice, s));
+  }
+  CK(cudaMemsetAsync(b.key.p, 0xFF, sizeof(uint64_t) * 3 * cap, s));
+  CK(cudaMemsetAsync(b.first.p, 0xFF, sizeof(uint32_t) * 3 * cap, s));
+  CK(cudaMemsetAsync(b.err.p, 0, sizeof(int), s));
+  CK(cudaMemsetAsync(b.err.as<char>() + 8, 0xFF, sizeof(uint64_t), s));  // the lowest bad row: none yet
+  InView v;
+  memset(&v, 0, sizeof(v));
+  v.T = T; v.E = E; v.D = D;
+  v.task_off = b.task_off.as<int64_t>();
+  DStr* dst[4] = {&v.grp, &v.ver, &v.id, &v.dep};
+  for (int k = 0; k < 4; k++) *dst[k] = DStr{b.bytes[k].as<uint8_t>(), b.off[k].as<int64_t>(), nb[k]};
+  v.dep_off = b.dep_off.as<int64_t>();
+  v.gmh = b.gmh.as<int32_t>();
+  const char* bits_env = getenv("EVG_INTERN_HASH_BITS");  // test hook: fewer hash bits force collisions; 32 when unset
+  const int bits = bits_env ? std::max(0, std::min(32, atoi(bits_env))) : 32;
+  v.hmask = bits >= 32 ? 0xFFFFFFFFu : (1u << bits) - 1u;
+  v.cap = cap;
+  v.key = b.key.as<unsigned long long>();
+  v.first = b.first.as<uint32_t>();
+  int* err = b.err.as<int>();
+  int64_t *gslot = b.gslot.as<int64_t>(), *vslot = b.vslot.as<int64_t>(), *pg = b.pg.as<int64_t>(), *pv = b.pv.as<int64_t>();
+  // ---- 1. every key into its table, every dependency id looked up; the row checks cross to the host
+  launch(c, s, k_in_keys, grid_for(T * 32, 256), 256, 0, v, gslot, vslot, err);
+  launch(c, s, k_in_deps, grid_for(T * 32, 256), 256, 0, v, b.res.as<int32_t>(), b.cnt.as<int32_t>(), err);
+  int bad = 0;
+  CK(cudaMemcpyAsync(&bad, err, sizeof(int), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  if (bad & kInErrDepOff) return check_offsets(in->dep_off, T, -1, who, "dep_off");
+  for (int k = 0; k < 4; k++)
+    if (bad & (kInErrGroupOff << k)) {
+      const int rc = check_offsets(cols[k]->off, rows[k], -1, who, kInColName[k]);
+      return rc != EVG_OK ? rc : fail(EVG_ERR_INVALID, "%s: %s breaks its byte column", who, kInColName[k]);
+    }
+  // ---- 2. first-appearance flags and their scans number each distro's groups and versions; ids, group tables, edge counts
+  launch(c, s, k_al_flag, grid_for(T, 256), 256, 0, T, gslot, vslot, v.first, b.fg.as<int32_t>(), b.fv.as<int32_t>());
+  CK(scan_counts(c, b.fg.as<int32_t>(), T, pg));
+  CK(scan_counts(c, b.fv.as<int32_t>(), T, pv));
+  launch(c, s, k_in_ids, grid_for(T, 256), 256, 0, v, gslot, vslot, pg, pv, gid.as<int32_t>(), vid.as<int32_t>(), b.gmax.as<int32_t>(),
+         b.gfirst.as<int64_t>(), reinterpret_cast<unsigned long long*>(b.err.as<char>() + 8));
+  CK(scan_counts(c, b.cnt.as<int32_t>(), T, dep_off.as<int64_t>()));
+  // ---- 3. groups, versions and edges at the distro boundaries, and the lowest bad row, cross to the host
+  int64_t* samp = b.samp.as<int64_t>();
+  launch(c, s, k_gather_i64, grid_for(D + 1, 256), 256, 0, pg, v.task_off, samp, D + 1);
+  launch(c, s, k_gather_i64, grid_for(D + 1, 256), 256, 0, pv, v.task_off, samp + (D + 1), D + 1);
+  launch(c, s, k_gather_i64, grid_for(D + 1, 256), 256, 0, dep_off.as<int64_t>(), v.task_off, samp + 2 * (D + 1), D + 1);
+  std::vector<int64_t> h(3 * size_t(D + 1));
+  unsigned long long bad_row = 0;
+  CK(cudaMemcpyAsync(h.data(), samp, sizeof(int64_t) * h.size(), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(&bad_row, b.err.as<char>() + 8, sizeof(bad_row), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  if (bad_row != kInEmpty)
+    return fail(EVG_ERR_INVALID, "%s: task group of row %lld: TaskGroupMaxHosts differs between members", who, (long long)bad_row);
+  z->group_off.assign(h.begin(), h.begin() + (D + 1));
+  z->edge_off.assign(h.begin() + 2 * (D + 1), h.end());
+  z->n_versions.resize(size_t(D));
+  for (int32_t d = 0; d < D; d++) z->n_versions[size_t(d)] = int32_t(h[size_t(D + 1 + d + 1)] - h[size_t(D + 1 + d)]);
+  // ---- 4. the kept edges in DependsOn order
+  if (z->edge_off[size_t(D)] > 0)
+    launch(c, s, k_in_edges, grid_for(T, 256), 256, 0, v, b.res.as<int32_t>(), dep_off.as<int64_t>(), dep_idx.as<int32_t>());
+  CK(cudaGetLastError());
+  return EVG_OK;
+}
+
+// Device to host on c->stream when both ends exist.
+#define D2H_IF(dst, src, count, type)                                                                                       \
+  do {                                                                                                                      \
+    if ((dst) && (count) > 0) CK(cudaMemcpyAsync((dst), (src), sizeof(type) * size_t(count), cudaMemcpyDeviceToHost, c->stream)); \
+  } while (0)
+
+int evg_intern_batch(evg_ctx* c, const evg_string_cols* in, evg_intern_out* out) {
+  ENTER(c, "evg_intern_batch");
+  c->launches = 0;
+  if (!in || !out) return fail(EVG_ERR_INVALID, "%s: null argument", who);
+  int rc = intern_check(who, in);
+  if (rc != EVG_OK) return rc;
+  const int64_t T = in->n_tasks;
+  const int32_t D = in->n_distros;
+  if (!out->group_off || (D > 0 && !out->n_versions)) return fail(EVG_ERR_INVALID, "%s: null distro arrays", who);
+  if (T > 0 && (!out->group_id || !out->version_id || !out->group_max_hosts || !out->group_first || !out->dep_off ||
+                (in->dep_off[T] > 0 && !out->dep_idx)))
+    return fail(EVG_ERR_INVALID, "%s: null output column", who);
+  if (T == 0) {  // what evg_intern_columns writes for a tick without tasks: no dep_off row
+    for (int32_t d = 0; d <= D; d++) out->group_off[d] = 0;
+    for (int32_t d = 0; d < D; d++) out->n_versions[d] = 0;
+    return EVG_OK;
+  }
+  auto& b = c->in;
+  InternSizes z;
+  rc = intern_strings(c, who, in, b.gid, b.vid, b.out_dep_off, b.out_dep_idx, &z);
+  if (rc != EVG_OK) return rc;
+  const int64_t G = z.group_off[size_t(D)], En = z.edge_off[size_t(D)];
+  memcpy(out->group_off, z.group_off.data(), sizeof(int64_t) * size_t(D + 1));
+  memcpy(out->n_versions, z.n_versions.data(), sizeof(int32_t) * size_t(D));
+  D2H_IF(out->group_id, b.gid.p, T, int32_t);
+  D2H_IF(out->version_id, b.vid.p, T, int32_t);
+  D2H_IF(out->group_max_hosts, b.gmax.p, G, int32_t);
+  D2H_IF(out->group_first, b.gfirst.p, G, int64_t);
+  D2H_IF(out->dep_off, b.out_dep_off.p, T + 1, int64_t);
+  D2H_IF(out->dep_idx, b.out_dep_idx.p, En, int32_t);
+  CK(cudaStreamSynchronize(c->stream));
+  return EVG_OK;
+}
+
+int evg_upload_strings(evg_ctx* c, const evg_task_soa* tasks, const evg_string_cols* strings, const evg_distro_cfg* cfg,
+                       const evg_host_soa* hosts, const int64_t* host_off, const evg_alloc_cfg* acfg, evg_intern_out* out) {
+  ENTER(c, "evg_upload_strings");
+  c->launches = 0;
+  // ---- every check the host can make, before anything resident changes
+  if (!tasks || !strings || !out) return fail(EVG_ERR_INVALID, "%s: null argument", who);
+  int rc = intern_check(who, strings);
+  if (rc != EVG_OK) return rc;
+  const int64_t T = strings->n_tasks;
+  const int32_t D = strings->n_distros;
+  if (tasks->n_tasks != T) return fail(EVG_ERR_INVALID, "%s: tasks has %lld rows, strings %lld", who, (long long)tasks->n_tasks, (long long)T);
+  if (tasks->group_id || tasks->version_id || tasks->dep_off || tasks->dep_idx)
+    return fail(EVG_ERR_INVALID, "%s: tasks->group_id, version_id, dep_off and dep_idx come from the strings and must be NULL", who);
+  if (T > 0 && TaskCols::missing(tasks, /*ids=*/false)) return fail(EVG_ERR_INVALID, "%s: null task column", who);
+  if (!out->group_off || (D > 0 && (!out->n_versions || !cfg))) return fail(EVG_ERR_INVALID, "%s: null cfg / output", who);
+  for (int32_t d = 0; d < D; d++)
+    if (strings->task_off[d + 1] - strings->task_off[d] > kMaxTasksPerDistro)
+      return fail(EVG_ERR_INVALID, "%s: distro %d holds %lld tasks (max %lld)", who, d,
+                  (long long)(strings->task_off[d + 1] - strings->task_off[d]), (long long)kMaxTasksPerDistro);
+  // ---- from here the previous tick is gone: the seven numeric columns and the interned ids fill the shadow set
+  cudaStream_t s = c->stream;
+  auto& e = c->ed;
+  drop_tick(c);
+  rc = e.out.size(T, s, /*zero_pad=*/true);
+  if (rc == EVG_OK) rc = e.out.copy_rows(tasks, 0, T, s, /*ids=*/false);
+  if (rc != EVG_OK) {
+    cudaGetLastError();  // as in intern_strings: a failed allocation leaves the context usable
+    return rc;
+  }
+  InternSizes z;
+  z.group_off.assign(size_t(D) + 1, 0);
+  z.edge_off.assign(size_t(D) + 1, 0);
+  z.n_versions.assign(size_t(D), 0);
+  if (T > 0) {
+    rc = intern_strings(c, who, strings, e.out.gid, e.out.vid, e.dep_off, e.dep_idx, &z);
+    if (rc != EVG_OK) return rc;
+  }
+  // ---- the group slots' max hosts (the upload stages them from the host) and what the caller asked for
+  const int64_t G = z.group_off[size_t(D)], En = z.edge_off[size_t(D)];
+  std::vector<int32_t> gmax(size_t(G) + 1);
+  D2H_IF(gmax.data(), c->in.gmax.p, G, int32_t);
+  D2H_IF(out->group_max_hosts, c->in.gmax.p, G, int32_t);
+  D2H_IF(out->group_first, c->in.gfirst.p, G, int64_t);
+  D2H_IF(out->group_id, e.out.gid.p, T, int32_t);
+  D2H_IF(out->version_id, e.out.vid.p, T, int32_t);
+  D2H_IF(out->dep_off, e.dep_off.p, T > 0 ? T + 1 : 0, int64_t);
+  D2H_IF(out->dep_idx, e.dep_idx.p, En, int32_t);
+  CK(cudaStreamSynchronize(s));
+  memcpy(out->group_off, z.group_off.data(), sizeof(int64_t) * size_t(D + 1));
+  if (D > 0) memcpy(out->n_versions, z.n_versions.data(), sizeof(int32_t) * size_t(D));
+  std::vector<evg_distro_cfg> cf(cfg, cfg + D);
+  for (int32_t d = 0; d < D; d++) cf[size_t(d)].n_versions = z.n_versions[size_t(d)];
+  evg_distro_table dt;
+  memset(&dt, 0, sizeof(dt));
+  dt.n_distros = D; dt.task_off = strings->task_off; dt.group_off = z.group_off.data(); dt.cfg = cf.data(); dt.group_max_hosts = gmax.data();
+  rc = install_composed(c, who, T, En, z.edge_off.data(), &dt);
+  if (rc != EVG_OK) return rc;
+  if (hosts) {
+    rc = upload_hosts(c, who, hosts, host_off, acfg, D);
+    if (rc != EVG_OK) return rc;
+    CK(cudaStreamSynchronize(s));
+  }
+  c->tick.kind = Tick::kOwn;
+  return EVG_OK;
+}
+#undef D2H_IF
 
 int evg_prioritize_legacy_batch(evg_ctx* c, const evg_legacy_soa* in, const int64_t* task_off, const uint8_t* list_mode,
                                 int32_t n_distros, int32_t* order, int64_t* count, int32_t* status) {

@@ -329,6 +329,31 @@ class Engine:
         self._has_hosts = False
         return task_off, group_off, n_versions[:D]
 
+    def intern_batch(self, strings: S.StringCols) -> dict:
+        """evg_intern_batch: evg_intern_columns computed on the device; the resident tick is left as it was.
+        -> dict(group_id, version_id, group_off, n_versions, group_max_hosts, group_first, dep_off, dep_idx)."""
+        out, outs = strings.intern_out()
+        L.check(self.lib.evg_intern_batch(self.ctx, C.byref(strings.struct()), C.byref(outs)))
+        return strings.trim(out)
+
+    def upload_strings(self, tasks: S.TaskSoA, strings: S.StringCols, cfg: np.ndarray, hosts: Optional[S.HostSoA] = None) -> dict:
+        """evg_upload_strings: evg_upload with the group / version ids, group tables and in-queue edges interned on the
+        device from `strings`.  `tasks` supplies the seven numeric columns (its ids and edges are not passed); cfg's
+        n_versions is filled in on the device.  -> the interned outputs, as intern_batch returns them."""
+        ts = tasks.struct()
+        ts.n_edges, ts.group_id, ts.version_id, ts.dep_off, ts.dep_idx = 0, None, None, None, None
+        D = strings.n_distros
+        cfg = np.ascontiguousarray(cfg, dtype=L.DISTRO_CFG_DTYPE)
+        out, outs = strings.intern_out()
+        hs = C.byref(hosts.struct()) if hosts is not None else None
+        L.check(self.lib.evg_upload_strings(self.ctx, C.byref(ts), C.byref(strings.struct()), L.ptr(cfg) if D else None, hs,
+                                            L.ptr(hosts.host_off) if hosts is not None else None,
+                                            L.ptr(hosts.cfg) if hosts is not None and hosts.cfg.shape[0] else None, C.byref(outs)))
+        out = strings.trim(out)
+        self._n_tasks, self._n_distros, self._n_groups = strings.n_tasks, D, int(out["group_off"][-1])
+        self._has_hosts = hosts is not None
+        return out
+
     def download_alias_map(self):
         """evg_download_alias_map: (source row of every resident row, global group id of every group slot)."""
         src = self._out("alias_source_row", self._n_tasks, np.int32)

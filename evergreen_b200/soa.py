@@ -431,13 +431,78 @@ def marshal_tasks(batch: Sequence[tuple], now: int, dependency_db: Optional[Dict
     return soa, table, keys
 
 
-def pack_strings(strings: Sequence[str]):
-    """[str] -> (uint8 bytes, int64 offsets[n+1]): an evg_str_col."""
-    enc = [x.encode() for x in strings]
+def pack_strings(strings: Sequence):
+    """[str or bytes] -> (uint8 bytes, int64 offsets[n+1]): an evg_str_col (a str is encoded as UTF-8)."""
+    enc = [x.encode() if isinstance(x, str) else bytes(x) for x in strings]
     off = np.zeros(len(enc) + 1, dtype=np.int64)
     if enc:
         np.cumsum([len(b) for b in enc], out=off[1:])
     return np.frombuffer(b"".join(enc), dtype=np.uint8).copy() if enc else np.zeros(0, np.uint8), off
+
+
+@dataclass
+class StringCols:
+    """evg_string_cols (include/evg_sched.h), packed once: each task's id, version, task-group key ("" without a task
+    group) and TaskGroupMaxHosts, and its DependsOn ids, concatenated distro by distro.  evg_intern_columns,
+    evg_intern_batch and evg_upload_strings all read this."""
+    task_off: np.ndarray
+    id: tuple          # pack_strings of Task.Id
+    version: tuple     # ... of Task.Version
+    group_key: tuple   # ... of Task.GetTaskGroupString(), "" when TaskGroup == ""
+    group_max_hosts: np.ndarray
+    dep_off: np.ndarray
+    dep_id: tuple      # ... of Dependency.TaskId, dep_off[-1] strings
+
+    @classmethod
+    def pack(cls, task_off, ids, versions, group_keys, group_max_hosts, dep_off, dep_ids) -> "StringCols":
+        return cls(np.ascontiguousarray(task_off, np.int64), pack_strings(ids), pack_strings(versions), pack_strings(group_keys),
+                   np.ascontiguousarray(group_max_hosts, np.int32), np.ascontiguousarray(dep_off, np.int64), pack_strings(dep_ids))
+
+    @property
+    def n_tasks(self) -> int:
+        return int(self.dep_off.shape[0]) - 1
+
+    @property
+    def n_distros(self) -> int:
+        return int(self.task_off.shape[0]) - 1
+
+    def struct(self) -> L.StringColsStruct:
+        col = lambda c: L.StrColStruct(L.ptr(c[0]) if c[0].shape[0] else None, L.ptr(c[1]))  # noqa: E731
+        return L.StringColsStruct(self.n_tasks, self.n_distros, L.ptr(self.task_off), col(self.id), col(self.version),
+                                  col(self.group_key), L.ptr(self.group_max_hosts) if self.n_tasks else None, L.ptr(self.dep_off),
+                                  col(self.dep_id))
+
+    def intern_out(self):
+        """Arrays for every evg_intern_out field, sized for this batch -> (dict, InternOutStruct over them)."""
+        T, D, E = self.n_tasks, self.n_distros, int(self.dep_off[-1])
+        out = dict(group_id=np.empty(T, np.int32), version_id=np.empty(T, np.int32), group_off=np.zeros(D + 1, np.int64),
+                   n_versions=np.zeros(D, np.int32), group_max_hosts=np.empty(max(T, 1), np.int32),
+                   group_first=np.empty(max(T, 1), np.int64), dep_off=np.zeros(T + 1, np.int64), dep_idx=np.empty(max(E, 1), np.int32))
+        return out, L.InternOutStruct(*[L.ptr(out[k]) for k in INTERN_OUT_FIELDS])
+
+    def trim(self, out: dict) -> dict:
+        """An intern_out dict after the call: the group tables and edges cut to the counts the offsets give."""
+        G, En = int(out["group_off"][-1]), int(out["dep_off"][-1])
+        out["group_max_hosts"], out["group_first"], out["dep_idx"] = out["group_max_hosts"][:G], out["group_first"][:G], out["dep_idx"][:En]
+        return out
+
+
+INTERN_OUT_FIELDS = ("group_id", "version_id", "group_off", "n_versions", "group_max_hosts", "group_first", "dep_off", "dep_idx")
+
+
+def string_cols(batch: Sequence[tuple]) -> StringCols:
+    """The strings of a tick, [(distro, [task])], packed as evg_string_cols."""
+    tasks = [t for _, ts in batch for t in ts]
+    task_off = np.zeros(len(batch) + 1, dtype=np.int64)
+    if batch:
+        np.cumsum([len(ts) for _, ts in batch], out=task_off[1:])
+    dep_off = np.zeros(len(tasks) + 1, dtype=np.int64)
+    if tasks:
+        np.cumsum([len(t.depends_on) for t in tasks], out=dep_off[1:])
+    return StringCols.pack(task_off, [t.id for t in tasks], [t.version for t in tasks],
+                           [t.get_task_group_string() if t.task_group != "" else "" for t in tasks],
+                           np.array([t.task_group_max_hosts for t in tasks], dtype=np.int32), dep_off,
+                           [dep.task_id for t in tasks for dep in t.depends_on])
 
 
 def intern_columns(batch: Sequence[tuple], threads: int = 0):
@@ -445,33 +510,10 @@ def intern_columns(batch: Sequence[tuple], threads: int = 0):
     first-appearance order, dependency ids to queue indices) in the library's C++ instead of Python dicts.
     -> dict(group_id, version_id, group_off, n_versions, group_max_hosts, group_first, dep_off, dep_idx)."""
     lib = L.load()
-    tasks = [t for _, ts in batch for t in ts]
-    T, D = len(tasks), len(batch)
-    task_off = np.zeros(D + 1, dtype=np.int64)
-    if D:
-        np.cumsum([len(ts) for _, ts in batch], out=task_off[1:])
-    idb, ido = pack_strings([t.id for t in tasks])
-    vb, vo = pack_strings([t.version for t in tasks])
-    gb, go = pack_strings([t.get_task_group_string() if t.task_group != "" else "" for t in tasks])
-    gmax = np.array([t.task_group_max_hosts for t in tasks], dtype=np.int32)
-    dep_off = np.zeros(T + 1, dtype=np.int64)
-    if T:
-        np.cumsum([len(t.depends_on) for t in tasks], out=dep_off[1:])
-    db, do = pack_strings([dep.task_id for t in tasks for dep in t.depends_on])
-    E = int(dep_off[-1])
-    out = dict(group_id=np.empty(T, np.int32), version_id=np.empty(T, np.int32), group_off=np.zeros(D + 1, np.int64),
-               n_versions=np.zeros(D, np.int32), group_max_hosts=np.empty(max(T, 1), np.int32), group_first=np.empty(max(T, 1), np.int64),
-               dep_off=np.zeros(T + 1, np.int64), dep_idx=np.empty(max(E, 1), np.int32))
-    col = lambda b, o: L.StrColStruct(L.ptr(b) if b.shape[0] else None, L.ptr(o))  # noqa: E731
-    ins = L.StringColsStruct(T, D, L.ptr(task_off), col(idb, ido), col(vb, vo), col(gb, go), L.ptr(gmax) if T else None,
-                             L.ptr(dep_off), col(db, do))
-    outs = L.InternOutStruct(*[L.ptr(out[k]) for k in ("group_id", "version_id", "group_off", "n_versions", "group_max_hosts",
-                                                       "group_first", "dep_off", "dep_idx")])
-    import ctypes as C
-    L.check(lib.evg_intern_columns(C.byref(ins), C.byref(outs), int(threads)))
-    G, En = int(out["group_off"][D]), int(out["dep_off"][T])
-    out["group_max_hosts"], out["group_first"], out["dep_idx"] = out["group_max_hosts"][:G], out["group_first"][:G], out["dep_idx"][:En]
-    return out
+    sc = string_cols(batch)
+    out, outs = sc.intern_out()
+    L.check(lib.evg_intern_columns(C.byref(sc.struct()), C.byref(outs), int(threads)))
+    return sc.trim(out)
 
 
 def provider_class(provider: str) -> int:

@@ -383,7 +383,8 @@ int evg_bind_result_buffer(evg_ctx* ctx, void* device_ptr, int64_t capacity);
  * evg_plan_and_alloc_batch it runs), evg_plan_and_alloc_batch's pipelined large ticks, evg_alloc_batch / evg_alloc_distro,
  * evg_deps_met_batch, evg_find_runnable_batch / _ex, evg_plan_from_finder / _ex, evg_edit_tasks, evg_plan_aliases,
  * evg_expected_durations_batch, evg_prioritize_legacy_batch, evg_dag_rebuild_batch, evg_rebuild_dispatchers,
- * evg_host_job, evg_host_drawdown, evg_idle_hosts, evg_find_next_batch, evg_find_next_tasks, evg_estimate_start_times and evg_estimate_start_batch.  Every other call adds the kernels it launches: the uploads (their range check), evg_update_tasks,
+ * evg_host_job, evg_host_drawdown, evg_idle_hosts, evg_find_next_batch, evg_find_next_tasks, evg_estimate_start_times,
+ * evg_estimate_start_batch, evg_intern_batch and evg_upload_strings.  Every other call adds the kernels it launches: the uploads (their range check), evg_update_tasks,
  * evg_download_queue and evg_resolve_durations. */
 int64_t evg_last_launch_count(evg_ctx* ctx);
 /* Device time in ms of the last evg_run_resident, from CUDA events on the context
@@ -682,6 +683,47 @@ typedef struct {
  * task_off that does not start at 0, end at n_tasks and never decrease, and for a dep_off that does not start at 0 or
  * decreases. */
 int evg_intern_columns(const evg_string_cols* in, evg_intern_out* out, int32_t threads);
+
+/* ---- the same string work on the device ----------------------------------- */
+
+/* evg_intern_columns computed on the device: same structs, same outputs, host pointers in and out.  Every output equals
+ * what evg_intern_columns returns for the same input, bit for bit:
+ *   - group and version ids are dense per distro, in first-appearance order;
+ *   - a group key of "" means no task group (group_id -1); a version of "" is an ordinary key;
+ *   - a repeated task id keeps its first index;
+ *   - a dependency resolves only to a task of its own distro; forward references resolve, unresolved ones are dropped,
+ *     and the kept edges stay in DependsOn order, duplicates included;
+ *   - group_max_hosts and group_first come from the group's first member.
+ * Keys are compared by their bytes; an equal hash never decides equality.  No output and no message depends on the
+ * order of atomics.  EVG_ERR_INVALID for null columns, negative sizes, tasks without distros, a task_off rejected as by
+ * evg_intern_columns (checked on the host), a dep_off row that does not lie in [0, dep_off[n_tasks]] or decreases, a
+ * string offset outside its column (the kernel that reads a row checks it; the message names the table), and members of
+ * one task group that disagree on TaskGroupMaxHosts (the message names the LOWEST such row).  EVG_ERR_NOMEM, before any
+ * work, for a batch the device cannot hold; the context stays usable.
+ * Needs no resident tick and leaves the tick as it was: the strings are staged into buffers of the call's own, which
+ * the first call allocates.  Test hook: the environment variable EVG_INTERN_HASH_BITS (read per call, 0..32, default
+ * 32) masks the hash value to that many bits so that tests can make every string collide; it selects no other code. */
+int evg_intern_batch(evg_ctx* ctx, const evg_string_cols* in, evg_intern_out* out);
+
+/* evg_upload, with the group / version ids, group_off, group_max_hosts, n_versions and in-queue edges interned on the
+ * device from `strings` (as evg_intern_batch) and written straight into the resident columns.  `tasks` carries the seven
+ * numeric columns (priority, expected_ns, both bases, num_dependents, task_group_order, flags) of strings->n_tasks rows;
+ * its group_id, version_id, dep_off and dep_idx must be NULL (EVG_ERR_INVALID otherwise) and n_edges is not read.
+ * strings->task_off is the distro table's task_off; cfg[d].n_versions is ignored and filled in from the device's count.
+ * hosts / host_off / acfg as for evg_upload (NULL: planner only).  `out` receives group_off and n_versions, and, where
+ * its pointers are not NULL, group_max_hosts, group_first (the shim names its TaskGroupInfos from these rows), group_id,
+ * version_id, dep_off and dep_idx.
+ * What crosses PCIe: the numeric columns and the strings once (host to device); in between, the host reads the group,
+ * version and edge offsets of every distro and the max hosts of every group slot -- nothing per task.
+ * Leaves the tick evg_upload leaves: the context's own columns, editable (evg_run_resident, evg_download,
+ * evg_download_queue, evg_update_tasks, evg_edit_tasks, evg_resolve_durations, evg_rebuild_dispatchers, the host jobs and
+ * the estimates work on it exactly as after evg_upload of the host-interned table).  EVG_ERR_INVALID as for
+ * evg_intern_batch: a table rejected on the host leaves the previous tick resident and runnable, one rejected on the
+ * device leaves no resident tick, as for evg_upload.
+ * Replaces: the string maps PrepareTasksForPlanning files units by (scheduler/planner.go:431-456) and the marshalling
+ * before them. */
+int evg_upload_strings(evg_ctx* ctx, const evg_task_soa* tasks, const evg_string_cols* strings, const evg_distro_cfg* cfg,
+                       const evg_host_soa* hosts, const int64_t* host_off, const evg_alloc_cfg* acfg, evg_intern_out* out);
 
 /* ---- expected-duration statistics (SURVEY.md §8f.2) ----------------------- */
 
