@@ -17,7 +17,7 @@ LIB_PATH = os.path.join(_HERE, "libevgsched.so")
 EVG_TIME_ZERO = -(2 ** 63)
 
 EVG_OK = 0
-EVG_ERR_INVALID, EVG_ERR_CUDA, EVG_ERR_NOMEM, EVG_ERR_STATE = -1, -2, -3, -4
+EVG_ERR_INVALID, EVG_ERR_CUDA, EVG_ERR_NOMEM, EVG_ERR_STATE, EVG_ERR_INTERNAL = -1, -2, -3, -4, -5
 EVG_ALLOC_OK, EVG_ALLOC_ERR_FUTURE_FRACTION, EVG_ALLOC_ERR_POOL_SIZE, EVG_ALLOC_ERR_PARENT_MISSING = 0, 1, 2, 3
 
 EVG_TF_REQ_OTHER, EVG_TF_REQ_PATCH, EVG_TF_REQ_MERGE_QUEUE = 0, 1, 2
@@ -26,6 +26,7 @@ EVG_HF_RUNNING, EVG_HF_TEARDOWN, EVG_HF_RT_FOUND = 0x1, 0x2, 0x4
 EVG_HG_NONE, EVG_HG_UNQUEUED = -1, -2
 EVG_PROVIDER_STATIC, EVG_PROVIDER_EPHEMERAL, EVG_PROVIDER_DOCKER = 0, 1, 2
 EVG_OPT_BREAKDOWN = 0x1
+EVG_OPT_QUEUE_BREAKDOWN = 0x2
 EVG_BD_N = 13
 (EVG_BD_TASK_GROUP_LENGTH, EVG_BD_TOTAL_VALUE, EVG_BD_P_INITIAL, EVG_BD_P_TASK_GROUP, EVG_BD_P_GENERATOR,
  EVG_BD_P_COMMIT_QUEUE, EVG_BD_R_COMMIT_QUEUE, EVG_BD_R_NUM_DEPENDENTS, EVG_BD_R_ESTIMATED_RUNTIME,
@@ -342,6 +343,7 @@ SYMBOLS = {
     "evg_run_resident": (C.c_int, [_P, C.c_int64, C.c_uint32]),
     "evg_download": (C.c_int, [_P, _P, _P]),
     "evg_download_queue": (C.c_int, [_P, C.c_int32, _P, _P, C.c_int64]),
+    "evg_download_queue_breakdown": (C.c_int, [_P, C.c_int32, _P, _P, C.c_int64]),
     "evg_device_result_ptr": (_P, [_P]),
     "evg_bind_result_buffer": (C.c_int, [_P, _P, C.c_int64]),
     "evg_last_launch_count": (C.c_int64, [_P]),

@@ -15,7 +15,9 @@
 //                                  queue + TotalValue
 //     k_finalize_info              DistroQueueInfo / TaskGroupInfo scalars (scheduler.go:144-158)
 // Both:
-//   k_breakdown           the 13-field SortingValueBreakdown per ranked task (EVG_OPT_BREAKDOWN)
+//   k_breakdown           the 13-field SortingValueBreakdown per ranked task (EVG_OPT_BREAKDOWN) or per persisted rank
+//                         (evg_download_queue_breakdown)
+//   k_bd_groups           Unit.info of the narrow distros' task groups, accumulated with atomics (evg_download_queue_breakdown)
 //   k_alloc<TPD>          utilization host allocator, a warp or a block per distro (utilization_based_host_allocator.go:26-409)
 //   k_validate            range check of the distro-local ids the planners index with
 // The rows either side of the path (SURVEY.md §8f):
@@ -251,10 +253,11 @@ __device__ __forceinline__ int find_distro(const int64_t* __restrict__ off, int 
 
 // Block-cooperative distro lookup: thread 0 / last thread bracket the block's
 // range, then each thread searches only inside the bracket.
+// `first0`: the item of thread 0 of block 0 (t = first0 + the thread's global index).
 __device__ __forceinline__ int block_find_distro(const int64_t* __restrict__ off, int n_distros, int64_t t,
-                                                 int64_t n_items) {
+                                                 int64_t n_items, int64_t first0 = 0) {
   __shared__ int s_lo, s_hi;
-  int64_t first = int64_t(blockIdx.x) * blockDim.x;
+  int64_t first = first0 + int64_t(blockIdx.x) * blockDim.x;
   if (threadIdx.x == 0) s_lo = find_distro(off, 0, n_distros - 1, first);
   if (threadIdx.x == blockDim.x - 1) {
     int64_t last = first + blockDim.x - 1;
@@ -1009,22 +1012,65 @@ __global__ void __launch_bounds__(256) k_dur_commit(DDurRows R, const int* __res
   }
 }
 
-// The 13-field SortingValueBreakdown of the unit each ranked task was emitted
-// from (planner.go:472-476, model/task/task.go:3990-4038); both paths.
+// A distro without GroupVersions and without in-queue dependency edges (upload_tasks' `narrow`): its units are its task
+// groups and its single tasks, and every task belongs to exactly one of them.
+__device__ __forceinline__ bool distro_narrow(const DTasks& T, const DDistros& D, int d) {
+  return !D.cfg[d].group_versions && (T.n_edges == 0 || T.dep_off[D.task_off[d + 1]] == T.dep_off[D.task_off[d]]);
+}
+
+// One task's Unit.info contribution (acc_add) folded into a shared accumulator.  Sums, maxima and flags do not depend
+// on the order the members arrive in, so the result is exact and deterministic (sums wrap like Go's int64).
+__device__ __forceinline__ void acc_add_atomic(UnitAcc* a, int64_t now, int32_t priority, int64_t expected_ns, int64_t queue_basis_ns,
+                                               int32_t num_dependents, int32_t group_id, uint32_t tflags) {
+  UnitAcc x;
+  acc_init(x);
+  acc_add(x, now, priority, expected_ns, queue_basis_ns, num_dependents, group_id, tflags);
+  atomicAdd(reinterpret_cast<unsigned long long*>(&a->tiq), (unsigned long long)x.tiq);
+  atomicAdd(reinterpret_cast<unsigned long long*>(&a->rt), (unsigned long long)x.rt);
+  atomicAdd(reinterpret_cast<unsigned long long*>(&a->n), 1ull);
+  atomicMax(reinterpret_cast<long long*>(&a->max_p), (long long)x.max_p);
+  atomicMax(reinterpret_cast<long long*>(&a->max_d), (long long)x.max_d);
+  if (x.flags) atomicOr(&a->flags, x.flags);
+}
+
+// Unit.info of every task-group slot of the narrow distros among the tasks [first0, n_items) (whole distros): one thread
+// per task, accumulators zeroed by the caller.
+__global__ void __launch_bounds__(256) k_bd_groups(DTasks T, DDistros D, int64_t first0, int64_t n_items, int64_t now, UnitAcc* acc) {
+  const int64_t t = first0 + int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  const int d = block_find_distro(D.task_off, D.n, t, n_items, first0);
+  if (d < 0) return;
+  const int32_t gid = T.gid[t];
+  if (gid < 0 || !distro_narrow(T, D, d)) return;
+  acc_add_atomic(acc + D.group_off[d] + gid, now, T.priority[t], T.expected[t], T.qbasis[t], T.numdep[t], gid, T.flags[t]);
+}
+
+// The 13-field SortingValueBreakdown of the unit each ranked task was emitted from (planner.go:472-476,
+// model/task/task.go:3990-4038); both paths.  Rows [first0, n_items) of the row table row_off (D+1 offsets; row j of
+// distro d is its rank j - row_off[d]) go to out[j - first0].  A run (EVG_OPT_BREAKDOWN) passes the task offsets and
+// every rank, `err` and no `group_acc`: every distro reads back the unit its run kept.  evg_download_queue_breakdown
+// passes the persisted rows and `group_acc` (k_bd_groups' accumulators): a narrow distro's task takes its group's unit
+// or its own, a complex distro's the unit its run kept; each row's TotalValue is compared with `tv` at its rank and
+// the first row that differs lands in *bad.
 __global__ void __launch_bounds__(256) k_breakdown(DTasks T, DDistros D, DWork W, const uint32_t* run_all, const URec* pay, const GUnit* units,
-                                                   int64_t now, int any_complex, const int32_t* order, int64_t* breakdown) {
-  if (*W.err) return;
-  const int64_t t = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
-  const int d = block_find_distro(D.task_off, D.n, t, T.n);
+                                                   int64_t now, int any_complex, const int32_t* order, const int64_t* row_off,
+                                                   int64_t first0, int64_t n_items, const int* err, const UnitAcc* group_acc,
+                                                   const int64_t* tv, unsigned long long* bad, int64_t* out) {
+  if (err && *err) return;
+  const int64_t j = first0 + int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  const int d = block_find_distro(row_off, D.n, j, n_items, first0);
   if (d < 0) return;
   const int64_t base = D.task_off[d];
+  const int64_t t = base + (j - row_off[d]);  // the rank slot
   const int64_t g = base + order[t];
   UnitAcc a;
   acc_init(a);
-  const uint32_t bp = any_complex ? W.best_pair[g] : kInactive;
-  if (bp == kInactive) {
+  const bool narrow = group_acc && distro_narrow(T, D, d);
+  const uint32_t bp = !narrow && any_complex ? W.best_pair[g] : kInactive;
+  if (narrow && T.gid[g] >= 0) {
+    a = group_acc[D.group_off[d] + T.gid[g]];
+  } else if (bp == kInactive) {
     acc_add(a, now, T.priority[g], T.expected[g], T.qbasis[g], T.numdep[g], T.gid[g], T.flags[g]);
-  } else if (W.route[d]) {  // on-chip planners leave member lists (breakdown mode only)
+  } else if (W.route[d]) {  // on-chip planners leave member lists (breakdown runs only)
     for (uint32_t q = W.head[W.pair_slot[bp]]; q < kEnd; q = W.next[q]) {
       const uint32_t tq = pair_task(T, W, q);
       acc_add(a, now, T.priority[tq], T.expected[tq], T.qbasis[tq], T.numdep[tq], T.gid[tq], T.flags[tq]);
@@ -1036,7 +1082,8 @@ __global__ void __launch_bounds__(256) k_breakdown(DTasks T, DDistros D, DWork W
   }
   int64_t bd[EVG_BD_N];
   unit_value(a, D.cfg[d], bd);
-  for (int k = 0; k < EVG_BD_N; k++) breakdown[t * EVG_BD_N + k] = bd[k];
+  for (int k = 0; k < EVG_BD_N; k++) out[(j - first0) * EVG_BD_N + k] = bd[k];
+  if (tv && bd[EVG_BD_TOTAL_VALUE] != tv[t]) atomicMin(bad, (unsigned long long)j);
 }
 
 // scheduler.go:144-158: scalars of DistroQueueInfo / TaskGroupInfo that are not sums.
@@ -1434,9 +1481,12 @@ struct evg_ctx {
   // from a run on this tick, into the result buffer bound now; evg_host_job reads them.  `host_job`: run state --
   // evg_host_job's reports in hj.out are from the current run; a chained evg_host_drawdown reads them.  `dispatchers`:
   // run state -- evg_rebuild_dispatchers built dp and nx from the current run; evg_find_next_tasks serves from them.
+  // `queue_breakdown`: run state -- the current run kept the units evg_download_queue_breakdown reads back, and the
+  // task columns it scores them from have not been written since.
   struct {
     Tick kind = Tick::kNone;
     bool hosts = false, deps = false, aliases = false, durations = false, allocated = false, host_job = false, dispatchers = false;
+    bool queue_breakdown = false;
   } tick;
   int64_t T = 0, E = 0, G = 0, H = 0, U = 0, NT = 0, t_pad = 0;
   int32_t Dn = 0;
@@ -1533,6 +1583,15 @@ struct evg_ctx {
   RouteList routes[kRoutes];
   int64_t max_cta_tasks = 0;  // largest distro routed to k_plan_cta: picks the fallback instance for what it hands back
   int32_t nNA_big = 0;  // leading entries of the largest-first kCtaA list that need the 128-thread instance
+  // Complex distros (GroupVersions or in-queue edges) in the tick, and the tiny ones: b_warpsplit holds the kWarp list
+  // with its nW_narrow narrow distros first (uploaded only when nW_complex > 0), so that an EVG_OPT_QUEUE_BREAKDOWN run
+  // plans just the complex ones with unit lists.
+  int32_t n_complex = 0, nW_narrow = 0, nW_complex = 0;
+  DevBuf b_warpsplit;
+  bool units_kept = false;  // the last run kept best_pair on the general path (k_gbest) for k_breakdown
+  int64_t run_now = 0;      // now_ns of the last evg_run_resident: the clock its units were scored at
+  // evg_download_queue_breakdown: the row staging, the narrow distros' group accumulators, the row offsets, the check word
+  struct { DevBuf stage, acc, off, bad; } qb;
   DevBuf b_alist;            // distros k_alloc plans itself (task groups, or more than kGrouplessHosts hosts), listed by upload_hosts
   int64_t n_alist = 0;
   bool alist_valid = false;
@@ -1597,7 +1656,8 @@ void drop_tick(evg_ctx* c) { c->tick = {}; }
 
 // What a call needs of the resident tick.  EVG_ERR_STATE names the call and the first unmet condition: a tick, then
 // its kind, then the state the call reads.
-enum class Need { kTick, kOwnColumns, kEditable, kHosts, kVerdicts, kAliasMap, kDurations, kAllocated, kHostJob, kDispatchers };
+enum class Need { kTick, kOwnColumns, kEditable, kHosts, kVerdicts, kAliasMap, kDurations, kAllocated, kHostJob, kDispatchers,
+                  kQueueBreakdown };
 int need_tick(const evg_ctx* c, const char* who, Need what) {
   const auto& t = c->tick;
   const bool own = what == Need::kOwnColumns || what == Need::kEditable;
@@ -1610,7 +1670,11 @@ int need_tick(const evg_ctx* c, const char* who, Need what) {
                       : what == Need::kAliasMap && !t.aliases             ? "the resident tick was not built by evg_plan_aliases"
                       : what == Need::kDurations && !t.durations          ? "no evg_resolve_durations on the resident tick's rows"
                       : what == Need::kHostJob && !t.host_job             ? "no evg_host_job on the resident tick's current run"
-                      : what == Need::kDispatchers && !t.dispatchers      ? "no evg_rebuild_dispatchers on the resident tick's current run" : nullptr;
+                      : what == Need::kDispatchers && !t.dispatchers      ? "no evg_rebuild_dispatchers on the resident tick's current run"
+                      : what == Need::kQueueBreakdown && !t.queue_breakdown
+                          ? "the current run is not an evg_run_resident with EVG_OPT_QUEUE_BREAKDOWN or EVG_OPT_BREAKDOWN, or the task "
+                            "columns were written after it (evg_update_tasks, evg_resolve_durations)"
+                          : nullptr;
   return unmet ? fail(EVG_ERR_STATE, "%s: %s", who, unmet) : EVG_OK;
 }
 
@@ -1652,12 +1716,17 @@ int upload_tasks(evg_ctx* c, const char* who, const evg_task_soa* t, const evg_d
   // Size class of distro d by its own shape (no side effects).  kBigUnits: a GroupVersions distro of k_plan_smem's
   // smallest class above kBigUnitTasks tasks, whose version units of dozens of tasks are walked member by member.
   constexpr int kBigUnits = kRoutes;
-  auto size_class = [&](int32_t d) -> int {
+  // No GroupVersions and no in-queue dependency edge: task groups are the only multi-member units (what k_plan_cta
+  // knows, and what lets evg_download_queue_breakdown score a task's unit without the planner; distro_narrow on the device)
+  auto narrow_of = [&](int32_t d) -> bool {
     const int64_t a = dt->task_off[d], b = dt->task_off[d + 1];
-    const int64_t n = b - a, g = dt->group_off[d + 1] - dt->group_off[d];
-    const evg_distro_cfg& cf = dt->cfg[d];
     const int64_t de = (E > 0) ? (edge_off ? edge_off[d + 1] - edge_off[d] : t->dep_off[b] - t->dep_off[a]) : 0;
-    const bool narrow = !cf.group_versions && de == 0;  // k_plan_cta: task groups are the only multi-member units it knows
+    return !dt->cfg[d].group_versions && de == 0;
+  };
+  auto size_class = [&](int32_t d) -> int {
+    const int64_t n = dt->task_off[d + 1] - dt->task_off[d], g = dt->group_off[d + 1] - dt->group_off[d];
+    const evg_distro_cfg& cf = dt->cfg[d];
+    const bool narrow = narrow_of(d);
     if (n <= kCapW) return kWarp;
     if (narrow && n <= kNCapA && g <= kGA) return kCtaA;
     if (narrow && n <= kNCapB && g <= kGB) return kCtaB;
@@ -1770,6 +1839,12 @@ int upload_tasks(evg_ctx* c, const char* who, const evg_task_soa* t, const evg_d
       for (int32_t x : list[r]) c->max_cta_tasks = std::max<int64_t>(c->max_cta_tasks, dt->task_off[x + 1] - dt->task_off[x]);
   for (int r = 0; r < kRoutes; r++)
     if (largest_first(r)) UP(s, c->routes[r].lpt, lpt[r].data(), int64_t(lpt[r].size()), int32_t);
+  c->n_complex = 0;
+  for (int32_t d = 0; d < D; d++) c->n_complex += narrow_of(d) ? 0 : 1;
+  std::vector<int32_t> wsplit = list[kWarp];
+  c->nW_narrow = int32_t(std::stable_partition(wsplit.begin(), wsplit.end(), narrow_of) - wsplit.begin());
+  c->nW_complex = int32_t(wsplit.size()) - c->nW_narrow;
+  if (c->nW_complex > 0) UP(s, c->b_warpsplit, wsplit.data(), int64_t(wsplit.size()), int32_t);
   // the staging vectors above must outlive the async copies
   CK(cudaStreamSynchronize(s));
   // work buffers
@@ -2042,7 +2117,7 @@ int run_general(evg_ctx* c, cudaStream_t st, const DTasks& dt, const DDistros& d
     launch(c, st, k_gfill, wl_grid, 256, 0, dt, dd, w, g);
     launch(c, st, k_gunit, wl_grid, 256, 0, dd, w, g, now);
     launch(c, st, k_grank, wl_grid, 256, 0, w, g);
-    launch(c, st, k_gbest, wl_grid, 256, 0, dt, dd, w, g, c->bd_valid ? 1 : 0);
+    launch(c, st, k_gbest, wl_grid, 256, 0, dt, dd, w, g, c->units_kept ? 1 : 0);
   }
   launch(c, st, k_gsched, grid_for(gcount, 128), 128, 0, g, gl, gcount);
   if (gc) {
@@ -2072,9 +2147,10 @@ int ensure_aux_streams(evg_ctx* c) {
   return EVG_OK;
 }
 
-// The resident tick, the resident tick with the unit lists EVG_OPT_BREAKDOWN reads, or one chunk of the pipelined
-// one-shot call.
-enum class Mode { kResident, kBreakdown, kPipelined };
+// The resident tick; the resident tick with the units EVG_OPT_QUEUE_BREAKDOWN reads back for its complex distros (the
+// tiny ones planned with unit lists, the rest as kResident); the resident tick with the unit lists EVG_OPT_BREAKDOWN
+// reads for every distro; or one chunk of the pipelined one-shot call.
+enum class Mode { kResident, kQueueBreakdown, kBreakdown, kPipelined };
 
 // The planner launch of size class r in `mode`: entries [first, first + n) of its list -- the largest-first copy on the
 // resident tick, the ascending list (cut by chunk) on the pipelined call -- on stream st.  The k_plan_cta classes hand
@@ -2092,7 +2168,7 @@ int plan_route(evg_ctx* c, int r, Mode mode, cudaStream_t st, const DTasks& dt, 
     case kCtaC: return launch_cta<kNT_C, kNCapC, kNOccC>(c, st, dt, dd, w, list, n, now, punt, punt_count);
     case kCtaB: return launch_cta<kNT_B, kNCapB, kNOccB>(c, st, dt, dd, w, list, n, now, punt, punt_count);
     case kCtaA:
-      if (mode == Mode::kResident) {  // the distros that fit the 64-thread instance are the tail of the largest-first list
+      if (mode != Mode::kPipelined) {  // the distros that fit the 64-thread instance are the tail of the largest-first list
         if ((rc = launch_cta<kNT_A, kNCapA, kNOccA>(c, st, dt, dd, w, list, c->nNA_big, now, punt, punt_count)) != EVG_OK) return rc;
         return launch_cta<kNT_S, kNCapS, kNOccS>(c, st, dt, dd, w, list + c->nNA_big, n - c->nNA_big, now, punt, punt_count);
       }
@@ -2101,13 +2177,19 @@ int plan_route(evg_ctx* c, int r, Mode mode, cudaStream_t st, const DTasks& dt, 
       // the resident tick takes the smallest k_plan_smem instance that holds the largest distro given to k_plan_cta (the
       // launch has one CTA per distro that COULD come back; CTAs beyond *punt_count exit at once, and 10^4 empty
       // 1024-thread CTAs are not free); the pipelined call always takes the largest
-      if (mode == Mode::kResident && c->max_cta_tasks <= kCapA) return launch_smem<128, 8, 8>(c, st, dt, dd, w, list, n, now, 0, punt_count);
-      if (mode == Mode::kResident && c->max_cta_tasks <= kCapB) return launch_smem<256, 16, 3>(c, st, dt, dd, w, list, n, now, 0, punt_count);
+      if (mode != Mode::kPipelined && c->max_cta_tasks <= kCapA) return launch_smem<128, 8, 8>(c, st, dt, dd, w, list, n, now, 0, punt_count);
+      if (mode != Mode::kPipelined && c->max_cta_tasks <= kCapB) return launch_smem<256, 16, 3>(c, st, dt, dd, w, list, n, now, 0, punt_count);
       return launch_smem<kThreadsC, kItemsC, 1>(c, st, dt, dd, w, list, n, now, 0, punt_count);
     case kSmemC: return launch_smem<kThreadsC, kItemsC, 1>(c, st, dt, dd, w, list, n, now, bd);
     case kSmemB: return launch_smem<256, 16, 3>(c, st, dt, dd, w, list, n, now, bd);
     case kSmemA: return launch_smem<128, 8, 8>(c, st, dt, dd, w, list, n, now, bd);
-    case kWarp: return launch_tiny(c, st, dt, dd, w, list, n, now, bd);
+    case kWarp:
+      if (mode == Mode::kQueueBreakdown && c->nW_complex > 0) {  // the narrow ones as before, the complex ones with lists
+        const int32_t* split = c->b_warpsplit.as<int32_t>();
+        if ((rc = launch_tiny(c, st, dt, dd, w, split, c->nW_narrow, now, 0)) != EVG_OK) return rc;
+        return launch_tiny(c, st, dt, dd, w, split + c->nW_narrow, c->nW_complex, now, 1);
+      }
+      return launch_tiny(c, st, dt, dd, w, list, n, now, bd);
     default: {  // kGeneral; the resident tick prepares all its general-path distros before the routes fork
       const std::vector<int32_t>& gh = c->routes[kGeneral].h;
       if (mode == Mode::kPipelined && (rc = prepare_general(c, st, gh[size_t(first)], gh[size_t(first + n - 1)] + 1)) != EVG_OK) return rc;
@@ -2137,8 +2219,12 @@ int run_plan(evg_ctx* c, int64_t now, uint32_t opts) {
   }
   const std::vector<int32_t>& gh = c->routes[kGeneral].h;
   const bool general = !gh.empty();
-  // breakdown mode reads best_pair for every task: tasks emitted from their own single-task unit keep kInactive
-  if (bd && c->any_complex) CK(cudaMemsetAsync(c->b_bestpair.p, 0xFF, sizeof(uint32_t) * size_t(T + 1), s));
+  // a queue-breakdown run of a tick without complex distros is the plain run: the narrow ones need nothing kept
+  const bool qbd = !bd && (opts & EVG_OPT_QUEUE_BREAKDOWN) && c->n_complex > 0;
+  c->units_kept = bd || qbd;
+  // k_breakdown reads best_pair for every task it reads a kept unit for: tasks emitted from their own single-task unit
+  // keep kInactive
+  if (c->units_kept && c->any_complex) CK(cudaMemsetAsync(c->b_bestpair.p, 0xFF, sizeof(uint32_t) * size_t(T + 1), s));
   const int32_t n_new = bd ? 0 : c->routes[kCtaA].n() + c->routes[kCtaB].n() + c->routes[kCtaC].n();  // could be handed back
   if (n_new > 0) CK(cudaMemsetAsync(c->b_puntcnt.p, 0, sizeof(int32_t), s));
   if (general) { int rcg = prepare_general(c, s, gh.front(), gh.back() + 1); if (rcg != EVG_OK) return rcg; }
@@ -2155,7 +2241,7 @@ int run_plan(evg_ctx* c, int64_t now, uint32_t opts) {
   }
   int rc;
   const int slot = int(c->runs % evg_ctx::kRing);
-  const Mode mode = bd ? Mode::kBreakdown : Mode::kResident;
+  const Mode mode = bd ? Mode::kBreakdown : qbd ? Mode::kQueueBreakdown : Mode::kResident;
   // stream 0: k_plan_cta (the dominant kernel of configs[1]-like ticks), then the distros it handed back; streams 1..3:
   // k_plan_smem (GroupVersions, in-queue dependency edges, very many task groups); 4: tiny distros; 5: the general path
   for (int r : {kCtaC, kCtaB, kCtaA, kPunted, kSmemC, kSmemB, kSmemA, kWarp, kGeneral}) {
@@ -2174,7 +2260,10 @@ int run_plan(evg_ctx* c, int64_t now, uint32_t opts) {
       CK(cudaStreamWaitEvent(s, c->ev_join[k], 0));
     }
   }
-  if (bd) launch(c, c->stream, k_breakdown, grid_for(T, 256), 256, 0, dt, dd, w, c->b_run.as<uint32_t>(), c->b_pay.as<URec>(), c->b_unit.as<GUnit>(), now, c->any_complex, c->b_order.as<int32_t>(), bd);
+  if (bd)
+    launch(c, c->stream, k_breakdown, grid_for(T, 256), 256, 0, dt, dd, w, c->b_run.as<uint32_t>(), c->b_pay.as<URec>(),
+           c->b_unit.as<GUnit>(), now, c->any_complex, c->b_order.as<int32_t>(), dd.task_off, int64_t(0), T, w.err,
+           static_cast<const UnitAcc*>(nullptr), static_cast<const int64_t*>(nullptr), static_cast<unsigned long long*>(nullptr), bd);
   CK(cudaGetLastError());
   return EVG_OK;
 }
@@ -2297,6 +2386,7 @@ int evg_update_tasks(evg_ctx* c, int64_t n_rows, const int64_t* rows, const evg_
   if (rc != EVG_OK) return rc;
   int* bad = reinterpret_cast<int*>(at);
   CK(cudaMemsetAsync(bad, 0, sizeof(int), s));
+  c->tick.queue_breakdown = false;  // the breakdowns are scored from the columns written below
   const EdDst o = c->tasks.dst();
   launch(c, s, k_update_rows, grid_for(n_rows, 256), 256, 0, n_rows, d_rows, c->T, o.priority, o.numdep, o.tgo, o.flags, o.expected,
          o.qbasis, o.wbasis, d.priority, d.num_dependents, d.task_group_order, d.flags, d.expected_ns, d.queue_basis_ns, d.wait_basis_ns, bad);
@@ -2335,10 +2425,12 @@ int evg_run_resident(evg_ctx* c, int64_t now_ns, uint32_t opts) {
   c->launches = 0;
   c->timed = true;
   c->general_timed = false;
-  c->tick.allocated = c->tick.host_job = c->tick.dispatchers = false;
+  c->tick.allocated = c->tick.host_job = c->tick.dispatchers = c->tick.queue_breakdown = false;
   CK(cudaEventRecord(c->ev_begin, c->stream));
   int rc = run_plan(c, now_ns, opts);
   if (rc != EVG_OK) return rc;
+  c->tick.queue_breakdown = (opts & (EVG_OPT_QUEUE_BREAKDOWN | EVG_OPT_BREAKDOWN)) != 0;
+  c->run_now = now_ns;
   if (c->tick.hosts) {
     rc = run_alloc(c, now_ns);
     if (rc != EVG_OK) return rc;
@@ -2423,6 +2515,71 @@ int evg_download_queue(evg_ctx* c, int32_t cap, int64_t* item_off, evg_queue_ite
   return EVG_OK;
 }
 
+// Rows of evg_download_queue_breakdown's device staging: 256 MB.  A distro holds at most kMaxTasksPerDistro rows, fewer
+// than this, so every chunk of whole distros holds at least one.
+constexpr int64_t kQueueBdStageRows = (int64_t(256) << 20) / (sizeof(int64_t) * EVG_BD_N);
+static_assert(kQueueBdStageRows >= kMaxTasksPerDistro, "a distro's rows must fit one staging chunk");
+
+int evg_download_queue_breakdown(evg_ctx* c, int32_t cap, int64_t* item_off, int64_t* breakdown, int64_t items_capacity) {
+  ENTER(c, "evg_download_queue_breakdown");
+  if (const int rc = need_tick(c, who, Need::kQueueBreakdown); rc != EVG_OK) return rc;
+  if (cap < 0 || !item_off) return fail(EVG_ERR_INVALID, "%s: bad argument", who);
+  if (cap == 0) cap = EVG_PERSISTED_QUEUE_CAP;
+  const int32_t D = c->Dn;
+  std::vector<int64_t> off(size_t(D) + 1);
+  const int64_t n = persisted_item_off(c, cap, off.data());
+  if (n > items_capacity || (n > 0 && !breakdown))
+    return fail(EVG_ERR_INVALID, "%s: %lld rows needed, %lld available", who, (long long)n, (long long)items_capacity);
+  std::copy(off.begin(), off.end(), item_off);
+  if (n == 0) return EVG_OK;
+  // every buffer before the first launch: a failed allocation leaves the tick as it was
+  auto& q = c->qb;
+  const int64_t stage_rows = std::min(n, kQueueBdStageRows);
+  cudaError_t e = q.stage.ensure(sizeof(int64_t) * EVG_BD_N * size_t(stage_rows));
+  if (e == cudaSuccess) e = q.acc.ensure(sizeof(UnitAcc) * size_t(c->G + 1));
+  if (e == cudaSuccess) e = q.off.ensure(sizeof(int64_t) * size_t(D + 1));
+  if (e == cudaSuccess) e = q.bad.ensure(sizeof(unsigned long long));
+  if (e != cudaSuccess) {
+    cudaGetLastError();  // not sticky: clear it so that no later call reports it
+    return fail(e == cudaErrorMemoryAllocation ? EVG_ERR_NOMEM : EVG_ERR_CUDA, "%s: staging of %lld rows: %s", who,
+                (long long)stage_rows, cudaGetErrorString(e));
+  }
+  cudaStream_t s = c->stream;
+  const DTasks dt = dtasks(c);
+  const DDistros dd = ddistros(c);
+  const DWork w = dwork(c);
+  UnitAcc* acc = q.acc.as<UnitAcc>();
+  unsigned long long* bad = q.bad.as<unsigned long long>();
+  CK(cudaMemcpyAsync(q.off.p, off.data(), sizeof(int64_t) * size_t(D + 1), cudaMemcpyHostToDevice, s));
+  CK(cudaMemsetAsync(bad, 0xFF, sizeof(unsigned long long), s));
+  // chunks of whole distros; the staging is reused in stream order (the next chunk's kernels follow this one's copy)
+  for (int32_t d0 = 0, d1; d0 < D; d0 = d1) {
+    for (d1 = d0 + 1; d1 < D && off[d1 + 1] - off[d0] <= stage_rows;) d1++;
+    const int64_t t0 = c->h_taskoff[d0], t1 = c->h_taskoff[d1], g0 = c->h_groupoff[d0], g1 = c->h_groupoff[d1];
+    if (off[d1] == off[d0]) continue;
+    if (g1 > g0) {
+      CK(cudaMemsetAsync(acc + g0, 0, sizeof(UnitAcc) * size_t(g1 - g0), s));
+      launch(c, s, k_bd_groups, grid_for(t1 - t0, 256), 256, 0, dt, dd, t0, t1, c->run_now, acc);
+    }
+    launch(c, s, k_breakdown, grid_for(off[d1] - off[d0], 256), 256, 0, dt, dd, w, c->b_run.as<uint32_t>(), c->b_pay.as<URec>(),
+           c->b_unit.as<GUnit>(), c->run_now, c->any_complex, c->b_order.as<int32_t>(), q.off.as<int64_t>(), off[d0], off[d1],
+           static_cast<const int*>(nullptr), static_cast<const UnitAcc*>(acc), c->b_tv.as<int64_t>(), bad, q.stage.as<int64_t>());
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(breakdown + off[d0] * EVG_BD_N, q.stage.p, sizeof(int64_t) * EVG_BD_N * size_t(off[d1] - off[d0]),
+                       cudaMemcpyDeviceToHost, s));
+  }
+  unsigned long long h_bad = 0;
+  CK(cudaMemcpyAsync(&h_bad, bad, sizeof(h_bad), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  if (h_bad != ~0ull) {
+    const int64_t j = int64_t(h_bad);
+    const int32_t d = int32_t(std::upper_bound(off.begin(), off.end(), j) - off.begin()) - 1;
+    return fail(EVG_ERR_INTERNAL, "%s: distro %d rank %lld: the breakdown's TotalValue differs from the planned total_value", who, d,
+                (long long)(j - off[size_t(d)]));
+  }
+  return EVG_OK;
+}
+
 // The two queries that return no status take the lock and leave the device alone.
 void* evg_device_result_ptr(evg_ctx* c) {
   if (!c) return nullptr;
@@ -2481,7 +2638,8 @@ int evg_plan_batch(evg_ctx* c, const evg_task_soa* tasks, const evg_distro_table
   ENTER(c, "evg_plan_batch");
   int rc = upload(c, who, tasks, distros, nullptr, nullptr, nullptr, Tick::kFixed);
   if (rc != EVG_OK) return rc;
-  rc = evg_run_resident(c, now_ns, opts);
+  rc = evg_run_resident(c, now_ns, opts & ~EVG_OPT_QUEUE_BREAKDOWN);
+  c->tick.queue_breakdown = false;  // one-shot calls leave no queue-breakdown run behind
   if (rc != EVG_OK) return rc;
   return evg_download(c, out, nullptr);
 }
@@ -2511,7 +2669,7 @@ static int plan_and_alloc_pipelined(evg_ctx* c, const evg_task_soa* t, const evg
   CK(c->b_gs.ensure(sizeof(GroupScratch) * size_t(c->G + 1)));
   c->launches = 0;
   c->timed = false;
-  c->bd_valid = false;
+  c->bd_valid = c->units_kept = false;
   CK(cudaMemsetAsync(c->b_puntcnt.p, 0, sizeof(int32_t) * (evg_ctx::kMaxChunks + 2), s));
   // chunk boundaries: whole distros, about equal task counts
   const int n_chunks = int(std::min<int64_t>(evg_ctx::kMaxChunks, std::max<int64_t>(1, T / (1 << 20))));
@@ -2600,7 +2758,8 @@ int evg_plan_and_alloc_batch(evg_ctx* c, const evg_task_soa* tasks, const evg_di
   }
   int rc = upload(c, who, tasks, distros, hosts, host_off, acfg, Tick::kFixed);
   if (rc != EVG_OK) return rc;
-  rc = evg_run_resident(c, now_ns, opts);
+  rc = evg_run_resident(c, now_ns, opts & ~EVG_OPT_QUEUE_BREAKDOWN);
+  c->tick.queue_breakdown = false;  // one-shot calls leave no queue-breakdown run behind
   if (rc != EVG_OK) return rc;
   return evg_download(c, plan_out, alloc_out);
 }
@@ -2824,6 +2983,7 @@ int evg_resolve_durations(evg_ctx* c, const evg_duration_in* in, int64_t now_ns)
   cudaStream_t s = c->stream;
   auto& d = c->dur;
   c->tick.durations = false;  // the staging below is overwritten whatever the outcome
+  c->tick.queue_breakdown = false;  // and the expected durations the breakdowns are scored from may be
   const int64_t Nt = in->tasks ? in->tasks->n_rows : 0, Nh = in->hosts ? in->hosts->n_rows : 0, N = Nt + Nh;
   // history -> per-key statistics, on the call's own buffers (evg_expected_durations_batch's scratch is not touched)
   UP(s, d.key, h ? h->key : nullptr, R, int32_t);

@@ -209,6 +209,18 @@ class Engine:
         L.check(self.lib.evg_download_queue(self.ctx, int(cap), L.ptr(item_off), L.ptr(items), int(max(n, 1))))
         return item_off, items[: int(item_off[D])]
 
+    def download_queue_breakdown(self, cap: int = 0, task_off=None):
+        """evg_download_queue_breakdown: (item_off, int64 [N, 13]) -- the SortingValueBreakdown of every row
+        download_queue(cap) returns, computed on the device for those rows only.  Needs a run with
+        EVG_OPT_QUEUE_BREAKDOWN (or EVG_OPT_BREAKDOWN) on the resident rows."""
+        D = self._n_distros
+        item_off = self._out("queue_bd_item_off", D + 1, np.int64)
+        cap_eff = cap or L.EVG_PERSISTED_QUEUE_CAP
+        n = self._n_tasks if task_off is None else int(np.minimum(np.diff(task_off), cap_eff).sum())
+        bd = self._out("queue_breakdown", (max(n, 1), L.EVG_BD_N), np.int64)
+        L.check(self.lib.evg_download_queue_breakdown(self.ctx, int(cap), L.ptr(item_off), L.ptr(bd), int(max(n, 1))))
+        return item_off, bd[: int(item_off[D])]
+
     def bind_result_buffer(self, device_ptr: int, capacity_rows: int) -> None:
         """The allocator kernel writes evg_alloc_result rows straight into this device buffer
         (the all-gather send buffer, evergreen_b200.dist)."""
@@ -876,28 +888,33 @@ class ResidentTick:
 
 
 def persist_task_queues(batch: Sequence[Tuple[M.Distro, List[M.Task]]], now: int, *, engine: Optional[Engine] = None,
-                        dependency_db: Optional[Dict[str, M.Task]] = None, cap: int = 0) -> List[M.TaskQueue]:
+                        dependency_db: Optional[Dict[str, M.Task]] = None, cap: int = 0,
+                        breakdown: bool = False) -> List[M.TaskQueue]:
     """Batched PersistTaskQueue minus the upsert (scheduler/task_queue_persister.go:14-42, TaskQueue.Save
     model/task_queue.go:216-219): plan every distro, then build each distro's TaskQueue document from the
     TaskQueueItem rows the device projected for the first min(length, 10 000) ranks -- only those rows are copied
     back -- plus the strings of the shim's own Task objects.  Tasks are stamped like the reference leaves them
     (ExpectedDuration scheduler.go:98, DependenciesMetTime task.go:653, ScheduledTime / DependenciesMetTime
-    task.go:1164-1195 at `now`)."""
+    task.go:1164-1195 at `now`).  With `breakdown`, every item and its task carry the full SortingValueBreakdown
+    (evg_download_queue_breakdown, persisted rows only); without it only TotalValue, as the items have always had."""
     eng = engine or default_engine()
     soa, table, keys = S.marshal_tasks(batch, now, dependency_db)
     _upload_with_device_deps(eng, batch, soa, table, None, now, dependency_db)
-    eng.run(now)
+    eng.run(now, L.EVG_OPT_QUEUE_BREAKDOWN if breakdown else 0)
     po, _ = eng.download(want_alloc=False)
     item_off, items = eng.download_queue(cap, table.task_off)
+    bd = eng.download_queue_breakdown(cap, table.task_off)[1] if breakdown else None
     out = []
     for d, (distro, tasks) in enumerate(batch):
         ga, gb = int(table.group_off[d]), int(table.group_off[d + 1])
         info = _queue_info_from_rows(po.info[d], po.group_info[ga:gb], keys[d].group_names)
         queue = []
-        for row in items[int(item_off[d]):int(item_off[d + 1])]:
+        for k in range(int(item_off[d]), int(item_off[d + 1])):
+            row = items[k]
             t = tasks[int(row["task"])]
             t.expected_duration = int(row["expected_ns"])
-            t.sorting_value_breakdown = M.SortingValueBreakdown(total_value=int(row["total_value"]))
+            t.sorting_value_breakdown = (M.SortingValueBreakdown.from_row(bd[k]) if breakdown else
+                                         M.SortingValueBreakdown(total_value=int(row["total_value"])))
             queue.append(M.TaskQueueItem(
                 id=t.id, display_name=t.display_name, build_variant=t.build_variant,
                 revision_order_number=t.revision_order_number, requester=t.requester, revision=t.revision, project=t.project,
@@ -916,9 +933,9 @@ def persist_task_queues(batch: Sequence[Tuple[M.Distro, List[M.Task]]], now: int
 
 
 def PersistTaskQueue(distro: M.Distro, tasks: List[M.Task], *, now: int, engine: Optional[Engine] = None,
-                     dependency_db: Optional[Dict[str, M.Task]] = None) -> M.TaskQueue:
+                     dependency_db: Optional[Dict[str, M.Task]] = None, breakdown: bool = False) -> M.TaskQueue:
     """scheduler.PersistTaskQueue for one distro; the caller upserts the returned document."""
-    return persist_task_queues([(distro, tasks)], now, engine=engine, dependency_db=dependency_db)[0]
+    return persist_task_queues([(distro, tasks)], now, engine=engine, dependency_db=dependency_db, breakdown=breakdown)[0]
 
 
 def PlanDistro(distro: M.Distro, find_tasks, *, now: int, engine: Optional[Engine] = None,
@@ -1244,28 +1261,35 @@ def plan_alias_queues(distros: Sequence[M.Distro], tasks: Sequence[M.Task], now:
 
 
 def persist_alias_task_queues(distros: Sequence[M.Distro], tasks: Sequence[M.Task], now: int, *, engine: Optional[Engine] = None,
-                              dependency_db: Optional[Dict[str, M.Task]] = None, cap: int = 0) -> List[M.TaskQueue]:
+                              dependency_db: Optional[Dict[str, M.Task]] = None, cap: int = 0,
+                              breakdown: bool = False) -> List[M.TaskQueue]:
     """persist_task_queues for the alias queues: every distro's secondary TaskQueue document (TaskQueue.collection() is
-    the alias queues' collection) from the TaskQueueItem rows evg_download_queue projects on the device."""
+    the alias queues' collection) from the TaskQueueItem rows evg_download_queue projects on the device.  With
+    `breakdown`, every item carries the full SortingValueBreakdown (evg_download_queue_breakdown); a task shared by
+    several alias queues has one breakdown in each, so the task itself is not stamped."""
     eng = engine or default_engine()
     task_off, group_off, src, names = _plan_aliases(eng, distros, tasks, now, dependency_db)
-    eng.run(now)
+    eng.run(now, L.EVG_OPT_QUEUE_BREAKDOWN if breakdown else 0)
     po, _ = eng.download(want_alloc=False)
     item_off, items = eng.download_queue(cap, task_off)
+    bd = eng.download_queue_breakdown(cap, task_off)[1] if breakdown else None
     out = []
     for d, distro in enumerate(distros):
         a, ga, gb = int(task_off[d]), int(group_off[d]), int(group_off[d + 1])
         info = _queue_info_from_rows(po.info[d], po.group_info[ga:gb], names[ga:gb])
         info.secondary_queue = True
         queue = []
-        for row in items[int(item_off[d]):int(item_off[d + 1])]:
+        for k in range(int(item_off[d]), int(item_off[d + 1])):
+            row = items[k]
             t = tasks[int(src[a + int(row["task"])])]
             t.expected_duration = int(row["expected_ns"])
+            svb = (M.SortingValueBreakdown.from_row(bd[k]) if breakdown else
+                   M.SortingValueBreakdown(total_value=int(row["total_value"])))
             queue.append(M.TaskQueueItem(
                 id=t.id, display_name=t.display_name, build_variant=t.build_variant,
                 revision_order_number=t.revision_order_number, requester=t.requester, revision=t.revision, project=t.project,
                 expected_duration=int(row["expected_ns"]), priority=int(row["priority"]),
-                sorting_value_breakdown=M.SortingValueBreakdown(total_value=int(row["total_value"])), group=t.task_group,
+                sorting_value_breakdown=svb, group=t.task_group,
                 group_max_hosts=t.task_group_max_hosts, group_index=int(row["group_index"]), version=t.version,
                 activated_by=t.activated_by, dependencies=[dep.task_id for dep in t.depends_on],
                 dependencies_met=bool(int(row["flags"]) & L.EVG_QI_DEPS_MET)))

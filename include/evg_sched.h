@@ -45,9 +45,10 @@ enum {
   EVG_ERR_INVALID = -1, /* bad argument / inconsistent offsets */
   EVG_ERR_CUDA = -2,    /* no usable sm_90 device, or a CUDA call failed */
   EVG_ERR_NOMEM = -3,   /* device or pinned allocation failed */
-  EVG_ERR_STATE = -4    /* the resident tick cannot serve the call: there is none, or it lacks what the call needs
+  EVG_ERR_STATE = -4,   /* the resident tick cannot serve the call: there is none, or it lacks what the call needs
                            (its own columns, editability, hosts, dependency verdicts, alias map, resolved durations,
-                           an allocator run since it was set, an evg_host_job on its current run) */
+                           an allocator run since it was set, an evg_host_job on its current run, a queue-breakdown run) */
+  EVG_ERR_INTERNAL = -5 /* a device-side consistency check failed; the message names where */
 };
 
 /* per-distro allocator status: the data errors UtilizationBasedHostAllocator
@@ -226,6 +227,14 @@ typedef struct {
 
 /* option bits */
 #define EVG_OPT_BREAKDOWN 0x1u /* materialise evg_plan_out.breakdown */
+/* evg_run_resident only (the one-shot calls ignore it): keep what evg_download_queue_breakdown needs, and nothing per
+ * task of the tick.  A distro is NARROW when it has no GroupVersions and no in-queue dependency edge: its units are its
+ * task groups and its single tasks, so the unit a task was emitted from is known without the planner and narrow
+ * distros are planned exactly as without the option (a tick of narrow distros only runs the same kernels).  Every
+ * other distro is COMPLEX: it is planned as under EVG_OPT_BREAKDOWN (unit lists kept, the tiny ones planned by
+ * k_plan_smem instead of k_plan_warp), so the unit the planner picked can be read back.  Plan outputs are identical
+ * either way. */
+#define EVG_OPT_QUEUE_BREAKDOWN 0x2u
 
 typedef struct evg_ctx evg_ctx;
 
@@ -371,6 +380,19 @@ typedef struct {
  * (scheduler/task_queue_persister.go:14-42, model/task_queue.go:216-219).  The upsert stays with the caller. */
 int evg_download_queue(evg_ctx* ctx, int32_t cap, int64_t* item_off, evg_queue_item* items, int64_t items_capacity);
 
+/* The full SortingValueBreakdown of every row evg_download_queue(cap) returns: the same rows, item_off and
+ * items_capacity rule (EVG_ERR_INVALID names the needed count and writes nothing), EVG_BD_N int64 per row in EVG_BD_*
+ * order -- what PersistTaskQueue copies from TaskPlan.Export into each TaskQueueItem (task_queue_persister.go:16-42,
+ * planner.go:472-476).  Computed at call time from the resident tick: a narrow distro's task (see
+ * EVG_OPT_QUEUE_BREAKDOWN) takes the breakdown of its whole task group, or of itself alone; a complex distro's that of
+ * the unit its run kept.  Whole distros go through a device staging buffer of at most 256 MB, a copy to the host per
+ * chunk; the staging is allocated before the first launch (EVG_ERR_NOMEM leaves the tick as it was).  Every row's
+ * TotalValue is checked on the device against the resident total_value at its rank: EVG_ERR_INTERNAL names the first
+ * distro and rank that differ.  Needs a run with EVG_OPT_QUEUE_BREAKDOWN or EVG_OPT_BREAKDOWN on the resident rows
+ * (EVG_ERR_STATE otherwise): a run without either, the one-shot calls, evg_update_tasks, evg_resolve_durations and
+ * anything that replaces the tick clear it.  Only reads the tick; works on alias ticks too. */
+int evg_download_queue_breakdown(evg_ctx* ctx, int32_t cap, int64_t* item_off, int64_t* breakdown, int64_t items_capacity);
+
 /* Device pointer to the resident evg_alloc_result[n_distros] vector, the
  * send buffer of the per-distro all-gather (SURVEY.md §8e). */
 void* evg_device_result_ptr(evg_ctx* ctx);
@@ -385,7 +407,7 @@ int evg_bind_result_buffer(evg_ctx* ctx, void* device_ptr, int64_t capacity);
  * evg_expected_durations_batch, evg_prioritize_legacy_batch, evg_dag_rebuild_batch, evg_rebuild_dispatchers,
  * evg_host_job, evg_host_drawdown, evg_idle_hosts, evg_find_next_batch, evg_find_next_tasks, evg_estimate_start_times,
  * evg_estimate_start_batch, evg_intern_batch and evg_upload_strings.  Every other call adds the kernels it launches: the uploads (their range check), evg_update_tasks,
- * evg_download_queue and evg_resolve_durations. */
+ * evg_download_queue, evg_download_queue_breakdown and evg_resolve_durations. */
 int64_t evg_last_launch_count(evg_ctx* ctx);
 /* Device time in ms of the last evg_run_resident, from CUDA events on the context
  * stream (valid after a sync / download): total_ms spans the whole tick; sort_ms is
