@@ -5082,8 +5082,10 @@ int evg_host_job(evg_ctx* c, const evg_host_job_cfg* cfg, const int32_t* spawned
     return fail(EVG_ERR_INVALID, "evg_host_job: null cfg or output");
   if (const int rc = need_tick(c, who, Need::kAllocated); rc != EVG_OK) return rc;
   const int32_t D = c->Dn;
-  for (int32_t d = 0; d < D; d++)
+  for (int32_t d = 0; d < D; d++) {
     if (cfg[d].n_provisioning < 0) return fail(EVG_ERR_INVALID, "evg_host_job: cfg[%d].n_provisioning is negative", d);
+    if (spawned && spawned[d] < 0) return fail(EVG_ERR_INVALID, "evg_host_job: spawned[%d] is negative", d);
+  }
   c->launches = 0;
   c->tick.host_job = false;  // until the reports below are written
   if (D == 0) return c->tick.host_job = true, EVG_OK;

@@ -1104,8 +1104,8 @@ typedef struct {
  *     allocator for it, whatever k_alloc wrote on the device);
  *   - any other distro: new_hosts, free_hosts and status of the allocator run; a status other than EVG_ALLOC_OK ends the
  *     job there (:192-195) and the report is zero;
- *   - spawned[d] = len(hostsSpawned) (:233); spawned == NULL means max(n_hosts, 0), what CreateIntentHosts creates
- *     without a container pool (scheduler/scheduler.go:172-215); a pool distro's shim calls again with the count
+ *   - spawned[d] = len(hostsSpawned) (:233), so never negative; spawned == NULL means max(n_hosts, 0), what
+ *     CreateIntentHosts creates without a container pool (scheduler/scheduler.go:172-215); a pool distro's shim calls again with the count
  *     MakeContainersAndParents returned;
  *   - report (:257-326): sums over the distro's group slots (its named TaskGroupInfos; the ungrouped info is excluded),
  *     int64 arithmetic with wrap, timeToEmpty truncated toward zero, 2532000 h when its host count is <= 0, both times
@@ -1120,7 +1120,8 @@ typedef struct {
  * the intent-host cap (:212-229) and a CreateIntentHosts error (:233-237) end the job before the report, so the shim
  * discards that distro's report; choosing the hosts to decommission is the drawdown job's (units/host_drawdown.go,
  * evg_host_drawdown below, which can read this call's reports where they are).
- * EVG_ERR_INVALID with nothing launched: null cfg or out (or a null array of out), a negative n_provisioning.
+ * EVG_ERR_INVALID with nothing launched and the tick as it was: null cfg or out (or a null array of out), a negative
+ * n_provisioning or a negative spawned count (the message names the row).
  * EVG_ERR_STATE: no resident tick, a tick without hosts, or no evg_run_resident on it since it was set (the one-shot
  * evg_plan_and_alloc_batch counts as one).  The first call allocates the call's own small buffers.
  * Replaces: the single-task bypass, the time-to-empty report and the drawdown decision of hostAllocatorJob.Run. */

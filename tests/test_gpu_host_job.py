@@ -273,8 +273,9 @@ def test_error_contract(world):
         out = {k: np.zeros(D, dt) for k, dt in (("n_hosts", np.int64), ("n_hosts_free", np.int64), ("status", np.int32),
                                                 ("report", L.HOST_REPORT_DTYPE))}
         st = L.HostJobOutStruct(*[L.ptr(out[f]) for f in ("n_hosts", "n_hosts_free", "status", "report")])
-        call = lambda c=cfg, o=st: eng.lib.evg_host_job(eng.ctx, L.ptr(c) if c is not None else None, None,  # noqa: E731
-                                                          C.byref(o) if o is not None else None)
+        call = lambda c=cfg, o=st, sp=None: eng.lib.evg_host_job(eng.ctx, L.ptr(c) if c is not None else None,  # noqa: E731
+                                                                   L.ptr(sp) if sp is not None else None,
+                                                                   C.byref(o) if o is not None else None)
         assert call() == L.EVG_ERR_STATE  # no tick
         eng.upload(p.tasks, p.distros)
         eng.run(p.now)
@@ -289,6 +290,12 @@ def test_error_contract(world):
         neg["n_provisioning"][1] = -1
         assert call(c=neg) == L.EVG_ERR_INVALID and "n_provisioning" in L.last_error()
         assert call() == L.EVG_OK
+        sp = np.full(D, 2, np.int32)
+        sp[D - 1] = -1  # len(hostsSpawned) is never negative
+        assert call(sp=sp) == L.EVG_ERR_INVALID and f"spawned[{D - 1}]" in L.last_error()
+        iw = synth.make_idle_hosts(np.full(D, 3), 1451)  # the rejected call left the last reports for a chained drawdown
+        eng.host_drawdown(S.marshal_idle_hosts(iw.groups), np.asarray(iw.existing, np.int64), iw.now)
+        assert call(sp=sp + 1) == L.EVG_OK
         eng.bind_result_buffer(0, 0)
         assert call() == L.EVG_ERR_STATE  # the run's rows are not in the buffer bound now
         eng.run(p.now)
