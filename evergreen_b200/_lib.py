@@ -113,6 +113,14 @@ class DepsInStruct(C.Structure):
                 ("ext_state", C.c_void_p), ("n_ext", C.c_int64)]
 
 
+class DepsEditStruct(C.Structure):
+    _fields_ = [("depart_ext", C.c_void_p), ("depart_finished_ns", C.c_void_p), ("n_ext", C.c_int64), ("ext_state", C.c_void_p),
+                ("ext_finished_ns", C.c_void_p), ("insert", C.POINTER(DepsInStruct)), ("insert_finished_ns", C.c_void_p),
+                ("n_add", C.c_int64), ("add_row", C.c_void_p), ("add_kind", C.c_void_p), ("add_ref", C.c_void_p),
+                ("add_want", C.c_void_p), ("add_finished_ns", C.c_void_p), ("n_set", C.c_int64), ("set_row", C.c_void_p),
+                ("set_state", C.c_void_p), ("set_pre", C.c_void_p)]
+
+
 EVG_DEP_IN_QUEUE, EVG_DEP_EXTERNAL, EVG_DEP_MISSING = 0, 1, 2
 EVG_WANT_SUCCESS, EVG_WANT_FAILED, EVG_WANT_ANY, EVG_WANT_OTHER = 0, 1, 2, 3
 EVG_TS_BLOCKED = 0x4
@@ -333,6 +341,7 @@ SYMBOLS = {
     "evg_upload_device": (C.c_int, [_P, _P, _P, _P, _P, _P]),
     "evg_update_tasks": (C.c_int, [_P, C.c_int64, _P, _P]),
     "evg_edit_tasks": (C.c_int, [_P, _P, _P, _P, _P, _P]),
+    "evg_edit_tasks_with_deps": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_int64, _P, _P, _P, C.c_int64]),
     "evg_plan_from_finder": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, C.c_int64, _P, _P]),
     "evg_plan_from_finder_ex": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int64, _P, _P]),
     "evg_plan_aliases": (C.c_int, [_P, _P, _P, C.c_int32, C.c_int64, _P]),

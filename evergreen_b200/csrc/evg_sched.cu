@@ -1477,7 +1477,8 @@ struct evg_ctx {
   cudaEvent_t ev_fork = nullptr, ev_join[kAux] = {};
   // The resident tick (need_tick checks it; upload_tasks and drop_tick replace it), and whether the allocator's tables,
   // evg_upload_with_deps' verdicts (`deps`), evg_plan_aliases' map (`al`) and evg_resolve_durations' results (`dur`)
-  // belong to it.  `allocated`: run state -- the allocator's results (queue and group infos, result rows, status) are
+  // belong to it.  `dep_table`: the staged dependency table in `deps` is the resident tick's own, with the stamps of its
+  // last evaluation (evg_upload_with_deps, evg_edit_tasks_with_deps), so evg_edit_tasks_with_deps can edit it.  `allocated`: run state -- the allocator's results (queue and group infos, result rows, status) are
   // from a run on this tick, into the result buffer bound now; evg_host_job reads them.  `host_job`: run state --
   // evg_host_job's reports in hj.out are from the current run; a chained evg_host_drawdown reads them.  `dispatchers`:
   // run state -- evg_rebuild_dispatchers built dp and nx from the current run; evg_find_next_tasks serves from them.
@@ -1486,7 +1487,7 @@ struct evg_ctx {
   struct {
     Tick kind = Tick::kNone;
     bool hosts = false, deps = false, aliases = false, durations = false, allocated = false, host_job = false, dispatchers = false;
-    bool queue_breakdown = false;
+    bool queue_breakdown = false, dep_table = false;
   } tick;
   int64_t T = 0, E = 0, G = 0, H = 0, U = 0, NT = 0, t_pad = 0;
   int32_t Dn = 0;
@@ -1501,6 +1502,13 @@ struct evg_ctx {
   struct {
     DevBuf off, kind, ref, want, state, pre, ext;  // an evg_deps_in table, staged
     DevBuf met, fin, stamp;                        // k_deps_met's verdicts, its dep_finished_ns input, its stamps
+    int64_t E = 0;                                 // while tick.dep_table: the table's entry count, and whether `fin`
+    bool has_fin = false;                          // holds their FinishedAt (else every one is the zero time)
+    // evg_edit_tasks_with_deps: the shadow set the composed table is written to (swapped with the one above), the
+    // staged dependency edit, the per-row entry counts and the error word
+    DevBuf s_off, s_kind, s_ref, s_want, s_state, s_pre, s_ext, s_fin, s_stamp;
+    DevBuf x_dext, x_dfin, x_efin, x_ioff, x_ikind, x_iref, x_iwant, x_ifin, x_istate, x_ipre;
+    DevBuf x_arow, x_akind, x_aref, x_awant, x_afin, x_srow, x_sstate, x_spre, cnt, err;
   } deps;
   struct {
     DevBuf task_off, sched, project, project_flags, valid_off, valid_idx, finder;  // the finder tables
@@ -1657,7 +1665,7 @@ void drop_tick(evg_ctx* c) { c->tick = {}; }
 // What a call needs of the resident tick.  EVG_ERR_STATE names the call and the first unmet condition: a tick, then
 // its kind, then the state the call reads.
 enum class Need { kTick, kOwnColumns, kEditable, kHosts, kVerdicts, kAliasMap, kDurations, kAllocated, kHostJob, kDispatchers,
-                  kQueueBreakdown };
+                  kQueueBreakdown, kDepTable };
 int need_tick(const evg_ctx* c, const char* who, Need what) {
   const auto& t = c->tick;
   const bool own = what == Need::kOwnColumns || what == Need::kEditable;
@@ -1667,6 +1675,8 @@ int need_tick(const evg_ctx* c, const char* who, Need what) {
                       : (what == Need::kHosts || what == Need::kAllocated) && !t.hosts ? "the resident tick has no hosts"
                       : what == Need::kAllocated && !t.allocated          ? "no allocator run on the resident tick since it was set or a result buffer was bound"
                       : what == Need::kVerdicts && !t.deps                ? "the resident tick was not uploaded with evg_upload_with_deps"
+                      : what == Need::kDepTable && !t.dep_table
+                          ? "the resident tick holds no dependency table (evg_upload_with_deps or evg_edit_tasks_with_deps set one)"
                       : what == Need::kAliasMap && !t.aliases             ? "the resident tick was not built by evg_plan_aliases"
                       : what == Need::kDurations && !t.durations          ? "no evg_resolve_durations on the resident tick's rows"
                       : what == Need::kHostJob && !t.host_job             ? "no evg_host_job on the resident tick's current run"
@@ -2359,14 +2369,11 @@ __global__ void __launch_bounds__(256) k_update_rows(int64_t n, const int64_t* _
   expected[r] = v_expected[i]; qbasis[r] = v_qbasis[i]; wbasis[r] = v_wbasis[i];
 }
 
-int evg_update_tasks(evg_ctx* c, int64_t n_rows, const int64_t* rows, const evg_task_soa* v) {
-  ENTER(c, "evg_update_tasks");
-  if (const int rc = need_tick(c, who, Need::kOwnColumns); rc != EVG_OK) return rc;
-  if (n_rows < 0) return fail(EVG_ERR_INVALID, "negative row count");
-  if (n_rows == 0) return EVG_OK;
+// evg_update_tasks' write of n_rows > 0 rows into the resident columns (the caller checked the tick).
+static int update_rows(evg_ctx* c, const char* who, int64_t n_rows, const int64_t* rows, const evg_task_soa* v) {
   if (!rows || !v || v->n_tasks != n_rows || TaskCols::missing(v, /*ids=*/false))
-    return fail(EVG_ERR_INVALID, "evg_update_tasks: rows and a %lld-row value table (priority, num_dependents, task_group_order, flags, "
-                                 "expected_ns, queue_basis_ns, wait_basis_ns) are required", (long long)n_rows);
+    return fail(EVG_ERR_INVALID, "%s: rows and a %lld-row value table (priority, num_dependents, task_group_order, flags, "
+                                 "expected_ns, queue_basis_ns, wait_basis_ns) are required", who, (long long)n_rows);
   cudaStream_t s = c->stream;
   const size_t n = size_t(n_rows);
   // staging: rows (8) + the nine columns but group_id and version_id, the 8-byte ones first = 48 B per changed row
@@ -2394,7 +2401,17 @@ int evg_update_tasks(evg_ctx* c, int64_t n_rows, const int64_t* rows, const evg_
   int h_bad = 0;
   CK(cudaMemcpyAsync(&h_bad, bad, sizeof(int), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));  // the caller's staging arrays are free again
-  if (h_bad) return fail(EVG_ERR_INVALID, "evg_update_tasks: a row index is outside [0, n_tasks)");
+  if (h_bad) return fail(EVG_ERR_INVALID, "%s: a row index is outside [0, n_tasks)", who);
+  return EVG_OK;
+}
+
+int evg_update_tasks(evg_ctx* c, int64_t n_rows, const int64_t* rows, const evg_task_soa* v) {
+  ENTER(c, "evg_update_tasks");
+  if (const int rc = need_tick(c, who, Need::kOwnColumns); rc != EVG_OK) return rc;
+  if (n_rows < 0) return fail(EVG_ERR_INVALID, "negative row count");
+  if (n_rows == 0) return EVG_OK;
+  const int rc = update_rows(c, who, n_rows, rows, v);
+  if (rc != EVG_OK) return rc;
   c->tick.deps = false;  // flags / wait bases written by a device-side dependency evaluation may have been replaced
   return EVG_OK;
 }
@@ -2800,14 +2817,15 @@ int evg_alloc_batch(evg_ctx* c, const evg_host_soa* hosts, const int64_t* host_o
 }
 
 // The device view of the dependency table deps_to_device staged from `in`.
-static DDeps ddeps(const evg_ctx* c, const evg_deps_in* in) {
+static DDeps ddeps_sized(const evg_ctx* c, int64_t T, int64_t E, int64_t X) {
   const auto& x = c->deps;
   DDeps d;
-  d.n_tasks = in->n_tasks; d.n_deps = in->n_deps; d.n_ext = in->n_ext;
+  d.n_tasks = T; d.n_deps = E; d.n_ext = X;
   d.dep_off = x.off.as<int64_t>(); d.dep_kind = x.kind.as<uint8_t>(); d.dep_ref = x.ref.as<int32_t>(); d.dep_want = x.want.as<uint8_t>();
   d.task_state = x.state.as<uint8_t>(); d.task_pre = x.pre.as<uint8_t>(); d.ext_state = x.ext.as<uint8_t>();
   return d;
 }
+static DDeps ddeps(const evg_ctx* c, const evg_deps_in* in) { return ddeps_sized(c, in->n_tasks, in->n_deps, in->n_ext); }
 
 // Stage an evg_deps_in table and run k_deps_met into deps.met (left on the device); `both` adds the no-short-circuit bit.
 // The host checks the ends of dep_off; its rows, n_tasks of them, are checked by k_deps_met (kErrDepOff).
@@ -2861,7 +2879,7 @@ int evg_deps_met_batch(evg_ctx* c, const evg_deps_in* in, uint8_t* met) {
   CK(c->b_err.ensure(sizeof(int) * 4));
   CK(cudaMemsetAsync(c->b_err.p, 0, sizeof(int) * 4, s));
   c->launches = 0;
-  c->tick.deps = false;  // deps_to_device overwrites the resident tick's verdicts and stamps
+  c->tick.deps = c->tick.dep_table = false;  // deps_to_device overwrites the resident tick's table, verdicts and stamps
   int rc = deps_to_device(c, who, in, 0);
   if (rc != EVG_OK) return rc;
   int bad = 0;
@@ -2881,7 +2899,12 @@ int evg_upload_with_deps(evg_ctx* c, const evg_task_soa* tasks, const evg_distro
   int rc = upload(c, who, tasks, distros, hosts, host_off, acfg, Tick::kOwn);
   if (rc != EVG_OK) return rc;
   const int64_t T = tasks->n_tasks;
-  if (T == 0) return EVG_OK;
+  c->deps.E = T > 0 ? deps->n_deps : 0;
+  c->deps.has_fin = T > 0 && dep_finished_ns && deps->n_deps > 0;
+  if (T == 0) {
+    c->tick.dep_table = true;
+    return EVG_OK;
+  }
   cudaStream_t s = c->stream;
   rc = deps_to_device(c, who, deps, 0, dep_finished_ns, now_ns, /*want_stamp=*/true);
   if (rc != EVG_OK) { drop_tick(c); return rc; }
@@ -2892,7 +2915,7 @@ int evg_upload_with_deps(evg_ctx* c, const evg_task_soa* tasks, const evg_distro
   CK(cudaMemcpyAsync(&bad, c->b_err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   if (bad) { drop_tick(c); return deps_bad(who, bad); }
-  c->tick.deps = true;
+  c->tick.deps = c->tick.dep_table = true;
   return EVG_OK;
 }
 
@@ -3569,29 +3592,33 @@ int evg_plan_from_finder_ex(evg_ctx* c, const evg_runnable_in* in, const evg_pip
 // --------------------------------------------------------------------------
 // evg_edit_tasks: the composed table (survivors, then inserted rows, per distro) built on the device
 // --------------------------------------------------------------------------
-int evg_edit_tasks(evg_ctx* c, const evg_task_edit* ed, const evg_distro_table* distros, const evg_host_soa* hosts,
-                   const int64_t* host_off, const evg_alloc_cfg* acfg) {
-  ENTER(c, "evg_edit_tasks");
-  if (const int rc = need_tick(c, who, Need::kEditable); rc != EVG_OK) return rc;
-  if (!ed || !distros) return fail(EVG_ERR_INVALID, "evg_edit_tasks: null edit / distro table");
-  // ---- every check the host can make, before anything resident changes
+// The host's half of an edit of the resident tick: every check the host can make, before anything resident changes, and
+// the per-distro tables apply_edit stages.
+struct EditPlan {
+  std::vector<int64_t> ins_off, old_vbase;  // D+1: the inserted rows' CSR over distros, prefix sum of the old n_versions
+  int64_t Tn = 0;                           // rows of the composed table
+};
+static int check_edit(evg_ctx* c, const char* who, const evg_task_edit* ed, const evg_distro_table* distros, EditPlan* p) {
+  if (!ed || !distros) return fail(EVG_ERR_INVALID, "%s: null edit / distro table", who);
   const int32_t D = c->Dn;
   const int64_t T0 = c->T, R = ed->n_remove, NA = ed->n_add_edges;
   const evg_task_soa* ins = ed->insert;
   const int64_t I = ins ? ins->n_tasks : 0, EI = ins ? ins->n_edges : 0;
-  if (distros->n_distros != D) return fail(EVG_ERR_INVALID, "evg_edit_tasks: n_distros %d, the resident tick has %d", distros->n_distros, D);
-  if (R < 0 || I < 0 || EI < 0 || NA < 0) return fail(EVG_ERR_INVALID, "evg_edit_tasks: negative sizes");
-  if (R > 0 && !ed->remove_rows) return fail(EVG_ERR_INVALID, "evg_edit_tasks: null remove_rows");
-  if (I > 0 && (!ed->insert_off || TaskCols::missing(ins))) return fail(EVG_ERR_INVALID, "evg_edit_tasks: null insert_off / inserted column");
-  if (EI > 0 && (I == 0 || !ins->dep_off || !ins->dep_idx)) return fail(EVG_ERR_INVALID, "evg_edit_tasks: inserted edges without dep_off / dep_idx");
-  if (NA > 0 && (!ed->add_edge_task || !ed->add_edge_dep)) return fail(EVG_ERR_INVALID, "evg_edit_tasks: null added edges");
-  if (D > 0 && (!distros->task_off || !distros->group_off || !distros->cfg)) return fail(EVG_ERR_INVALID, "evg_edit_tasks: null distro arrays");
-  if (D == 0 && (R > 0 || I > 0)) return fail(EVG_ERR_INVALID, "evg_edit_tasks: rows without distros");
-  std::vector<int64_t> removed(size_t(D) + 1, 0), ins_off(size_t(D) + 1, 0), old_vbase(size_t(D) + 1, 0);
+  if (distros->n_distros != D) return fail(EVG_ERR_INVALID, "%s: n_distros %d, the resident tick has %d", who, distros->n_distros, D);
+  if (R < 0 || I < 0 || EI < 0 || NA < 0) return fail(EVG_ERR_INVALID, "%s: negative sizes", who);
+  if (R > 0 && !ed->remove_rows) return fail(EVG_ERR_INVALID, "%s: null remove_rows", who);
+  if (I > 0 && (!ed->insert_off || TaskCols::missing(ins))) return fail(EVG_ERR_INVALID, "%s: null insert_off / inserted column", who);
+  if (EI > 0 && (I == 0 || !ins->dep_off || !ins->dep_idx)) return fail(EVG_ERR_INVALID, "%s: inserted edges without dep_off / dep_idx", who);
+  if (NA > 0 && (!ed->add_edge_task || !ed->add_edge_dep)) return fail(EVG_ERR_INVALID, "%s: null added edges", who);
+  if (D > 0 && (!distros->task_off || !distros->group_off || !distros->cfg)) return fail(EVG_ERR_INVALID, "%s: null distro arrays", who);
+  if (D == 0 && (R > 0 || I > 0)) return fail(EVG_ERR_INVALID, "%s: rows without distros", who);
+  std::vector<int64_t> removed(size_t(D) + 1, 0), &ins_off = p->ins_off, &old_vbase = p->old_vbase;
+  ins_off.assign(size_t(D) + 1, 0);
+  old_vbase.assign(size_t(D) + 1, 0);
   for (int64_t k = 0; k < R; k++) {
     const int64_t r = ed->remove_rows[k];
     if (r < 0 || r >= T0 || (k > 0 && r <= ed->remove_rows[k - 1]))
-      return fail(EVG_ERR_INVALID, "evg_edit_tasks: remove_rows[%lld] = %lld is not ascending inside [0, %lld)", (long long)k, (long long)r, (long long)T0);
+      return fail(EVG_ERR_INVALID, "%s: remove_rows[%lld] = %lld is not ascending inside [0, %lld)", who, (long long)k, (long long)r, (long long)T0);
     removed[size_t(std::upper_bound(c->h_taskoff.begin(), c->h_taskoff.end(), r) - c->h_taskoff.begin() - 1)]++;
   }
   int rc = I > 0 ? check_offsets(ed->insert_off, D, I, who, "insert_off") : EVG_OK;
@@ -3603,23 +3630,34 @@ int evg_edit_tasks(evg_ctx* c, const evg_task_edit* ed, const evg_distro_table* 
   for (int32_t d = 0; d < D; d++) {
     const int64_t want = (c->h_taskoff[d + 1] - c->h_taskoff[d]) - removed[d] + (ins_off[d + 1] - ins_off[d]);
     if (distros->task_off[d + 1] - distros->task_off[d] != want)
-      return fail(EVG_ERR_INVALID, "evg_edit_tasks: distro %d holds %lld tasks after the edit, task_off says %lld", d, (long long)want,
+      return fail(EVG_ERR_INVALID, "%s: distro %d holds %lld tasks after the edit, task_off says %lld", who, d, (long long)want,
                   (long long)(distros->task_off[d + 1] - distros->task_off[d]));
     old_vbase[d + 1] = old_vbase[d] + c->h_nver[d];
   }
-  const int64_t Tn = D > 0 ? distros->task_off[D] : 0;
+  const int64_t Tn = p->Tn = D > 0 ? distros->task_off[D] : 0;
   for (int64_t k = 0, d = 0; k < NA; k++) {
     const int64_t row = ed->add_edge_task[k];
-    if (k > 0 && row < ed->add_edge_task[k - 1]) return fail(EVG_ERR_INVALID, "evg_edit_tasks: add_edge_task is not ascending at %lld", (long long)k);
-    if (row < 0 || row >= Tn) return fail(EVG_ERR_INVALID, "evg_edit_tasks: add_edge_task[%lld] = %lld is outside the composed table", (long long)k, (long long)row);
+    if (k > 0 && row < ed->add_edge_task[k - 1]) return fail(EVG_ERR_INVALID, "%s: add_edge_task is not ascending at %lld", who, (long long)k);
+    if (row < 0 || row >= Tn) return fail(EVG_ERR_INVALID, "%s: add_edge_task[%lld] = %lld is outside the composed table", who, (long long)k, (long long)row);
     while (distros->task_off[d + 1] <= row) d++;
     const int64_t survivors = (c->h_taskoff[d + 1] - c->h_taskoff[d]) - removed[d];
     if (row - distros->task_off[d] >= survivors)
-      return fail(EVG_ERR_INVALID, "evg_edit_tasks: add_edge_task[%lld] = %lld is not a surviving task", (long long)k, (long long)row);
+      return fail(EVG_ERR_INVALID, "%s: add_edge_task[%lld] = %lld is not a surviving task", who, (long long)k, (long long)row);
   }
+  return EVG_OK;
+}
+
+// The device's half: the composed table becomes the resident tick (a device-side error leaves none).
+static int apply_edit(evg_ctx* c, const char* who, const evg_task_edit* ed, const evg_distro_table* distros, const evg_host_soa* hosts,
+                      const int64_t* host_off, const evg_alloc_cfg* acfg, const EditPlan& p) {
+  const int32_t D = c->Dn;
+  const int64_t T0 = c->T, R = ed->n_remove, NA = ed->n_add_edges;
+  const evg_task_soa* ins = ed->insert;
+  const int64_t I = ins ? ins->n_tasks : 0, EI = ins ? ins->n_edges : 0;
+  const std::vector<int64_t>&ins_off = p.ins_off, &old_vbase = p.old_vbase;
+  int rc = EVG_OK;
   cudaStream_t s = c->stream;
   auto& e = c->ed;
-  c->launches = 0;
   // ---- stage the edit
   UP(s, e.rm, ed->remove_rows, R, int64_t);
   if (I > 0 && (rc = e.ins.stage(ins, I, s)) != EVG_OK) return rc;
@@ -3653,6 +3691,282 @@ int evg_edit_tasks(evg_ctx* c, const evg_task_edit* ed, const evg_distro_table* 
     CK(cudaStreamSynchronize(s));
   }
   c->tick.kind = Tick::kOwn;
+  return EVG_OK;
+}
+
+int evg_edit_tasks(evg_ctx* c, const evg_task_edit* ed, const evg_distro_table* distros, const evg_host_soa* hosts,
+                   const int64_t* host_off, const evg_alloc_cfg* acfg) {
+  ENTER(c, "evg_edit_tasks");
+  if (const int rc = need_tick(c, who, Need::kEditable); rc != EVG_OK) return rc;
+  EditPlan p;
+  if (const int rc = check_edit(c, who, ed, distros, &p); rc != EVG_OK) return rc;
+  c->launches = 0;
+  return apply_edit(c, who, ed, distros, hosts, host_off, acfg, p);
+}
+
+// --------------------------------------------------------------------------
+// evg_edit_tasks_with_deps: the edit, the update, then the dependency table composed on the device and evaluated
+// --------------------------------------------------------------------------
+// The previous tick's table (c->deps), the staged dependency edit and the shadow set the composed table goes to.
+struct DxEdit {
+  int64_t T0, Xn;  // rows of the previous table, ids of the new external table
+  const int64_t* off; const uint8_t* kind; const int32_t* ref; const uint8_t* want; const int64_t* fin;  // fin: NULL = zero
+  const uint8_t* state; const uint8_t* pre; const int64_t* stamp;  // per previous row; stamp: its last evaluation's
+  const int32_t* dext; const int64_t* dfin; const int64_t* efin;   // per removed row (dfin may be NULL), per ext id (NULL)
+  const int64_t* ioff; const uint8_t* ikind; const int32_t* iref; const uint8_t* iwant; const int64_t* ifin;  // inserted rows'
+  const uint8_t* istate; const uint8_t* ipre;
+  int64_t n_add; const int64_t* arow; const uint8_t* akind; const int32_t* aref; const uint8_t* awant; const int64_t* afin;
+  int64_t* o_off; uint8_t* o_kind; int32_t* o_ref; uint8_t* o_want; int64_t* o_fin; uint8_t* o_state; uint8_t* o_pre;
+};
+// Error bits of the composition: a previous in-queue ref outside the previous table, a survivor's entry on a removed
+// row whose depart_ext is -1, a survivor's external ref outside the new external table.
+constexpr int kDxBadRef = 1, kDxDeparted = 2, kDxBadExt = 4;
+__device__ __forceinline__ bool dx_stamped(int64_t s) { return s != EVG_TIME_ZERO && s != 0; }  // !IsZeroTime(DependenciesMetTime)
+// Per composed row i: its entry count, and its task_state / task_pre (a survivor's previous ones, task_pre with the
+// write-back of its last stamp; an inserted row's own).
+__global__ void __launch_bounds__(256) k_dx_count(int64_t n_new, EdMap m, DxEdit X, int32_t* __restrict__ cnt) {
+  const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  const int d = block_find_distro(m.new_off, m.D, i, n_new);
+  if (d < 0) return;
+  const int64_t k = i - m.new_off[d], S = ed_survivors(m, d);
+  if (k < S) {
+    const int64_t t = m.src[i];
+    int64_t n = X.off[t + 1] - X.off[t];
+    if (X.n_add > 0)
+      for (int64_t a = ed_lower(X.arow, X.n_add, i); a < X.n_add && X.arow[a] == i; a++) n++;
+    cnt[i] = int32_t(n);
+    X.o_state[i] = X.state[t];
+    X.o_pre[i] = uint8_t(X.pre[t] | (dx_stamped(X.stamp[t]) ? EVG_TP_MET_TIME : 0u));
+  } else {
+    const int64_t j = m.ins_off[d] + (k - S);
+    cnt[i] = int32_t(X.ioff[j + 1] - X.ioff[j]);
+    X.o_state[i] = X.istate[j];
+    X.o_pre[i] = X.ipre[j];
+  }
+}
+// Per composed row i: its entries at o_off[i] (see evg_edit_tasks_with_deps for the rules).
+__global__ void __launch_bounds__(256) k_dx_write(int64_t n_new, EdMap m, DxEdit X, int* __restrict__ err) {
+  const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  const int d = block_find_distro(m.new_off, m.D, i, n_new);
+  if (d < 0) return;
+  const int64_t k = i - m.new_off[d], S = ed_survivors(m, d);
+  int64_t w = X.o_off[i];
+  int bad = 0;
+  auto put = [&](uint8_t kind, int32_t ref, uint8_t want, int64_t fin) {
+    if (kind == EVG_DEP_EXTERNAL && X.efin && ref >= 0 && ref < X.Xn) fin = X.efin[ref];
+    X.o_kind[w] = kind; X.o_ref[w] = ref; X.o_want[w] = want; X.o_fin[w] = fin;
+    w++;
+  };
+  if (k < S) {
+    const int64_t t = m.src[i];
+    for (int64_t e = X.off[t]; e < X.off[t + 1]; e++) {
+      uint8_t kind = X.kind[e];
+      int32_t ref = X.ref[e];
+      int64_t fin = X.fin ? X.fin[e] : EVG_TIME_ZERO;
+      if (kind == EVG_DEP_IN_QUEUE) {
+        if (ref < 0 || ref >= X.T0) {
+          bad |= kDxBadRef;
+        } else if (m.keep[ref]) {
+          ref = int32_t(m.pos[ref] + m.ins_off[find_distro(m.old_off, 0, m.D - 1, ref)]);
+        } else {
+          const int64_t r = ref - m.pos[ref];  // the removed row's index in remove_rows
+          kind = EVG_DEP_EXTERNAL;
+          ref = X.dext[r];
+          if (ref < 0) bad |= kDxDeparted;
+          if (X.dfin) fin = X.dfin[r];
+        }
+      } else if (kind == EVG_DEP_EXTERNAL && (ref < 0 || ref >= X.Xn)) {
+        bad |= kDxBadExt;
+      }
+      put(kind, ref, X.want[e], fin);
+    }
+    if (X.n_add > 0)
+      for (int64_t a = ed_lower(X.arow, X.n_add, i); a < X.n_add && X.arow[a] == i; a++)
+        put(X.akind[a], X.aref[a], X.awant[a], X.afin ? X.afin[a] : EVG_TIME_ZERO);
+  } else {
+    const int64_t j = m.ins_off[d] + (k - S);
+    for (int64_t e = X.ioff[j]; e < X.ioff[j + 1]; e++) put(X.ikind[e], X.iref[e], X.iwant[e], X.ifin ? X.ifin[e] : EVG_TIME_ZERO);
+  }
+  if (bad) atomicOr(err, bad);
+}
+__global__ void __launch_bounds__(256) k_dx_set(int64_t n, const int64_t* __restrict__ row, const uint8_t* __restrict__ state,
+                                                const uint8_t* __restrict__ pre, uint8_t* __restrict__ o_state, uint8_t* __restrict__ o_pre) {
+  const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  o_state[row[i]] = state[i];
+  o_pre[row[i]] = pre[i];
+}
+
+// What the host can check of a dependency edit against the edit it goes with (p: check_edit's plan).
+static int check_deps_edit(const char* who, const evg_task_edit* ed, const evg_distro_table* distros, const EditPlan& p,
+                           const evg_deps_edit* x) {
+  const int64_t R = ed->n_remove, I = ed->insert ? ed->insert->n_tasks : 0, Tn = p.Tn, X = x->n_ext;
+  if (X < 0 || x->n_add < 0 || x->n_set < 0) return fail(EVG_ERR_INVALID, "%s: negative dependency-edit sizes", who);
+  if (R > 0 && !x->depart_ext) return fail(EVG_ERR_INVALID, "%s: null depart_ext", who);
+  if (X > 0 && !x->ext_state) return fail(EVG_ERR_INVALID, "%s: null ext_state", who);
+  for (int64_t k = 0; k < R; k++)
+    if (x->depart_ext[k] < -1 || x->depart_ext[k] >= X)
+      return fail(EVG_ERR_INVALID, "%s: depart_ext[%lld] = %d is outside [-1, n_ext = %lld)", who, (long long)k, x->depart_ext[k], (long long)X);
+  // one entry list (kind, ref) checked against the composed table and the new external table
+  auto refs_ok = [&](const char* what, int64_t n, const uint8_t* kind, const int32_t* ref) -> int {
+    for (int64_t e = 0; e < n; e++) {
+      const int64_t hi = kind[e] == EVG_DEP_IN_QUEUE ? Tn : kind[e] == EVG_DEP_EXTERNAL ? X : INT64_MAX;
+      if (hi != INT64_MAX && (ref[e] < 0 || ref[e] >= hi))
+        return fail(EVG_ERR_INVALID, "%s: %s[%lld] = %d is outside the table it indexes (%lld rows)", who, what, (long long)e, ref[e], (long long)hi);
+    }
+    return EVG_OK;
+  };
+  const evg_deps_in* in = x->insert;
+  if (I > 0 || (in && in->n_tasks > 0)) {
+    if (!in || in->n_tasks != I) return fail(EVG_ERR_INVALID, "%s: the inserted rows' dependency table covers %lld rows, the edit inserts %lld",
+                                             who, in ? (long long)in->n_tasks : 0ll, (long long)I);
+    if (in->n_deps < 0) return fail(EVG_ERR_INVALID, "%s: negative sizes", who);
+    if (!in->dep_off || !in->task_state || !in->task_pre) return fail(EVG_ERR_INVALID, "%s: null inserted task arrays", who);
+    if (in->n_deps > 0 && (!in->dep_kind || !in->dep_ref || !in->dep_want)) return fail(EVG_ERR_INVALID, "%s: null inserted dependency arrays", who);
+    if (const int rc = check_offsets(in->dep_off, I, in->n_deps, who, "deps->insert->dep_off"); rc != EVG_OK) return rc;
+    if (const int rc = refs_ok("deps->insert->dep_ref", in->n_deps, in->dep_kind, in->dep_ref); rc != EVG_OK) return rc;
+  }
+  if (x->n_add > 0) {
+    if (!x->add_row || !x->add_kind || !x->add_ref || !x->add_want) return fail(EVG_ERR_INVALID, "%s: null added entries", who);
+    for (int64_t k = 0, d = 0; k < x->n_add; k++) {
+      const int64_t row = x->add_row[k];
+      if (k > 0 && row < x->add_row[k - 1]) return fail(EVG_ERR_INVALID, "%s: deps->add_row is not ascending at %lld", who, (long long)k);
+      if (row < 0 || row >= Tn) return fail(EVG_ERR_INVALID, "%s: deps->add_row[%lld] = %lld is outside the composed table", who, (long long)k, (long long)row);
+      while (distros->task_off[d + 1] <= row) d++;
+      const int64_t survivors = (distros->task_off[d + 1] - distros->task_off[d]) - (p.ins_off[d + 1] - p.ins_off[d]);
+      if (row - distros->task_off[d] >= survivors)
+        return fail(EVG_ERR_INVALID, "%s: deps->add_row[%lld] = %lld is not a surviving task", who, (long long)k, (long long)row);
+    }
+    if (const int rc = refs_ok("deps->add_ref", x->n_add, x->add_kind, x->add_ref); rc != EVG_OK) return rc;
+  }
+  if (x->n_set > 0) {
+    if (!x->set_row || !x->set_state || !x->set_pre) return fail(EVG_ERR_INVALID, "%s: null state changes", who);
+    for (int64_t k = 0; k < x->n_set; k++)
+      if (x->set_row[k] < 0 || x->set_row[k] >= Tn)
+        return fail(EVG_ERR_INVALID, "%s: deps->set_row[%lld] = %lld is outside the composed table", who, (long long)k, (long long)x->set_row[k]);
+  }
+  return EVG_OK;
+}
+
+int evg_edit_tasks_with_deps(evg_ctx* c, const evg_task_edit* ed, const evg_distro_table* distros, const evg_host_soa* hosts,
+                             const int64_t* host_off, const evg_alloc_cfg* acfg, int64_t n_rows, const int64_t* rows,
+                             const evg_task_soa* v, const evg_deps_edit* x, int64_t now_ns) {
+  ENTER(c, "evg_edit_tasks_with_deps");
+  if (const int rc = need_tick(c, who, Need::kEditable); rc != EVG_OK) return rc;
+  if (const int rc = need_tick(c, who, Need::kDepTable); rc != EVG_OK) return rc;
+  if (!x) return fail(EVG_ERR_INVALID, "%s: null dependency edit", who);
+  // ---- every check the host can make, before anything resident changes
+  EditPlan p;
+  int rc = check_edit(c, who, ed, distros, &p);
+  if (rc == EVG_OK) rc = check_deps_edit(who, ed, distros, p, x);
+  if (rc != EVG_OK) return rc;
+  if (n_rows < 0) return fail(EVG_ERR_INVALID, "negative row count");
+  for (int64_t k = 0; k < n_rows; k++)
+    if (!rows || rows[k] < 0 || rows[k] >= p.Tn)
+      return fail(EVG_ERR_INVALID, "%s: rows[%lld] is outside the composed table", who, (long long)k);
+  if (n_rows > 0 && (!v || v->n_tasks != n_rows || TaskCols::missing(v, /*ids=*/false)))
+    return fail(EVG_ERR_INVALID, "%s: rows and a %lld-row value table (priority, num_dependents, task_group_order, flags, "
+                                 "expected_ns, queue_basis_ns, wait_basis_ns) are required", who, (long long)n_rows);
+  const int64_t T0 = c->T, E0 = c->deps.E, R = ed->n_remove, Tn = p.Tn, Xn = x->n_ext;
+  const evg_deps_in* in = x->insert;
+  const int64_t I = ed->insert ? ed->insert->n_tasks : 0, EI = I > 0 ? in->n_deps : 0, NA = x->n_add;
+  const int64_t En_max = E0 + EI + NA;  // entries only move or join: the composed table has at most these
+  const bool old_fin = c->deps.has_fin;
+  c->launches = 0;
+  // ---- 1-2. the task edit, then the changed rows (its checks passed above)
+  rc = apply_edit(c, who, ed, distros, hosts, host_off, acfg, p);
+  if (rc != EVG_OK) return rc;
+  if (n_rows > 0 && (rc = update_rows(c, who, n_rows, rows, v)) != EVG_OK) return rc;
+  // ---- 3. the composed dependency table into the shadow set: counts and states, the scan, the entries, the changes
+  cudaStream_t s = c->stream;
+  auto& y = c->deps;
+  UP(s, y.x_dext, x->depart_ext, R, int32_t);
+  UP(s, y.x_dfin, x->depart_finished_ns, x->depart_finished_ns ? R : 0, int64_t);
+  UP(s, y.x_efin, x->ext_finished_ns, x->ext_finished_ns ? Xn : 0, int64_t);
+  UP(s, y.x_ioff, I > 0 ? in->dep_off : nullptr, I > 0 ? I + 1 : 0, int64_t);
+  UP(s, y.x_ikind, I > 0 ? in->dep_kind : nullptr, EI, uint8_t);
+  UP(s, y.x_iref, I > 0 ? in->dep_ref : nullptr, EI, int32_t);
+  UP(s, y.x_iwant, I > 0 ? in->dep_want : nullptr, EI, uint8_t);
+  UP(s, y.x_ifin, x->insert_finished_ns, x->insert_finished_ns ? EI : 0, int64_t);
+  UP(s, y.x_istate, I > 0 ? in->task_state : nullptr, I, uint8_t);
+  UP(s, y.x_ipre, I > 0 ? in->task_pre : nullptr, I, uint8_t);
+  UP(s, y.x_arow, x->add_row, NA, int64_t);
+  UP(s, y.x_akind, x->add_kind, NA, uint8_t);
+  UP(s, y.x_aref, x->add_ref, NA, int32_t);
+  UP(s, y.x_awant, x->add_want, NA, uint8_t);
+  UP(s, y.x_afin, x->add_finished_ns, x->add_finished_ns ? NA : 0, int64_t);
+  UP(s, y.x_srow, x->set_row, x->n_set, int64_t);
+  UP(s, y.x_sstate, x->set_state, x->n_set, uint8_t);
+  UP(s, y.x_spre, x->set_pre, x->n_set, uint8_t);
+  UP(s, y.s_ext, x->ext_state, Xn, uint8_t);
+  CK(y.s_off.ensure(sizeof(int64_t) * size_t(Tn + 1)));
+  CK(y.s_kind.ensure(size_t(En_max) + 1));
+  CK(y.s_ref.ensure(sizeof(int32_t) * size_t(En_max + 1)));
+  CK(y.s_want.ensure(size_t(En_max) + 1));
+  CK(y.s_fin.ensure(sizeof(int64_t) * size_t(En_max + 1)));
+  CK(y.s_state.ensure(size_t(Tn) + 1));
+  CK(y.s_pre.ensure(size_t(Tn) + 1));
+  CK(y.s_stamp.ensure(sizeof(int64_t) * size_t(Tn + 1)));
+  CK(y.cnt.ensure(sizeof(int32_t) * size_t(Tn + 1)));
+  CK(y.err.ensure(sizeof(int) * 2));
+  CK(y.met.ensure(size_t(Tn) + 1));
+  CK(c->b_err.ensure(sizeof(int) * 4));
+  CK(cudaMemsetAsync(y.err.p, 0, sizeof(int) * 2, s));
+  CK(cudaMemsetAsync(c->b_err.p, 0, sizeof(int) * 4, s));
+  const auto& e = c->ed;  // compose_tick's map of the edit just applied
+  EdMap m;
+  memset(&m, 0, sizeof(m));
+  m.D = c->Dn; m.new_off = e.new_off.as<int64_t>(); m.old_off = e.old_off.as<int64_t>(); m.ins_off = e.ins_off.as<int64_t>();
+  m.keep = e.keep.as<int32_t>(); m.pos = e.pos.as<int64_t>(); m.src = e.src.as<int32_t>();
+  DxEdit X;
+  memset(&X, 0, sizeof(X));
+  X.T0 = T0; X.Xn = Xn;
+  X.off = y.off.as<int64_t>(); X.kind = y.kind.as<uint8_t>(); X.ref = y.ref.as<int32_t>(); X.want = y.want.as<uint8_t>();
+  X.fin = old_fin ? y.fin.as<int64_t>() : nullptr;
+  X.state = y.state.as<uint8_t>(); X.pre = y.pre.as<uint8_t>(); X.stamp = y.stamp.as<int64_t>();
+  X.dext = y.x_dext.as<int32_t>(); X.dfin = x->depart_finished_ns ? y.x_dfin.as<int64_t>() : nullptr;
+  X.efin = x->ext_finished_ns ? y.x_efin.as<int64_t>() : nullptr;
+  X.ioff = y.x_ioff.as<int64_t>(); X.ikind = y.x_ikind.as<uint8_t>(); X.iref = y.x_iref.as<int32_t>(); X.iwant = y.x_iwant.as<uint8_t>();
+  X.ifin = x->insert_finished_ns ? y.x_ifin.as<int64_t>() : nullptr;
+  X.istate = y.x_istate.as<uint8_t>(); X.ipre = y.x_ipre.as<uint8_t>();
+  X.n_add = NA; X.arow = y.x_arow.as<int64_t>(); X.akind = y.x_akind.as<uint8_t>(); X.aref = y.x_aref.as<int32_t>();
+  X.awant = y.x_awant.as<uint8_t>(); X.afin = x->add_finished_ns ? y.x_afin.as<int64_t>() : nullptr;
+  X.o_off = y.s_off.as<int64_t>(); X.o_kind = y.s_kind.as<uint8_t>(); X.o_ref = y.s_ref.as<int32_t>(); X.o_want = y.s_want.as<uint8_t>();
+  X.o_fin = y.s_fin.as<int64_t>(); X.o_state = y.s_state.as<uint8_t>(); X.o_pre = y.s_pre.as<uint8_t>();
+  int64_t En = 0;
+  if (Tn > 0) {
+    launch(c, s, k_dx_count, grid_for(Tn, 256), 256, 0, Tn, m, X, y.cnt.as<int32_t>());
+    CK(scan_counts(c, y.cnt.as<int32_t>(), Tn, y.s_off.as<int64_t>()));
+    launch(c, s, k_dx_write, grid_for(Tn, 256), 256, 0, Tn, m, X, y.err.as<int>());
+    launch(c, s, k_dx_set, grid_for(x->n_set, 256), 256, 0, x->n_set, y.x_srow.as<int64_t>(), y.x_sstate.as<uint8_t>(),
+           y.x_spre.as<uint8_t>(), y.s_state.as<uint8_t>(), y.s_pre.as<uint8_t>());
+    CK(cudaMemcpyAsync(&En, y.s_off.as<int64_t>() + Tn, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+  }
+  // the shadow set becomes the resident table (the launches above hold the previous one's pointers)
+  y.off.swap(y.s_off); y.kind.swap(y.s_kind); y.ref.swap(y.s_ref); y.want.swap(y.s_want); y.fin.swap(y.s_fin);
+  y.state.swap(y.s_state); y.pre.swap(y.s_pre); y.ext.swap(y.s_ext); y.stamp.swap(y.s_stamp);
+  // ---- 4. Task.DependenciesMet and the stamps over the composed table, applied to the resident columns
+  if (Tn > 0) {
+    launch(c, s, k_deps_met, grid_for(Tn, 256), 256, 0, ddeps_sized(c, Tn, En_max, Xn), y.met.as<uint8_t>(), c->b_err.as<int>(), 0,
+           En_max > 0 ? y.fin.as<int64_t>() : nullptr, now_ns, y.stamp.as<int64_t>());
+    launch(c, s, k_apply_deps, grid_for(Tn, 256), 256, 0, Tn, y.met.as<uint8_t>(), y.stamp.as<int64_t>(), c->tasks.flags.as<uint32_t>(),
+           c->tasks.wb.as<int64_t>());
+  }
+  CK(cudaGetLastError());
+  int bad[2] = {0, 0}, bad_met = 0;
+  CK(cudaMemcpyAsync(bad, y.err.p, sizeof(int) * 2, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(&bad_met, c->b_err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  if (bad[0] || bad_met) {
+    drop_tick(c);
+    if (bad[0] & kDxDeparted) return fail(EVG_ERR_INVALID, "%s: a surviving task depends on a removed row whose depart_ext is -1", who);
+    if (bad[0] & kDxBadExt) return fail(EVG_ERR_INVALID, "%s: a surviving task's external ref is outside the new external table", who);
+    if (bad[0] & kDxBadRef) return fail(EVG_ERR_INVALID, "%s: an in-queue ref of the previous dependency table is outside it", who);
+    return deps_bad(who, bad_met);
+  }
+  y.E = En;
+  y.has_fin = En > 0;
+  c->tick.deps = c->tick.dep_table = true;
   return EVG_OK;
 }
 

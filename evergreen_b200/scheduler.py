@@ -179,6 +179,28 @@ class Engine:
         self._n_tasks, self._n_distros, self._n_groups = int(distros.task_off[-1]), distros.n_distros, distros.n_groups
         self._has_hosts = hosts is not None
 
+    def edit_tasks_with_deps(self, edit: S.TaskEdit, distros: S.DistroTable, rows: np.ndarray, values: S.TaskSoA,
+                             deps: "S.DepsEdit", now: int, hosts: Optional[S.HostSoA] = None) -> None:
+        """evg_edit_tasks_with_deps: edit_tasks, update_tasks of the composed `rows`, then the resident dependency table
+        edited by `deps` and Task.DependenciesMet evaluated over it on the device, as upload_with_deps would."""
+        es, keep = edit.normalize().struct()
+        xs, xkeep = deps.struct()
+        ds = distros.struct()
+        rows = np.ascontiguousarray(rows, dtype=np.int64)
+        values = values.normalize()
+        if values.n_tasks != rows.shape[0]:
+            raise ValueError("one value row per updated task slot")
+        vs = values.struct()
+        hargs = (None, None, None)
+        if hosts is not None:
+            hs = hosts.struct()
+            hargs = (C.byref(hs), L.ptr(hosts.host_off), L.ptr(hosts.cfg) if hosts.cfg.shape[0] else None)
+        L.check(self.lib.evg_edit_tasks_with_deps(self.ctx, C.byref(es), C.byref(ds), *hargs, int(rows.shape[0]),
+                                                  L.ptr(rows) if rows.shape[0] else None, C.byref(vs), C.byref(xs), int(now)))
+        del keep, xkeep
+        self._n_tasks, self._n_distros, self._n_groups = int(distros.task_off[-1]), distros.n_distros, distros.n_groups
+        self._has_hosts = hosts is not None
+
     def run(self, now: int, opts: int = 0) -> None:
         L.check(self.lib.evg_run_resident(self.ctx, int(now), int(opts)))
 
@@ -646,6 +668,11 @@ def _upload_with_device_deps(eng: Engine, batch, soa, table, hosts, now: int, de
     DependenciesMetTime stamps it made are written back on the Task objects, like tasks[i] = task (scheduler.go:137)."""
     pairs = [(d, t) for d, t in ((b[0], b[1]) for b in batch)]
     eng.upload_with_deps(soa, table, hosts, S.marshal_deps(pairs, dependency_db), S.marshal_dep_finished(pairs), now)
+    _write_back_stamps(eng, pairs)
+
+
+def _write_back_stamps(eng: Engine, pairs) -> None:
+    """The DependenciesMetTime stamps of the resident tick's last evaluation onto its Task objects (task.go:652-665)."""
     _, stamp = eng.download_deps()
     k = 0
     for _, tasks in pairs:
@@ -726,13 +753,18 @@ class ResidentTick:
     Canonical input order: survivors in their previous order, then arrivals in batch order (input order reaches the
     output only through the tie policy, and the reference's is arbitrary).  Task.DependenciesMet is evaluated on the host
     for every task of the batch (soa.dependencies_met), so the inserted rows carry their bit and survivors whose verdict
-    changed are updated.  The engine must not run other ticks between two plan() calls."""
+    changed are updated.  With device_deps=True the device keeps the tick's dependency table instead: the first tick
+    and any change an edit cannot express upload with evg_upload_with_deps, every other tick sends only the dependency
+    events (soa.DepsShim) with evg_edit_tasks_with_deps, and the stamps the device makes are written back onto the
+    Task objects.  The engine must not run other ticks between two plan() calls."""
 
     SCALARS = ("priority", "expected_ns", "queue_basis_ns", "wait_basis_ns", "num_dependents", "task_group_order", "flags")
 
-    def __init__(self, engine: Optional[Engine] = None, dependency_db: Optional[Dict[str, M.Task]] = None):
+    def __init__(self, engine: Optional[Engine] = None, dependency_db: Optional[Dict[str, M.Task]] = None,
+                 device_deps: bool = False):
         self.engine = engine  # None: default_engine() at the first plan()
         self.dependency_db = dependency_db
+        self.deps = S.DepsShim(dependency_db) if device_deps else None
         self.distro_ids: Optional[List[str]] = None
         self.ids: List[List[str]] = []   # per distro: task ids in resident order
         self.row: Dict[str, int] = {}    # task id -> row of the resident table
@@ -830,9 +862,20 @@ class ResidentTick:
         """One tick: what plan_distros returns for the batch in canonical order (self.canonical)."""
         eng = self.engine = self.engine or default_engine()
         canon = self.canonical(batch)
-        soa, table, keys = S.marshal_tasks(canon, now, self.dependency_db, resolve_deps=True)
+        soa, table, keys = S.marshal_tasks(canon, now, self.dependency_db, resolve_deps=self.deps is None)
         change = self.diff(canon, soa, table, keys)
-        if change is None:
+        if self.deps is not None:
+            dx = None if change is None else self.deps.edit(self.ids, canon, change[0].remove_rows)
+            if dx is None:
+                change = None
+                deps, fin = self.deps.upload(canon)
+                eng.upload_with_deps(soa, table, None, deps, fin, now)
+            else:
+                edit, rows, values = change
+                eng.edit_tasks_with_deps(edit, table, rows, values, dx, now)
+            _write_back_stamps(eng, canon)
+            self.deps.remember(canon)
+        elif change is None:
             eng.upload(soa, table)
         else:
             edit, rows, values = change

@@ -795,11 +795,14 @@ def marshal_dep_finished(batch: Sequence[tuple]) -> np.ndarray:
     return np.array([d.finished_at for _, tasks in batch for t in tasks for d in t.depends_on], dtype=np.int64)
 
 
-def marshal_deps(batch: Sequence[tuple], dependency_db: Optional[Dict[str, M.Task]] = None) -> DepsTable:
+def marshal_deps(batch: Sequence[tuple], dependency_db: Optional[Dict[str, M.Task]] = None,
+                 ext_index: Optional[Dict[str, int]] = None) -> DepsTable:
     """[(Distro, [Task])] -> DepsTable.  A dependency resolves against the distro's own queue first (the
-    depCache of scheduler.go:61-64), then against `dependency_db` (the tasks collection), else it is MISSING."""
+    depCache of scheduler.go:61-64), then against `dependency_db` (the tasks collection), else it is MISSING.
+    `ext_index`, when given, is filled with the external id of every task id the table's external rows stand for."""
     dep_off, kind, ref, want, tstate, pre, ext_state = [0], [], [], [], [], [], []
-    ext_index: Dict[str, int] = {}
+    ext_index = {} if ext_index is None else ext_index
+    ext_index.clear()
     db = dependency_db or {}
     base = 0
     for _, tasks in batch:
@@ -826,6 +829,271 @@ def marshal_deps(batch: Sequence[tuple], dependency_db: Optional[Dict[str, M.Tas
     return DepsTable(np.array(dep_off, np.int64), np.array(kind, np.uint8), np.array(ref, np.int32),
                      np.array(want, np.uint8), np.array(tstate, np.uint8), np.array(pre, np.uint8),
                      np.array(ext_state, np.uint8))
+
+
+def _task_pre(t: M.Task) -> int:
+    return (L.EVG_TP_OVERRIDE if t.override_dependencies else 0) | (0 if M.is_zero_time(t.dependencies_met_time) else L.EVG_TP_MET_TIME)
+
+
+def deps_verdicts(deps: DepsTable, dep_finished: Optional[np.ndarray], now: int):
+    """Task.DependenciesMet and the DependenciesMetTime stamp of every row of an evg_deps_in table, in numpy: what
+    evg_upload_with_deps computes on the device (k_deps_met) -> (met uint8, stamp int64, EVG_TIME_ZERO = none)."""
+    T = deps.n_tasks
+    E = int(deps.dep_ref.shape[0])
+    deg = np.diff(deps.dep_off)
+    owner = np.repeat(np.arange(T, dtype=np.int64), deg)
+    kind, ref = deps.dep_kind, deps.dep_ref.astype(np.int64)
+    st = np.full(E, 2, dtype=np.uint8)
+    inq, ext = kind == L.EVG_DEP_IN_QUEUE, kind == L.EVG_DEP_EXTERNAL
+    st[inq] = deps.task_state[ref[inq]]
+    st[ext] = deps.ext_state[ref[ext]]
+    status = st & 3
+    want = deps.dep_want
+    ok = np.where(want == L.EVG_WANT_SUCCESS, status == 0,
+                  np.where(want == L.EVG_WANT_FAILED, status == 1,
+                           np.where(want == L.EVG_WANT_ANY, (status < 2) | ((st & L.EVG_TS_BLOCKED) != 0), False)))
+    ok &= inq | ext
+    row_ok = np.bincount(owner[~ok], minlength=T) == 0
+    shortcut = (deps.task_pre & (L.EVG_TP_OVERRIDE | L.EVG_TP_MET_TIME)) != 0
+    met = (row_ok | shortcut).astype(np.uint8)
+    best = np.full(T, L.EVG_TIME_ZERO, dtype=np.int64)
+    if dep_finished is not None and E:
+        f = np.asarray(dep_finished, dtype=np.int64)
+        live = (f != L.EVG_TIME_ZERO) & (f != 0)
+        np.maximum.at(best, owner[live], f[live])
+    fresh = row_ok & ~shortcut & (deg > 0)
+    stamp = np.where(fresh, np.where(best == L.EVG_TIME_ZERO, np.int64(now), best), np.int64(L.EVG_TIME_ZERO)).astype(np.int64)
+    return met, stamp
+
+
+@dataclass
+class DepsEdit:
+    """evg_deps_edit: what changed in a resident tick's dependency table between two ticks (include/evg_sched.h)."""
+    depart_ext: np.ndarray                          # int32 [n_remove]: external id a removed row becomes, -1 = none
+    ext_state: np.ndarray                           # uint8 [n_ext]: the new external table, EVG_TS_*
+    insert: DepsTable                               # the inserted rows' own entries (its ext_state is not read)
+    add_row: np.ndarray                             # int64, ascending new global row of a surviving task
+    add_kind: np.ndarray                            # uint8 EVG_DEP_*
+    add_ref: np.ndarray                             # int32: new global row or new external id
+    add_want: np.ndarray                            # uint8 EVG_WANT_*
+    set_row: np.ndarray                             # int64: surviving tasks whose task_state / task_pre change
+    set_state: np.ndarray                           # uint8
+    set_pre: np.ndarray                             # uint8
+    depart_finished: Optional[np.ndarray] = None    # int64 [n_remove]: FinishedAt of the entries that pointed there
+    ext_finished: Optional[np.ndarray] = None       # int64 [n_ext]: FinishedAt of every entry on that id
+    insert_finished: Optional[np.ndarray] = None    # int64 per inserted entry
+    add_finished: Optional[np.ndarray] = None       # int64 per added entry
+
+    def normalize(self) -> "DepsEdit":
+        for f, dt in (("depart_ext", np.int32), ("ext_state", np.uint8), ("add_row", np.int64), ("add_kind", np.uint8),
+                      ("add_ref", np.int32), ("add_want", np.uint8), ("set_row", np.int64), ("set_state", np.uint8),
+                      ("set_pre", np.uint8)):
+            setattr(self, f, np.ascontiguousarray(getattr(self, f), dtype=dt))
+        for f in ("depart_finished", "ext_finished", "insert_finished", "add_finished"):
+            if getattr(self, f) is not None:
+                setattr(self, f, np.ascontiguousarray(getattr(self, f), dtype=np.int64))
+        return self
+
+    def struct(self):
+        """-> (DepsEditStruct, the inserted rows' struct it points to: keep both alive for the call)."""
+        self.normalize()
+        ins = self.insert.struct()
+        p = lambda a: L.ptr(a) if a is not None and a.shape[0] else None  # noqa: E731
+        s = L.DepsEditStruct(p(self.depart_ext), p(self.depart_finished), int(self.ext_state.shape[0]), p(self.ext_state),
+                             p(self.ext_finished), C.pointer(ins), p(self.insert_finished), int(self.add_row.shape[0]),
+                             p(self.add_row), p(self.add_kind), p(self.add_ref), p(self.add_want), p(self.add_finished),
+                             int(self.set_row.shape[0]), p(self.set_row), p(self.set_state), p(self.set_pre))
+        return s, ins
+
+    def nbytes(self) -> int:
+        arrays = [getattr(self, f) for f in ("depart_ext", "ext_state", "add_row", "add_kind", "add_ref", "add_want", "set_row",
+                                            "set_state", "set_pre", "depart_finished", "ext_finished", "insert_finished",
+                                            "add_finished")]
+        ins = self.insert
+        arrays += [ins.dep_off, ins.dep_kind, ins.dep_ref, ins.dep_want, ins.task_state, ins.task_pre]
+        return sum(a.nbytes for a in arrays if a is not None)
+
+
+def apply_deps_edit(deps: DepsTable, task_off: np.ndarray, edit: TaskEdit, x: DepsEdit,
+                    dep_finished: Optional[np.ndarray] = None, stamp: Optional[np.ndarray] = None):
+    """The composed dependency table of evg_edit_tasks_with_deps, in numpy -> (DepsTable, FinishedAt per entry).
+    `deps` / `dep_finished` are the previous tick's table over the previous distro offsets `task_off`, `stamp` its last
+    evaluation's stamps (written back into task_pre as EVG_TP_MET_TIME); of `edit` only the removed rows and the
+    inserted counts are read.  Raises ValueError where the device reports EVG_ERR_INVALID."""
+    edit.normalize()
+    x.normalize()
+    T0, E0 = deps.n_tasks, int(deps.dep_ref.shape[0])
+    Xn = int(x.ext_state.shape[0])
+    fin0 = np.full(E0, L.EVG_TIME_ZERO, np.int64) if dep_finished is None or E0 == 0 else np.asarray(dep_finished, np.int64)
+    D = int(task_off.shape[0]) - 1
+    distro_of = np.repeat(np.arange(D, dtype=np.int64), np.diff(task_off))
+    keep = np.ones(T0, dtype=bool)
+    keep[edit.remove_rows] = False
+    pos = np.cumsum(keep) - keep                       # survivors before each previous row
+    n_ins = np.diff(edit.insert_off)
+    ins_before = np.concatenate([[0], np.cumsum(n_ins)]).astype(np.int64)
+    n_surv = np.bincount(distro_of[keep], minlength=D).astype(np.int64)
+    new_off = np.concatenate([[0], np.cumsum(n_surv + n_ins)]).astype(np.int64)
+    Tn = int(new_off[-1])
+    new_row = np.where(keep, pos + ins_before[distro_of], -1)
+    ins_d = np.repeat(np.arange(D, dtype=np.int64), n_ins)
+    ins_new = new_off[ins_d] + n_surv[ins_d] + np.arange(ins_d.shape[0]) - edit.insert_off[ins_d]
+    # the survivors' previous entries, rewritten
+    own = np.repeat(np.arange(T0, dtype=np.int64), np.diff(deps.dep_off))
+    live = keep[own]
+    kind, ref = deps.dep_kind[live].copy(), deps.dep_ref[live].astype(np.int64)
+    want, fin = deps.dep_want[live].copy(), fin0[live].copy()
+    inq = kind == L.EVG_DEP_IN_QUEUE
+    if np.any(inq & ((ref < 0) | (ref >= T0))):
+        raise ValueError("an in-queue ref of the previous dependency table is outside it")
+    if np.any((kind == L.EVG_DEP_EXTERNAL) & ((ref < 0) | (ref >= Xn))):
+        raise ValueError("a surviving task's external ref is outside the new external table")
+    gone = inq.copy()
+    gone[inq] = ~keep[ref[inq]]
+    stay = inq & ~gone
+    ref[stay] = new_row[ref[stay]]
+    k = ref[gone] - pos[ref[gone]]                    # index in remove_rows
+    ref[gone] = x.depart_ext[k]
+    kind[gone] = L.EVG_DEP_EXTERNAL
+    if np.any(ref[gone] < 0):
+        raise ValueError("a surviving task depends on a removed row whose depart_ext is -1")
+    if x.depart_finished is not None:
+        fin[gone] = x.depart_finished[k]
+    ins = x.insert
+    EI = int(ins.dep_ref.shape[0])
+    zero = lambda n: np.full(n, L.EVG_TIME_ZERO, np.int64)  # noqa: E731
+    owner = np.concatenate([new_row[own[live]], x.add_row, np.repeat(ins_new, np.diff(ins.dep_off))]).astype(np.int64)
+    kind = np.concatenate([kind, x.add_kind, ins.dep_kind]).astype(np.uint8)
+    ref = np.concatenate([ref, x.add_ref, ins.dep_ref]).astype(np.int32)
+    want = np.concatenate([want, x.add_want, ins.dep_want]).astype(np.uint8)
+    fin = np.concatenate([fin, zero(x.add_row.shape[0]) if x.add_finished is None else x.add_finished,
+                          zero(EI) if x.insert_finished is None else x.insert_finished]).astype(np.int64)
+    if x.ext_finished is not None:
+        e = kind == L.EVG_DEP_EXTERNAL
+        fin[e] = x.ext_finished[ref[e]]
+    o = np.argsort(owner, kind="stable")
+    dep_off = np.concatenate([[0], np.cumsum(np.bincount(owner, minlength=Tn))]).astype(np.int64)
+    state = np.zeros(Tn, np.uint8)
+    pre = np.zeros(Tn, np.uint8)
+    st = np.full(T0, L.EVG_TIME_ZERO, np.int64) if stamp is None else np.asarray(stamp, np.int64)
+    sv = np.nonzero(keep)[0]
+    state[new_row[sv]] = deps.task_state[sv]
+    pre[new_row[sv]] = deps.task_pre[sv] | np.where((st[sv] != L.EVG_TIME_ZERO) & (st[sv] != 0), L.EVG_TP_MET_TIME, 0).astype(np.uint8)
+    state[ins_new] = ins.task_state
+    pre[ins_new] = ins.task_pre
+    state[x.set_row] = x.set_state
+    pre[x.set_row] = x.set_pre
+    return DepsTable(dep_off, kind[o], ref[o], want[o], state, pre, x.ext_state.copy()), fin[o]
+
+
+class DepsShim:
+    """What a shim keeps to send a tick's dependency changes as an evg_deps_edit instead of the whole table: the
+    external id of every task id the resident table's external rows stand for (ids only grow until the next full
+    upload), and per queued task its entries (dependency id, wanted status, FinishedAt) and its task_state / task_pre
+    as the device holds them after the last tick's stamps were written back."""
+
+    def __init__(self, dependency_db: Optional[Dict[str, M.Task]] = None):
+        self.db = dependency_db or {}
+        self.ext: Dict[str, int] = {}
+        self.entries: Dict[str, list] = {}
+        self.rows: Dict[str, tuple] = {}
+
+    def upload(self, batch: Sequence[tuple]):
+        """A full upload of `batch`: -> (DepsTable, FinishedAt per entry), and the id map starts over from it."""
+        pairs = [(b[0], b[1]) for b in batch]
+        return marshal_deps(pairs, self.db, self.ext), marshal_dep_finished(pairs)
+
+    def remember(self, batch: Sequence[tuple]) -> None:
+        """After the tick's stamps were written back onto the Task objects."""
+        self.entries = {}
+        for _, ts in batch:
+            q = {t.id for t in ts}
+            for t in ts:  # the last element: the entry resolved to MISSING, which an edit keeps
+                self.entries[t.id] = [(d.task_id, d.status, d.finished_at, d.task_id not in q and d.task_id not in self.db)
+                                      for d in t.depends_on]
+        self.rows = {t.id: (_task_state(t), _task_pre(t)) for _, ts in batch for t in ts}
+
+    def _ext_id(self, task_id: str) -> int:
+        k = self.ext.get(task_id)
+        if k is None:
+            k = self.ext[task_id] = len(self.ext)
+        return k
+
+    def edit(self, prev_ids: Sequence[Sequence[str]], batch: Sequence[tuple], remove_rows: np.ndarray) -> Optional[DepsEdit]:
+        """The DepsEdit from the remembered tick (`prev_ids`: its task ids per distro in resident order) to `batch` in
+        canonical order (survivors in their previous order, then arrivals) with `remove_rows` (ascending previous rows)
+        gone.  Departures become external ids; their FinishedAt comes from the survivors' entries on them.  None when
+        an edit cannot express the change: a survivor whose entries are not its previous ones plus new ones at the end,
+        a kept entry whose FinishedAt or resolution (queue, collection, missing) changed otherwise."""
+        flat_prev = [i for ids in prev_ids for i in ids]
+        gone_ids = [flat_prev[int(r)] for r in remove_rows]
+        gone_k = {i: k for k, i in enumerate(gone_ids)}
+        depart_fin = np.full(len(gone_ids), L.EVG_TIME_ZERO, np.int64)
+        depart_seen = np.zeros(len(gone_ids), dtype=bool)
+        base = 0
+        queue_of = []
+        for _, ts in batch:
+            queue_of.append({t.id: base + j for j, t in enumerate(ts)})
+            base += len(ts)
+        add = ([], [], [], [], [])
+        sets = ([], [], [])
+        ins_off, ikind, iref, iwant, ifin, istate, ipre = [0], [], [], [], [], [], []
+
+        def resolve(dep_id: str, q: dict):
+            j = q.get(dep_id)
+            if j is not None:
+                return L.EVG_DEP_IN_QUEUE, j
+            if dep_id in self.db:
+                return L.EVG_DEP_EXTERNAL, self._ext_id(dep_id)
+            return L.EVG_DEP_MISSING, 0
+
+        for d, (_, ts) in enumerate(batch):
+            q = queue_of[d]
+            prev_q = set(prev_ids[d])
+            n_prev = len(prev_q) - sum(1 for i in prev_ids[d] if i in gone_k)
+            for j, t in enumerate(ts):
+                row = q[t.id]
+                cur = [(x.task_id, x.status, x.finished_at) for x in t.depends_on]
+                if j >= n_prev:  # an arrival brings its own entries
+                    for dep_id, status, f in cur:
+                        kd, rf = resolve(dep_id, q)
+                        ikind.append(kd); iref.append(rf); iwant.append(_want(status)); ifin.append(f)
+                    ins_off.append(len(iref))
+                    istate.append(_task_state(t)); ipre.append(_task_pre(t))
+                    continue
+                old = self.entries.get(t.id)
+                if old is None or len(cur) < len(old):
+                    return None
+                for (dep_id, status, f), (o_id, o_status, o_f, o_missing) in zip(cur, old):
+                    if (dep_id, status) != (o_id, o_status):
+                        return None
+                    k = gone_k.get(dep_id)
+                    if k is not None:  # departs now: every entry on it must agree on its FinishedAt
+                        if depart_seen[k] and depart_fin[k] != f:
+                            return None
+                        depart_seen[k], depart_fin[k] = True, f
+                        continue
+                    if f != o_f:
+                        return None
+                    if (dep_id in prev_q) != (dep_id in q) or (o_missing and dep_id in self.db):
+                        return None  # the dependency joined the queue, or a missing one turned up
+                for dep_id, status, f in cur[len(old):]:
+                    kd, rf = resolve(dep_id, q)
+                    add[0].append(row); add[1].append(kd); add[2].append(rf); add[3].append(_want(status)); add[4].append(f)
+                now = (_task_state(t), _task_pre(t))
+                if now != self.rows.get(t.id):
+                    sets[0].append(row); sets[1].append(now[0]); sets[2].append(now[1])
+        depart_ext = np.array([self._ext_id(i) if depart_seen[k] else -1 for k, i in enumerate(gone_ids)], np.int32)
+        ext_state = np.full(len(self.ext), 2, np.uint8)  # an id no longer in the collection satisfies nothing, as MISSING
+        for i, k in self.ext.items():
+            if i in self.db:
+                ext_state[k] = _task_state(self.db[i])
+        insert = DepsTable(np.array(ins_off, np.int64), np.array(ikind, np.uint8), np.array(iref, np.int32),
+                           np.array(iwant, np.uint8), np.array(istate, np.uint8), np.array(ipre, np.uint8), np.zeros(0, np.uint8))
+        return DepsEdit(depart_ext, ext_state, insert, np.array(add[0], np.int64), np.array(add[1], np.uint8),
+                        np.array(add[2], np.int32), np.array(add[3], np.uint8), np.array(sets[0], np.int64),
+                        np.array(sets[1], np.uint8), np.array(sets[2], np.uint8), depart_finished=depart_fin,
+                        insert_finished=np.array(ifin, np.int64), add_finished=np.array(add[4], np.int64)).normalize()
 
 
 @dataclass

@@ -330,7 +330,8 @@ typedef struct {
  * gathered from the resident columns into a second column set the first edit allocates, which then becomes the
  * resident one.  A survivor cannot LOSE an in-queue dependency that stays in the queue (upload again for that), and
  * dependencies are not re-evaluated: pass EVG_TF_DEPS_MET for inserted rows and flip it for survivors with
- * evg_update_tasks.  Any device-side dependency state of evg_upload_with_deps is dropped.
+ * evg_update_tasks.  Any device-side dependency state of evg_upload_with_deps is dropped (evg_edit_tasks_with_deps
+ * keeps it).
  * Allowed after evg_upload, evg_upload_with_deps, evg_plan_from_finder(_ex), evg_edit_tasks and evg_plan_aliases;
  * EVG_ERR_STATE otherwise (no table, borrowed columns of evg_upload_device, the tick a one-shot call left).
  * EVG_ERR_INVALID for an edit the
@@ -403,7 +404,7 @@ int evg_bind_result_buffer(evg_ctx* ctx, void* device_ptr, int64_t capacity);
 /* Number of kernels the context launched since the last call that reset the count; 0 for a NULL ctx.  These calls
  * reset it to 0 before their first launch: evg_run_resident (so evg_plan_batch, evg_plan_distro and the
  * evg_plan_and_alloc_batch it runs), evg_plan_and_alloc_batch's pipelined large ticks, evg_alloc_batch / evg_alloc_distro,
- * evg_deps_met_batch, evg_find_runnable_batch / _ex, evg_plan_from_finder / _ex, evg_edit_tasks, evg_plan_aliases,
+ * evg_deps_met_batch, evg_find_runnable_batch / _ex, evg_plan_from_finder / _ex, evg_edit_tasks, evg_edit_tasks_with_deps, evg_plan_aliases,
  * evg_expected_durations_batch, evg_prioritize_legacy_batch, evg_dag_rebuild_batch, evg_rebuild_dispatchers,
  * evg_host_job, evg_host_drawdown, evg_idle_hosts, evg_find_next_batch, evg_find_next_tasks, evg_estimate_start_times,
  * evg_estimate_start_batch, evg_intern_batch and evg_upload_strings.  Every other call adds the kernels it launches: the uploads (their range check), evg_update_tasks,
@@ -482,6 +483,57 @@ int evg_upload_with_deps(evg_ctx* ctx, const evg_task_soa* tasks, const evg_dist
  * evg_upload_with_deps' (evg_deps_met_batch and evg_update_tasks drop them; evg_resolve_durations and
  * evg_rebuild_dispatchers keep them). */
 int evg_download_deps(evg_ctx* ctx, uint8_t* met, int64_t* met_time_ns);
+
+/* What changed in a resident tick's dependency table between two ticks (evg_edit_tasks_with_deps).  Host pointers. */
+typedef struct {
+  const int32_t* depart_ext;          /* edit->n_remove: the external id removed row k becomes for the survivors that
+                                         depend on it, -1 = none may (a survivor that still does is EVG_ERR_INVALID) */
+  const int64_t* depart_finished_ns;  /* edit->n_remove (NULL = none): Dependency.FinishedAt written into every entry
+                                         that pointed at removed row k (MarkDependenciesFinished) */
+  int64_t n_ext;                      /* the new external table, replaced whole; a survivor's external refs keep their ids */
+  const uint8_t* ext_state;           /* n_ext, EVG_TS_* */
+  const int64_t* ext_finished_ns;     /* n_ext (NULL = none): FinishedAt written into every entry that references the id */
+  const evg_deps_in* insert;          /* the inserted rows' own entries, CSR over edit->insert's rows with their task_state
+                                         and task_pre (n_ext / ext_state not read); in-queue refs are NEW global rows,
+                                         external ones index the new external table.  NULL when nothing is inserted */
+  const int64_t* insert_finished_ns;  /* insert->n_deps (NULL = zero time): their Dependency.FinishedAt */
+  int64_t n_add;                      /* entries appended to surviving tasks, after their own, in the order given */
+  const int64_t* add_row;             /* ascending NEW global row of a surviving task */
+  const uint8_t* add_kind;            /* EVG_DEP_* */
+  const int32_t* add_ref;             /* NEW global row (EVG_DEP_IN_QUEUE) or new external id (EVG_DEP_EXTERNAL) */
+  const uint8_t* add_want;            /* EVG_WANT_* */
+  const int64_t* add_finished_ns;     /* NULL = zero time */
+  int64_t n_set;                      /* surviving tasks whose own task_state / task_pre change (each row at most once) */
+  const int64_t* set_row;             /* NEW global rows */
+  const uint8_t* set_state;           /* EVG_TS_* */
+  const uint8_t* set_pre;             /* EVG_TP_*, the whole byte */
+} evg_deps_edit;
+
+/* One call per tick that keeps the dependency table on the device: evg_edit_tasks(edit, distros, hosts, host_off,
+ * acfg), then evg_update_tasks(n_rows, rows, values) (rows are rows of the composed table; the caller's
+ * EVG_TF_DEPS_MET bit is ignored), then the composed dependency table, then Task.DependenciesMet and the stamps as
+ * evg_upload_with_deps evaluates them (now_ns), so that the context holds what evg_upload_with_deps of the composed
+ * task table and the composed dependency table would.  The composed dependency table, row by row:
+ *   - a survivor's entries in their order: an in-queue ref is re-indexed to its row in the composed table, or, when that
+ *     row was removed as row k, becomes EVG_DEP_EXTERNAL depart_ext[k]; external and missing entries are kept; then its
+ *     added entries; an inserted row's entries are its own;
+ *   - an entry's FinishedAt: ext_finished_ns[ref] for an external entry when ext_finished_ns is given, else
+ *     depart_finished_ns[k] for an entry that departed in this call when that is given, else its own (the previous
+ *     tick's, or the one given with it);
+ *   - task_state / task_pre: a survivor's previous ones, its task_pre gaining EVG_TP_MET_TIME when the previous tick
+ *     stamped it (the reference writes DependenciesMetTime back, model/task/task.go:652-665), then set_*; an inserted
+ *     row's own.
+ * Allowed where evg_edit_tasks is and the tick holds a dependency table: after evg_upload_with_deps or this call,
+ * with evg_update_tasks in between (EVG_ERR_STATE otherwise).  EVG_ERR_INVALID for what the host can check (what
+ * evg_edit_tasks rejects, rows outside the composed table, counts or offsets that disagree, a ref outside the table it
+ * indexes, an added entry on a task that is not a survivor) leaves the previous tick resident and runnable; a survivor
+ * whose entry points at a removed row with depart_ext -1, or whose external ref is outside the new table, is found on
+ * the device and leaves no resident tick.  evg_download_deps then returns this call's verdicts and stamps.
+ * Replaces: checkDependenciesMet inside GetDistroQueueInfo (scheduler/scheduler.go:82-98,161-168) on an edited tick. */
+int evg_edit_tasks_with_deps(evg_ctx* ctx, const evg_task_edit* edit, const evg_distro_table* distros,
+                             const evg_host_soa* hosts, const int64_t* host_off, const evg_alloc_cfg* acfg,
+                             int64_t n_rows, const int64_t* rows, const evg_task_soa* values,
+                             const evg_deps_edit* deps, int64_t now_ns);
 
 /* ---- runnable-task filter: the task finders (SURVEY.md §8f.1) ------------- */
 
