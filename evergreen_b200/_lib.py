@@ -78,6 +78,11 @@ class InternOutStruct(C.Structure):
                 ("group_max_hosts", C.c_void_p), ("group_first", C.c_void_p), ("dep_off", C.c_void_p), ("dep_idx", C.c_void_p)]
 
 
+class QueueIndexOutStruct(C.Structure):
+    _fields_ = [("min_position", C.c_void_p), ("dup_item", C.c_void_p), ("dup_off", C.c_void_p), ("dup_queue", C.c_void_p),
+                ("n_dups", C.c_int64)]
+
+
 class TaskSoAStruct(C.Structure):
     _fields_ = [("n_tasks", C.c_int64), ("n_edges", C.c_int64),
                 ("priority", C.c_void_p), ("expected_ns", C.c_void_p), ("queue_basis_ns", C.c_void_p),
@@ -349,6 +354,7 @@ SYMBOLS = {
     "evg_intern_columns": (C.c_int, [_P, _P, C.c_int32]),
     "evg_intern_batch": (C.c_int, [_P, _P, _P]),
     "evg_upload_strings": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P]),
+    "evg_queue_index_batch": (C.c_int, [_P, _P, _P, C.c_int32, _P]),
     "evg_run_resident": (C.c_int, [_P, C.c_int64, C.c_uint32]),
     "evg_download": (C.c_int, [_P, _P, _P]),
     "evg_download_queue": (C.c_int, [_P, C.c_int32, _P, _P, C.c_int64]),

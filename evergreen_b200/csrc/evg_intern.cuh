@@ -166,3 +166,104 @@ __global__ void __launch_bounds__(256) k_in_edges(InView v, const int32_t* __res
   for (int64_t e = v.dep_off[t]; e < v.dep_off[t + 1]; e++)
     if (res[e] >= 0) dep_idx[w++] = res[e];
 }
+
+// ---- evg_queue_index_batch: every persisted queue's items joined by task id --------------------------------------
+// FindMinimumQueuePositionForTask and FindDuplicateEnqueuedTasks (model/task_queue.go:407-435, 505-547) for every id at
+// once.  The whole item list is one range: one task-id table spans every queue, so the distro mixed into the hash is 0
+// and every claimant counts.  The ids sit in InView's first column (grp) and the table in its first region of cap slots.
+struct QxView {
+  InView v;                 // v.grp: the ids, one row per item; v.key / v.first: cap slots
+  int64_t N;                // items
+  int32_t Q;                // queues
+  const int64_t* item_off;  // Q + 1: the items of queue q are [item_off[q], item_off[q + 1])
+};
+constexpr int kQxErrIdOff = 1;  // an id row outside its byte column
+
+// A warp per item: its id into the table (slot[i]) and its queue (queue[i]); atomicMin gives each slot its first item.
+__global__ void __launch_bounds__(256) k_qx_keys(QxView x, int64_t* __restrict__ slot, int32_t* __restrict__ queue, int* err) {
+  const int64_t i = (int64_t(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (i >= x.N) return;
+  const DStr& s = x.v.grp;
+  const int64_t o0 = s.off[i], o1 = s.off[i + 1];
+  int64_t k = -1;
+  if (in_row_bad(s, o0, o1)) {
+    if (lane == 0) atomicOr(err, kQxErrIdOff);
+  } else {
+    k = in_probe(x.v, kInGroup, s, o0, o1 - o0, in_hash(s, o0, o1 - o0, 0, x.v.hmask, lane), i, 0, x.N, lane);
+    if (lane == 0) atomicMin(x.v.first + k, uint32_t(i));
+  }
+  if (lane == 0) {
+    slot[i] = k;
+    queue[i] = find_distro(x.item_off, 0, x.Q - 1, i);
+  }
+}
+
+// first-appearance flags: their exclusive scan numbers the distinct ids in first-appearance order
+__global__ void __launch_bounds__(256) k_qx_flag(int64_t n, const int64_t* __restrict__ slot, const uint32_t* __restrict__ first,
+                                                 int32_t* __restrict__ f) {
+  const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  f[i] = first[slot[i]] == uint32_t(i);
+}
+
+// Per item, after the scan pk of the flags: its id's dense number (key[i]); per id the smallest index in any queue and
+// the lowest and highest queue that hold it (two distinct queues: lo != hi).  Mins and maxes: no order of atomics shows.
+__global__ void __launch_bounds__(256) k_qx_reduce(QxView x, const int64_t* __restrict__ slot, const int32_t* __restrict__ queue,
+                                                   const int64_t* __restrict__ pk, int32_t* __restrict__ key, int32_t* pos, int32_t* qlo,
+                                                   int32_t* qhi) {
+  const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= x.N) return;
+  const int64_t k = pk[x.v.first[slot[i]]];
+  const int32_t q = queue[i];
+  key[i] = int32_t(k);
+  atomicMin(pos + k, int32_t(i - x.item_off[q]));
+  atomicMin(qlo + k, q);
+  atomicMax(qhi + k, q);
+}
+
+// Per item: min_position = 1 + its id's smallest index; fm[i] = the id is duplicated; f[i] (the first-appearance flag)
+// is kept only for a duplicated id, so its scan numbers the duplicated ids in first-appearance order.
+__global__ void __launch_bounds__(256) k_qx_dup(int64_t n, const int32_t* __restrict__ key, const int32_t* __restrict__ pos,
+                                                const int32_t* __restrict__ qlo, const int32_t* __restrict__ qhi,
+                                                int32_t* __restrict__ min_position, int32_t* __restrict__ f, int32_t* __restrict__ fm) {
+  const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int32_t k = key[i];
+  const bool dup = qlo[k] != qhi[k];
+  min_position[i] = pos[k] + 1;
+  fm[i] = dup;
+  f[i] = f[i] && dup;
+}
+
+// Per item of a duplicated id, at pm[i]: the pair (duplicate number << 32 | queue), in item order and so in queue order
+// within each id; per duplicated id, its first item (dup_item).
+__global__ void __launch_bounds__(256) k_qx_pairs(QxView x, const int64_t* __restrict__ slot, const int32_t* __restrict__ queue,
+                                                  const int32_t* __restrict__ fm, const int64_t* __restrict__ pd,
+                                                  const int64_t* __restrict__ pm, uint64_t* __restrict__ pairs, int64_t* __restrict__ dup_item) {
+  const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= x.N || !fm[i]) return;
+  const int64_t f = x.v.first[slot[i]];
+  pairs[pm[i]] = (uint64_t(pd[f]) << 32) | uint32_t(queue[i]);
+  if (f == i) dup_item[pd[i]] = i;
+}
+
+// After the pairs are sorted by duplicate number (stably, so each id's queues stay ascending): u[j] = pair j is the
+// first of its (id, queue).
+__global__ void __launch_bounds__(256) k_qx_uniq(int64_t m, const uint64_t* __restrict__ pairs, int32_t* __restrict__ u) {
+  const int64_t j = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (j >= m) return;
+  u[j] = j == 0 || pairs[j] != pairs[j - 1];
+}
+
+// Per pair, after the scan pu of u: the distinct queues at pu[j], and each id's row of dup_off at its first pair.
+__global__ void __launch_bounds__(256) k_qx_write(int64_t m, int64_t n_dups, const uint64_t* __restrict__ pairs,
+                                                  const int64_t* __restrict__ pu, int64_t* __restrict__ dup_off,
+                                                  int32_t* __restrict__ dup_queue) {
+  const int64_t j = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (j >= m) return;
+  const uint64_t p = pairs[j];
+  if (j == 0 || p != pairs[j - 1]) dup_queue[pu[j]] = int32_t(uint32_t(p));
+  if (j == 0 || (p >> 32) != (pairs[j - 1] >> 32)) dup_off[p >> 32] = pu[j];
+  if (j == m - 1) dup_off[n_dups] = pu[m];
+}

@@ -33,6 +33,8 @@
 //   k_host_job            hostAllocatorJob.Run past the allocator: single-task bypass, report, drawdown (units/host_allocator.go:180-425)
 //   k_next_verdict/serve  the DAG dispatcher's FindNextTask, a warp per distro (model/task_queue_service_dependency.go:258-692)
 //   k_in_*                evg_intern_columns on the device: string keys to dense ids, dependency ids to queue indices
+//   k_qx_*                the saved queues joined by task id: minimum queue positions, duplicate enqueued tasks
+//                         (model/task_queue.go:407-435, 505-547)
 // No CPU fallback exists in this file: without a device every entry point fails.
 #include <cuda_runtime.h>
 #include <stdarg.h>
@@ -1577,6 +1579,13 @@ struct evg_ctx {
     DevBuf task_off, gmh, dep_off, bytes[4], off[4], key, first, gslot, vslot, fg, fv, pg, pv, res, cnt, samp, err;
     DevBuf gid, vid, gmax, gfirst, out_dep_off, out_dep_idx;
   } in;
+  // evg_queue_index_batch (the first call allocates these): the staged ids and item_off, the task-id table, each item's
+  // slot, queue and id number, the flags and their scans, the per-id reductions, the pairs (two copies: the radix
+  // sort's) with its histograms, the outputs and the error word
+  struct {
+    DevBuf item_off, off, bytes, key, first, slot, queue, f, fm, pk, pm, kid, pos, qlo, qhi, pairs[2], hist, hoff;
+    DevBuf min_position, dup_item, dup_off, dup_queue, err;
+  } qx;
   DevBuf b_err;
   DevBuf b_scansum;  // scan_counts' per-block sums
   DevBuf b_route, b_unitv, b_unita, b_unitn, b_unitmask;
@@ -4514,6 +4523,14 @@ static int intern_check(const char* who, const evg_string_cols* in) {
   return EVG_OK;
 }
 
+// Test hook of the string tables: EVG_INTERN_HASH_BITS (read per call, 0..32) masks the hash to fewer bits so that
+// strings collide; 32 when unset.
+static uint32_t intern_hash_mask() {
+  const char* bits_env = getenv("EVG_INTERN_HASH_BITS");
+  const int bits = bits_env ? std::max(0, std::min(32, atoi(bits_env))) : 32;
+  return bits >= 32 ? 0xFFFFFFFFu : (1u << bits) - 1u;
+}
+
 // What the host reads back of an interned tick: O(n_distros) values.
 struct InternSizes {
   std::vector<int64_t> group_off;  // D + 1
@@ -4574,9 +4591,7 @@ static int intern_strings(evg_ctx* c, const char* who, const evg_string_cols* in
   for (int k = 0; k < 4; k++) *dst[k] = DStr{b.bytes[k].as<uint8_t>(), b.off[k].as<int64_t>(), nb[k]};
   v.dep_off = b.dep_off.as<int64_t>();
   v.gmh = b.gmh.as<int32_t>();
-  const char* bits_env = getenv("EVG_INTERN_HASH_BITS");  // test hook: fewer hash bits force collisions; 32 when unset
-  const int bits = bits_env ? std::max(0, std::min(32, atoi(bits_env))) : 32;
-  v.hmask = bits >= 32 ? 0xFFFFFFFFu : (1u << bits) - 1u;
+  v.hmask = intern_hash_mask();
   v.cap = cap;
   v.key = b.key.as<unsigned long long>();
   v.first = b.first.as<uint32_t>();
@@ -4729,6 +4744,134 @@ int evg_upload_strings(evg_ctx* c, const evg_task_soa* tasks, const evg_string_c
     CK(cudaStreamSynchronize(s));
   }
   c->tick.kind = Tick::kOwn;
+  return EVG_OK;
+}
+
+// --------------------------------------------------------------------------
+// evg_queue_index_batch: minimum queue positions and duplicate enqueued tasks over every saved queue (evg_intern.cuh)
+// --------------------------------------------------------------------------
+int evg_queue_index_batch(evg_ctx* c, const evg_str_col* ids, const int64_t* item_off, int32_t n_queues, evg_queue_index_out* out) {
+  ENTER(c, "evg_queue_index_batch");
+  c->launches = 0;
+  if (!ids || !item_off || !out) return fail(EVG_ERR_INVALID, "%s: null argument", who);
+  const int32_t Q = n_queues;
+  if (Q < 0) return fail(EVG_ERR_INVALID, "%s: negative sizes", who);
+  int rc = check_offsets(item_off, Q, -1, who, "item_off");
+  if (rc != EVG_OK) return rc;
+  const int64_t N = item_off[Q];
+  if (N > (int64_t(1) << 31) - 2) return fail(EVG_ERR_INVALID, "%s: %lld items exceed 2^31-2", who, (long long)N);
+  if (!out->dup_off || (N > 0 && (!out->min_position || !out->dup_item || !out->dup_queue)))
+    return fail(EVG_ERR_INVALID, "%s: null output column", who);
+  out->n_dups = 0;
+  if (N == 0) {
+    out->dup_off[0] = 0;
+    return EVG_OK;
+  }
+  if (!ids->off) return fail(EVG_ERR_INVALID, "%s: null ids.off", who);
+  const int64_t nb = ids->off[N];
+  if (nb < 0) return check_offsets(ids->off, N, -1, who, "ids.off");
+  if (nb > 0 && !ids->bytes) return fail(EVG_ERR_INVALID, "%s: null bytes for ids.off", who);
+  // ---- every buffer sized before the first launch: at most N ids, N duplicated ones, N pairs
+  cudaStream_t s = c->stream;
+  auto& b = c->qx;
+  uint64_t cap = 64;
+  while (cap < 2 * uint64_t(N)) cap <<= 1;  // load factor <= 1/2
+  const int64_t n_tiles = (N + kAlTile - 1) / kAlTile, nh = 256 * n_tiles;
+  {
+    cudaError_t e = cudaSuccess;
+    auto need = [&](DevBuf& x, int64_t bytes) { if (e == cudaSuccess) e = x.ensure(size_t(std::max<int64_t>(bytes, 1))); };
+    need(b.item_off, 8 * (int64_t(Q) + 1)); need(b.off, 8 * (N + 1)); need(b.bytes, nb);
+    need(b.key, 8 * int64_t(cap)); need(b.first, 4 * int64_t(cap));
+    need(b.slot, 8 * N); need(b.queue, 4 * N); need(b.f, 4 * N); need(b.fm, 4 * N); need(b.pk, 8 * (N + 1)); need(b.pm, 8 * (N + 1));
+    need(b.kid, 4 * N); need(b.pos, 4 * N); need(b.qlo, 4 * N); need(b.qhi, 4 * N);
+    need(b.pairs[0], 8 * N); need(b.pairs[1], 8 * N); need(b.hist, 4 * nh); need(b.hoff, 8 * (nh + 1));
+    need(b.min_position, 4 * N); need(b.dup_item, 8 * N); need(b.dup_off, 8 * (N + 1)); need(b.dup_queue, 4 * N); need(b.err, 16);
+    need(c->b_scansum, 8 * ((std::max(N, nh) + 1023) / 1024 + 1));
+    if (e != cudaSuccess) {
+      cudaGetLastError();  // as in intern_strings: a failed allocation leaves the context usable
+      return fail(e == cudaErrorMemoryAllocation ? EVG_ERR_NOMEM : EVG_ERR_CUDA, "%s: %s while sizing %lld items", who,
+                  cudaGetErrorString(e), (long long)N);
+    }
+  }
+  // ---- stage the ids and the queues; the table empty, the reductions at their identities
+  CK(cudaMemcpyAsync(b.item_off.p, item_off, sizeof(int64_t) * size_t(Q + 1), cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(b.off.p, ids->off, sizeof(int64_t) * size_t(N + 1), cudaMemcpyHostToDevice, s));
+  if (nb > 0) CK(cudaMemcpyAsync(b.bytes.p, ids->bytes, size_t(nb), cudaMemcpyHostToDevice, s));
+  CK(cudaMemsetAsync(b.key.p, 0xFF, sizeof(uint64_t) * cap, s));
+  CK(cudaMemsetAsync(b.first.p, 0xFF, sizeof(uint32_t) * cap, s));
+  CK(cudaMemsetAsync(b.pos.p, 0x7F, sizeof(int32_t) * size_t(N), s));
+  CK(cudaMemsetAsync(b.qlo.p, 0x7F, sizeof(int32_t) * size_t(N), s));
+  CK(cudaMemsetAsync(b.qhi.p, 0xFF, sizeof(int32_t) * size_t(N), s));  // -1
+  CK(cudaMemsetAsync(b.err.p, 0, sizeof(int), s));
+  QxView x;
+  memset(&x, 0, sizeof(x));
+  x.v.grp = DStr{b.bytes.as<uint8_t>(), b.off.as<int64_t>(), nb};
+  x.v.hmask = intern_hash_mask();
+  x.v.cap = cap;
+  x.v.key = b.key.as<unsigned long long>();
+  x.v.first = b.first.as<uint32_t>();
+  x.N = N; x.Q = Q;
+  x.item_off = b.item_off.as<int64_t>();
+  int64_t *slot = b.slot.as<int64_t>(), *pk = b.pk.as<int64_t>(), *pm = b.pm.as<int64_t>();
+  int32_t *queue = b.queue.as<int32_t>(), *f = b.f.as<int32_t>(), *fm = b.fm.as<int32_t>();
+  // ---- 1. every id into the table; the row checks cross to the host
+  launch(c, s, k_qx_keys, grid_for(N * 32, 256), 256, 0, x, slot, queue, b.err.as<int>());
+  int bad = 0;
+  CK(cudaMemcpyAsync(&bad, b.err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  if (bad) {
+    rc = check_offsets(ids->off, N, -1, who, "ids.off");
+    return rc != EVG_OK ? rc : fail(EVG_ERR_INVALID, "%s: ids.off breaks its byte column", who);
+  }
+  // ---- 2. ids numbered in first-appearance order; per id its smallest index and its lowest and highest queue
+  launch(c, s, k_qx_flag, grid_for(N, 256), 256, 0, N, slot, x.v.first, f);
+  CK(scan_counts(c, f, N, pk));
+  launch(c, s, k_qx_reduce, grid_for(N, 256), 256, 0, x, slot, queue, pk, b.kid.as<int32_t>(), b.pos.as<int32_t>(), b.qlo.as<int32_t>(),
+         b.qhi.as<int32_t>());
+  // ---- 3. positions; the duplicated ids numbered (into pk) and their items' pairs placed (pm); two counts cross
+  launch(c, s, k_qx_dup, grid_for(N, 256), 256, 0, N, b.kid.as<int32_t>(), b.pos.as<int32_t>(), b.qlo.as<int32_t>(), b.qhi.as<int32_t>(),
+         b.min_position.as<int32_t>(), f, fm);
+  CK(scan_counts(c, f, N, pk));
+  CK(scan_counts(c, fm, N, pm));
+  launch(c, s, k_qx_pairs, grid_for(N, 256), 256, 0, x, slot, queue, fm, pk, pm, b.pairs[0].as<uint64_t>(), b.dup_item.as<int64_t>());
+  int64_t counts[2] = {0, 0};  // duplicated ids, their items
+  CK(cudaMemcpyAsync(&counts[0], pk + N, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(&counts[1], pm + N, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  const int64_t n_dups = counts[0], M = counts[1];
+  // ---- 4. the pairs sorted by duplicate number with the alias queues' stable radix sort; the distinct queues per id
+  int cur = 0;
+  if (n_dups > 0) {
+    int bits = 0;
+    while (bits < 31 && (int64_t(1) << bits) < n_dups) bits++;
+    const int64_t m_tiles = (M + kAlTile - 1) / kAlTile, mh = 256 * m_tiles;
+    for (int shift = 32; shift < 32 + bits; shift += 8, cur ^= 1) {
+      launch(c, s, k_al_hist, unsigned(m_tiles), 256, 0, b.pairs[cur].as<uint64_t>(), M, shift, b.hist.as<int32_t>(), m_tiles);
+      CK(scan_counts(c, b.hist.as<int32_t>(), mh, b.hoff.as<int64_t>()));
+      launch(c, s, k_al_scatter, unsigned(m_tiles), 256, 0, b.pairs[cur].as<uint64_t>(), b.pairs[cur ^ 1].as<uint64_t>(), M, shift,
+             b.hoff.as<int64_t>(), m_tiles);
+    }
+    const uint64_t* pairs = b.pairs[cur].as<uint64_t>();
+    launch(c, s, k_qx_uniq, grid_for(M, 256), 256, 0, M, pairs, fm);
+    CK(scan_counts(c, fm, M, pm));
+    launch(c, s, k_qx_write, grid_for(M, 256), 256, 0, M, n_dups, pairs, pm, b.dup_off.as<int64_t>(), b.dup_queue.as<int32_t>());
+  } else {
+    CK(cudaMemsetAsync(b.dup_off.p, 0, sizeof(int64_t), s));
+  }
+  // ---- 5. the outputs
+  CK(cudaMemcpyAsync(out->min_position, b.min_position.p, sizeof(int32_t) * size_t(N), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(out->dup_off, b.dup_off.p, sizeof(int64_t) * size_t(n_dups + 1), cudaMemcpyDeviceToHost, s));
+  if (n_dups > 0) CK(cudaMemcpyAsync(out->dup_item, b.dup_item.p, sizeof(int64_t) * size_t(n_dups), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  const int64_t n_pairs = out->dup_off[n_dups];
+  if (n_pairs > 0) {
+    CK(cudaMemcpyAsync(out->dup_queue, b.dup_queue.p, sizeof(int32_t) * size_t(n_pairs), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+  }
+  out->n_dups = n_dups;
   return EVG_OK;
 }
 #undef D2H_IF

@@ -372,6 +372,12 @@ class TaskQueue:  # model/task_queue.go:117-123
 
 
 @dataclass
+class DuplicateEnqueuedTasksResult:  # model/task_queue.go:500-503
+    task_id: str = ""
+    distro_ids: List[str] = field(default_factory=list)
+
+
+@dataclass
 class SortingValueBreakdown:  # model/task/task.go:3990-4038 (flattened)
     task_group_length: int = 0
     total_value: int = 0

@@ -388,6 +388,26 @@ class Engine:
         self._has_hosts = hosts is not None
         return out
 
+    def queue_index(self, ids, item_off) -> dict:
+        """evg_queue_index_batch over saved queues: `ids` the queue[]._id of every queue concatenated (a list of str /
+        bytes, or a (bytes, offsets) pair from soa.pack_strings), item_off the CSR over the queues.  The resident tick is
+        left as it was.  -> dict(min_position [n_items] int32, dup_item [n_dups] int64, dup_off [n_dups + 1] int64,
+        dup_queue [dup_off[-1]] int32): per item 1 + the smallest index of its id in any queue; per id held by two or more
+        queues, in the order of its first item, that item and the queues, ascending."""
+        data, off = ids if isinstance(ids, tuple) else S.pack_strings(ids)
+        data, off = np.ascontiguousarray(data, np.uint8), np.ascontiguousarray(off, np.int64)
+        item_off = np.ascontiguousarray(item_off, np.int64)
+        N = int(item_off[-1])
+        out = dict(min_position=np.empty(max(N, 1), np.int32), dup_item=np.empty(max(N, 1), np.int64),
+                   dup_off=np.zeros(N + 1, np.int64), dup_queue=np.empty(max(N, 1), np.int32))
+        st = L.QueueIndexOutStruct(*[L.ptr(out[k]) for k in ("min_position", "dup_item", "dup_off", "dup_queue")], 0)
+        col = L.StrColStruct(L.ptr(data) if data.shape[0] else None, L.ptr(off))
+        L.check(self.lib.evg_queue_index_batch(self.ctx, C.byref(col), L.ptr(item_off), item_off.shape[0] - 1, C.byref(st)))
+        n = int(st.n_dups)
+        off_d = out["dup_off"][:n + 1]
+        return dict(min_position=out["min_position"][:N], dup_item=out["dup_item"][:n], dup_off=off_d,
+                    dup_queue=out["dup_queue"][:int(off_d[-1])])
+
     def download_alias_map(self):
         """evg_download_alias_map: (source row of every resident row, global group id of every group slot)."""
         src = self._out("alias_source_row", self._n_tasks, np.int32)
@@ -918,6 +938,21 @@ class ResidentTick:
         that is not there is not queued, for which the reference returns -1."""
         io, start, _ = self.engine.estimate_start_times(S.marshal_estimate_hosts(hosts_by_distro, running_tasks), now, cap, self.table.task_off)
         return [dict(zip(ids, start[int(io[d]):int(io[d + 1])].tolist())) for d, ids in enumerate(self.ranked)]
+
+    def queue_index(self, cap: int = 0):
+        """The cross-queue views of the last plan()'s persisted queues (evg_queue_index_batch): each distro's first
+        min(length, cap) ranks (cap 0 = the reference's 10 000), the queues persist_task_queues would save.
+        -> ({task id: minQueuePosition, as FindMinimumQueuePositionForTask returns it}, {task id held by two or more
+        distros' queues: those distro ids}), both in the order of each id's first item, the distros in batch order."""
+        cap = cap or L.EVG_PERSISTED_QUEUE_CAP
+        queues = [ids[:cap] for ids in self.ranked]
+        flat = [i for q in queues for i in q]
+        item_off = np.concatenate([[0], np.cumsum([len(q) for q in queues])]).astype(np.int64)
+        r = self.engine.queue_index(flat, item_off)
+        positions = dict(zip(flat, r["min_position"].tolist()))
+        off, dq = r["dup_off"].tolist(), r["dup_queue"].tolist()
+        dups = {flat[int(i)]: [self.distro_ids[q] for q in dq[off[k]:off[k + 1]]] for k, i in enumerate(r["dup_item"].tolist())}
+        return positions, dups
 
     def remember(self, canon, soa: S.TaskSoA, table: S.DistroTable, keys) -> None:
         """Make the marshalled `canon` the resident tick the next diff starts from."""
@@ -1535,6 +1570,36 @@ def get_estimated_start_time(task: M.Task, queue: Optional[M.TaskQueue], hosts: 
     if pos == -1:
         return -1
     return estimated_start_times([queue], [hosts], running_tasks, now, engine=engine)[0][pos]
+
+
+def find_minimum_queue_position_for_task(queues: Sequence[M.TaskQueue], task_id: str) -> int:
+    """FindMinimumQueuePositionForTask (model/task_queue.go:407-435) over the saved documents of one collection, on the
+    host: 1 + the smallest array index of an item with this id in any queue, dispatched items included; -1 when no
+    queue holds it (the minQueuePosition resolver shows that as 0, graphql/task_resolver.go:570-581)."""
+    best = -1
+    for q in queues:
+        for k, item in enumerate(q.queue):
+            if item.id == task_id:
+                if best < 0 or k < best:
+                    best = k
+                break
+    return best + 1 if best >= 0 else -1
+
+
+def find_duplicate_enqueued_tasks(queues: Sequence[M.TaskQueue]) -> List[M.DuplicateEnqueuedTasksResult]:
+    """FindDuplicateEnqueuedTasks (model/task_queue.go:505-547) over the saved documents of one collection, on the host:
+    every task id that occurs more than once and in more than one distro's queue, with those distros.  The aggregation
+    leaves both orders open; this returns ids in the order of their first item and each id's distros in queue order,
+    the order evg_queue_index_batch pins."""
+    distros: Dict[str, List[str]] = {}
+    count: Dict[str, int] = {}
+    for q in queues:
+        for item in q.queue:
+            ds = distros.setdefault(item.id, [])
+            if q.distro not in ds:
+                ds.append(q.distro)
+            count[item.id] = count.get(item.id, 0) + 1
+    return [M.DuplicateEnqueuedTasksResult(task_id=i, distro_ids=list(ds)) for i, ds in distros.items() if count[i] > 1 and len(ds) > 1]
 
 
 def rebuild_dag_dispatchers(queues: Sequence[M.TaskQueue], *, engine: Optional[Engine] = None):

@@ -407,7 +407,7 @@ int evg_bind_result_buffer(evg_ctx* ctx, void* device_ptr, int64_t capacity);
  * evg_deps_met_batch, evg_find_runnable_batch / _ex, evg_plan_from_finder / _ex, evg_edit_tasks, evg_edit_tasks_with_deps, evg_plan_aliases,
  * evg_expected_durations_batch, evg_prioritize_legacy_batch, evg_dag_rebuild_batch, evg_rebuild_dispatchers,
  * evg_host_job, evg_host_drawdown, evg_idle_hosts, evg_find_next_batch, evg_find_next_tasks, evg_estimate_start_times,
- * evg_estimate_start_batch, evg_intern_batch and evg_upload_strings.  Every other call adds the kernels it launches: the uploads (their range check), evg_update_tasks,
+ * evg_estimate_start_batch, evg_intern_batch, evg_upload_strings and evg_queue_index_batch.  Every other call adds the kernels it launches: the uploads (their range check), evg_update_tasks,
  * evg_download_queue, evg_download_queue_breakdown and evg_resolve_durations. */
 int64_t evg_last_launch_count(evg_ctx* ctx);
 /* Device time in ms of the last evg_run_resident, from CUDA events on the context
@@ -798,6 +798,38 @@ int evg_intern_batch(evg_ctx* ctx, const evg_string_cols* in, evg_intern_out* ou
  * before them. */
 int evg_upload_strings(evg_ctx* ctx, const evg_task_soa* tasks, const evg_string_cols* strings, const evg_distro_cfg* cfg,
                        const evg_host_soa* hosts, const int64_t* host_off, const evg_alloc_cfg* acfg, evg_intern_out* out);
+
+/* ---- cross-queue views of the saved queues -------------------------------- */
+
+/* What evg_queue_index_batch writes; every array is caller-allocated. */
+typedef struct {
+  int32_t* min_position; /* n_items: 1 + the smallest index of this item's id in any queue (FindMinimumQueuePositionForTask) */
+  int64_t* dup_item;     /* capacity n_items: per duplicated id, the first item that carries it (to name it) */
+  int64_t* dup_off;      /* capacity n_items + 1 (n_dups + 1 written): CSR of dup_queue */
+  int32_t* dup_queue;    /* capacity n_items: the distinct queues holding that id, ascending */
+  int64_t  n_dups;       /* written: the number of duplicated ids */
+} evg_queue_index_out;
+
+/* The two readers of the whole task_queues collection, for every id at once: FindMinimumQueuePositionForTask
+ * (model/task_queue.go:407-435, GraphQL minQueuePosition) and FindDuplicateEnqueuedTasks (:505-547, the
+ * duplicate-task-check job).  `ids` holds the saved queue[]._id of every queue, concatenated (item_off[n_queues]
+ * strings); item_off (n_queues + 1) is a CSR over the queues, one queue being one distro's document of one collection.
+ * The arrays are taken as saved: for a resident tick, item_off and the rows evg_download_queue(ctx, 0, ...) returned,
+ * with the id of tasks[item.task].
+ *   - Positions: an index counts every item of the saved array, dispatched ones included (the aggregation has no
+ *     IsDispatched filter); an id repeated in one queue counts at its first index; min_position is the same on every
+ *     item of an id.  An id no queue holds has no item: the reference's -1, which the resolver shows as 0.
+ *   - Duplicates: an id is reported when it occurs in at least two distinct queues (an id twice in one queue and nowhere
+ *     else is not); empty queues contribute nothing.  Duplicated ids come in the order of their first item, each with
+ *     its distinct queues ascending (the aggregation leaves both orders open).
+ *   - Ids are compared byte for byte; "" is an ordinary id.  No output depends on the order of atomics.
+ * EVG_ERR_INVALID for null arguments or outputs, n_queues < 0, an item_off that does not start at 0 or decreases (named
+ * by row), more than 2^31-2 items, and an id offset outside the byte column (the kernel that reads the row checks it;
+ * the message names ids.off).  EVG_ERR_NOMEM, before any work, for a batch the device cannot hold; the context stays
+ * usable.  Needs no resident tick and leaves the tick, every flag and all run state as they were: it stages into buffers
+ * of its own, which the first call allocates.  EVG_INTERN_HASH_BITS masks the hash as for evg_intern_batch. */
+int evg_queue_index_batch(evg_ctx* ctx, const evg_str_col* ids, const int64_t* item_off, int32_t n_queues,
+                          evg_queue_index_out* out);
 
 /* ---- expected-duration statistics (SURVEY.md §8f.2) ----------------------- */
 
