@@ -102,6 +102,11 @@ class TaskEditStruct(C.Structure):
                 ("add_edge_dep", C.c_void_p), ("group_remap", C.c_void_p), ("version_remap", C.c_void_p)]
 
 
+class StringEditStruct(C.Structure):
+    _fields_ = [("n_remove", C.c_int64), ("remove_rows", C.c_void_p), ("insert", C.POINTER(TaskSoAStruct)),
+                ("insert_off", C.c_void_p), ("strings", C.POINTER(StringColsStruct))]
+
+
 class PlanOutStruct(C.Structure):
     _fields_ = [("order", C.c_void_p), ("total_value", C.c_void_p), ("breakdown", C.c_void_p),
                 ("info", C.c_void_p), ("group_info", C.c_void_p)]
@@ -354,6 +359,7 @@ SYMBOLS = {
     "evg_intern_columns": (C.c_int, [_P, _P, C.c_int32]),
     "evg_intern_batch": (C.c_int, [_P, _P, _P]),
     "evg_upload_strings": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P]),
+    "evg_edit_strings": (C.c_int, [_P, _P, _P, _P, _P, _P, _P]),
     "evg_queue_index_batch": (C.c_int, [_P, _P, _P, C.c_int32, _P]),
     "evg_run_resident": (C.c_int, [_P, C.c_int64, C.c_uint32]),
     "evg_download": (C.c_int, [_P, _P, _P]),

@@ -267,3 +267,102 @@ __global__ void __launch_bounds__(256) k_qx_write(int64_t m, int64_t n_dups, con
   if (j == 0 || (p >> 32) != (pairs[j - 1] >> 32)) dup_off[p >> 32] = pu[j];
   if (j == m - 1) dup_off[n_dups] = pu[m];
 }
+
+// ---- evg_edit_strings: the string table of an edited tick, composed on the device ---------------------------------
+// Composed row i of distro d is its survivors in their previous order (resident row src[i]), then its inserted rows
+// ins_off[d] .. ins_off[d+1] of the staged edit -- compose_tick's map.  Each composed string has a source code: >= 0 a
+// row of the resident column, < 0 row ~code of the staged one.  A staged row outside its column raises the lowest
+// composed row that holds it (bad_row); it gets length 0, so nothing reads through it.
+struct SxMap {
+  int32_t D;
+  const int64_t* new_off;  // D + 1: composed task_off
+  const int64_t* ins_off;  // D + 1: the staged rows' CSR over distros
+  const int32_t* src;      // composed row -> resident row, for survivors
+};
+struct SxCol {  // one string column: the resident one, the staged one, the composed one written here
+  DStr res, ins;
+  int64_t* out_off;
+  uint8_t* out_bytes;
+};
+
+// Per composed row: its source code, its TaskGroupMaxHosts and its DependsOn count (a staged dep_off row checked here).
+__global__ void __launch_bounds__(256) k_sx_rows(int64_t n, SxMap m, const int32_t* __restrict__ res_gmh, const int32_t* __restrict__ ins_gmh,
+                                                 const int64_t* __restrict__ res_dep_off, const int64_t* __restrict__ ins_dep_off,
+                                                 int64_t ins_E, int64_t* __restrict__ code, int32_t* __restrict__ gmh,
+                                                 int32_t* __restrict__ dep_cnt, unsigned long long* bad_row) {
+  const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  const int d = block_find_distro(m.new_off, m.D, i, n);
+  if (d < 0) return;
+  const int64_t k = i - m.new_off[d], S = (m.new_off[d + 1] - m.new_off[d]) - (m.ins_off[d + 1] - m.ins_off[d]);
+  if (k < S) {
+    const int64_t t = m.src[i];
+    code[i] = t;
+    gmh[i] = res_gmh[t];
+    dep_cnt[i] = int32_t(res_dep_off[t + 1] - res_dep_off[t]);
+  } else {
+    const int64_t j = m.ins_off[d] + (k - S), e0 = ins_dep_off[j], e1 = ins_dep_off[j + 1];
+    const bool bad = e0 < 0 || e1 < e0 || e1 > ins_E || e1 - e0 > INT32_MAX;
+    if (bad) atomicMin(bad_row, (unsigned long long)i);
+    code[i] = ~j;
+    gmh[i] = ins_gmh[j];
+    dep_cnt[i] = bad ? 0 : int32_t(e1 - e0);
+  }
+}
+
+// Per composed row, after the scan dep_off of the counts: the source code of each of its DependsOn ids.
+__global__ void __launch_bounds__(256) k_sx_edges(int64_t n, const int64_t* __restrict__ code, const int64_t* __restrict__ res_dep_off,
+                                                  const int64_t* __restrict__ ins_dep_off, const int64_t* __restrict__ dep_off,
+                                                  int64_t* __restrict__ ecode) {
+  const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int64_t c = code[i], w0 = dep_off[i], w1 = dep_off[i + 1];
+  const int64_t e0 = c >= 0 ? res_dep_off[c] : ins_dep_off[~c];
+  for (int64_t w = w0; w < w1; w++) ecode[w] = c >= 0 ? e0 + (w - w0) : ~(e0 + (w - w0));
+}
+
+// Per composed string: its length (scanned into out_off next).  owner_off: the composed dep_off when the strings are
+// DependsOn ids (a bad one names its row), NULL when string r is row r.
+__global__ void __launch_bounds__(256) k_sx_len(int64_t n, const int64_t* __restrict__ code, SxCol col, const int64_t* __restrict__ owner_off,
+                                                int32_t n_owner, int32_t* __restrict__ len, unsigned long long* bad_row) {
+  const int64_t r = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (r >= n) return;
+  const int64_t c = code[r], q = c >= 0 ? c : ~c;
+  const int64_t* __restrict__ off = c >= 0 ? col.res.off : col.ins.off;
+  const int64_t o0 = off[q], o1 = off[q + 1];
+  if (c < 0 && (in_row_bad(col.ins, o0, o1) || o1 - o0 > INT32_MAX)) {
+    atomicMin(bad_row, (unsigned long long)(owner_off ? find_distro(owner_off, 0, n_owner - 1, r) : r));
+    len[r] = 0;
+  } else {
+    len[r] = int32_t(o1 - o0);
+  }
+}
+
+// Bytes [0, n) of src to dst by one warp, V-wide where both are V-aligned (their distance is a multiple of V).
+template <class V>
+__device__ __forceinline__ void sx_copy_as(uint8_t* __restrict__ dst, const uint8_t* __restrict__ src, int64_t n, int lane) {
+  constexpr int W = sizeof(V);
+  const int64_t head = min(n, int64_t((W - (reinterpret_cast<uintptr_t>(dst) & (W - 1))) & (W - 1)));
+  for (int64_t i = lane; i < head; i += 32) dst[i] = src[i];
+  const int64_t nv = (n - head) / W;
+  V* __restrict__ d = reinterpret_cast<V*>(dst + head);
+  const V* __restrict__ s = reinterpret_cast<const V*>(src + head);
+  for (int64_t v = lane; v < nv; v += 32) d[v] = s[v];
+  for (int64_t i = head + nv * W + lane; i < n; i += 32) dst[i] = src[i];
+}
+
+// A warp per composed string: its bytes from its source column to out_off[r].
+__global__ void __launch_bounds__(256) k_sx_copy(int64_t n, const int64_t* __restrict__ code, SxCol col) {
+  const int64_t r = (int64_t(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (r >= n) return;
+  const int64_t o = col.out_off[r], len = col.out_off[r + 1] - o;
+  if (len == 0) return;
+  const int64_t c = code[r];
+  const uint8_t* src = c >= 0 ? col.res.bytes + col.res.off[c] : col.ins.bytes + col.ins.off[~c];
+  uint8_t* dst = col.out_bytes + o;
+  const uintptr_t mis = reinterpret_cast<uintptr_t>(src) ^ reinterpret_cast<uintptr_t>(dst);
+  if ((mis & 15) == 0) sx_copy_as<uint4>(dst, src, len, lane);
+  else if ((mis & 7) == 0) sx_copy_as<uint2>(dst, src, len, lane);
+  else if ((mis & 3) == 0) sx_copy_as<uint32_t>(dst, src, len, lane);
+  else sx_copy_as<uint8_t>(dst, src, len, lane);
+}

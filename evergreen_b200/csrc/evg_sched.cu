@@ -33,6 +33,7 @@
 //   k_host_job            hostAllocatorJob.Run past the allocator: single-task bypass, report, drawdown (units/host_allocator.go:180-425)
 //   k_next_verdict/serve  the DAG dispatcher's FindNextTask, a warp per distro (model/task_queue_service_dependency.go:258-692)
 //   k_in_*                evg_intern_columns on the device: string keys to dense ids, dependency ids to queue indices
+//   k_sx_*                evg_edit_strings: the resident string table and an edit composed into the next tick's
 //   k_qx_*                the saved queues joined by task id: minimum queue positions, duplicate enqueued tasks
 //                         (model/task_queue.go:407-435, 505-547)
 // No CPU fallback exists in this file: without a device every entry point fails.
@@ -1485,11 +1486,12 @@ struct evg_ctx {
   // evg_host_job's reports in hj.out are from the current run; a chained evg_host_drawdown reads them.  `dispatchers`:
   // run state -- evg_rebuild_dispatchers built dp and nx from the current run; evg_find_next_tasks serves from them.
   // `queue_breakdown`: run state -- the current run kept the units evg_download_queue_breakdown reads back, and the
-  // task columns it scores them from have not been written since.
+  // task columns it scores them from have not been written since.  `strings`: `st` holds the string table the resident
+  // tick was interned from (evg_upload_strings, evg_edit_strings), so evg_edit_strings can edit it.
   struct {
     Tick kind = Tick::kNone;
     bool hosts = false, deps = false, aliases = false, durations = false, allocated = false, host_job = false, dispatchers = false;
-    bool queue_breakdown = false, dep_table = false;
+    bool queue_breakdown = false, dep_table = false, strings = false;
   } tick;
   int64_t T = 0, E = 0, G = 0, H = 0, U = 0, NT = 0, t_pad = 0;
   int32_t Dn = 0;
@@ -1579,6 +1581,15 @@ struct evg_ctx {
     DevBuf task_off, gmh, dep_off, bytes[4], off[4], key, first, gslot, vslot, fg, fv, pg, pv, res, cnt, samp, err;
     DevBuf gid, vid, gmax, gfirst, out_dep_off, out_dep_idx;
   } in;
+  // While tick.strings: the resident tick's string table, swapped in from `in` after interning -- the four columns in
+  // InView order (bytes and offsets), every row's TaskGroupMaxHosts and its dep_off over ALL its DependsOn ids -- with
+  // the bytes of each column and the id count.  Then evg_edit_strings' staged edit (the same columns of the inserted
+  // rows), the composed strings' source codes and lengths, and its error word.
+  struct {
+    DevBuf gmh, dep_off, bytes[4], off[4];
+    int64_t nb[4] = {0, 0, 0, 0}, E = 0;
+    DevBuf x_gmh, x_dep_off, x_bytes[4], x_off[4], code, ecode, len, bad;
+  } st;
   // evg_queue_index_batch (the first call allocates these): the staged ids and item_off, the task-id table, each item's
   // slot, queue and id number, the flags and their scans, the per-id reductions, the pairs (two copies: the radix
   // sort's) with its histograms, the outputs and the error word
@@ -1674,7 +1685,7 @@ void drop_tick(evg_ctx* c) { c->tick = {}; }
 // What a call needs of the resident tick.  EVG_ERR_STATE names the call and the first unmet condition: a tick, then
 // its kind, then the state the call reads.
 enum class Need { kTick, kOwnColumns, kEditable, kHosts, kVerdicts, kAliasMap, kDurations, kAllocated, kHostJob, kDispatchers,
-                  kQueueBreakdown, kDepTable };
+                  kQueueBreakdown, kDepTable, kStrings };
 int need_tick(const evg_ctx* c, const char* who, Need what) {
   const auto& t = c->tick;
   const bool own = what == Need::kOwnColumns || what == Need::kEditable;
@@ -1686,6 +1697,8 @@ int need_tick(const evg_ctx* c, const char* who, Need what) {
                       : what == Need::kVerdicts && !t.deps                ? "the resident tick was not uploaded with evg_upload_with_deps"
                       : what == Need::kDepTable && !t.dep_table
                           ? "the resident tick holds no dependency table (evg_upload_with_deps or evg_edit_tasks_with_deps set one)"
+                      : what == Need::kStrings && !t.strings
+                          ? "the resident tick holds no string table (evg_upload_strings or evg_edit_strings set one)"
                       : what == Need::kAliasMap && !t.aliases             ? "the resident tick was not built by evg_plan_aliases"
                       : what == Need::kDurations && !t.durations          ? "no evg_resolve_durations on the resident tick's rows"
                       : what == Need::kHostJob && !t.host_job             ? "no evg_host_job on the resident tick's current run"
@@ -4538,47 +4551,51 @@ struct InternSizes {
   std::vector<int64_t> edge_off;   // D + 1: the in-queue dep_off at the distro boundaries
 };
 
-// The strings of `in` (passed by intern_check, n_tasks > 0) interned on c->stream: group and version ids into gid / vid,
-// the in-queue edges into dep_off / dep_idx, the group tables into c->in.gmax / c->in.gfirst (one entry per group slot),
-// the per-distro sizes into *z.  Every buffer is sized before the first launch, so a tick too large for the device
-// fails with EVG_ERR_NOMEM before any work and leaves the context usable.  Three syncs: the row checks, the sizes, the end.
-static int intern_strings(evg_ctx* c, const char* who, const evg_string_cols* in, DevBuf& gid, DevBuf& vid, DevBuf& dep_off,
-                          DevBuf& dep_idx, InternSizes* z) {
+// Grows buffers and remembers the first failure.  A call sizes everything it will use with one of these before its
+// first launch, so that a tick too large for the device fails with EVG_ERR_NOMEM before any work and leaves the context
+// usable.
+struct Sizing {
+  cudaError_t e = cudaSuccess;
+  void operator()(DevBuf& x, int64_t bytes) {
+    if (e == cudaSuccess) e = x.ensure(size_t(std::max<int64_t>(bytes, 1)));
+  }
+  int result(const char* who, int64_t T) const {
+    if (e == cudaSuccess) return EVG_OK;
+    cudaGetLastError();  // a failed allocation is not sticky: clear it so that the next call starts clean
+    return fail(e == cudaErrorMemoryAllocation ? EVG_ERR_NOMEM : EVG_ERR_CUDA, "%s: %s while sizing %lld tasks", who,
+                cudaGetErrorString(e), (long long)T);
+  }
+};
+
+// The interning pipeline's buffers for T rows over D distros, E DependsOn ids and nb[k] bytes in string column k (InView
+// order): the columns it reads from c->in, its tables and scratch, and the outputs gid / vid / dep_off / dep_idx.
+static void intern_size(Sizing& need, evg_ctx* c, int64_t T, int32_t D, int64_t E, const int64_t nb[4], DevBuf& gid, DevBuf& vid,
+                        DevBuf& dep_off, DevBuf& dep_idx) {
+  auto& b = c->in;
+  uint64_t cap = 64;
+  while (cap < 2 * uint64_t(T)) cap <<= 1;
+  const int64_t rows[4] = {T, T, T, E};
+  need(b.task_off, 8 * (D + 1)); need(b.gmh, 4 * T); need(b.dep_off, 8 * (T + 1));
+  for (int k = 0; k < 4; k++) { need(b.off[k], 8 * (rows[k] + 1)); need(b.bytes[k], nb[k]); }
+  need(b.key, 8 * 3 * int64_t(cap)); need(b.first, 4 * 3 * int64_t(cap));
+  need(b.gslot, 8 * T); need(b.vslot, 8 * T); need(b.fg, 4 * T); need(b.fv, 4 * T); need(b.pg, 8 * (T + 1)); need(b.pv, 8 * (T + 1));
+  need(b.res, 4 * E); need(b.cnt, 4 * T); need(b.samp, 8 * 3 * (D + 1)); need(b.err, 16);
+  need(b.gmax, 4 * T); need(b.gfirst, 8 * T); need(c->b_scansum, 8 * ((T + 1023) / 1024 + 1));
+  need(gid, 4 * (T + kColPad)); need(vid, 4 * (T + kColPad)); need(dep_off, 8 * (T + 1 + kColPad)); need(dep_idx, 4 * (E + kColPad));
+}
+
+// The interning pipeline over the columns in c->in (T > 0 rows over D distros, E DependsOn ids, nb[k] bytes in column
+// k, task_off staged too), on c->stream: group and version ids into gid / vid, the in-queue edges into dep_off / dep_idx,
+// the group tables into c->in.gmax / c->in.gfirst (one entry per group slot), the per-distro sizes into *z.  `host`: the
+// host columns they were staged from, which a failed row check reads to name the row; NULL when the columns were
+// composed on the device (every row was checked there).  intern_size sized every buffer.  Three syncs: the row checks,
+// the sizes, the end.
+static int intern_run(evg_ctx* c, const char* who, int64_t T, int32_t D, int64_t E, const int64_t nb[4], const evg_string_cols* host,
+                      DevBuf& gid, DevBuf& vid, DevBuf& dep_off, DevBuf& dep_idx, InternSizes* z) {
   cudaStream_t s = c->stream;
   auto& b = c->in;
-  const int64_t T = in->n_tasks;
-  const int32_t D = in->n_distros;
-  const evg_str_col* cols[4];
-  int64_t rows[4], nb[4];
-  intern_cols(in, cols, rows);
-  const int64_t E = rows[3];
-  for (int k = 0; k < 4; k++) nb[k] = rows[k] > 0 ? cols[k]->off[rows[k]] : 0;
   uint64_t cap = 64;
   while (cap < 2 * uint64_t(T)) cap <<= 1;  // at most T keys a column: load factor <= 1/2
-  {
-    cudaError_t e = cudaSuccess;
-    auto need = [&](DevBuf& x, int64_t bytes) { if (e == cudaSuccess) e = x.ensure(size_t(std::max<int64_t>(bytes, 1))); };
-    need(b.task_off, 8 * (D + 1)); need(b.gmh, 4 * T); need(b.dep_off, 8 * (T + 1));
-    for (int k = 0; k < 4; k++) { need(b.off[k], 8 * (rows[k] + 1)); need(b.bytes[k], nb[k]); }
-    need(b.key, 8 * 3 * int64_t(cap)); need(b.first, 4 * 3 * int64_t(cap));
-    need(b.gslot, 8 * T); need(b.vslot, 8 * T); need(b.fg, 4 * T); need(b.fv, 4 * T); need(b.pg, 8 * (T + 1)); need(b.pv, 8 * (T + 1));
-    need(b.res, 4 * E); need(b.cnt, 4 * T); need(b.samp, 8 * 3 * (D + 1)); need(b.err, 16);
-    need(b.gmax, 4 * T); need(b.gfirst, 8 * T); need(c->b_scansum, 8 * ((T + 1023) / 1024 + 1));
-    need(gid, 4 * (T + kColPad)); need(vid, 4 * (T + kColPad)); need(dep_off, 8 * (T + 1 + kColPad)); need(dep_idx, 4 * (E + kColPad));
-    if (e != cudaSuccess) {
-      cudaGetLastError();  // a failed allocation is not sticky: clear it so that the next call starts clean
-      return fail(e == cudaErrorMemoryAllocation ? EVG_ERR_NOMEM : EVG_ERR_CUDA, "%s: %s while sizing %lld tasks", who,
-                  cudaGetErrorString(e), (long long)T);
-    }
-  }
-  // ---- stage the columns; the tables empty
-  CK(cudaMemcpyAsync(b.task_off.p, in->task_off, sizeof(int64_t) * size_t(D + 1), cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(b.gmh.p, in->group_max_hosts, sizeof(int32_t) * size_t(T), cudaMemcpyHostToDevice, s));
-  CK(cudaMemcpyAsync(b.dep_off.p, in->dep_off, sizeof(int64_t) * size_t(T + 1), cudaMemcpyHostToDevice, s));
-  for (int k = 0; k < 4; k++) {
-    if (rows[k] > 0) CK(cudaMemcpyAsync(b.off[k].p, cols[k]->off, sizeof(int64_t) * size_t(rows[k] + 1), cudaMemcpyHostToDevice, s));
-    if (nb[k] > 0) CK(cudaMemcpyAsync(b.bytes[k].p, cols[k]->bytes, size_t(nb[k]), cudaMemcpyHostToDevice, s));
-  }
   CK(cudaMemsetAsync(b.key.p, 0xFF, sizeof(uint64_t) * 3 * cap, s));
   CK(cudaMemsetAsync(b.first.p, 0xFF, sizeof(uint32_t) * 3 * cap, s));
   CK(cudaMemsetAsync(b.err.p, 0, sizeof(int), s));
@@ -4604,12 +4621,17 @@ static int intern_strings(evg_ctx* c, const char* who, const evg_string_cols* in
   CK(cudaMemcpyAsync(&bad, err, sizeof(int), cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
   CK(cudaGetLastError());
-  if (bad & kInErrDepOff) return check_offsets(in->dep_off, T, -1, who, "dep_off");
-  for (int k = 0; k < 4; k++)
-    if (bad & (kInErrGroupOff << k)) {
-      const int rc = check_offsets(cols[k]->off, rows[k], -1, who, kInColName[k]);
-      return rc != EVG_OK ? rc : fail(EVG_ERR_INVALID, "%s: %s breaks its byte column", who, kInColName[k]);
-    }
+  if (bad) {
+    const evg_str_col* cols[4];
+    int64_t rows[4];
+    if (host) intern_cols(host, cols, rows);
+    if (bad & kInErrDepOff) return host ? check_offsets(host->dep_off, T, -1, who, "dep_off") : fail(EVG_ERR_INVALID, "%s: dep_off breaks its column", who);
+    for (int k = 0; k < 4; k++)
+      if (bad & (kInErrGroupOff << k)) {
+        const int rc = host ? check_offsets(cols[k]->off, rows[k], -1, who, kInColName[k]) : EVG_OK;
+        return rc != EVG_OK ? rc : fail(EVG_ERR_INVALID, "%s: %s breaks its byte column", who, kInColName[k]);
+      }
+  }
   // ---- 2. first-appearance flags and their scans number each distro's groups and versions; ids, group tables, edge counts
   launch(c, s, k_al_flag, grid_for(T, 256), 256, 0, T, gslot, vslot, v.first, b.fg.as<int32_t>(), b.fv.as<int32_t>());
   CK(scan_counts(c, b.fg.as<int32_t>(), T, pg));
@@ -4641,11 +4663,87 @@ static int intern_strings(evg_ctx* c, const char* who, const evg_string_cols* in
   return EVG_OK;
 }
 
+// The strings of `in` (passed by intern_check, n_tasks > 0) sized for, staged into c->in and interned (intern_run).
+static int intern_strings(evg_ctx* c, const char* who, const evg_string_cols* in, DevBuf& gid, DevBuf& vid, DevBuf& dep_off,
+                          DevBuf& dep_idx, InternSizes* z) {
+  cudaStream_t s = c->stream;
+  auto& b = c->in;
+  const int64_t T = in->n_tasks;
+  const int32_t D = in->n_distros;
+  const evg_str_col* cols[4];
+  int64_t rows[4], nb[4];
+  intern_cols(in, cols, rows);
+  for (int k = 0; k < 4; k++) nb[k] = rows[k] > 0 ? cols[k]->off[rows[k]] : 0;
+  Sizing need;
+  intern_size(need, c, T, D, rows[3], nb, gid, vid, dep_off, dep_idx);
+  if (const int rc = need.result(who, T); rc != EVG_OK) return rc;
+  CK(cudaMemcpyAsync(b.task_off.p, in->task_off, sizeof(int64_t) * size_t(D + 1), cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(b.gmh.p, in->group_max_hosts, sizeof(int32_t) * size_t(T), cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(b.dep_off.p, in->dep_off, sizeof(int64_t) * size_t(T + 1), cudaMemcpyHostToDevice, s));
+  for (int k = 0; k < 4; k++) {
+    if (rows[k] > 0) CK(cudaMemcpyAsync(b.off[k].p, cols[k]->off, sizeof(int64_t) * size_t(rows[k] + 1), cudaMemcpyHostToDevice, s));
+    if (nb[k] > 0) CK(cudaMemcpyAsync(b.bytes[k].p, cols[k]->bytes, size_t(nb[k]), cudaMemcpyHostToDevice, s));
+  }
+  return intern_run(c, who, T, D, rows[3], nb, in, gid, vid, dep_off, dep_idx, z);
+}
+
 // Device to host on c->stream when both ends exist.
 #define D2H_IF(dst, src, count, type)                                                                                       \
   do {                                                                                                                      \
     if ((dst) && (count) > 0) CK(cudaMemcpyAsync((dst), (src), sizeof(type) * size_t(count), cudaMemcpyDeviceToHost, c->stream)); \
   } while (0)
+
+// The interned tick in the shadow set (T rows over task_off; ids in ed.out, edges in ed.dep_off / ed.dep_idx, group
+// tables in `in`, sizes in z) becomes the resident one, the caller's outputs are filled, and the composed string table
+// staged in `in` (nb[k] bytes per column, z's DependsOn ids) becomes the tick's own -- evg_upload_strings and
+// evg_edit_strings.  cfg[d].n_versions is taken from z.
+static int install_interned(evg_ctx* c, const char* who, int64_t T, const int64_t* task_off, const evg_distro_cfg* cfg, const InternSizes& z,
+                            const evg_host_soa* hosts, const int64_t* host_off, const evg_alloc_cfg* acfg, evg_intern_out* out,
+                            const int64_t nb[4]) {
+  cudaStream_t s = c->stream;
+  auto& e = c->ed;
+  const int32_t D = int32_t(z.n_versions.size());
+  // ---- the group slots' max hosts (the upload stages them from the host) and what the caller asked for
+  const int64_t G = z.group_off[size_t(D)], En = z.edge_off[size_t(D)];
+  std::vector<int32_t> gmax(size_t(G) + 1);
+  int64_t E_all = 0;  // the staged dep_off's last row: every DependsOn id of the table
+  D2H_IF(gmax.data(), c->in.gmax.p, G, int32_t);
+  D2H_IF(&E_all, c->in.dep_off.as<int64_t>() + T, T > 0 ? 1 : 0, int64_t);
+  D2H_IF(out->group_max_hosts, c->in.gmax.p, G, int32_t);
+  D2H_IF(out->group_first, c->in.gfirst.p, G, int64_t);
+  D2H_IF(out->group_id, e.out.gid.p, T, int32_t);
+  D2H_IF(out->version_id, e.out.vid.p, T, int32_t);
+  D2H_IF(out->dep_off, e.dep_off.p, T > 0 ? T + 1 : 0, int64_t);
+  D2H_IF(out->dep_idx, e.dep_idx.p, En, int32_t);
+  CK(cudaStreamSynchronize(s));
+  memcpy(out->group_off, z.group_off.data(), sizeof(int64_t) * size_t(D + 1));
+  if (D > 0) memcpy(out->n_versions, z.n_versions.data(), sizeof(int32_t) * size_t(D));
+  std::vector<evg_distro_cfg> cf(cfg, cfg + D);
+  for (int32_t d = 0; d < D; d++) cf[size_t(d)].n_versions = z.n_versions[size_t(d)];
+  evg_distro_table dt;
+  memset(&dt, 0, sizeof(dt));
+  dt.n_distros = D; dt.task_off = task_off; dt.group_off = z.group_off.data(); dt.cfg = cf.data(); dt.group_max_hosts = gmax.data();
+  int rc = install_composed(c, who, T, En, z.edge_off.data(), &dt);
+  if (rc != EVG_OK) return rc;
+  if (hosts) {
+    rc = upload_hosts(c, who, hosts, host_off, acfg, D);
+    if (rc != EVG_OK) return rc;
+    CK(cudaStreamSynchronize(s));
+  }
+  c->tick.kind = Tick::kOwn;
+  auto& b = c->in;
+  auto& x = c->st;
+  b.gmh.swap(x.gmh);
+  b.dep_off.swap(x.dep_off);
+  for (int k = 0; k < 4; k++) {
+    b.bytes[k].swap(x.bytes[k]);
+    b.off[k].swap(x.off[k]);
+    x.nb[k] = nb[k];
+  }
+  x.E = E_all;
+  c->tick.strings = true;
+  return EVG_OK;
+}
 
 int evg_intern_batch(evg_ctx* c, const evg_string_cols* in, evg_intern_out* out) {
   ENTER(c, "evg_intern_batch");
@@ -4707,7 +4805,7 @@ int evg_upload_strings(evg_ctx* c, const evg_task_soa* tasks, const evg_string_c
   rc = e.out.size(T, s, /*zero_pad=*/true);
   if (rc == EVG_OK) rc = e.out.copy_rows(tasks, 0, T, s, /*ids=*/false);
   if (rc != EVG_OK) {
-    cudaGetLastError();  // as in intern_strings: a failed allocation leaves the context usable
+    cudaGetLastError();  // as in Sizing: a failed allocation leaves the context usable
     return rc;
   }
   InternSizes z;
@@ -4718,33 +4816,161 @@ int evg_upload_strings(evg_ctx* c, const evg_task_soa* tasks, const evg_string_c
     rc = intern_strings(c, who, strings, e.out.gid, e.out.vid, e.dep_off, e.dep_idx, &z);
     if (rc != EVG_OK) return rc;
   }
-  // ---- the group slots' max hosts (the upload stages them from the host) and what the caller asked for
-  const int64_t G = z.group_off[size_t(D)], En = z.edge_off[size_t(D)];
-  std::vector<int32_t> gmax(size_t(G) + 1);
-  D2H_IF(gmax.data(), c->in.gmax.p, G, int32_t);
-  D2H_IF(out->group_max_hosts, c->in.gmax.p, G, int32_t);
-  D2H_IF(out->group_first, c->in.gfirst.p, G, int64_t);
-  D2H_IF(out->group_id, e.out.gid.p, T, int32_t);
-  D2H_IF(out->version_id, e.out.vid.p, T, int32_t);
-  D2H_IF(out->dep_off, e.dep_off.p, T > 0 ? T + 1 : 0, int64_t);
-  D2H_IF(out->dep_idx, e.dep_idx.p, En, int32_t);
-  CK(cudaStreamSynchronize(s));
-  memcpy(out->group_off, z.group_off.data(), sizeof(int64_t) * size_t(D + 1));
-  if (D > 0) memcpy(out->n_versions, z.n_versions.data(), sizeof(int32_t) * size_t(D));
-  std::vector<evg_distro_cfg> cf(cfg, cfg + D);
-  for (int32_t d = 0; d < D; d++) cf[size_t(d)].n_versions = z.n_versions[size_t(d)];
-  evg_distro_table dt;
-  memset(&dt, 0, sizeof(dt));
-  dt.n_distros = D; dt.task_off = strings->task_off; dt.group_off = z.group_off.data(); dt.cfg = cf.data(); dt.group_max_hosts = gmax.data();
-  rc = install_composed(c, who, T, En, z.edge_off.data(), &dt);
+  const evg_str_col* cols[4];
+  int64_t rows[4], nb[4];
+  intern_cols(strings, cols, rows);
+  for (int k = 0; k < 4; k++) nb[k] = rows[k] > 0 ? cols[k]->off[rows[k]] : 0;
+  return install_interned(c, who, T, strings->task_off, cfg, z, hosts, host_off, acfg, out, nb);
+}
+
+// evg_edit_strings: the survivors' strings gathered from the resident string table, the inserted rows' appended, the
+// composed table interned as evg_upload_strings interns a staged one (evg_intern.cuh: k_sx_*)
+int evg_edit_strings(evg_ctx* c, const evg_string_edit* ed, const evg_distro_cfg* cfg, const evg_host_soa* hosts,
+                     const int64_t* host_off, const evg_alloc_cfg* acfg, evg_intern_out* out) {
+  ENTER(c, "evg_edit_strings");
+  c->launches = 0;
+  // ---- every check the host can make, before anything resident changes
+  if (!ed || !out) return fail(EVG_ERR_INVALID, "%s: null argument", who);
+  if (const int rc = need_tick(c, who, Need::kStrings); rc != EVG_OK) return rc;
+  const evg_task_soa* ins = ed->insert;
+  const evg_string_cols* str = ed->strings;
+  if (!ins || !str || !ed->insert_off) return fail(EVG_ERR_INVALID, "%s: null insert / insert_off / strings", who);
+  const int32_t D = c->Dn;
+  const int64_t T0 = c->T, R = ed->n_remove, I = ins->n_tasks;
+  if (R < 0 || I < 0) return fail(EVG_ERR_INVALID, "%s: negative sizes", who);
+  if (R > 0 && !ed->remove_rows) return fail(EVG_ERR_INVALID, "%s: null remove_rows", who);
+  if (str->n_distros != D) return fail(EVG_ERR_INVALID, "%s: n_distros %d, the resident tick has %d", who, str->n_distros, D);
+  if (str->n_tasks != I) return fail(EVG_ERR_INVALID, "%s: insert has %lld rows, strings %lld", who, (long long)I, (long long)str->n_tasks);
+  if (ins->group_id || ins->version_id || ins->dep_off || ins->dep_idx)
+    return fail(EVG_ERR_INVALID, "%s: insert->group_id, version_id, dep_off and dep_idx come from the strings and must be NULL", who);
+  if (I > 0 && TaskCols::missing(ins, /*ids=*/false)) return fail(EVG_ERR_INVALID, "%s: null inserted column", who);
+  if (!out->group_off || (D > 0 && (!out->n_versions || !cfg))) return fail(EVG_ERR_INVALID, "%s: null cfg / output", who);
+  int rc = D > 0 ? check_offsets(ed->insert_off, D, I, who, "insert_off") : EVG_OK;
+  if (rc == EVG_OK) rc = intern_check(who, str);
   if (rc != EVG_OK) return rc;
-  if (hosts) {
-    rc = upload_hosts(c, who, hosts, host_off, acfg, D);
-    if (rc != EVG_OK) return rc;
-    CK(cudaStreamSynchronize(s));
+  for (int32_t d = 0; d <= D && D > 0; d++)
+    if (str->task_off[d] != ed->insert_off[d]) return fail(EVG_ERR_INVALID, "%s: strings->task_off differs from insert_off at %d", who, d);
+  std::vector<int64_t> new_off(size_t(D) + 1, 0), removed(size_t(D) + 1, 0);
+  for (int64_t k = 0; k < R; k++) {
+    const int64_t r = ed->remove_rows[k];
+    if (r < 0 || r >= T0 || (k > 0 && r <= ed->remove_rows[k - 1]))
+      return fail(EVG_ERR_INVALID, "%s: remove_rows[%lld] = %lld is not ascending inside [0, %lld)", who, (long long)k, (long long)r, (long long)T0);
+    removed[size_t(std::upper_bound(c->h_taskoff.begin(), c->h_taskoff.end(), r) - c->h_taskoff.begin() - 1)]++;
   }
-  c->tick.kind = Tick::kOwn;
-  return EVG_OK;
+  for (int32_t d = 0; d < D; d++) {
+    const int64_t n = (c->h_taskoff[d + 1] - c->h_taskoff[d]) - removed[d] + (ed->insert_off[d + 1] - ed->insert_off[d]);
+    if (n > kMaxTasksPerDistro) return fail(EVG_ERR_INVALID, "%s: distro %d holds %lld tasks (max %lld)", who, d, (long long)n, (long long)kMaxTasksPerDistro);
+    new_off[size_t(d) + 1] = new_off[size_t(d)] + n;
+  }
+  const int64_t Tn = new_off[size_t(D)];
+  if (Tn > (int64_t(1) << 31) - 2) return fail(EVG_ERR_INVALID, "%s: %lld tasks exceed 2^31-2", who, (long long)Tn);
+  // ---- every buffer sized before the first launch; the composed strings by the resident plus the inserted ones
+  cudaStream_t s = c->stream;
+  auto& e = c->ed;
+  auto& x = c->st;
+  auto& b = c->in;
+  const evg_str_col* cols[4];
+  int64_t rows[4], nb_ins[4], nb_max[4];
+  intern_cols(str, cols, rows);
+  for (int k = 0; k < 4; k++) {
+    nb_ins[k] = rows[k] > 0 ? cols[k]->off[rows[k]] : 0;
+    nb_max[k] = x.nb[k] + nb_ins[k];
+  }
+  const int64_t E_ins = rows[3], E_max = x.E + E_ins;
+  {
+    Sizing need;
+    if (Tn > 0) intern_size(need, c, Tn, D, E_max, nb_max, e.out.gid, e.out.vid, e.dep_off, e.dep_idx);
+    need(e.rm, 8 * R); need(e.old_off, 8 * (D + 1)); need(e.ins_off, 8 * (D + 1)); need(e.new_off, 8 * (D + 1));
+    need(e.keep, 4 * (T0 + 1)); need(e.pos, 8 * (T0 + 1)); need(e.src, 4 * (Tn + 1)); need(e.err, 4);
+    need(x.x_gmh, 4 * I); need(x.x_dep_off, 8 * (I + 1));
+    for (int k = 0; k < 4; k++) { need(x.x_off[k], 8 * (rows[k] + 1)); need(x.x_bytes[k], nb_ins[k]); }
+    need(x.code, 8 * Tn); need(x.ecode, 8 * E_max); need(x.len, 4 * std::max(Tn, E_max)); need(x.bad, 8);
+    need(c->b_scansum, 8 * ((std::max({T0, Tn, E_max}) + 1023) / 1024 + 1));
+    if ((rc = need.result(who, Tn)) != EVG_OK) return rc;
+    rc = e.out.size(Tn, s, /*zero_pad=*/true);
+    if (rc == EVG_OK) rc = e.ins.size(I);
+    if (rc != EVG_OK) {
+      cudaGetLastError();  // as in Sizing: a failed allocation leaves the context usable
+      return rc;
+    }
+  }
+  // ---- stage the edit: from the first launch on, an error leaves no resident tick
+  drop_tick(c);
+  auto h2d = [&](DevBuf& dst, const void* src, int64_t bytes) {
+    return bytes > 0 ? cudaMemcpyAsync(dst.p, src, size_t(bytes), cudaMemcpyHostToDevice, s) : cudaSuccess;
+  };
+  CK(h2d(e.rm, ed->remove_rows, 8 * R));
+  CK(h2d(e.old_off, c->h_taskoff.data(), 8 * (D + 1)));
+  CK(h2d(e.ins_off, ed->insert_off, 8 * (D + 1)));
+  CK(h2d(e.new_off, new_off.data(), 8 * (D + 1)));
+  if ((rc = e.ins.copy_rows(ins, 0, I, s, /*ids=*/false)) != EVG_OK) return rc;
+  CK(h2d(x.x_gmh, str->group_max_hosts, 4 * I));
+  CK(h2d(x.x_dep_off, str->dep_off, I > 0 ? 8 * (I + 1) : 0));
+  for (int k = 0; k < 4; k++) {
+    CK(h2d(x.x_off[k], cols[k]->off, rows[k] > 0 ? 8 * (rows[k] + 1) : 0));
+    CK(h2d(x.x_bytes[k], cols[k]->bytes, nb_ins[k]));
+  }
+  unsigned long long* bad = x.bad.as<unsigned long long>();
+  CK(cudaMemsetAsync(bad, 0xFF, sizeof(unsigned long long), s));  // the lowest bad composed row: none yet
+  // ---- 1. compose_tick's map: each survivor's place, composed row -> resident row
+  EdMap m;
+  memset(&m, 0, sizeof(m));
+  m.D = D; m.new_off = e.new_off.as<int64_t>(); m.old_off = e.old_off.as<int64_t>(); m.ins_off = e.ins_off.as<int64_t>();
+  m.keep = e.keep.as<int32_t>(); m.pos = e.pos.as<int64_t>(); m.src = e.src.as<int32_t>();
+  launch(c, s, k_ed_keep, grid_for(T0, 256), 256, 0, T0, e.rm.as<int64_t>(), R, e.keep.as<int32_t>());
+  if (T0 > 0) {
+    CK(scan_counts(c, e.keep.as<int32_t>(), T0, e.pos.as<int64_t>()));
+    launch(c, s, k_ed_src, grid_for(T0, 256), 256, 0, T0, m, e.src.as<int32_t>());
+  }
+  InternSizes z;
+  z.group_off.assign(size_t(D) + 1, 0);
+  z.edge_off.assign(size_t(D) + 1, 0);
+  z.n_versions.assign(size_t(D), 0);
+  int64_t nb[4] = {0, 0, 0, 0}, En = 0;
+  if (Tn > 0) {
+    // ---- 2. per composed row its source, TaskGroupMaxHosts and DependsOn count; the DependsOn ids' sources
+    CK(h2d(b.task_off, new_off.data(), 8 * (D + 1)));
+    int64_t *code = x.code.as<int64_t>(), *ecode = x.ecode.as<int64_t>();
+    int32_t* len = x.len.as<int32_t>();
+    const SxMap sm{D, m.new_off, m.ins_off, m.src};
+    launch(c, s, k_sx_rows, grid_for(Tn, 256), 256, 0, Tn, sm, x.gmh.as<int32_t>(), x.x_gmh.as<int32_t>(), x.dep_off.as<int64_t>(),
+           x.x_dep_off.as<int64_t>(), E_ins, code, b.gmh.as<int32_t>(), len, bad);
+    CK(scan_counts(c, len, Tn, b.dep_off.as<int64_t>()));
+    unsigned long long bad_row = 0;
+    CK(cudaMemcpyAsync(&En, b.dep_off.as<int64_t>() + Tn, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(&bad_row, bad, sizeof(bad_row), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    CK(cudaGetLastError());
+    if (bad_row != kInEmpty) return fail(EVG_ERR_INVALID, "%s: composed row %lld: its dep_off row breaks strings->dep_off", who, (long long)bad_row);
+    launch(c, s, k_sx_edges, grid_for(Tn, 256), 256, 0, Tn, code, x.dep_off.as<int64_t>(), x.x_dep_off.as<int64_t>(), b.dep_off.as<int64_t>(),
+           ecode);
+    // ---- 3. each string column: lengths, their scan into the composed offsets, then the bytes
+    SxCol col[4];
+    const int64_t n_str[4] = {Tn, Tn, Tn, En};
+    for (int k = 0; k < 4; k++) {
+      col[k] = SxCol{DStr{x.bytes[k].as<uint8_t>(), x.off[k].as<int64_t>(), x.nb[k]}, DStr{x.x_bytes[k].as<uint8_t>(), x.x_off[k].as<int64_t>(), nb_ins[k]},
+                     b.off[k].as<int64_t>(), b.bytes[k].as<uint8_t>()};
+      if (n_str[k] == 0) {
+        CK(cudaMemsetAsync(b.off[k].p, 0, sizeof(int64_t), s));
+        continue;
+      }
+      launch(c, s, k_sx_len, grid_for(n_str[k], 256), 256, 0, n_str[k], k == 3 ? ecode : code, col[k], k == 3 ? b.dep_off.as<int64_t>() : nullptr,
+             int32_t(Tn), len, bad);
+      CK(scan_counts(c, len, n_str[k], b.off[k].as<int64_t>()));
+      CK(cudaMemcpyAsync(nb + k, b.off[k].as<int64_t>() + n_str[k], sizeof(int64_t), cudaMemcpyDeviceToHost, s));
+    }
+    CK(cudaMemcpyAsync(&bad_row, bad, sizeof(bad_row), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    CK(cudaGetLastError());
+    if (bad_row != kInEmpty) return fail(EVG_ERR_INVALID, "%s: composed row %lld: a string offset of strings breaks its byte column", who, (long long)bad_row);
+    for (int k = 0; k < 4; k++) launch(c, s, k_sx_copy, grid_for(n_str[k] * 32, 256), 256, 0, n_str[k], k == 3 ? ecode : code, col[k]);
+    // ---- 4. the numeric columns gathered as evg_edit_tasks gathers them (ids: the interning below writes them)
+    launch(c, s, k_ed_gather, grid_for(Tn, 256), 256, 0, Tn, m, dtasks(c), e.ins.view(I), e.out.dst(), e.err.as<int>());
+    CK(cudaGetLastError());
+    // ---- 5. the composed table interned in place of a staged one
+    if ((rc = intern_run(c, who, Tn, D, En, nb, nullptr, e.out.gid, e.out.vid, e.dep_off, e.dep_idx, &z)) != EVG_OK) return rc;
+  }
+  return install_interned(c, who, Tn, new_off.data(), cfg, z, hosts, host_off, acfg, out, nb);
 }
 
 // --------------------------------------------------------------------------

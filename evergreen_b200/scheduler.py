@@ -388,6 +388,37 @@ class Engine:
         self._has_hosts = hosts is not None
         return out
 
+    def edit_strings(self, edit: S.StringEdit, cfg: np.ndarray, hosts: Optional[S.HostSoA] = None,
+                     n_dep_ids: Optional[int] = None) -> dict:
+        """evg_edit_strings: rows leave and join a tick whose strings the device keeps (after upload_strings or this
+        call); the composed string table (soa.compose_strings) is re-interned on the device and only the edit crosses
+        PCIe.  cfg is the new distro configuration (its n_versions is filled in on the device).  -> dict(group_off,
+        n_versions, group_max_hosts, group_first) of the composed tick; with n_dep_ids, the DependsOn id count of the
+        composed table, also the per-task group_id, version_id, dep_off and dep_idx, as upload_strings returns them."""
+        es, keep = edit.struct()
+        D = edit.strings.n_distros
+        Tn = self._n_tasks - int(edit.remove_rows.shape[0]) + edit.strings.n_tasks
+        cfg = np.ascontiguousarray(cfg, dtype=L.DISTRO_CFG_DTYPE)
+        out = dict(group_off=np.zeros(D + 1, np.int64), n_versions=np.zeros(max(D, 1), np.int32),
+                   group_max_hosts=np.empty(max(Tn, 1), np.int32), group_first=np.empty(max(Tn, 1), np.int64))
+        if n_dep_ids is not None:
+            out.update(group_id=np.empty(max(Tn, 1), np.int32), version_id=np.empty(max(Tn, 1), np.int32),
+                       dep_off=np.zeros(Tn + 1, np.int64), dep_idx=np.empty(max(int(n_dep_ids), 1), np.int32))
+        outs = L.InternOutStruct(*[L.ptr(out[k]) if k in out else None for k in S.INTERN_OUT_FIELDS])
+        hs = C.byref(hosts.struct()) if hosts is not None else None
+        L.check(self.lib.evg_edit_strings(self.ctx, C.byref(es), L.ptr(cfg) if D else None, hs,
+                                          L.ptr(hosts.host_off) if hosts is not None else None,
+                                          L.ptr(hosts.cfg) if hosts is not None and hosts.cfg.shape[0] else None, C.byref(outs)))
+        del keep
+        G = int(out["group_off"][-1])
+        out["n_versions"], out["group_max_hosts"], out["group_first"] = out["n_versions"][:D], out["group_max_hosts"][:G], out["group_first"][:G]
+        if n_dep_ids is not None:
+            out["group_id"], out["version_id"] = out["group_id"][:Tn], out["version_id"][:Tn]
+            out["dep_idx"] = out["dep_idx"][:int(out["dep_off"][-1])]
+        self._n_tasks, self._n_distros, self._n_groups = Tn, D, G
+        self._has_hosts = hosts is not None
+        return out
+
     def queue_index(self, ids, item_off) -> dict:
         """evg_queue_index_batch over saved queues: `ids` the queue[]._id of every queue concatenated (a list of str /
         bytes, or a (bytes, offsets) pair from soa.pack_strings), item_off the CSR over the queues.  The resident tick is
@@ -762,6 +793,13 @@ def _ranked_results(eng: Engine, batch, table, keys, now: int, breakdown: bool, 
     return out
 
 
+def _string_sig(t: M.Task) -> tuple:
+    """What evg_edit_strings keeps of a task on the device: its Version, task-group key, TaskGroupMaxHosts and
+    DependsOn ids."""
+    return (t.version, t.get_task_group_string() if t.task_group != "" else "", t.task_group_max_hosts,
+            tuple(d.task_id for d in t.depends_on))
+
+
 class ResidentTick:
     """The tick-to-tick cache a shim keeps so that only changes cross PCIe: the last batch's marshalled columns, each
     distro's task ids in resident order and a map from task id to row.  plan() takes the next Go-level batch, derives
@@ -776,13 +814,24 @@ class ResidentTick:
     changed are updated.  With device_deps=True the device keeps the tick's dependency table instead: the first tick
     and any change an edit cannot express upload with evg_upload_with_deps, every other tick sends only the dependency
     events (soa.DepsShim) with evg_edit_tasks_with_deps, and the stamps the device makes are written back onto the
-    Task objects.  The engine must not run other ticks between two plan() calls."""
+    Task objects.  With device_strings=True the device keeps the tick's strings and interns them: the first tick and
+    any change an edit cannot express (another distro list) upload with evg_upload_strings, every other tick sends the
+    departures' rows and the arrivals' numeric columns and strings with evg_edit_strings and the changed scalars with
+    evg_update_tasks.  A survivor whose strings changed (Version, task-group key, TaskGroupMaxHosts or DependsOn ids:
+    generate.tasks appends to the DependsOn of queued tasks) cannot be expressed either and uploads the batch.  The
+    host marshals the numeric columns only (marshal_tasks(intern=False)) and names each TaskGroupInfo from the group's
+    first row.  It cannot be combined with device_deps.
+    The engine must not run other ticks between two plan() calls."""
 
     SCALARS = ("priority", "expected_ns", "queue_basis_ns", "wait_basis_ns", "num_dependents", "task_group_order", "flags")
 
     def __init__(self, engine: Optional[Engine] = None, dependency_db: Optional[Dict[str, M.Task]] = None,
-                 device_deps: bool = False):
+                 device_deps: bool = False, device_strings: bool = False):
+        if device_deps and device_strings:
+            raise ValueError("device_strings cannot be combined with device_deps: evg_edit_strings keeps no dependency table")
         self.engine = engine  # None: default_engine() at the first plan()
+        self.device_strings = device_strings
+        self._sig: Dict[str, tuple] = {}  # device_strings: task id -> the strings the device holds for it
         self.dependency_db = dependency_db
         self.deps = S.DepsShim(dependency_db) if device_deps else None
         self.distro_ids: Optional[List[str]] = None
@@ -882,6 +931,8 @@ class ResidentTick:
         """One tick: what plan_distros returns for the batch in canonical order (self.canonical)."""
         eng = self.engine = self.engine or default_engine()
         canon = self.canonical(batch)
+        if self.device_strings:
+            return self._plan_strings(eng, canon, now, breakdown, secondary)
         soa, table, keys = S.marshal_tasks(canon, now, self.dependency_db, resolve_deps=self.deps is None)
         change = self.diff(canon, soa, table, keys)
         if self.deps is not None:
@@ -907,6 +958,55 @@ class ResidentTick:
         res = _ranked_results(eng, canon, table, keys, now, breakdown, secondary)
         self.ranked = [[t.id for t in ranked] for ranked, _ in res]
         self._disp = None  # the run ended the last dispatchers
+        return res
+
+    def _plan_strings(self, eng: Engine, canon, now: int, breakdown: bool, secondary: bool):
+        """plan() with device_strings: the strings stay on the device, only the edit's cross PCIe."""
+        soa, table, _ = S.marshal_tasks(canon, now, self.dependency_db, resolve_deps=True, intern=False)
+        change = None
+        sig = {t.id: _string_sig(t) for _, ts in canon for t in ts}
+        if self.distro_ids is None or [d.id for d, _ in canon] != self.distro_ids or any(
+                sig[i] != self._sig.get(i) for ids in self.ids for i in ids if i in sig):
+            # first tick, another distro list, or a survivor whose strings changed (generate.tasks appends to the
+            # DependsOn of queued tasks): the resident strings cannot express it, so the whole batch is uploaded
+            out = eng.upload_strings(soa, S.string_cols(canon), table.cfg)
+        else:
+            toff = table.task_off
+            remove, arrivals, old_rows, new_rows, ins_rows = [], [], [], [], []
+            for d, ((dist, ts), prev) in enumerate(zip(canon, self.ids)):
+                ids = {t.id for t in ts}
+                kept = [self.row[i] for i in prev if i in ids]
+                remove.extend(self.row[i] for i in prev if i not in ids)
+                n = len(kept)
+                old_rows.append(np.array(kept, dtype=np.int64))
+                new_rows.append(np.arange(toff[d], toff[d] + n, dtype=np.int64))
+                ins_rows.append(np.arange(toff[d] + n, toff[d + 1], dtype=np.int64))
+                arrivals.append((dist, ts[n:]))
+            ins_rows = np.concatenate(ins_rows)
+            edit = S.StringEdit(np.sort(np.array(remove, dtype=np.int64)),
+                                S.TaskSoA(**{name: getattr(soa, name)[ins_rows] for name, _ in S.TaskSoA.COLUMNS}), S.string_cols(arrivals))
+            out = eng.edit_strings(edit, table.cfg)
+            old_rows, new_rows = np.concatenate(old_rows), np.concatenate(new_rows)
+            changed = np.zeros(new_rows.shape[0], dtype=bool)
+            for name in self.SCALARS:
+                changed |= getattr(self.soa, name)[old_rows] != getattr(soa, name)[new_rows]
+            rows = new_rows[changed]
+            if rows.shape[0]:
+                eng.update_tasks(rows, S.TaskSoA(**{name: getattr(soa, name)[rows] for name, _ in S.TaskSoA.COLUMNS}))
+            change = (edit, rows)
+        cfg = np.array(table.cfg, copy=True)
+        cfg["n_versions"] = out["n_versions"]
+        table = S.DistroTable(table.task_off, out["group_off"], cfg, out["group_max_hosts"]).normalize()
+        flat = [t for _, ts in canon for t in ts]
+        first = out["group_first"].tolist()
+        keys = [S.MarshalledDistro([flat[r].get_task_group_string() for r in first[int(table.group_off[d]):int(table.group_off[d + 1])]])
+                for d in range(table.n_distros)]
+        self.last = change
+        self.remember(canon, soa, table, keys)
+        self._sig = sig
+        res = _ranked_results(eng, canon, table, keys, now, breakdown, secondary)
+        self.ranked = [[t.id for t in ranked] for ranked, _ in res]
+        self._disp = None
         return res
 
     def dispatchers(self, cap: int = 0):

@@ -343,7 +343,8 @@ class MarshalledDistro:
 
 
 def marshal_tasks(batch: Sequence[tuple], now: int, dependency_db: Optional[Dict[str, M.Task]] = None,
-                  duration_history: Optional[dict] = None, resolve_deps: bool = False, resolve_durations: bool = True):
+                  duration_history: Optional[dict] = None, resolve_deps: bool = False, resolve_durations: bool = True,
+                  intern: bool = True):
     """[(Distro, [Task])] -> (TaskSoA, DistroTable, [MarshalledDistro]).
 
     Per task this resolves FetchExpectedDuration (PopulateCaches, setup_funcs.go:20-67), which writes the task's
@@ -352,7 +353,9 @@ def marshal_tasks(batch: Sequence[tuple], now: int, dependency_db: Optional[Dict
     (scheduler.go:161-168) is the DEVICE's job: the product path pairs these columns with marshal_deps() and
     Engine.upload_with_deps(), which sets the EVG_TF_DEPS_MET bit and the stamped wait basis on the GPU.
     resolve_deps=True evaluates it here instead (host restatement, kept for tests and for callers of the plain
-    one-shot entry points that want self-contained columns)."""
+    one-shot entry points that want self-contained columns).  intern=False skips the string work (task groups,
+    versions, in-queue edges) for callers that let the device intern the strings (evg_upload_strings,
+    evg_edit_strings): group_id is then -1, version_id 0, there are no edges, no groups and no key tables."""
     cols = {name: [] for name, _ in TaskSoA.COLUMNS}
     dep_off, dep_idx = [0], []
     task_off, group_off, cfg_rows, gmax, keys = [0], [0], [], [], []
@@ -360,7 +363,7 @@ def marshal_tasks(batch: Sequence[tuple], now: int, dependency_db: Optional[Dict
         if len(tasks) > L.MAX_TASKS_PER_DISTRO:
             raise ValueError(f"distro {d.id!r}: {len(tasks)} tasks exceed {L.MAX_TASKS_PER_DISTRO}")
         incl = d.dispatcher_settings.version == M.DISPATCHER_VERSION_REVISED_WITH_DEPENDENCIES  # scheduler.go:28
-        index = {t.id: i for i, t in enumerate(tasks)}
+        index = {t.id: i for i, t in enumerate(tasks)} if intern else {}
         by_id = {t.id: t for t in tasks}
         groups: Dict[str, int] = {}
         versions: Dict[str, int] = {}
@@ -371,8 +374,8 @@ def marshal_tasks(batch: Sequence[tuple], now: int, dependency_db: Optional[Dict
                 avg, _ = M.fetch_expected_duration(t, now, hist)
             else:
                 avg = t.expected_duration
-            gid = -1
-            if t.task_group != "":
+            gid, vid = -1, 0
+            if intern and t.task_group != "":
                 name = t.get_task_group_string()
                 gid = groups.get(name)
                 if gid is None:
@@ -384,10 +387,11 @@ def marshal_tasks(batch: Sequence[tuple], now: int, dependency_db: Optional[Dict
                     # a per-group table can only carry one value, so members must agree (they do: it is a project setting)
                     raise ValueError(f"task group {name!r}: TaskGroupMaxHosts differs between members "
                                      f"({gmax[group_off[-1] + gid]} vs {t.task_group_max_hosts} on {t.id!r})")
-            vid = versions.get(t.version)
-            if vid is None:
-                vid = versions[t.version] = len(versions)
-                md.versions.append(t.version)
+            if intern:
+                vid = versions.get(t.version)
+                if vid is None:
+                    vid = versions[t.version] = len(versions)
+                    md.versions.append(t.version)
             qb = t.activated_time if t.activated_time != M.ZERO_TIME else t.ingest_time  # planner.go:318-322
             # checkDependenciesMet runs first (scheduler.go:82-98) and, on a fresh evaluation, stamps DependenciesMetTime
             # on the task (task.go:653); the wait is measured after that (scheduler.go:119-123)
@@ -415,7 +419,7 @@ def marshal_tasks(batch: Sequence[tuple], now: int, dependency_db: Optional[Dict
             cols["group_id"].append(gid)
             cols["version_id"].append(vid)
             cols["flags"].append(fl)
-            for dep in t.depends_on:  # only dependencies that are in this queue join units (planner.go:453)
+            for dep in t.depends_on if intern else ():  # only dependencies that are in this queue join units (planner.go:453)
                 j = index.get(dep.task_id)
                 if j is not None:
                     dep_idx.append(j)
@@ -514,6 +518,73 @@ def intern_columns(batch: Sequence[tuple], threads: int = 0):
     out, outs = sc.intern_out()
     L.check(lib.evg_intern_columns(C.byref(sc.struct()), C.byref(outs), int(threads)))
     return sc.trim(out)
+
+
+@dataclass
+class StringEdit:
+    """evg_string_edit (include/evg_sched.h): rows leave and join a tick whose strings the device keeps.  The inserted
+    rows bring their numeric columns (their ids and edges come from their strings, so `insert`'s group_id, version_id
+    and edges are not sent) and their strings; the strings' task_off is the inserted rows' CSR over distros."""
+    remove_rows: np.ndarray   # int64, strictly ascending rows of the resident table
+    insert: TaskSoA
+    strings: StringCols
+
+    @property
+    def insert_off(self) -> np.ndarray:
+        return self.strings.task_off
+
+    def struct(self):
+        """-> (StringEditStruct, the structs it points to: keep both alive for the call)."""
+        self.remove_rows = np.ascontiguousarray(self.remove_rows, dtype=np.int64)
+        ins = self.insert.normalize().struct()
+        ins.n_edges, ins.group_id, ins.version_id, ins.dep_off, ins.dep_idx = 0, None, None, None, None
+        st = self.strings.struct()
+        R = int(self.remove_rows.shape[0])
+        s = L.StringEditStruct(R, L.ptr(self.remove_rows) if R else None, C.pointer(ins), L.ptr(self.insert_off), C.pointer(st))
+        return s, (ins, st)
+
+    def nbytes(self) -> int:
+        """What the edit moves to the device: the removed rows, the inserted rows' seven numeric columns and strings."""
+        sc = self.strings
+        n = self.remove_rows.nbytes + sum(getattr(self.insert, name).nbytes for name in
+                                          ("priority", "expected_ns", "queue_basis_ns", "wait_basis_ns", "num_dependents",
+                                           "task_group_order", "flags"))
+        n += sc.task_off.nbytes + sc.group_max_hosts.nbytes + sc.dep_off.nbytes
+        return n + sum(c[0].nbytes + c[1].nbytes for c in (sc.id, sc.version, sc.group_key, sc.dep_id))
+
+
+def _gather_strings(cols: Sequence[tuple], rows: np.ndarray) -> tuple:
+    """Strings `rows` of the concatenation of the string columns `cols`, in that order -> (bytes, offsets)."""
+    data = np.concatenate([c[0] for c in cols]) if cols else np.zeros(0, np.uint8)
+    base = np.cumsum([0] + [c[0].shape[0] for c in cols])[:-1]
+    start = np.concatenate([c[1][:-1] + b for c, b in zip(cols, base)]).astype(np.int64)
+    lens = np.concatenate([np.diff(c[1]) for c in cols]).astype(np.int64)
+    ln = lens[rows]
+    off = np.concatenate([[0], np.cumsum(ln)]).astype(np.int64)
+    idx = np.repeat(start[rows] - off[:-1], ln) + np.arange(int(off[-1]), dtype=np.int64)
+    return np.ascontiguousarray(data[idx], np.uint8), off
+
+
+def compose_strings(old: StringCols, edit: StringEdit) -> StringCols:
+    """The composed string table of evg_edit_strings, in numpy: distro d's rows are its rows of `old` that
+    edit.remove_rows does not name, in their order, then its rows of edit.strings."""
+    ins = edit.strings
+    T0, I, D = old.n_tasks, ins.n_tasks, old.n_distros
+    keep = np.ones(T0, dtype=bool)
+    keep[np.asarray(edit.remove_rows, np.int64)] = False
+    distro = np.concatenate([np.repeat(np.arange(D), np.diff(old.task_off)), np.repeat(np.arange(D), np.diff(ins.task_off))])
+    src = np.nonzero(np.concatenate([keep, np.ones(I, dtype=bool)]))[0]
+    rows = src[np.argsort(distro[src], kind="stable")]  # old rows (< T0) sit before inserted ones within a distro
+    task_off = np.concatenate([[0], np.cumsum(np.bincount(distro[src], minlength=D))]).astype(np.int64)
+    # the DependsOn ids of each composed row: its range of the concatenated dep_off
+    dstart = np.concatenate([old.dep_off[:-1], ins.dep_off[:-1] + old.dep_off[-1]]).astype(np.int64)
+    dlen = np.concatenate([np.diff(old.dep_off), np.diff(ins.dep_off)]).astype(np.int64)[rows]
+    dep_off = np.concatenate([[0], np.cumsum(dlen)]).astype(np.int64)
+    edges = np.repeat(dstart[rows] - dep_off[:-1], dlen) + np.arange(int(dep_off[-1]), dtype=np.int64)
+    return StringCols(task_off, _gather_strings([old.id, ins.id], rows), _gather_strings([old.version, ins.version], rows),
+                      _gather_strings([old.group_key, ins.group_key], rows),
+                      np.ascontiguousarray(np.concatenate([old.group_max_hosts, ins.group_max_hosts])[rows], np.int32), dep_off,
+                      _gather_strings([old.dep_id, ins.dep_id], edges))
 
 
 def provider_class(provider: str) -> int:

@@ -407,7 +407,7 @@ int evg_bind_result_buffer(evg_ctx* ctx, void* device_ptr, int64_t capacity);
  * evg_deps_met_batch, evg_find_runnable_batch / _ex, evg_plan_from_finder / _ex, evg_edit_tasks, evg_edit_tasks_with_deps, evg_plan_aliases,
  * evg_expected_durations_batch, evg_prioritize_legacy_batch, evg_dag_rebuild_batch, evg_rebuild_dispatchers,
  * evg_host_job, evg_host_drawdown, evg_idle_hosts, evg_find_next_batch, evg_find_next_tasks, evg_estimate_start_times,
- * evg_estimate_start_batch, evg_intern_batch, evg_upload_strings and evg_queue_index_batch.  Every other call adds the kernels it launches: the uploads (their range check), evg_update_tasks,
+ * evg_estimate_start_batch, evg_intern_batch, evg_upload_strings, evg_edit_strings and evg_queue_index_batch.  Every other call adds the kernels it launches: the uploads (their range check), evg_update_tasks,
  * evg_download_queue, evg_download_queue_breakdown and evg_resolve_durations. */
 int64_t evg_last_launch_count(evg_ctx* ctx);
 /* Device time in ms of the last evg_run_resident, from CUDA events on the context
@@ -798,6 +798,52 @@ int evg_intern_batch(evg_ctx* ctx, const evg_string_cols* in, evg_intern_out* ou
  * before them. */
 int evg_upload_strings(evg_ctx* ctx, const evg_task_soa* tasks, const evg_string_cols* strings, const evg_distro_cfg* cfg,
                        const evg_host_soa* hosts, const int64_t* host_off, const evg_alloc_cfg* acfg, evg_intern_out* out);
+
+/* A change in queue membership of a tick whose strings the device keeps (evg_edit_strings).  Host pointers. */
+typedef struct {
+  int64_t n_remove;
+  const int64_t* remove_rows;     /* strictly ascending rows of the resident table */
+  const evg_task_soa* insert;     /* the 7 numeric columns of the inserted rows; group_id, version_id, dep_off, dep_idx NULL */
+  const int64_t* insert_off;      /* n_distros + 1: CSR of the inserted rows over distros */
+  const evg_string_cols* strings; /* the inserted rows' id, version, group_key, group_max_hosts, dep_off and dep_id;
+                                     strings->task_off == insert_off */
+} evg_string_edit;
+
+/* A tick from evg_upload_strings (or this call) keeps its string table on the device: every row's id, version, task-
+ * group key, TaskGroupMaxHosts and DependsOn ids (all of them, resolved or not).  This call edits that table and
+ * re-interns it: afterwards the context holds, bit for bit, the tick evg_upload_strings of the COMPOSED string table
+ * would leave -- the `out` arrays, evg_download (with and without EVG_OPT_BREAKDOWN), evg_download_queue,
+ * evg_download_queue_breakdown, evg_rebuild_dispatchers and evg_host_job.  The composed table is each distro's
+ * surviving rows in their previous order, then its inserted rows insert_off[d] .. insert_off[d+1].  Since the whole
+ * table is re-interned, group and version ids come out dense in first-appearance order of the composed table, and a
+ * survivor gains the edge to an arriving task it names in DependsOn and loses the edge to a departed one: there are no
+ * remaps and no added edges to pass, and no restriction on the edges a survivor loses.  cfg (n_distros entries) is the
+ * new distro configuration; cfg[d].n_versions is ignored and filled in from the device's count.  hosts / host_off / acfg
+ * as for evg_upload (NULL: planner only).
+ * Precondition: a survivor's strings are the ones the table holds.  A task whose Version, task-group key,
+ * TaskGroupMaxHosts or DependsOn ids changed since it was uploaded (generate.tasks appends to the DependsOn of queued
+ * tasks) must be removed and inserted again, or the tick uploaded again; the call cannot see the change.
+ * What crosses PCIe: the edit (the inserted rows' numeric columns and strings, the removed rows) host to device; back,
+ * the composed string sizes, the group, version and edge offsets of every distro, and the max hosts of every group slot
+ * (the distro table's group_max_hosts, which the install stages from the host) -- O(n_distros + task groups) values,
+ * which is O(tasks) for a tick of many small groups.
+ * Needs a resident string table (EVG_ERR_STATE otherwise): evg_upload_strings and this call set it; evg_update_tasks,
+ * evg_resolve_durations, runs, downloads, the dispatchers, host jobs and estimates, evg_intern_batch and
+ * evg_queue_index_batch keep it; every call that replaces the tick clears it, and so does evg_edit_tasks (its id remaps
+ * are not in the strings).  A string tick holds no dependency table, so evg_edit_tasks_with_deps refuses it
+ * (EVG_ERR_STATE) and leaves it as it was.
+ * EVG_ERR_INVALID, previous tick still resident and runnable: null arguments, remove rows not strictly ascending or out
+ * of range, an insert_off that is not a CSR over n_distros distros or differs from strings->task_off, another
+ * n_distros, non-NULL id columns in `insert`, strings rejected on the host as by evg_intern_batch, a distro above the
+ * task limit.  EVG_ERR_INVALID with no resident tick: a dep_off or string offset inside the inserted columns that breaks
+ * its column, members of one task group (survivors or arrivals) that disagree on TaskGroupMaxHosts; the message names
+ * the LOWEST composed row.  EVG_ERR_NOMEM before any launch for an edit the device cannot hold; the context and the
+ * tick stay usable.  EVG_INTERN_HASH_BITS applies as for evg_intern_batch.
+ * Out of scope: dependency tables (evg_edit_tasks_with_deps edits those; this call leaves none) and alias ticks.
+ * Replaces: the string maps PrepareTasksForPlanning files units by (scheduler/planner.go:431-456), per tick, for the
+ * rows that did not change. */
+int evg_edit_strings(evg_ctx* ctx, const evg_string_edit* edit, const evg_distro_cfg* cfg, const evg_host_soa* hosts,
+                     const int64_t* host_off, const evg_alloc_cfg* acfg, evg_intern_out* out);
 
 /* ---- cross-queue views of the saved queues -------------------------------- */
 
